@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — candidate-sites/sec of the Clair3 network forward on B200 (BASELINE.json metric).
+"""bench.py — candidate-sites/sec of the Clair3 network forward on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workloads pileup,fa,fa_dwell,cascade]
+                    [--dump-outputs DIR]
 
 ONE command measures the whole metric and prints ONE JSON line.  The top-level ``value`` / ``e2e`` / ``roofline`` are the
 pileup network on BASELINE.json configs[1] (the configuration the metric is quoted on); ``workloads`` carries one
@@ -16,11 +17,11 @@ sub-record per configuration:
     pileup_counts  SURVEY.md 8f row N4: the pileup feature counter (calculate_clair3_pileup, src/clair3_pileup.c:142-476) on
               decoded alignment records, aligned bases/s (its own metric; HBM-bound integer work)          weak
 
-A *step* is one forward of the hot path over one synthetic candidate-site batch.  Every timed region issues the K steps
-``repeats`` times back to back so that it lasts >= 2 s whatever K is (``timed_region_s``, ``repeats`` in the record;
-``ms_per_step`` = region / (K * repeats)); W warm-up steps precede it.  Steps go round-robin over a few CUDA streams of ONE
-model (each stream owns an activation workspace); device-resident inputs are rotated over > 126 MB of distinct batches so
-no step re-reads its input from L2; regions are bracketed by barrier + synchronize, timed with CUDA events, max over ranks;
+A *step* is one forward of the hot path over one synthetic candidate-site batch.  Every timed region issues exactly K steps
+(``--min-region-s S`` instead repeats the K steps until the region lasts >= S seconds: ``timed_region_s``, ``repeats`` in the
+record; ``ms_per_step`` = region / (K * repeats)); W warm-up steps precede it.  Steps go round-robin over a few CUDA streams of ONE
+model (each stream owns an activation workspace); device-resident inputs are rotated over > 140 MB of distinct batches (H100's
+L2 holds 50 MB) so no step re-reads its input from L2; regions are bracketed by barrier + synchronize, timed with CUDA events, max over ranks;
 ``nvidia-smi`` clocks are sampled every 100 ms DURING each region.  ``e2e`` is the same metric through the module API with
 pinned HOST input and HOST output (H2D and D2H inside the timed region): pipelined (``forward_async`` over the streams),
 through the ``predict_stream`` helper, and synchronous per step (the reference's ``_torch_predict`` shape).
@@ -29,7 +30,13 @@ N > 1: one process per GPU (torchrun), one NCCL broadcast of the packed weight i
 (``c3b_bcast_weights``), no data-path collective.
 
 ``--impl reference`` times the reference's own CPU implementation of the same steps (torch CPU ops, all host threads)
-through ``oracle/torch_port.py`` (the Python reference cannot travel to the GPU box; see DESIGN.md).
+through ``oracle/torch_port.py`` (see DESIGN.md).
+
+``--dump-outputs DIR`` writes, after the timed steps, what the last timed step of each workload returned: the probabilities
+of each network workload (``DIR/<workload>_probs.npy``, float32 [batch, out_dim]), the cascade's last batches of both phases
+(``cascade_pileup_probs.npy``, ``cascade_fa_probs.npy``) and the feature counter's arrays (``pileup_counts_*.npy``, float64: a
+fixed seeded sample of 65,536 columns of matrix / major / stats, all candidate columns and flags).  Inputs and weights are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -49,7 +56,7 @@ if ROOT not in sys.path:
 
 from clair3_b200 import synth  # noqa: E402
 
-MIN_REGION_S = 2.0
+MIN_REGION_S = 0.0
 
 # algorithmic FLOPs per site (SURVEY.md 8d) and per tensor-core kernel (2*M*N*K of the layer shapes, clair3/model.py:96-110, 317-344)
 WORKLOADS = {
@@ -87,7 +94,8 @@ def peaks():
         d = json.load(open(p))
         return {"bf16_burst": d["bf16_tflops"], "bf16_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "hbm": d["hbm_gbs"], "which": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_burst": 1590.0, "bf16_sustained": 1400.0, "hbm": 6650.0, "which": "fallback (B200_PROFILING.md)"}
+    # NVIDIA's H100 SXM data sheet (dense BF16, HBM3; a 700 W card): a ceiling, not a measured rate
+    return {"bf16_burst": 989.0, "bf16_sustained": 989.0, "hbm": 3350.0, "which": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -339,7 +347,7 @@ def run_reference_arm(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
-# ------------------------------------------------------------------------------------------------------- B200 arm
+# ------------------------------------------------------------------------------------------------------- GPU arm
 class Ctx:
     def __init__(self, args, rank, world, device, sampler):
         self.args, self.rank, self.world, self.device, self.sampler = args, rank, world, device, sampler
@@ -384,8 +392,12 @@ class Ctx:
         return ms, clocks
 
     def calibrated(self, issue, steps, est_calls=None):
-        """Run `steps` once untimed-for-the-record to estimate the step time, then a region of `repeats` x `steps` calls that
-        lasts >= MIN_REGION_S.  Returns dict(ms, repeats, clocks)."""
+        """One timed region of exactly `steps` calls; with MIN_REGION_S > 0, first run `steps` once untimed-for-the-record to
+        estimate the step time, then a region of `repeats` x `steps` calls that lasts >= MIN_REGION_S.
+        Returns dict(ms, repeats, clocks)."""
+        if MIN_REGION_S <= 0:
+            ms, clocks = self.timed(issue, steps)
+            return {"ms": ms, "repeats": 1, "clocks": clocks}
         n0 = est_calls or max(steps, 2 * len(self.streams))
         ms0, _ = self.timed(issue, n0)
         per_call = max(ms0 / n0, 1e-4)
@@ -448,19 +460,7 @@ def profile_kernels(ctx, model, w, xs_dev, value, clocks):
         k["sm_time_share"] = k["sm_time_ms"] / tot_sm
     # dominant = the tensor-core kernel with the largest SM-time (a 2-CTA launch with a long latency does not bound throughput)
     dom = max((n for n in kernels if n in kflops), key=lambda n: kernels[n]["sm_time_ms"])
-    # DRAM bytes per launch from the committed ncu capture (profiles/traffic.json, written by tools/ncu_summary.py from
-    # `ncu --set full`: dram__bytes_read.sum + dram__bytes_write.sum), if it was taken at this workload's batch size
-    traffic, traffic_all = None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        tw = tj.get("fa" if w["kind"] == "fa" else "pileup", {})
-        ent = tw.get(dom)
-        if ent and ent.get("batch") == b:
-            traffic = ent["dram_bytes_per_launch"]
-        if all(tw.get(n, {}).get("batch") == b for n in kernels if n in tw):
-            traffic_all = sum(tw[n]["dram_bytes_per_launch"] for n in kernels if n in tw) or None
-    except (OSError, ValueError):
-        pass
+    traffic, traffic_all = None, None                                 # DRAM bytes are not measured (no hardware counters)
     whole = w["flop"] * value / ctx.world / 1e12
     roofline = {"bound": "tensor", "kernel": dom, "achieved": kernels[dom]["tflops"], "peak": pk["bf16_burst"],
                 "unit": "TFLOP/s", "frac": kernels[dom]["tflops"] / pk["bf16_burst"], "traffic": traffic,
@@ -479,11 +479,18 @@ def profile_kernels(ctx, model, w, xs_dev, value, clocks):
         units = 128 if dom == "lstm1" else 160
         ctas = int(kernels[dom]["ctas"])
         mufu = 5.0 * 33 * 2 * units * b
-        clk_hz = ((clocks or {}).get("sm_mhz") or 1965.0) * 1e6
+        clk_hz = ((clocks or {}).get("sm_mhz") or 1980.0) * 1e6
         per_clk_sm = mufu / (kernels[dom]["ms_per_launch"] * 1e-3 * clk_hz) / ctas
         roofline["limiter"] = {"resource": "SFU (MUFU.TANH) issue, 16 lanes/clk/SM", "mufu_ops_per_launch": mufu, "ctas": ctas,
                                "achieved_per_clk_per_sm": per_clk_sm, "peak_per_clk_per_sm": 16.0, "frac": per_clk_sm / 16.0}
     return kernels, roofline
+
+
+def dump_output(out_dir, name, y):
+    """--dump-outputs: one array the timed path returned, as .npy (float64 arrays stay float64, everything else float32)."""
+    os.makedirs(out_dir, exist_ok=True)
+    y = y.detach().cpu()
+    np.save(os.path.join(out_dir, name + ".npy"), (y if y.dtype == torch.float64 else y.float()).numpy())
 
 
 def run_forward_workload(ctx, wname, model):
@@ -513,14 +520,16 @@ def run_forward_workload(ctx, wname, model):
     issue_dev(args.warmup)                                            # W warm-up steps
     launches0 = model.launch_count
     r = ctx.calibrated(issue_dev, K)
-    est = max(K, 2 * n_streams)                                       # calls of the calibration pass before the final region
+    if args.dump_outputs and ctx.rank == 0:
+        dump_output(args.dump_outputs, wname + "_probs", ys_dev[(counter[0] - 1) % len(ys_dev)])
+    est = max(K, 2 * n_streams) if MIN_REGION_S > 0 else 0            # calls of the calibration pass before the final region
     launches = (model.launch_count - launches0) * (K * r["repeats"]) // (K * r["repeats"] + est)   # the final region's share
     value = b * K * r["repeats"] * ctx.world / (r["ms"] * 1e-3)
     rec = {"value": value, "unit": "sites/s", "scaling": "weak", "steps": K, "repeats": r["repeats"],
            "timed_region_s": r["ms"] * 1e-3, "ms_per_step": r["ms"] / (K * r["repeats"]), "clocks": r["clocks"],
            "gpu_launches": int(launches), "parity_max_abs_dp": parity, "config": config_of(wname),
            "run": {"streams_in_flight": n_streams, "lstm_subtile_sites": (args.lstm_tile or "auto (64 stream-ordered / 16 synchronous)") if w["kind"] == "pileup" else None,
-                   "l2_policy": "inputs rotated over %d distinct device-resident batches (> 126 MB L2)" % pool}}
+                   "l2_policy": "inputs rotated over %d distinct device-resident batches (> 50 MB L2)" % pool}}
 
     # ---- e2e: pinned host tensors in and out through the module API, H2D and D2H inside the timed region
     xs_pin = [torch.from_numpy(x).pin_memory() for x in xs_host[:max(8, n_streams)]]
@@ -674,6 +683,11 @@ def run_cascade(ctx, model_p, model_f):
         if ms >= MIN_REGION_S * 1e3 or MIN_REGION_S <= 0:
             break
         passes = int(math.ceil(passes * MIN_REGION_S * 1e3 * 1.15 / max(ms, 1e-3)))
+    if args.dump_outputs and ctx.rank == 0:
+        # the buffers hold the last n_streams batches of each phase of the last timed pass
+        for name, lst, ys in (("cascade_pileup_probs", bp_list, yp), ("cascade_fa_probs", bf_list, yf)):
+            idx = range(max(0, len(lst) - n_streams), len(lst))
+            dump_output(args.dump_outputs, name, torch.cat([ys[i % n_streams][:lst[i]] for i in idx]))
     total = CASCADE_PILEUP_SITES + CASCADE_FA_SITES
     value = total * passes / (ms * 1e-3)
     h2d = (hi_p - lo_p) * site_bytes(wp) + (hi_f - lo_f) * site_bytes(wf)
@@ -743,6 +757,13 @@ def run_pileup_counts(ctx):
     issue_dev(args.warmup)
     r = ctx.calibrated(issue_dev, K)
     value = bases * K * r["repeats"] * ctx.world / (r["ms"] * 1e-3)
+    if args.dump_outputs and ctx.rank == 0:
+        last = counters[(cnt[0] - 1) % n_ctr].fetch()
+        rows = np.sort(np.random.default_rng(0).choice(len(last["major"]), min(65536, len(last["major"])), replace=False))
+        for k in ("matrix", "major", "stats"):
+            dump_output(args.dump_outputs, "pileup_counts_" + k, torch.from_numpy(np.asarray(last[k])[rows].astype(np.float64)))
+        for k in ("cand_cols", "cand_ok"):
+            dump_output(args.dump_outputs, "pileup_counts_" + k, torch.from_numpy(np.asarray(last[k]).astype(np.float64)))
 
     # e2e: pinned host records in, results out, synchronous per call (the shape of the reference's per-chunk call)
     pin = pc.BamRecords(**{k: torch.from_numpy(getattr(host, k).view({"uint16": np.int16, "uint32": np.int32}.get(getattr(host, k).dtype.name, getattr(host, k).dtype))).pin_memory().numpy().view(getattr(host, k).dtype)
@@ -764,13 +785,6 @@ def run_pileup_counts(ctx):
     # compulsory bytes of one call: the records and reference read once, the emitted arrays written once
     alg_bytes = h2d + d2h + n_cand * 8
     ach = alg_bytes / (ms_alone * 1e-3) / 1e9
-    traffic = None
-    try:
-        ent = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))["pileup_counts"]["count_tile"]
-        if ent.get("region_columns") == cfg["region"] and ent.get("depth") == cfg["depth"]:
-            traffic = ent["dram_bytes_per_launch"]
-    except (OSError, ValueError, KeyError):
-        pass
     out = {"metric": "aligned-bases/sec", "value": value, "unit": "bases/s", "scaling": "weak", "steps": K, "repeats": r["repeats"],
            "timed_region_s": r["ms"] * 1e-3, "ms_per_step": r["ms"] / (K * r["repeats"]), "clocks": r["clocks"],
            "columns_per_s": n_cols * K * r["repeats"] * ctx.world / (r["ms"] * 1e-3),
@@ -781,13 +795,11 @@ def run_pileup_counts(ctx):
            "e2e": {"value": e2e_value, "unit": "bases/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "steps": max(2, K // 4),
                    "repeats": re["repeats"], "timed_region_s": re["ms"] * 1e-3,
                    "mode": "PileupCounter.count(pinned host records).fetch(pinned=True): H2D of the records, 8 kernels, D2H of matrix / major / stats / candidates into page-locked buffers, synchronous per call"},
-           "roofline": {"bound": "hbm", "achieved": ach, "peak": pk["hbm"], "unit": "GB/s", "frac": ach / pk["hbm"], "traffic": traffic,
+           "roofline": {"bound": "hbm", "achieved": ach, "peak": pk["hbm"], "unit": "GB/s", "frac": ach / pk["hbm"], "traffic": None,
                         "peak_source": pk["which"], "kernel": "all 8 kernels of one call, timed alone with CUDA events on its stream (c3b_plp_last_ms): %.3f ms" % ms_alone,
                         "algorithmic_bytes_per_call": alg_bytes,
-                        "note": "achieved = compulsory bytes (records + reference in, emitted arrays out) / the call's device time; traffic = DRAM bytes "
-                                "of the dominant kernel (plp_count_tile, 86 % of the call) from the committed ncu capture.  That kernel is issue-bound "
-                                "(ncu: 76 % of the issue slots busy, ~470 warp instructions per read and warp: a binary search over the CIGAR prefix "
-                                "sums per read and column, single-lane indel bookkeeping), not bandwidth-bound"}}
+                        "note": "achieved = compulsory bytes (records + reference in, emitted arrays out) / the call's device time; DRAM "
+                                "traffic is not measured (no hardware counters)"}}
     if ctx.rank == 0 and ctx.world == 1 and not args.no_cpu_baseline:
         out["cpu_baseline"] = {"value": sample_bases / cpu_s, "unit": "bases/s", "cores": 1, "kind": "port",
                                "sample": "oracle/pileup_oracle.c (plain-C restatement of calculate_clair3_pileup, single thread like the reference's "
@@ -856,20 +868,22 @@ def select_workloads(spec, explicit, world):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20, help="K: steps per repeat (every timed region repeats the K steps until it lasts >= 2 s)")
+    ap.add_argument("--steps", type=int, default=20, help="K: timed steps per region")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workloads", default="pileup,fa,fa_dwell,cascade,pileup_counts")
     ap.add_argument("--workload", default=None, help="alias: run a single workload")
     ap.add_argument("--streams", type=int, default=12)
-    ap.add_argument("--lstm-wg", type=int, default=0, help="epilogue warpgroups per LSTM sub-tile (0 = library default)")
+    ap.add_argument("--lstm-wg", type=int, default=0, help="warpgroups per LSTM CTA (0 = library default)")
     ap.add_argument("--lstm-tile", type=int, default=0,
                     help="sites per LSTM1 sub-tile (16|32|64; 0 = library choice by call shape: 64 for stream-ordered calls, the "
                          "smallest GPU-filling tile for synchronous host-buffer calls)")
     ap.add_argument("--opt", action="append", default=[], help="library option name=value for the pileup model (tuning runs), repeatable")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--min-region-s", type=float, default=2.0,
-                    help="minimum length of every timed region (profiling runs under ncu pass 0: one pass of the K steps)")
+    ap.add_argument("--min-region-s", type=float, default=0.0,
+                    help="repeat the K steps until every timed region lasts at least this long (0: exactly K steps)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last timed step's outputs of each network workload as DIR/<name>.npy")
     args = ap.parse_args()
     explicit = args.workload is not None or any(a.startswith("--workloads") for a in sys.argv[1:])
     args.workloads = select_workloads(args.workload or args.workloads, explicit, int(os.environ.get("WORLD_SIZE", "1")))

@@ -1,4 +1,4 @@
-"""clair3_b200 — B200 (sm_100a) implementation of Clair3's variant-calling network forward pass.
+"""clair3_b200 — H100 (sm_90a) implementation of Clair3's variant-calling network forward pass.
 
 Public surface: ``clair3_b200.model.Clair3_P`` / ``Clair3_F`` (drop-in for ``clair3.model``), ``clair3_b200.dropin``
 (patches the reference in place), ``clair3_b200.sharding`` (site-range sharding + weight broadcast),

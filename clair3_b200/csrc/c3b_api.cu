@@ -21,7 +21,7 @@ void c3b_set_error(const char *fmt, ...) {
 extern "C" const char *c3b_last_error(void) { return g_err; }
 static thread_local long long g_last_grid = 0;
 void c3b_note_grid(long long ctas) { g_last_grid = ctas; }
-extern "C" const char *c3b_version(void) { return "clair3_b200 0.1 (sm_100a)"; }
+extern "C" const char *c3b_version(void) { return "clair3_b200 0.1 (sm_90a)"; }
 
 // ------------------------------------------------------------------------------------------------ helpers
 uint16_t c3b_f2op(float f) {
@@ -139,7 +139,7 @@ void build_expected(c3b_model *m) {
 
 const std::vector<float> &P(const c3b_model *m, const std::string &k) { return m->params.at(k).data; }
 
-// UMMA SWIZZLE_NONE K-major operand image of a [rows][k] matrix: [chunk][rowblock][8 kgroups][rb rows][8] fp16.
+// wgmma no-swizzle K-major operand image of a [rows][k] matrix: [chunk][rowblock][8 kgroups][rb rows][8] fp16.
 // get(row, k) supplies the (already folded / permuted) element; out-of-range k is zero.
 template <typename F>
 std::vector<uint16_t> pack_operand(int rows, int kgroups, int rb, F get) {
@@ -156,13 +156,6 @@ std::vector<uint16_t> pack_operand(int rows, int kgroups, int rb, F get) {
                         img[((((size_t)c * nrb + b) * 8 + kg) * rb + r) * 8 + e] = c3b_f2op(get(b * rb + r, g * 8 + e));
             }
     return img;
-}
-
-// torch gate-row index for LSTM2's permuted row R in [0,640): blocks 0..3 = gate m, units 0..127; block 4 = [i f g o] x units 128..159
-int lstm2_torch_row(int r640) {
-    const int blk = r640 / 128, r = r640 % 128;
-    if (blk < 4) return blk * C3B_H2 + r;
-    return (r / 32) * C3B_H2 + 128 + (r % 32);
 }
 
 }  // namespace
@@ -186,8 +179,8 @@ extern "C" int c3b_create(c3b_model **out, int kind, int channels, int add_indel
     if (device_ordinal < 0 || device_ordinal >= ndev) { c3b_set_error("bad device ordinal %d", device_ordinal); return 1; }
     cudaDeviceProp prop;
     C3B_CUDA(cudaGetDeviceProperties(&prop, device_ordinal));
-    if (prop.major != 10) {
-        c3b_set_error("device %d is sm_%d%d; this library contains only sm_100a code", device_ordinal, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        c3b_set_error("device %d is sm_%d%d; this library contains only sm_90a code", device_ordinal, prop.major, prop.minor);
         return 2;
     }
     C3B_CUDA(cudaSetDevice(device_ordinal));
@@ -258,15 +251,6 @@ extern "C" int c3b_set_option(c3b_model *m, const char *name, int value) {
     } else if (!strcmp(name, "lstm_wg")) {
         if (value != 1 && value != 2) { c3b_set_error("lstm_wg must be 1 or 2"); return 1; }
         m->lstm_wg = (int)value;
-    } else if (!strcmp(name, "lstm1_impl")) {
-        if (value != 0 && value != 1) { c3b_set_error("lstm1_impl must be 0 (gate rows on the lanes) or 1 (CTA-pair kernel)"); return 1; }
-        m->lstm1_impl = value;
-    } else if (!strcmp(name, "pconv_impl")) {
-        if (value != 0 && value != 1) { c3b_set_error("pconv_impl must be 0 (one CTA per tile) or 1 (block-pipelined / CTA-pair form)"); return 1; }
-        m->pconv_impl = value;
-    } else if (!strcmp(name, "lstm2_impl")) {
-        if (value != 0 && value != 1) { c3b_set_error("lstm2_impl must be 0 (gate rows on the lanes) or 1 (CTA-pair kernel)"); return 1; }
-        m->lstm2_impl = value;
     } else if (!strcmp(name, "lstm_mufu16")) {
         m->lstm_mufu16 = value ? 1 : 0;
     } else if (!strcmp(name, "tap_ws")) {
@@ -275,7 +259,6 @@ extern "C" int c3b_set_option(c3b_model *m, const char *name, int value) {
         m->taps = value ? 1 : 0;
         if (!value) for (Workspace *w : m->ws) w->taps.clear();
     } else if (!strcmp(name, "lstm_trace")) {
-        m->trace_conv = value >= 10 ? (int)value - 10 : 1;       // 10..18: Clair3_F conv index; 30: the LSTM2 input projection
         if (value && !m->lstm_trace) {
             C3B_CUDA(cudaSetDevice(m->device));
             C3B_CUDA(cudaMalloc(&m->lstm_trace, sizeof(long long) * 2 * C3B_T * 4));
@@ -347,32 +330,12 @@ static int finalize_impl(c3b_model *m) {
         for (int o = 0; o < m->d4; ++o)
             for (int k = 0; k < m->l4_in; ++k) w4t[(size_t)k * m->d4 + o] = w4[(size_t)o * m->l4_in + k];
         put(fb, w4t.data(), w4t.size() * 4, (const void **)&m->l4_f32_t, true);
-        // tensor-core tail (tail_tc.cu): L4 as the B operand of a sites-on-lanes GEMM, one contiguous piece per 64-wide k-chunk
+        // tensor-core L4 (tail_tc.cu): the B operand of a sites-on-rows GEMM, one contiguous piece per 64-wide k-chunk
         const int kg = m->l4_in / 8;
         const int l4_in = m->l4_in, d4 = m->d4;
         m->tail = TailW();
         std::vector<uint16_t> img = pack_operand(d4, kg, d4, [&](int r, int k) { return w4[(size_t)r * l4_in + k]; });
         put(blob, img.data(), img.size() * 2, (const void **)&m->tail.w4, false);
-        put(blob, P(m, "L4.bias").data(), (size_t)d4 * 4, (const void **)&m->tail.b4, false);
-        int toff = 0;
-        for (int h = 0; h < m->nheads; ++h) {
-            const std::vector<float> &w5 = P(m, std::string(kHeadNames[h][0]) + ".weight");   // [128][d4]
-            const std::vector<float> &wy = P(m, std::string(kHeadNames[h][1]) + ".weight");   // [n][128]
-            const std::vector<float> &byv = P(m, std::string(kHeadNames[h][1]) + ".bias");
-            const int n = kHeadDims[h], npad = (n + 15) / 16 * 16;
-            std::vector<uint16_t> i5 = pack_operand(128, d4 / 8, 128, [&](int r, int k) { return w5[(size_t)r * d4 + k]; });
-            std::vector<uint16_t> iy = pack_operand(npad, 16, npad, [&](int r, int k) { return r < n ? wy[(size_t)r * 128 + k] : 0.f; });
-            std::vector<float> byp(npad, 0.f);
-            for (int o = 0; o < n; ++o) byp[o] = byv[o];
-            put(blob, i5.data(), i5.size() * 2, (const void **)&m->tail.w5[h], false);
-            put(blob, P(m, std::string(kHeadNames[h][0]) + ".bias").data(), 128 * 4, (const void **)&m->tail.b5[h], false);
-            put(blob, iy.data(), iy.size() * 2, (const void **)&m->tail.wy[h], false);
-            put(blob, byp.data(), byp.size() * 4, (const void **)&m->tail.by[h], false);
-            m->tail.n[h] = n;
-            m->tail.npad[h] = npad;
-            m->tail.off[h] = toff;
-            toff += n;
-        }
     }
 
     if (m->kind == C3B_PILEUP) {
@@ -396,62 +359,38 @@ static int finalize_impl(c3b_model *m) {
                 put(fb, whh_t.data(), whh_t.size() * 4, (const void **)&m->lstm_f32[l][d].whh_t, true);
                 put(fb, bias.data(), bias.size() * 4, (const void **)&m->lstm_f32[l][d].bias, true);
             }
-        // tensor-core LSTM1 image: [dir][4 blocks][22 kgroups][128][8]; K = [x columns (48) ; h (128)] with the x columns
-        // [hi(x) (I) | 1 | lo(x) (I) | 0..]: W_ih multiplies both halves of the hi/lo split of the raw counts, the constant-1 column
-        // carries b_ih + b_hh (lstm_tc.cu)
+        // tensor-core LSTM1 image: [dir][8 blocks][22 kgroups][64][8], rows in c3b_lstm_row order; K = [x columns (48) ; h (128)]
+        // with the x columns [hi(x) (I) | 1 | lo(x) (I) | 0..]: W_ih multiplies both halves of the hi/lo split of the raw counts, the
+        // constant-1 column carries b_ih + b_hh (lstm_tc.cu)
         {
             const int KX = C3B_X1_COLS, KG = (KX + 128) / 8;
-            std::vector<uint16_t> img((size_t)2 * 4 * KG * 128 * 8, 0);
+            std::vector<uint16_t> img((size_t)2 * 512 * KG * 8, 0);
             for (int d = 0; d < 2; ++d) {
                 const std::string sfx = d ? "_l0_reverse" : "_l0";
                 const std::vector<float> &wih = P(m, "LSTM1.weight_ih" + sfx), &whh = P(m, "LSTM1.weight_hh" + sfx);
                 const std::vector<float> &bih = P(m, "LSTM1.bias_ih" + sfx), &bhh = P(m, "LSTM1.bias_hh" + sfx);
                 const int I = m->channels;
-                for (int blk = 0; blk < 4; ++blk)
-                    for (int r = 0; r < 128; ++r) {
-                        const int row = blk * 128 + r;
-                        // sigmoid gates (i,f,o) are pre-halved: sigma(x) = 0.5*tanh(x/2)+0.5 costs one MUFU + one FMA
-                        const float gs = (blk == 2) ? 1.0f : 0.5f;
-                        for (int k = 0; k < KX + 128; ++k) {
-                            float v = 0.f;
-                            if (k < I) v = wih[(size_t)row * I + k];
-                            else if (k == I) v = bih[row] + bhh[row];
-                            else if (k <= 2 * I) v = wih[(size_t)row * I + (k - I - 1)];
-                            else if (k >= KX) v = whh[(size_t)row * 128 + (k - KX)];
-                            img[((((size_t)d * 4 + blk) * KG + k / 8) * 128 + r) * 8 + k % 8] = c3b_f2op(v * gs);
-                        }
+                for (int R = 0; R < 512; ++R) {
+                    const int row = c3b_lstm_row(R, C3B_H1);
+                    // sigmoid gates (i,f,o) are pre-halved: sigma(x) = 0.5*tanh(x/2)+0.5 costs one MUFU + one FMA
+                    const float gs = (row / C3B_H1 == 2) ? 1.0f : 0.5f;
+                    for (int k = 0; k < KX + 128; ++k) {
+                        float v = 0.f;
+                        if (k < I) v = wih[(size_t)row * I + k];
+                        else if (k == I) v = bih[row] + bhh[row];
+                        else if (k <= 2 * I) v = wih[(size_t)row * I + (k - I - 1)];
+                        else if (k >= KX) v = whh[(size_t)row * 128 + (k - KX)];
+                        img[((((size_t)d * 8 + R / 64) * KG + k / 8) * 64 + R % 64) * 8 + k % 8] = c3b_f2op(v * gs);
                     }
+                }
             }
             put(blob, img.data(), img.size() * 2, (const void **)&m->lstm_tc[0][0].w_img, false);
             m->lstm_tc[0][0].bias = nullptr;
-            // the same matrix as B-operand halves for the CTA-pair kernel: [dir][rank][phase 4][22 kg][64 rows][8],
-            // rank 0 = gates (i, f), rank 1 = (g, o) of units 32 ph .. 32 ph + 31
-            std::vector<uint16_t> wx((size_t)2 * 2 * 4 * KG * 64 * 8, 0);
-            for (int d = 0; d < 2; ++d) {
-                const std::string sfx = d ? "_l0_reverse" : "_l0";
-                const std::vector<float> &wih = P(m, "LSTM1.weight_ih" + sfx), &whh = P(m, "LSTM1.weight_hh" + sfx);
-                const std::vector<float> &bih = P(m, "LSTM1.bias_ih" + sfx), &bhh = P(m, "LSTM1.bias_hh" + sfx);
-                const int I = m->channels;
-                for (int rk = 0; rk < 2; ++rk)
-                    for (int ph = 0; ph < 4; ++ph)
-                        for (int r = 0; r < 64; ++r) {
-                            const int gate = 2 * rk + r / 32, row = gate * C3B_H1 + 32 * ph + r % 32;
-                            const float gs = gate == 2 ? 1.0f : 0.5f;
-                            for (int k = 0; k < KX + 128; ++k) {
-                                float v = 0.f;
-                                if (k < I) v = wih[(size_t)row * I + k];
-                                else if (k == I) v = bih[row] + bhh[row];
-                                else if (k <= 2 * I) v = wih[(size_t)row * I + (k - I - 1)];
-                                else if (k >= KX) v = whh[(size_t)row * 128 + (k - KX)];
-                                wx[(((((size_t)d * 2 + rk) * 4 + ph) * KG + k / 8) * 64 + r) * 8 + k % 8] = c3b_f2op(v * gs);
-                            }
-                        }
-            }
-            put(blob, wx.data(), wx.size() * 2, (const void **)&m->lstm1x_w, false);
         }
-        // tensor-core LSTM2: recurrent image [dir][5 blocks][20][128][8] (permuted rows) + input projection GEMM (1280 rows)
+        // tensor-core LSTM2: recurrent image [dir][10 blocks][20][64][8] (c3b_lstm_row order) + input projection GEMM (1280 columns
+        // in the same order per direction, bias folded into the projection)
         {
-            std::vector<uint16_t> img((size_t)2 * 5 * 20 * 128 * 8, 0);
+            std::vector<uint16_t> img((size_t)2 * 640 * 20 * 8, 0);
             std::vector<float> pbias(1280);
             const std::vector<float> *wih_d[2];
             for (int d = 0; d < 2; ++d) {
@@ -460,21 +399,19 @@ static int finalize_impl(c3b_model *m) {
                 const std::vector<float> &bih = P(m, "LSTM2.bias_ih" + sfx), &bhh = P(m, "LSTM2.bias_hh" + sfx);
                 wih_d[d] = &P(m, "LSTM2.weight_ih" + sfx);
                 for (int R = 0; R < 640; ++R) {
-                    const int row = lstm2_torch_row(R);
+                    const int row = c3b_lstm_row(R, C3B_H2);
                     const float gs = (row / C3B_H2 == 2) ? 1.0f : 0.5f;      // pre-halved sigmoid gates
                     pbias[(size_t)d * 640 + R] = (bih[row] + bhh[row]) * gs;
                     for (int k = 0; k < 160; ++k)
-                        img[((((size_t)d * 5 + R / 128) * 20 + k / 8) * 128 + R % 128) * 8 + k % 8] =
-                            c3b_f2op(whh[(size_t)row * 160 + k] * gs);
+                        img[((((size_t)d * 10 + R / 64) * 20 + k / 8) * 64 + R % 64) * 8 + k % 8] = c3b_f2op(whh[(size_t)row * 160 + k] * gs);
                 }
             }
             put(blob, img.data(), img.size() * 2, (const void **)&m->lstm_tc[1][0].w_img, false);
             m->lstm_tc[1][0].bias = nullptr;
-            // one 256-row slab per column group of the projection kernel (proj_tc.cu): [chunk 4][group 5][8 kg][256 rows][8]
-            std::vector<uint16_t> pimg = pack_operand(1280, 32, 256, [&](int R, int k) {
-                const int d = R / 640;
-                const int row = lstm2_torch_row(R % 640);
-                return (*wih_d[d])[(size_t)row * 256 + k] * ((row / C3B_H2 == 2) ? 1.0f : 0.5f);
+            // one 128-column slab per column block of the projection kernel (proj_tc.cu): [chunk 4][block 10][8 kg][128 rows][8]
+            std::vector<uint16_t> pimg = pack_operand(1280, 32, 128, [&](int R, int k) {
+                const int row = c3b_lstm_row(R % 640, C3B_H2);
+                return (*wih_d[R / 640])[(size_t)row * 256 + k] * ((row / C3B_H2 == 2) ? 1.0f : 0.5f);
             });
             m->proj2 = IgemmW();
             m->proj2.n = 1280;
@@ -482,37 +419,6 @@ static int finalize_impl(c3b_model *m) {
             m->proj2.nchunks = 4;
             put(blob, pimg.data(), pimg.size() * 2, (const void **)&m->proj2.w_img, false);
             put(blob, pbias.data(), pbias.size() * 4, (const void **)&m->proj2.bias, false);
-            // ---- the CTA-pair LSTM2 kernel (lstm2x_tc.cu): per direction the 640 gate columns are ordered
-            // [phase 5][gate 4 (i,f,g,o)][unit-in-phase 32], i.e. column R2 -> torch row gate*160 + 32*phase + u
-            auto x_row = [](int R2) { return ((R2 % 128) / 32) * C3B_H2 + 32 * (R2 / 128) + (R2 % 32); };
-            auto x_gs = [](int R2) { return ((R2 % 128) / 32) == 2 ? 1.0f : 0.5f; };
-            std::vector<float> pbias2(1280);
-            for (int d = 0; d < 2; ++d) {
-                const std::string sfx = d ? "_l0_reverse" : "_l0";
-                const std::vector<float> &bih = P(m, "LSTM2.bias_ih" + sfx), &bhh = P(m, "LSTM2.bias_hh" + sfx);
-                for (int R2 = 0; R2 < 640; ++R2) pbias2[(size_t)d * 640 + R2] = (bih[x_row(R2)] + bhh[x_row(R2)]) * x_gs(R2);
-            }
-            std::vector<uint16_t> pimg2 = pack_operand(1280, 32, 256, [&](int R, int k) {
-                return (*wih_d[R / 640])[(size_t)x_row(R % 640) * 256 + k] * x_gs(R % 640);
-            });
-            m->proj2x = m->proj2;
-            put(blob, pimg2.data(), pimg2.size() * 2, (const void **)&m->proj2x.w_img, false);
-            put(blob, pbias2.data(), pbias2.size() * 4, (const void **)&m->proj2x.bias, false);
-            // W_hh as B-operand halves: [dir][rank][phase][20 kg][64 rows][8]; rank 0 = gates (i, f), rank 1 = (g, o)
-            std::vector<uint16_t> wx((size_t)2 * 2 * 5 * 20 * 64 * 8, 0);
-            for (int d = 0; d < 2; ++d) {
-                const std::vector<float> &whh = P(m, std::string("LSTM2.weight_hh") + (d ? "_l0_reverse" : "_l0"));
-                for (int rk = 0; rk < 2; ++rk)
-                    for (int ph = 0; ph < 5; ++ph)
-                        for (int r = 0; r < 64; ++r) {
-                            const int gate = 2 * rk + r / 32, unit = 32 * ph + r % 32;
-                            const float gs = gate == 2 ? 1.0f : 0.5f;
-                            for (int k = 0; k < 160; ++k)
-                                wx[(((((size_t)d * 2 + rk) * 5 + ph) * 20 + k / 8) * 64 + r) * 8 + k % 8] =
-                                    c3b_f2op(whh[(size_t)(gate * C3B_H2 + unit) * 160 + k] * gs);
-                        }
-            }
-            put(blob, wx.data(), wx.size() * 2, (const void **)&m->lstm2x_w, false);
         }
     } else {
         for (int i = 0; i < 9; ++i) {
@@ -535,7 +441,7 @@ static int finalize_impl(c3b_model *m) {
             m->conv_f32[i].stride = kConvStride[i];
             put(fb, wf.data(), wf.size() * 4, (const void **)&m->conv_f32[i].w, true);
             put(fb, bf.data(), bf.size() * 4, (const void **)&m->conv_f32[i].bias, true);
-            // tensor-core image: k = tap*cin_pad + ci; conv1's input channels are padded to one UMMA k-step (16)
+            // tensor-core image: k = tap*cin_pad + ci; conv1's input channels are padded to one wgmma k-step (16)
             const int cin_pad = (i == 0) ? 16 : cin;
             const int kg = 9 * cin_pad / 8;
             std::vector<uint16_t> img = pack_operand(cout, kg, cout, [&](int co, int k) {
@@ -548,14 +454,6 @@ static int finalize_impl(c3b_model *m) {
             m->conv_tc[i].nchunks = (kg + 7) / 8;
             put(blob, img.data(), img.size() * 2, (const void **)&m->conv_tc[i].w_img, false);
             put(blob, bf.data(), bf.size() * 4, (const void **)&m->conv_tc[i].bias, false);
-            if (cout >= 128) {
-                // the streamed-weight convs run on CTA pairs (pconv_tc.cu): each CTA's half of a piece's output channels contiguous
-                std::vector<uint16_t> img2 = pack_operand(cout, kg, cout / 2, [&](int co, int k) {
-                    const int t = k / cin_pad, ci = k % cin_pad;
-                    return ci < cin ? wf[((size_t)t * cin + ci) * cout + co] : 0.f;
-                });
-                put(blob, img2.data(), img2.size() * 2, (const void **)&m->conv_tc[i].w_img_pair, false);
-            }
         }
     }
 
@@ -618,11 +516,10 @@ extern "C" int c3b_bcast_weights(c3b_model *m, void *nccl_comm, int root, void *
 
 // ------------------------------------------------------------------------------------------------ workspaces
 static int64_t round128(int64_t b) { return (b + 127) / 128 * 128; }
-static int64_t round256(int64_t b) { return (b + 255) / 256 * 256; }   // pileup: a CTA pair of the LSTM2 kernel covers 256 sites
 static int conv_out(int v) { return (v - 1) / 2 + 1; }   // 3x3, stride 2, pad 1
 
 static size_t ws_bytes_needed(const c3b_model *m, int64_t sites, int depth) {
-    const int64_t bp = m->kind == C3B_PILEUP ? round256(sites) : round128(sites);
+    const int64_t bp = round128(sites);
     size_t total = 0;
     auto al = [&](size_t b) { total += (b + 255) / 256 * 256; };
     if (m->kind == C3B_PILEUP) {
@@ -762,7 +659,7 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
     const void *x = src.x;
     const int x_dtype = src.dtype;
     Carver cv{w->dev};
-    const int64_t bp = round256(n);
+    const int64_t bp = round128(n);
     std::map<std::string, Tap> &taps = w->taps;
     tap = tap && m->taps;
     if (m->precision == C3B_PREC_FP32) {
@@ -792,39 +689,23 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
     b.h2 = cv.take<op_t>((size_t)bp * C3B_T * 320 * 2);
     b.z4 = cv.take<float>((size_t)16 * bp * 128 * 4);
     b.bp = (int)bp;
-    // sub-tile width (sites per MMA column block); a CTA ping-pongs two sub-tiles -> 2 directions x bp / (2*tile) CTAs
-    // sub-tile width of lstm_tc_kernel (sites per MMA column block; a CTA ping-pongs two sub-tiles -> 2 directions x bp / (2*tile)
-    // CTAs): 64 = fewest SM-microseconds per site, the smallest tile that still fills the GPU = shortest single-batch latency
-    int tile1 = m->lstm_tile, tile2;
+    // sub-tile width of lstm_tc_kernel (sites per warpgroup): 64 = fewest SM-microseconds per site, the smallest tile that still
+    // fills the GPU = shortest single-batch latency.  LSTM2's weights leave room for at most 32-site sub-tiles.
+    int tile1 = m->lstm_tile;
     if (tile1 == 0) tile1 = !latency ? 64 : (bp / 64 >= m->sm_count) ? 64 : (bp / 32 >= m->sm_count) ? 32 : 16;
-    tile2 = tile1 > 32 ? 32 : tile1;
-    // LSTM2: always the CTA-pair kernel unless forced (the two kernels round differently - packed fp16 gate activations - and
-    // the answer must not depend on the call shape); the latency / throughput choice only picks bit-identical variants
-    // (LSTM1 tile width, the projection's grid)
-    const int lstm2_impl = m->lstm2_impl;
-    { PROF("ingest"); if (c3b_launch_ingest_pileup_tc(x, x_dtype, m->channels, src.starts, src.n_cols, b.xs, n, (int)bp, m->lstm1_impl, s)) return 1; }
+    const int tile2 = tile1 > 32 ? 32 : tile1;
+    { PROF("ingest"); if (c3b_launch_ingest_pileup_tc(x, x_dtype, m->channels, src.starts, src.n_cols, b.xs, n, (int)bp, s)) return 1; }
     m->launches += 1;
-    if (m->lstm1_impl == 1) {
-        PROF("lstm1");
-        if (c3b_launch_lstm1x(m, m->lstm1x_w, b.xs, b.h1, (int)bp, (m->lstm_trace && m->trace_conv == 1) ? m->lstm_trace : nullptr, s)) return 1;
-    } else {
-        PROF("lstm1");
-        if (c3b_launch_lstm1_tc(m, b, n, tile1, s)) return 1;
-    }
-    long long *ptrace = (m->lstm_trace && m->trace_conv == 20) ? m->lstm_trace : nullptr;
-    if (lstm2_impl == 1) {
-        { PROF("proj2"); if (c3b_launch_proj2(m, b.h1, m->proj2x, b.pg, (int)bp, 0, latency, ptrace, s)) return 1; }
-        { PROF("lstm2");
-          if (c3b_launch_lstm2x(m, m->lstm2x_w, b.pg, b.h2, (int)bp, (m->lstm_trace && m->trace_conv == 1) ? m->lstm_trace + C3B_T * 4 : nullptr, s)) return 1; }
-    } else {
-        { PROF("proj2"); if (c3b_launch_proj2(m, b.h1, m->proj2, b.pg, (int)bp, tile2, latency, ptrace, s)) return 1; }
-        { PROF("lstm2"); if (c3b_launch_lstm2_tc(m, b, n, tile2, s)) return 1; }
-    }
-    { PROF("tail"); if (c3b_launch_tail(m, b.h2, n, (int)bp, y, tap ? b.z4 : nullptr, s)) return 1; }
+    { PROF("lstm1"); if (c3b_launch_lstm1_tc(m, b, n, tile1, s)) return 1; }
+    { PROF("proj2"); if (c3b_launch_proj2(m, b.h1, m->proj2, b.pg, (int)bp, s)) return 1; }
+    { PROF("lstm2"); if (c3b_launch_lstm2_tc(m, b, n, tile2, s)) return 1; }
+    int nsplit = 1;
+    { PROF("tail"); if (c3b_launch_tail(m, b.h2, n, (int)bp, y, b.z4, &nsplit, s)) return 1; }
     if (tap) {
         taps["lstm1"] = {b.h1, 1, 3, 256, (int)bp, {}};
         taps["lstm2"] = {b.h2, 1, 2, (int64_t)C3B_T * 320, (int)bp, {}};
-        taps["l4_pre"] = {b.z4, 0, 0, 128, 0, {}};
+        taps["l4_pre"] = {b.z4, 0, 5, 128, (int)bp, {}};
+        taps["l4_pre"].nsplit = nsplit;
     }
     return 0;
 }
@@ -877,7 +758,7 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
     // ---- tensor-core path: zero-padded channel-group-planar feature maps (pconv_tc.cu).  Every stride-2 stem conv reads its
     // input as FOUR PARITY PLANES in its own output geometry (written by the ingest kernel / the previous residual block's
     // epilogue), which turns it into the same shifted-view implicit GEMM as the stride-1 convs: no gathers anywhere.
-    const int cpad = 16;                       // conv1 input channels padded to one UMMA k-step
+    const int cpad = 16;                       // conv1 input channels padded to one wgmma k-step
     PlanarGeom geo[3];
     op_t *stem_in[3];                          // parity planes feeding conv1 / conv3 / conv5: [4][cin/8][geo[l].p][8]
     op_t *act[3][3];
@@ -912,22 +793,19 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
         // stem conv (stride 2): shifted views of the four parity planes
         pa.c = stem_c[l]; pa.n = co; pa.stride2 = 1;
         pa.in = stem_in[l]; pa.out = a0; pa.residual = nullptr; pa.w = m->conv_tc[3 * l];
-        auto trace_of = [&](int ci) { return (m->lstm_trace && m->trace_conv == ci) ? m->lstm_trace : nullptr; };
-        pa.trace = trace_of(3 * l);
-        { PROF(cn[3 * l]); if ((m->pconv_impl ? c3b_launch_pconv2(m, pa, s) : c3b_launch_pconv(m, pa, s))) return 1; }
+        { PROF(cn[3 * l]); if (c3b_launch_pconv(m, pa, s)) return 1; }
         // residual block: two stride-1 shifted-view convolutions; the second one scatters its output into the next stem's
         // parity planes (levels 0, 1) or writes the plain planar map SPP reads (level 2)
         pa.c = co; pa.stride2 = 0;
-        pa.trace = trace_of(3 * l + 1);
         pa.in = a0; pa.out = a1; pa.w = m->conv_tc[3 * l + 1];
-        { PROF(cn[3 * l + 1]); if ((m->pconv_impl ? c3b_launch_pconv2(m, pa, s) : c3b_launch_pconv(m, pa, s))) return 1; }
-        pa.trace = trace_of(3 * l + 2);
+        { PROF(cn[3 * l + 1]); if (c3b_launch_pconv(m, pa, s)) return 1; }
         pa.in = a1; pa.out = a2; pa.residual = a0; pa.w = m->conv_tc[3 * l + 2];
         if (l < 2) { pa.out_parity = 1; pa.next = geo[l + 1]; }
-        { PROF(cn[3 * l + 2]); if ((m->pconv_impl ? c3b_launch_pconv2(m, pa, s) : c3b_launch_pconv(m, pa, s))) return 1; }
+        { PROF(cn[3 * l + 2]); if (c3b_launch_pconv(m, pa, s)) return 1; }
     }
     { PROF("spp"); if (c3b_launch_spp_tc(act[2][2], geo[2], sp, n, 256, (int)bp, s)) return 1; }
-    { PROF("tail"); if (c3b_launch_tail(m, sp, n, (int)bp, y, tap ? z4 : nullptr, s)) return 1; }
+    int nsplit = 1;
+    { PROF("tail"); if (c3b_launch_tail(m, sp, n, (int)bp, y, z4, &nsplit, s)) return 1; }
     m->launches += 1;          // spp (ingest, the convolutions and the tail count themselves)
     if (tap) {
         for (int l = 0; l < 3; ++l) {
@@ -941,7 +819,8 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
             }
         }
         taps["spp"] = {sp, 1, 2, 3584, (int)bp, {}};
-        taps["l4_pre"] = {z4, 0, 0, 256, 0, {}};
+        taps["l4_pre"] = {z4, 0, 5, 256, (int)bp, {}};
+        taps["l4_pre"].nsplit = nsplit;
     }
     return 0;
 }

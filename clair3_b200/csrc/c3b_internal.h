@@ -21,7 +21,7 @@
 void c3b_set_error(const char *fmt, ...);
 void c3b_note_grid(long long ctas);      // launchers report their grid size (CTAs) for the per-kernel profile (SM-time = CTAs x duration)
 
-// Tensor-core operand type.  fp16 (11-bit significand) rather than bf16 (8-bit): same tcgen05 rate, 8x smaller rounding
+// Tensor-core operand type.  fp16 (11-bit significand) rather than bf16 (8-bit): same wgmma rate, 8x smaller rounding
 // error; every operand on this path is bounded (counts <= 2048 exact, |h| <= 1, BN-normalised feature maps) and stores
 // saturate at +-65504 instead of overflowing.
 typedef __half op_t;
@@ -46,8 +46,7 @@ __device__ __forceinline__ uint32_t f2op2_sat(float lo, float hi) {
 __device__ __forceinline__ float op2f(op_t v) { return __half2float(v); }
 #endif
 // "Tile-major k-group-planar" activation matrices (h1, h2, spp): [row tile of 128][K/8 k-groups][128 rows][8] fp16.  A GEMM
-// tile's 64-wide k-chunk (8 k-groups) is then ONE contiguous 16 KB run = one cp.async.bulk (measured: a 2 KB bulk copy costs
-// ~150 cycles of the SM's TMA issue whatever its size, so eight 2 KB runs per chunk bound the streaming kernels at ~14 B/clk).
+// tile's 64-wide k-chunk (8 k-groups) is then ONE contiguous 16 KB run = one cp.async.bulk instead of eight 2 KB ones.
 // Returns the element offset of (row, k-group kg, lane 0).
 #ifdef __CUDACC__
 __host__ __device__
@@ -56,6 +55,12 @@ inline size_t c3b_tile_major_offset(size_t row, int kg, int kgroups) {
     return (((row >> 7) * (size_t)kgroups + (size_t)kg) * 128 + (row & 127)) * 8;
 }
 uint16_t c3b_f2op(float f);     // host: fp32 -> fp16 bits, round-to-nearest-even, saturating
+// Torch gate row (gate*H + unit) of row R in [0, 4H) of the recurrent kernels' permuted gate order (lstm_tc.cu): 64-row block
+// 2p holds gates i (rows 16w + q, q < 8) and f (rows 16w + q + 8) of units 32p + 8w + q, block 2p + 1 gates g and o.
+inline int c3b_lstm_row(int R, int H) {
+    const int pp = R / 128, blk = (R / 64) & 1, r = R % 64, w = r / 16, q = r % 16;
+    return (2 * blk + (q >= 8)) * H + 32 * pp + 8 * w + (q & 7);
+}
 float c3b_op2f(uint16_t h);     // host: fp16 bits -> fp32
 
 #define C3B_CUDA(expr)                                                                          \
@@ -105,27 +110,20 @@ struct ConvF32 {
 
 // ---- tensor-core path packed operands (device pointers into the weight blob) ----
 struct LstmTC {
-    const op_t *w_img;   // UMMA A-operand image: [nblk][K/8][128 rows][8] fp16, rows permuted (see lstm_tc.cu)
+    const op_t *w_img;   // wgmma A-operand image: [dir][2H/64 blocks][K/8][64 rows][8] fp16, rows permuted (c3b_lstm_row)
     const float *bias;            // unused (LSTM1's bias is a weight column against the constant-1 input; LSTM2's rides in the projection)
 };
 struct IgemmW {
-    const op_t *w_img;   // UMMA B-operand image per k-chunk: [nchunks][8 kgroups][N rows][8] fp16
-    const op_t *w_img_pair;       // convs with N >= 128: the same as [nchunks][2 halves of N][8 kgroups][N/2 rows][8] (CTA-pair form)
+    const op_t *w_img;   // wgmma B-operand image per k-chunk: [nchunks][8 kgroups][N rows][8] fp16
     const float *bias;            // [N]
     int n;                        // output columns (Cout / gate rows / dense units)
     int kgroups;                  // K/8 (16-byte k-groups), real
     int nchunks;                  // ceil(kgroups/8)
 };
 
-// fused dense tail (tail_tc.cu): L4 as a [d4 rows] B-operand image per k-chunk, per head L5 / Y operand images + fp32 biases
+// dense tail (tail_tc.cu): L4 as a [d4 rows] B-operand image per k-chunk (the heads run on the fp32 HeadsParams weights)
 struct TailW {
     const op_t *w4;                      // [l4_in/64 chunks][8 kg][d4 rows][8]
-    const float *b4;                     // [d4]
-    const op_t *w5[C3B_MAX_HEADS];       // [d4/8 kg][128 rows][8]
-    const float *b5[C3B_MAX_HEADS];      // [128]
-    const op_t *wy[C3B_MAX_HEADS];       // [16 kg][npad rows][8], rows >= n zero
-    const float *by[C3B_MAX_HEADS];      // [npad]
-    int n[C3B_MAX_HEADS], npad[C3B_MAX_HEADS], off[C3B_MAX_HEADS];
 };
 
 struct ConvGeom {
@@ -193,19 +191,15 @@ struct c3b_model {
     int chunk_sites = 0;
     int lstm_tile = 0;
     int profile = 0;
-    int lstm_wg = 2;                   // epilogue warpgroups per LSTM sub-tile (option "lstm_wg": 1 or 2)
-    int lstm1_impl = 0;                // the same choice for LSTM1 (default 0: measured equal SM-time, lower latency)
-    int pconv_impl = 0;                // 0 (default): pconv_tc.cu; 1: the block-pipelined / CTA-pair form (pconv2_tc.cu)
-    int lstm2_impl = 1;                // 1 (default): CTA-pair kernel with the sites on the lanes (lstm2x_tc.cu), 0: gate rows on the lanes (lstm_tc.cu)
+    int lstm_wg = 2;                   // warpgroups (one sub-tile of sites each) per LSTM CTA (option "lstm_wg": 1 or 2)
     int lstm_mufu16 = 0;               // 1: packed tanh.approx.f16x2 gate activations, 0 (default, faster: the epilogue is issue-bound): fp32 tanh.approx
     int tap_ws = -1;                   // debug: workspace index c3b_get_tap reads
     int taps = 0;                      // debug option "taps": record where the intermediate activations of a forward live
     bool weights_by_broadcast = false; // the packed images arrived by c3b_bcast_weights (no host-side parameters behind them)
     long long *lstm_trace = nullptr;   // device [2][33][4] clock stamps (debug option "lstm_trace")
-    int trace_conv = 1;            // which Clair3_F conv (0..8) stamps the trace buffer (option lstm_trace = 10 + index)
     std::map<std::string, std::pair<double, int64_t>> prof_total;   // name -> (ms, launches)
     std::map<std::string, double> prof_ctas;                         // name -> sum of CTAs launched
-    int sm_count = 148;
+    int sm_count = 132;
     bool finalized = false;
     std::map<std::string, HostParam> params;
     std::vector<std::string> expected;
@@ -224,11 +218,8 @@ struct c3b_model {
     ConvF32 conv_f32[9];
     // tc path
     LstmTC lstm_tc[2][2];
-    IgemmW proj2;                      // LSTM2 input projection, both directions: N = 1280 (row order of lstm_tc.cu)
-    IgemmW proj2x;                     // the same projection in the column order of the CTA-pair kernel (lstm2x_tc.cu)
-    const op_t *lstm1x_w = nullptr;    // LSTM1 [W_ih (hi | bias | lo columns) ; W_hh] as B-operand halves [dir][rank][phase 4][22][64][8]
-    const op_t *lstm2x_w = nullptr;    // W_hh as B-operand halves [dir][rank][phase][20][64][8]
-    TailW tail;                        // L4 + heads on the tensor cores
+    IgemmW proj2;                      // LSTM2 input projection, both directions: N = 1280 (row order c3b_lstm_row)
+    TailW tail;                        // L4 on the tensor cores
     IgemmW conv_tc[9];
 
     std::vector<Workspace *> ws;
@@ -263,20 +254,17 @@ struct TcPileupBuffers {
     op_t *h1;     // tile-major k-group-planar, 32 k-groups: row = t*Bp + b, k = dir*128 + j  (projection GEMM operand)
     __half *pg;            // [33*B][1280] fp16 pre-gates of LSTM2 (bias included), permuted gate columns
     op_t *h2;     // tile-major k-group-planar, 1320 k-groups: row = b, k = t*320 + dir*160 + j (flatten order of clair3/model.py:135)
-    float *z4;             // [B][128] fp32, L4 pre-activation without bias (debug tap only)
-    int bp;                // padded batch: multiple of 256 (a CTA pair of the LSTM2 kernel covers 256 sites)
+    float *z4;             // [16][B][128] fp32 split-K partial sums of the L4 pre-activation (no bias)
+    int bp;                // padded batch: multiple of 128
 };
 // starts == nullptr: x is the dense [batch][33][channels] tensor; otherwise x is the per-column matrix [n_cols][channels] and
 // site b is its rows [starts[b], starts[b] + 33) (rows outside the matrix read as zero)
 int c3b_launch_ingest_pileup_tc(const void *x, int dtype, int channels, const int64_t *starts, int64_t n_cols, op_t *xs, int64_t batch,
-                                int bp, int tiled, cudaStream_t s);
+                                int bp, cudaStream_t s);
 int c3b_launch_gather_windows_f32(const void *cols, int dtype, int channels, const int64_t *starts, int64_t n_cols, float *out,
                                   int64_t batch, cudaStream_t s);
-int c3b_launch_proj2(const c3b_model *m, const op_t *h1, const IgemmW &w, __half *pg, int bp, int nbl, bool latency, long long *trace,
-                     cudaStream_t s);
-int c3b_launch_lstm2x(const c3b_model *m, const op_t *w_img, const __half *pg2, op_t *h2, int bp, long long *trace, cudaStream_t s);
-int c3b_launch_lstm1x(const c3b_model *m, const op_t *w_img, const op_t *xs2, op_t *h1, int bp, long long *trace, cudaStream_t s);
-int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, float *out, float *z4_tap, cudaStream_t s);
+int c3b_launch_proj2(const c3b_model *m, const op_t *h1, const IgemmW &w, __half *pg, int bp, cudaStream_t s);
+int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, float *out, float *z4, int *nsplit_out, cudaStream_t s);
 int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s);
 int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s);
 
@@ -290,14 +278,12 @@ struct PconvArgs {
     int stride2;               // 1: `in` holds the four parity planes of the previous level, each [c/8][geom.p][8] (see pconv_tc.cu)
     int out_parity;            // 1: `out` receives the real pixels scattered into the four parity planes of `next` ([n/8][next.p][8] each)
     PlanarGeom next;
-    long long *trace;          // debug: clock stamps of CTA 0 (see pconv_tc.cu)
 };
 // offset (elements) of padded pixel (hp, wp) of site b, channel group 0, inside a parity-plane set of geometry g with c channels
 inline size_t c3b_parity_offset(const PlanarGeom &g, int c, int64_t b, int hp, int wp) {
     return (size_t)((hp & 1) * 2 + (wp & 1)) * ((size_t)(c / 8) * g.p * 8) + ((size_t)g.g + b * g.s + (size_t)((hp >> 1) + 1) * g.wp + ((wp >> 1) + 1)) * 8;
 }
 int c3b_launch_pconv(const c3b_model *m, const PconvArgs &a, cudaStream_t s);
-int c3b_launch_pconv2(const c3b_model *m, const PconvArgs &a, cudaStream_t s);   // block-pipelined / CTA-pair form (pconv2_tc.cu)
 
 int c3b_launch_ingest_fa_tc(const void *x, int dtype, int channels, int cpad, op_t *out, int64_t batch, int depth, const PlanarGeom &g1,
                             cudaStream_t s);

@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(HEADS_THREADS) heads_kernel(const float *__res
     asm volatile("cp.async.commit_group;" ::: "memory");
     // a is stored [k][G] so the L5 loop reads the 8 sites of one k with two 16-byte broadcast loads
     // (all split-K partial loads of a thread are independent: issue them together, then add in a fixed order - a rolled
-    //  loop with a running sum serialises ~64 L2 round trips per thread, which was 60 % of this kernel's time)
+    //  loop with a running sum serialises up to 16 L2 round trips per thread)
 #pragma unroll 2
     for (int i = tid; i < HEADS_G * d4; i += HEADS_THREADS) {
         const int g = i / d4, k = i - g * d4;              // consecutive threads -> consecutive k: coalesced partial-sum reads
@@ -228,7 +228,7 @@ int c3b_launch_heads(const float *z4, int nsplit, int64_t split_stride, const He
                      cudaStream_t s) {
     if (batch == 0) return 0;
     if (nsplit < 1 || nsplit > 16) { c3b_set_error("heads: %d split-K partials (1..16 supported)", nsplit); return 1; }
-    int sms = 148;
+    int sms = 132;
     { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
     const int G = batch >= 512 ? 16 : 8;      // SM-time per site (weight streaming) matters more than block count once a launch has 32+ blocks
     size_t smem = sizeof(float) * ((size_t)G * hp.d4 + (size_t)C3B_MAX_HEADS * G * 128 + (size_t)G * 96 + HEADS_STAGES * 2 * HEADS_KT * 128 +

@@ -1,34 +1,30 @@
-// Stride-1 3x3 convolution (the six residual-block convs of Clair3_F, 83 % of its FLOPs; clair3/model.py:200-235) as an
-// implicit GEMM over SHIFTED VIEWS of a shared-memory-resident, zero-padded, channel-group-planar feature map.
+// 3x3 convolutions of Clair3_F (clair3/model.py:200-235) as an implicit GEMM over SHIFTED VIEWS of a shared-memory-resident,
+// zero-padded, channel-group-planar feature map, on warpgroup MMAs.
 //
 // Activation layout ("planar padded"): [C/8][P][8] fp16.  A site's H x W feature map is stored as its (H+2) x (W+2)
 // zero-bordered raster, sites back to back: slot g = b*S + (h+1)*Wp + (w+1), S = (H+2)*Wp, Wp = W+2, at plane offset G + g
 // (G guard slots of zeros at both ends).  With that layout
-//   * the input of a macro-tile (MT x 128 consecutive output slots plus a (Wp+1)-slot halo on each side) is C/8 CONTIGUOUS
-//     runs of memory: it lands in shared memory with C/8 cp.async.bulk (TMA engine, async proxy; no per-thread gathers,
-//     no im2col expansion, no proxy fences) in exactly the SWIZZLE_NONE K-major UMMA layout [k-group][slot][8];
+//   * the input of a tile (128 consecutive output slots plus a G-slot halo on each side) is C/8 CONTIGUOUS runs of memory: it
+//     lands in shared memory with C/8 cp.async.bulk copies (TMA engine; no per-thread gathers, no im2col expansion) in exactly
+//     the no-swizzle K-major wgmma layout [k-group][slot][8];
 //   * the A operand of tap (dh,dw) is the SAME image viewed (dh-1)*Wp + (dw-1) slots later: only the descriptor's start
-//     address changes, so every input byte is fetched once per macro-tile and used by all nine taps;
+//     address changes, so every input byte is fetched once per tile and used by all nine taps;
+//   * stride-2 stem convs read FOUR parity planes of the previous level (each a planar padded tensor in THIS conv's geometry):
+//     tap (dh,dw) = plane (dh&1, dw&1) viewed (dh>>1)*Wp + (dw>>1) slots later - shifted views again;
 //   * border slots are computed like any other row but never stored: they keep the zeros of the one-time workspace clear,
 //     so the output is again a valid planar padded tensor for the next convolution (and the residual add reads the same
 //     slot of its own input).
-// Weights: the host-packed per-chunk operand images (pack_operand, c3b_api.cu) ([tap*C/64 + kc][8 k-groups][N][8]); resident when they fit
-// (res_block1: 72 KB), otherwise streamed through a ring with each piece applied to MT accumulators.
-//
-// Roles (320 threads): warp 9 lane 0 issues all bulk copies, warp 8 issues tcgen05.mma (one elected lane), warps 0-7 run
-// the epilogue as two groups of four (one TMEM lane quadrant per warp, alternating 16-column chunks per group): bias +
-// residual + ReLU + border mask, 16-byte coalesced planar stores.
-#include <cstdio>
-#include <cstdlib>
-
+// Weights: the host-packed operand image (pack_operand, c3b_api.cu) [k-chunk][8 k-groups][N][8], k = tap*C + ci, streams
+// through a two-stage ring, one 64-wide k-chunk per stage.  Two warpgroups own 64 output slots each (N = Cout, in wgmma
+// widths of at most 128); the epilogue adds bias and residual, applies ReLU and stores the real pixels - into the planar map
+// of this level, or scattered into the four parity planes the next level's stem conv reads.
 #include "c3b_internal.h"
 #include "ptx.cuh"
 
 namespace {
 
-constexpr int kThreads = 320;
-constexpr int kMaxWStages = 8;
-constexpr int kMetaSlots = 1024;
+constexpr int kThreads = 256;
+constexpr int kWStages = 2;
 
 struct PconvDev {
     const op_t *in;
@@ -36,432 +32,162 @@ struct PconvDev {
     const float *bias;
     const op_t *residual;
     op_t *out;
-    int C, N;
-    int H, W, Wp, S, G;
-    long long T, P;
-    int MT, n_macro, n_in;
-    int nchunks, cpt;
-    int w_resident, w_stages, img_bufs, acc_stages;
-    int relu;
-    // stride-2 stem convs read FOUR parity planes of the previous level (each a planar padded tensor in THIS conv's
-    // geometry): tap (dh,dw) = plane (dh&1, dw&1) viewed (dh>>1)*Wp + (dw>>1) slots later - shifted views again
-    int nplanes;           // 1 (stride 1) or 4 (stride 2)
-    long long plane_elems; // elements between input planes
-    int kpt_shift;         // log2(C/16): k-steps per tap
-    int nksteps;           // 9 * C/16
-    int halo_lo;           // slots loaded before the macro-tile (Wp+1 for stride 1, 0 for stride 2)
-    // output: 0 = planar padded (same geometry); 1 = scatter real pixels into the four parity planes of the NEXT level
-    int out_parity;
-    long long out_plane_elems;
-    int nS, nWp, nG;       // next level: slots per site, padded width, guard
-    long long nP;          // next level: plane pitch
-    long long *trace;      // optional: CTA 0 stamps [macro][8] (debug option "lstm_trace")
+    PlanarGeom g, nx;          // this level; the next level (parity output)
+    int c, relu, par, nksteps, nchunks;
+    uint32_t rows;             // slots of input per tile and plane: 128 + 2G
 };
 
-// Border mask and parity-scatter target of slot l of a site (the epilogue looks this up instead of dividing per tile).
-__device__ __forceinline__ uint32_t slot_meta(const PconvDev &p, int l) {
-    const int hh = l / p.Wp, ww = l - hh * p.Wp;
-    if (!(hh >= 1 && hh <= p.H && ww >= 1 && ww <= p.W)) return 0u;
-    uint32_t m = 0x80000000u;
-    if (p.out_parity) m |= (uint32_t)((hh & 1) * 2 + (ww & 1)) << 20 | (uint32_t)(((hh >> 1) + 1) * p.nWp + ((ww >> 1) + 1));
-    return m;
+template <int N>
+__device__ __forceinline__ void wgmma_n(float (&d)[N == 64 ? 32 : 64], uint64_t a, uint64_t b) {
+    if constexpr (N == 64) ptx::wgmma_m64n64k16(d, a, b, 1);
+    else ptx::wgmma_m64n128k16(d, a, b, 1);
 }
 
-// Epilogue of one macro-tile for one thread (TMEM lane = output slot): bias + residual + ReLU + border mask + fp16 pack +
-// 16-byte stores, over the 16-column chunks of this thread's warp group.  TMEM reads are software-pipelined (the load of the
-// next chunk - of this or the next tile - is in flight while the current one is finished); residuals are fetched one chunk
-// ahead.  RES / PAR are compile-time so the no-residual and planar-output cases carry no dead work.
-template <int MT, bool RES, bool PAR>
-__device__ __forceinline__ void epilogue_tiles(const PconvDev &p, uint32_t tbase, long long g0, int eg, const float *bias_s,
-                                               const uint32_t *meta_s) {
-    const int cpg = p.N >> 5;                                            // chunks per group per tile (2, 4 or 8)
-    const uint32_t in_pitch = (uint32_t)p.P * 16u;                       // bytes between k-group planes (< 4 GB, host-checked)
-    const uint32_t out_pitch = PAR ? (uint32_t)p.nP * 16u : in_pitch;
-    float v0[16], v1[16];
-    ptx::tmem_ld16(tbase, v0);
-#pragma unroll
-    for (int ti = 0; ti < MT; ++ti) {
-        const long long g = g0 + 128LL * ti;                             // output slot
-        const bool in_data = g < p.T;
-        bool real = false;
-        size_t par_off = 0;                                              // parity-scatter destination (plane + slot of the next level)
-        if (in_data) {
-            const uint32_t b = (uint32_t)g / (uint32_t)p.S;              // T < 2^31 (checked on the host)
-            const int l = (int)((uint32_t)g - b * (uint32_t)p.S);
-            const uint32_t meta = p.S <= kMetaSlots ? meta_s[l] : slot_meta(p, l);
-            real = (meta >> 31) != 0;
-            if (PAR && real)
-                par_off = (size_t)((meta >> 20) & 3u) * p.out_plane_elems + ((size_t)p.nG + (size_t)b * p.nS + (meta & 0xFFFFFu)) * 8;
-        }
-        const bool wr = real;       // border slots are never written: they stay zero from the workspace clear (one clear per geometry)
-        const size_t slot_off = ((size_t)p.G + (size_t)g) * 8;
-        const uint32_t taddr = tbase + (uint32_t)(ti * p.N);
-        char *const obase = reinterpret_cast<char *>(PAR ? p.out + par_off : p.out + slot_off);
-        const char *const rbase = reinterpret_cast<const char *>(p.residual + slot_off);
-        uint4 res[2], rn[2];
-        if (RES && real) {
-            res[0] = *reinterpret_cast<const uint4 *>(rbase + (uint32_t)(2 * eg) * in_pitch);
-            res[1] = *reinterpret_cast<const uint4 *>(rbase + (uint32_t)(2 * eg + 1) * in_pitch);
-        }
-        auto finish = [&](const float *v, int j0) {       // one chunk: 16 channels of this slot
-            if (!wr) return;
-            uint4 pk[2];
-            {
-                uint32_t *pw = reinterpret_cast<uint32_t *>(pk);
-                const float4 *b4 = reinterpret_cast<const float4 *>(bias_s + j0);
-                const op2_t *rp = reinterpret_cast<const op2_t *>(res);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float4 bb = b4[i];
-                    float x0 = v[4 * i] + bb.x, x1 = v[4 * i + 1] + bb.y, x2 = v[4 * i + 2] + bb.z, x3 = v[4 * i + 3] + bb.w;
-                    if (RES) {
-                        const float2 ra = op22f2(rp[2 * i]), rb = op22f2(rp[2 * i + 1]);
-                        x0 += ra.x; x1 += ra.y; x2 += rb.x; x3 += rb.y;
-                    }
-                    if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f); }
-                    pw[2 * i] = f2op2_sat(x0, x1);
-                    pw[2 * i + 1] = f2op2_sat(x2, x3);
-                }
-            }
-            char *d0p = obase + (uint32_t)(j0 >> 3) * out_pitch;
-            *reinterpret_cast<uint4 *>(d0p) = pk[0];
-            *reinterpret_cast<uint4 *>(d0p + out_pitch) = pk[1];
-        };
-        auto next_res = [&](int j0n) {                     // residual of the chunk after the current one
-            if (RES && real && j0n < p.N) {
-                rn[0] = *reinterpret_cast<const uint4 *>(rbase + (uint32_t)(j0n >> 3) * in_pitch);
-                rn[1] = *reinterpret_cast<const uint4 *>(rbase + (uint32_t)((j0n >> 3) + 1) * in_pitch);
-            }
-        };
-        for (int jc = 0; jc < cpg; jc += 2) {
-            const int j0 = 16 * eg + 32 * jc;
-            ptx::tmem_ld_wait();                                         // v0 = chunk jc
-            ptx::tmem_ld16(taddr + (uint32_t)(32 * (jc + 1)), v1);
-            next_res(j0 + 32);
-            finish(v0, j0);
-            if (RES) { res[0] = rn[0]; res[1] = rn[1]; }
-            ptx::tmem_ld_wait();                                         // v1 = chunk jc + 1
-            if (jc + 2 < cpg) ptx::tmem_ld16(taddr + (uint32_t)(32 * (jc + 2)), v0);
-            else if (ti + 1 < MT) ptx::tmem_ld16(taddr + (uint32_t)p.N, v0);      // first chunk of the next tile
-            next_res(j0 + 64);
-            finish(v1, j0 + 32);
-            if (RES) { res[0] = rn[0]; res[1] = rn[1]; }
-        }
-    }
-}
-
-template <int MT>
+template <int N, bool S2>
 __global__ void __launch_bounds__(kThreads, 1) pconv_kernel(const PconvDev p) {
+    constexpr int NW = N == 64 ? 64 : 128;      // wgmma width
+    constexpr int NT = N / NW;
+    constexpr int NPL = S2 ? 4 : 1;
+    constexpr uint32_t W_STAGE = 8 * N * 16;
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t w_full[kMaxWStages], w_empty[kMaxWStages];
-    __shared__ uint64_t img_full[2], img_empty[2], tmem_full[2], tmem_empty[2], w_res_bar;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ __align__(16) float bias_s[256];
-    __shared__ uint32_t a_off_s[144];
-    __shared__ uint32_t meta_s[kMetaSlots];   // per slot-in-site: bit 31 = real pixel, bits 20..21 = parity plane, low 20 = slot in the next level's site
+    __shared__ uint64_t a_bar, w_bar[kWStages];
+    const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31;
+    const PlanarGeom &g = p.g;
+    const long long t0 = (long long)blockIdx.x * 128;          // first output slot of the tile (data-slot index)
+    const int cg = p.c / 8;
+    const uint32_t a_base = ptx::smem_u32(smem);
+    const uint32_t w_base = a_base + NPL * cg * p.rows * 16;
+    const uint32_t a_bytes = NPL * cg * p.rows * 16;
 
-    const int tid = threadIdx.x;
-    const int warp = tid >> 5;
-    const int lane = tid & 31;
-    const uint32_t w_bytes = (uint32_t)p.N * 128u;
-    const uint32_t img_bytes = (uint32_t)p.nplanes * (uint32_t)(p.C / 8) * (uint32_t)p.n_in * 16u;
-    const uint32_t lbo_img = (uint32_t)p.n_in * 16u;
-    const uint32_t lbo_w = (uint32_t)p.N * 16u;
-    const uint32_t smem_base = ptx::smem_u32(smem);
-    const uint32_t w_region = p.w_resident ? (uint32_t)p.nchunks * w_bytes : (uint32_t)p.w_stages * w_bytes;
-    const uint32_t img_base = smem_base + w_region;
-
+    auto issue_w = [&](int ch) {
+        const int st = ch % kWStages;
+        ptx::mbar_arrive_expect_tx(&w_bar[st], W_STAGE);
+        ptx::bulk_g2s(w_base + st * W_STAGE, p.w_img + (size_t)ch * 8 * N * 8, W_STAGE, &w_bar[st]);
+    };
     if (tid == 0) {
-        for (int s = 0; s < kMaxWStages; ++s) { ptx::mbar_init(&w_full[s], 1); ptx::mbar_init(&w_empty[s], 1); }
-        for (int s = 0; s < 2; ++s) {
-            ptx::mbar_init(&img_full[s], 1);
-            ptx::mbar_init(&img_empty[s], 1);
-            ptx::mbar_init(&tmem_full[s], 1);
-            ptx::mbar_init(&tmem_empty[s], 256);
-        }
-        ptx::mbar_init(&w_res_bar, 1);
+        ptx::mbar_init(&a_bar, 1);
+        for (int s = 0; s < kWStages; ++s) ptx::mbar_init(&w_bar[s], 1);
         ptx::fence_barrier_init();
+        ptx::mbar_arrive_expect_tx(&a_bar, a_bytes);
+        for (int ch = 0; ch < kWStages && ch < p.nchunks; ++ch) issue_w(ch);
     }
-    if (warp == 8) ptx::tmem_alloc<512>(&tmem_base_smem);
-    for (int i = tid; i < p.N; i += kThreads) bias_s[i] = p.bias ? p.bias[i] : 0.f;
-    for (int l = tid; l < p.S && l < kMetaSlots; l += kThreads) meta_s[l] = slot_meta(p, l);
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
+    if (tid < 32) {
+        // plane pl, channel group k: slots [G + t0 - G, G + t0 + 128 + G) of that plane
+        for (int i = lane; i < NPL * cg; i += 32)
+            ptx::bulk_g2s(a_base + i * p.rows * 16, p.in + ((size_t)i * g.p + (size_t)t0) * 8, p.rows * 16, &a_bar);
+    }
 
-    if (warp == 9) {
-        // ===================================================== loader (one thread): image chunks + weight pieces
-        if (lane == 0) {
-            if (p.w_resident) {
-                ptx::mbar_arrive_expect_tx(&w_res_bar, (uint32_t)p.nchunks * w_bytes);
-                for (int c = 0; c < p.nchunks; ++c)
-                    ptx::bulk_g2s(smem_base + (uint32_t)c * w_bytes, (const char *)p.w_img + (size_t)c * w_bytes, w_bytes, &w_res_bar);
-            }
-            auto load_img = [&](int macro, int li) {
-                const int buf = li % p.img_bufs;
-                const uint32_t ph = (uint32_t)(li / p.img_bufs) & 1u;
-                ptx::mbar_wait(&img_empty[buf], ph ^ 1u);
-                ptx::mbar_arrive_expect_tx(&img_full[buf], img_bytes);
-                const long long slot0 = (long long)p.G + 128LL * MT * macro - p.halo_lo;
-                const uint32_t dst = img_base + (uint32_t)buf * img_bytes;
-                for (int pl = 0; pl < p.nplanes; ++pl)
-                    for (int kg = 0; kg < p.C / 8; ++kg)
-                        ptx::bulk_g2s(dst + (uint32_t)(pl * (p.C / 8) + kg) * lbo_img,
-                                      (const char *)(p.in + (size_t)pl * p.plane_elems) + ((size_t)kg * p.P + slot0) * 16, lbo_img,
-                                      &img_full[buf]);
-            };
-            int li = 0, w_stage = 0;
-            uint32_t w_phase = 0;
-            if ((int)blockIdx.x < p.n_macro) load_img(blockIdx.x, 0);
-            for (int macro = blockIdx.x; macro < p.n_macro; macro += gridDim.x, ++li) {
-                const int next = macro + gridDim.x;
-                if (p.img_bufs == 2 && next < p.n_macro) load_img(next, li + 1);      // prefetch while this tile computes
-                if (!p.w_resident) {
-                    for (int c = 0; c < p.nchunks; ++c) {
-                        ptx::mbar_wait(&w_empty[w_stage], w_phase ^ 1u);
-                        ptx::mbar_arrive_expect_tx(&w_full[w_stage], w_bytes);
-                        ptx::bulk_g2s(smem_base + (uint32_t)w_stage * w_bytes, (const char *)p.w_img + (size_t)c * w_bytes, w_bytes, &w_full[w_stage]);
-                        if (++w_stage == p.w_stages) { w_stage = 0; w_phase ^= 1u; }
-                    }
-                }
-                if (p.img_bufs == 1 && next < p.n_macro) load_img(next, li + 1);      // single buffer: after this tile's MMAs
-            }
-        }
-    } else if (warp == 8) {
-        // ===================================================== MMA issuer
-        const uint32_t idesc = ptx::umma_idesc_f16(128, (uint32_t)p.N);
-        // per-k-step A-view offsets (descriptor start-address units of 16 B): tap (dh,dw), channel block kk ->
-        // plane (stride 2 only), k-group pair 2*kk, slot shift
-        for (int q = lane; q < p.nksteps; q += 32) {
-            const int tap = q >> p.kpt_shift, kk = q - (tap << p.kpt_shift);
-            const int dh = tap / 3, dw = tap - dh * 3;
-            const int plane = p.nplanes == 4 ? ((dh & 1) * 2 + (dw & 1)) : 0;
-            const int shift = p.nplanes == 4 ? (dh >> 1) * p.Wp + (dw >> 1) : dh * p.Wp + dw;   // slots into the chunk
-            a_off_s[q] = ((uint32_t)(plane * (p.C / 8) + 2 * kk) * lbo_img + (uint32_t)shift * 16u) >> 4;
-        }
-        __syncwarp();
-        const uint64_t a_desc0 = ptx::umma_desc_nosw(0, lbo_img, 128u), w_desc0 = ptx::umma_desc_nosw(0, lbo_w, 128u);
-        const uint32_t a_desc_lo = (uint32_t)a_desc0, a_desc_hi = (uint32_t)(a_desc0 >> 32);
-        const uint32_t w_desc_lo = (uint32_t)w_desc0, w_desc_hi = (uint32_t)(w_desc0 >> 32);
-        const uint32_t b_step = (2u * lbo_w) >> 4;
-        int li = 0, w_stage = 0;
-        uint32_t w_phase = 0;
-        // ONE elected thread runs the whole loop (barrier waits included): no per-chunk elect / reconvergence / warp sync
-        if (ptx::elect_one()) {
-        if (p.w_resident) ptx::mbar_wait(&w_res_bar, 0);
-        for (int macro = blockIdx.x; macro < p.n_macro; macro += gridDim.x, ++li) {
-            const int buf = li % p.img_bufs;
-            const uint32_t iph = (uint32_t)(li / p.img_bufs) & 1u;
-            const int acc = li % p.acc_stages;
-            const uint32_t aph = (uint32_t)(li / p.acc_stages) & 1u;
-            const bool tr = p.trace != nullptr && blockIdx.x == 0 && li < 8;
-            if (tr) p.trace[li * 8 + 0] = clock64();
-            ptx::mbar_wait(&img_full[buf], iph);
-            if (tr) p.trace[li * 8 + 1] = clock64();
-            ptx::mbar_wait(&tmem_empty[acc], aph ^ 1u);
-            ptx::tc_fence_after();
-            if (tr) p.trace[li * 8 + 2] = clock64();
-            const uint32_t img = img_base + (uint32_t)buf * img_bytes;
-            const uint32_t d0 = tmem_base + (uint32_t)(acc * MT * p.N);
-            // The issuing thread is a single in-order instruction stream and tcgen05.mma issue does not run ahead of the tensor
-            // pipe by more than an MMA or so: every integer instruction between two MMAs is tensor-pipe idle time (measured:
-            // 185 cycles per k-step with the tap decode inline, against 49/65/129 cycles per MMA at N = 64/128/256 when the
-            // descriptors are ready).  So: taps unrolled at compile time, descriptors advanced by 32-bit adds on their
-            // start-address field (shared memory < 256 KB: no carry out of the 14 bits), ring stage / phase kept as counters.
-            const uint32_t a_lo = a_desc_lo + (img >> 4);
-            auto acquire_w = [&](int c) -> uint32_t {
-                if (p.w_resident) return smem_base + (uint32_t)c * w_bytes;
-                ptx::mbar_wait(&w_full[w_stage], w_phase);
-                ptx::tc_fence_after();
-                return smem_base + (uint32_t)w_stage * w_bytes;
-            };
-            auto release_w = [&](bool last) {
-                if (!p.w_resident) ptx::umma_commit(&w_empty[w_stage]);
-                if (last) {
-                    ptx::umma_commit(&tmem_full[acc]);
-                    ptx::umma_commit(&img_empty[buf]);
-                }
-            };
-            auto advance_w = [&]() {
-                if (!p.w_resident && ++w_stage == p.w_stages) { w_stage = 0; w_phase ^= 1u; }
-            };
-            if (p.kpt_shift >= 2) {
-                // C >= 64: a chunk (4 k-steps) lies inside one tap
-                const uint32_t kstep_a = (2u * lbo_img) >> 4;
-                int c = 0;
+    float acc[NT][NW / 2];
 #pragma unroll
-                for (int tap = 0; tap < 9; ++tap) {
-                    const int dh = tap / 3, dw = tap % 3;
-                    const uint32_t tap_off =
-                        p.nplanes == 4 ? ((uint32_t)(((dh & 1) * 2 + (dw & 1)) * (p.C / 8)) * lbo_img + (uint32_t)((dh >> 1) * p.Wp + (dw >> 1)) * 16u) >> 4
-                                       : (uint32_t)(dh * p.Wp + dw);
-                    uint32_t a_c = a_lo + tap_off;
-                    for (int kc = 0; kc < p.cpt; ++kc, ++c, a_c += 4u * kstep_a) {
-                        const uint32_t w_addr = acquire_w(c);
-                        const uint32_t b_lo = w_desc_lo + (w_addr >> 4);
+    for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) {
-                            const uint64_t b_desc = ((uint64_t)w_desc_hi << 32) | (uint64_t)(b_lo + (uint32_t)ks * b_step);
+        for (int j = 0; j < NW / 2; ++j) acc[nt][j] = 0.f;
+    ptx::mbar_wait(&a_bar, 0);
+    const uint32_t a_lbo = p.rows * 16;
+    for (int ch = 0; ch < p.nchunks; ++ch) {
+        const int st = ch % kWStages;
+        ptx::mbar_wait(&w_bar[st], (uint32_t)(ch / kWStages) & 1u);
+        ptx::wgmma_fence();
+        // always four k-steps per chunk: the packed weight image is zero past the last real k-group, so the padding steps of
+        // conv1's last chunk add nothing; their A view is clamped onto the last real tap (finite data)
 #pragma unroll
-                            for (int ti = 0; ti < MT; ++ti)
-                                ptx::umma_f16(d0 + (uint32_t)(ti * p.N),
-                                              ((uint64_t)a_desc_hi << 32) | (uint64_t)(a_c + (uint32_t)ks * kstep_a + (uint32_t)(ti * 128)), b_desc, idesc,
-                                              (tap > 0 || ks > 0 || kc > 0) ? 1u : 0u);
-                        }
-                        release_w(tap == 8 && kc + 1 == p.cpt);
-                        advance_w();
-                    }
-                }
+        for (int kk = 0; kk < 4; ++kk) {
+            const int ks = min(ch * 4 + kk, p.nksteps - 1);
+            const int k0 = ks * 16, tap = k0 / p.c, ci = (k0 % p.c) / 8, dh = tap / 3, dw = tap % 3;
+            int pl = 0, off;
+            if (S2) {
+                pl = (dh & 1) * 2 + (dw & 1);
+                off = g.g + (dh >> 1) * g.wp + (dw >> 1);
             } else {
-                // C = 16 (conv1): one k-step per tap, A-view offsets from the table
-                for (int c = 0; c < p.nchunks; ++c) {
-                    const uint32_t w_addr = acquire_w(c);
-                    const uint32_t b_lo = w_desc_lo + (w_addr >> 4);
-#pragma unroll
-                    for (int ks = 0; ks < 4; ++ks) {
-                        const int q = 4 * c + ks;
-                        if (q < p.nksteps) {
-                            const uint32_t ao = a_lo + a_off_s[q];
-                            const uint64_t b_desc = ((uint64_t)w_desc_hi << 32) | (uint64_t)(b_lo + (uint32_t)ks * b_step);
-#pragma unroll
-                            for (int ti = 0; ti < MT; ++ti)
-                                ptx::umma_f16(d0 + (uint32_t)(ti * p.N), ((uint64_t)a_desc_hi << 32) | (uint64_t)(ao + (uint32_t)(ti * 128)), b_desc,
-                                              idesc, q > 0 ? 1u : 0u);
-                        }
-                    }
-                    release_w(c + 1 == p.nchunks);
-                    advance_w();
-                }
+                off = g.g + (dh - 1) * g.wp + (dw - 1);
             }
-            if (tr) p.trace[li * 8 + 3] = clock64();
+            const uint64_t ad = ptx::wgmma_desc(a_base + ((pl * cg + ci) * p.rows + off + wg * 64) * 16, a_lbo, 128);
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt)
+                wgmma_n<N>(acc[nt], ad, ptx::wgmma_desc(w_base + st * W_STAGE + (2 * kk) * N * 16 + nt * 128 * 16, N * 16, 128));
         }
-        }
-        __syncwarp();
-    } else if (warp < 8) {
-        // ===================================================== epilogue: two groups of four warps (one TMEM lane quadrant per
-        // warp), group e takes the 16-column chunks with (chunk & 1) == e; residuals are fetched one chunk ahead
-        const int q = warp & 3;
-        const int eg = warp >> 2;
-        const int r = q * 32 + lane;
-        int li = 0;
-        for (int macro = blockIdx.x; macro < p.n_macro; macro += gridDim.x, ++li) {
-            const int acc = li % p.acc_stages;
-            const uint32_t aph = (uint32_t)(li / p.acc_stages) & 1u;
-            const bool tr = p.trace != nullptr && blockIdx.x == 0 && tid == 128 && li < 8;
-            if (tr) p.trace[li * 8 + 4] = clock64();
-            ptx::mbar_wait(&tmem_full[acc], aph);
-            ptx::tc_fence_after();
-            if (tr) p.trace[li * 8 + 5] = clock64();
-            const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * MT * p.N) + (uint32_t)(16 * eg);
-            const long long g0 = (128LL * MT) * macro + r;
-            if (p.residual) {
-                if (p.out_parity) epilogue_tiles<MT, true, true>(p, tbase, g0, eg, bias_s, meta_s);
-                else epilogue_tiles<MT, true, false>(p, tbase, g0, eg, bias_s, meta_s);
-            } else {
-                if (p.out_parity) epilogue_tiles<MT, false, true>(p, tbase, g0, eg, bias_s, meta_s);
-                else epilogue_tiles<MT, false, false>(p, tbase, g0, eg, bias_s, meta_s);
-            }
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&tmem_empty[acc]);
-            if (tr) p.trace[li * 8 + 6] = clock64();
-        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) ptx::fence_operand(acc[nt]);
+        __syncthreads();                        // both warpgroups are done with the stage
+        if (tid == 0 && ch + kWStages < p.nchunks) issue_w(ch + kWStages);
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 8) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<512>(tmem_base);
+
+    // epilogue: thread rows t0 + 64 wg + 16 w + lane/4 (+ 8)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const long long t = t0 + wg * 64 + 16 * w + (lane >> 2) + 8 * h;
+        if (t >= g.t) continue;
+        const long long b = t / g.s;
+        const int rem = (int)(t - b * g.s), hp = rem / g.wp, wq = rem - hp * g.wp;
+        if (hp < 1 || hp > g.h || wq < 1 || wq > g.w) continue;
+        const size_t slot_off = ((size_t)g.g + (size_t)t) * 8;
+        size_t out_off = slot_off, out_pitch = (size_t)g.p * 8;
+        if (p.par) {
+            const PlanarGeom &n = p.nx;
+            out_off = (size_t)((hp & 1) * 2 + (wq & 1)) * ((size_t)(N / 8) * n.p * 8) +
+                      ((size_t)n.g + (size_t)b * n.s + (size_t)((hp >> 1) + 1) * n.wp + ((wq >> 1) + 1)) * 8;
+            out_pitch = (size_t)n.p * 8;
+        }
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int i = 0; i < NW / 8; ++i) {
+                const int col = nt * NW + 8 * i + 2 * (lane & 3);
+                const float2 bb = *reinterpret_cast<const float2 *>(p.bias + col);
+                float x0 = acc[nt][4 * i + 2 * h] + bb.x, x1 = acc[nt][4 * i + 2 * h + 1] + bb.y;
+                if (p.residual) {
+                    const float2 r = op22f2(*reinterpret_cast<const op2_t *>(p.residual + slot_off + (size_t)(col >> 3) * g.p * 8 + (col & 7)));
+                    x0 += r.x;
+                    x1 += r.y;
+                }
+                if (p.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                *reinterpret_cast<uint32_t *>(p.out + out_off + (size_t)(col >> 3) * out_pitch + (col & 7)) = f2op2_sat(x0, x1);
+            }
     }
 }
+
+template <int N, bool S2>
+int launch(const PconvDev &p, cudaStream_t s) {
+    const int smem = (S2 ? 4 : 1) * (p.c / 8) * (int)p.rows * 16 + kWStages * 8 * N * 16;
+    auto kern = pconv_kernel<N, S2>;
+    C3B_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const unsigned grid = (unsigned)((p.g.t + 127) / 128);
+    c3b_note_grid(grid);
+    kern<<<grid, kThreads, smem, s>>>(p);
+    C3B_CUDA(cudaGetLastError());
+    return 0;
+}
+
+template <int N>
+int launch_n(const PconvDev &p, bool s2, cudaStream_t s) { return s2 ? launch<N, true>(p, s) : launch<N, false>(p, s); }
 
 }  // namespace
 
 int c3b_launch_pconv(const c3b_model *m, const PconvArgs &a, cudaStream_t s) {
-    const PlanarGeom &g = a.geom;
-    const bool c_ok = a.c == 16 || a.c == 64 || a.c == 128 || a.c == 256;
-    if (!c_ok || a.n % 16 || a.n > 256 || a.n < 16) { c3b_set_error("pconv: unsupported channels %d -> %d", a.c, a.n); return 1; }
-    if (g.p * 2 * a.n >= (1LL << 32) || (a.out_parity && a.next.p * 2 * a.n >= (1LL << 32)) || g.t >= (1LL << 31) || (a.out_parity && a.next.s >= (1 << 20))) { c3b_set_error("pconv: batch too large for one launch"); return 1; }
-    PconvDev p = {};
-    p.in = a.in; p.w_img = a.w.w_img; p.bias = a.w.bias; p.residual = a.residual; p.out = a.out;
-    p.C = a.c; p.N = a.n;
-    p.H = g.h; p.W = g.w; p.Wp = g.wp; p.S = g.s; p.G = g.g; p.T = g.t; p.P = g.p;
+    PconvDev p;
+    p.in = a.in;
+    p.w_img = a.w.w_img;
+    p.bias = a.w.bias;
+    p.residual = a.residual;
+    p.out = a.out;
+    p.g = a.geom;
+    p.nx = a.next;
+    p.c = a.c;
     p.relu = a.relu;
-    p.trace = a.trace;
+    p.par = a.out_parity;
     p.nksteps = 9 * a.c / 16;
-    p.nchunks = (p.nksteps + 3) / 4;
-    p.cpt = a.c / 64;
-    p.kpt_shift = a.c == 16 ? 0 : a.c == 64 ? 2 : a.c == 128 ? 3 : 4;
-    p.nplanes = a.stride2 ? 4 : 1;
-    p.plane_elems = (long long)(a.c / 8) * g.p * 8;
-    p.halo_lo = a.stride2 ? 0 : g.wp + 1;
-    p.out_parity = a.out_parity;
-    if (a.out_parity) {
-        p.out_plane_elems = (long long)(a.n / 8) * a.next.p * 8;
-        p.nS = a.next.s; p.nWp = a.next.wp; p.nG = a.next.g; p.nP = a.next.p;
-    }
-    if (p.nchunks != a.w.nchunks) { c3b_set_error("pconv: weight image has %d chunks, expected %d", a.w.nchunks, p.nchunks); return 1; }
-    const size_t budget = 221 * 1024 - 256;      // 227 KB per CTA minus the static barriers, bias and slot tables
-    const size_t w_bytes = (size_t)a.n * 128;
-    const size_t w_all = (size_t)p.nchunks * w_bytes;
-    // Configuration search over MT in {4,2,1}: resident weights when they fit (then small MT only costs halo re-reads and
-    // balances the tile count over the SMs); streamed weights want MT >= 2 (every piece feeds MT accumulators) and a deep
-    // ring, so the image is single-buffered there.  Cost model = rounds of macro-tiles x MMAs per macro-tile.
-    long long best_cost = -1;
-    static const int force_mt = getenv("C3B_PCONV_MT") ? atoi(getenv("C3B_PCONV_MT")) : 0;   // tuning sweeps only
-    for (int mt = (a.n <= 64 ? 4 : 2); mt >= 1; mt >>= 1) {
-        if (mt * a.n > 512) continue;
-        const int n_in = a.stride2 ? (128 * mt + g.wp + 1 + 7) / 8 * 8 : 128 * mt + 2 * (g.wp + 1);
-        const size_t img_bytes = (size_t)p.nplanes * (a.c / 8) * n_in * 16;
-        int resident = 0, bufs = 0, stages = 0;
-        if (w_all + 2 * img_bytes <= budget) { resident = 1; bufs = 2; }
-        else if (w_all + img_bytes <= budget) { resident = 1; bufs = 1; }
-        else if (mt >= 2 || a.n <= 64 || a.stride2) {
-            if (img_bytes + 2 * w_bytes <= budget) { bufs = 1; stages = (int)((budget - img_bytes) / w_bytes); }
-            if (2 * img_bytes + 6 * w_bytes <= budget) { bufs = 2; stages = (int)((budget - 2 * img_bytes) / w_bytes); }
-            if (!bufs) continue;
-        } else continue;
-        const long long n_macro = (g.t + 128LL * mt - 1) / (128LL * mt);
-        const long long rounds = (n_macro + m->sm_count - 1) / m->sm_count;
-        // + a fixed per-macro-tile cost: measured, MT = 1 is 1.2-1.5x slower than MT = 2/4 on every level even with resident
-        // weights (each macro-tile pays an image-chunk round trip that only several tiles of MMAs hide)
-        long long cost = rounds * mt * 100 + rounds * 60 + (bufs == 1 ? rounds * 12 : 0) + (resident ? 0 : 5);
-        if (force_mt > 0) cost = (mt == force_mt) ? 1 : 1000000 + cost;
-        if (best_cost < 0 || cost < best_cost) {
-            best_cost = cost;
-            p.MT = mt; p.n_in = n_in; p.w_resident = resident; p.img_bufs = bufs; p.w_stages = stages;
-            p.acc_stages = (mt * a.n * 2 <= 512) ? 2 : 1;
-        }
-    }
-    if (best_cost < 0) { c3b_set_error("pconv: feature map does not fit shared memory"); return 1; }
-    static const bool dbg = getenv("C3B_DEBUG_PCONV") != nullptr;
-    if (dbg)
-        fprintf(stderr, "[pconv] C=%d N=%d stride2=%d T=%lld: MT=%d resident=%d img_bufs=%d w_stages=%d cost=%lld\n", a.c, a.n, a.stride2,
-                (long long)g.t, p.MT, p.w_resident, p.img_bufs, p.w_stages, best_cost);
-    if (p.w_stages > kMaxWStages) p.w_stages = kMaxWStages;
-    const long long per_macro = 128LL * p.MT;
-    p.n_macro = (int)((g.t + per_macro - 1) / per_macro);
-    if ((long long)p.n_macro * per_macro + g.g > g.p - g.g + per_macro) { /* plane pitch covers the rounded-up slot range by construction */ }
-    const size_t img_bytes = (size_t)p.nplanes * (a.c / 8) * p.n_in * 16;
-    const size_t smem = (p.w_resident ? (size_t)p.nchunks * w_bytes : (size_t)p.w_stages * w_bytes) + p.img_bufs * img_bytes + 256;
-    const int grid = p.n_macro < m->sm_count ? p.n_macro : m->sm_count;
+    p.nchunks = a.w.nchunks;
+    p.rows = 128 + 2 * (uint32_t)a.geom.g;
+    if (a.c % 16 != 0 || a.w.n != a.n) { c3b_set_error("pconv: channels %d / %d not supported", a.c, a.n); return 1; }
     const_cast<c3b_model *>(m)->launches++;
-    c3b_note_grid(grid);
-    switch (p.MT) {
-        case 1:
-            C3B_CUDA(cudaFuncSetAttribute(pconv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024));
-            pconv_kernel<1><<<grid, kThreads, smem, s>>>(p);
-            break;
-        case 2:
-            C3B_CUDA(cudaFuncSetAttribute(pconv_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024));
-            pconv_kernel<2><<<grid, kThreads, smem, s>>>(p);
-            break;
-        case 4:
-            C3B_CUDA(cudaFuncSetAttribute(pconv_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024));
-            pconv_kernel<4><<<grid, kThreads, smem, s>>>(p);
-            break;
-        default: c3b_set_error("pconv: unsupported MT %d", p.MT); return 1;
+    switch (a.n) {
+        case 64: return launch_n<64>(p, a.stride2 != 0, s);
+        case 128: return launch_n<128>(p, a.stride2 != 0, s);
+        case 256: return launch_n<256>(p, a.stride2 != 0, s);
     }
-    C3B_CUDA(cudaGetLastError());
-    return 0;
+    c3b_set_error("pconv: unsupported output channels %d", a.n);
+    return 1;
 }

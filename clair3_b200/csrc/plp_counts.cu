@@ -1,7 +1,7 @@
 // plp_counts.cu - the pileup feature counter on the GPU (include/clair3_b200_pileup.h; SURVEY.md 8f row N4, pileup half).
 //
 // Reference: calculate_clair3_pileup(), HKU-BAL/Clair3 src/clair3_pileup.c:142-476 - a column-by-column loop over htslib's
-// bam_mplp_auto() with one incremental CIGAR cursor per read.  Here the work is turned around for a machine with 148 SMs and no
+// bam_mplp_auto() with one incremental CIGAR cursor per read.  Here the work is turned around for a machine with 132 SMs and no
 // cheap serial cursor:
 //
 //   K1 plp_scan_reads    one warp per read: read filter (src/medaka_bamiter.c:21-24) and a warp prefix sum over its CIGAR words ->
@@ -284,10 +284,7 @@ __device__ __forceinline__ bool plp_visit(const CountArgs &A, int32_t *cnt, cons
     return true;
 }
 
-// Measured alternatives that did NOT pay (1,048,576 columns, depth 40, all bit-exact; profiles/r2_plp_ab.md): resolving 2 / 4 reads
-// side by side (1.106 / 1.386 ms against 1.109: the extra registers cost occupancy), a fixed-trip branch-free search (0.934 ms
-// against 0.894) and batching the indel bookkeeping across the warp until six lanes have an allele pending (0.903 ms).  What did
-// pay: per-warp instead of per-tile read ranges and six CTAs per SM (1.109 -> 0.894 ms).
+// Per-warp read ranges and six CTAs per SM keep enough reads in flight to hide the per-read CIGAR searches.
 __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     int32_t *cnt = reinterpret_cast<int32_t *>(smem_raw);                       // [NCNT][TILE]
@@ -650,8 +647,8 @@ int c3b_plp_create(c3b_plp **out, int device_ordinal) {
     if (device_ordinal < 0 || device_ordinal >= ndev) { c3b_set_error("bad device ordinal %d", device_ordinal); return 1; }
     cudaDeviceProp prop;
     C3B_CUDA(cudaGetDeviceProperties(&prop, device_ordinal));
-    if (prop.major != 10) {
-        c3b_set_error("device %d is sm_%d%d; this library contains only sm_100a code", device_ordinal, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        c3b_set_error("device %d is sm_%d%d; this library contains only sm_90a code", device_ordinal, prop.major, prop.minor);
         return 1;
     }
     C3B_CUDA(cudaSetDevice(device_ordinal));
@@ -757,7 +754,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     if (W > 0) {
         if (n > 0) {
             int blocks = (int)((n * 32 + 255) / 256);
-            if (blocks > 148 * 8) blocks = 148 * 8;
+            if (blocks > 132 * 8) blocks = 132 * 8;
             plp_scan_reads_kernel<<<blocks, 256, 0, s>>>(R, params->min_mq, w->opx.as<int32_t>(), w->opy.as<int32_t>(), w->rend.as<int64_t>(), status);
             plp_prefix_max_kernel<<<1, 1024, 0, s>>>(w->rend.as<int64_t>(), w->pmax.as<int64_t>(), n);
             w->launches += 2;

@@ -1,242 +1,81 @@
-// LSTM2 input projection of Clair3_P (the W_ih half of nn.LSTM's gate GEMM, clair3/model.py:102-107,133) on tcgen05:
+// LSTM2's input projection (clair3/model.py:132-133 -> torch nn.LSTM's W_ih x_t + b_ih + b_hh, both directions) as one
+// warpgroup-MMA GEMM over every time step at once:
 //
-//   pg[pos][R] = sum_k h1[pos][k] * W_ih[R][k] + (b_ih + b_hh)[R]        pos = t*Bp + b (33*Bp rows), R = 1280 permuted gate rows, K = 256
+//   pg[t*bp + b][col] = sum_k h1[t*bp + b][k] * Wp[col][k] + bias[col]      col = dir*640 + R (c3b_lstm_row order), K = 256
 //
-// Orientation: the 128 positions of a tile sit on the TMEM lanes (A operand = k-group-planar h1, eight contiguous 2 KB runs per
-// 64-wide k-chunk -> cp.async.bulk), a 256-column slab of W_ih is the B operand and stays resident in shared memory for the
-// CTA's whole life (128 KB; five column groups x up to 29 CTAs).  Why this way round (round 1 had the weights on the lanes, two
-// 128-row blocks per tile): a 128 x 256 x 16 MMA is math-bound (128 cycles for 96 shared-memory wavefronts), so a quarter of the
-// shared-memory pipe is left for the epilogue, while the 128 x 128 x 16 MMAs of the old orientation saturate it (64 wavefronts in
-// 64 cycles) and every epilogue store stalls the tensor pipe (measured: 4.1 k epilogue + 2.8 k MMA cycles per tile, serialised).
-//
-// Output layout = what the recurrent kernel reads (lstm_tc.cu): pgT[dir][t][sub-tile][blk 0..4][row 0..127][NBL sites] fp16.
-// An epilogue thread owns one position (site) and walks 128 gate rows: element (row, site) is a 2-byte store, and the 32 lanes
-// of a warp (32 consecutive sites = one or two sub-tiles) write 64 contiguous bytes per instruction - one LSU wavefront per
-// instruction, no shared-memory transposition (which would cost twice the wavefronts).
-//
-// Roles (320 threads): warps 0-7 epilogue (two warpgroups: lane quadrant = warp & 3, column half = warp >> 2), warp 8 issues
-// tcgen05.mma (one elected thread for the whole loop), warp 9 loads (resident slab once, then the activation ring).
-#include <cstdlib>
-
+// One CTA = 128 rows x 128 columns; the whole K fits in shared memory, so the operands arrive with five cp.async.bulk copies
+// (the tile-major h1 tile is one 64 KB run, the weight slab four 16 KB runs) and two warpgroups each issue 16 m64n128k16 MMAs.
+// fp16 output: the recurrent kernel adds these pre-gates to its fp32 accumulators.
 #include "c3b_internal.h"
 #include "ptx.cuh"
 
 namespace {
 
-constexpr int kThreads = 320;
-constexpr int kStages = 5;                      // activation ring: 16 KB per stage (128 positions x 64 k)
-constexpr uint32_t kStageBytes = 8 * 2048;
-constexpr uint32_t kSlabBytes = 4 * 8 * 4096;   // 256 weight rows x K = 256: 4 chunks x 8 k-groups x 4 KB
+constexpr int kThreads = 256;
+constexpr uint32_t kTileBytes = 32 * 128 * 16;      // [32 k-groups][128 rows][8] fp16
 
 struct ProjDev {
-    const op_t *act;        // h1, tile-major k-group-planar [ld_rows/128][32][128][8]
-    const op_t *w_img;      // [chunk 4][group 5][8 kg][256 rows][8]
-    const float *bias;      // [1280]
-    __half *out;            // pgT
-    long long ld_rows;      // 33 * bp
-    int n_tiles;            // ld_rows / 128
-    int bp;
-    long long *trace;
+    const op_t *h1;            // tile-major [33*bp/128][32][128][8]
+    const op_t *w;             // [4 chunks][10 column blocks][8][128][8]
+    const float *bias;         // [1280]
+    __half *pg;                // [33*bp][1280]
 };
 
-// NBL > 0: pgT layout for the round-1 recurrent kernel with NBL-site sub-tiles (2-byte stores, 64 contiguous bytes per warp
-// instruction); NBL == 0: pg2 layout for the CTA-pair kernel (lstm2x_tc.cu): [dir][t][128-site tile][80 column groups][128][8],
-// two 16-byte stores per 16 columns, 512 contiguous bytes per warp instruction.
-template <int NBL>
 __global__ void __launch_bounds__(kThreads, 1) proj2_kernel(const ProjDev p) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t full_bar[kStages], empty_bar[kStages], tmem_full[2], tmem_empty[2], w_bar;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ __align__(16) float bias_s[256];
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int group = blockIdx.x % 5;                 // which 256-column slab of the 1280 gate rows
-    const int at0 = blockIdx.x / 5, at_step = gridDim.x / 5;
-    const uint32_t slab = ptx::smem_u32(smem);
-    const uint32_t ring = slab + kSlabBytes;
-
+    __shared__ uint64_t bar;
+    const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31;
+    const int tile = blockIdx.x, cb = blockIdx.y;
+    const uint32_t a_addr = ptx::smem_u32(smem), b_addr = a_addr + kTileBytes;
     if (tid == 0) {
-        for (int s = 0; s < kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-        for (int a = 0; a < 2; ++a) { ptx::mbar_init(&tmem_full[a], 1); ptx::mbar_init(&tmem_empty[a], 256); }
-        ptx::mbar_init(&w_bar, 1);
+        ptx::mbar_init(&bar, 1);
         ptx::fence_barrier_init();
+        ptx::mbar_arrive_expect_tx(&bar, 2 * kTileBytes);
+        ptx::bulk_g2s(a_addr, p.h1 + (size_t)tile * (kTileBytes / 2), kTileBytes, &bar);
+        for (int c = 0; c < 4; ++c)
+            ptx::bulk_g2s(b_addr + c * (kTileBytes / 4), p.w + ((size_t)c * 10 + cb) * (kTileBytes / 8), kTileBytes / 4, &bar);
     }
-    if (warp == 8) ptx::tmem_alloc<512>(&tmem_base_smem);
-    for (int i = tid; i < 256; i += kThreads) bias_s[i] = p.bias[group * 256 + i];
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
+    ptx::mbar_wait(&bar, 0);
 
-    if (warp == 9) {
-        // ===================================================== loader
-        if (lane == 0) {
-            ptx::mbar_arrive_expect_tx(&w_bar, kSlabBytes);
-            for (int c = 0; c < 4; ++c)
-                ptx::bulk_g2s(slab + (uint32_t)c * 32768u, (const char *)p.w_img + ((size_t)c * 5 + group) * 32768u, 32768u, &w_bar);
-        }
-        // h1 is tile-major: the 64-wide k-chunk c of position tile `at` is one contiguous 16 KB run
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            for (int at = at0; at < p.n_tiles; at += at_step) {
-                const char *src = (const char *)p.act + (size_t)at * (32 * 2048);
-                for (int c = 0; c < 4; ++c, src += kStageBytes) {
-                    ptx::mbar_wait(&empty_bar[s], ph ^ 1u);
-                    ptx::mbar_arrive_expect_tx(&full_bar[s], kStageBytes);
-                    ptx::bulk_g2s(ring + (uint32_t)s * kStageBytes, src, kStageBytes, &full_bar[s]);
-                    if (++s == kStages) { s = 0; ph ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == 8) {
-        // ===================================================== MMA issuer: one elected thread, descriptors advanced by 32-bit adds
-        if (ptx::elect_one()) {
-            const uint32_t idesc = ptx::umma_idesc_f16(128, 256);
-            const uint64_t a_d0 = ptx::umma_desc_nosw(0, 2048u, 128u), b_d0 = ptx::umma_desc_nosw(0, 4096u, 128u);
-            const uint32_t a_lo0 = (uint32_t)a_d0, a_hi = (uint32_t)(a_d0 >> 32);
-            const uint32_t b_lo0 = (uint32_t)b_d0 + (slab >> 4), b_hi = (uint32_t)(b_d0 >> 32);
-            constexpr uint32_t a_kstep = (2u * 2048u) >> 4, b_kstep = (2u * 4096u) >> 4, b_cstep = 32768u >> 4;
-            int s = 0, tcount = 0;
-            uint32_t ph = 0;
-            ptx::mbar_wait(&w_bar, 0);
-            for (int at = at0; at < p.n_tiles; at += at_step, ++tcount) {
-                const int acc = tcount & 1;
-                const uint32_t acc_ph = (uint32_t)(tcount >> 1) & 1u;
-                const bool tr = p.trace != nullptr && blockIdx.x == 0 && tcount < 8;
-                if (tr) p.trace[tcount * 8 + 0] = clock64();
-                ptx::mbar_wait(&tmem_empty[acc], acc_ph ^ 1u);
-                ptx::tc_fence_after();
-                if (tr) p.trace[tcount * 8 + 1] = clock64();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 256);
+    float acc[64];
+    ptx::wgmma_fence();
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    ptx::mbar_wait(&full_bar[s], ph);
-                    ptx::tc_fence_after();
-                    if (tr && c == 0) p.trace[tcount * 8 + 2] = clock64();
-                    const uint32_t a_lo = a_lo0 + ((ring + (uint32_t)s * kStageBytes) >> 4);
-                    const uint32_t b_lo = b_lo0 + (uint32_t)c * b_cstep;
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        ptx::umma_f16(d_tmem, ((uint64_t)a_hi << 32) | (uint64_t)(a_lo + (uint32_t)k * a_kstep),
-                                      ((uint64_t)b_hi << 32) | (uint64_t)(b_lo + (uint32_t)k * b_kstep), idesc, (c > 0 || k > 0) ? 1u : 0u);
-                    ptx::umma_commit(&empty_bar[s]);
-                    if (c == 3) ptx::umma_commit(&tmem_full[acc]);
-                    if (++s == kStages) { s = 0; ph ^= 1u; }
-                }
-                if (tr) p.trace[tcount * 8 + 3] = clock64();
-            }
-        }
-        __syncwarp();
-    } else {
-        // ===================================================== epilogue: thread = position (site), 128 gate rows of one (dir, blk)
-        const int q = warp & 3, g = warp >> 2;
-        const int R0 = group * 256 + g * 128;                 // first permuted gate row of this half: one direction, 128 rows
-        const int dir = R0 / 640, blk = (R0 % 640) >> 7;
-        constexpr int NB1 = NBL > 0 ? NBL : 1;
-        const int ntl = p.bp / NB1;
-        const float4 *b4 = reinterpret_cast<const float4 *>(bias_s + g * 128);
-        int tcount = 0;
-        for (int at = at0; at < p.n_tiles; at += at_step, ++tcount) {
-            const int acc = tcount & 1;
-            const uint32_t acc_ph = (uint32_t)(tcount >> 1) & 1u;
-            const long long pos0 = (long long)at * 128;
-            const int t = (int)(pos0 / p.bp);
-            const int b = (int)(pos0 % p.bp) + q * 32 + lane;     // site index in the padded batch
-            __half *dst = NBL > 0 ? p.out + ((((size_t)(dir * C3B_T + t) * ntl + b / NB1) * 5 + blk) * 128) * NB1 + b % NB1
-                                  : p.out + ((((size_t)(dir * C3B_T + t) * (p.bp >> 7) + (b >> 7)) * 80 + (size_t)blk * 16) * 128 + (b & 127)) * 8;
-            const bool tr = p.trace != nullptr && blockIdx.x == 0 && tid == 0 && tcount < 8;
-            if (tr) p.trace[tcount * 8 + 4] = clock64();
-            ptx::mbar_wait(&tmem_full[acc], acc_ph);
-            ptx::tc_fence_after();
-            if (tr) p.trace[tcount * 8 + 5] = clock64();
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 256 + g * 128);
-            float v0[16], v1[16];
-            ptx::tmem_ld16(taddr, v0);
-            auto emit = [&](const float *v, int ch) {          // 16 gate columns ch*16 .. +16 of this half
-                if (NBL > 0) {
-#pragma unroll
-                    for (int i4 = 0; i4 < 4; ++i4) {
-                        const float4 bb = b4[ch * 4 + i4];
-                        __half *d = dst + (size_t)(ch * 16 + i4 * 4) * NB1;
-                        d[0 * NB1] = f2op(v[i4 * 4 + 0] + bb.x);
-                        d[1 * NB1] = f2op(v[i4 * 4 + 1] + bb.y);
-                        d[2 * NB1] = f2op(v[i4 * 4 + 2] + bb.z);
-                        d[3 * NB1] = f2op(v[i4 * 4 + 3] + bb.w);
-                    }
-                } else {
-                    uint4 pk[2];
-                    uint32_t *pw = reinterpret_cast<uint32_t *>(pk);
-#pragma unroll
-                    for (int i4 = 0; i4 < 4; ++i4) {
-                        const float4 bb = b4[ch * 4 + i4];
-                        pw[2 * i4] = f2op2_sat(v[i4 * 4 + 0] + bb.x, v[i4 * 4 + 1] + bb.y);
-                        pw[2 * i4 + 1] = f2op2_sat(v[i4 * 4 + 2] + bb.z, v[i4 * 4 + 3] + bb.w);
-                    }
-                    *reinterpret_cast<uint4 *>(dst + (size_t)(2 * ch) * 128 * 8) = pk[0];
-                    *reinterpret_cast<uint4 *>(dst + (size_t)(2 * ch + 1) * 128 * 8) = pk[1];
-                }
-            };
-#pragma unroll
-            for (int ch = 0; ch < 8; ch += 2) {
-                ptx::tmem_ld_wait();
-                ptx::tmem_ld16(taddr + (uint32_t)(16 * (ch + 1)), v1);
-                emit(v0, ch);
-                ptx::tmem_ld_wait();
-                if (ch + 2 < 8) ptx::tmem_ld16(taddr + (uint32_t)(16 * (ch + 2)), v0);
-                emit(v1, ch + 1);
-            }
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&tmem_empty[acc]);
-            if (tr) p.trace[tcount * 8 + 6] = clock64();
-        }
+    for (int ks = 0; ks < 16; ++ks) {
+        const uint64_t ad = ptx::wgmma_desc(a_addr + wg * 64 * 16 + ks * 2 * 2048, 2048, 128);
+        const uint64_t bd = ptx::wgmma_desc(b_addr + ks * 2 * 2048, 2048, 128);
+        ptx::wgmma_m64n128k16(acc, ad, bd, ks > 0);
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 8) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<512>(tmem_base);
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_operand(acc);
+
+    const size_t row0 = (size_t)tile * 128 + wg * 64 + 16 * w + (lane >> 2);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+        const int col = cb * 128 + 8 * i + 2 * (lane & 3);
+        const float2 bb = *reinterpret_cast<const float2 *>(p.bias + col);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+            *reinterpret_cast<__half2 *>(p.pg + (row0 + 8 * h) * 1280 + col) =
+                __floats2half2_rn(acc[4 * i + 2 * h] + bb.x, acc[4 * i + 2 * h + 1] + bb.y);
     }
 }
 
 }  // namespace
 
-// h1: k-group-planar [32][33*bp][8]; w_img: pack_igemm(1280, 32, 256) image; pg: pgT for LSTM2 sub-tiles of `nbl` sites
-// nbl = 16 | 32: pgT for the round-1 recurrent kernel; nbl = 0: pg2 for the CTA-pair kernel
-int c3b_launch_proj2(const c3b_model *m, const op_t *h1, const IgemmW &w, __half *pg, int bp, int nbl, bool latency, long long *trace,
-                     cudaStream_t s) {
-    if (bp % 128 || (nbl != 0 && nbl != 16 && nbl != 32)) { c3b_set_error("proj2: bad geometry bp=%d nbl=%d", bp, nbl); return 1; }
-    ProjDev p = {};
-    p.act = h1; p.w_img = w.w_img; p.bias = w.bias; p.out = pg;
-    p.ld_rows = (long long)C3B_T * bp;
-    p.n_tiles = (int)(p.ld_rows / 128);
-    p.bp = bp;
-    p.trace = trace;
-    // The kernel is bound by the write of its output (86 MB of pre-gates per 1024 sites): ~3.2 TB/s of HBM writes with 145 CTAs
-    // (31 us), and ~16 B/clk of store bandwidth per SM with fewer (60 CTAs: 63 us) - its SM-time is ~4 ms per launch either way,
-    // so 16 CTAs per column group trade a little latency for SMs the recurrent kernels of the other in-flight batches can use.
-    // Handing the output to the TMA engine instead (8 KB pieces staged in shared memory, cp.async.bulk shared -> global) was
-    // measured slower: 55 us against 45 us at 80 CTAs, 79 us at 50, 36 us at 145 - the ~13 B/clk per SM is not an LSU limit.
-    // (C3B_PROJ_CTAS: tuning sweeps only.)
-    static const int per_env = getenv("C3B_PROJ_CTAS") ? atoi(getenv("C3B_PROJ_CTAS")) : 0;
-    int per = per_env > 0 ? per_env : latency ? m->sm_count / 5 : 16;       // one batch in flight: every SM (32 us instead of 45)
-    if (per > m->sm_count / 5) per = m->sm_count / 5;
-    if (per > p.n_tiles) per = p.n_tiles;
-    if (per < 1) per = 1;
-    const int grid = 5 * per;
-    const size_t smem = kSlabBytes + kStages * kStageBytes + 128;
-    const_cast<c3b_model *>(m)->launches++;
-    c3b_note_grid(grid);
-    if (nbl == 32) {
-        C3B_CUDA(cudaFuncSetAttribute(proj2_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        proj2_kernel<32><<<grid, kThreads, smem, s>>>(p);
-    } else if (nbl == 16) {
-        C3B_CUDA(cudaFuncSetAttribute(proj2_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        proj2_kernel<16><<<grid, kThreads, smem, s>>>(p);
-    } else {
-        C3B_CUDA(cudaFuncSetAttribute(proj2_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        proj2_kernel<0><<<grid, kThreads, smem, s>>>(p);
-    }
+int c3b_launch_proj2(const c3b_model *m, const op_t *h1, const IgemmW &w, __half *pg, int bp, cudaStream_t s) {
+    ProjDev p;
+    p.h1 = h1;
+    p.w = w.w_img;
+    p.bias = w.bias;
+    p.pg = pg;
+    const int smem = 2 * kTileBytes;
+    C3B_CUDA(cudaFuncSetAttribute(proj2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    dim3 grid((unsigned)(C3B_T * (int64_t)bp / 128), 10);
+    c3b_note_grid((long long)grid.x * grid.y);
+    proj2_kernel<<<grid, kThreads, smem, s>>>(p);
     C3B_CUDA(cudaGetLastError());
+    const_cast<c3b_model *>(m)->launches++;
     return 0;
 }

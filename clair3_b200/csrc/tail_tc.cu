@@ -1,295 +1,128 @@
-// The dense tail of both networks as ONE tcgen05 kernel (clair3/model.py:136-159 pileup, :391-411 full-alignment):
+// The dense tail of both networks (clair3/model.py:136-159 pileup, :391-411 full-alignment):
 //
 //   a4 = SELU(L4 . x + b4)                         x = flattened LSTM2 output [10560] / pyramid-pooled features [3584]
 //   per head k:  a5 = SELU(L5_k . a4 + b5_k) ; y_k = softmax(SELU(Y_k . a5 + by_k)) ; out = cat(y_k)
 //
-// One CTA owns 128 candidate sites (TMEM lanes) for the whole chain:
-//   phase 1  L4 as a full-K GEMM (no split-K, no partial sums in HBM): the loader warp streams 64-wide k-chunks of the
-//            k-group-planar activations (eight 2 KB runs) and of the host-packed L4 operand image through a shared-memory ring
-//            with cp.async.bulk; one elected thread issues 128 x d4 x 16 MMAs into TMEM columns [0, d4).
-//   phase 2  thread = site.  bias + SELU on the accumulator row -> fp16 A-operand image a4 in shared memory (the ring's memory,
-//            free by now) -> per head: L5_k MMAs (N = 128, K = d4, weights bulk-copied while the previous head's epilogue runs)
-//            -> bias + SELU -> a5 operand image -> Y_k MMAs (N = 16|32|48, K = 128) -> bias + SELU + softmax in registers ->
-//            global store of the site's probabilities.
-// Replaces round 1's split-K L4 launch (40 CTAs whose time was pipeline fill) + fp32 CUDA-core heads kernel (64 blocks
-// streaming the same L5 weights): 13 % of the pileup SM-time.  Everything after the L4 accumulator stays on chip.
+// L4 carries almost all of the tail's FLOPs and runs on warpgroup MMAs: one CTA owns 128 candidate sites (two warpgroups of 64
+// rows, N = d4) and one split of K; 64-wide k-chunks of the tile-major activations (one 16 KB run) and of the host-packed L4
+// operand image (one d4 x 128 B run) stream through a three-stage shared-memory ring with cp.async.bulk.  Split-K keeps the
+// GPU busy at a few hundred sites; the fp32 partial sums [nsplit][bp][d4] go to the heads kernel (kernels_common.cu), which
+// adds them in a fixed order with the bias and runs SELU, the per-head layers and the softmax.
+#include <algorithm>
+
 #include "c3b_internal.h"
 #include "ptx.cuh"
 
 namespace {
 
-constexpr int kThreads = 320;                 // warps 0-7 epilogue (thread = site, two warpgroups split the columns), warp 8 MMA, warp 9 loader
-constexpr float kSeluAlpha = 1.6732632423543772f;
-constexpr float kSeluScale = 1.0507009873554805f;
-// SELU with the hardware exponential: the result is rounded to fp16 (operand images) or fed to a softmax right after, so the
-// ~1e-7 absolute error of exp(x) - 1 near zero is far below what survives; expm1f costs ~40 instructions per element.
-__device__ __forceinline__ float selu(float x) { return kSeluScale * (x > 0.f ? x : kSeluAlpha * (__expf(x) - 1.f)); }
+constexpr int kThreads = 256;
+constexpr int kStages = 3;
+constexpr int kMaxSplit = 16;                  // the heads kernel sums at most 16 partials
 
-struct TailDev {
-    const op_t *act;          // tile-major k-group-planar [bp/128][K/8][128][8]
-    const op_t *w4;           // [nchunks][8 kg][d4 rows][8]
-    const float *b4;          // [d4]
-    const op_t *w5[C3B_MAX_HEADS];    // per head [d4/8 kg][128 rows][8]
-    const float *b5[C3B_MAX_HEADS];   // [128]
-    const op_t *wy[C3B_MAX_HEADS];    // per head [16 kg][npad rows][8]
-    const float *by[C3B_MAX_HEADS];   // [npad] (zero padded)
-    int n[C3B_MAX_HEADS], npad[C3B_MAX_HEADS], off[C3B_MAX_HEADS];
-    float *out;               // [batch][out_dim]
-    float *z4_tap;            // optional [bp][d4] fp32 L4 pre-activation without bias (debug option "taps")
-    long long batch;
-    int bp, nchunks, nheads, out_dim, stages;
+struct L4Dev {
+    const op_t *act;          // tile-major k-group-planar [bp/128][KG][128][8]
+    const op_t *w4;           // [KG][d4 rows][8]
+    float *z4;                // [nsplit][bp][d4] partial sums, no bias
+    int kg, bp, chunks_per_split, nchunks;
 };
 
 template <int D4>
-__global__ void __launch_bounds__(kThreads, 1) tail_kernel(const TailDev p) {
-    constexpr uint32_t kActBytes = 8 * 2048;              // 128 sites x 64 k
-    constexpr uint32_t kW4Bytes = D4 * 128;               // d4 rows x 64 k
-    constexpr uint32_t kStageBytes = kActBytes + kW4Bytes;
-    constexpr uint32_t kA4Bytes = (D4 / 8) * 2048;        // phase 2 operand images
-    constexpr uint32_t kW5Bytes = (D4 / 8) * 2048;        // 128 rows x d4
-    constexpr uint32_t kA5Bytes = 16 * 2048;
-    constexpr uint32_t kWyMax = 16 * 48 * 16;             // up to 48 rows x 128 k
-    constexpr uint32_t L5_COL = 256, Y_COL = 384;
-
+__global__ void __launch_bounds__(kThreads, 1) l4_kernel(const L4Dev p) {
+    constexpr int NT = D4 / 128;
+    constexpr uint32_t A_BYTES = 8 * 128 * 16, B_BYTES = 8 * D4 * 16, STAGE = A_BYTES + B_BYTES;
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t full_bar[8], empty_bar[8], l4_done, a4_ready, w5_full, wy_full, l5_done, a5_ready, y_done;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ __align__(16) float b4_s[D4];
-    __shared__ __align__(16) float b5_s[C3B_MAX_HEADS][128];
-    __shared__ __align__(16) float by_s[C3B_MAX_HEADS][48];
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int at = blockIdx.x;
+    __shared__ uint64_t full[kStages];
+    const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31;
+    const int tile = blockIdx.x, split = blockIdx.y;
+    const int c0 = split * p.chunks_per_split;
+    const int nc = min(p.chunks_per_split, p.nchunks - c0);
     const uint32_t base = ptx::smem_u32(smem);
-    const uint32_t a4_addr = base, w5_addr = base + kA4Bytes, a5_addr = w5_addr + kW5Bytes, wy_addr = a5_addr + kA5Bytes;
-    const int S = p.stages;
+    const op_t *a_src = p.act + (size_t)tile * p.kg * 128 * 8;
 
+    auto issue = [&](int i) {                   // chunk c0 + i -> stage i % kStages (thread 0)
+        const int st = i % kStages, c = c0 + i;
+        ptx::mbar_arrive_expect_tx(&full[st], STAGE);
+        ptx::bulk_g2s(base + st * STAGE, a_src + (size_t)c * 8 * 128 * 8, A_BYTES, &full[st]);
+        ptx::bulk_g2s(base + st * STAGE + A_BYTES, p.w4 + (size_t)c * 8 * D4 * 8, B_BYTES, &full[st]);
+    };
     if (tid == 0) {
-        for (int s = 0; s < 8; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-        ptx::mbar_init(&l4_done, 1);
-        ptx::mbar_init(&a4_ready, 256);
-        ptx::mbar_init(&w5_full, 1);
-        ptx::mbar_init(&wy_full, 1);
-        ptx::mbar_init(&l5_done, 1);
-        ptx::mbar_init(&a5_ready, 256);
-        ptx::mbar_init(&y_done, 1);
+        for (int s = 0; s < kStages; ++s) ptx::mbar_init(&full[s], 1);
         ptx::fence_barrier_init();
+        for (int i = 0; i < kStages && i < nc; ++i) issue(i);
     }
-    if (warp == 8) ptx::tmem_alloc<512>(&tmem_base_smem);
-    for (int i = tid; i < D4; i += kThreads) b4_s[i] = p.b4[i];
-    for (int i = tid; i < p.nheads * 128; i += kThreads) b5_s[i >> 7][i & 127] = p.b5[i >> 7][i & 127];
-    for (int i = tid; i < p.nheads * 48; i += kThreads) by_s[i / 48][i % 48] = (i % 48) < p.npad[i / 48] ? p.by[i / 48][i % 48] : 0.f;
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
 
-    if (warp == 9) {
-        // ===================================================== loader
-        // activations are tile-major: k-chunk c of this CTA's 128-site tile is one contiguous 16 KB run
-        if (lane == 0) {
-            const char *src = (const char *)p.act + (size_t)at * ((size_t)p.nchunks * kActBytes);
-            int s = 0;
-            uint32_t ph = 0;
-            for (int c = 0; c < p.nchunks; ++c, src += kActBytes) {
-                ptx::mbar_wait(&empty_bar[s], ph ^ 1u);
-                const uint32_t stage = base + (uint32_t)s * kStageBytes;
-                ptx::mbar_arrive_expect_tx(&full_bar[s], kStageBytes);
-                ptx::bulk_g2s(stage, src, kActBytes, &full_bar[s]);
-                ptx::bulk_g2s(stage + kActBytes, (const char *)p.w4 + (size_t)c * kW4Bytes, kW4Bytes, &full_bar[s]);
-                if (++s == S) { s = 0; ph ^= 1u; }
-            }
+    float acc[NT][64];
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int j = 0; j < 64; ++j) acc[nt][j] = 0.f;
+    for (int i = 0; i < nc; ++i) {
+        const int st = i % kStages;
+        ptx::mbar_wait(&full[st], (uint32_t)(i / kStages) & 1u);
+        const uint32_t a_addr = base + st * STAGE, b_addr = a_addr + A_BYTES;
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+            const uint64_t ad = ptx::wgmma_desc(a_addr + wg * 64 * 16 + ks * 2 * 2048, 2048, 128);
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt)
+                ptx::wgmma_m64n128k16(acc[nt], ad, ptx::wgmma_desc(b_addr + nt * 128 * 16 + ks * 2 * D4 * 16, D4 * 16, 128), 1);
         }
-        if (lane == 0) {
-            // phase 2 weights land in the ring's memory: wait until every L4 MMA has read its operands
-            ptx::mbar_wait(&l4_done, 0);
-            uint32_t wy_bytes = 0;
-            for (int h = 0; h < p.nheads; ++h) wy_bytes += (uint32_t)p.npad[h] * 256u;
-            ptx::mbar_arrive_expect_tx(&wy_full, wy_bytes);
-            uint32_t wo = 0;
-            for (int h = 0; h < p.nheads; ++h) {
-                ptx::bulk_g2s(wy_addr + wo, p.wy[h], (uint32_t)p.npad[h] * 256u, &wy_full);
-                wo += (uint32_t)p.npad[h] * 256u;
-            }
-            for (int h = 0; h < p.nheads; ++h) {
-                if (h > 0) ptx::mbar_wait(&l5_done, (uint32_t)(h - 1) & 1u);       // the previous head's L5 MMAs have read w5
-                ptx::mbar_arrive_expect_tx(&w5_full, kW5Bytes);
-                ptx::bulk_g2s(w5_addr, p.w5[h], kW5Bytes, &w5_full);
-            }
-        }
-    } else if (warp == 8) {
-        // ===================================================== MMA issuer
-        if (ptx::elect_one()) {
-            const uint32_t idesc4 = ptx::umma_idesc_f16(128, D4);
-            const uint64_t a_d0 = ptx::umma_desc_nosw(0, 2048u, 128u), b_d0 = ptx::umma_desc_nosw(0, (uint32_t)D4 * 16u, 128u);
-            const uint32_t a_lo0 = (uint32_t)a_d0, a_hi = (uint32_t)(a_d0 >> 32);
-            const uint32_t b_lo0 = (uint32_t)b_d0, b_hi = (uint32_t)(b_d0 >> 32);
-            constexpr uint32_t a_kstep = (2u * 2048u) >> 4, b_kstep = (2u * (uint32_t)D4 * 16u) >> 4;
-            int s = 0;
-            uint32_t ph = 0;
-            for (int c = 0; c < p.nchunks; ++c) {
-                ptx::mbar_wait(&full_bar[s], ph);
-                ptx::tc_fence_after();
-                const uint32_t stage = base + (uint32_t)s * kStageBytes;
-                const uint32_t a_lo = a_lo0 + (stage >> 4), b_lo = b_lo0 + ((stage + kActBytes) >> 4);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
 #pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    ptx::umma_f16(tmem_base, ((uint64_t)a_hi << 32) | (uint64_t)(a_lo + (uint32_t)k * a_kstep),
-                                  ((uint64_t)b_hi << 32) | (uint64_t)(b_lo + (uint32_t)k * b_kstep), idesc4, (c > 0 || k > 0) ? 1u : 0u);
-                ptx::umma_commit(&empty_bar[s]);
-                if (++s == S) { s = 0; ph ^= 1u; }
-            }
-            ptx::umma_commit(&l4_done);
-            // ---- phase 2: per head L5 (A = a4 image, B = w5) then Y (A = a5 image, B = wy_h)
-            const uint32_t idesc5 = ptx::umma_idesc_f16(128, 128);
-            ptx::mbar_wait(&a4_ready, 0);
-            ptx::tc_fence_after();
-            ptx::mbar_wait(&wy_full, 0);
-            uint32_t wo = 0;
-            for (int h = 0; h < p.nheads; ++h) {
-                ptx::mbar_wait(&w5_full, (uint32_t)h & 1u);
-                ptx::tc_fence_after();
-                for (int k = 0; k < D4 / 16; ++k)
-                    ptx::umma_f16(tmem_base + L5_COL, ptx::umma_desc_nosw(a4_addr + (uint32_t)k * 4096u, 2048u, 128u),
-                                  ptx::umma_desc_nosw(w5_addr + (uint32_t)k * 4096u, 2048u, 128u), idesc5, k > 0 ? 1u : 0u);
-                ptx::umma_commit(&l5_done);
-                ptx::mbar_wait(&a5_ready, (uint32_t)h & 1u);
-                ptx::tc_fence_after();
-                const uint32_t npad = (uint32_t)p.npad[h];
-                const uint32_t idescy = ptx::umma_idesc_f16(128, npad);
-                for (int k = 0; k < 8; ++k)
-                    ptx::umma_f16(tmem_base + Y_COL, ptx::umma_desc_nosw(a5_addr + (uint32_t)k * 4096u, 2048u, 128u),
-                                  ptx::umma_desc_nosw(wy_addr + wo + (uint32_t)k * 2u * npad * 16u, npad * 16u, 128u), idescy, k > 0 ? 1u : 0u);
-                ptx::umma_commit(&y_done);
-                wo += npad * 256u;
-            }
-        }
-        __syncwarp();
-    } else {
-        // ===================================================== epilogue: thread = site; warpgroup wg takes half of the L4 / L5
-        // columns, warpgroup 0 alone the (tiny) output layer + softmax
-        const int wg = warp >> 2, q = warp & 3;
-        const int r = q * 32 + lane;                        // TMEM lane = site within the tile
-        const long long site = (long long)at * 128 + r;
-        const bool valid = site < p.batch;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-        ptx::mbar_wait(&l4_done, 0);
-        ptx::tc_fence_after();
-        // a4 = SELU(z4 + b4) -> fp16 operand image [k-group][site][8]
-#pragma unroll 1
-        for (int j0 = wg * (D4 / 2); j0 < (wg + 1) * (D4 / 2); j0 += 16) {
-            float v[16];
-            ptx::tmem_ld16(taddr + (uint32_t)j0, v);
-            ptx::tmem_ld_wait();
-            if (p.z4_tap && valid) {
-#pragma unroll
-                for (int i = 0; i < 16; i += 4)
-                    *reinterpret_cast<float4 *>(p.z4_tap + site * D4 + j0 + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-            }
-            uint4 pk[2];
-            uint32_t *pw = reinterpret_cast<uint32_t *>(pk);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) pw[i] = f2op2_sat(selu(v[2 * i] + b4_s[j0 + 2 * i]), selu(v[2 * i + 1] + b4_s[j0 + 2 * i + 1]));
-            *reinterpret_cast<uint4 *>(smem + (uint32_t)(j0 >> 3) * 2048u + (uint32_t)r * 16u) = pk[0];
-            *reinterpret_cast<uint4 *>(smem + (uint32_t)((j0 >> 3) + 1) * 2048u + (uint32_t)r * 16u) = pk[1];
-        }
-        ptx::fence_proxy_async_smem();
-        ptx::tc_fence_before();
-        ptx::mbar_arrive(&a4_ready);
-        for (int h = 0; h < p.nheads; ++h) {
-            ptx::mbar_wait(&l5_done, (uint32_t)h & 1u);
-            ptx::tc_fence_after();
-#pragma unroll 1
-            for (int j0 = wg * 64; j0 < (wg + 1) * 64; j0 += 16) {
-                float v[16];
-                ptx::tmem_ld16(taddr + L5_COL + (uint32_t)j0, v);
-                ptx::tmem_ld_wait();
-                uint4 pk[2];
-                uint32_t *pw = reinterpret_cast<uint32_t *>(pk);
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    pw[i] = f2op2_sat(selu(v[2 * i] + b5_s[h][j0 + 2 * i]), selu(v[2 * i + 1] + b5_s[h][j0 + 2 * i + 1]));
-                uint8_t *a5 = smem + kA4Bytes + kW5Bytes;
-                *reinterpret_cast<uint4 *>(a5 + (uint32_t)(j0 >> 3) * 2048u + (uint32_t)r * 16u) = pk[0];
-                *reinterpret_cast<uint4 *>(a5 + (uint32_t)((j0 >> 3) + 1) * 2048u + (uint32_t)r * 16u) = pk[1];
-            }
-            ptx::fence_proxy_async_smem();
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&a5_ready);
-            if (wg != 0) continue;          // the second warpgroup goes straight to the next head's L5 accumulator
-            ptx::mbar_wait(&y_done, (uint32_t)h & 1u);
-            ptx::tc_fence_after();
-            // SELU(y + by) -> softmax over the head's n outputs (<= 48 columns, three 16-column TMEM loads)
-            float y[48];
-            ptx::tmem_ld16(taddr + Y_COL, y);
-            if (p.npad[h] > 16) ptx::tmem_ld16(taddr + Y_COL + 16, y + 16);
-            if (p.npad[h] > 32) ptx::tmem_ld16(taddr + Y_COL + 32, y + 32);
-            ptx::tmem_ld_wait();
-            const int n = p.n[h];
-            float mx = -3.0e38f;
-#pragma unroll
-            for (int o = 0; o < 48; ++o) {
-                if (o < n) {
-                    y[o] = selu(y[o] + by_s[h][o]);
-                    mx = fmaxf(mx, y[o]);
-                }
-            }
-            float sum = 0.f;
-#pragma unroll
-            for (int o = 0; o < 48; ++o) {
-                if (o < n) {
-                    y[o] = __expf(y[o] - mx);
-                    sum += y[o];
-                }
-            }
-            const float inv = 1.f / sum;
-            if (valid) {
-                float *dst = p.out + site * p.out_dim + p.off[h];
-#pragma unroll
-                for (int o = 0; o < 48; ++o)
-                    if (o < n) dst[o] = y[o] * inv;
-            }
-            ptx::tc_fence_before();       // this head's TMEM reads are done before the next head's MMAs overwrite the columns
-        }
+        for (int nt = 0; nt < NT; ++nt) ptx::fence_operand(acc[nt]);
+        __syncthreads();                        // both warpgroups are done with the stage
+        if (tid == 0 && i + kStages < nc) issue(i + kStages);
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 8) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc<512>(tmem_base);
-    }
+
+    const size_t row0 = (size_t)tile * 128 + wg * 64 + 16 * w + (lane >> 2);
+    float *z = p.z4 + (size_t)split * p.bp * D4;
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const int col = nt * 128 + 8 * i + 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                *reinterpret_cast<float2 *>(z + (row0 + 8 * h) * D4 + col) = make_float2(acc[nt][4 * i + 2 * h], acc[nt][4 * i + 2 * h + 1]);
+        }
+}
+
+template <int D4>
+int launch_l4(const L4Dev &p, int tiles, int nsplit, cudaStream_t s) {
+    const int smem = kStages * (8 * 128 * 16 + 8 * D4 * 16);
+    C3B_CUDA(cudaFuncSetAttribute(l4_kernel<D4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    dim3 grid(tiles, nsplit);
+    c3b_note_grid((long long)grid.x * grid.y);
+    l4_kernel<D4><<<grid, kThreads, smem, s>>>(p);
+    C3B_CUDA(cudaGetLastError());
+    return 0;
 }
 
 }  // namespace
 
-int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, float *out, float *z4_tap, cudaStream_t s) {
-    if (batch <= 0) return 0;
-    const TailW &t = m->tail;
-    TailDev p = {};
-    p.act = act; p.w4 = t.w4; p.b4 = t.b4;
-    for (int h = 0; h < m->nheads; ++h) {
-        p.w5[h] = t.w5[h]; p.b5[h] = t.b5[h]; p.wy[h] = t.wy[h]; p.by[h] = t.by[h];
-        p.n[h] = t.n[h]; p.npad[h] = t.npad[h]; p.off[h] = t.off[h];
-    }
-    p.out = out; p.z4_tap = z4_tap; p.batch = batch; p.bp = bp;
-    p.nchunks = m->l4_in / 64; p.nheads = m->nheads; p.out_dim = m->out_dim;
-    const int d4 = m->d4;
-    const size_t stage = 16384 + (size_t)d4 * 128;
-    const size_t phase2 = (size_t)(d4 / 8) * 2048 * 2 + 16 * 2048 + (size_t)C3B_MAX_HEADS * 48 * 256;
-    p.stages = d4 == 128 ? 6 : 4;
-    size_t smem = stage * p.stages;
-    if (smem < phase2) smem = phase2;
-    smem += 128;
-    const int grid = (int)((batch + 127) / 128);
-    const_cast<c3b_model *>(m)->launches++;
-    c3b_note_grid(grid);
-    if (d4 == 128) {
-        C3B_CUDA(cudaFuncSetAttribute(tail_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        tail_kernel<128><<<grid, kThreads, smem, s>>>(p);
-    } else {
-        C3B_CUDA(cudaFuncSetAttribute(tail_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        tail_kernel<256><<<grid, kThreads, smem, s>>>(p);
-    }
-    C3B_CUDA(cudaGetLastError());
+// act: tile-major [bp/128][l4_in/8][128][8]; z4: scratch for up to 16 x [bp][d4] fp32 partial sums.  Returns the split count
+// through *nsplit_out (the "l4_pre" tap sums the partials).
+int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, float *out, float *z4, int *nsplit_out, cudaStream_t s) {
+    L4Dev p;
+    p.act = act;
+    p.w4 = m->tail.w4;
+    p.z4 = z4;
+    p.kg = m->l4_in / 8;
+    p.bp = bp;
+    p.nchunks = p.kg / 8;
+    const int tiles = bp / 128;
+    // enough CTAs for two waves of the GPU, at least four k-chunks per split
+    int nsplit = (2 * m->sm_count + tiles - 1) / tiles;
+    nsplit = std::max(1, std::min(std::min(nsplit, kMaxSplit), p.nchunks / 4));
+    p.chunks_per_split = (p.nchunks + nsplit - 1) / nsplit;
+    nsplit = (p.nchunks + p.chunks_per_split - 1) / p.chunks_per_split;
+    const int rc = m->d4 == 128 ? launch_l4<128>(p, tiles, nsplit, s) : launch_l4<256>(p, tiles, nsplit, s);
+    if (rc) return rc;
+    if (c3b_launch_heads(z4, nsplit, (int64_t)bp * m->d4, m->heads, out, batch, s)) return 1;
+    const_cast<c3b_model *>(m)->launches += 2;
+    if (nsplit_out) *nsplit_out = nsplit;
     return 0;
 }

@@ -1,10 +1,10 @@
-"""Install the B200 modules behind the reference's entry points without editing the reference.
+"""Install the H100 modules behind the reference's entry points without editing the reference.
 
 The reference callers import the classes lazily, inside the calling functions
 (``from clair3.model import Clair3_P`` at ``clair3/CallVariantsFromCffi.py:230,239`` and
 ``clair3/CallVariants.py:1466,1471,1714,1718``), so replacing the two attributes of the already-imported
 ``clair3.model`` module is enough for ``run_clair3.py`` / ``CallVarBam`` / ``CallVariants`` /
-``CallVariantsFromCffi`` to construct the sm_100a-backed modules.  See INTEGRATION.md.
+``CallVariantsFromCffi`` to construct the sm_90a-backed modules.  See INTEGRATION.md.
 """
 from __future__ import annotations
 

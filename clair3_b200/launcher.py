@@ -27,7 +27,7 @@ This module replaces that launcher for the network stage:
 
 The tensors keep the reference's wire dtypes (int8 ``.npy``, the GPU-mode narrowing of ``CreateTensorPileupFromCffi.py:447``).
 Host-side logic (file split, batching, shard writing) has no CUDA dependency and is covered by the gloo CPU tests with a stub
-model; the product path constructs the sm_100a modules and fails without a B200.
+model; the product path constructs the sm_90a modules and fails without an H100.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Drop-in ``Clair3_P`` / ``Clair3_F`` for the reference's callers, backed by the sm_100a kernels.
+"""Drop-in ``Clair3_P`` / ``Clair3_F`` for the reference's callers, backed by the sm_90a kernels.
 
 Mirrors the module protocol the reference uses (HKU-BAL/Clair3 paths):
 
@@ -8,7 +8,7 @@ Mirrors the module protocol the reference uses (HKU-BAL/Clair3 paths):
 
 Constructor arguments, state_dict keys (strict), output head order and dtype are the reference's
 (``clair3/model.py:58-161`` and ``:282-416``).  Everything numeric happens in ``libclair3b200.so``; there is no
-PyTorch or CPU implementation behind these classes, and constructing one without a B200 raises.
+PyTorch or CPU implementation behind these classes, and constructing one without an H100 raises.
 """
 from __future__ import annotations
 
@@ -41,7 +41,7 @@ class _C3BModule:
     def to(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise C3BError("clair3_b200 runs only on a CUDA (sm_100a) device; there is no CPU path "
+            raise C3BError("clair3_b200 runs only on a CUDA (sm_90a) device; there is no CPU path "
                            "(requested device: %s)" % device)
         index = device.index if device.index is not None else torch.cuda.current_device()
         if self._handle is not None and self._device is not None and self._device.index == index:

@@ -3,7 +3,7 @@
 Mirrors the reference's binding of ``calculate_clair3_pileup`` (HKU-BAL/Clair3 ``preprocess/CreateTensorPileupFromCffi.py:30-85,
 127-180``: ``pileup_counts_clair3`` -> ``lib.calculate_clair3_pileup`` -> ``_plp_data_to_numpy``) from the point where htslib has
 decoded the alignment records: the caller hands over the ``bam1_t`` fields as arrays (``BamRecords``), the counting, candidate
-selection and - optionally - the Clair3_P forward over the candidates' windows run on the B200 without the count matrix ever
+selection and - optionally - the Clair3_P forward over the candidates' windows run on the H100 without the count matrix ever
 leaving HBM.  No CPU fallback: everything here calls ``libclair3b200.so``.
 """
 from __future__ import annotations
@@ -94,7 +94,7 @@ class DeviceBamRecords:
 
 
 class PileupCounter:
-    """One counting workspace on one B200 (``c3b_plp``).  ``count()`` is asynchronous on the current torch stream of the device;
+    """One counting workspace on one H100 (``c3b_plp``).  ``count()`` is asynchronous on the current torch stream of the device;
     ``sizes()`` / ``fetch()`` wait for it."""
 
     def __init__(self, device=0):

@@ -2,7 +2,7 @@
 
 No released ``.pt`` checkpoint or BAM exists offline, so parity tests, golden fixtures and
 ``bench.py`` all draw weights and inputs from here.  Everything is generated with
-``numpy.random.Generator(PCG64(seed))`` so the very same arrays are rebuilt on the GPU box
+``numpy.random.Generator(PCG64(seed))`` so the very same arrays are rebuilt on the GPU machine
 without shipping multi-megabyte fixtures.
 
 State-dict key names / shapes follow the reference modules

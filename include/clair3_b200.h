@@ -1,5 +1,5 @@
 /*
- * clair3_b200.h — C-ABI of libclair3b200.so: the B200 (sm_100a) inference forward pass of Clair3's two
+ * clair3_b200.h — C-ABI of libclair3b200.so: the H100 (sm_90a) inference forward pass of Clair3's two
  * networks, the drop-in boundary for the one hot path this project replaces.
  *
  * The reference has no plugin/operator registry for this path; its seam is the torch module protocol used by its
@@ -43,11 +43,11 @@ typedef struct c3b_model c3b_model;
 #define C3B_DT_I64  3             /* BatchNorm num_batches_tracked in c3b_set_param; libclair3's size_t count matrix in c3b_forward_windows */
 
 /* arithmetic used by the kernels (c3b_set_option "precision") */
-#define C3B_PREC_F16_TC  0        /* production: fp16 operands on tcgen05 tensor cores, fp32 accumulate / cell state / SELU / softmax */
+#define C3B_PREC_F16_TC  0        /* production: fp16 operands on wgmma tensor cores, fp32 accumulate / cell state / SELU / softmax */
 #define C3B_PREC_FP32    1        /* debug: the same layer graph on fp32 CUDA cores (separates layout bugs from precision) */
 
 /* Replaces Clair3_P.__init__ / Clair3_F.__init__ (clair3/model.py:61-128, 285-368) + m.to(device) (CallVariantsFromCffi.py:246).
- * channels: 18 (pileup) | 8 | 9 with dwell (full-alignment).  Fails if the device is not compute capability 10.x. */
+ * channels: 18 (pileup) | 8 | 9 with dwell (full-alignment).  Fails if the device is not compute capability 9.0. */
 int c3b_create(c3b_model **out, int kind, int channels, int add_indel_length, int device_ordinal);
 
 /* Replaces one entry of m.load_state_dict(state_dict) (clair3/CallVariantsFromCffi.py:19-28).  key is the reference
@@ -58,17 +58,13 @@ int c3b_set_param(c3b_model *m, const char *key, const void *host_data, int dtyp
 
 /* Ends load_state_dict: checks every expected key is present (strict), folds BatchNorm into the convolutions
  * (eps 1e-3, clair3/model.py:192), sums the LSTM bias pairs, folds 1/NORMALIZE_NUM (shared/param_f.py:36) into conv1,
- * packs fp16 UMMA operand images and uploads them once. */
+ * packs fp16 wgmma operand images and uploads them once. */
 int c3b_finalize(c3b_model *m);
 
 /* name: "precision" (C3B_PREC_*), "chunk_sites" (sites per internal pass), "lstm_tile" (batch columns per LSTM CTA sub-tile:
- * 16|32|64, 0 = auto), "lstm_wg" (epilogue warpgroups per LSTM sub-tile: 1|2),
- * "lstm1_impl" / "lstm2_impl" (recurrent kernel of each layer: 0 = gate rows on the TMEM lanes, lstm_tc.cu; 1 = CTA-pair kernel with the
- * sites on the lanes, lstm2x_tc.cu; defaults 0 / 1).  With lstm_tile 0 the library picks by call shape between bit-identical
- * variants: synchronous host-buffer calls (one batch in flight) get the LSTM1 tile and projection grid with the shortest latency,
- * stream-ordered calls the ones with the least SM-time,
- * "pconv_impl" (Clair3_F convolutions: 0 = one CTA per macro-tile, pconv_tc.cu, default; 1 = block-pipelined loads and CTA pairs
- * (tcgen05 cta_group::2) for the streamed-weight convs, pconv2_tc.cu),
+ * 16|32|64, 0 = auto; LSTM2 uses at most 32), "lstm_wg" (warpgroups per LSTM CTA, one sub-tile each: 1|2).  With lstm_tile 0
+ * the library picks by call shape between bit-identical variants: synchronous host-buffer calls (one batch in flight) get the
+ * LSTM tile with the shortest latency, stream-ordered calls the one with the least SM-time,
  * "profile" (1: bracket every kernel launch with CUDA events on its stream and accumulate per-kernel time; setting it resets the
  * totals), "taps" (1: remember where the intermediate activations of a forward live, for c3b_get_tap in clair3_b200_debug.h).
  * Debug-only options are listed in clair3_b200_debug.h. */

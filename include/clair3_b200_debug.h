@@ -1,10 +1,10 @@
 /*
  * clair3_b200_debug.h - debug / measurement hooks of libclair3b200.so.  NOT part of the drop-in surface (clair3_b200.h):
- * activation taps for the parity tests, clock-stamp traces and hardware probes (tools/diag.py).
+ * activation taps for the parity tests and clock-stamp traces.
  *
  * Extra c3b_set_option names that exist only for these hooks: "tap_ws" (which stream workspace c3b_get_tap reads, -1 = first
- * that has the tap), "lstm_trace" (clock stamps of one CTA: 1 = LSTM kernels, 10+i = Clair3_F conv i, 30 = LSTM2 projection),
- * "lstm_mufu16" (1: gate activations with packed tanh.approx.f16x2; 0 default: fp32 tanh.approx, measured faster).
+ * that has the tap), "lstm_trace" (1: clock stamps of one CTA of each LSTM kernel),
+ * "lstm_mufu16" (1: gate activations with packed tanh.approx.f16x2; 0 default: fp32 tanh.approx).
  */
 #ifndef CLAIR3_B200_DEBUG_H
 #define CLAIR3_B200_DEBUG_H
@@ -21,16 +21,8 @@ extern "C" {
 int c3b_get_tap(c3b_model *m, const char *name, float *host_out, int64_t *count_inout);
 
 /* With option "lstm_trace" on, CTA (0,0) of each LSTM kernel stamps clock64 at four points of every step (operands ready,
- * MMAs issued, accumulator ready, epilogue done); copies [2 layers][33 steps][4] stamps out. */
+ * first accumulator ready, epilogue done, next operands stored); copies [2 layers][33 steps][4] stamps out. */
 int c3b_debug_lstm_trace(c3b_model *m, int64_t *out264);
-
-/* Hardware probe (tools/diag.py probe): one tcgen05.mma with its A operand in TMEM (checks the assumed layout) and the
- * cycles of `reps` back-to-back MMAs with A from shared memory vs TMEM.  a[128][16], b[n][16] -> out_d[128][n]. */
-int c3b_debug_ts_probe(const float *a, const float *b, int n, int reps, float *out_d, int64_t *timing10);
-/* cycles for back-to-back tcgen05.mma under operand / accumulator switching (tools/diag.py mmaprobe) */
-int c3b_debug_mma_probe(int n, int reps, int nmodes, const int *modes, int64_t *timing);
-/* cycles of TMEM reads / an epilogue chunk with the tensor pipe idle and busy (tools/diag.py tmemprobe) */
-int c3b_debug_tmem_probe(int reps, int64_t *timing6);
 
 #ifdef __cplusplus
 }

@@ -1,6 +1,6 @@
 /*
  * clair3_b200_pileup.h - C-ABI of the GPU pileup feature counter in libclair3b200.so (SURVEY.md 8f, row N4, pileup half): the
- * per-column count matrix that feeds Clair3_P, built on the B200 from DECODED alignment records.
+ * per-column count matrix that feeds Clair3_P, built on the GPU from DECODED alignment records.
  *
  * Replaces (paths relative to HKU-BAL/Clair3)
  *     plp_data calculate_clair3_pileup(region, bam_set, fasta_path, min_depth, min_snp_af, min_indel_af, min_mq,

@@ -1,7 +1,7 @@
 """ORACLE — test infrastructure only (never imported by the product path).
 
 Plain-numpy CPU restatement of the Clair3 inference forward pass, used by ``tests/``,
-``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` leg to check the sm_100a kernels.
+``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` leg to check the sm_90a kernels.
 Each function cites the reference lines it restates (paths relative to the HKU-BAL/Clair3 repo):
 
 * ``pileup_forward``  -> ``clair3/model.py:130-161``  (``Clair3_P.forward``)
@@ -21,7 +21,7 @@ scale=1.0507009873554805), eval-mode BatchNorm, softmax.
 
 Pinning: the reference holds no golden vectors for this path (SURVEY.md §4), so the oracle is pinned
 against outputs of the reference itself: ``tests/golden/make_golden.py`` imports
-``/root/reference/clair3/model.py`` in the build container, runs it in fp32 on seeded inputs and
+the reference's ``clair3/model.py`` (a checkout named by ``CLAIR3_REFERENCE``), runs it in fp32 on seeded inputs and
 commits outputs + taps under ``tests/golden/``; ``tests/test_oracle.py`` checks this file against them.
 
 Computation dtype defaults to float64 so the oracle is "the math"; the fp32 reference differs from

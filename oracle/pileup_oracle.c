@@ -7,7 +7,7 @@
  * time, every overlapping read resolved with an incremental per-read CIGAR cursor, a per-column deletion-length table and
  * insertion-string counters, then the column's statistics and candidate test.
  *
- * The per-read / per-column resolution lives in a THIRD-PARTY dependency that /root/reference does not vendor: htslib 1.15.1
+ * The per-read / per-column resolution lives in a THIRD-PARTY dependency that the reference does not vendor: htslib 1.15.1
  * (downloaded by the reference's Makefile:32-46; only its public header src/sam.h is in the tree).  Restated here from htslib's
  * published behaviour:
  *     bam_plp_push / bam_plp_next (sam.c): a read is on column pos iff beg <= pos < beg + reference length of its CIGAR; columns

@@ -17,7 +17,7 @@ LIB = os.path.join(OUT_DIR, "libpileup_oracle.so")
 
 
 def build(force=False):
-    """gcc -O2 -shared oracle/pileup_oracle.c -> oracle/_build/libpileup_oracle.so (git-ignored; travels to the GPU box)."""
+    """gcc -O2 -shared oracle/pileup_oracle.c -> oracle/_build/libpileup_oracle.so (a git-ignored build product)."""
     if force or not os.path.exists(LIB) or os.path.getmtime(LIB) < os.path.getmtime(SRC):
         os.makedirs(OUT_DIR, exist_ok=True)
         subprocess.run(["gcc", "-O2", "-shared", "-fPIC", "-o", LIB, SRC], check=True)

@@ -3,7 +3,7 @@
 The reference's CPU implementation of the hot path is ``torch.nn`` modules executed by ATen/oneDNN
 (``clair3/model.py:96-125,130-161`` pileup; ``:183-279,317-416`` full-alignment), run under
 ``torch.inference_mode`` by ``_torch_predict`` (``clair3/CallVariantsFromCffi.py:48-52``).
-``/root/reference`` cannot travel to the GPU box, so this file restates the two forwards with the
+The reference's source is not part of this repository, so this file restates the two forwards with the
 same torch CPU operators (``torch.lstm``, ``conv2d``, ``batch_norm``, ``max_pool2d``, ``linear``,
 ``selu``, ``softmax``) so ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs time the very
 kernels the reference would execute (kind = "port").  Pinned against the golden fixtures minted

@@ -13,20 +13,20 @@ GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by `pytest -m gpu` on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with `pytest -m gpu` on a GPU machine)")
 
 
 def pytest_collection_modifyitems(config, items):
-    """`gpu`-marked tests need a B200 (compute capability 10.x): skip them cleanly anywhere else, so a plain `pytest` on a CPU
+    """`gpu`-marked tests need an H100 (compute capability 9.0): skip them cleanly anywhere else, so a plain `pytest` on a CPU
     host passes instead of dying in the CUDA driver."""
     try:
         import torch
-        ok = torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 10
+        ok = torch.cuda.is_available() and torch.cuda.get_device_capability(0) == (9, 0)
     except Exception:
         ok = False
     if ok:
         return
-    skip = pytest.mark.skip(reason="needs a B200 (sm_100) GPU")
+    skip = pytest.mark.skip(reason="needs an H100 (sm_90) GPU")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -1,9 +1,9 @@
-"""Mint the golden vectors of the decoder's first stage from the REAL reference (build container only).
+"""Mint the golden vectors of the decoder's first stage from the REAL reference (a Clair3 checkout, named by CLAIR3_REFERENCE).
 
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_decode_golden.py
+    CLAIR3_REFERENCE=/path/to/Clair3 PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_decode_golden.py
 
 Calls the reference's own ``possible_outcome_probabilites_from`` and ``quality_score_from``
-(``/root/reference/clair3/CallVariants.py:510-576,375-381``) and ``gt21_enum_from_label`` site by site on seeded
+(``clair3/CallVariants.py:510-576,375-381``) and ``gt21_enum_from_label`` site by site on seeded
 probability rows (a mix of confident homozygous-reference rows, confident variants and rows sitting exactly on the 0.5
 thresholds) and stores inputs + the early-out flag, the returned probability and the un-rounded QUAL as a small ``.npz``.
 """
@@ -14,7 +14,7 @@ from math import log
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["CLAIR3_REFERENCE"])
 sys.dont_write_bytecode = True
 
 from clair3.CallVariants import Phred_Trans, possible_outcome_probabilites_from, quality_score_from  # noqa: E402

@@ -1,13 +1,13 @@
-"""Mint golden vectors from the REAL reference (run in the build container only).
+"""Mint golden vectors from the REAL reference (a Clair3 checkout, named by CLAIR3_REFERENCE).
 
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    CLAIR3_REFERENCE=/path/to/Clair3 PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 
-Imports ``/root/reference/clair3/model.py`` unmodified, loads the seeded synthetic checkpoints of
+Imports the reference's ``clair3/model.py`` unmodified, loads the seeded synthetic checkpoints of
 ``clair3_b200.synth`` through the reference's own ``load_state_dict`` (strict), runs the fp32 CPU
 forward under ``torch.inference_mode`` exactly like ``_torch_predict``
 (``clair3/CallVariantsFromCffi.py:48-52``) and stores outputs plus intermediate taps as small
 ``.npz`` fixtures.  Inputs/weights are NOT stored: tests rebuild them from the recorded seeds.
-The GPU box has no /root/reference; only the committed fixtures travel.
+The tests read only the committed fixtures.
 """
 import os
 import sys
@@ -18,7 +18,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["CLAIR3_REFERENCE"])
 sys.dont_write_bytecode = True
 
 from clair3.model import Clair3_P, Clair3_F  # noqa: E402  (the reference)

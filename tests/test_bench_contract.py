@@ -65,7 +65,7 @@ def test_counter_cpu_baseline_in_the_reference_deployment_shape():
 
 
 def test_summary_tool_renders_the_committed_line():
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "bench_summary.py"), os.path.join(ROOT, "profiles", "r2_bench_line.json")],
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "bench_summary.py"), os.path.join(ROOT, "profiles", "h100_bench_line.json")],
                        capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stderr[-1000:]
     for needle in ("| pileup |", "| fa |", "| cascade |", "## pileup_counts", "bases/s"):

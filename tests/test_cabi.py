@@ -1,5 +1,5 @@
 """CPU-side checks: the C-ABI library builds, loads and exports every symbol include/clair3_b200.h declares; the
-product path fails loudly (no CPU fallback) when no B200 is present."""
+product path fails loudly (no CPU fallback) when no H100 is present."""
 import ctypes
 import os
 
@@ -70,7 +70,7 @@ int main(void) {
 
 def test_version_and_error_strings():
     L = _ffi.lib()
-    assert b"sm_100a" in _ffi.ffi.string(L.c3b_version())
+    assert b"sm_90a" in _ffi.ffi.string(L.c3b_version())
     assert L.c3b_out_dim(_ffi.ffi.NULL) == -1
 
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: ``pytest -m gpu``).  Everything goes through the C-ABI
+"""GPU parity tests (run on an H100: ``pytest -m gpu``).  Everything goes through the C-ABI
 (``libclair3b200.so`` via cffi); the checker is the oracle / the golden vectors minted from the reference.
 
 Tolerances (stated, SURVEY.md §8c):
@@ -121,7 +121,8 @@ def test_lstm_tiles_agree():
 
 @pytest.mark.parametrize("tile", [16, 32, 64])
 def test_lstm_warpgroup_layouts_agree(tile):
-    """One or two epilogue warpgroups per LSTM sub-tile (option lstm_wg) run the same per-cell arithmetic: identical output."""
+    """One or two warpgroups (one sub-tile of sites each) per LSTM CTA (option lstm_wg) run the same per-cell arithmetic:
+    identical output."""
     z, meta, sd, x = golden_case("p90")
     outs = []
     for wg in (1, 2):

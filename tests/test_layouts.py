@@ -1,5 +1,5 @@
 """CPU model of the HBM layouts and the shifted-view index arithmetic the CUDA convolution kernel relies on
-(clair3_b200/csrc/pconv_tc.cu, c3b_internal.h: c3b_planar_geom / c3b_parity_offset; DESIGN.md 2 and 3.3).
+(clair3_b200/csrc/pconv_tc.cu, c3b_internal.h: c3b_planar_geom / c3b_parity_offset; DESIGN.md 2).
 
 The kernel never gathers: a 3x3 tap is the SAME zero-padded planar image (stride 1) or one of four parity planes (stride 2)
 viewed a constant number of slots later.  These tests restate that claim in numpy and check it against the oracle's

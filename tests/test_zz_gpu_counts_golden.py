@@ -1,7 +1,6 @@
 """The feature counter against the COMMITTED fixtures of tests/golden/pileup_counts.npz, through the C-ABI (counts, candidates, gVCF
-arrays, all_alt_info).  Kept in its own module, collected last: the fixtures were minted after the round's last GPU session, so
-this is the one GPU test of the counter that has not itself run on a B200 yet (every operation it composes has - see
-tests/test_gpu_pileup_counts.py)."""
+arrays, all_alt_info).  Kept in its own module, collected last, after the counter's operation-by-operation tests in
+tests/test_gpu_pileup_counts.py."""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""Render a bench.py JSON line as the markdown summary committed under profiles/ (python tools/bench_summary.py line.json > profiles/rN_bench_summary.md)."""
+"""Render a bench.py JSON line as a markdown summary (python tools/bench_summary.py line.json)."""
 import json
 import sys
 
