@@ -408,8 +408,8 @@ static int finalize_impl(c3b_model *m) {
             }
             put(blob, img.data(), img.size() * 2, (const void **)&m->lstm_tc[1][0].w_img, false);
             m->lstm_tc[1][0].bias = nullptr;
-            // one 128-column slab per column block of the projection kernel (proj_tc.cu): [chunk 4][block 10][8 kg][128 rows][8]
-            std::vector<uint16_t> pimg = pack_operand(1280, 32, 128, [&](int R, int k) {
+            // one 256-column weight slab per CTA of the projection kernel (proj_tc.cu): [chunk 4][slab 5][8 kg][256 rows][8]
+            std::vector<uint16_t> pimg = pack_operand(1280, 32, 256, [&](int R, int k) {
                 const int row = c3b_lstm_row(R % 640, C3B_H2);
                 return (*wih_d[R / 640])[(size_t)row * 256 + k] * ((row / C3B_H2 == 2) ? 1.0f : 0.5f);
             });
