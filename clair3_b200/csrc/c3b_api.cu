@@ -387,8 +387,8 @@ static int finalize_impl(c3b_model *m) {
             put(blob, img.data(), img.size() * 2, (const void **)&m->lstm_tc[0][0].w_img, false);
             m->lstm_tc[0][0].bias = nullptr;
         }
-        // tensor-core LSTM2: recurrent image [dir][10 blocks][20][64][8] (c3b_lstm_row order) + input projection GEMM (1280 columns
-        // in the same order per direction, bias folded into the projection)
+        // tensor-core LSTM2: recurrent image [dir][10 blocks][20][64][8] (c3b_lstm_row order) + input projection GEMM (1280 columns,
+        // gate-quad order c3b_lstm2_pg_row per direction, bias folded into the projection)
         {
             std::vector<uint16_t> img((size_t)2 * 640 * 20 * 8, 0);
             std::vector<float> pbias(1280);
@@ -401,17 +401,20 @@ static int finalize_impl(c3b_model *m) {
                 for (int R = 0; R < 640; ++R) {
                     const int row = c3b_lstm_row(R, C3B_H2);
                     const float gs = (row / C3B_H2 == 2) ? 1.0f : 0.5f;      // pre-halved sigmoid gates
-                    pbias[(size_t)d * 640 + R] = (bih[row] + bhh[row]) * gs;
                     for (int k = 0; k < 160; ++k)
                         img[((((size_t)d * 10 + R / 64) * 20 + k / 8) * 64 + R % 64) * 8 + k % 8] = c3b_f2op(whh[(size_t)row * 160 + k] * gs);
+                }
+                for (int C = 0; C < 640; ++C) {
+                    const int row = c3b_lstm2_pg_row(C);
+                    pbias[(size_t)d * 640 + C] = (bih[row] + bhh[row]) * ((row / C3B_H2 == 2) ? 1.0f : 0.5f);
                 }
             }
             put(blob, img.data(), img.size() * 2, (const void **)&m->lstm_tc[1][0].w_img, false);
             m->lstm_tc[1][0].bias = nullptr;
             // one 256-column weight slab per CTA of the projection kernel (proj_tc.cu): [chunk 4][slab 5][8 kg][256 rows][8]
-            std::vector<uint16_t> pimg = pack_operand(1280, 32, 256, [&](int R, int k) {
-                const int row = c3b_lstm_row(R % 640, C3B_H2);
-                return (*wih_d[R / 640])[(size_t)row * 256 + k] * ((row / C3B_H2 == 2) ? 1.0f : 0.5f);
+            std::vector<uint16_t> pimg = pack_operand(1280, 32, 256, [&](int C, int k) {
+                const int row = c3b_lstm2_pg_row(C % 640);
+                return (*wih_d[C / 640])[(size_t)row * 256 + k] * ((row / C3B_H2 == 2) ? 1.0f : 0.5f);
             });
             m->proj2 = IgemmW();
             m->proj2.n = 1280;

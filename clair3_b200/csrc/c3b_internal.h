@@ -61,6 +61,12 @@ inline int c3b_lstm_row(int R, int H) {
     const int pp = R / 128, blk = (R / 64) & 1, r = R % 64, w = r / 16, q = r % 16;
     return (2 * blk + (q >= 8)) * H + 32 * pp + 8 * w + (q & 7);
 }
+// Torch gate row of LSTM2 pre-gate column C in [0, 640) of one direction (the output columns of proj2): "gate-quad" order, the
+// four gates i, f, g, o of unit 32p + u (u < 32) in the adjacent columns 128p + 4u .. +3, so the recurrent kernel's thread that
+// owns the unit in block pair p reads them with one 8-byte load.
+inline int c3b_lstm2_pg_row(int C) {
+    return (C & 3) * C3B_H2 + 32 * (C >> 7) + ((C & 127) >> 2);
+}
 float c3b_op2f(uint16_t h);     // host: fp16 bits -> fp32
 
 #define C3B_CUDA(expr)                                                                          \
@@ -218,7 +224,7 @@ struct c3b_model {
     ConvF32 conv_f32[9];
     // tc path
     LstmTC lstm_tc[2][2];
-    IgemmW proj2;                      // LSTM2 input projection, both directions: N = 1280 (row order c3b_lstm_row)
+    IgemmW proj2;                      // LSTM2 input projection, both directions: N = 1280 (column order c3b_lstm2_pg_row)
     TailW tail;                        // L4 on the tensor cores
     IgemmW conv_tc[9];
 
@@ -252,7 +258,7 @@ int c3b_launch_spp_f32(const float *x, float *out, int64_t batch, int h, int w, 
 struct TcPileupBuffers {
     op_t *xs;     // [33][B][48] fp16, time-major: hi(x) | 1 | lo(x) columns
     op_t *h1;     // tile-major k-group-planar, 32 k-groups: row = t*Bp + b, k = dir*128 + j  (projection GEMM operand)
-    __half *pg;            // [33*B][1280] fp16 pre-gates of LSTM2 (bias included), permuted gate columns
+    __half *pg;            // [33*B][1280] fp16 pre-gates of LSTM2 (bias included), column dir*640 + C in gate-quad order (c3b_lstm2_pg_row)
     op_t *h2;     // tile-major k-group-planar, 1320 k-groups: row = b, k = t*320 + dir*160 + j (flatten order of clair3/model.py:135)
     float *z4;             // [16][B][128] fp32 split-K partial sums of the L4 pre-activation (no bias)
     int bp;                // padded batch: multiple of 128

@@ -19,8 +19,17 @@
 // and W_ih multiplies both parts (fp32 accumulate: the same result as an exact-input product).  Column 18 is a constant 1 that
 // carries b_ih + b_hh, so the x projection and the bias are fused into the same MMAs.
 // LSTM2 (H=160, input 256): the input projection W_ih*h1 (+bias) is a separate big GEMM (proj_tc.cu) that leaves fp16
-// pre-gates pg[t*bp + site][dir*640 + row] in the same permuted row order; this kernel keeps only W_hh on chip (K = 160).
+// pre-gates pg[t*bp + site][dir*640 + C] in gate-quad order (c3b_lstm2_pg_row: columns 128p + 4u .. +3 = gates i, f, g, o of
+// unit 32p + u), so a thread loads its unit's four pre-gates of one site as one 8-byte word; a warp load covers 4 sites x 64
+// contiguous bytes.  This kernel keeps only W_hh on chip (K = 160).
 // The sigmoid gates' rows are pre-halved on the host so sigma(x) = 0.5*tanh(x/2)+0.5 is one MUFU + one FMA.
+//
+// Schedule.  Per step and block pair a warpgroup issues 2 x K/16 wgmmas (two dependent accumulation chains), waits for them,
+// then runs the cell math.  The two warpgroups of a CTA run this independently; their MMA chains interleave on the tensor pipe.
+// (Strict turn-taking between them, so that one's cell math runs under the other's MMAs, measured slower on H100 for LSTM1 and
+// no faster for LSTM2: it serialises the two warpgroups' MMA chains, which otherwise overlap.)  LSTM2's pre-gates of block pair
+// p + 1 (after the last pair: the next step's first) are loaded right after the MMAs of pair p are issued, so their DRAM
+// latency hides behind a whole MMA / cell-math phase instead of stalling the start of every pair.
 #include "c3b_internal.h"
 #include "ptx.cuh"
 
@@ -80,6 +89,10 @@ __device__ __forceinline__ uint32_t lstm_cell_h2(const float *gi, const float *g
     const uint32_t ov = sigm_f16x2(pack_f16x2(go[0], go[1]));
     return mul_f16x2(ov, tanh_f16x2(pack_f16x2(c[0], c[1])));
 }
+
+// fp16 in the low / high half of a 32-bit word -> fp32
+__device__ __forceinline__ float half_lo(uint32_t v) { return __half2float(__ushort_as_half((unsigned short)(v & 0xffffu))); }
+__device__ __forceinline__ float half_hi(uint32_t v) { return __half2float(__ushort_as_half((unsigned short)(v >> 16))); }
 
 // Element offset of the 8-unit group `kgh` of site `b` at time t in the layer's output, TILE-MAJOR k-group-planar
 // [row tile of 128][k-groups][128 rows][8] (c3b_tile_major_offset): LSTM1 -> h1 (row = t*bp + b, 32 k-groups: dir*16 + kgh),
@@ -157,6 +170,19 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
         for (int i = 0; i < NB / 4; ++i) c[pp][i] = 0.f;
     uint32_t hq[NP][NB / 8];                        // this step's h as packed (site, site+1) fp16 pairs
 
+    // LSTM2 pre-gates of this thread's unit for the next block pair: one 8-byte word (i, f, g, o) per site, loaded a pair early
+    constexpr int PGN = LAYER2 ? NB / 4 : 1;
+    uint2 pgn[PGN];
+    auto load_pg = [&](int tt, int pp) {
+        const __half *pgp = p.pg + (size_t)dir * 640 + pp * 128 + 4 * (8 * w + q0);
+#pragma unroll
+        for (int i = 0; i < NB / 8; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+                pgn[2 * i + e] = *reinterpret_cast<const uint2 *>(pgp + ((size_t)tt * p.bp + b0 + 8 * i + s0 + e) * 1280);
+    };
+    if constexpr (LAYER2) load_pg(dir ? C3B_T - 1 : 0, 0);
+
     ptx::mbar_wait(&w_bar, 0);
     const bool tr = p.trace != nullptr && tid == 0 && blockIdx.x == 0 && blockIdx.y == 0;
     for (int step = 0; step < C3B_T; ++step) {
@@ -188,21 +214,6 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
         }
 #pragma unroll
         for (int pp = 0; pp < NP; ++pp) {
-            // LSTM2 pre-gates of this thread's unit: i, f, g, o at rows r, r + 8 of blocks 2pp, 2pp + 1
-            __half pgv[LAYER2 ? NB / 4 : 1][4];
-            if constexpr (LAYER2) {
-                const __half *pgp = p.pg + (size_t)dir * 640 + pp * 128 + 16 * w + q0;
-#pragma unroll
-                for (int i = 0; i < NB / 8; ++i)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const __half *r = pgp + ((size_t)t * p.bp + b0 + 8 * i + s0 + e) * 1280;
-                        pgv[2 * i + e][0] = r[0];
-                        pgv[2 * i + e][1] = r[8];
-                        pgv[2 * i + e][2] = r[64];
-                        pgv[2 * i + e][3] = r[72];
-                    }
-            }
             float acc0[NB / 2], acc1[NB / 2];
             ptx::wgmma_fence();
 #pragma unroll
@@ -213,6 +224,15 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
                 wgmma_nb<NB>(acc1, ptx::wgmma_desc(a0 + kBlkBytes, 1024, 128), bd, ks > 0);
             }
             ptx::wgmma_commit();
+            // LSTM2: this pair's pre-gates were loaded one block pair ago; start the next pair's (after the last pair: the next
+            // step's first) so that they arrive while this pair's MMAs and cell math run
+            uint2 pgv[PGN];
+            if constexpr (LAYER2) {
+#pragma unroll
+                for (int i = 0; i < PGN; ++i) pgv[i] = pgn[i];
+                if (pp + 1 < NP) load_pg(t, pp + 1);
+                else if (step + 1 < C3B_T) load_pg(dir ? t - 1 : t + 1, 0);
+            }
             ptx::wgmma_wait<0>();
             ptx::fence_operand(acc0);
             ptx::fence_operand(acc1);
@@ -227,10 +247,10 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
                     gg[e] = acc1[4 * i + e];
                     go[e] = acc1[4 * i + 2 + e];
                     if constexpr (LAYER2) {
-                        gi[e] += __half2float(pgv[2 * i + e][0]);
-                        gf[e] += __half2float(pgv[2 * i + e][1]);
-                        gg[e] += __half2float(pgv[2 * i + e][2]);
-                        go[e] += __half2float(pgv[2 * i + e][3]);
+                        gi[e] += half_lo(pgv[2 * i + e].x);
+                        gf[e] += half_hi(pgv[2 * i + e].x);
+                        gg[e] += half_lo(pgv[2 * i + e].y);
+                        go[e] += half_hi(pgv[2 * i + e].y);
                     }
                 }
                 if (MUFU16) {

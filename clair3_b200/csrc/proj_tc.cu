@@ -1,7 +1,11 @@
 // LSTM2's input projection (clair3/model.py:132-133 -> torch nn.LSTM's W_ih x_t + b_ih + b_hh, both directions) as one
 // warpgroup-MMA GEMM over every time step at once:
 //
-//   pg[t*bp + b][col] = sum_k h1[t*bp + b][k] * Wp[col][k] + bias[col]      col = dir*640 + R (c3b_lstm_row order), K = 256
+//   pg[t*bp + b][col] = sum_k h1[t*bp + b][k] * Wp[col][k] + bias[col]      col = dir*640 + C, K = 256
+//
+// C is in gate-quad order (c3b_lstm2_pg_row): columns 128p + 4u .. +3 are gates i, f, g, o of hidden unit 32p + u, so the
+// recurrent kernel loads a unit's four pre-gates of one site as one 8-byte word.  The order lives only in the host-packed
+// weight slabs and bias; this kernel does not depend on it.
 //
 // M = 33*bp rows, N = 1280, K = 256: at bp = 1024 that is 22 GFLOP, 17 MB of h1 read and 86 MB of pre-gates written, and on
 // H100 the MMAs and the traffic each need about 30 us, so the copies, the MMAs and the stores must overlap.  Weight-stationary
