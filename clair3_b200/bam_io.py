@@ -40,11 +40,37 @@ def read_header(buf):
     return refs, off
 
 
-def read_bam(path, ref_name=None, start=None, end=None, with_names=False):
+_AUX_SIZE = {ord("A"): 1, ord("c"): 1, ord("C"): 1, ord("s"): 2, ord("S"): 2, ord("i"): 4, ord("I"): 4, ord("f"): 4}
+_B_DTYPE = {ord("c"): "<i1", ord("C"): "<u1", ord("s"): "<i2", ord("S"): "<u2", ord("i"): "<i4", ord("I"): "<u4"}
+
+
+def _aux_mv(buf, p, e):
+    """The values of the ``mv`` B-array among the auxiliary fields buf[p:e] (SAM/BAM specification 4.2.4), widened to int32, or
+    None when the record has no such tag."""
+    while p + 3 <= e:
+        tag, t = buf[p:p + 2], buf[p + 2]
+        if t == ord("B"):
+            sub = buf[p + 3]
+            cnt, = struct.unpack_from("<i", buf, p + 4)
+            if tag == b"mv" and sub in _B_DTYPE:
+                return np.frombuffer(buf, dtype=_B_DTYPE[sub], count=cnt, offset=p + 8).astype(np.int32)
+            p += 8 + cnt * (_AUX_SIZE.get(sub, 4))
+        elif t in (ord("Z"), ord("H")):
+            z = buf.index(b"\0", p + 3)
+            p = z + 1
+        else:
+            p += 3 + _AUX_SIZE[t]
+    return None
+
+
+def read_bam(path, ref_name=None, start=None, end=None, with_names=False, fa_fields=False):
     """Alignment records of a coordinate-sorted BAM as the arrays of ``clair3_b200.pileup_counts.BamRecords`` (plus ``tid``), in
     file order.  ``ref_name`` / ``start`` / ``end`` (0-based, end-exclusive) keep what an indexed fetch of that region returns:
     records of that contig whose alignment overlaps [start, end).  Unmapped-without-position records (refID -1) are skipped.
-    Returns (records dict, [(reference name, length)])."""
+    ``fa_fields``: also the fields the full-alignment tensor builder reads (``clair3_b200.fa_tensor``): ``qual`` / ``qual_off``
+    (bam_get_qual), ``qname`` / ``qname_off`` (read names without the NUL, concatenated bytes) and ``mv`` / ``mv_off`` (the
+    ``mv`` B-array including its leading stride element, any integer subtype widened to int32; an empty range when the record has
+    no ``mv`` tag).  Returns (records dict, [(reference name, length)])."""
     with gzip.open(path, "rb") as f:
         buf = f.read()
     refs, off = read_header(buf)
@@ -57,6 +83,7 @@ def read_bam(path, ref_name=None, start=None, end=None, with_names=False):
     lo = -1 if start is None else int(start)
     hi = 1 << 62 if end is None else int(end)
     pos, flag, mapq, lq, tids, names_out = [], [], [], [], [], []
+    quals, qnames, mvs = [], [], []
     cig_parts, seq_parts, coff, soff = [], [], [0], [0]
     n = len(buf)
     while off + 4 <= n:
@@ -90,6 +117,12 @@ def read_bam(path, ref_name=None, start=None, end=None, with_names=False):
         soff.append(soff[-1] + nb)
         if with_names:
             names_out.append(buf[rec0 + 32:rec0 + 32 + l_name - 1].decode())
+        if fa_fields:
+            q0 = s0 + nb
+            quals.append(buf[q0:q0 + l_seq])
+            qnames.append(buf[rec0 + 32:rec0 + 32 + l_name - 1])
+            mv = _aux_mv(buf, q0 + l_seq, off)
+            mvs.append(mv if mv is not None else np.zeros(0, np.int32))
     rec = {"pos": np.array(pos, np.int64), "flag": np.array(flag, np.uint16), "mapq": np.array(mapq, np.uint8),
            "l_qseq": np.array(lq, np.int32), "cigar_off": np.array(coff, np.int64),
            "cigar": np.concatenate(cig_parts).astype(np.uint32) if cig_parts else np.zeros(0, np.uint32),
@@ -97,6 +130,15 @@ def read_bam(path, ref_name=None, start=None, end=None, with_names=False):
            "tid": np.array(tids, np.int32)}
     if with_names:
         rec["names"] = names_out
+    if fa_fields:
+        def offsets(parts):
+            return np.concatenate([[0], np.cumsum([len(x) for x in parts], dtype=np.int64)]).astype(np.int64)
+        rec["qual"] = np.frombuffer(b"".join(quals), dtype=np.uint8).copy()
+        rec["qual_off"] = offsets(quals)
+        rec["qname"] = np.frombuffer(b"".join(qnames), dtype=np.uint8).copy()
+        rec["qname_off"] = offsets(qnames)
+        rec["mv"] = np.concatenate(mvs).astype(np.int32) if mvs else np.zeros(0, np.int32)
+        rec["mv_off"] = offsets(mvs)
     return rec, refs
 
 
@@ -119,7 +161,10 @@ def _bgzf_block(payload):
 
 def write_bam(path, rec, refs, tid=0, names=None, header_text=None):
     """Writes the records (arrays as ``read_bam`` returns them; every record on contig ``tid`` unless ``rec['tid']`` is given) as a
-    BGZF-compressed BAM: ``refs`` = [(name, length)].  Qualities are written as 0xFF (absent), no auxiliary fields."""
+    BGZF-compressed BAM: ``refs`` = [(name, length)].  Without ``rec['qual']`` the qualities are written as 0xFF (absent); read names
+    come from ``names``, else ``rec['qname']`` / ``rec['qname_off']``, else ``r<i>``; ``rec['mv']`` / ``rec['mv_off']`` become an
+    ``mv:B:c`` tag (``mv:B:i`` when a value does not fit int8) on every record with a non-empty range, as ``read_bam(...,
+    fa_fields=True)`` returns them."""
     text = (header_text or "@HD\tVN:1.6\tSO:coordinate\n" + "".join("@SQ\tSN:%s\tLN:%d\n" % r for r in refs)).encode()
     out = bytearray(b"BAM\x01" + struct.pack("<i", len(text)) + text + struct.pack("<i", len(refs)))
     for name, length in refs:
@@ -131,11 +176,25 @@ def write_bam(path, rec, refs, tid=0, names=None, header_text=None):
         cig = np.ascontiguousarray(rec["cigar"][rec["cigar_off"][i]:rec["cigar_off"][i + 1]], dtype="<u4")
         seq = bytes(rec["seq"][rec["seq_off"][i]:rec["seq_off"][i + 1]])
         l_seq = int(rec["l_qseq"][i])
-        nm = ((names[i] if names else "r%d" % i).encode()) + b"\x00"
+        if names:
+            nm = names[i].encode() + b"\x00"
+        elif rec.get("qname_off") is not None:
+            nm = bytes(rec["qname"][rec["qname_off"][i]:rec["qname_off"][i + 1]]) + b"\x00"
+        else:
+            nm = ("r%d" % i).encode() + b"\x00"
+        if rec.get("qual_off") is not None:
+            qual = bytes(np.asarray(rec["qual"][rec["qual_off"][i]:rec["qual_off"][i + 1]], dtype=np.uint8))
+        else:
+            qual = b"\xff" * l_seq
+        aux = b""
+        if rec.get("mv_off") is not None and rec["mv_off"][i + 1] > rec["mv_off"][i]:
+            mv = np.asarray(rec["mv"][rec["mv_off"][i]:rec["mv_off"][i + 1]], dtype=np.int64)
+            small = mv.min() >= -128 and mv.max() <= 127
+            aux = b"mvB" + (b"c" if small else b"i") + struct.pack("<i", len(mv)) + mv.astype("<i1" if small else "<i4").tobytes()
         p = int(rec["pos"][i])
         span = int((cig >> 4)[np.isin(cig & 15, _REF_CONSUMING)].sum())
         body = _CORE.pack(int(tids[i]), p, len(nm), int(rec["mapq"][i]), _reg2bin(p, p + max(span, 1)), len(cig), int(rec["flag"][i]),
-                          l_seq, -1, -1, 0) + nm + cig.tobytes() + seq[:(l_seq + 1) // 2] + b"\xff" * l_seq
+                          l_seq, -1, -1, 0) + nm + cig.tobytes() + seq[:(l_seq + 1) // 2] + qual + aux
         out += struct.pack("<i", len(body)) + body
     with open(path, "wb") as f:
         for b0 in range(0, len(out), 0xFF00):                # BGZF: at most 64 KiB of payload per block

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libclair3b200.so")
 OBJ_DIR = os.path.join(HERE, "csrc", "_obj")
-SOURCES = ["c3b_api.cu", "kernels_common.cu", "kernels_fp32.cu", "lstm_tc.cu", "fa_tc.cu", "pconv_tc.cu", "decode.cu", "proj_tc.cu", "tail_tc.cu", "plp_counts.cu"]
+SOURCES = ["c3b_api.cu", "kernels_common.cu", "kernels_fp32.cu", "lstm_tc.cu", "fa_tc.cu", "pconv_tc.cu", "decode.cu", "proj_tc.cu", "tail_tc.cu", "plp_counts.cu", "fa_tensor.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
@@ -36,7 +36,7 @@ def _stale(target, deps):
 
 def build_library(force=False, verbose=False):
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
-    for h in ("clair3_b200.h", "clair3_b200_debug.h", "clair3_b200_pileup.h"):
+    for h in ("clair3_b200.h", "clair3_b200_debug.h", "clair3_b200_pileup.h", "clair3_b200_fa.h"):
         headers.append(os.path.join(os.path.dirname(HERE), "include", h))
     os.makedirs(OBJ_DIR, exist_ok=True)
     nvcc = _nvcc()

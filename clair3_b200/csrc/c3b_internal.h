@@ -295,3 +295,39 @@ int c3b_launch_ingest_fa_tc(const void *x, int dtype, int channels, int cpad, op
                             cudaStream_t s);
 int c3b_launch_spp_tc(const op_t *x, const PlanarGeom &g, op_t *out, int64_t batch, int c, int bp, cudaStream_t s);
 
+
+// A device buffer that grows on demand (25 % headroom); used by the pileup counter and the full-alignment builder for their
+// per-call inputs and scratch.  `what` names the owner in the error message.
+struct C3bBuf {
+    void *p = nullptr;
+    size_t cap = 0;
+    int ensure(size_t bytes, const char *what = "clair3_b200") {
+        if (bytes <= cap) return 0;
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
+        const size_t want = bytes + bytes / 4 + 256;
+        if (cudaMalloc(&p, want) != cudaSuccess) {
+            c3b_set_error("%s: cudaMalloc of %zu bytes failed", what, want);
+            return 1;
+        }
+        cap = want;
+        return 0;
+    }
+    void release() {
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
+    template <class T> T *as() const { return reinterpret_cast<T *>(p); }
+};
+
+// One input array of a call: a device pointer passes through, host memory is copied into b on stream s.
+static inline int c3b_upload(C3bBuf &b, const void *src, size_t bytes, int on_device, const void **dev, cudaStream_t s,
+                             const char *what) {
+    if (on_device) { *dev = src; return 0; }
+    if (b.ensure(bytes ? bytes : 1, what)) return 1;
+    if (bytes) C3B_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, s));
+    *dev = b.p;
+    return 0;
+}

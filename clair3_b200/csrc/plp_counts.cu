@@ -587,28 +587,8 @@ __global__ void __launch_bounds__(TILE) plp_cands_kernel(CandArgs A) {
     }
 }
 
-struct DBuf {
-    void *p = nullptr;
-    size_t cap = 0;
-    int ensure(size_t bytes) {
-        if (bytes <= cap) return 0;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        size_t want = bytes + bytes / 4 + 256;
-        if (cudaMalloc(&p, want) != cudaSuccess) {
-            c3b_set_error("c3b_plp: cudaMalloc of %zu bytes failed", want);
-            return 1;
-        }
-        cap = want;
-        return 0;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-    template <class T> T *as() const { return reinterpret_cast<T *>(p); }
+struct DBuf : C3bBuf {
+    int ensure(size_t bytes) { return C3bBuf::ensure(bytes, "c3b_plp"); }
 };
 
 }  // namespace
@@ -665,11 +645,7 @@ int c3b_plp_create(c3b_plp **out, int device_ordinal) {
 }
 
 static int plp_upload(DBuf &b, const void *src, size_t bytes, int on_device, const void **dev, cudaStream_t s) {
-    if (on_device) { *dev = src; return 0; }
-    if (b.ensure(bytes ? bytes : 1)) return 1;
-    if (bytes) C3B_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, s));
-    *dev = b.p;
-    return 0;
+    return c3b_upload(b, src, bytes, on_device, dev, s, "c3b_plp");
 }
 
 int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64_t start, int64_t end, const char *ref_seq,

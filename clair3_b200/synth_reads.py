@@ -157,3 +157,56 @@ def aligned_bases(rec):
     ops = rec["cigar"] & 15
     lens = rec["cigar"] >> 4
     return int(lens[np.isin(ops, list(_REF))].sum())
+
+
+def random_fa_case(seed, region_len=3000, depth=30, read_len=1500, n_cand=40, n_var=12, dup_frac=0.05, dwell=False, n_base_rate=0.003,
+                   long_ins=True, clip_frac=0.3, mv_missing_frac=0.1):
+    """A full-alignment test case on a contig that starts at position 0: records with base qualities, read names (``dup_frac`` of
+    them repeating an earlier name) and, with ``dwell``, ``mv`` move tables; strictly ascending candidates (>= 16) and sorted
+    phased heterozygous SNPs ``(position, ref_base, alt_base, genotype, phase_set)``.  Query bases are A/C/G/T with a few N; the
+    reference has soft-masked (lower-case) stretches and a few N.  Returns (records, ref_seq, candidates, variants)."""
+    rng = np.random.default_rng(seed + 7919)
+    rec, ref, rs = random_alignment(region_len, depth, read_len=read_len, seed=seed, n_rate=0.0, origin=read_len,
+                                    clip_frac=clip_frac, short_ins=not long_ins)
+    assert rs == 0
+    n = len(rec["pos"])
+    lq = rec["l_qseq"].astype(np.int64)
+    seq = rec["seq"].copy()
+    for r in range(n):                                    # a few N read bases (nt16 15): alt 100, counted as A
+        k = rng.binomial(int(lq[r]), n_base_rate)
+        for q in rng.integers(0, max(int(lq[r]), 1), k):
+            b = int(rec["seq_off"][r]) + int(q >> 1)
+            seq[b] = (seq[b] & 0x0F) | 0xF0 if q % 2 == 0 else (seq[b] & 0xF0) | 0x0F
+    rec["seq"] = seq
+    rec["qual"] = rng.integers(0, 61, int(lq.sum())).astype(np.uint8)
+    rec["qual_off"] = np.concatenate([[0], np.cumsum(lq)]).astype(np.int64)
+    names = []
+    for r in range(n):
+        names.append(names[rng.integers(0, r)] if r and rng.random() < dup_frac else "read_%d_%d" % (seed, r))
+    enc = [s.encode() for s in names]
+    rec["qname"] = np.frombuffer(b"".join(enc), dtype=np.uint8).copy()
+    rec["qname_off"] = np.concatenate([[0], np.cumsum([len(e) for e in enc])]).astype(np.int64)
+    if dwell:
+        mv, off = [], [0]
+        for r in range(n):
+            if rng.random() < mv_missing_frac:
+                off.append(off[-1])
+                continue
+            runs = rng.geometric(0.3, int(lq[r]) + int(rng.integers(-3, 4)))      # samples per base, a few bases more or less
+            runs[rng.random(len(runs)) < 0.01] += 140                             # > 127: the int8 channel wraps
+            m = np.zeros(1 + int(runs.sum()), np.int32)
+            m[0] = 5                                                              # the stride element
+            m[1 + np.concatenate([[0], np.cumsum(runs)[:-1]])] = 1
+            mv.append(m)
+            off.append(off[-1] + len(m))
+        rec["mv"] = np.concatenate(mv) if mv else np.zeros(0, np.int32)
+        rec["mv_off"] = np.array(off, np.int64)
+    lo, hi = read_len, read_len + region_len
+    cand = np.unique(rng.integers(lo, hi, n_cand)).astype(np.int64)
+    vpos = np.unique(rng.integers(lo - 200, hi + 200, n_var))
+    variants = []
+    for p in vpos:
+        rb = ref[int(p)].upper()
+        ab = "ACGT".replace(rb, "")[int(rng.integers(0, 3))] if rb in "ACGT" else "A"
+        variants.append((int(p), rb, ab, int(rng.integers(1, 3)), int(1000 + (p // 700))))
+    return rec, ref, cand, variants
