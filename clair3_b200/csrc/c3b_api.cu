@@ -709,6 +709,8 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
         taps["lstm2"] = {b.h2, 1, 2, (int64_t)C3B_T * 320, (int)bp, {}};
         taps["l4_pre"] = {b.z4, 0, 5, 128, (int)bp, {}};
         taps["l4_pre"].nsplit = nsplit;
+        taps["lstm1_x"] = {b.xs, 1, 7, C3B_X1_COLS, (int)bp, {}};
+        taps["lstm2_pregates"] = {b.pg, 1, 7, 1280, (int)bp, {}};
     }
     return 0;
 }
@@ -723,7 +725,8 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
     for (int i = 1; i < 4; ++i) { hh[i] = conv_out(hh[i - 1]); ww[i] = conv_out(ww[i - 1]); }
     const int chans[4] = {m->channels, 64, 128, 256};
     const bool f32 = m->precision == C3B_PREC_FP32;
-    const char *tapname[3][2] = {{"conv1", "res_block1"}, {"conv3", "res_block2"}, {"conv5", "res_block3"}};
+    const char *tapname[3][3] = {{"conv1", "res_block1", "res_block1_mid"}, {"conv3", "res_block2", "res_block2_mid"},
+                                 {"conv5", "res_block3", "res_block3_mid"}};
 
     if (f32) {
         w->fa_zeroed = false;       // this path overwrites the region the tensor-core path keeps zero-bordered
@@ -813,6 +816,7 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
     if (tap) {
         for (int l = 0; l < 3; ++l) {
             taps[tapname[l][0]] = {act[l][0], 1, 4, chans[l + 1], 0, geo[l]};
+            taps[tapname[l][2]] = {act[l][1], 1, 4, chans[l + 1], 0, geo[l]};
             if (l < 2) {
                 taps[tapname[l][1]] = {act[l][2], 1, 6, chans[l + 1], 0, geo[l + 1]};
                 taps[tapname[l][1]].h = geo[l].h;
@@ -1019,7 +1023,7 @@ extern "C" int c3b_get_tap(c3b_model *m, const char *name, float *host_out, int6
         const int64_t n = m->last_batch;
         const int64_t per_site = t.layout == 4 ? t.inner * t.geom.h * t.geom.w
                                  : t.layout == 6 ? t.inner * t.h * t.w
-                                                 : t.inner * (t.layout == 3 ? C3B_T : 1);
+                                                 : t.inner * (t.layout == 3 || t.layout == 7 ? C3B_T : 1);
         const int64_t count = n * per_site;
         if (*count_inout < count || !host_out) { *count_inout = count; c3b_set_error("c3b_get_tap: buffer too small"); return 1; }
         C3B_CUDA(cudaStreamSynchronize(w->stream));
@@ -1027,7 +1031,7 @@ extern "C" int c3b_get_tap(c3b_model *m, const char *name, float *host_out, int6
                                   : t.layout == 5 ? (int64_t)t.nsplit * t.bp * t.inner
                                   : t.layout == 4 ? (t.inner / 8) * t.geom.p * 8
                                   : t.layout == 6 ? 4 * (t.inner / 8) * t.geom.p * 8
-                                                  : t.inner * (int64_t)t.bp * (t.layout == 3 ? C3B_T : 1);
+                                                  : t.inner * (int64_t)t.bp * (t.layout == 3 || t.layout == 7 ? C3B_T : 1);
         std::vector<float> tmp((size_t)src_count);
         if (t.fmt == 0) {
             C3B_CUDA(cudaMemcpy(tmp.data(), t.ptr, (size_t)src_count * 4, cudaMemcpyDeviceToHost));
@@ -1064,6 +1068,10 @@ extern "C" int c3b_get_tap(c3b_model *m, const char *name, float *host_out, int6
                         for (int64_t k = 0; k < t.inner; ++k)
                             host_out[((b * t.h + hh) * t.w + wv) * t.inner + k] =
                                 tmp[c3b_parity_offset(g, (int)t.inner, b, hh + 1, wv + 1) + (size_t)(k >> 3) * g.p * 8 + (k & 7)];
+        } else if (t.layout == 7) {        // row-major time-major [33*bp][inner] (row t*bp + b) -> [n][33][inner]
+            for (int64_t b = 0; b < n; ++b)
+                for (int tt = 0; tt < C3B_T; ++tt)
+                    memcpy(host_out + (b * C3B_T + tt) * t.inner, tmp.data() + ((size_t)tt * t.bp + b) * t.inner, (size_t)t.inner * 4);
         } else {                           // tile-major, rows t*bp + b: [33*bp/128][inner/8][128][8] -> [n][33][inner]
             for (int64_t b = 0; b < n; ++b)
                 for (int tt = 0; tt < C3B_T; ++tt)

@@ -160,6 +160,7 @@ struct Tap {
     int layout;     // 0 [B][inner] row-major; 2 k-group-planar [inner/8][bp][8] (row = site);
                     // 3 k-group-planar time-major [inner/8][33*bp][8] (row = t*bp + site) -> [B][33][inner]
                     // 4 zero-padded planar feature map [inner/8][geom.p][8] -> NHWC [B][h][w][inner]
+                    // 7 row-major time-major [33*bp][inner] (row = t*bp + site) -> [B][33][inner]
     int64_t inner;
     int bp;
     PlanarGeom geom;

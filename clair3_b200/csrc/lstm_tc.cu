@@ -15,8 +15,8 @@
 //
 // LSTM1 (H=128): K = 48 + 128.  The 48 x columns are [hi(x) (18) | 1 | lo(x) (18) | 0...]: the raw counts are unbounded integers
 // (the reference's GPU branch does not rescale depth, clair3/CallVariantsFromCffi.py:299-353), fp16 is exact only to 2048, so
-// every count is split as x = hi + lo with hi = fp16(x) and lo = fp16(x - hi) - exact for |x| <= 131 008, saturating beyond -
-// and W_ih multiplies both parts (fp32 accumulate: the same result as an exact-input product).  Column 18 is a constant 1 that
+// every count is split as x = hi + lo with hi = fp16(x) and lo = fp16(x - hi) - exact for |x| <= 67 552; beyond that lo is
+// rounded (error <= 16, <= 2^-12 relative) up to 131 008, and saturates past it - and W_ih multiplies both parts (fp32 accumulate: the same result as an exact-input product).  Column 18 is a constant 1 that
 // carries b_ih + b_hh, so the x projection and the bias are fused into the same MMAs.
 // LSTM2 (H=160, input 256): the input projection W_ih*h1 (+bias) is a separate big GEMM (proj_tc.cu) that leaves fp16
 // pre-gates pg[t*bp + site][dir*640 + C] in gate-quad order (c3b_lstm2_pg_row: columns 128p + 4u .. +3 = gates i, f, g, o of
@@ -303,7 +303,8 @@ __device__ __forceinline__ float ingest_to_float(T v) { return (float)v; }
 // Dense [batch][33][channels] tensor, or (starts != nullptr) 33-row windows of the per-column count matrix [n_cols][channels]
 // (libclair3's plp_data.matrix; preprocess/CreateTensorPileupFromCffi.py:362-394 slices the same windows on the host, zero
 // rows where a window overhangs the matrix) -> xs[t][bp][48] fp16 with columns [hi(x) | 1 | lo(x) | 0..]: hi = fp16(x)
-// (saturating at +-65504), lo = fp16(x - hi), so hi + lo == x exactly for |x| <= 131 008; column `channels` = constant 1
+// (saturating at +-65504), lo = fp16(x - hi), so hi + lo == x exactly for |x| <= 67 552 (past 65 519 hi stays at 65 504 and
+// lo > 2048 is itself rounded: error <= 16, <= 2^-12 relative, up to 131 008; saturating beyond); column `channels` = constant 1
 // (LSTM1's bias column).
 template <typename T>
 __global__ void ingest_pileup_tc_kernel(const T *__restrict__ x, const int64_t *__restrict__ starts, int64_t n_cols,
