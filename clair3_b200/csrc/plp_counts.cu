@@ -161,6 +161,7 @@ struct CountArgs {
     // optional export of the candidate columns' allele lists (for the all_alt_info text): null = off
     uint32_t *al_meta, *al_read, *al_qpos, *al_cnt;
     int32_t *al_off, *al_n;   // [W] first record / number of records of a column
+    int32_t *ins_last;        // [W] last read with an insertion on a candidate column, -1 = none
     int *al_used;
     int al_cap;
 };
@@ -321,6 +322,7 @@ __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
     }
 
     int depth = 0, head = -1;
+    int ins_last = -1;       // the last read with an insertion here: did a put of a present key follow the last new string?
     bool covered = false;
     for (int64_t r = lo; r < hi; ++r) {                      // warp-uniform trip count
         const int64_t rp = __ldg(A.R.pos + r), re = __ldg(A.rend + r);
@@ -344,8 +346,10 @@ __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
             int nb = 0;
             if (op != 2u && op != 3u)
                 nb = nib_at(A.R.seq + __ldg(A.R.seq_off + r), __ldg(A.R.l_qseq + r), (long long)y0 + (off - (xend - (int)(cw >> 4))));
-            if (plp_visit(A, cnt, tid, cb, nc, off, k, cw, xend, y0, rev, nb, depth, e_meta, e_q0))
+            if (plp_visit(A, cnt, tid, cb, nc, off, k, cw, xend, y0, rev, nb, depth, e_meta, e_q0)) {
                 plp_event(A, P, cnt, tid, e_meta, e_q0, (uint32_t)r, head);
+                if (e_meta >> 31) ins_last = (int)r;
+            }
         }
     }
 
@@ -400,6 +404,7 @@ __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
                 if (base + n > A.al_cap) { atomicOr(A.status, 8); n = 0; base = 0; }
                 A.al_off[p - A.start] = base;
                 A.al_n[p - A.start] = n;
+                A.ins_last[p - A.start] = pass ? ins_last : -1;
                 int wr = base + n - 1;
                 for (int i = head; i >= 0 && wr >= base; i = NODE(next, i), --wr) {
                     A.al_meta[wr] = NODE(meta, i);
@@ -414,7 +419,7 @@ __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
             }
         } else {
             ds[0] = ds[1] = ds[2] = ds[3] = ds[4] = ds[5] = 0;
-            if (A.al_meta) { A.al_off[p - A.start] = 0; A.al_n[p - A.start] = 0; }
+            if (A.al_meta) { A.al_off[p - A.start] = 0; A.al_n[p - A.start] = 0; A.ins_last[p - A.start] = -1; }
         }
         A.nquirk[p - A.start] = cnt[NFEAT * TILE + tid];
     }
@@ -600,7 +605,7 @@ struct c3b_plp {
     // scratch
     DBuf opx, opy, rend, pmax, rows32, dstats, nquirk, dci, tile_cov, tile_off, tile_cand, tile_coff;
     DBuf g_meta, g_read, g_qpos, g_cnt, g_next;
-    DBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n;   // allele export (params.alt_info)
+    DBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n, ins_last;   // allele export (params.alt_info)
     DBuf counters;      // int64 n_cols, int64 n_cand, int g_used, int status
     // outputs
     DBuf matrix, major, stats, cand_cols, wstart, cand_ok, gv_ref, gv_tot;
@@ -712,7 +717,8 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     if (w->gvcf && (w->gv_ref.ensure(Wz * 8) || w->gv_tot.ensure(Wz * 8))) return 1;
     w->alleles = params->alt_info != 0;
     if (w->alleles && (w->al_meta.ensure((size_t)AL_CAP * 4) || w->al_read.ensure((size_t)AL_CAP * 4) || w->al_qpos.ensure((size_t)AL_CAP * 4) ||
-                       w->al_cnt.ensure((size_t)AL_CAP * 4) || w->al_off.ensure(Wz * 4) || w->al_n.ensure(Wz * 4)))
+                       w->al_cnt.ensure((size_t)AL_CAP * 4) || w->al_off.ensure(Wz * 4) || w->al_n.ensure(Wz * 4) ||
+                       w->ins_last.ensure(Wz * 4)))
         return 1;
     C3B_CUDA(cudaMemsetAsync(w->counters.p, 0, 32, s));
     if (w->gvcf && W > 0) {
@@ -746,7 +752,8 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         A.g_meta = w->g_meta.as<uint32_t>(); A.g_read = w->g_read.as<uint32_t>(); A.g_qpos = w->g_qpos.as<uint32_t>();
         A.g_cnt = w->g_cnt.as<uint32_t>(); A.g_next = w->g_next.as<int32_t>(); A.g_used = g_used; A.status = status;
         A.al_meta = w->alleles ? w->al_meta.as<uint32_t>() : nullptr; A.al_read = w->al_read.as<uint32_t>(); A.al_qpos = w->al_qpos.as<uint32_t>();
-        A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_off = w->al_off.as<int32_t>(); A.al_n = w->al_n.as<int32_t>(); A.al_used = al_used; A.al_cap = AL_CAP;
+        A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_off = w->al_off.as<int32_t>(); A.al_n = w->al_n.as<int32_t>();
+        A.ins_last = w->ins_last.as<int32_t>(); A.al_used = al_used; A.al_cap = AL_CAP;
         const size_t smem = (size_t)NCNT * TILE * 4 + (size_t)NP * 20;
         plp_count_tile_kernel<<<tiles, TILE, smem, s>>>(A);
         plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(w->tile_cov.as<int32_t>(), w->tile_off.as<int64_t>(), tiles, n_cols_dev);
@@ -808,7 +815,7 @@ int c3b_plp_fetch(c3b_plp *w, int64_t *matrix, int64_t *major, int32_t *stats, i
     return 0;
 }
 
-int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, uint32_t *meta, uint32_t *read, uint32_t *qpos, uint32_t *cnt,
+int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, int32_t *ins_last, uint32_t *meta, uint32_t *read, uint32_t *qpos, uint32_t *cnt,
                           int64_t capacity, int64_t *n_alleles) {
     if (!w) { c3b_set_error("c3b_plp_fetch_alleles: null workspace"); return 1; }
     if (w->n_cols < 0 && c3b_plp_sizes(w, nullptr, nullptr)) return 1;
@@ -818,6 +825,7 @@ int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, uint32_t *
     cudaStream_t s = w->stream;
     if (al_off && w->W) C3B_CUDA(cudaMemcpyAsync(al_off, w->al_off.p, (size_t)w->W * 4, cudaMemcpyDeviceToHost, s));
     if (al_n && w->W) C3B_CUDA(cudaMemcpyAsync(al_n, w->al_n.p, (size_t)w->W * 4, cudaMemcpyDeviceToHost, s));
+    if (ins_last && w->W) C3B_CUDA(cudaMemcpyAsync(ins_last, w->ins_last.p, (size_t)w->W * 4, cudaMemcpyDeviceToHost, s));
     if (meta || read || qpos || cnt) {
         if (capacity < n) { c3b_set_error("c3b_plp_fetch_alleles: capacity %lld < %lld records", (long long)capacity, (long long)n); return 1; }
         if (n) {
@@ -860,7 +868,7 @@ void c3b_plp_destroy(c3b_plp *w) {
                    &w->opx, &w->opy, &w->rend, &w->pmax, &w->rows32, &w->dstats, &w->nquirk, &w->dci, &w->tile_cov, &w->tile_off,
                    &w->tile_cand, &w->tile_coff, &w->g_meta, &w->g_read, &w->g_qpos, &w->g_cnt, &w->g_next, &w->counters,
                    &w->matrix, &w->major, &w->stats, &w->cand_cols, &w->wstart, &w->cand_ok, &w->gv_ref, &w->gv_tot,
-                   &w->al_meta, &w->al_read, &w->al_qpos, &w->al_cnt, &w->al_off, &w->al_n};
+                   &w->al_meta, &w->al_read, &w->al_qpos, &w->al_cnt, &w->al_off, &w->al_n, &w->ins_last};
     for (DBuf *b : all) b->release();
     if (w->ev0) cudaEventDestroy(w->ev0);
     if (w->ev1) cudaEventDestroy(w->ev1);

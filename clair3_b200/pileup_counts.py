@@ -162,7 +162,7 @@ class PileupCounter:
                                   ffi.cast("void *", stream)))
         self._keep = (rec, ref, refbuf, st)          # buffers stay alive while the copies / kernels are in flight
         self._shape = (int(end) - int(start), bool(gvcf))
-        self._alt = (bool(alt_info), int(start), int(ref_start), int(max_indel_length))
+        self._alt = (bool(alt_info), int(start), int(end), int(ref_start), int(max_indel_length))
         return self
 
     def sizes(self):
@@ -210,7 +210,7 @@ class PileupCounter:
         SNP alleles in A C G T order, deletions by length, insertions in the iteration order of the reference's khash string
         counter, the remaining reference depth last.  The GPU supplies the allele lists (``c3b_plp_fetch_alleles``), the text is
         formatted here from the HOST records of the count (the inserted bases are read from the representative reads)."""
-        want, start, ref_start, max_indel = self._alt
+        want, start, end, ref_start, max_indel = self._alt
         if not want:
             raise C3BError("alt_info_strings: count(..., alt_info=True) first")
         rec, ref = self._keep[0], self._keep[1]
@@ -219,12 +219,13 @@ class PileupCounter:
         r = fetched if fetched is not None else self.fetch()
         W = self._shape[0]
         n = ffi.new("int64_t *")
-        check(lib().c3b_plp_fetch_alleles(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, 0, n))
+        check(lib().c3b_plp_fetch_alleles(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, 0, n))
         na = int(n[0])
-        al_off, al_n = np.zeros(W, np.int32), np.zeros(W, np.int32)
+        al_off, al_n, ins_last = np.zeros(W, np.int32), np.zeros(W, np.int32), np.zeros(W, np.int32)
         meta, rd, qp, cn = (np.zeros(max(na, 1), np.uint32) for _ in range(4))
         c = ffi.cast
         check(lib().c3b_plp_fetch_alleles(self._h, c("int32_t *", al_off.ctypes.data), c("int32_t *", al_n.ctypes.data),
+                                          c("int32_t *", ins_last.ctypes.data),
                                           c("uint32_t *", meta.ctypes.data), c("uint32_t *", rd.ctypes.data),
                                           c("uint32_t *", qp.ctypes.data), c("uint32_t *", cn.ctypes.data), len(meta), n))
         out = []
@@ -233,7 +234,8 @@ class PileupCounter:
             a0 = int(al_off[p - start])
             sl = slice(a0, a0 + int(al_n[p - start]))
             out.append(format_alt_info(p, r["matrix"][ci], r["stats"][ci], ref, ref_start, max_indel,
-                                       meta[sl], rd[sl], qp[sl], cn[sl], rec))
+                                       meta[sl], rd[sl], qp[sl], cn[sl], rec, ins_last=int(ins_last[p - start]),
+                                       fetch_end=end + FETCH_EXPAND + 1))
         return out
 
     def forward(self, model):
@@ -354,8 +356,15 @@ def _insertion_bytes(rec, read, q0, length):
     return bytes(out)
 
 
-def format_alt_info(pos, row, stats, ref, ref_start, max_indel_length, meta, read, qpos, cnt, rec):
-    """One ``all_alt_info`` string (src/clair3_pileup.c:391-450) from a candidate's matrix row, its stats and its allele records."""
+FETCH_EXPAND = 1000      # mpileup_expand_reference_region (src/clair3_pileup.h:63): the reference fetches [start - 1000, end + 1000]
+
+
+def format_alt_info(pos, row, stats, ref, ref_start, max_indel_length, meta, read, qpos, cnt, rec, ins_last=-1, fetch_end=None):
+    """One ``all_alt_info`` string (src/clair3_pileup.c:391-450) from a candidate's matrix row, its stats and its allele records.
+    ``ins_last``: the last read with an insertion on the column - when it comes after the first read of the last new insertion
+    string, that put of a present string still grows a full khash table first (src/khash.h:310-318), which reorders the text.
+    ``fetch_end``: the end (exclusive) of the reference's FASTA fetch, ``end + 1001`` (src/clair3_pileup.c:188-190) - the deletion
+    text stops there; None = the end of ``ref``."""
     off = pos - ref_start
     rb = ref[off:off + 1].upper() if 0 <= off < len(ref) else b"N"
     rbc = rb.decode("latin-1")
@@ -382,11 +391,13 @@ def format_alt_info(pos, row, stats, ref, ref_start, max_indel_length, meta, rea
         d = dels[length]
         ref_depth -= d
         if d > 0 and length <= max_indel_length:
-            tail = ref[off + 1:off + 1 + length]
+            stop = off + 1 + length if fetch_end is None else min(off + 1 + length, fetch_end - ref_start)
+            tail = ref[off + 1:stop]
             nul = tail.find(b"\0")
             parts.append("D%s %d " % ((tail if nul < 0 else tail[:nul]).decode("latin-1"), d))
     ins_order.sort(key=lambda k: ins_cnt[k][1])           # first occurrence over both strands = the reference's insertion order
-    for j in khash_iteration_order(ins_order):
+    again = bool(ins_order) and ins_last > ins_cnt[ins_order[-1]][1]
+    for j in khash_iteration_order(ins_order, put_after_last=again):
         key = ins_order[j]
         val = ins_cnt[key][0]
         ref_depth -= val

@@ -87,13 +87,17 @@ int c3b_plp_fetch(c3b_plp *w, int64_t *matrix, int64_t *major, int32_t *stats, i
 /* The distinct indel alleles of every column that passed the allele-frequency test (needs params.alt_info), in order of first
  * occurrence - what the reference keeps per column in dels_f / dels_r and its three insertion-string counters:
  *   al_off / al_n [end - start] int32   first record and number of records of the column at position start + i (0 elsewhere)
+ *   ins_last [end - start] int32        the last read (index into the records of the count) with an insertion on that column, -1
+ *                                       for none or for a column that did not pass: the reference's insertion counter grows a full
+ *                                       table on every put, so whether a read after the last new string put a present one again
+ *                                       changes the counter's bucket order (src/khash.h:310-318)
  *   meta  [n]  uint32   insertion << 31 | reverse strand << 30 | length
  *   read  [n]  uint32   index (into the records of the count) of the first read that showed the allele
  *   qpos  [n]  uint32   query offset of its first inserted base in that read (insertions)
  *   cnt   [n]  uint32   reads of that strand showing it
  * Any pointer may be NULL; n_alleles alone sizes the buffers.  clair3_b200/pileup_counts.py formats the all_alt_info strings
  * (src/clair3_pileup.c:391-450, insertion alleles in the reference's khash bucket order) from these on the host. */
-int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, uint32_t *meta, uint32_t *read, uint32_t *qpos, uint32_t *cnt,
+int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, int32_t *ins_last, uint32_t *meta, uint32_t *read, uint32_t *qpos, uint32_t *cnt,
                           int64_t capacity, int64_t *n_alleles);
 
 /* Device views of the same results, valid until the next c3b_plp_count on w: matrix and window_starts

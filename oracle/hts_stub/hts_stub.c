@@ -1,10 +1,13 @@
 /*
- * In-memory stand-in for the htslib calls of the reference's full-alignment tensor builder (see htslib/sam.h, htslib/faidx.h and
- * fa_ref_shim.h next to this file).  Written from the SAM/BAM specification; no htslib code.  TEST INFRASTRUCTURE ONLY.
+ * In-memory stand-in for the htslib calls of the reference's full-alignment tensor builder and pileup feature counter (see
+ * htslib/sam.h, htslib/faidx.h and fa_ref_shim.h next to this file).  Written from the SAM/BAM specification and htslib's documented
+ * pileup behaviour; no htslib code.  TEST INFRASTRUCTURE ONLY.
  *
- * The binding registers one contig (fa_ref_set_contig) and the decoded records of that contig (fa_ref_set_records) before each
- * call of calculate_clair3_full_alignment; every file / index / header handle is a dummy that refers to them.
+ * The bindings (oracle/fa_ref.py, oracle/pileup_ref.py) register one contig (fa_ref_set_contig) and the decoded records of that
+ * contig (fa_ref_set_records) before each call of calculate_clair3_full_alignment / calculate_clair3_pileup; every file / index /
+ * header handle is a dummy that refers to them.
  */
+#include <errno.h>
 #include <limits.h>
 #include <stdarg.h>
 #include <stdint.h>
@@ -114,17 +117,36 @@ void fa_ref_set_records(int64_t n, const int64_t *pos, const uint16_t *flag, con
 /* ------------------------------------------------------------------------------------------------ handles */
 struct htsFile { int dummy; };
 struct hts_idx_t { int dummy; };
-struct sam_hdr_t { int dummy; };
 struct faidx_t { int dummy; };
 struct hts_itr_t { int64_t next; hts_pos_t beg, end; int tid; };
 
 htsFile *sam_open(const char *fn, const char *mode) { (void)fn; (void)mode; return (htsFile *)calloc(1, sizeof(htsFile)); }
+htsFile *hts_open(const char *fn, const char *mode) { return sam_open(fn, mode); }
 int hts_set_opt(htsFile *fp, enum hts_fmt_option opt, ...) { (void)fp; (void)opt; return 0; }
 hts_idx_t *sam_index_load(htsFile *fp, const char *fn) { (void)fp; (void)fn; return (hts_idx_t *)calloc(1, sizeof(hts_idx_t)); }
-sam_hdr_t *sam_hdr_read(htsFile *fp) { (void)fp; return (sam_hdr_t *)calloc(1, sizeof(sam_hdr_t)); }
+
+sam_hdr_t *sam_hdr_read(htsFile *fp) {
+    (void)fp;
+    sam_hdr_t *h = (sam_hdr_t *)calloc(1, sizeof(sam_hdr_t));
+    if (!h) return NULL;
+    const char *nm = g_contig_name ? g_contig_name : "";
+    h->target_name = (char **)calloc(1, sizeof(char *));
+    if (h->target_name) h->target_name[0] = (char *)malloc(strlen(nm) + 1);
+    if (!h->target_name || !h->target_name[0]) { free(h->target_name); free(h); return NULL; }
+    strcpy(h->target_name[0], nm);
+    h->n_targets = 1;
+    return h;
+}
+
 int bam_name2id(sam_hdr_t *h, const char *ref) { (void)h; return g_contig_name && strcmp(ref, g_contig_name) == 0 ? 0 : -1; }
 void hts_itr_destroy(hts_itr_t *itr) { free(itr); }
-void sam_hdr_destroy(sam_hdr_t *h) { free(h); }
+
+void sam_hdr_destroy(sam_hdr_t *h) {
+    if (!h) return;
+    for (int32_t i = 0; i < h->n_targets; ++i) free(h->target_name[i]);
+    free(h->target_name);
+    free(h);
+}
 void hts_idx_destroy(hts_idx_t *idx) { free(idx); }
 int hts_close(htsFile *fp) { free(fp); return 0; }
 
@@ -226,6 +248,205 @@ void bam_destroy1(bam1_t *b) {
     if (!b) return;
     free(b->data);
     free(b);
+}
+
+int sam_read1(htsFile *fp, sam_hdr_t *h, bam1_t *b) { (void)fp; (void)h; (void)b; return -1; }
+int64_t bam_aux2i(const uint8_t *s) { (void)s; errno = EINVAL; return 0; }
+char *bam_aux2Z(const uint8_t *s) { (void)s; errno = EINVAL; return NULL; }
+
+hts_itr_t *sam_itr_querys(const hts_idx_t *idx, sam_hdr_t *hdr, const char *region) {
+    (void)hdr;
+    const char *colon = strrchr(region, ':');
+    const size_t nlen = colon ? (size_t)(colon - region) : strlen(region);
+    int beg, end;
+    if (!g_contig_name || strlen(g_contig_name) != nlen || strncmp(region, g_contig_name, nlen) != 0) return NULL;
+    hts_parse_reg(region, &beg, &end);
+    return sam_itr_queryi(idx, 0, beg, end);
+}
+
+/* ------------------------------------------------------------------------------------------------ pileup engine
+ * bam_mplp_* over ONE input, restated from htslib's documented pileup semantics (no htslib code):
+ *   - records are pulled one at a time through the caller's callback (the reference's read_bam, which applies its own flag and
+ *     MAPQ filters); they must come coordinate-sorted, and a record whose raw reference length (M/D/N/=/X) is 0 is dropped;
+ *   - a read is on column pos iff beg <= pos < beg + raw reference length; only columns with at least one read are reported, in
+ *     position order, reads in the order they were pulled; a column whose reads are all reference skips is still reported;
+ *   - overlapping mates are NOT removed (the reference never calls bam_mplp_init_overlaps);
+ *   - the operation under a column is located afresh from the start of the CIGAR: x / y = reference / query offset of its first
+ *     base (I and S advance y before it, M/=/X advance both, D/N only x);
+ *   - on M/=/X: qpos = y + (pos - x); on D or N: is_del = 1 and qpos = y; is_refskip = 1 on N;
+ *   - on the LAST base of an operation the next one is peeked: D, when the current one is not a D, gives indel = -(the run of
+ *     adjacent D's); I gives indel = +(the I's that follow, merged across P); P gives +(the I's after the pads, up to the next
+ *     reference-consuming operation), or 0 when there are none;
+ *   - the depth cap (bam_mplp_set_maxcnt) is asserted, not modelled: reaching it is an error.
+ * CIGAR operations of length 0 are rejected (htslib's incremental cursor can stop on them; a fresh location steps over them). */
+typedef struct {
+    bam1_t b;
+    hts_pos_t beg, end;
+} plp_read_t;
+
+struct bam_mplp_s {
+    bam_plp_auto_f func;
+    void *data;
+    int maxcnt;
+    plp_read_t *rd;            /* reads that may still cover the next column, in the order they were pulled */
+    int n, cap;
+    bam1_t next;               /* one record of lookahead */
+    int have_next, eof, error;
+    hts_pos_t pos, last_beg;
+    bam_pileup1_t *plp;
+    int plp_cap;
+};
+
+static int consumes_ref(int op) { return op == BAM_CMATCH || op == BAM_CDEL || op == BAM_CREF_SKIP || op == BAM_CEQUAL || op == BAM_CDIFF; }
+static int is_match_op(int op) { return op == BAM_CMATCH || op == BAM_CEQUAL || op == BAM_CDIFF; }
+
+bam_mplp_t bam_mplp_init(int n, bam_plp_auto_f func, void **data) {
+    if (n != 1) { fprintf(stderr, "hts_stub: bam_mplp_init supports one input, not %d\n", n); return NULL; }
+    bam_mplp_t m = (bam_mplp_t)calloc(1, sizeof(struct bam_mplp_s));
+    if (!m) return NULL;
+    m->func = func;
+    m->data = data[0];
+    m->maxcnt = 8000;
+    m->last_beg = -1;
+    return m;
+}
+
+void bam_mplp_set_maxcnt(bam_mplp_t m, int maxcnt) { m->maxcnt = maxcnt; }
+
+void bam_mplp_destroy(bam_mplp_t m) {
+    if (!m) return;
+    for (int i = 0; i < m->n; ++i) free(m->rd[i].b.data);
+    free(m->rd);
+    free(m->next.data);
+    free(m->plp);
+    free(m);
+}
+
+/* pull the next record with a non-zero reference length into the lookahead; 0 = none left, -1 = error */
+static int pull(bam_mplp_t m) {
+    while (!m->eof) {
+        int ret = m->func(m->data, &m->next);
+        if (ret < 0) { m->eof = 1; break; }
+        const uint32_t *cig = bam_get_cigar(&m->next);
+        hts_pos_t rlen = 0;
+        for (uint32_t k = 0; k < m->next.core.n_cigar; ++k) {
+            if (bam_cigar_oplen(cig[k]) == 0) { fprintf(stderr, "hts_stub: zero-length CIGAR operation\n"); return -1; }
+            if (consumes_ref(bam_cigar_op(cig[k]))) rlen += bam_cigar_oplen(cig[k]);
+        }
+        if (m->next.core.pos < m->last_beg) { fprintf(stderr, "hts_stub: records are not coordinate-sorted\n"); return -1; }
+        m->last_beg = m->next.core.pos;
+        if (rlen == 0) continue;
+        m->have_next = 1;
+        return 1;
+    }
+    return 0;
+}
+
+/* move the lookahead record into the set of active reads */
+static int admit(bam_mplp_t m) {
+    if (m->n == m->cap) {
+        int nc = m->cap ? 2 * m->cap : 64;
+        plp_read_t *r = (plp_read_t *)realloc(m->rd, sizeof(plp_read_t) * (size_t)nc);
+        if (!r) return -1;
+        m->rd = r;
+        m->cap = nc;
+    }
+    plp_read_t *r = &m->rd[m->n];
+    memset(r, 0, sizeof(*r));
+    r->b = m->next;
+    r->b.data = (uint8_t *)malloc(m->next.l_data > 0 ? (size_t)m->next.l_data : 1);
+    if (!r->b.data) return -1;
+    memcpy(r->b.data, m->next.data, (size_t)m->next.l_data);
+    r->b.m_data = (uint32_t)(m->next.l_data > 0 ? m->next.l_data : 1);
+    r->beg = m->next.core.pos;
+    r->end = r->beg;
+    const uint32_t *cig = bam_get_cigar(&r->b);
+    for (uint32_t k = 0; k < r->b.core.n_cigar; ++k)
+        if (consumes_ref(bam_cigar_op(cig[k]))) r->end += bam_cigar_oplen(cig[k]);
+    ++m->n;
+    m->have_next = 0;
+    return 0;
+}
+
+/* what read b shows on column pos (beg <= pos < end) */
+static void describe(bam1_t *b, hts_pos_t pos, bam_pileup1_t *p) {
+    const uint32_t *cig = bam_get_cigar(b);
+    const int n = (int)b->core.n_cigar;
+    hts_pos_t x = b->core.pos, y = 0;
+    int k;
+    for (k = 0; k < n; ++k) {
+        const int op = bam_cigar_op(cig[k]);
+        const hts_pos_t l = bam_cigar_oplen(cig[k]);
+        if (consumes_ref(op)) {
+            if (pos < x + l) break;
+            x += l;
+            if (is_match_op(op)) y += l;
+        } else if (op == BAM_CINS || op == BAM_CSOFT_CLIP) {
+            y += l;
+        }
+    }
+    const int op = bam_cigar_op(cig[k]);
+    const hts_pos_t l = bam_cigar_oplen(cig[k]);
+    memset(p, 0, sizeof(*p));
+    p->b = b;
+    p->cigar_ind = k;
+    if (pos == x + l - 1 && k + 1 < n) {
+        const int op2 = bam_cigar_op(cig[k + 1]);
+        int j;
+        if (op2 == BAM_CDEL && op != BAM_CDEL) {
+            for (j = k + 1; j < n && bam_cigar_op(cig[j]) == BAM_CDEL; ++j) p->indel -= (int)bam_cigar_oplen(cig[j]);
+        } else if (op2 == BAM_CINS) {
+            for (j = k + 1; j < n && (bam_cigar_op(cig[j]) == BAM_CINS || bam_cigar_op(cig[j]) == BAM_CPAD); ++j)
+                if (bam_cigar_op(cig[j]) == BAM_CINS) p->indel += (int)bam_cigar_oplen(cig[j]);
+        } else if (op2 == BAM_CPAD) {
+            for (j = k + 1; j < n && !consumes_ref(bam_cigar_op(cig[j])); ++j)
+                if (bam_cigar_op(cig[j]) == BAM_CINS) p->indel += (int)bam_cigar_oplen(cig[j]);
+        }
+    }
+    if (is_match_op(op)) {
+        p->qpos = (int32_t)(y + (pos - x));
+    } else {
+        p->is_del = 1;
+        p->qpos = (int32_t)y;
+        p->is_refskip = op == BAM_CREF_SKIP;
+    }
+    p->is_head = pos == b->core.pos;
+}
+
+int bam_mplp_auto(bam_mplp_t m, int *tid, int *pos, int *n_plp, const bam_pileup1_t **plp) {
+    if (m->error) return -1;
+    for (;;) {
+        if (!m->have_next && pull(m) < 0) { m->error = 1; return -1; }
+        if (m->n == 0) {
+            if (!m->have_next) return 0;
+            if (m->pos < m->next.core.pos) m->pos = m->next.core.pos;         /* jump over the uncovered columns */
+        }
+        while (m->have_next && m->next.core.pos <= m->pos) {
+            if (admit(m)) { m->error = 1; return -1; }
+            if (pull(m) < 0) { m->error = 1; return -1; }
+        }
+        int w = 0;                                                            /* retire reads that ended before this column */
+        for (int i = 0; i < m->n; ++i) {
+            if (m->rd[i].end <= m->pos) free(m->rd[i].b.data);
+            else m->rd[w++] = m->rd[i];
+        }
+        m->n = w;
+        if (m->n == 0) continue;
+        if (m->n >= m->maxcnt) { fprintf(stderr, "hts_stub: depth %d reaches the pileup cap %d\n", m->n, m->maxcnt); m->error = 1; return -1; }
+        if (m->n > m->plp_cap) {
+            bam_pileup1_t *q = (bam_pileup1_t *)realloc(m->plp, sizeof(bam_pileup1_t) * (size_t)m->n);
+            if (!q) { m->error = 1; return -1; }
+            m->plp = q;
+            m->plp_cap = m->n;
+        }
+        for (int i = 0; i < m->n; ++i) describe(&m->rd[i].b, m->pos, &m->plp[i]);
+        *tid = 0;
+        *pos = (int)m->pos;
+        *n_plp = m->n;
+        plp[0] = m->plp;
+        ++m->pos;
+        return 1;
+    }
 }
 
 const char *hts_parse_reg(const char *s, int *beg, int *end) {

@@ -24,8 +24,9 @@
  *     - contiguous_flanking_num restarts whenever pre_pos == 0 (src/clair3_pileup.c:227-230);
  *     - all_alt_count accumulates the running maximum (src/clair3_pileup.c:356-360).
  *
- * PARITY UNPINNED: neither htslib nor libclair3 can be built in this image (no htslib, no network), the reference ships no
- * golden vectors for this function, so this restatement is pinned only by hand-worked known-answer cases (tests/test_pileup_oracle.py).
+ * Pinned against the reference's own C: oracle/pileup_ref.py compiles src/clair3_pileup.c and src/medaka_bamiter.c against the
+ * in-memory htslib stand-in of oracle/hts_stub/ (its pileup engine written independently of resolve() below), and
+ * tests/test_pileup_reference_cpu.py requires this restatement to equal it bit for bit on the cases of tests/plp_ref_cases.py.
  *
  * Build: oracle/build_oracle.py (gcc -O2 -shared) -> oracle/_build/libpileup_oracle.so
  */
@@ -46,6 +47,7 @@
 
 #define FEAT 18
 #define FLANK 16              /* pileup_flanking_base_num, src/clair3_pileup.h:93 */
+#define FETCH_EXPAND 1000     /* mpileup_expand_reference_region, src/clair3_pileup.h:63 */
 
 /* src/clair3_pileup.h:96-101 */
 static const int num2countbaseclair3[32] = {
@@ -167,8 +169,9 @@ typedef struct {
  * The insertion alleles are printed in the ITERATION ORDER of the reference's khash string counter ins_counts_all, i.e. by bucket.
  * khash (klib, vendored as src/khash.h) restated for an insert-only table: X31 string hash (:395-400), n_buckets a power of two >= 4,
  * triangular probing i = (i + ++step) & mask (:329), growth to the next power of two whenever n_occupied >= 0.77 * n_buckets at the
- * START of a put (:312-320), and the in-place "kick-out" rehash of kh_resize (:268-292).  Only the order of first occurrence of the
- * distinct keys matters (a put of a present key never moves anything). */
+ * START of EVERY put (:310-318), and the in-place "kick-out" rehash of kh_resize (:268-292).  What matters is the order of first
+ * occurrence of the distinct keys, and whether a put of a present key came after the last new one: that put does not move a key
+ * itself, but it still grows a full table first (3, 6, 12, 25, 49 ... keys). */
 typedef struct {
     uint32_t n, size, upper;
     int *slot;              /* bucket -> key index, -1 = empty */
@@ -219,8 +222,9 @@ static void khs_resize(khs_t *h, uint32_t want, const uint32_t *hashes) {
     h->upper = (uint32_t)(nn * 0.77 + 0.5);
 }
 
-/* order[0..n_keys): the key indices (first-occurrence order in, bucket order out) */
-static void khash_iteration_order(const uint32_t *hashes, int n_keys, int *order) {
+/* order[0..n_keys): the key indices (first-occurrence order in, bucket order out).  put_after_last: a put of a present key came
+ * after the last new one - kh_put still grows a full table first (:310-318), which changes the bucket order. */
+static void khash_iteration_order(const uint32_t *hashes, int n_keys, int put_after_last, int *order) {
     khs_t h = {0, 0, 0, NULL};
     for (int key = 0; key < n_keys; ++key) {
         if (h.size >= h.upper) khs_resize(&h, h.n + 1, hashes);
@@ -229,6 +233,7 @@ static void khash_iteration_order(const uint32_t *hashes, int n_keys, int *order
         h.slot[i] = key;
         ++h.size;
     }
+    if (put_after_last && h.size >= h.upper) khs_resize(&h, h.n + 1, hashes);
     int k = 0;
     for (uint32_t j = 0; j < h.n; ++j)
         if (h.slot[j] >= 0) order[k++] = h.slot[j];
@@ -299,6 +304,7 @@ int oracle_clair3_pileup(int64_t n_reads, const int64_t *rpos, const uint16_t *f
         int64_t del_cap = 32, *dels_f = NULL, *dels_r = NULL;
         ins_t *ins = NULL;
         int64_t n_ins = 0, cap_ins = 0;
+        int ins_again = 0;          /* the latest insertion put was of a string already present */
         int in_region = pos >= start;
         if (in_region) {
             dels_f = (int64_t *)calloc((size_t)del_cap, sizeof(int64_t));
@@ -352,8 +358,10 @@ int oracle_clair3_pileup(int64_t n_reads, const int64_t *rpos, const uint16_t *f
                     ins[n_ins].nibs = s;
                     ins[n_ins].cnt_f = ins[n_ins].cnt_r = 0;
                     ++n_ins;
+                    ins_again = 0;
                 } else {
                     free(s);
+                    ins_again = 1;
                 }
                 if (rev) ins[i].cnt_r += 1; else ins[i].cnt_f += 1;
             }
@@ -430,8 +438,8 @@ int oracle_clair3_pileup(int64_t n_reads, const int64_t *rpos, const uint16_t *f
                 if (d > 0 && i + 1 <= prm->max_indel_length) {
                     text_add(&txt, "D", 1);
                     for (int64_t q = 0; q <= i; ++q) {                          /* "%.*s" of ref_seq + offset + 1: raw case, stops at the end */
-                        int64_t o = off + 1 + q;
-                        if (o < 0 || o >= ref_len || ref_seq[o] == 0) break;
+                        int64_t o = off + 1 + q;                                /* of the contig or of the fetch, end + 1000 inclusive (:188-190) */
+                        if (o < 0 || o >= ref_len || ref_seq[o] == 0 || ref_start + o > end + FETCH_EXPAND) break;
                         text_add(&txt, ref_seq + o, 1);
                     }
                     n = snprintf(tmp, sizeof tmp, " %lld ", (long long)d);
@@ -442,7 +450,7 @@ int oracle_clair3_pileup(int64_t n_reads, const int64_t *rpos, const uint16_t *f
                 uint32_t *hs = (uint32_t *)malloc(sizeof(uint32_t) * (size_t)n_ins);
                 int *order = (int *)malloc(sizeof(int) * (size_t)n_ins);
                 for (int64_t i = 0; i < n_ins; ++i) hs[i] = x31(ins[i].nibs, ins[i].len);
-                khash_iteration_order(hs, (int)n_ins, order);
+                khash_iteration_order(hs, (int)n_ins, ins_again, order);
                 for (int64_t q = 0; q < n_ins; ++q) {
                     const ins_t *e = &ins[order[q]];
                     int64_t val = e->cnt_f + e->cnt_r;

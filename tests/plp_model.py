@@ -27,6 +27,7 @@ def model_pileup(rec, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.
     dels = [dict() for _ in range(W)]          # (strand, length) -> count
     ins = [dict() for _ in range(W)]           # (strand, string) -> count
     alle = [dict() for _ in range(W)]          # allele -> [first read, first inserted base in it, count], in order of first occurrence
+    ins_last = np.full(W, -1, np.int64)        # the last read with an insertion on the column (c3b_plp_fetch_alleles: ins_last)
     n = len(rec["pos"])
     for r in range(n):
         fl = int(rec["flag"][r])
@@ -92,7 +93,8 @@ def model_pileup(rec, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.
                 s = tuple(_nib(rec["seq"], so, lq, qpos + f0 + i) for i in range(indel))
                 ins[c][(rev, s)] = ins[c].get((rev, s), 0) + 1
                 alle[c].setdefault((1, rev, indel, s), [r, qpos + f0, 0])[2] += 1
-    rows, major, stats, alleles = [], [], [], []
+                ins_last[c] = r
+    rows, major, stats, alleles, last = [], [], [], [], []
     prev_emitted = None
     for c in range(W):
         if not covered[c]:
@@ -139,6 +141,7 @@ def model_pileup(rec, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.
         rows.append(m)
         major.append(p)
         alleles.append([((k[0] << 31) | (k[1] << 30) | k[2], v[0], v[1], v[2]) for k, v in alle[c].items()])
+        last.append(int(ins_last[c]))
         stats.append([d, ref_count, alt, del_count, ins_count, 1 if ok else 0])
     matrix = np.array(rows, np.int64).reshape(-1, 18)
     stats = np.array(stats, np.int32).reshape(-1, 6)
@@ -152,4 +155,5 @@ def model_pileup(rec, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.
         g = g and not (stats[c - 16:c + 17, 5] & 2).any()
         okw.append(1 if g else 0)
     return {"matrix": matrix, "major": major, "stats": stats, "cand_cols": cand, "cand_ok": np.array(okw, np.uint8),
-            "alleles": alleles}        # per emitted column: (meta, first read, query offset, count) as c3b_plp_fetch_alleles exports them
+            "alleles": alleles,        # per emitted column: (meta, first read, query offset, count) as c3b_plp_fetch_alleles exports them
+            "ins_last": np.array(last, np.int64)}

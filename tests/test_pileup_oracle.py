@@ -1,9 +1,9 @@
 """CPU checks of the pileup feature counter's oracle (oracle/pileup_oracle.c, the plain-C restatement of
 ``calculate_clair3_pileup``, HKU-BAL/Clair3 src/clair3_pileup.c:142-476) and of the host side of the GPU counter.
 
-The reference ships no golden vectors for this function and neither libclair3 nor htslib can be built here, so the oracle is
-pinned by hand-worked known-answer cases (every expected number below is derived in the comments from the reference's source
-lines) and cross-checked against an independent random-access Python model (tests/plp_model.py)."""
+The oracle is pinned against the reference's own calculate_clair3_pileup, compiled by oracle/pileup_ref.py, in
+tests/test_pileup_reference_cpu.py.  Here it is also checked against hand-worked known-answer cases (every expected number below
+is derived in the comments from the reference's source lines) and an independent random-access Python model (tests/plp_model.py)."""
 import os
 import sys
 
@@ -230,10 +230,12 @@ def test_counts_are_additive_over_read_subsets():
 
 
 @pytest.mark.parametrize("seed", range(6))
-def test_alt_info_text_host_formatter_matches_oracle(seed):
+def test_host_formatter_text_matches_oracle(seed):
     """The all_alt_info strings (src/clair3_pileup.c:391-450): the product's host formatter (clair3_b200.pileup_counts.format_alt_info,
     with its own restatement of khash's bucket order), fed with allele lists in the layout the GPU exports (taken here from the
-    random-access model), against the C oracle's text (which restates khash separately)."""
+    random-access model) - including the last read with an insertion on the column, from which the formatter replays the growth of a
+    full khash table on a put of a present string (src/khash.h:310-318; it reorders seeds 1 and 5) - against the C oracle's text
+    (which restates khash separately)."""
     from clair3_b200 import pileup_counts as pc
     wild = seed % 2 == 0
     rec, ref, rs = sr.random_alignment(400, depth=[15, 40, 28][seed % 3], read_len=[100, 300, 200][seed % 3], seed=40 + seed, wild=wild,
@@ -248,7 +250,8 @@ def test_alt_info_text_host_formatter_matches_oracle(seed):
     for ci in m["cand_cols"]:
         al = m["alleles"][ci]
         cols = [np.array([a[j] for a in al], dtype=np.uint32) for j in range(4)]
-        got.append(pc.format_alt_info(int(m["major"][ci]), m["matrix"][ci], m["stats"][ci], refb, rs, max_indel, *cols, host))
+        got.append(pc.format_alt_info(int(m["major"][ci]), m["matrix"][ci], m["stats"][ci], refb, rs, max_indel, *cols, host,
+                                      ins_last=int(m["ins_last"][ci]), fetch_end=1400 + pc.FETCH_EXPAND + 1))
     assert got == want["alt_info"]
 
 
@@ -283,7 +286,8 @@ def test_alt_info_many_insertion_alleles_follow_khash_bucket_order():
     al = m["alleles"][ci]
     assert len({a[0] & 0x3FFFFFFF for a in al}) >= 5 and len(seen) == 40
     cols = [np.array([a[j] for a in al], dtype=np.uint32) for j in range(4)]
-    text = pc.format_alt_info(3, m["matrix"][ci], m["stats"][ci], ref.encode(), 0, 50, *cols, pc.BamRecords.from_dict(rec))
+    text = pc.format_alt_info(3, m["matrix"][ci], m["stats"][ci], ref.encode(), 0, 50, *cols, pc.BamRecords.from_dict(rec),
+                              ins_last=int(m["ins_last"][ci]))
     assert text == want["alt_info"][m["cand_cols"].tolist().index(ci)]
     assert text.count(" IT") + text.startswith("4-60-T-IT") == 40
     first_seen = []
@@ -370,9 +374,10 @@ def load_counts_golden(tag):
 
 
 @pytest.mark.parametrize("tag", ["a", "b"])
-def test_oracle_against_committed_vectors(tag):
-    """tests/golden/pileup_counts.npz (tests/golden/make_pileup_counts_golden.py) freezes the hand-verified oracle: records in,
-    every output array and the all_alt_info strings out."""
+def test_oracle_against_reference_confirmed_vectors(tag):
+    """tests/golden/pileup_counts.npz (tests/golden/make_pileup_counts_golden.py): records in, every output array and the
+    all_alt_info strings out, minted from the reference's own calculate_clair3_pileup (stats and cand_ok, which the reference does
+    not have, from the oracle after it was checked equal on everything else)."""
     rec, ref, rs, start, end, kw, want = load_counts_golden(tag)
     got = po.clair3_pileup(rec, start, end, ref, rs, alt_info=True, **kw)
     for k in ("matrix", "major", "stats", "cand_cols", "cand_ok") + (("pos_ref_count", "pos_total_count") if kw["gvcf"] else ()):

@@ -1,4 +1,4 @@
-"""The feature counter against the COMMITTED fixtures of tests/golden/pileup_counts.npz, through the C-ABI (counts, candidates, gVCF
+"""The feature counter against the COMMITTED, reference-minted fixtures of tests/golden/pileup_counts.npz, through the C-ABI (counts, candidates, gVCF
 arrays, all_alt_info).  Kept in its own module, collected last, after the counter's operation-by-operation tests in
 tests/test_gpu_pileup_counts.py."""
 import os
@@ -21,7 +21,8 @@ def counter():
 
 
 @pytest.mark.parametrize("tag", ["a", "b"])
-def test_committed_golden_vectors(counter, tag):
+def test_reference_confirmed_golden_vectors(counter, tag):
+    """The counter against tests/golden/pileup_counts.npz, minted from the reference's own calculate_clair3_pileup."""
     from test_pileup_oracle import load_counts_golden
     rec, ref, rs, start, end, kw, want = load_counts_golden(tag)
     got = counter.count(rec, start, end, ref, rs, alt_info=True, **kw).fetch()
