@@ -1009,6 +1009,65 @@ extern "C" int c3b_decode_stage1(c3b_model *m, const float *y, const uint8_t *re
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ decode, stage 2
+extern "C" int c3b_decode_stage2(c3b_model *m, const float *y, const uint8_t *ref_gt21, int64_t batch, const int32_t *sites,
+                                 const int32_t *n_sites, int64_t max_sites, int k, int on_device, uint8_t *cat, uint16_t *idx,
+                                 float *prob, uint16_t *tie_mask, int32_t *count, uint8_t *complete, void *cuda_stream) {
+    if (!m) { c3b_set_error("c3b_decode_stage2: null model"); return 1; }
+    if (batch < 0 || max_sites < 0) { c3b_set_error("c3b_decode_stage2: negative batch or max_sites"); return 1; }
+    if (k < 1 || k > 1024) { c3b_set_error("c3b_decode_stage2: k must be in [1, 1024]"); return 1; }
+    if (!sites && max_sites > batch) { c3b_set_error("c3b_decode_stage2: without a site list max_sites cannot exceed batch"); return 1; }
+    if (max_sites == 0) return 0;
+    if ((batch > 0 && (!y || !ref_gt21)) || !cat || !idx || !prob || !tie_mask || !count || !complete) {
+        c3b_set_error("c3b_decode_stage2: null buffer");
+        return 1;
+    }
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    C3B_CUDA(cudaSetDevice(m->device));
+    if (on_device) {
+        m->launches++;
+        return c3b_launch_decode_stage2(y, ref_gt21, batch, m->out_dim, sites, n_sites, max_sites, k, cat, idx, prob, tie_mask,
+                                        count, complete, s);
+    }
+    const int64_t n = n_sites ? (int64_t)*n_sites : max_sites;
+    if (n < 0 || n > max_sites) { c3b_set_error("c3b_decode_stage2: n_sites must be in [0, max_sites]"); return 1; }
+    if (sites)
+        for (int64_t i = 0; i < n; ++i)
+            if (sites[i] < 0 || sites[i] >= batch) { c3b_set_error("c3b_decode_stage2: site index out of range [0, batch)"); return 1; }
+    // host buffers: stage through the stream's workspace, one packed region [prob | y | sites | count | n | idx | mask | gt | cat | complete]
+    Workspace *w = get_workspace(m, s);
+    if (!w) return 1;
+    const size_t B = (size_t)batch, S = (size_t)max_sites, SK = S * (size_t)k;
+    auto up16 = [](size_t v) { return (v + 15) / 16 * 16; };
+    size_t o_prob = 0, o_y = o_prob + up16(SK * 4), o_sites = o_y + up16(B * m->out_dim * 4), o_cnt = o_sites + up16(S * 4),
+           o_n = o_cnt + up16(S * 4), o_idx = o_n + 16, o_mask = o_idx + up16(SK * 2), o_gt = o_mask + up16(SK * 2),
+           o_cat = o_gt + up16(B), o_done = o_cat + up16(SK), total = o_done + up16(S);
+    if (w->dev_aux_bytes < total) C3B_CUDA(cudaStreamSynchronize(s));
+    if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, total)) return 1;
+    char *d = (char *)w->dev_aux;
+    const int32_t n32 = (int32_t)n;
+    if (B) {
+        C3B_CUDA(cudaMemcpyAsync(d + o_y, y, B * m->out_dim * 4, cudaMemcpyHostToDevice, s));
+        C3B_CUDA(cudaMemcpyAsync(d + o_gt, ref_gt21, B, cudaMemcpyHostToDevice, s));
+    }
+    if (sites && n) C3B_CUDA(cudaMemcpyAsync(d + o_sites, sites, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    C3B_CUDA(cudaMemcpyAsync(d + o_n, &n32, 4, cudaMemcpyHostToDevice, s));
+    m->launches++;
+    if (c3b_launch_decode_stage2((const float *)(d + o_y), (const uint8_t *)(d + o_gt), batch, m->out_dim,
+                                 sites ? (const int32_t *)(d + o_sites) : nullptr, (const int32_t *)(d + o_n), max_sites, k,
+                                 (uint8_t *)(d + o_cat), (uint16_t *)(d + o_idx), (float *)(d + o_prob), (uint16_t *)(d + o_mask),
+                                 (int32_t *)(d + o_cnt), (uint8_t *)(d + o_done), s))
+        return 1;
+    C3B_CUDA(cudaMemcpyAsync(cat, d + o_cat, SK, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaMemcpyAsync(idx, d + o_idx, SK * 2, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaMemcpyAsync(prob, d + o_prob, SK * 4, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaMemcpyAsync(tie_mask, d + o_mask, SK * 2, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaMemcpyAsync(count, d + o_cnt, S * 4, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaMemcpyAsync(complete, d + o_done, S, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaStreamSynchronize(s));
+    return 0;
+}
+
 // ------------------------------------------------------------------------------------------------ taps (debug)
 extern "C" int c3b_get_tap(c3b_model *m, const char *name, float *host_out, int64_t *count_inout) {
     if (!m || !name || !count_inout) { c3b_set_error("c3b_get_tap: null argument"); return 1; }

@@ -246,6 +246,10 @@ int c3b_launch_heads(const float *z4, int nsplit, int64_t split_stride, const He
 // ---- decode.cu ----
 int c3b_launch_decode_stage1(const float *y, const uint8_t *ref_gt21, int64_t batch, int out_dim, uint8_t *is_ref, float *ref_prob,
                              int32_t *argmax, float *maxprob, double *qual, int32_t *nonref_idx, int32_t *n_nonref, cudaStream_t s);
+// sites == nullptr: site s is row s; n_sites == nullptr: max_sites sites (else min(*n_sites, max_sites), read on the device)
+int c3b_launch_decode_stage2(const float *y, const uint8_t *ref_gt21, int64_t batch, int out_dim, const int32_t *sites,
+                             const int32_t *n_sites, int64_t max_sites, int k, uint8_t *cat, uint16_t *idx, float *prob,
+                             uint16_t *tie_mask, int32_t *count, uint8_t *complete, cudaStream_t s);
 
 // ---- kernels_fp32.cu ----
 int c3b_launch_lstm_f32(const float *x, const LstmF32 &fwd, const LstmF32 &bwd, float *out, int64_t batch, int in_dim,

@@ -24,6 +24,10 @@ This module replaces that launcher for the network stage:
 * ``--drop_ref_calls``: rows that the GPU-side first stage of the decoder (``c3b_decode_stage1``) marks as early-out
   homozygous-reference calls - which ``output_with`` drops unless ``--showRef`` (``clair3/CallVariants.py:1182-1186``) - are not
   written at all, so the per-site Python decoder only sees the sites that can become variants.
+* ``--decode_rows``: each rank also decodes its shard in-process (``clair3_b200.decode.batch_output``: stage 1 and the
+  outcome ranking of stage 2 on the GPU, the alt-info checks and row formatting on the host) and writes
+  ``<out_prefix>_<rank>.vcf_rows`` - the VCF body (no header lines) that the replay command above writes for the shard with
+  its default options.
 
 The tensors keep the reference's wire dtypes (int8 ``.npy``, the GPU-mode narrowing of ``CreateTensorPileupFromCffi.py:447``).
 Host-side logic (file split, batching, shard writing) has no CUDA dependency and is covered by the gloo CPU tests with a stub
@@ -128,11 +132,16 @@ class ShardWriter:
         return self.n
 
 
-def run_rank(model, files, out_prefix, kind, drop_ref_calls=False, streams=8, decode=None):
+def run_rank(model, files, out_prefix, kind, drop_ref_calls=False, streams=8, decode=None, decode_rows=None):
     """Network stage of one rank: files -> shard.  ``model`` follows the module protocol (``predict_stream`` and, for
-    ``drop_ref_calls``, ``decode_stage1``); returns (sites read, rows written)."""
+    ``drop_ref_calls``, ``decode_stage1``); returns (sites read, rows written).  ``decode_rows``: an OutputConfig; the shard's
+    rows are also decoded (``decode_stage1`` / ``decode_stage2`` of ``model``) into ``<out_prefix>.vcf_rows``."""
     batch_sites = BATCH_SITES[kind]
     metas = []
+    vcf = None
+    if decode_rows is not None:
+        from . import decode as host_decode
+        vcf = open(out_prefix + ".vcf_rows", "w")
 
     def tensors():
         for x, positions, alt_infos in iter_batches(files, batch_sites):
@@ -155,6 +164,10 @@ def run_rank(model, files, out_prefix, kind, drop_ref_calls=False, streams=8, de
             positions = [positions[i] for i in keep]
             alt_infos = [alt_infos[i] for i in keep]
         writer.append(y, positions, alt_infos)
+        if vcf is not None and len(y):
+            vcf.write(host_decode.batch_output(model, positions, alt_infos, y, decode_rows))
+    if vcf is not None:
+        vcf.close()
     return read, writer.close()
 
 
@@ -190,6 +203,8 @@ def main(argv=None):
     ap.add_argument("--enable_dwell_time", action="store_true")
     ap.add_argument("--platform", default="ont")
     ap.add_argument("--drop_ref_calls", action="store_true")
+    ap.add_argument("--decode_rows", action="store_true",
+                    help="also decode every shard in-process into <out_prefix>_<rank>.vcf_rows (VCF body, no header)")
     ap.add_argument("--streams", type=int, default=8)
     ap.add_argument("--clair3_entry", default=None, help="path to the reference's clair3.py: run its decoder on every shard")
     ap.add_argument("--call_dir", default=None)
@@ -229,7 +244,12 @@ def main(argv=None):
 
     files = split_file_list(read_file_list(args.file_list), world)[rank]
     shard = "%s_%d" % (args.out_prefix, rank)
-    read, written = run_rank(m, files, shard, kind, drop_ref_calls=args.drop_ref_calls, streams=args.streams)
+    rows_config = None
+    if args.decode_rows:
+        from .decode import replay_config
+        rows_config = replay_config(args.pileup, args.add_indel_length)
+    read, written = run_rank(m, files, shard, kind, drop_ref_calls=args.drop_ref_calls, streams=args.streams,
+                             decode_rows=rows_config)
     cmd = decode_command(args, rank, shard)
     with open(shard + ".decode_cmd", "w") as f:
         f.write(" ".join(cmd) + "\n")

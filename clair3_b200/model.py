@@ -248,6 +248,63 @@ class _C3BModule:
                                       c("void *", stream)))
         return out
 
+    def decode_stage2(self, y, ref_gt21, sites=None, n_sites=None, k=16):
+        """``c3b_decode_stage2``: each listed site's genotype outcomes in the order the reference's ``output_from`` tries them
+        (``clair3/CallVariants.py:676-1012``), first ``k`` (1..1024) entries, ending at homo_Ref.  ``y`` / ``ref_gt21`` as for
+        ``decode_stage1``; ``sites`` int32 [S] row indices (default: every row) and ``n_sites`` int32 [1] how many of them are
+        listed (default S) - stage 1's ``nonref_idx`` / ``n_nonref`` chain in with no host synchronisation.  All on y's device
+        (cuda: asynchronous on the current stream; cpu: complete on return).  Returns a dict of tensors: cat uint8 [S,k]
+        (0 homo_Ref .. 9 hetero_InsDel, 255 unused), idx int16 [S,k] (index in the category's list), prob float32 [S,k],
+        tie_mask int16 [S,k] (bit c: the is_* flag of category c if this attempt succeeds), count int32 [S], complete uint8 [S]."""
+        if self._handle is None:
+            raise C3BError("model has no device yet")
+        if isinstance(y, np.ndarray):
+            y = torch.from_numpy(y)
+        if isinstance(ref_gt21, np.ndarray):
+            ref_gt21 = torch.from_numpy(ref_gt21)
+        if isinstance(sites, np.ndarray):
+            sites = torch.from_numpy(sites)
+        if isinstance(n_sites, np.ndarray):
+            n_sites = torch.from_numpy(n_sites)
+        if y.ndim != 2 or y.shape[1] != self.out_dim or y.dtype != torch.float32:
+            raise C3BError("decode_stage2: y must be float32 [B, %d]" % self.out_dim)
+        ref_gt21 = ref_gt21.to(torch.uint8)
+        if ref_gt21.shape != (y.shape[0],) or ref_gt21.device != y.device:
+            raise C3BError("decode_stage2: ref_gt21 must be [B] on y's device")
+        if ref_gt21.numel() and int(ref_gt21.max()) > 20:
+            raise C3BError("decode_stage2: ref_gt21 holds gt21 indices (0..20)")
+        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= int(k) <= 1024:
+            raise C3BError("decode_stage2: k must be an integer in [1, 1024], got %r" % (k,))
+        k = int(k)
+        if sites is not None:
+            if sites.ndim != 1 or sites.device != y.device or sites.dtype not in (torch.int32, torch.int64):
+                raise C3BError("decode_stage2: sites must be a 1-D int32 tensor on y's device")
+            sites = sites.to(torch.int32).contiguous()
+        if n_sites is not None:
+            if n_sites.numel() != 1 or n_sites.device != y.device or n_sites.dtype != torch.int32:
+                raise C3BError("decode_stage2: n_sites must be one int32 on y's device")
+            n_sites = n_sites.reshape(1).contiguous()
+        y = y.contiguous()
+        ref_gt21 = ref_gt21.contiguous()
+        B, dev = y.shape[0], y.device
+        S = B if sites is None else sites.shape[0]
+        out = {"cat": torch.empty((S, k), dtype=torch.uint8, device=dev), "idx": torch.empty((S, k), dtype=torch.int16, device=dev),
+               "prob": torch.empty((S, k), dtype=torch.float32, device=dev),
+               "tie_mask": torch.empty((S, k), dtype=torch.int16, device=dev),
+               "count": torch.zeros(S, dtype=torch.int32, device=dev), "complete": torch.zeros(S, dtype=torch.uint8, device=dev)}
+        if S == 0:
+            return out
+        stream = torch.cuda.current_stream(self._device).cuda_stream
+        c = ffi.cast
+        ptr = lambda t, ty: c(ty, t.data_ptr()) if t is not None else ffi.NULL          # noqa: E731
+        check(lib().c3b_decode_stage2(self._handle, c("float *", y.data_ptr()), c("uint8_t *", ref_gt21.data_ptr()), B,
+                                      ptr(sites, "int32_t *"), ptr(n_sites, "int32_t *"), S, k, int(dev.type == "cuda"),
+                                      c("uint8_t *", out["cat"].data_ptr()), c("uint16_t *", out["idx"].data_ptr()),
+                                      c("float *", out["prob"].data_ptr()), c("uint16_t *", out["tie_mask"].data_ptr()),
+                                      c("int32_t *", out["count"].data_ptr()), c("uint8_t *", out["complete"].data_ptr()),
+                                      c("void *", stream)))
+        return out
+
     def predict_stream(self, batches, streams=8):
         """Pipelined ``_torch_predict`` (``clair3/CallVariantsFromCffi.py:48-52,300-331``): consume an iterable of host batches
         (numpy arrays or CPU tensors, ragged sizes allowed) and yield one float32 numpy ``Y`` per batch, in order, while up to

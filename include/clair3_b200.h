@@ -117,6 +117,27 @@ int c3b_decode_stage1(c3b_model *m, const float *y, const uint8_t *ref_gt21, int
                       uint8_t *is_ref, float *ref_prob, int32_t *argmax, float *maxprob, double *qual,
                       int32_t *nonref_idx, int32_t *n_nonref, void *cuda_stream);
 
+/* Second stage of the decoder: ranks every listed site's genotype outcomes in the order the reference's output_from tries them
+ * (CallVariants.py:676-1012 over the lists of possible_outcome_probabilites_from, :406-659), so that the host only checks
+ * the ranked outcomes against alt_info:
+ *   y, ref_gt21  as for c3b_decode_stage1, [batch] rows
+ *   sites     [max_sites] row indices to rank (e.g. stage 1's nonref_idx), or NULL for rows 0 .. max_sites-1
+ *   n_sites   number of listed sites (e.g. stage 1's n_nonref, read on the device when on_device), or NULL for max_sites
+ *   k         entries per site, 1 .. 1024 (804 ranks every outcome of the 90-output model, 24 of the 24-output one)
+ *   cat, idx, prob, tie_mask  [max_sites][k]: the site's first k attempts, probability descending, then category, then index
+ *             ascending, ending at homo_Ref.  cat: 0 homo_Ref, 1 homo_SNP, 2 hetero_SNP, 3 homo_Ins, 4 hetero_ACGT_Ins,
+ *             5 hetero_InsIns, 6 homo_Del, 7 hetero_ACGT_Del, 8 hetero_DelDel, 9 hetero_InsDel (output_from's elif order);
+ *             idx: position in that category's list; prob: the float32 product (bit-exact, multiplies only); tie_mask bit c:
+ *             category c holds an entry of the same probability at this position or later (the is_* flags output_from
+ *             returns if this attempt succeeds).  Unused entries: cat 255, idx 0, prob 0, tie_mask 0.
+ *   count     [max_sites] entries written    complete [max_sites] 1 = homo_Ref is among them (0 for unlisted sites and for
+ *             listed indices outside [0, batch), which a host-pointer call rejects instead)
+ * on_device: every pointer is a device pointer and the call is asynchronous on cuda_stream; else host pointers, returns when
+ * the outputs are complete. */
+int c3b_decode_stage2(c3b_model *m, const float *y, const uint8_t *ref_gt21, int64_t batch, const int32_t *sites,
+                      const int32_t *n_sites, int64_t max_sites, int k, int on_device, uint8_t *cat, uint16_t *idx,
+                      float *prob, uint16_t *tie_mask, int32_t *count, uint8_t *complete, void *cuda_stream);
+
 /* Packed device weight images (what one rank broadcasts to the others at start-up; SURVEY.md 8e).
  * which: 0 = fp16 tensor-core operand images + fp32 head weights, 1 = fp32 debug-path weights. */
 int c3b_weight_blob(c3b_model *m, int which, void **device_ptr, size_t *bytes);
