@@ -45,13 +45,14 @@ constexpr int NPOS = 33;            // no_of_positions
 constexpr int MAXSEL = 1536;        // reads overlapping one candidate window that K11 can hold
 constexpr int CAND_THREADS = 256;
 constexpr int MAX_PS = 64;          // distinct phase sets one read may touch (K7)
+constexpr int MAX_OVERWRITTEN = 64; // insertions on one candidate that a later insertion of the same read and anchor overwrote (K11)
 constexpr int JUMP_BITS = 63;       // rand() offsets below 2^63
 constexpr int AL_CAP = 1 << 22;     // exported allele records per call
 
 struct PosInfo {                    // Pos_info (src/clair3_full_alignment_dwell.h:138-146); alt 0 = not covered by M / D
     int8_t alt;                     // nt16 code, -1 deleted
     int8_t bq;
-    int16_t pad;
+    int16_t n_ins;                  // insertion operations anchored on this base (2I1I, 1I1P1I: 2); ins_q / ins_len hold the last
     int32_t del_len;
     int32_t ins_q;
     int32_t ins_len;
@@ -496,6 +497,7 @@ __global__ void fa_pos_info_kernel(FaReads R, Kept K, int64_t n_kept, const int6
             if (a >= 0) {
                 pi[a].ins_q = (int32_t)query_pos;
                 pi[a].ins_len = (int32_t)length;
+                if (pi[a].n_ins < SHRT_MAX) ++pi[a].n_ins;
                 if (sg) {
                     int32_t s = 0;
                     for (int64_t t = 0; t < length; ++t)
@@ -571,9 +573,11 @@ __device__ __forceinline__ bool same_ins(const FaReads &R, const Kept &K, int64_
 }
 
 
-__device__ __forceinline__ int8_t norm_af(int64_t count, int depth) {          // normalize_af(count / (float)depth), float32
+// normalize_af(count / (float)depth) (.h:13, :926): the macro does not parenthesise its argument, so its `100 * x` is
+// `100 * count / (float)depth` - (float)(100 count) / depth in float32, not 100 * (count / depth) (53 / 100: 53, not 52)
+__device__ __forceinline__ int8_t norm_af(int64_t count, int depth) {
     const float x = __fdiv_rn((float)count, (float)depth);
-    return (int8_t)(int)(x < 1.0f ? __fmul_rn(100.0f, x) : 100.0f);
+    return (int8_t)(int)(x < 1.0f ? __fdiv_rn((float)(100 * count), (float)depth) : 100.0f);
 }
 
 __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) {
@@ -587,8 +591,13 @@ __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) 
     __shared__ int32_t rows[256];         // kept-read index of every matrix row, -1 padding
     __shared__ int8_t row_af[256];
     __shared__ int8_t spill[256 * NPOS];  // channel 6 of every row
+    // the insertions that Pos_info lost to a later one on the same read and anchor (2I1I, 1I1P1I): the reference's counter still
+    // saw them (:746-752), before the kept one.  Sorted by read (stable: each read's run is in CIGAR order).
+    __shared__ int32_t ow_i[MAX_OVERWRITTEN];       // index in sel
+    __shared__ int32_t ow_len[MAX_OVERWRITTEN], ow_q[MAX_OVERWRITTEN];
+    __shared__ int16_t ow_cnt[MAX_OVERWRITTEN];     // first occurrence of its string: reads showing it, else 0
     __shared__ int32_t wsum[CAND_THREADS / 32];
-    __shared__ int s_depth, s_acgt[4];
+    __shared__ int s_depth, s_acgt[4], s_now;
     __shared__ uint32_t st[32];
     const int64_t ci = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -600,7 +609,7 @@ __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) 
         if (tid == 0) atomicOr(A.status, 1);
         return;
     }
-    if (tid == 0) { s_depth = 0; s_acgt[0] = s_acgt[1] = s_acgt[2] = s_acgt[3] = 0; }
+    if (tid == 0) { s_depth = 0; s_acgt[0] = s_acgt[1] = s_acgt[2] = s_acgt[3] = 0; s_now = 0; }
     // ordered compaction of the window's reads (the reference's loop at :805-814)
     int base = 0;
     for (int64_t j0 = a; j0 < b; j0 += CAND_THREADS) {
@@ -636,9 +645,67 @@ __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) 
         ev_del[i] = e.del_len;
         ev_ins[i] = e.ins_len;
         ev_q[i] = e.ins_q;
+        if (e.n_ins > 1) {                // walk the read's CIGAR again for the insertions anchored on c before the kept one
+            const int64_t r = A.K.orig[k];
+            const int n_ow = e.n_ins - 1;
+            const int slot = atomicAdd(&s_now, n_ow);
+            if (slot + n_ow > MAX_OVERWRITTEN) {
+                atomicOr(A.status, 8);
+                continue;
+            }
+            int64_t ref_pos = A.K.start[k], query_pos = 0;
+            int w = 0;
+            for (int64_t x = A.R.cigar_off[r]; x < A.R.cigar_off[r + 1] && w < n_ow; ++x) {
+                const uint32_t op = A.R.cigar[x] & 15u;
+                const int64_t length = A.R.cigar[x] >> 4;
+                if (op == 0 || op == 7 || op == 8) { ref_pos += length; query_pos += length; }
+                else if (op == 2 || op == 3) ref_pos += length;
+                else if (op == 4) query_pos += length;
+                else if (op == 1) {
+                    if (ref_pos - 1 == c) {
+                        ow_i[slot + w] = i;
+                        ow_len[slot + w] = (int32_t)length;
+                        ow_q[slot + w++] = (int32_t)query_pos;
+                    }
+                    query_pos += length;
+                }
+            }
+        }
     }
     __syncthreads();
-    // distinct alleles and their counts; first occurrence in kept order = the order in which the reference's counters saw them
+    const int n_ow = s_now <= MAX_OVERWRITTEN ? s_now : 0;   // beyond the capacity: an error from c3b_fa_sizes, nothing exported
+    if (tid == 0) {
+        for (int x = 1; x < n_ow; ++x) {  // stable insertion sort by read: put order
+            const int32_t vi = ow_i[x], vl = ow_len[x], vq = ow_q[x];
+            int y = x;
+            for (; y > 0 && ow_i[y - 1] > vi; --y) {
+                ow_i[y] = ow_i[y - 1];
+                ow_len[y] = ow_len[y - 1];
+                ow_q[y] = ow_q[y - 1];
+            }
+            ow_i[y] = vi;
+            ow_len[y] = vl;
+            ow_q[y] = vq;
+        }
+    }
+    __syncthreads();
+    // the insertion puts in order: for each read (kept order) its overwritten insertions, then its kept one (key i << 16 | 0xFFFF);
+    // overwritten insertion x of read i has key i << 16 | x
+    auto count_ins = [&](int64_t key, int64_t kr, int q, int len) -> int {   // reads showing the string, 0 unless key is its first
+        int cnt = 0;
+        for (int t = 0; t < n_all; ++t)
+            if (ev_ins[t] == len && same_ins(A.R, A.K, sel[t], ev_q[t], kr, q, len)) {
+                if ((((int64_t)t << 16) | 0xFFFF) < key) return 0;
+                ++cnt;
+            }
+        for (int x = 0; x < n_ow; ++x)
+            if (ow_len[x] == len && same_ins(A.R, A.K, sel[ow_i[x]], ow_q[x], kr, q, len)) {
+                if ((((int64_t)ow_i[x] << 16) | x) < key) return 0;
+                ++cnt;
+            }
+        return cnt;
+    };
+    // distinct alleles and their counts; first occurrence in put order = the order in which the reference's counters saw them
     for (int i = tid; i < n_all; i += CAND_THREADS) {
         int dc = 0, ic = 0;
         if (ev_del[i] > 0) {
@@ -648,20 +715,16 @@ __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) 
                     ++dc;
                 }
         }
-        if (ev_ins[i] > 0) {
-            for (int t = 0; t < n_all; ++t)
-                if (ev_ins[t] == ev_ins[i] && same_ins(A.R, A.K, sel[t], ev_q[t], sel[i], ev_q[i], ev_ins[i])) {
-                    if (t < i) { ic = 0; break; }
-                    ++ic;
-                }
-        }
+        if (ev_ins[i] > 0) ic = count_ins(((int64_t)i << 16) | 0xFFFF, sel[i], ev_q[i], ev_ins[i]);
         ev_dcnt[i] = (int16_t)dc;
         ev_icnt[i] = (int16_t)ic;
     }
+    for (int x = tid; x < n_ow; x += CAND_THREADS) ow_cnt[x] = (int16_t)count_ins(((int64_t)ow_i[x] << 16) | x, sel[ow_i[x]], ow_q[x], ow_len[x]);
     __syncthreads();
     if (tid == 0) {
         int nal = 0;
         for (int i = 0; i < n_all; ++i) nal += (ev_dcnt[i] > 0) + (ev_icnt[i] > 0);
+        for (int x = 0; x < n_ow; ++x) nal += ow_cnt[x] > 0;
         const unsigned long long o = nal ? atomicAdd(A.al_used, (unsigned long long)nal) : 0ull;
         if (o + (unsigned long long)nal > (unsigned long long)AL_CAP) {
             atomicOr(A.status, 2);
@@ -672,29 +735,39 @@ __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) 
             A.al_n[ci] = nal;
             // bit 30 of the last allele of a kind: a later read showed an allele of that kind again - that put grows a full
             // khash before it finds the key, which changes the table's bucket order (khash.h:310-318)
-            int last_d = -1, last_i = -1;
-            for (int i = 0; i < n_all; ++i) {
+            // insertion puts are numbered in put order (p); deletions by read
+            int last_d = -1, last_p = -1, n_put = 0;
+            for (int i = 0, x = 0; i < n_all; ++i) {
                 if (ev_dcnt[i] > 0) last_d = i;
-                if (ev_icnt[i] > 0) last_i = i;
+                for (; x < n_ow && ow_i[x] == i; ++x, ++n_put)
+                    if (ow_cnt[x] > 0) last_p = n_put;
+                if (ev_ins[i] > 0) {
+                    if (ev_icnt[i] > 0) last_p = n_put;
+                    ++n_put;
+                }
             }
-            bool tail_d = false, tail_i = false;
-            for (int i = 0; i < n_all; ++i) {
-                tail_d |= i > last_d && ev_del[i] > 0;
-                tail_i |= i > last_i && ev_ins[i] > 0;
-            }
+            bool tail_d = false;
+            for (int i = 0; i < n_all; ++i) tail_d |= i > last_d && ev_del[i] > 0;
+            const bool tail_i = last_p < n_put - 1;
             int w = (int)o;
-            for (int i = 0; i < n_all; ++i) {
+            auto put_ins = [&](int p, int i, int len, int q, int cnt) {
+                A.al_meta[w] = 0x80000000u | (uint32_t)len | (p == last_p && tail_i ? 0x40000000u : 0u);
+                A.al_read[w] = (uint32_t)A.K.orig[sel[i]];
+                A.al_qpos[w] = (uint32_t)q;
+                A.al_cnt[w++] = (uint32_t)cnt;
+            };
+            for (int i = 0, x = 0, p = 0; i < n_all; ++i) {
                 if (ev_dcnt[i] > 0) {
                     A.al_meta[w] = (uint32_t)ev_del[i] | (i == last_d && tail_d ? 0x40000000u : 0u);
                     A.al_read[w] = (uint32_t)A.K.orig[sel[i]];
                     A.al_qpos[w] = 0;
                     A.al_cnt[w++] = (uint32_t)ev_dcnt[i];
                 }
-                if (ev_icnt[i] > 0) {
-                    A.al_meta[w] = 0x80000000u | (uint32_t)ev_ins[i] | (i == last_i && tail_i ? 0x40000000u : 0u);
-                    A.al_read[w] = (uint32_t)A.K.orig[sel[i]];
-                    A.al_qpos[w] = (uint32_t)ev_q[i];
-                    A.al_cnt[w++] = (uint32_t)ev_icnt[i];
+                for (; x < n_ow && ow_i[x] == i; ++x, ++p)
+                    if (ow_cnt[x] > 0) put_ins(p, i, ow_len[x], ow_q[x], ow_cnt[x]);
+                if (ev_ins[i] > 0) {
+                    if (ev_icnt[i] > 0) put_ins(p, i, ev_ins[i], ev_q[i], ev_icnt[i]);
+                    ++p;
                 }
             }
         }
@@ -770,11 +843,17 @@ __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) 
             const PosInfo e = A.pool[A.K.pi[k] + off];
             const char altc = NT16[e.alt > 0 ? e.alt : 0];
             if (e.alt <= 0) {
-            } else if (e.ins_len > 0) {
-                for (int i = 0; i < n_all; ++i)
+            } else if (e.ins_len > 0) {         // the counter's value for the kept string, overwritten insertions included
+                bool found = false;
+                for (int i = 0; i < n_all && !found; ++i)
                     if (ev_icnt[i] > 0 && ev_ins[i] == e.ins_len && same_ins(A.R, A.K, sel[i], ev_q[i], k, e.ins_q, e.ins_len)) {
                         af = norm_af(ev_icnt[i], s_depth);
-                        break;
+                        found = true;
+                    }
+                for (int x = 0; x < n_ow && !found; ++x)
+                    if (ow_cnt[x] > 0 && ow_len[x] == e.ins_len && same_ins(A.R, A.K, sel[ow_i[x]], ow_q[x], k, e.ins_q, e.ins_len)) {
+                        af = norm_af(ow_cnt[x], s_depth);
+                        found = true;
                     }
             } else if (e.del_len > 0) {
                 for (int i = 0; i < n_all; ++i)
@@ -1162,6 +1241,11 @@ int c3b_fa_sizes(c3b_fa *w, int64_t *n_cand, int64_t *n_kept, int64_t *rand_draw
     if (status & 1) { c3b_set_error("c3b_fa_build: more than %d reads overlap one candidate window", MAXSEL); return 1; }
     if (status & 2) { c3b_set_error("c3b_fa_build: more than %d distinct indel alleles to export; build fewer candidates per call", AL_CAP); return 1; }
     if (status & 4) { c3b_set_error("c3b_fa_build: a read touches variants of more than %d phase sets", MAX_PS); return 1; }
+    if (status & 8) {
+        c3b_set_error("c3b_fa_build: more than %d insertions on one candidate are overwritten by a later insertion on the same anchor",
+                      MAX_OVERWRITTEN);
+        return 1;
+    }
     if (n_cand) *n_cand = w->n_cand;
     if (n_kept) *n_kept = w->n_kept;
     if (rand_draws) *rand_draws = w->host_counters[4];

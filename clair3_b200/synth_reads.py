@@ -58,14 +58,17 @@ _JUNCTIONS_WILD = [
     [("I", 2), ("P", 1), ("I", 1)], [("P", 2), ("I", 3)], [("D", 2), ("I", 2)], [("I", 1), ("D", 1)], [("N", 5), ("D", 2)],
     [("D", 4), ("N", 3)], [("P", 1)], [("I", 1), ("I", 2)],
 ]
+# the same without reference skips: a skip over a full-alignment candidate window is input the reference leaves undefined
+_JUNCTIONS_WILD_NO_SKIP = [j for j in _JUNCTIONS_WILD if all(o != "N" for o, _ in j)]
 
 
 def random_alignment(region_len, depth, read_len=2000, seed=0, indel_rate=0.04, sub_rate=0.03, n_rate=0.002, wild=False,
-                     origin=1000, gaps=(), filtered_frac=0.08, clip_frac=0.3, short_ins=False):
+                     origin=1000, gaps=(), filtered_frac=0.08, clip_frac=0.3, short_ins=False, ref_skips=True):
     """Reads of mean length ``read_len`` tiling [origin - read_len, origin + region_len + read_len) at mean depth ``depth`` on a
     random reference.  ``wild``: junctions between match segments are drawn from a list of awkward operation runs (adjacent
-    deletions, pads, skips, insertion after deletion) - slower, for tests.  ``gaps``: (begin, end) intervals no read may start in
-    (coverage holes).  Returns (records, ref_seq, ref_start)."""
+    deletions, pads, skips, insertion after deletion) - slower, for tests; ``ref_skips=False`` leaves the skips (N) out of it.
+    ``gaps``: (begin, end) intervals no read may start in (coverage holes).  Returns (records, ref_seq, ref_start)."""
+    junctions = _JUNCTIONS_WILD if ref_skips else _JUNCTIONS_WILD_NO_SKIP
     rng = np.random.default_rng(seed)
     lo = max(0, origin - read_len)
     hi = origin + region_len + read_len
@@ -97,7 +100,7 @@ def random_alignment(region_len, depth, read_len=2000, seed=0, indel_rate=0.04, 
                 ops.append(rng.choice([0, 7, 8], p=[0.8, 0.1, 0.1]))
                 lens.append(int(seg[i]))
                 if i + 1 < k:
-                    for o, l in _JUNCTIONS_WILD[rng.integers(0, len(_JUNCTIONS_WILD))]:
+                    for o, l in junctions[rng.integers(0, len(junctions))]:
                         ops.append(OP[o])
                         lens.append(l)
             ops = np.array(ops, np.int64)
@@ -160,14 +163,15 @@ def aligned_bases(rec):
 
 
 def random_fa_case(seed, region_len=3000, depth=30, read_len=1500, n_cand=40, n_var=12, dup_frac=0.05, dwell=False, n_base_rate=0.003,
-                   long_ins=True, clip_frac=0.3, mv_missing_frac=0.1):
+                   long_ins=True, clip_frac=0.3, mv_missing_frac=0.1, wild=False):
     """A full-alignment test case on a contig that starts at position 0: records with base qualities, read names (``dup_frac`` of
     them repeating an earlier name) and, with ``dwell``, ``mv`` move tables; strictly ascending candidates (>= 16) and sorted
     phased heterozygous SNPs ``(position, ref_base, alt_base, genotype, phase_set)``.  Query bases are A/C/G/T with a few N; the
-    reference has soft-masked (lower-case) stretches and a few N.  Returns (records, ref_seq, candidates, variants)."""
+    reference has soft-masked (lower-case) stretches and a few N.  ``wild``: ``random_alignment``'s awkward operation runs, without
+    reference skips.  Returns (records, ref_seq, candidates, variants)."""
     rng = np.random.default_rng(seed + 7919)
     rec, ref, rs = random_alignment(region_len, depth, read_len=read_len, seed=seed, n_rate=0.0, origin=read_len,
-                                    clip_frac=clip_frac, short_ins=not long_ins)
+                                    clip_frac=clip_frac, short_ins=not long_ins, wild=wild, ref_skips=False)
     assert rs == 0
     n = len(rec["pos"])
     lq = rec["l_qseq"].astype(np.int64)

@@ -22,6 +22,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 STUB = os.path.join(HERE, "hts_stub")
 OUT_DIR = os.path.join(HERE, "_ref")
 LIB = os.path.join(OUT_DIR, "libclair3_fa_ref.so")
+SKIP_SRC = os.path.join(HERE, "rand_skip.c")
+SKIP_LIB = os.path.join(HERE, "_build", "librand_skip.so")
 REF_SOURCES = ("clair3_full_alignment_dwell.c", "levenshtein.c", "medaka_khcounter.c", "medaka_common.c")
 CONTIG = "ctg"
 
@@ -49,6 +51,17 @@ def reference_src():
 
 def available():
     return os.path.exists(LIB)
+
+
+def build_rand_skip(out=SKIP_LIB):
+    """gcc -O2 -shared oracle/rand_skip.c -> oracle/_build/librand_skip.so (git-ignored).  Project source only, so it is built
+    whether or not a reference checkout is found; an ``oracle/_ref/`` kept from an earlier build never lacks it."""
+    if not os.path.exists(out) or os.path.getmtime(out) < os.path.getmtime(SKIP_SRC):
+        os.makedirs(os.path.dirname(out), exist_ok=True)
+        tmp = out + ".tmp%d" % os.getpid()
+        subprocess.run(["gcc", "-O2", "-shared", "-fPIC", "-o", tmp, SKIP_SRC], check=True)
+        os.replace(tmp, out)
+    return out
 
 
 def build(force=False):
@@ -83,10 +96,22 @@ class _FaData(ctypes.Structure):
 
 _lib = None
 _libc = None
+_skip = None
+
+
+def _load_rand_skip():
+    try:
+        path = build_rand_skip()
+    except (OSError, subprocess.CalledProcessError):          # a read-only tree: build it in a temporary directory
+        import tempfile
+        path = build_rand_skip(os.path.join(tempfile.mkdtemp(prefix="clair3_fa_ref_"), "librand_skip.so"))
+    S = ctypes.CDLL(path)
+    S.fa_ref_skip_rand.argtypes = [ctypes.c_uint64]
+    return S
 
 
 def _load():
-    global _lib, _libc
+    global _lib, _libc, _skip
     if _lib is None:
         path = build()
         if path is None:
@@ -101,15 +126,17 @@ def _load():
         L.fa_ref_set_contig.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.c_int64]
         L.fa_ref_set_records.argtypes = [ctypes.c_int64] + [ctypes.c_void_p] * 14
         L.fa_ref_rand_draws.restype = ctypes.c_longlong
+        _skip = _load_rand_skip()
         _lib = L
         _libc = ctypes.CDLL(None)
     return _lib
 
 
-def libc_rand(seed, n):
-    """The first ``n`` values of glibc ``rand()`` after ``srand(seed)`` (the generator the reference shuffles with)."""
+def libc_rand(seed, n, skip=0):
+    """``n`` values of glibc ``rand()`` after ``srand(seed)`` and ``skip`` draws (the generator the reference shuffles with)."""
     _load()
     _libc.srand(ctypes.c_uint(seed))
+    _skip.fa_ref_skip_rand(int(skip))
     return np.array([_libc.rand() for _ in range(n)], dtype=np.int64)
 
 
@@ -151,8 +178,7 @@ def full_alignment(rec, candidates, ref_seq, variants=(), need_haplotagging=Fals
                         int(gt), int(ps))
         vp[i] = ctypes.pointer(vs[i])
     _libc.srand(ctypes.c_uint(rand_seed))
-    for _ in range(int(rand_skip)):
-        _libc.rand()
+    _skip.fa_ref_skip_rand(int(rand_skip))  # a C loop: about 2^32 draws take tens of seconds
     L.fa_ref_reset_rand_draws()
     region = ("%s:1-%d" % (CONTIG, len(ref))).encode()
     d = L.calculate_clair3_full_alignment(region, b"in-memory.bam", b"in-memory.fa", vp, nv,

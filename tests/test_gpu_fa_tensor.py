@@ -9,6 +9,7 @@ from clair3_b200 import synth_reads as sr
 from clair3_b200._ffi import C3BError
 from clair3_b200.fa_tensor import FullAlignmentBuilder, create_tensor_full_alignment
 from fa_golden import builder_kwargs, load_fa_golden
+import fa_ref_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -44,22 +45,7 @@ def test_golden_fixture(builder):
     _check(builder, rec, ref, cand, var, params, m, alt, draws)
 
 
-CASES = [  # seed, generator arguments, parameters
-    (1, dict(depth=30), dict(need_haplotagging=True, matrix_depth=89, enable_dwell_time=False)),
-    (2, dict(depth=30), dict(need_haplotagging=False, matrix_depth=89, enable_dwell_time=False)),
-    (3, dict(depth=40, dwell=True), dict(need_haplotagging=True, matrix_depth=89, enable_dwell_time=True)),
-    (4, dict(depth=40, dwell=True), dict(need_haplotagging=False, matrix_depth=55, enable_dwell_time=True)),
-    (5, dict(depth=150), dict(need_haplotagging=True, matrix_depth=89, enable_dwell_time=False)),
-    (6, dict(depth=150, dwell=True), dict(need_haplotagging=True, matrix_depth=89, enable_dwell_time=True)),
-    (7, dict(depth=90, dup_frac=0.3), dict(need_haplotagging=True, matrix_depth=55, enable_dwell_time=False)),
-    (8, dict(depth=60, clip_frac=0.9), dict(need_haplotagging=True, matrix_depth=55, enable_dwell_time=False)),
-    (9, dict(depth=50, long_ins=True, n_var=40), dict(need_haplotagging=True, matrix_depth=89, enable_dwell_time=False)),
-    (10, dict(depth=50, long_ins=False, n_base_rate=0.02), dict(need_haplotagging=True, matrix_depth=89, enable_dwell_time=False)),
-    (11, dict(depth=200, read_len=3000, n_cand=80), dict(need_haplotagging=True, matrix_depth=89, enable_dwell_time=False)),
-    (12, dict(depth=20, n_var=0), dict(need_haplotagging=True, matrix_depth=89, enable_dwell_time=False, min_mq=20)),
-    (13, dict(depth=120, dwell=True, dup_frac=0.2), dict(need_haplotagging=True, matrix_depth=55, enable_dwell_time=True,
-                                                         max_indel_length=5)),
-]
+CASES = [c for c in fa_ref_cases.GEN if not c[1].get("wild")]   # seed, generator arguments, parameters: one list, shared
 
 
 @pytest.mark.parametrize("seed,gen,params", CASES, ids=[str(c[0]) for c in CASES])
