@@ -646,11 +646,13 @@ extern "C" int c3b_get_profile_ctas(c3b_model *m, const char *kernel, double *ct
 
 // ------------------------------------------------------------------------------------------------ forward passes
 // Where a pileup chunk's sites come from: a dense [n,33,C] tensor, or 33-row windows of a per-column count matrix
-// ([n_cols][C], libclair3's plp_data.matrix) starting at rows starts[b] (rows outside the matrix read as zero)
+// ([n_cols][C], libclair3's plp_data.matrix) starting at rows starts[b] (rows outside the matrix, or outside [bounds[b][0],
+// bounds[b][1]) when bounds are given, read as zero)
 struct PileupSrc {
     const void *x;          // dense: first site of the chunk; windows: the column matrix
     int dtype;
     const int64_t *starts;  // windows: device pointer to this chunk's first start row; nullptr = dense
+    const int64_t *bounds;  // windows: device pointer to this chunk's first [lo, hi) row pair; nullptr = [0, n_cols)
     int64_t n_cols;
 };
 
@@ -671,7 +673,7 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
         float *l2 = cv.take<float>((size_t)n * C3B_T * 320 * 4);
         float *z4 = cv.take<float>((size_t)bp * 128 * 4);
         if (src.starts) {
-            if (c3b_launch_gather_windows_f32(x, x_dtype, m->channels, src.starts, src.n_cols, xf, n, s)) return 1;
+            if (c3b_launch_gather_windows_f32(x, x_dtype, m->channels, src.starts, src.bounds, src.n_cols, xf, n, s)) return 1;
         } else if (c3b_launch_ingest_pileup_f32(x, x_dtype, xf, n * C3B_T * m->channels, s)) return 1;
         if (c3b_launch_lstm_f32(xf, m->lstm_f32[0][0], m->lstm_f32[0][1], l1, n, m->channels, C3B_H1, s)) return 1;
         if (c3b_launch_lstm_f32(l1, m->lstm_f32[1][0], m->lstm_f32[1][1], l2, n, 256, C3B_H2, s)) return 1;
@@ -697,7 +699,7 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
     int tile1 = m->lstm_tile;
     if (tile1 == 0) tile1 = !latency ? 64 : (bp / 64 >= m->sm_count) ? 64 : (bp / 32 >= m->sm_count) ? 32 : 16;
     const int tile2 = tile1 > 32 ? 32 : tile1;
-    { PROF("ingest"); if (c3b_launch_ingest_pileup_tc(x, x_dtype, m->channels, src.starts, src.n_cols, b.xs, n, (int)bp, s)) return 1; }
+    { PROF("ingest"); if (c3b_launch_ingest_pileup_tc(x, x_dtype, m->channels, src.starts, src.bounds, src.n_cols, b.xs, n, (int)bp, s)) return 1; }
     m->launches += 1;
     { PROF("lstm1"); if (c3b_launch_lstm1_tc(m, b, n, tile1, s)) return 1; }
     { PROF("proj2"); if (c3b_launch_proj2(m, b.h1, m->proj2, b.pg, (int)bp, s)) return 1; }
@@ -842,11 +844,12 @@ static size_t dtype_size(int dt) {
     return 0;
 }
 
-// Shared body of c3b_forward / c3b_forward_async / c3b_forward_windows.  starts != nullptr: x is the per-column count matrix
-// [n_cols][channels] and site b is its rows [starts[b], starts[b]+33).  sync_host: block until y is complete when a host
+// Shared body of c3b_forward / c3b_forward_async / c3b_forward_windows(_bounded).  starts != nullptr: x is the per-column count
+// matrix [n_cols][channels] and site b is its rows [starts[b], starts[b]+33), those outside [bounds[b][0], bounds[b][1]) (bounds
+// != nullptr) or outside the matrix read as zero.  sync_host: block until y is complete when a host
 // buffer is involved (the _torch_predict contract); otherwise everything stays stream-ordered (pinned host buffers).
 static int forward_impl(c3b_model *m, const void *x, int x_dtype, int x_on_device, int64_t batch, int depth, const int64_t *starts,
-                        int64_t n_cols, float *y, int y_on_device, cudaStream_t s, bool sync_host, const char *who) {
+                        const int64_t *bounds, int64_t n_cols, float *y, int y_on_device, cudaStream_t s, bool sync_host, const char *who) {
     if (!m) { c3b_set_error("%s: null model", who); return 1; }
     if (!m->finalized) { c3b_set_error("%s: load_state_dict/c3b_finalize has not completed", who); return 1; }
     if (batch < 0) { c3b_set_error("%s: negative batch", who); return 1; }
@@ -891,7 +894,7 @@ static int forward_impl(c3b_model *m, const void *x, int x_dtype, int x_on_devic
         w->fa_zeroed = false;       // fresh memory: the planar maps' borders / guards must be cleared again
     }
     const void *xd = x;
-    const int64_t *sd = starts;
+    const int64_t *sd = starts, *bd = bounds;
     float *yd = y;
     if (!x_on_device) {
         const size_t xbytes = starts ? (size_t)n_cols * m->channels * esz : (size_t)batch * site_elems * esz;
@@ -900,10 +903,16 @@ static int forward_impl(c3b_model *m, const void *x, int x_dtype, int x_on_devic
         C3B_CUDA(cudaMemcpyAsync(w->dev_x, x, xbytes, cudaMemcpyHostToDevice, s));
         xd = w->dev_x;
         if (starts) {
-            if (w->dev_aux_bytes < (size_t)batch * 8) C3B_CUDA(cudaStreamSynchronize(s));
-            if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, (size_t)batch * 8)) return 1;
+            const size_t aux = (size_t)batch * (bounds ? 24 : 8);        // starts, then the bounds pairs
+            if (w->dev_aux_bytes < aux) C3B_CUDA(cudaStreamSynchronize(s));
+            if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, aux)) return 1;
             C3B_CUDA(cudaMemcpyAsync(w->dev_aux, starts, (size_t)batch * 8, cudaMemcpyHostToDevice, s));
             sd = (const int64_t *)w->dev_aux;
+            if (bounds) {
+                int64_t *bdev = (int64_t *)w->dev_aux + batch;
+                C3B_CUDA(cudaMemcpyAsync(bdev, bounds, (size_t)batch * 16, cudaMemcpyHostToDevice, s));
+                bd = bdev;
+            }
         }
     }
     if (!y_on_device) {
@@ -921,6 +930,7 @@ static int forward_impl(c3b_model *m, const void *x, int x_dtype, int x_on_devic
             src.dtype = x_dtype;
             src.n_cols = n_cols;
             src.starts = starts ? sd + b0 : nullptr;
+            src.bounds = starts && bounds ? bd + 2 * b0 : nullptr;
             src.x = starts ? xd : (const void *)((const char *)xd + (size_t)b0 * site_elems * esz);
             rc = forward_pileup_chunk(m, w, src, n, yc, b0 == 0, sync_host && (!x_on_device || !y_on_device), s);
         } else {
@@ -940,22 +950,29 @@ static int forward_impl(c3b_model *m, const void *x, int x_dtype, int x_on_devic
 
 extern "C" int c3b_forward(c3b_model *m, const void *x, int x_dtype, int x_on_device, int64_t batch, int depth, float *y,
                            int y_on_device, void *cuda_stream) {
-    return forward_impl(m, x, x_dtype, x_on_device, batch, depth, nullptr, 0, y, y_on_device, (cudaStream_t)cuda_stream, true,
+    return forward_impl(m, x, x_dtype, x_on_device, batch, depth, nullptr, nullptr, 0, y, y_on_device, (cudaStream_t)cuda_stream, true,
                         "c3b_forward");
 }
 
 extern "C" int c3b_forward_async(c3b_model *m, const void *x_pinned, int x_dtype, int64_t batch, int depth, float *y_pinned,
                                  void *cuda_stream) {
-    return forward_impl(m, x_pinned, x_dtype, 0, batch, depth, nullptr, 0, y_pinned, 0, (cudaStream_t)cuda_stream, false,
+    return forward_impl(m, x_pinned, x_dtype, 0, batch, depth, nullptr, nullptr, 0, y_pinned, 0, (cudaStream_t)cuda_stream, false,
                         "c3b_forward_async");
+}
+
+extern "C" int c3b_forward_windows_bounded(c3b_model *m, const void *cols, int cols_dtype, int64_t n_cols, const int64_t *starts,
+                                           const int64_t *bounds, int on_device, int64_t batch, float *y, int y_on_device,
+                                           int host_sync, void *cuda_stream) {
+    if (m && m->kind != C3B_PILEUP) { c3b_set_error("c3b_forward_windows: pileup models only"); return 1; }
+    if (batch > 0 && (!starts || n_cols <= 0)) { c3b_set_error("c3b_forward_windows: null starts / empty matrix"); return 1; }
+    return forward_impl(m, cols, cols_dtype, on_device, batch, 0, starts, bounds, n_cols, y, y_on_device, (cudaStream_t)cuda_stream,
+                        host_sync != 0, "c3b_forward_windows");
 }
 
 extern "C" int c3b_forward_windows(c3b_model *m, const void *cols, int cols_dtype, int64_t n_cols, const int64_t *starts,
                                    int on_device, int64_t batch, float *y, int y_on_device, int host_sync, void *cuda_stream) {
-    if (m && m->kind != C3B_PILEUP) { c3b_set_error("c3b_forward_windows: pileup models only"); return 1; }
-    if (batch > 0 && (!starts || n_cols <= 0)) { c3b_set_error("c3b_forward_windows: null starts / empty matrix"); return 1; }
-    return forward_impl(m, cols, cols_dtype, on_device, batch, 0, starts, n_cols, y, y_on_device, (cudaStream_t)cuda_stream,
-                        host_sync != 0, "c3b_forward_windows");
+    return c3b_forward_windows_bounded(m, cols, cols_dtype, n_cols, starts, nullptr, on_device, batch, y, y_on_device, host_sync,
+                                       cuda_stream);
 }
 
 // ------------------------------------------------------------------------------------------------ decode, stage 1 (N1)

@@ -269,11 +269,12 @@ struct TcPileupBuffers {
     int bp;                // padded batch: multiple of 128
 };
 // starts == nullptr: x is the dense [batch][33][channels] tensor; otherwise x is the per-column matrix [n_cols][channels] and
-// site b is its rows [starts[b], starts[b] + 33) (rows outside the matrix read as zero)
-int c3b_launch_ingest_pileup_tc(const void *x, int dtype, int channels, const int64_t *starts, int64_t n_cols, op_t *xs, int64_t batch,
-                                int bp, cudaStream_t s);
-int c3b_launch_gather_windows_f32(const void *cols, int dtype, int channels, const int64_t *starts, int64_t n_cols, float *out,
-                                  int64_t batch, cudaStream_t s);
+// site b is its rows [starts[b], starts[b] + 33) (rows outside the matrix, and with bounds != nullptr rows outside
+// [bounds[2b], bounds[2b+1]), read as zero)
+int c3b_launch_ingest_pileup_tc(const void *x, int dtype, int channels, const int64_t *starts, const int64_t *bounds, int64_t n_cols,
+                                op_t *xs, int64_t batch, int bp, cudaStream_t s);
+int c3b_launch_gather_windows_f32(const void *cols, int dtype, int channels, const int64_t *starts, const int64_t *bounds,
+                                  int64_t n_cols, float *out, int64_t batch, cudaStream_t s);
 int c3b_launch_proj2(const c3b_model *m, const op_t *h1, const IgemmW &w, __half *pg, int bp, cudaStream_t s);
 int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, float *out, float *z4, int *nsplit_out, cudaStream_t s);
 int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s);

@@ -18,17 +18,20 @@ __global__ void ingest_f32_kernel(const T *__restrict__ x, float *__restrict__ o
     for (; i < n; i += stride) out[i] = (float)x[i];
 }
 
-// fp32 debug path of c3b_forward_windows: out[b][t][c] = cols[starts[b] + t][c], zero outside the matrix
+// fp32 debug path of c3b_forward_windows(_bounded): out[b][t][c] = cols[starts[b] + t][c], zero outside the matrix and outside
+// [bounds[b][0], bounds[b][1]) when bounds are given
 template <typename T>
-__global__ void gather_windows_f32_kernel(const T *__restrict__ cols, const int64_t *__restrict__ starts, int64_t n_cols, int channels,
-                                          float *__restrict__ out, int64_t n) {
+__global__ void gather_windows_f32_kernel(const T *__restrict__ cols, const int64_t *__restrict__ starts,
+                                          const int64_t *__restrict__ bounds, int64_t n_cols, int channels, float *__restrict__ out,
+                                          int64_t n) {
     const int per = C3B_T * channels;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n * per; i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t b = i / per;
         const int r = (int)(i - b * per);
         const int t = r / channels, c = r - t * channels;
         const int64_t row = starts[b] + t;
-        out[i] = (row >= 0 && row < n_cols) ? (float)cols[row * channels + c] : 0.f;
+        const bool have = row >= 0 && row < n_cols && (!bounds || (row >= bounds[2 * b] && row < bounds[2 * b + 1]));
+        out[i] = have ? (float)cols[row * channels + c] : 0.f;
     }
 }
 
@@ -201,16 +204,16 @@ int ingest_any(const void *x, int dtype, float *out, int64_t n, cudaStream_t s) 
 
 }  // namespace
 
-int c3b_launch_gather_windows_f32(const void *cols, int dtype, int channels, const int64_t *starts, int64_t n_cols, float *out,
-                                  int64_t batch, cudaStream_t s) {
+int c3b_launch_gather_windows_f32(const void *cols, int dtype, int channels, const int64_t *starts, const int64_t *bounds,
+                                  int64_t n_cols, float *out, int64_t batch, cudaStream_t s) {
     if (batch == 0) return 0;
     const int64_t n = batch * C3B_T * channels;
     const int blocks = (int)min((int64_t)4096, (n + 255) / 256);
     switch (dtype) {
-        case C3B_DT_I8: gather_windows_f32_kernel<int8_t><<<blocks, 256, 0, s>>>((const int8_t *)cols, starts, n_cols, channels, out, batch); break;
-        case C3B_DT_I32: gather_windows_f32_kernel<int32_t><<<blocks, 256, 0, s>>>((const int32_t *)cols, starts, n_cols, channels, out, batch); break;
-        case C3B_DT_I64: gather_windows_f32_kernel<int64_t><<<blocks, 256, 0, s>>>((const int64_t *)cols, starts, n_cols, channels, out, batch); break;
-        case C3B_DT_F32: gather_windows_f32_kernel<float><<<blocks, 256, 0, s>>>((const float *)cols, starts, n_cols, channels, out, batch); break;
+        case C3B_DT_I8: gather_windows_f32_kernel<int8_t><<<blocks, 256, 0, s>>>((const int8_t *)cols, starts, bounds, n_cols, channels, out, batch); break;
+        case C3B_DT_I32: gather_windows_f32_kernel<int32_t><<<blocks, 256, 0, s>>>((const int32_t *)cols, starts, bounds, n_cols, channels, out, batch); break;
+        case C3B_DT_I64: gather_windows_f32_kernel<int64_t><<<blocks, 256, 0, s>>>((const int64_t *)cols, starts, bounds, n_cols, channels, out, batch); break;
+        case C3B_DT_F32: gather_windows_f32_kernel<float><<<blocks, 256, 0, s>>>((const float *)cols, starts, bounds, n_cols, channels, out, batch); break;
         default: c3b_set_error("unsupported input dtype %d", dtype); return 1;
     }
     C3B_CUDA(cudaGetLastError());

@@ -301,14 +301,15 @@ template <typename T>
 __device__ __forceinline__ float ingest_to_float(T v) { return (float)v; }
 
 // Dense [batch][33][channels] tensor, or (starts != nullptr) 33-row windows of the per-column count matrix [n_cols][channels]
-// (libclair3's plp_data.matrix; preprocess/CreateTensorPileupFromCffi.py:362-394 slices the same windows on the host, zero
-// rows where a window overhangs the matrix) -> xs[t][bp][48] fp16 with columns [hi(x) | 1 | lo(x) | 0..]: hi = fp16(x)
+// (libclair3's plp_data.matrix; preprocess/CreateTensorPileupFromCffi.py:356-396 slices the same windows on the host, zero
+// rows where a window overhangs its contiguous run: rows outside [bounds[b][0], bounds[b][1]) and outside the matrix read as 0) -> xs[t][bp][48] fp16 with columns [hi(x) | 1 | lo(x) | 0..]: hi = fp16(x)
 // (saturating at +-65504), lo = fp16(x - hi), so hi + lo == x exactly for |x| <= 67 552 (past 65 519 hi stays at 65 504 and
 // lo > 2048 is itself rounded: error <= 16, <= 2^-12 relative, up to 131 008; saturating beyond); column `channels` = constant 1
 // (LSTM1's bias column).
 template <typename T>
-__global__ void ingest_pileup_tc_kernel(const T *__restrict__ x, const int64_t *__restrict__ starts, int64_t n_cols,
-                                        op_t *__restrict__ xs, int64_t batch, int bp, int channels) {
+__global__ void ingest_pileup_tc_kernel(const T *__restrict__ x, const int64_t *__restrict__ starts,
+                                        const int64_t *__restrict__ bounds, int64_t n_cols, op_t *__restrict__ xs, int64_t batch,
+                                        int bp, int channels) {
     // one thread per (t, site): six 16-byte stores
     const int64_t total = (int64_t)C3B_T * bp;
     for (int64_t tb = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; tb < total; tb += (int64_t)gridDim.x * blockDim.x) {
@@ -319,7 +320,7 @@ __global__ void ingest_pileup_tc_kernel(const T *__restrict__ x, const int64_t *
         if (have) {
             if (starts) {
                 const int64_t row = starts[b] + t;
-                have = row >= 0 && row < n_cols;
+                have = row >= 0 && row < n_cols && (!bounds || (row >= bounds[2 * b] && row < bounds[2 * b + 1]));
                 src = x + row * channels;
             } else {
                 src = x + ((int64_t)b * C3B_T + t) * channels;
@@ -381,16 +382,16 @@ int launch_lstm(const LstmDev &p, bool mufu16, int wg, cudaStream_t s) {
 
 }  // namespace
 
-int c3b_launch_ingest_pileup_tc(const void *x, int dtype, int channels, const int64_t *starts, int64_t n_cols, op_t *xs, int64_t batch,
-                                int bp, cudaStream_t s) {
+int c3b_launch_ingest_pileup_tc(const void *x, int dtype, int channels, const int64_t *starts, const int64_t *bounds, int64_t n_cols,
+                                op_t *xs, int64_t batch, int bp, cudaStream_t s) {
     const int64_t total = (int64_t)C3B_T * bp;
     const int blocks = (int)((total + 127) / 128 < 2048 ? (total + 127) / 128 : 2048);
     c3b_note_grid(blocks);
     switch (dtype) {
-        case C3B_DT_I8: ingest_pileup_tc_kernel<int8_t><<<blocks, 128, 0, s>>>((const int8_t *)x, starts, n_cols, xs, batch, bp, channels); break;
-        case C3B_DT_I32: ingest_pileup_tc_kernel<int32_t><<<blocks, 128, 0, s>>>((const int32_t *)x, starts, n_cols, xs, batch, bp, channels); break;
-        case C3B_DT_I64: ingest_pileup_tc_kernel<int64_t><<<blocks, 128, 0, s>>>((const int64_t *)x, starts, n_cols, xs, batch, bp, channels); break;
-        case C3B_DT_F32: ingest_pileup_tc_kernel<float><<<blocks, 128, 0, s>>>((const float *)x, starts, n_cols, xs, batch, bp, channels); break;
+        case C3B_DT_I8: ingest_pileup_tc_kernel<int8_t><<<blocks, 128, 0, s>>>((const int8_t *)x, starts, bounds, n_cols, xs, batch, bp, channels); break;
+        case C3B_DT_I32: ingest_pileup_tc_kernel<int32_t><<<blocks, 128, 0, s>>>((const int32_t *)x, starts, bounds, n_cols, xs, batch, bp, channels); break;
+        case C3B_DT_I64: ingest_pileup_tc_kernel<int64_t><<<blocks, 128, 0, s>>>((const int64_t *)x, starts, bounds, n_cols, xs, batch, bp, channels); break;
+        case C3B_DT_F32: ingest_pileup_tc_kernel<float><<<blocks, 128, 0, s>>>((const float *)x, starts, bounds, n_cols, xs, batch, bp, channels); break;
         default: c3b_set_error("unsupported input dtype %d", dtype); return 1;
     }
     C3B_CUDA(cudaGetLastError());

@@ -22,7 +22,8 @@
 //                        so the matrix is a compaction of the region).
 //   K5 plp_emit          compaction: int64 rows (plp_data.matrix is size_t), major, stats, the 16-column flanking test.
 //   K6 plp_quirk         the reference's index -1 quirk: a non-ACGT read base increments feature 17 of the PREVIOUS emitted column.
-//   K8 plp_cands         candidate list, window starts for c3b_forward_windows, window completeness test.
+//   K8 plp_cands         candidate list, window starts and run bounds for c3b_forward_windows_bounded, and the reference's verdict
+//                        on each candidate's window (plain, or with call_ht the zero-padded head / tail windows).
 //
 // Bound: HBM / L2 latency (integer work, no tensor cores).  Algorithmic bytes per call: 8 B per CIGAR word (read + offsets
 // written and re-read), 0.5 B per aligned base (packed sequence), ~27 B per read, and per column 72 + 24 + 4 B dense (written, read
@@ -555,6 +556,7 @@ __global__ void plp_quirk_kernel(const int64_t *n_cols_dev, const int64_t *__res
 // ---------------------------------------------------------------------------------------------------------------- K8
 struct CandArgs {
     int64_t start, end;
+    int call_ht;
     const int64_t *n_cols_dev;
     const int32_t *dci;
     const int32_t *stats;
@@ -562,6 +564,7 @@ struct CandArgs {
     const int64_t *tile_coff;
     int64_t *cand_cols;
     int64_t *wstart;
+    int64_t *wbounds;     // [n_cand][2]: the window rows [lo, hi) inside the candidate's contiguous run
     uint8_t *cand_ok;
 };
 
@@ -584,11 +587,22 @@ __global__ void __launch_bounds__(TILE) plp_cands_kernel(CandArgs A) {
         const int64_t j = A.tile_coff[blockIdx.x] + pre + __popc(bal & ((1u << lane) - 1u));
         A.cand_cols[j] = ci;
         A.wstart[j] = ci - FLANK;
-        // preprocess/CreateTensorPileupFromCffi.py:357-369: a full 33-row window, contiguous positions, no all-zero column
-        bool ok = ci - FLANK >= 0 && ci + FLANK < n;
-        if (ok) ok = A.major[ci + FLANK] - A.major[ci - FLANK] == 2 * FLANK;
-        for (int64_t q = ci - FLANK; ok && q <= ci + FLANK; ++q) ok = (A.stats[q * 6 + 5] & 2) == 0;
+        // preprocess/CreateTensorPileupFromCffi.py:356-396 over the contiguous chunks of :180-236 (oracle/pileup_oracle.c states
+        // it line by line): the candidate's run of consecutive positions, looked at from row ci - 16 to row ci + 18
+        int64_t lo = ci, hi = ci;
+        while (lo > ci - FLANK && lo > 0 && A.major[lo - 1] == A.major[lo] - 1) --lo;
+        while (hi < ci + FLANK + 2 && hi + 1 < n && A.major[hi + 1] == A.major[hi] + 1) ++hi;
+        const bool head_full = lo == ci - FLANK;
+        bool ok;
+        if (head_full && hi == ci + FLANK + 2) {            // :358 the run reaches two rows past the window; :365 no all-zero row
+            ok = true;
+            for (int64_t q = ci - FLANK; ok && q <= ci + FLANK; ++q) ok = (A.stats[q * 6 + 5] & 2) == 0;
+        } else {                                            // :370-396 head / tail windows, zero-padded, no all-zero test
+            ok = A.call_ht && hi > ci && (head_full || hi >= ci + FLANK);
+        }
         A.cand_ok[j] = ok ? 1 : 0;
+        A.wbounds[2 * j] = lo;
+        A.wbounds[2 * j + 1] = (hi < ci + FLANK ? hi : ci + FLANK) + 1;
     }
 }
 
@@ -608,7 +622,7 @@ struct c3b_plp {
     DBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n, ins_last;   // allele export (params.alt_info)
     DBuf counters;      // int64 n_cols, int64 n_cand, int g_used, int status
     // outputs
-    DBuf matrix, major, stats, cand_cols, wstart, cand_ok, gv_ref, gv_tot;
+    DBuf matrix, major, stats, cand_cols, wstart, wbounds, cand_ok, gv_ref, gv_tot;
     int64_t W = 0;
     bool gvcf = false, counted = false, alleles = false;
     cudaStream_t stream = nullptr;
@@ -712,7 +726,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         w->g_read.ensure((size_t)G_POOL * 4) || w->g_qpos.ensure((size_t)G_POOL * 4) || w->g_cnt.ensure((size_t)G_POOL * 4) ||
         w->g_next.ensure((size_t)G_POOL * 4) || w->counters.ensure(32) || w->matrix.ensure(Wz * NFEAT * 8) ||
         w->major.ensure(Wz * 8) || w->stats.ensure(Wz * 6 * 4) || w->cand_cols.ensure(Wz * 8) || w->wstart.ensure(Wz * 8) ||
-        w->cand_ok.ensure(Wz))
+        w->wbounds.ensure(Wz * 16) || w->cand_ok.ensure(Wz))
         return 1;
     if (w->gvcf && (w->gv_ref.ensure(Wz * 8) || w->gv_tot.ensure(Wz * 8))) return 1;
     w->alleles = params->alt_info != 0;
@@ -769,7 +783,8 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         CandArgs C;
         C.start = start; C.end = end; C.n_cols_dev = n_cols_dev; C.dci = w->dci.as<int32_t>(); C.stats = w->stats.as<int32_t>();
         C.major = w->major.as<int64_t>(); C.tile_coff = w->tile_coff.as<int64_t>(); C.cand_cols = w->cand_cols.as<int64_t>();
-        C.wstart = w->wstart.as<int64_t>(); C.cand_ok = w->cand_ok.as<uint8_t>();
+        C.wstart = w->wstart.as<int64_t>(); C.wbounds = w->wbounds.as<int64_t>(); C.cand_ok = w->cand_ok.as<uint8_t>();
+        C.call_ht = params->call_ht;
         plp_cands_kernel<<<tiles, TILE, 0, s>>>(C);
         w->launches += 6;
     }
@@ -850,6 +865,20 @@ int c3b_plp_device(c3b_plp *w, const int64_t **matrix, const int64_t **major, co
     return 0;
 }
 
+int c3b_plp_window_bounds(c3b_plp *w, int64_t *bounds, const int64_t **device_bounds) {
+    if (!w) { c3b_set_error("c3b_plp_window_bounds: null workspace"); return 1; }
+    if (device_bounds) {
+        if (!w->counted) { c3b_set_error("c3b_plp_window_bounds: no c3b_plp_count has been issued"); return 1; }
+        *device_bounds = w->wbounds.as<int64_t>();
+    }
+    if (bounds) {
+        if (w->n_cols < 0 && c3b_plp_sizes(w, nullptr, nullptr)) return 1;
+        if (w->n_cand) C3B_CUDA(cudaMemcpyAsync(bounds, w->wbounds.p, (size_t)w->n_cand * 16, cudaMemcpyDeviceToHost, w->stream));
+        C3B_CUDA(cudaStreamSynchronize(w->stream));
+    }
+    return 0;
+}
+
 int c3b_plp_last_ms(c3b_plp *w, float *ms, int *launches) {
     if (!w || !w->counted) { c3b_set_error("c3b_plp_last_ms: no c3b_plp_count has been issued"); return 1; }
     C3B_CUDA(cudaSetDevice(w->device));
@@ -867,7 +896,7 @@ void c3b_plp_destroy(c3b_plp *w) {
     DBuf *all[] = {&w->in_pos, &w->in_flag, &w->in_mapq, &w->in_coff, &w->in_cigar, &w->in_soff, &w->in_seq, &w->in_lq, &w->in_ref,
                    &w->opx, &w->opy, &w->rend, &w->pmax, &w->rows32, &w->dstats, &w->nquirk, &w->dci, &w->tile_cov, &w->tile_off,
                    &w->tile_cand, &w->tile_coff, &w->g_meta, &w->g_read, &w->g_qpos, &w->g_cnt, &w->g_next, &w->counters,
-                   &w->matrix, &w->major, &w->stats, &w->cand_cols, &w->wstart, &w->cand_ok, &w->gv_ref, &w->gv_tot,
+                   &w->matrix, &w->major, &w->stats, &w->cand_cols, &w->wstart, &w->wbounds, &w->cand_ok, &w->gv_ref, &w->gv_tot,
                    &w->al_meta, &w->al_read, &w->al_qpos, &w->al_cnt, &w->al_off, &w->al_n, &w->ins_last};
     for (DBuf *b : all) b->release();
     if (w->ev0) cudaEventDestroy(w->ev0);

@@ -173,11 +173,14 @@ class _C3BModule:
                                       ffi.cast("float *", y_host.data_ptr()), ffi.cast("void *", stream)))
         return y_host
 
-    def forward_windows(self, cols, starts, y=None, sync=True):
+    def forward_windows(self, cols, starts, y=None, sync=True, bounds=None):
         """Pileup only: ``c3b_forward_windows``.  ``cols`` is the per-column count matrix [n_cols, 18] (int64 = libclair3's
         ``plp_data.matrix``, or int32 / int8 / float32), ``starts`` the int64 first row of every candidate's 33-row window
-        (``preprocess/CreateTensorPileupFromCffi.py:362-366``: ``offset = pos - flanking - first_pos - 1``); both on the host
-        or both on the model's device.  Returns float32 [len(starts), 24|90] on the same side."""
+        (``preprocess/CreateTensorPileupFromCffi.py:359``: ``offset = pos - flanking - first_pos - 1``); both on the host
+        or both on the model's device.  ``bounds`` (optional, int64 [len(starts), 2] on the same side; pinned with
+        ``sync=False``): window b reads only rows [bounds[b, 0], bounds[b, 1]) and zeros elsewhere
+        (``c3b_forward_windows_bounded``) - the reference's zero padding outside a candidate's contiguous run (:374-391), as
+        ``PileupCounter.window_bounds()`` gives it.  Returns float32 [len(starts), 24|90] on the same side."""
         if self._handle is None:
             raise C3BError("model has no device/weights yet: call .to(device) and .load_state_dict() first")
         if self._kind != K["C3B_PILEUP"]:
@@ -198,19 +201,27 @@ class _C3BModule:
         starts = starts.to(torch.int64).contiguous()
         on_dev = cols.device.type == "cuda"
         batch = starts.shape[0]
+        if bounds is not None:
+            if isinstance(bounds, np.ndarray):
+                bounds = torch.from_numpy(bounds)
+            if tuple(bounds.shape) != (batch, 2) or bounds.device != starts.device:
+                raise C3BError("forward_windows: bounds must be [len(starts), 2] on the same device as starts")
+            bounds = bounds.to(torch.int64).contiguous()
         if y is None:
             y = torch.empty((batch, self.out_dim), dtype=torch.float32, device=cols.device)
         if tuple(y.shape) != (batch, self.out_dim) or y.dtype != torch.float32 or not y.is_contiguous():
             raise C3BError("forward_windows: y must be contiguous float32 [batch, %d]" % self.out_dim)
-        if not sync and not on_dev and not (cols.is_pinned() and starts.is_pinned() and y.is_pinned()):
+        if not sync and not on_dev and not (cols.is_pinned() and starts.is_pinned() and y.is_pinned()
+                                            and (bounds is None or bounds.is_pinned())):
             raise C3BError("forward_windows(sync=False) needs pinned host tensors")
         if batch == 0:
             return y
         stream = torch.cuda.current_stream(self._device).cuda_stream
-        check(lib().c3b_forward_windows(self._handle, ffi.cast("void *", cols.data_ptr()), dt[cols.dtype], cols.shape[0],
-                                        ffi.cast("int64_t *", starts.data_ptr()), int(on_dev), batch,
-                                        ffi.cast("float *", y.data_ptr()), int(y.device.type == "cuda"), int(bool(sync)),
-                                        ffi.cast("void *", stream)))
+        bptr = ffi.NULL if bounds is None else ffi.cast("int64_t *", bounds.data_ptr())
+        check(lib().c3b_forward_windows_bounded(self._handle, ffi.cast("void *", cols.data_ptr()), dt[cols.dtype], cols.shape[0],
+                                                ffi.cast("int64_t *", starts.data_ptr()), bptr, int(on_dev), batch,
+                                                ffi.cast("float *", y.data_ptr()), int(y.device.type == "cuda"), int(bool(sync)),
+                                                ffi.cast("void *", stream)))
         return y
 
     def decode_stage1(self, y, ref_gt21):

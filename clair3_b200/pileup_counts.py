@@ -238,11 +238,21 @@ class PileupCounter:
                                        fetch_end=end + FETCH_EXPAND + 1))
         return out
 
+    def window_bounds(self):
+        """int64 [n_cand, 2]: the rows [lo, hi) of each candidate's 33-row window (from ``cand_cols - 16``) that lie in its
+        contiguous run of positions (``c3b_plp_window_bounds``); the reference's tensor is zero on the window's other rows
+        (``preprocess/CreateTensorPileupFromCffi.py:374-391``)."""
+        _, nk = self.sizes()
+        out = np.zeros((nk, 2), np.int64)
+        check(lib().c3b_plp_window_bounds(self._h, ffi.cast("int64_t *", out.ctypes.data), ffi.NULL))
+        return out
+
     def forward(self, model):
         """Clair3_P over the 33-column window of EVERY candidate of the last count, straight from the device-resident matrix
-        (``c3b_forward_windows`` with ``on_device = 1``).  Returns (probabilities float32 [n_cand, 24|90] on the device, cand_ok
-        uint8 [n_cand] on the host): rows whose window is incomplete (``cand_ok == 0`` - the reference drops those candidates,
-        ``preprocess/CreateTensorPileupFromCffi.py:362-369``) are computed on zero-padded windows and must be ignored."""
+        (``c3b_forward_windows_bounded`` with ``on_device = 1``): each window reads its candidate's contiguous run and zeros
+        outside it, which is the tensor the reference builds (``preprocess/CreateTensorPileupFromCffi.py:356-396``).  Returns
+        (probabilities float32 [n_cand, 24|90] on the device, cand_ok uint8 [n_cand] on the host): ``cand_ok == 0``: the
+        reference drops that candidate, and its row must be ignored."""
         if getattr(model, "_handle", None) is None:
             raise C3BError("forward: the model has no device / weights yet (.to(device), .load_state_dict())")
         if getattr(model, "input_channels", CHANNELS) != CHANNELS or model._kind != lib_const("C3B_PILEUP"):
@@ -254,11 +264,13 @@ class PileupCounter:
         ok = np.zeros(nk, np.uint8)
         if nk == 0:
             return y, ok
-        pm, ps, pk = ffi.new("const int64_t **"), ffi.new("const int64_t **"), ffi.new("const uint8_t **")
+        pm, ps, pk, pb = (ffi.new("const int64_t **"), ffi.new("const int64_t **"), ffi.new("const uint8_t **"),
+                          ffi.new("const int64_t **"))
         check(lib().c3b_plp_device(self._h, pm, ffi.NULL, ffi.NULL, ps, pk))
+        check(lib().c3b_plp_window_bounds(self._h, ffi.NULL, pb))
         stream = torch.cuda.current_stream(self._device).cuda_stream
-        check(lib().c3b_forward_windows(model._handle, ffi.cast("void *", pm[0]), lib_const("C3B_DT_I64"), nc, ps[0], 1, nk,
-                                        ffi.cast("float *", y.data_ptr()), 1, 0, ffi.cast("void *", stream)))
+        check(lib().c3b_forward_windows_bounded(model._handle, ffi.cast("void *", pm[0]), lib_const("C3B_DT_I64"), nc, ps[0], pb[0],
+                                                1, nk, ffi.cast("float *", y.data_ptr()), 1, 0, ffi.cast("void *", stream)))
         check(lib().c3b_plp_fetch(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.cast("uint8_t *", ok.ctypes.data), ffi.NULL, ffi.NULL))
         return y, ok
 

@@ -91,12 +91,21 @@ int c3b_forward_async(c3b_model *m, const void *x_pinned, int x_dtype, int64_t b
  * materialising one [33,18] tensor per candidate (windows of neighbouring candidates overlap in 32 of 33 rows), hand over
  * libclair3's per-column count matrix once - plp_data.matrix, size_t[n_cols][18] (src/clair3_pileup.h:5-17), i.e.
  * cols_dtype C3B_DT_I64; C3B_DT_I32 / I8 / F32 also accepted - plus the first row of every candidate's window:
- * site b = rows [starts[b], starts[b]+33) of cols; rows outside [0, n_cols) read as zero (the reference's zero padding at a
- * sequence head / tail, :372-394).  The windows are gathered on the GPU straight into the LSTM operand layout.
+ * site b = rows [starts[b], starts[b]+33) of cols; rows outside [0, n_cols) read as zero.  That alone is not the reference's
+ * zero padding: its head / tail windows (:370-396) are zero outside the candidate's CONTIGUOUS RUN of positions, and at a
+ * coverage gap the matrix holds the neighbouring run's columns there - c3b_forward_windows_bounded takes those bounds.
+ * The windows are gathered on the GPU straight into the LSTM operand layout.
  * on_device: cols and starts are device pointers (else host; they are copied on cuda_stream).  host_sync: 1 = return after y
  * is complete when a host buffer is involved, 0 = stay stream-ordered (pinned buffers, caller synchronises). */
 int c3b_forward_windows(c3b_model *m, const void *cols, int cols_dtype, int64_t n_cols, const int64_t *starts,
                         int on_device, int64_t batch, float *y, int y_on_device, int host_sync, void *cuda_stream);
+
+/* c3b_forward_windows with per-window row bounds: bounds (NULL, or [batch][2] int64 on the same side as starts) = {lo, hi};
+ * site b's rows outside [lo, hi) read as zero as well.  c3b_plp_window_bounds (clair3_b200_pileup.h) yields the bounds of the
+ * reference's windows; NULL bounds is c3b_forward_windows. */
+int c3b_forward_windows_bounded(c3b_model *m, const void *cols, int cols_dtype, int64_t n_cols, const int64_t *starts,
+                                const int64_t *bounds, int on_device, int64_t batch, float *y, int y_on_device, int host_sync,
+                                void *cuda_stream);
 
 /* 24 or 90 (clair3/model.py:153-159). */
 int c3b_out_dim(const c3b_model *m);

@@ -52,7 +52,8 @@ typedef struct c3b_plp_params {
     float min_indel_af;
     int32_t min_mq;
     int32_t call_snp_only;
-    int32_t call_ht;            /* 1: no 16-column flanking requirement (src/clair3_pileup.c:385-387) */
+    int32_t call_ht;            /* 1: no 16-column flanking requirement (src/clair3_pileup.c:385-387), and cand_ok keeps the head /
+                                   tail windows of preprocess/CreateTensorPileupFromCffi.py:370-396 */
     int32_t gvcf;               /* 1: also fill pos_ref_count / pos_total_count (:205-210, :453-456) */
     int32_t alt_info;           /* 1: also export every pre-candidate column's distinct indel alleles (c3b_plp_fetch_alleles), from
                                    which the host formats the all_alt_info text of :391-450 */
@@ -78,8 +79,14 @@ int c3b_plp_sizes(c3b_plp *w, int64_t *n_cols, int64_t *n_candidates);
  *   stats        [n_cols][6]  int32   depth, ref_count, alt_count, del_count, ins_count, flags (bit 0: candidate = pass_af of
  *                                     :371-387; bit 1: all 18 features are zero)
  *   cand_cols    [n_cand]     int64   column index of every candidate, ascending (all_alt_info order)
- *   cand_ok      [n_cand]     uint8   1: the 33-column window around the candidate is complete, contiguous in position and has no
- *                                     all-zero column - the test of preprocess/CreateTensorPileupFromCffi.py:357-369
+ *   cand_ok      [n_cand]     uint8   1: the reference keeps a tensor for this candidate - the candidate loop of
+ *                                     preprocess/CreateTensorPileupFromCffi.py:356-396 over the contiguous runs of :180-236.
+ *                                     Plain (:358-366): the candidate's run of consecutive positions covers the window's first
+ *                                     row and reaches TWO rows past its last (column c + 18), and no row of the window is
+ *                                     all-zero.  Only with params.call_ht, when that fails (:370-396): the candidate is not on
+ *                                     its run's last column, and either the run starts inside the window and reaches column
+ *                                     c + 16 (head) or the run covers the window's first row (tail); these windows are
+ *                                     zero-padded outside the run (c3b_plp_window_bounds) and skip the all-zero test.
  *   pos_ref_count / pos_total_count [end - start] int64 (only with params.gvcf)                                  */
 int c3b_plp_fetch(c3b_plp *w, int64_t *matrix, int64_t *major, int32_t *stats, int64_t *cand_cols, uint8_t *cand_ok,
                   int64_t *pos_ref_count, int64_t *pos_total_count);
@@ -106,6 +113,12 @@ int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, int32_t *i
  * Clair3_P. */
 int c3b_plp_device(c3b_plp *w, const int64_t **matrix, const int64_t **major, const int64_t **cand_cols,
                    const int64_t **window_starts, const uint8_t **cand_ok);
+
+/* The rows of every candidate's window that belong to its contiguous run, [n_cand][2] int64 = {lo, hi}: matrix rows [lo, hi)
+ * with cand_cols - 16 <= lo <= cand_cols < hi <= cand_cols + 17.  The reference's tensor holds zeros for the window's other rows
+ * (:374-391); the matrix holds the neighbouring runs' columns there.  These are the `bounds` of c3b_forward_windows_bounded.
+ * bounds: host copy (waits for the count); device_bounds: device view, valid until the next c3b_plp_count.  Either may be NULL. */
+int c3b_plp_window_bounds(c3b_plp *w, int64_t *bounds, const int64_t **device_bounds);
 
 /* Device time of the last c3b_plp_count (CUDA events on its stream around all of its kernels, input copies excluded), and the
  * number of kernels it launched. */

@@ -262,13 +262,14 @@ typedef struct {
 
 /* Outputs (caller-allocated for W = end - start columns): matrix [W][18], major [W], stats [W][6] = depth, ref_count, alt_count,
  * del_count, ins_count, flags (bit 0 = candidate, bit 1 = all 18 features zero); cand_cols / cand_ok [W]; pos_ref_count /
- * pos_total_count [W] (only written with gvcf).  Returns 0, or 1 on an allocation failure. */
+ * pos_total_count [W] (only written with gvcf); win_bounds [W][2] (optional: each candidate's window rows [lo, hi) inside its
+ * contiguous run).  Returns 0, or 1 on an allocation failure. */
 int oracle_clair3_pileup(int64_t n_reads, const int64_t *rpos, const uint16_t *flag, const uint8_t *mapq,
                          const int64_t *cigar_off, const uint32_t *cigar, const int64_t *seq_off, const uint8_t *seq,
                          const int32_t *l_qseq, int64_t start, int64_t end, const char *ref_seq, int64_t ref_start, int64_t ref_len,
                          const plp_params_t *prm, int64_t *n_cols_out, int64_t *matrix, int64_t *major, int32_t *stats,
                          int64_t *cand_cols, uint8_t *cand_ok, int64_t *n_cand_out, int64_t *pos_ref_count,
-                         int64_t *pos_total_count, char *alt_text, int64_t alt_cap, int64_t *alt_len) {
+                         int64_t *pos_total_count, char *alt_text, int64_t alt_cap, int64_t *alt_len, int64_t *win_bounds) {
     /* alt_text (optional): the all_alt_info strings of the candidates, one per line, in candidate order */
     text_t txt = {alt_text, 0, alt_cap};
     if (alt_text && alt_cap > 0) alt_text[0] = 0;
@@ -487,20 +488,42 @@ int oracle_clair3_pileup(int64_t n_reads, const int64_t *rpos, const uint16_t *f
         for (int64_t i = 0; i < n_ins; ++i) free(ins[i].nibs);
         free(ins); free(dels_f); free(dels_r);
     }
-    /* the quirk may have made a previously all-zero row non-zero (or the reverse cannot happen): recompute the zero flags, then the
-     * window test of preprocess/CreateTensorPileupFromCffi.py:357-369 for every candidate: 33 emitted columns around it, contiguous
-     * in position, none of them all-zero */
+    /* the quirk may have made a previously all-zero row non-zero (or the reverse cannot happen): recompute the zero flags */
     for (int64_t c = 0; c < n_cols; ++c) {
         int zero = 1;
         for (int i = 0; i < FEAT; ++i) if (matrix[c * FEAT + i]) zero = 0;
         stats[c * 6 + 5] = (stats[c * 6 + 5] & 1) | (zero ? 2 : 0);
     }
+    /* The candidate loop of preprocess/CreateTensorPileupFromCffi.py:356-396 over the contiguous chunks of :180-236 (runs of
+     * consecutive positions).  The candidate is on matrix row c, 1-based position pos = major[c] + 1; its run is looked at from
+     * row c - 16 (lo) to row c + 18 (hi) at most.
+     *   :358  start - 1 >= first and end <= last: the run covers row c - 16 and reaches row c + 18, two rows past the window;
+     *   :365  ... and none of the 33 rows is all-zero.
+     * With call_ht (:370-396), when that fails:
+     *   :371  pos > last: a candidate on the run's last row is skipped;
+     *   :374  head: the run starts after row c - 16 and reaches row c + 16 - zero rows in front, no all-zero test;
+     *   :384  tail: the run covers row c - 16 and ends before row c + 18 - zero rows behind (from row c + 16 on, none), no test.
+     * win_bounds (optional) [n_cand][2]: the window rows [lo, hi) that belong to the run; the others are the reference's zeros. */
     for (int64_t j = 0; j < n_cand; ++j) {
-        int64_t c = cand_cols[j];
-        int ok = c - FLANK >= 0 && c + FLANK < n_cols && major[c + FLANK] - major[c - FLANK] == 2 * FLANK;
-        for (int64_t q = c - FLANK; ok && q <= c + FLANK; ++q)
-            if (stats[q * 6 + 5] & 2) ok = 0;
+        int64_t c = cand_cols[j], lo = c, hi = c;
+        while (lo > c - FLANK && lo > 0 && major[lo - 1] == major[lo] - 1) --lo;
+        while (hi < c + FLANK + 2 && hi + 1 < n_cols && major[hi + 1] == major[hi] + 1) ++hi;
+        int head_full = lo == c - FLANK;
+        int ok;
+        if (head_full && hi == c + FLANK + 2) {
+            ok = 1;
+            for (int64_t q = c - FLANK; ok && q <= c + FLANK; ++q)
+                if (stats[q * 6 + 5] & 2) ok = 0;
+        } else if (prm->call_ht) {
+            ok = hi > c && (head_full || hi >= c + FLANK);
+        } else {
+            ok = 0;
+        }
         cand_ok[j] = (uint8_t)ok;
+        if (win_bounds) {
+            win_bounds[2 * j] = lo;
+            win_bounds[2 * j + 1] = (hi < c + FLANK ? hi : c + FLANK) + 1;
+        }
     }
     *n_cols_out = n_cols;
     *n_cand_out = n_cand;

@@ -49,7 +49,9 @@ def clair3_pileup(reads, start, end, ref_seq, ref_start, min_depth=2, min_snp_af
                   call_snp_only=False, call_ht=False, gvcf=False, max_indel_length=50, alt_info=False):
     """reads: dict of numpy arrays with the keys of ``clair3_b200.pileup_counts.BamRecords`` (pos, flag, mapq, cigar_off, cigar,
     seq_off, seq, l_qseq).  Returns a dict: matrix [n_cols,18] int64, major [n_cols] int64, stats [n_cols,6] int32, cand_cols,
-    cand_ok, pos_ref_count, pos_total_count (+ alt_info: the all_alt_info strings of the candidates, with ``alt_info=True``)."""
+    cand_ok, pos_ref_count, pos_total_count, window_bounds [n_cand,2] int64 (the rows [lo, hi) of each candidate's window that
+    lie in its contiguous run; the reference reads the others as zero) (+ alt_info: the all_alt_info strings of the candidates,
+    with ``alt_info=True``)."""
     L = _load()
     n = int(len(reads["pos"]))
     W = max(int(end - start), 0)
@@ -76,11 +78,12 @@ def clair3_pileup(reads, start, end, ref_seq, ref_start, min_depth=2, min_snp_af
     alt_cap = 64 * 1024 * 1024 if alt_info else 0
     alt_buf = ctypes.create_string_buffer(alt_cap) if alt_info else None
     alt_len = ctypes.c_int64(0)
+    bounds = np.zeros((W, 2), dtype=np.int64)
     rc = L.oracle_clair3_pileup(ctypes.c_int64(n), _p(pos), _p(flag), _p(mapq), _p(cigar_off), _p(cigar), _p(seq_off), _p(seq),
                                 _p(l_qseq), ctypes.c_int64(int(start)), ctypes.c_int64(int(end)), _p(ref),
                                 ctypes.c_int64(int(ref_start)), ctypes.c_int64(len(ref)), ctypes.byref(prm),
                                 ctypes.byref(n_cols), _p(matrix), _p(major), _p(stats), _p(cand), _p(ok), ctypes.byref(n_cand),
-                                _p(prc), _p(ptc), alt_buf, ctypes.c_int64(alt_cap), ctypes.byref(alt_len))
+                                _p(prc), _p(ptc), alt_buf, ctypes.c_int64(alt_cap), ctypes.byref(alt_len), _p(bounds))
     if rc != 0:
         raise MemoryError("oracle_clair3_pileup failed")
     nc, nk = n_cols.value, n_cand.value
@@ -90,7 +93,7 @@ def clair3_pileup(reads, start, end, ref_seq, ref_start, min_depth=2, min_snp_af
             raise MemoryError("alt_info text buffer too small")
         extra["alt_info"] = alt_buf.raw[:alt_len.value].decode().split("\n")[:-1]
     return {**extra, "matrix": matrix[:nc].copy(), "major": major[:nc].copy(), "stats": stats[:nc].copy(), "cand_cols": cand[:nk].copy(),
-            "cand_ok": ok[:nk].copy(), "pos_ref_count": prc, "pos_total_count": ptc}
+            "cand_ok": ok[:nk].copy(), "pos_ref_count": prc, "pos_total_count": ptc, "window_bounds": bounds[:nk].copy()}
 
 
 def _reads_overlapping(rec, lo, hi):

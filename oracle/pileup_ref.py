@@ -98,17 +98,11 @@ def kept_reads(rec, min_mq):
     return np.nonzero(keep)[0], rend
 
 
-def clair3_pileup(reads, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.08, min_indel_af=0.15, min_mq=5,
-                  call_snp_only=False, call_ht=False, gvcf=False, max_indel_length=50, alt_info=True):
-    """The reference function on in-memory records, with the arguments of ``oracle.pileup_oracle.clair3_pileup``: records as
-    ``clair3_b200.pileup_counts.BamRecords`` arrays, region [start, end) 0-based, reference bases [ref_start, ref_start +
-    len(ref_seq)).  The contig is registered as ``'N' * ref_start + ref_seq`` and queried as ``ctg:{start+1}-{end}``.  Returns a
-    dict: matrix [n_cols, 18] int64, major [n_cols] int64, alt_info (the candidates' strings), cand_cols (the column of each
-    candidate, from its string), pos_ref_count / pos_total_count [end - start] (with ``gvcf``; zeros otherwise).  ``alt_info`` is
-    accepted for signature parity; the strings are always returned.
-
-    Raises ValueError when a read the reference keeps reaches past the contig end: the reference would read the reference
-    sequence out of bounds there (see DESIGN.md, the pileup counter's deviations)."""
+def register(reads, ref_seq, ref_start, min_mq):
+    """Registers the records and the contig ``'N' * ref_start + ref_seq`` (named ``CONTIG``) with the stand-in, for the next
+    ``calculate_clair3_pileup``.  Returns (the record arrays, the contig bytes): the stand-in keeps pointers into them, so the
+    caller holds on to them until its calls are done.  Raises ValueError when a read the reference keeps reaches past the contig
+    end: the reference would read the reference sequence out of bounds there (see DESIGN.md, the pileup counter's deviations)."""
     L = _load()
     ref = ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq)
     contig = b"N" * int(ref_start) + ref
@@ -126,6 +120,22 @@ def clair3_pileup(reads, start, end, ref_seq, ref_start, min_depth=2, min_snp_af
     L.fa_ref_set_contig(CONTIG.encode(), contig, len(contig))
     L.fa_ref_set_records(n, *[_ptr(arr[k]) for k in ("pos", "flag", "mapq", "cigar_off", "cigar", "seq_off", "seq", "l_qseq")],
                          None, None, None, None, None, None)
+    return arr, contig
+
+
+def clair3_pileup(reads, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.08, min_indel_af=0.15, min_mq=5,
+                  call_snp_only=False, call_ht=False, gvcf=False, max_indel_length=50, alt_info=True):
+    """The reference function on in-memory records, with the arguments of ``oracle.pileup_oracle.clair3_pileup``: records as
+    ``clair3_b200.pileup_counts.BamRecords`` arrays, region [start, end) 0-based, reference bases [ref_start, ref_start +
+    len(ref_seq)).  The contig is registered as ``'N' * ref_start + ref_seq`` and queried as ``ctg:{start+1}-{end}``.  Returns a
+    dict: matrix [n_cols, 18] int64, major [n_cols] int64, alt_info (the candidates' strings), cand_cols (the column of each
+    candidate, from its string), pos_ref_count / pos_total_count [end - start] (with ``gvcf``; zeros otherwise).  ``alt_info`` is
+    accepted for signature parity; the strings are always returned.
+
+    Raises ValueError when a read the reference keeps reaches past the contig end: the reference would read the reference
+    sequence out of bounds there (see DESIGN.md, the pileup counter's deviations)."""
+    L = _load()
+    keep = register(reads, ref_seq, ref_start, min_mq)     # noqa: F841 - the stand-in reads these arrays during the call
     fset = L.create_bam_fset(b"in-memory.bam", b"in-memory.fa")
     region = ("%s:%d-%d" % (CONTIG, int(start) + 1, int(end))).encode()
     try:

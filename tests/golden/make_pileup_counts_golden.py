@@ -4,7 +4,9 @@ compiled by oracle/pileup_ref.py (needs the reference checkout: CLAIR3_REFERENCE
 pileup_counts.npz: two small seeded record sets, INPUT RECORDS INCLUDED, so that the committed vectors pin both the C oracle and
 (on a GPU) the CUDA counter against drift.  matrix, major, cand_cols, the all_alt_info strings and the gVCF arrays are the
 reference's outputs; stats and cand_ok, which the reference does not have, come from oracle/pileup_oracle.c, and the script
-refuses to write anything unless the oracle equals the reference on every shared output.  These vectors are reference-confirmed.
+refuses to write anything unless the oracle equals the reference on every shared output - cand_ok included: the positions it
+keeps must be those the reference's own CreateTensorPileup keeps (oracle/pileup_tensor_ref.py) for the 1-based slice whose
+counter region is the case's region.  These vectors are reference-confirmed.
 
 pileup_ref_cases.npz: the reference's outputs on every targeted case of tests/plp_ref_cases.py (the inputs are rebuilt from that
 module's code), so those cases pin the oracle even where oracle/_ref/ was not built.
@@ -19,11 +21,12 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from clair3_b200 import synth_reads as sr  # noqa: E402
-from oracle import pileup_oracle as po, pileup_ref as pr  # noqa: E402
+from clair3_b200.pileup_counts import counting_region  # noqa: E402
+from oracle import pileup_oracle as po, pileup_ref as pr, pileup_tensor_ref as ptr  # noqa: E402
 import plp_ref_cases as cases  # noqa: E402
 from test_pileup_reference_cpu import compare  # noqa: E402
 
-if pr.build() is None:
+if pr.build() is None or not ptr.available():
     sys.exit("the reference checkout is needed: set CLAIR3_REFERENCE")
 
 out = {}
@@ -35,6 +38,12 @@ for tag, kw, cnt in (("a", dict(region_len=600, depth=25, read_len=300, seed=71,
     want = pr.clair3_pileup(rec, start, end, ref, rs, **cnt)
     r = po.clair3_pileup(rec, start, end, ref, rs, alt_info=True, **cnt)
     compare("pileup_counts_%s" % tag, r, want, True)
+    ctg_start, ctg_end = start + 35, end - 33
+    assert counting_region(ctg_start, ctg_end) == (start, end)
+    _, pos_info, _ = ptr.create_tensor_pileup(rec, ref, rs, ctg_start, ctg_end, call_ht=cnt.get("call_ht", False))
+    kept = r["major"][r["cand_cols"][r["cand_ok"] == 1]] + 1
+    if not np.array_equal(kept, ptr.kept_positions(pos_info)):
+        sys.exit("pileup_counts_%s: the oracle's cand_ok keeps %s, the reference %s" % (tag, kept.tolist(), ptr.kept_positions(pos_info).tolist()))
     for k, v in rec.items():
         out["%s_rec_%s" % (tag, k)] = v
     out["%s_ref" % tag] = np.frombuffer(ref.encode(), dtype=np.uint8)

@@ -149,11 +149,20 @@ def model_pileup(rec, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.
         stats[:, 5] |= np.where((matrix == 0).all(axis=1), 2, 0).astype(np.int32)
     major = np.array(major, np.int64)
     cand = np.nonzero(stats[:, 5] & 1)[0].astype(np.int64) if len(stats) else np.zeros(0, np.int64)
-    okw = []
-    for c in cand:
-        g = c - 16 >= 0 and c + 16 < len(major) and major[c + 16] - major[c - 16] == 32
-        g = g and not (stats[c - 16:c + 17, 5] & 2).any()
+    okw, bounds = [], []
+    for c in cand:            # preprocess/CreateTensorPileupFromCffi.py:356-396 (see oracle/pileup_oracle.c)
+        lo, hi = c, c
+        while lo > max(c - 16, 0) and major[lo - 1] == major[lo] - 1:
+            lo -= 1
+        while hi < min(c + 18, len(major) - 1) and major[hi + 1] == major[hi] + 1:
+            hi += 1
+        if lo == c - 16 and hi == c + 18:
+            g = not (stats[c - 16:c + 17, 5] & 2).any()
+        else:
+            g = call_ht and hi > c and (lo == c - 16 or hi >= c + 16)
         okw.append(1 if g else 0)
+        bounds.append((lo, min(hi, c + 16) + 1))
     return {"matrix": matrix, "major": major, "stats": stats, "cand_cols": cand, "cand_ok": np.array(okw, np.uint8),
+            "window_bounds": np.array(bounds, np.int64).reshape(-1, 2),
             "alleles": alleles,        # per emitted column: (meta, first read, query offset, count) as c3b_plp_fetch_alleles exports them
             "ins_last": np.array(last, np.int64)}

@@ -16,7 +16,7 @@ from clair3_b200 import synth_reads as sr
 from oracle import pileup_oracle as po
 from plp_model import model_pileup
 
-KEYS = ("matrix", "major", "stats", "cand_cols", "cand_ok")
+KEYS = ("matrix", "major", "stats", "cand_cols", "cand_ok", "window_bounds")
 
 
 def case_indels():
@@ -117,7 +117,9 @@ def test_adjacent_deletions_merge_and_insertion_after_deletion():
 
 
 @pytest.mark.parametrize("seed", range(8))
-def test_oracle_matches_random_access_model(seed):
+def test_oracle_matches_random_access_model_with_reference_windows(seed):
+    """Every output, including the window verdict and bounds of the reference's candidate loop
+    (preprocess/CreateTensorPileupFromCffi.py:356-396; tests/test_pileup_windows_cpu.py holds both to the reference itself)."""
     wild = seed % 2 == 0
     origin = [1000, 0, 5, 300][seed % 4]
     gaps = [(origin + 100, origin + 160)] if seed % 3 == 0 else ()
@@ -339,9 +341,10 @@ def test_forward_argument_checks_without_a_gpu():
 
 
 @pytest.mark.parametrize("block", range(4))
-def test_arbitrary_operation_orders(block):
+def test_arbitrary_operation_orders_with_reference_windows(block):
     """CIGARs with the nine operations in ANY order (leading deletions / skips / pads, trailing insertions, runs of the same
-    operation, clips in the middle): the oracle's incremental htslib cursor and the random-access model still agree on every output."""
+    operation, clips in the middle): the oracle's incremental htslib cursor and the random-access model still agree on every output,
+    the reference's window verdict and bounds included."""
     ops_all = "MIDNSHP=X"
     for seed in range(block * 15, block * 15 + 15):
         rng = np.random.default_rng(1000 + seed)
@@ -374,10 +377,11 @@ def load_counts_golden(tag):
 
 
 @pytest.mark.parametrize("tag", ["a", "b"])
-def test_oracle_against_reference_confirmed_vectors(tag):
+def test_oracle_against_reference_confirmed_vectors_and_windows(tag):
     """tests/golden/pileup_counts.npz (tests/golden/make_pileup_counts_golden.py): records in, every output array and the
-    all_alt_info strings out, minted from the reference's own calculate_clair3_pileup (stats and cand_ok, which the reference does
-    not have, from the oracle after it was checked equal on everything else)."""
+    all_alt_info strings out, minted from the reference's own calculate_clair3_pileup.  stats, which the reference does not have,
+    come from the oracle after it was checked equal on everything else; cand_ok is the oracle's window verdict after it was
+    checked equal to the positions the reference's own CreateTensorPileup keeps."""
     rec, ref, rs, start, end, kw, want = load_counts_golden(tag)
     got = po.clair3_pileup(rec, start, end, ref, rs, alt_info=True, **kw)
     for k in ("matrix", "major", "stats", "cand_cols", "cand_ok") + (("pos_ref_count", "pos_total_count") if kw["gvcf"] else ()):

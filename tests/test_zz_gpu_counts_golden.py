@@ -21,11 +21,14 @@ def counter():
 
 
 @pytest.mark.parametrize("tag", ["a", "b"])
-def test_reference_confirmed_golden_vectors(counter, tag):
-    """The counter against tests/golden/pileup_counts.npz, minted from the reference's own calculate_clair3_pileup."""
+def test_reference_confirmed_golden_vectors_and_windows(counter, tag):
+    """The counter against tests/golden/pileup_counts.npz, minted from the reference's own calculate_clair3_pileup, with cand_ok
+    confirmed against the reference's own CreateTensorPileup; the window bounds against the C oracle."""
+    from oracle import pileup_oracle as po
     from test_pileup_oracle import load_counts_golden
     rec, ref, rs, start, end, kw, want = load_counts_golden(tag)
     got = counter.count(rec, start, end, ref, rs, alt_info=True, **kw).fetch()
     for k in ("major", "matrix", "stats", "cand_cols", "cand_ok") + (("pos_ref_count", "pos_total_count") if kw["gvcf"] else ()):
         assert got[k].shape == want[k].shape and np.array_equal(got[k], want[k]), k
     assert counter.alt_info_strings(got) == want["alt_info"]
+    assert np.array_equal(counter.window_bounds(), po.clair3_pileup(rec, start, end, ref, rs, **kw)["window_bounds"])
