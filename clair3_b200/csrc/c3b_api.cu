@@ -1085,6 +1085,62 @@ extern "C" int c3b_decode_stage2(c3b_model *m, const float *y, const uint8_t *re
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ decode, stage 3 (calls)
+extern "C" int c3b_decode_calls(c3b_model *m, const float *y, const uint8_t *ref_base, int64_t batch, const char *alt_bytes,
+                                const int64_t *alt_offsets, int64_t n_alt_bytes, uint32_t config, int64_t max_infer_len, int k,
+                                int on_device, c3b_call *calls, char *text, int64_t *ad, void *cuda_stream) {
+    if (!m) { c3b_set_error("c3b_decode_calls: null model"); return 1; }
+    if (batch < 0 || n_alt_bytes < 0) { c3b_set_error("c3b_decode_calls: negative batch or n_alt_bytes"); return 1; }
+    if (k < 1 || k > 1024) { c3b_set_error("c3b_decode_calls: k must be in [1, 1024]"); return 1; }
+    if (config & ~31u) { c3b_set_error("c3b_decode_calls: unknown config bits 0x%x", config & ~31u); return 1; }
+    if (batch == 0) return 0;
+    if (!y || !ref_base || !alt_offsets || !calls || !text || !ad || (n_alt_bytes > 0 && !alt_bytes)) {
+        c3b_set_error("c3b_decode_calls: null buffer");
+        return 1;
+    }
+    if (batch > INT32_MAX || n_alt_bytes > ((int64_t)1 << 40)) { c3b_set_error("c3b_decode_calls: batch or alt_info too large"); return 1; }
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    C3B_CUDA(cudaSetDevice(m->device));
+    const size_t B = (size_t)batch, NB = (size_t)n_alt_bytes, pool = 2 * NB + 8 * B;
+    auto up = [](size_t v) { return (v + 255) / 256 * 256; };
+    const size_t scratch = up(c3b_calls_scratch_bytes(batch, m->out_dim, k, n_alt_bytes));
+    Workspace *w = get_workspace(m, s);
+    if (!w) return 1;
+    if (on_device) {
+        if (w->dev_aux_bytes < scratch) C3B_CUDA(cudaStreamSynchronize(s));
+        if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, scratch)) return 1;
+        m->launches++;
+        return c3b_launch_decode_calls(y, ref_base, batch, m->out_dim, alt_bytes, alt_offsets, n_alt_bytes, config, max_infer_len, k,
+                                       calls, text, ad, w->dev_aux, s);
+    }
+    if (alt_offsets[0] < 0) { c3b_set_error("c3b_decode_calls: alt_offsets[0] < 0"); return 1; }
+    for (int64_t i = 0; i < batch; ++i)
+        if (alt_offsets[i + 1] < alt_offsets[i] || alt_offsets[i + 1] > n_alt_bytes) {
+            c3b_set_error("c3b_decode_calls: alt_offsets must be non-decreasing within [0, n_alt_bytes] (site %lld)", (long long)i);
+            return 1;
+        }
+    // host buffers: stage through the stream's workspace after the scratch [y | offsets | ad | calls | ref_base | bytes | text]
+    size_t o_y = scratch, o_off = o_y + up(B * m->out_dim * 4), o_ad = o_off + up((B + 1) * 8), o_calls = o_ad + up(pool * 8),
+           o_ref = o_calls + up(B * sizeof(c3b_call)), o_bytes = o_ref + up(B), o_text = o_bytes + up(NB), total = o_text + up(pool);
+    if (w->dev_aux_bytes < total) C3B_CUDA(cudaStreamSynchronize(s));
+    if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, total)) return 1;
+    char *d = (char *)w->dev_aux;
+    C3B_CUDA(cudaMemcpyAsync(d + o_y, y, B * m->out_dim * 4, cudaMemcpyHostToDevice, s));
+    C3B_CUDA(cudaMemcpyAsync(d + o_off, alt_offsets, (B + 1) * 8, cudaMemcpyHostToDevice, s));
+    C3B_CUDA(cudaMemcpyAsync(d + o_ref, ref_base, B, cudaMemcpyHostToDevice, s));
+    if (NB) C3B_CUDA(cudaMemcpyAsync(d + o_bytes, alt_bytes, NB, cudaMemcpyHostToDevice, s));
+    m->launches++;
+    if (c3b_launch_decode_calls((const float *)(d + o_y), (const uint8_t *)(d + o_ref), batch, m->out_dim, d + o_bytes,
+                                (const int64_t *)(d + o_off), n_alt_bytes, config, max_infer_len, k, (c3b_call *)(d + o_calls),
+                                d + o_text, (int64_t *)(d + o_ad), d, s))
+        return 1;
+    C3B_CUDA(cudaMemcpyAsync(calls, d + o_calls, B * sizeof(c3b_call), cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaMemcpyAsync(text, d + o_text, pool, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaMemcpyAsync(ad, d + o_ad, pool * 8, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaStreamSynchronize(s));
+    return 0;
+}
+
 // ------------------------------------------------------------------------------------------------ taps (debug)
 extern "C" int c3b_get_tap(c3b_model *m, const char *name, float *host_out, int64_t *count_inout) {
     if (!m || !name || !count_inout) { c3b_set_error("c3b_get_tap: null argument"); return 1; }

@@ -251,6 +251,12 @@ int c3b_launch_decode_stage2(const float *y, const uint8_t *ref_gt21, int64_t ba
                              const int32_t *n_sites, int64_t max_sites, int k, uint8_t *cat, uint16_t *idx, float *prob,
                              uint16_t *tie_mask, int32_t *count, uint8_t *complete, cudaStream_t s);
 
+// stage 3 (c3b_decode_calls): stage 1, stage 2 and the walks on device pointers; scratch holds c3b_calls_scratch_bytes()
+size_t c3b_calls_scratch_bytes(int64_t batch, int out_dim, int k, int64_t n_alt_bytes);
+int c3b_launch_decode_calls(const float *y, const uint8_t *ref_base, int64_t batch, int out_dim, const char *alt_bytes,
+                            const int64_t *alt_offsets, int64_t n_alt_bytes, uint32_t cfg, int64_t max_infer_len, int k,
+                            c3b_call *calls, char *text, int64_t *ad, void *scratch, cudaStream_t s);
+
 // ---- kernels_fp32.cu ----
 int c3b_launch_lstm_f32(const float *x, const LstmF32 &fwd, const LstmF32 &bwd, float *out, int64_t batch, int in_dim,
                         int hidden, cudaStream_t s);

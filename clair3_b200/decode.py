@@ -281,6 +281,17 @@ def format_row(chromosome, position, read_depth, alt_info_dict, output_info, out
         return None
     if output_config.is_haploid_sensitive_mode_enabled and is_multi:
         return None
+    fields = row_fields(read_depth, alt_info_dict, output_info, output_config)
+    return row_text(chromosome, position, read_depth, probability, is_ref, fields, output_config)
+
+
+def row_fields(read_depth, alt_info_dict, output_info, output_config):
+    """The data of ``output_with``'s row for a call ``format_row`` prints: (genotype, REF, ALT, ref_count, allele counts,
+    support), REF / ALT as the row prints them.  Only for a printed call (the filters of ``format_row`` passed)."""
+    flags, (reference_base, alternate_base), probability = output_info
+    (is_ref, is_homo_snp, is_het_snp, is_homo_ins, is_het_acgt_ins, is_het_insins, is_homo_del, is_het_acgt_del,
+     is_het_deldel, is_insdel) = flags
+    is_multi = "," in str(alternate_base)
     genotype = None
     if is_ref:
         genotype = "0/0"
@@ -360,20 +371,26 @@ def format_row(chromosome, position, read_depth, alt_info_dict, output_info, out
             counts.append(n)
             support += n
 
+    if output_config.is_haploid_precise_mode_enabled or output_config.is_haploid_sensitive_mode_enabled:
+        genotype = "1" if "1" in genotype else "0"
+    if not output_config.keep_iupac_bases:
+        reference_base = convert_iupac_to_n(reference_base)
+        alternate_base = convert_iupac_to_n(alternate_base)
+    return genotype, reference_base, alternate_base, ref_count, counts, support
+
+
+def row_text(chromosome, position, read_depth, probability, is_ref, fields, output_config):
+    """The VCF row of a printed call from its ``row_fields``: QUAL, FILTER and AF are computed here."""
+    genotype, reference_base, alternate_base, ref_count, counts, support = fields
     af = ((support + 0.0) / read_depth) if read_depth != 0 else 0.0
     af = 1 if af > 1 else af
     qual = quality_score_from(probability)
-    if output_config.is_haploid_precise_mode_enabled or output_config.is_haploid_sensitive_mode_enabled:
-        genotype = "1" if "1" in genotype else "0"
     if is_ref:
         filt = "RefCall"
     elif output_config.quality_score_for_pass is None or qual >= output_config.quality_score_for_pass:
         filt = "PASS"
     else:
         filt = "LowQual"
-    if not output_config.keep_iupac_bases:
-        reference_base = convert_iupac_to_n(reference_base)
-        alternate_base = convert_iupac_to_n(alternate_base)
     ad = str(ref_count) + ("," + ",".join(str(c) for c in counts) if counts else "")
     af_s = "%.4f" % af if len(counts) <= 1 else ",".join("%.4f" % min(1.0, 1.0 * c / read_depth) for c in counts)
     return "%s\t%d\t.\t%s\t%s\t%.2f\t%s\t%s\tGT:GQ:DP:AD:AF\t%s:%d:%d:%s:%s\n" % (
@@ -401,7 +418,8 @@ def _numpy(d):
 
 def batch_output(model, batch_chr_pos_seq, alt_info_list, Y, output_config, k=16):
     """The reference's ``batch_output`` (CallVariants.py:1069-1116) for one batch: returns the VCF rows as one string.
-    ``model`` provides ``decode_stage1`` / ``decode_stage2`` (a ``Clair3_P`` / ``Clair3_F``); ``Y`` float32 [B, 24|90];
+    ``model`` provides ``decode_calls`` (a ``Clair3_P`` / ``Clair3_F``: the walk runs on the GPU, ``batch_calls``) or only
+    ``decode_stage1`` / ``decode_stage2`` (the walk runs here, ``output_from_ranked``); ``Y`` float32 [B, 24|90];
     ``output_config`` any object with the reference's ``OutputConfig`` field names."""
     _check_config(output_config)
     Y = np.ascontiguousarray(np.asarray(Y.cpu() if hasattr(Y, "cpu") else Y, dtype=np.float32))
@@ -410,6 +428,8 @@ def batch_output(model, batch_chr_pos_seq, alt_info_list, Y, output_config, k=16
         raise ValueError("Inconsistent shape between input tensor and output predictions %d/%d" % (B, len(Y)))
     if B == 0:
         return ""
+    if hasattr(model, "decode_calls"):
+        return calls_text(batch_calls(model, batch_chr_pos_seq, alt_info_list, Y, output_config, k=k), output_config)
     add_indel_length = bool(output_config.add_indel_length)
     if Y.shape[1] != (90 if add_indel_length else 24):
         raise ValueError("Y has %d columns but add_indel_length=%s" % (Y.shape[1], add_indel_length))
@@ -449,4 +469,73 @@ def batch_output(model, batch_chr_pos_seq, alt_info_list, Y, output_config, k=16
         row = format_row(chromosome, position, depth, alt, info, output_config)
         if row is not None:
             rows.append(row)
+    return "".join(rows)
+
+
+# ------------------------------------------------------------------------------------------------ calls as data
+GENOTYPES = {0: "0/0", 1: "0/1", 2: "1/1", 3: "1/2", 4: "0", 5: "1", 255: None}
+_STATUS_ERRORS = {1: ValueError, 2: IndexError, 3: TypeError, 4: ValueError, 5: ValueError}
+_STATUS_TEXT = {1: "alt_info does not parse as 'depth-KEY count ...' (int() raises)",
+                2: "alt_info holds an empty or a bare 'X' key, which output_from / output_with index",
+                3: "the row takes len() of a missing deletion (enable_long_indel with a one-base REF under a deletion flag)",
+                4: "alt_info holds a non-ASCII byte or a count beyond +-2**62",
+                5: "bad alt_info offsets or reference base"}
+
+
+def _as_bytes(s):
+    if isinstance(s, np.ndarray):
+        s = s.reshape(-1)[0]
+    if isinstance(s, (bytes, np.bytes_)):
+        return bytes(s)
+    return str(s).encode()
+
+
+def batch_calls(model, batch_chr_pos_seq, alt_info_list, Y, output_config, k=16):
+    """Every site's call as arrays (``model.decode_calls``: the walk, the re-rank and the row's counts on the GPU).  Returns a
+    dict: ``chromosome`` (list of str), ``position`` int64 [B], ``calls`` (``model.CALL_DTYPE`` records [B]: probability,
+    flags, genotype code (``GENOTYPES``), printed, DP, AD's ref count, AF support, REF / ALT lengths, allele-count count),
+    ``text`` / ``ad`` (the pools) and ``start`` int64 [B] (site s's REF, then ALT, at ``text[start[s]:]``, its allele counts
+    at ``ad[start[s]:]``).  Raises what ``batch_output``'s host walk raises on an alt_info string it cannot decode."""
+    from .model import CALL_DTYPE
+    _check_config(output_config)
+    Y = np.ascontiguousarray(np.asarray(Y.cpu() if hasattr(Y, "cpu") else Y, dtype=np.float32))
+    B = len(batch_chr_pos_seq)
+    if len(Y) != B:
+        raise ValueError("Inconsistent shape between input tensor and output predictions %d/%d" % (B, len(Y)))
+    if Y.shape[1] != (90 if output_config.add_indel_length else 24):
+        raise ValueError("Y has %d columns but add_indel_length=%s" % (Y.shape[1], bool(output_config.add_indel_length)))
+    chromosomes, positions, ref_base = [], np.zeros(B, np.int64), np.zeros(B, np.uint8)
+    for i, chr_pos_seq in enumerate(batch_chr_pos_seq):
+        chromosome, position, seq = parse_chr_pos_seq(chr_pos_seq)
+        base = seq[FLANKING_BASE_NUM if len(seq) > 1 else 0]
+        BASE2ACGT[base]                                  # the host path's KeyError on a base outside the IUPAC table
+        chromosomes.append(chromosome)
+        positions[i] = position
+        ref_base[i] = ord(base)
+    alts = [_as_bytes(a) for a in alt_info_list]
+    offsets = np.zeros(B + 1, np.int64)
+    np.cumsum([len(a) for a in alts], out=offsets[1:])
+    alt_bytes = np.frombuffer(bytearray(b"".join(alts)), dtype=np.uint8)
+    out = _numpy(model.decode_calls(Y, ref_base, alt_bytes, offsets, output_config, k=k))
+    calls = out["calls"].view(CALL_DTYPE).reshape(B)
+    status = calls["status"]
+    if status.any():
+        early = np.isin(status, (1, 4, 5))                      # what the host path rejects before it decodes any site
+        s = int(np.argmax(early)) if early.any() else int(np.argmax(status != 0))
+        raise _STATUS_ERRORS[int(status[s])]("site %d (%s:%d): %s" % (s, chromosomes[s], positions[s], _STATUS_TEXT[int(status[s])]))
+    return {"chromosome": chromosomes, "position": positions, "calls": calls, "text": out["text"], "ad": out["ad"],
+            "start": 2 * offsets[:-1] + 8 * np.arange(B, dtype=np.int64)}
+
+
+def calls_text(res, output_config):
+    """The VCF rows of ``batch_calls``' printed calls (QUAL, FILTER and AF formatted here)."""
+    calls, text, ad, start = res["calls"], res["text"], res["ad"], res["start"]
+    rows = []
+    for s in np.nonzero(calls["printed"])[0]:
+        c = calls[s]
+        o, rl, al, na = int(start[s]), int(c["ref_len"]), int(c["alt_len"]), int(c["n_ad"])
+        fields = (GENOTYPES[int(c["genotype"])], text[o:o + rl].tobytes().decode(), text[o + rl:o + rl + al].tobytes().decode(),
+                  int(c["ref_count"]), [int(v) for v in ad[o:o + na]], int(c["support"]))
+        rows.append(row_text(res["chromosome"][s], int(res["position"][s]), int(c["dp"]), c["prob"], bool(c["flags"] & 1), fields,
+                             output_config))
     return "".join(rows)

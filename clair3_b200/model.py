@@ -20,6 +20,26 @@ from ._ffi import C3BError, check, ffi, lib
 
 _DT = {torch.int8: K["C3B_DT_I8"], torch.int32: K["C3B_DT_I32"], torch.float32: K["C3B_DT_F32"]}
 
+# c3b_call (include/clair3_b200.h) as a numpy record
+CALL_DTYPE = np.dtype([("dp", "<i8"), ("support", "<i8"), ("ref_count", "<i8"), ("prob", "<f4"), ("ref_len", "<i4"),
+                       ("alt_len", "<i4"), ("n_ad", "<i4"), ("flags", "<u2"), ("genotype", "u1"), ("printed", "u1"),
+                       ("status", "u1"), ("pad", "u1", (3,))])
+assert CALL_DTYPE.itemsize == ffi.sizeof("c3b_call")
+
+
+def call_config(output_config):
+    """(C3B_CALL_* bits, maximum_variant_length_that_need_infer) of an object with the reference's OutputConfig fields."""
+    bits = 0
+    for name, bit in (("is_show_reference", "C3B_CALL_SHOW_REF"), ("is_haploid_precise_mode_enabled", "C3B_CALL_HAPLOID_PRECISE"),
+                      ("is_haploid_sensitive_mode_enabled", "C3B_CALL_HAPLOID_SENSITIVE"),
+                      ("enable_long_indel", "C3B_CALL_LONG_INDEL"), ("keep_iupac_bases", "C3B_CALL_KEEP_IUPAC")):
+        if getattr(output_config, name):
+            bits |= K[bit]
+    max_len = output_config.maximum_variant_length_that_need_infer
+    if isinstance(max_len, bool) or not isinstance(max_len, (int, np.integer)):
+        raise C3BError("maximum_variant_length_that_need_infer must be an integer, got %r" % (max_len,))
+    return bits, int(np.clip(int(max_len), -(1 << 62), 1 << 62))
+
 
 class _C3BModule:
     _kind = None
@@ -314,6 +334,49 @@ class _C3BModule:
                                       c("float *", out["prob"].data_ptr()), c("uint16_t *", out["tie_mask"].data_ptr()),
                                       c("int32_t *", out["count"].data_ptr()), c("uint8_t *", out["complete"].data_ptr()),
                                       c("void *", stream)))
+        return out
+
+    def decode_calls(self, y, ref_base, alt_bytes, alt_offsets, config, k=16):
+        """``c3b_decode_calls``: every site's call as data - stage 1, stage 2 (first ``k`` entries), the walk of each
+        non-reference site's ranked outcomes against its alt_info, the full re-rank of the sites whose k entries run out, and
+        what ``output_with`` reads for the row (``clair3_b200.decode.format_row`` without the QUAL, FILTER and AF text).
+        ``y`` float32 [B, out_dim]; ``ref_base`` uint8 [B] the raw reference character at each window's centre;
+        ``alt_bytes`` uint8 [N] the alt_info strings concatenated, site s at ``alt_bytes[alt_offsets[s]:alt_offsets[s + 1]]``
+        (``alt_offsets`` int64 [B + 1]); all on y's device (cuda: asynchronous on the current stream; cpu: complete on
+        return).  ``config``: an object with the reference's ``OutputConfig`` field names.  Returns a dict of tensors:
+        ``calls`` uint8 [B, 48] (``CALL_DTYPE`` records), ``text`` uint8 and ``ad`` int64, both [2 N + 8 B] (site s's REF,
+        ALT and allele counts from index ``2 * alt_offsets[s] + 8 * s``)."""
+        if self._handle is None:
+            raise C3BError("model has no device yet")
+        t = lambda a: torch.from_numpy(np.ascontiguousarray(a)) if isinstance(a, np.ndarray) else a      # noqa: E731
+        y, ref_base, alt_bytes, alt_offsets = t(y), t(ref_base), t(alt_bytes), t(alt_offsets)
+        if y.ndim != 2 or y.shape[1] != self.out_dim or y.dtype != torch.float32:
+            raise C3BError("decode_calls: y must be float32 [B, %d]" % self.out_dim)
+        B, dev = y.shape[0], y.device
+        if ref_base.shape != (B,) or ref_base.dtype != torch.uint8 or ref_base.device != dev:
+            raise C3BError("decode_calls: ref_base must be uint8 [B] on y's device")
+        if alt_bytes.ndim != 1 or alt_bytes.dtype != torch.uint8 or alt_bytes.device != dev:
+            raise C3BError("decode_calls: alt_bytes must be a 1-D uint8 tensor on y's device")
+        if alt_offsets.shape != (B + 1,) or alt_offsets.dtype != torch.int64 or alt_offsets.device != dev:
+            raise C3BError("decode_calls: alt_offsets must be int64 [B + 1] on y's device")
+        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= int(k) <= 1024:
+            raise C3BError("decode_calls: k must be an integer in [1, 1024], got %r" % (k,))
+        if bool(config.add_indel_length) != self.add_indel_length:
+            raise C3BError("decode_calls: config.add_indel_length must match the model")
+        bits, max_len = call_config(config)
+        y, ref_base, alt_bytes, alt_offsets = y.contiguous(), ref_base.contiguous(), alt_bytes.contiguous(), alt_offsets.contiguous()
+        N = alt_bytes.shape[0]
+        out = {"calls": torch.zeros((B, CALL_DTYPE.itemsize), dtype=torch.uint8, device=dev),
+               "text": torch.zeros(2 * N + 8 * B, dtype=torch.uint8, device=dev),
+               "ad": torch.zeros(2 * N + 8 * B, dtype=torch.int64, device=dev)}
+        if B == 0:
+            return out
+        stream = torch.cuda.current_stream(self._device).cuda_stream
+        c = ffi.cast
+        check(lib().c3b_decode_calls(self._handle, c("float *", y.data_ptr()), c("uint8_t *", ref_base.data_ptr()), B,
+                                     c("char *", alt_bytes.data_ptr()), c("int64_t *", alt_offsets.data_ptr()), N, bits, max_len,
+                                     int(k), int(dev.type == "cuda"), c("c3b_call *", out["calls"].data_ptr()),
+                                     c("char *", out["text"].data_ptr()), c("int64_t *", out["ad"].data_ptr()), c("void *", stream)))
         return out
 
     def predict_stream(self, batches, streams=8):

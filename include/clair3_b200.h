@@ -147,6 +147,54 @@ int c3b_decode_stage2(c3b_model *m, const float *y, const uint8_t *ref_gt21, int
                       const int32_t *n_sites, int64_t max_sites, int k, int on_device, uint8_t *cat, uint16_t *idx,
                       float *prob, uint16_t *tie_mask, int32_t *count, uint8_t *complete, void *cuda_stream);
 
+/* Third stage of the decoder: each site's call as data.  Runs stage 1 and stage 2 (k entries), walks every non-reference
+ * site's ranked outcomes against its alt_info (decode.py's output_from_ranked / _try_outcome), re-ranks the sites whose k
+ * entries run out with the full list (804 or 24) and walks them again, then computes what output_with's row reads
+ * (format_row without the QUAL, FILTER and AF text).  All of it stream-ordered, with no host synchronisation inside.
+ *   y          [batch, out_dim] probabilities
+ *   ref_base   [batch] the raw reference character at the window centre (seq[center]; IUPAC allowed)
+ *   alt_bytes  the alt_info strings ("depth-KEY count KEY count ..."), concatenated; site s is
+ *              alt_bytes[alt_offsets[s] .. alt_offsets[s+1]) with 0 <= alt_offsets[s] <= alt_offsets[s+1] <= n_alt_bytes
+ *   config     C3B_CALL_* bits; max_infer_len: maximum_variant_length_that_need_infer      k: stage 2's first pass, 1 .. 1024
+ *   calls      [batch] records (below)
+ *   text       [2 * n_alt_bytes + 8 * batch] bytes: site s owns the region from 2 * alt_offsets[s] + 8 * s; REF (ref_len bytes)
+ *              then ALT (alt_len bytes) as the VCF row prints them ('.' for a reference call; IUPAC -> N unless
+ *              C3B_CALL_KEEP_IUPAC)
+ *   ad         [2 * n_alt_bytes + 8 * batch] int64: site s's n_ad allele counts (AD after its first entry, ref_count) start
+ *              at the same index as its text region
+ * on_device: every pointer is a device pointer and the call is asynchronous on cuda_stream; else host pointers (checked
+ * before the launch), complete on return.  A site whose alt_info the host decoder would reject has status != 0 and no
+ * meaningful fields. */
+#define C3B_CALL_SHOW_REF           1
+#define C3B_CALL_HAPLOID_PRECISE    2
+#define C3B_CALL_HAPLOID_SENSITIVE  4
+#define C3B_CALL_LONG_INDEL         8
+#define C3B_CALL_KEEP_IUPAC         16
+
+/* status: 0 ok; 1 alt_info does not parse (int() would raise ValueError); 2 the walk or the printed row indexes an empty key
+ * or a bare "X" key (IndexError); 3 the printed row takes len() of a missing deletion (TypeError: enable_long_indel with a
+ * one-base REF under a deletion flag); 4 unsupported: a non-ASCII byte or a count outside +-2^62; 5 bad offsets or a
+ * reference base outside ACGTURYSWKMBDHVN.
+ * genotype: 0 "0/0", 1 "0/1", 2 "1/1", 3 "1/2", 4 "0", 5 "1" (haploid modes), 255 none. */
+typedef struct {
+    int64_t dp;          /* read depth: alt_info's number before the first '-' */
+    int64_t support;     /* the reads AF is computed from: AF = min(support / dp, 1), 0 when dp == 0 */
+    int64_t ref_count;   /* AD's first entry: the 'R' count, at least 0 */
+    float prob;          /* the QUAL input: stage 1's ref_prob for an early-out site, else the successful entry's probability */
+    int32_t ref_len;     /* bytes of REF in text */
+    int32_t alt_len;     /* bytes of ALT in text, right after REF */
+    int32_t n_ad;        /* allele counts in ad (usually 0..2; a row whose flags tie across categories can have more) */
+    uint16_t flags;      /* bit c: is_* flag c in output_from's order (0 homo_Ref .. 9 hetero_InsDel) */
+    uint8_t genotype;
+    uint8_t printed;     /* 1: output_with prints a row for this call (showRef, REF != ALT, both haploid modes) */
+    uint8_t status;
+    uint8_t pad[3];
+} c3b_call;
+
+int c3b_decode_calls(c3b_model *m, const float *y, const uint8_t *ref_base, int64_t batch, const char *alt_bytes,
+                     const int64_t *alt_offsets, int64_t n_alt_bytes, uint32_t config, int64_t max_infer_len, int k, int on_device,
+                     c3b_call *calls, char *text, int64_t *ad, void *cuda_stream);
+
 /* Packed device weight images (what one rank broadcasts to the others at start-up; SURVEY.md 8e).
  * which: 0 = fp16 tensor-core operand images + fp32 head weights, 1 = fp32 debug-path weights. */
 int c3b_weight_blob(c3b_model *m, int which, void **device_ptr, size_t *bytes);

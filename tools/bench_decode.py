@@ -7,8 +7,12 @@ With a GPU it prints one JSON line per measurement:
 
 * ``device``: device time of stage 1 + stage 2 (k = 16, chained on ``nonref_idx`` / ``n_nonref``) per 256-site Clair3_F batch
   (90 outputs) and per 1024-site Clair3_P batch (24 outputs), from CUDA events around ``--iters`` back-to-back batches;
-* ``host``: wall time of ``decode.batch_output`` per non-reference site on seeded rows and alt_info strings, split into the
-  time spent in the two stage calls (host pointers: copies and synchronisation included) and the host walk + formatting.
+* ``device_calls``: device time per batch of each kernel ``c3b_decode_calls`` launches (device pointers, k = 16);
+* ``host``, ``route: host_walk``: wall time of ``decode.batch_output`` with only the two stages (the host walk) per
+  non-reference site on seeded rows and alt_info strings, split into the time spent in the two stage calls (host pointers:
+  copies and synchronisation included) and the host walk + formatting;
+* ``host``, ``route: device_calls``: the same rows through ``decode.batch_output``'s records route (``c3b_decode_calls`` on host
+  pointers, then ``calls_text``), and the part of it spent formatting the rows.
 
 ``--reference`` (no GPU needed; reads the reference named by ``CLAIR3_REFERENCE``) times the reference's own ``batch_output``
 on the same rows, and the host walk of ``decode.batch_output`` with the numpy oracle standing in for the GPU stages, both per
@@ -99,6 +103,32 @@ def host_cost(m, out_dim, sites, batch, seed=5):
             "stage_calls_us_per_nonref_site": 1e6 * tm.t / nonref, "walk_us_per_nonref_site": 1e6 * (total - tm.t) / nonref}
 
 
+def calls_cost(m, out_dim, sites, batch, nonref, seed=5):
+    """decode.batch_output through the records route (decode.batch_calls + calls_text) on the same rows, per non-reference
+    site: the whole call, and the part spent formatting the printed rows."""
+    y, pos, alts = rows(sites, out_dim, seed)
+    cfg = decode.replay_config(pileup=out_dim == 24, add_indel_length=out_dim == 90)
+    decode.batch_output(m, pos[:batch], alts[:batch], y[:batch], cfg)        # warm-up
+    t_fmt = 0.0
+    t0 = time.perf_counter()
+    for s in range(0, sites, batch):
+        res = decode.batch_calls(m, pos[s:s + batch], alts[s:s + batch], y[s:s + batch], cfg)
+        t1 = time.perf_counter()
+        decode.calls_text(res, cfg)
+        t_fmt += time.perf_counter() - t1
+    total = time.perf_counter() - t0
+    return {"sites": sites, "nonref_sites": nonref, "us_per_nonref_site": 1e6 * total / nonref,
+            "row_format_us_per_nonref_site": 1e6 * t_fmt / nonref}
+
+
+def card():
+    """The GPU's name and power limit, as nvidia-smi reports them when the bench runs (part of every number)."""
+    import subprocess
+    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                         capture_output=True, text=True).stdout.strip().split(", ")
+    return {"device": out[0], "power_limit_w": float(out[1])} if len(out) == 2 else {"device": "unknown", "power_limit_w": None}
+
+
 def gpu(args):
     import torch
 
@@ -110,6 +140,7 @@ def gpu(args):
     p = Clair3_P(add_indel_length=False, predict=True, input_channels=18)
     p.to(torch.device("cuda"))
     p.load_state_dict({k: torch.from_numpy(np.asarray(v)) for k, v in synth.pileup_state_dict(False, seed=1).items()})
+    gpu_card = card()
     for name, m, out_dim, batch in (("Clair3_F", f, 90, 256), ("Clair3_P", p, 24, 1024)):
         y, pos, _ = rows(batch, out_dim, seed=out_dim)
         yd = torch.from_numpy(y).cuda()
@@ -140,11 +171,34 @@ def gpu(args):
                 kern["stage1" if "stage1" in ev.key else "stage2"] = ev.device_time_total / args.iters
         print(json.dumps({"measure": "device", "model": name, "out_dim": out_dim, "batch_sites": batch, "k": 16,
                           "us_per_batch_stage1_plus_stage2": round(us, 2),
-                          "kernel_us_per_batch": {k: round(v, 2) for k, v in sorted(kern.items())}, "iters": args.iters,
-                          "device": torch.cuda.get_device_name()}), flush=True)
+                          "kernel_us_per_batch": {k: round(v, 2) for k, v in sorted(kern.items())}, "iters": args.iters, **gpu_card}), flush=True)
+        # stage 3 (c3b_decode_calls: stages 1 and 2, the walk, the full re-rank and the row counts), device pointers
+        ab = [a.encode() for a in rows(batch, out_dim, seed=out_dim)[2]]
+        off = np.zeros(batch + 1, np.int64)
+        np.cumsum([len(a) for a in ab], out=off[1:])
+        abd, offd = torch.from_numpy(np.frombuffer(b"".join(ab), np.uint8).copy()).cuda(), torch.from_numpy(off).cuda()
+        rbd = torch.from_numpy(np.array([ord(s[-17]) for s in pos], np.uint8)).cuda()
+        cfg = decode.replay_config(pileup=out_dim == 24, add_indel_length=out_dim == 90)
+        for _ in range(5):
+            m.decode_calls(yd, rbd, abd, offd, cfg)
+        torch.cuda.synchronize()
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.iters):
+                m.decode_calls(yd, rbd, abd, offd, cfg)
+            torch.cuda.synchronize()
+        calls_kern = {}
+        for ev in prof.key_averages():
+            if "decode" in ev.key or "calls_" in ev.key:
+                key = next(n for n in ("decode_calls_kernel", "calls_compact", "calls_gt21", "stage1", "stage2") if n in ev.key)
+                calls_kern[key] = calls_kern.get(key, 0.0) + ev.device_time_total / args.iters
+        print(json.dumps({"measure": "device_calls", "model": name, "out_dim": out_dim, "batch_sites": batch, "k": 16,
+                          "kernel_us_per_batch": {k: round(v, 2) for k, v in sorted(calls_kern.items())}, "iters": args.iters, **gpu_card}), flush=True)
         res = host_cost(m, out_dim, args.sites, batch)
-        print(json.dumps({"measure": "host", "model": name, "out_dim": out_dim, "batch_sites": batch,
-                          **{k: (round(v, 2) if isinstance(v, float) else v) for k, v in res.items()}}), flush=True)
+        print(json.dumps({"measure": "host", "route": "host_walk", "model": name, "out_dim": out_dim, "batch_sites": batch,
+                          **{k: (round(v, 2) if isinstance(v, float) else v) for k, v in res.items()}, **gpu_card}), flush=True)
+        res = calls_cost(m, out_dim, args.sites, batch, res["nonref_sites"])
+        print(json.dumps({"measure": "host", "route": "device_calls", "model": name, "out_dim": out_dim, "batch_sites": batch,
+                          **{k: (round(v, 2) if isinstance(v, float) else v) for k, v in res.items()}, **gpu_card}), flush=True)
 
 
 def reference(args):
