@@ -64,6 +64,34 @@ float c3b_op2f(uint16_t h) {
     return f;
 }
 
+int c3b_use_device(int ordinal, int unsupported, int *sm_count) {
+    int ndev = 0;
+    const cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || ndev == 0) {
+        c3b_set_error("no CUDA device: %s (clair3_b200 has no CPU fallback)", cudaGetErrorString(e));
+        return unsupported;
+    }
+    if (ordinal < 0 || ordinal >= ndev) { c3b_set_error("bad device ordinal %d", ordinal); return 1; }
+    cudaDeviceProp prop;
+    C3B_CUDA(cudaGetDeviceProperties(&prop, ordinal));
+    if (prop.major != 9 || prop.minor != 0) {
+        c3b_set_error("device %d is sm_%d%d; this library contains only sm_90a code", ordinal, prop.major, prop.minor);
+        return unsupported;
+    }
+    C3B_CUDA(cudaSetDevice(ordinal));
+    if (sm_count) *sm_count = prop.multiProcessorCount;
+    return 0;
+}
+
+int c3b_last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s, int64_t *last) {
+    *last = 0;
+    if (!off) return 0;
+    if (!on_device) { *last = off[n]; return 0; }
+    C3B_CUDA(cudaMemcpyAsync(last, off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaStreamSynchronize(s));
+    return 0;
+}
+
 namespace {
 
 struct Blob {
@@ -170,20 +198,8 @@ extern "C" int c3b_create(c3b_model **out, int kind, int channels, int add_indel
         return 1;
     }
     if (kind == C3B_FULL_ALIGNMENT && (channels < 1 || channels > 16)) { c3b_set_error("full-alignment channels must be in [1,16], got %d", channels); return 1; }
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0) {
-        c3b_set_error("no CUDA device: %s (clair3_b200 has no CPU fallback)", cudaGetErrorString(e));
-        return 2;
-    }
-    if (device_ordinal < 0 || device_ordinal >= ndev) { c3b_set_error("bad device ordinal %d", device_ordinal); return 1; }
-    cudaDeviceProp prop;
-    C3B_CUDA(cudaGetDeviceProperties(&prop, device_ordinal));
-    if (prop.major != 9 || prop.minor != 0) {
-        c3b_set_error("device %d is sm_%d%d; this library contains only sm_90a code", device_ordinal, prop.major, prop.minor);
-        return 2;
-    }
-    C3B_CUDA(cudaSetDevice(device_ordinal));
+    int sm_count = 0;
+    if (int rc = c3b_use_device(device_ordinal, 2, &sm_count)) return rc;
     c3b_model *m = new c3b_model();
     m->kind = kind;
     m->channels = channels;
@@ -193,7 +209,7 @@ extern "C" int c3b_create(c3b_model **out, int kind, int channels, int add_indel
     m->out_dim = add_indel_length ? 90 : 24;
     m->d4 = kind == C3B_PILEUP ? 128 : 256;
     m->l4_in = kind == C3B_PILEUP ? 2 * C3B_H2 * C3B_T : 3584;
-    m->sm_count = prop.multiProcessorCount;
+    m->sm_count = sm_count;
     build_expected(m);
     *out = m;
     return 0;
@@ -460,15 +476,12 @@ static int finalize_impl(c3b_model *m) {
         }
     }
 
-    if (m->blob) { cudaFree(m->blob); m->blob = nullptr; }
-    if (m->f32blob) { cudaFree(m->f32blob); m->f32blob = nullptr; }
-    m->blob_bytes = (blob.data.size() + 255) / 256 * 256;
-    m->f32blob_bytes = (fb.data.size() + 255) / 256 * 256;
-    C3B_CUDA(cudaMalloc(&m->blob, m->blob_bytes));
-    C3B_CUDA(cudaMalloc(&m->f32blob, m->f32blob_bytes));
-    C3B_CUDA(cudaMemcpy(m->blob, blob.data.data(), blob.data.size(), cudaMemcpyHostToDevice));
-    C3B_CUDA(cudaMemcpy(m->f32blob, fb.data.data(), fb.data.size(), cudaMemcpyHostToDevice));
-    for (const Fix &f : fixes) *f.dst = (f.f32blob ? m->f32blob : m->blob) + f.off;
+    if (m->blob.ensure((blob.data.size() + 255) / 256 * 256, nullptr, "c3b_finalize") ||
+        m->f32blob.ensure((fb.data.size() + 255) / 256 * 256, nullptr, "c3b_finalize"))
+        return 1;
+    C3B_CUDA(cudaMemcpy(m->blob.p, blob.data.data(), blob.data.size(), cudaMemcpyHostToDevice));
+    C3B_CUDA(cudaMemcpy(m->f32blob.p, fb.data.data(), fb.data.size(), cudaMemcpyHostToDevice));
+    for (const Fix &f : fixes) *f.dst = (f.f32blob ? m->f32blob : m->blob).as<char>() + f.off;
     m->lstm_tc[0][1] = m->lstm_tc[0][0];
     m->lstm_tc[1][1] = m->lstm_tc[1][0];
     m->finalized = true;
@@ -488,8 +501,9 @@ extern "C" int c3b_finalize(c3b_model *m) {
 extern "C" int c3b_weight_blob(c3b_model *m, int which, void **device_ptr, size_t *bytes) {
     if (!m || !m->finalized) { c3b_set_error("c3b_weight_blob: model not finalized"); return 1; }
     if (which != 0 && which != 1) { c3b_set_error("c3b_weight_blob: image %d (0 = tensor-core operands + heads, 1 = fp32 debug weights)", which); return 1; }
-    if (device_ptr) *device_ptr = which ? m->f32blob : m->blob;
-    if (bytes) *bytes = which ? m->f32blob_bytes : m->blob_bytes;
+    const C3bBuf &b = which ? m->f32blob : m->blob;
+    if (device_ptr) *device_ptr = b.p;
+    if (bytes) *bytes = b.cap;
     return 0;
 }
 
@@ -510,8 +524,8 @@ extern "C" int c3b_bcast_weights(c3b_model *m, void *nccl_comm, int root, void *
     C3B_CUDA(cudaSetDevice(m->device));
     // both packed images travel: the tensor-core operands / head weights and the fp32 debug weights, so every option keeps
     // working on the receiving ranks
-    int rc = fn(m->blob, m->blob, m->blob_bytes, /*ncclUint8*/ 1, root, nccl_comm, (cudaStream_t)cuda_stream);
-    if (rc == 0) rc = fn(m->f32blob, m->f32blob, m->f32blob_bytes, /*ncclUint8*/ 1, root, nccl_comm, (cudaStream_t)cuda_stream);
+    int rc = fn(m->blob.p, m->blob.p, m->blob.cap, /*ncclUint8*/ 1, root, nccl_comm, (cudaStream_t)cuda_stream);
+    if (rc == 0) rc = fn(m->f32blob.p, m->f32blob.p, m->f32blob.cap, /*ncclUint8*/ 1, root, nccl_comm, (cudaStream_t)cuda_stream);
     if (rc != 0) { c3b_set_error("ncclBroadcast failed with %d", rc); return 1; }
     m->weights_by_broadcast = true;
     return 0;
@@ -521,44 +535,6 @@ extern "C" int c3b_bcast_weights(c3b_model *m, void *nccl_comm, int root, void *
 static int64_t round128(int64_t b) { return (b + 127) / 128 * 128; }
 static int conv_out(int v) { return (v - 1) / 2 + 1; }   // 3x3, stride 2, pad 1
 
-static size_t ws_bytes_needed(const c3b_model *m, int64_t sites, int depth) {
-    const int64_t bp = round128(sites);
-    size_t total = 0;
-    auto al = [&](size_t b) { total += (b + 255) / 256 * 256; };
-    if (m->kind == C3B_PILEUP) {
-        if (m->precision == C3B_PREC_FP32) {
-            al((size_t)sites * C3B_T * m->channels * 4);
-            al((size_t)sites * C3B_T * 256 * 4);
-            al((size_t)sites * C3B_T * 320 * 4);
-        } else {
-            al((size_t)C3B_T * bp * C3B_X1_COLS * 2);
-            al((size_t)C3B_T * bp * 256 * 2);
-            al((size_t)C3B_T * bp * 1280 * 2);
-            al((size_t)bp * C3B_T * 320 * 2);
-        }
-        al((size_t)16 * bp * 128 * 4);
-    } else {
-        const int h1 = conv_out(depth), w1 = conv_out(33), h2 = conv_out(h1), w2 = conv_out(w1), h3 = conv_out(h2), w3 = conv_out(w2);
-        if (m->precision == C3B_PREC_FP32) {
-            al((size_t)sites * depth * 33 * m->channels * 4);
-            for (int i = 0; i < 3; ++i) al((size_t)sites * h1 * w1 * 64 * 4);
-            for (int i = 0; i < 3; ++i) al((size_t)sites * h2 * w2 * 128 * 4);
-            for (int i = 0; i < 3; ++i) al((size_t)sites * h3 * w3 * 256 * 4);
-            al((size_t)bp * 3584 * 4);
-        } else {
-            const int hh[3] = {h1, h2, h3}, ww[3] = {w1, w2, w3}, cc[3] = {64, 128, 256}, sc[3] = {16, 64, 128};
-            for (int l = 0; l < 3; ++l) {
-                const PlanarGeom g = c3b_planar_geom(sites, hh[l], ww[l]);
-                al((size_t)4 * (sc[l] / 8) * g.p * 16);                              // parity planes feeding the stem conv
-                for (int i = 0; i < (l == 2 ? 3 : 2); ++i) al((size_t)(cc[l] / 8) * g.p * 16);
-            }
-            al((size_t)bp * 3584 * 2);
-        }
-        al((size_t)16 * bp * 256 * 4);
-    }
-    return total + 4096;
-}
-
 static Workspace *get_workspace(c3b_model *m, cudaStream_t stream) {
     for (Workspace *w : m->ws)
         if (w->stream == stream) return w;
@@ -567,16 +543,6 @@ static Workspace *get_workspace(c3b_model *m, cudaStream_t stream) {
     w->stream = stream;
     m->ws.push_back(w);
     return w;
-}
-
-static int ensure_dev(void **p, size_t *have, size_t need) {
-    if (*have >= need) return 0;
-    if (*p) C3B_CUDA(cudaFree(*p));
-    *p = nullptr;
-    *have = 0;
-    C3B_CUDA(cudaMalloc(p, need));
-    *have = need;
-    return 0;
 }
 
 struct Carver {
@@ -589,6 +555,141 @@ struct Carver {
         return p;
     }
 };
+
+// ------------------------------------------------------------------------------------------------ staging
+// The arguments of one call that live in host memory, staged through the stream workspace's `stage` buffer.  in() / out()
+// register an argument; a device pointer, or a null one, passes through.  upload() grows the buffer to `lead` bytes of kernel
+// scratch (at `scratch`) followed by one slot per host argument, queues the host-to-device copies of the inputs and points each
+// registered pointer at its slot.  After the launch, download() queues the device-to-host copies of the outputs and, with
+// `sync`, waits for them.  Neither touches the workspace, nor waits, when nothing is staged.
+struct Staging {
+    struct Arg {
+        void *ref;                              // the caller's pointer variable, re-pointed at the slot by point()
+        void (*point)(void *ref, char *dev);
+        const void *host;
+        size_t bytes;
+        bool out;
+        char *dev;
+    };
+    c3b_model *m;
+    cudaStream_t s;
+    const char *who;
+    size_t lead = 0;                            // a multiple of 256
+    char *scratch = nullptr;
+    std::vector<Arg> args;
+
+    template <class T> void in(T *&p, size_t bytes, bool on_device) { add(p, bytes, on_device, false); }
+    template <class T> void out(T *&p, size_t bytes, bool on_device) { add(p, bytes, on_device, true); }
+    template <class T> void add(T *&p, size_t bytes, bool on_device, bool out) {
+        if (!p || on_device) return;
+        args.push_back({&p, [](void *ref, char *dev) { *static_cast<T **>(ref) = static_cast<T *>(static_cast<void *>(dev)); }, p, bytes,
+                        out, nullptr});
+    }
+
+    int upload() {
+        if (args.empty() && !lead) return 0;
+        Workspace *w = get_workspace(m, s);
+        if (!w) return 1;
+        Carver layout{nullptr, lead};
+        for (const Arg &a : args) layout.take<char>(a.bytes);
+        if (w->stage.ensure(layout.off, s, who)) return 1;
+        scratch = w->stage.as<char>();
+        Carver cv{scratch, lead};
+        for (Arg &a : args) {
+            a.dev = cv.take<char>(a.bytes);
+            if (!a.out && a.bytes) C3B_CUDA(cudaMemcpyAsync(a.dev, a.host, a.bytes, cudaMemcpyHostToDevice, s));
+            a.point(a.ref, a.dev);
+        }
+        return 0;
+    }
+
+    int download(bool sync) {
+        if (args.empty()) return 0;
+        for (const Arg &a : args)
+            if (a.out && a.bytes) C3B_CUDA(cudaMemcpyAsync(const_cast<void *>(a.host), a.dev, a.bytes, cudaMemcpyDeviceToHost, s));
+        if (sync) {
+            C3B_CUDA(cudaStreamSynchronize(s));
+            C3B_CUDA(cudaGetLastError());
+        }
+        return 0;
+    }
+};
+
+// ------------------------------------------------------------------------------------------------ chunk layouts
+// Where a forward chunk's buffers lie in the workspace.  The same function carves them for the chunk (forward_*_chunk) and,
+// on a Carver with a null base, sizes the workspace for the largest chunk (forward_impl).
+struct PileupChunk {
+    float *xf, *l1, *l2, *z4;       // fp32 debug path
+    TcPileupBuffers tc;             // tensor-core path
+};
+
+static PileupChunk carve_pileup(const c3b_model *m, Carver &cv, int64_t n) {
+    PileupChunk c = {};
+    const int64_t bp = round128(n);
+    if (m->precision == C3B_PREC_FP32) {
+        c.xf = cv.take<float>((size_t)n * C3B_T * m->channels * 4);
+        c.l1 = cv.take<float>((size_t)n * C3B_T * 256 * 4);
+        c.l2 = cv.take<float>((size_t)n * C3B_T * 320 * 4);
+        c.z4 = cv.take<float>((size_t)bp * 128 * 4);
+    } else {
+        c.tc.xs = cv.take<op_t>((size_t)C3B_T * bp * C3B_X1_COLS * 2);
+        c.tc.h1 = cv.take<op_t>((size_t)C3B_T * bp * 256 * 2);
+        c.tc.pg = cv.take<__half>((size_t)C3B_T * bp * 1280 * 2);
+        c.tc.h2 = cv.take<op_t>((size_t)bp * C3B_T * 320 * 2);
+        c.tc.z4 = cv.take<float>((size_t)16 * bp * 128 * 4);
+        c.tc.bp = (int)bp;
+    }
+    return c;
+}
+
+// feature-map heights / widths of the full-alignment levels: [0] the input (depth x 33), [1..3] after conv1 / conv3 / conv5
+struct FaDims { int h[4], w[4]; };
+static FaDims fa_dims(int depth) {
+    FaDims d = {{depth}, {33}};
+    for (int i = 1; i < 4; ++i) { d.h[i] = conv_out(d.h[i - 1]); d.w[i] = conv_out(d.w[i - 1]); }
+    return d;
+}
+static const int kFaChans[4] = {0, 64, 128, 256};   // output channels of levels 1..3
+static const int kFaCpad = 16;                      // conv1 input channels padded to one wgmma k-step
+
+struct FaChunk {
+    // fp32 debug path
+    float *xin, *act32[3][3], *sp32;
+    // tensor-core path: planar feature maps laid out for `cap` sites, all of them in [planar_begin, planar_end)
+    PlanarGeom geo[3];
+    op_t *stem_in[3];               // parity planes feeding conv1 / conv3 / conv5: [4][cin/8][geo[l].p][8]
+    op_t *act[3][3];
+    size_t planar_begin, planar_end;
+    op_t *sp;
+    float *z4;
+};
+
+static FaChunk carve_fa(const c3b_model *m, Carver &cv, int64_t n, int depth, int64_t cap) {
+    FaChunk c = {};
+    const FaDims d = fa_dims(depth);
+    const int64_t bp = round128(n);
+    if (m->precision == C3B_PREC_FP32) {
+        c.xin = cv.take<float>((size_t)n * depth * 33 * m->channels * 4);
+        for (int l = 0; l < 3; ++l)
+            for (int i = 0; i < 3; ++i) c.act32[l][i] = cv.take<float>((size_t)n * d.h[l + 1] * d.w[l + 1] * kFaChans[l + 1] * 4);
+        c.sp32 = cv.take<float>((size_t)bp * 3584 * 4);
+        c.z4 = cv.take<float>((size_t)bp * 256 * 4);
+        return c;
+    }
+    const int stem_c[3] = {kFaCpad, 64, 128};
+    c.planar_begin = cv.off;
+    for (int l = 0; l < 3; ++l) {
+        c.geo[l] = c3b_planar_geom(n, d.h[l + 1], d.w[l + 1], cap);
+        c.stem_in[l] = cv.take<op_t>((size_t)4 * (stem_c[l] / 8) * c.geo[l].p * 16);
+        for (int i = 0; i < (l == 2 ? 3 : 2); ++i) c.act[l][i] = cv.take<op_t>((size_t)(kFaChans[l + 1] / 8) * c.geo[l].p * 16);
+    }
+    c.act[0][2] = c.stem_in[1];
+    c.act[1][2] = c.stem_in[2];
+    c.planar_end = cv.off;
+    c.sp = cv.take<op_t>((size_t)bp * 3584 * 2);
+    c.z4 = cv.take<float>((size_t)16 * bp * 256 * 4);
+    return c;
+}
 
 // ------------------------------------------------------------------------------------------------ profiling
 struct ProfScope {
@@ -663,15 +764,12 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
                                 cudaStream_t s) {
     const void *x = src.x;
     const int x_dtype = src.dtype;
-    Carver cv{w->dev};
-    const int64_t bp = round128(n);
+    Carver cv{w->dev.as<char>()};
+    const PileupChunk c = carve_pileup(m, cv, n);
     std::map<std::string, Tap> &taps = w->taps;
     tap = tap && m->taps;
     if (m->precision == C3B_PREC_FP32) {
-        float *xf = cv.take<float>((size_t)n * C3B_T * m->channels * 4);
-        float *l1 = cv.take<float>((size_t)n * C3B_T * 256 * 4);
-        float *l2 = cv.take<float>((size_t)n * C3B_T * 320 * 4);
-        float *z4 = cv.take<float>((size_t)bp * 128 * 4);
+        float *xf = c.xf, *l1 = c.l1, *l2 = c.l2, *z4 = c.z4;
         if (src.starts) {
             if (c3b_launch_gather_windows_f32(x, x_dtype, m->channels, src.starts, src.bounds, src.n_cols, xf, n, s)) return 1;
         } else if (c3b_launch_ingest_pileup_f32(x, x_dtype, xf, n * C3B_T * m->channels, s)) return 1;
@@ -687,13 +785,8 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
         }
         return 0;
     }
-    TcPileupBuffers b;
-    b.xs = cv.take<op_t>((size_t)C3B_T * bp * C3B_X1_COLS * 2);
-    b.h1 = cv.take<op_t>((size_t)C3B_T * bp * 256 * 2);
-    b.pg = cv.take<__half>((size_t)C3B_T * bp * 1280 * 2);
-    b.h2 = cv.take<op_t>((size_t)bp * C3B_T * 320 * 2);
-    b.z4 = cv.take<float>((size_t)16 * bp * 128 * 4);
-    b.bp = (int)bp;
+    const TcPileupBuffers &b = c.tc;
+    const int64_t bp = b.bp;
     // sub-tile width of lstm_tc_kernel (sites per warpgroup): 64 = fewest SM-microseconds per site, the smallest tile that still
     // fills the GPU = shortest single-batch latency.  LSTM2's weights leave room for at most 32-site sub-tiles.
     int tile1 = m->lstm_tile;
@@ -719,29 +812,24 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
 
 static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dtype, int64_t n, int depth, float *y, bool tap,
                             cudaStream_t s) {
-    Carver cv{w->dev};
+    Carver cv{w->dev.as<char>()};
+    const FaChunk c = carve_fa(m, cv, n, depth, w->fa_cap_sites);
     const int64_t bp = round128(n);
     std::map<std::string, Tap> &taps = w->taps;
     tap = tap && m->taps;
-    int hh[4] = {depth, 0, 0, 0}, ww[4] = {33, 0, 0, 0};
-    for (int i = 1; i < 4; ++i) { hh[i] = conv_out(hh[i - 1]); ww[i] = conv_out(ww[i - 1]); }
-    const int chans[4] = {m->channels, 64, 128, 256};
+    const FaDims d = fa_dims(depth);
+    const int *hh = d.h, *ww = d.w, *chans = kFaChans;
     const bool f32 = m->precision == C3B_PREC_FP32;
     const char *tapname[3][3] = {{"conv1", "res_block1", "res_block1_mid"}, {"conv3", "res_block2", "res_block2_mid"},
                                  {"conv5", "res_block3", "res_block3_mid"}};
 
     if (f32) {
         w->fa_zeroed = false;       // this path overwrites the region the tensor-core path keeps zero-bordered
-        float *xin = cv.take<float>((size_t)n * depth * 33 * m->channels * 4);
-        float *act[3][3];
-        for (int l = 0; l < 3; ++l)
-            for (int i = 0; i < 3; ++i) act[l][i] = cv.take<float>((size_t)n * hh[l + 1] * ww[l + 1] * chans[l + 1] * 4);
-        float *sp = cv.take<float>((size_t)bp * 3584 * 4);
-        float *z4 = cv.take<float>((size_t)bp * 256 * 4);
-        if (c3b_launch_ingest_fa_f32(x, x_dtype, xin, n * depth * 33 * m->channels, s)) return 1;
-        const float *cur = xin;
+        float *sp = c.sp32, *z4 = c.z4;
+        if (c3b_launch_ingest_fa_f32(x, x_dtype, c.xin, n * depth * 33 * m->channels, s)) return 1;
+        const float *cur = c.xin;
         for (int l = 0; l < 3; ++l) {
-            float *a0 = act[l][0], *a1 = act[l][1], *a2 = act[l][2];
+            float *a0 = c.act32[l][0], *a1 = c.act32[l][1], *a2 = c.act32[l][2];
             if (c3b_launch_conv_f32(cur, m->conv_f32[3 * l], nullptr, a0, n, hh[l], ww[l], hh[l + 1], ww[l + 1], s)) return 1;
             if (c3b_launch_conv_f32(a0, m->conv_f32[3 * l + 1], nullptr, a1, n, hh[l + 1], ww[l + 1], hh[l + 1], ww[l + 1], s)) return 1;
             if (c3b_launch_conv_f32(a1, m->conv_f32[3 * l + 2], a0, a2, n, hh[l + 1], ww[l + 1], hh[l + 1], ww[l + 1], s)) return 1;
@@ -754,8 +842,8 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
         if (tap) {
             for (int l = 0; l < 3; ++l) {
                 const int64_t inner = (int64_t)hh[l + 1] * ww[l + 1] * chans[l + 1];
-                taps[tapname[l][0]] = {act[l][0], 0, 0, inner, 0, {}};
-                taps[tapname[l][1]] = {act[l][2], 0, 0, inner, 0, {}};
+                taps[tapname[l][0]] = {c.act32[l][0], 0, 0, inner, 0, {}};
+                taps[tapname[l][1]] = {c.act32[l][2], 0, 0, inner, 0, {}};
             }
             taps["spp"] = {sp, 0, 0, 3584, 0, {}};
             taps["l4_pre"] = {z4, 0, 0, 256, 0, {}};
@@ -766,31 +854,20 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
     // ---- tensor-core path: zero-padded channel-group-planar feature maps (pconv_tc.cu).  Every stride-2 stem conv reads its
     // input as FOUR PARITY PLANES in its own output geometry (written by the ingest kernel / the previous residual block's
     // epilogue), which turns it into the same shifted-view implicit GEMM as the stride-1 convs: no gathers anywhere.
-    const int cpad = 16;                       // conv1 input channels padded to one wgmma k-step
-    PlanarGeom geo[3];
-    op_t *stem_in[3];                          // parity planes feeding conv1 / conv3 / conv5: [4][cin/8][geo[l].p][8]
-    op_t *act[3][3];
-    const int stem_c[3] = {cpad, 64, 128};
-    const size_t planar_begin = cv.off;
-    for (int l = 0; l < 3; ++l) {
-        geo[l] = c3b_planar_geom(n, hh[l + 1], ww[l + 1], w->fa_cap_sites);
-        stem_in[l] = cv.take<op_t>((size_t)4 * (stem_c[l] / 8) * geo[l].p * 16);
-        for (int i = 0; i < (l == 2 ? 3 : 2); ++i) act[l][i] = cv.take<op_t>((size_t)(chans[l + 1] / 8) * geo[l].p * 16);
-    }
-    act[0][2] = stem_in[1];
-    act[1][2] = stem_in[2];
-    const size_t planar_end = cv.off;
-    op_t *sp = cv.take<op_t>((size_t)bp * 3584 * 2);
-    float *z4 = cv.take<float>((size_t)16 * bp * 256 * 4);
+    const PlanarGeom *geo = c.geo;
+    op_t *const(*act)[3] = c.act;
+    const int stem_c[3] = {kFaCpad, 64, 128};
+    op_t *sp = c.sp;
+    float *z4 = c.z4;
     // borders / guards of the planar maps must be zero; the convs only ever store real pixels and the layout is that of the
     // workspace's largest chunk (fa_cap_sites), so one clear per (workspace, capacity, depth) is enough: a ragged tail chunk
     // reuses the zeros already there (stale pixels of sites >= n only feed outputs of sites >= n, which are never stored)
     if (!w->fa_zeroed) {
-        C3B_CUDA(cudaMemsetAsync(w->dev + planar_begin, 0, planar_end - planar_begin, s));
+        C3B_CUDA(cudaMemsetAsync(w->dev.as<char>() + c.planar_begin, 0, c.planar_end - c.planar_begin, s));
         w->fa_zeroed = true;
     }
     static const char *cn[9] = {"conv0", "conv1", "conv2", "conv3", "conv4", "conv5", "conv6", "conv7", "conv8"};
-    { PROF("ingest"); if (c3b_launch_ingest_fa_tc(x, x_dtype, m->channels, cpad, stem_in[0], n, depth, geo[0], s)) return 1; }
+    { PROF("ingest"); if (c3b_launch_ingest_fa_tc(x, x_dtype, m->channels, kFaCpad, c.stem_in[0], n, depth, geo[0], s)) return 1; }
     m->launches += 1;
     for (int l = 0; l < 3; ++l) {
         op_t *a0 = act[l][0], *a1 = act[l][1], *a2 = act[l][2];
@@ -800,7 +877,7 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
         pa.relu = 1;
         // stem conv (stride 2): shifted views of the four parity planes
         pa.c = stem_c[l]; pa.n = co; pa.stride2 = 1;
-        pa.in = stem_in[l]; pa.out = a0; pa.residual = nullptr; pa.w = m->conv_tc[3 * l];
+        pa.in = c.stem_in[l]; pa.out = a0; pa.residual = nullptr; pa.w = m->conv_tc[3 * l];
         { PROF(cn[3 * l]); if (c3b_launch_pconv(m, pa, s)) return 1; }
         // residual block: two stride-1 shifted-view convolutions; the second one scatters its output into the next stem's
         // parity planes (levels 0, 1) or writes the plain planar map SPP reads (level 2)
@@ -860,8 +937,8 @@ static int forward_impl(c3b_model *m, const void *x, int x_dtype, int x_on_devic
     if (m->kind == C3B_FULL_ALIGNMENT) {
         if (starts) { c3b_set_error("%s: window input is a pileup feature", who); return 1; }
         if (depth < 8 || depth > 512) { c3b_set_error("%s: bad full-alignment depth %d", who, depth); return 1; }
-        int h = depth, w = 33;
-        for (int i = 0; i < 3; ++i) { h = conv_out(h); w = conv_out(w); }
+        const FaDims d = fa_dims(depth);
+        const int h = d.h[3], w = d.w[3];
         for (int p = 1; p <= 3; ++p) {
             const int wh = (h + p - 1) / p, ww = (w + p - 1) / p;
             if ((h + wh - 1) / wh != p || (w + ww - 1) / ww != p) {
@@ -887,65 +964,40 @@ static int forward_impl(c3b_model *m, const void *x, int x_dtype, int x_on_devic
         w->fa_cap_sites = cap;
     }
 
-    const size_t need = ws_bytes_needed(m, cap, depth);
-    if (w->dev_bytes < need) {
-        C3B_CUDA(cudaStreamSynchronize(s));
-        if (ensure_dev((void **)&w->dev, &w->dev_bytes, need)) return 1;
+    Carver layout{nullptr};
+    if (m->kind == C3B_PILEUP) carve_pileup(m, layout, cap);
+    else carve_fa(m, layout, cap, depth, cap);
+    if (w->dev.cap < layout.off) {
+        if (w->dev.ensure(layout.off, s, who)) return 1;
         w->fa_zeroed = false;       // fresh memory: the planar maps' borders / guards must be cleared again
     }
-    const void *xd = x;
-    const int64_t *sd = starts, *bd = bounds;
-    float *yd = y;
-    if (!x_on_device) {
-        const size_t xbytes = starts ? (size_t)n_cols * m->channels * esz : (size_t)batch * site_elems * esz;
-        if (w->dev_x_bytes < xbytes) C3B_CUDA(cudaStreamSynchronize(s));
-        if (ensure_dev(&w->dev_x, &w->dev_x_bytes, xbytes)) return 1;
-        C3B_CUDA(cudaMemcpyAsync(w->dev_x, x, xbytes, cudaMemcpyHostToDevice, s));
-        xd = w->dev_x;
-        if (starts) {
-            const size_t aux = (size_t)batch * (bounds ? 24 : 8);        // starts, then the bounds pairs
-            if (w->dev_aux_bytes < aux) C3B_CUDA(cudaStreamSynchronize(s));
-            if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, aux)) return 1;
-            C3B_CUDA(cudaMemcpyAsync(w->dev_aux, starts, (size_t)batch * 8, cudaMemcpyHostToDevice, s));
-            sd = (const int64_t *)w->dev_aux;
-            if (bounds) {
-                int64_t *bdev = (int64_t *)w->dev_aux + batch;
-                C3B_CUDA(cudaMemcpyAsync(bdev, bounds, (size_t)batch * 16, cudaMemcpyHostToDevice, s));
-                bd = bdev;
-            }
-        }
-    }
-    if (!y_on_device) {
-        if (w->dev_y_bytes < (size_t)batch * m->out_dim * 4) C3B_CUDA(cudaStreamSynchronize(s));
-        if (ensure_dev((void **)&w->dev_y, &w->dev_y_bytes, (size_t)batch * m->out_dim * 4)) return 1;
-        yd = w->dev_y;
-    }
+    Staging st{m, s, who};
+    st.in(x, starts ? (size_t)n_cols * m->channels * esz : (size_t)batch * site_elems * esz, x_on_device);
+    st.in(starts, (size_t)batch * 8, x_on_device);
+    st.in(bounds, (size_t)batch * 16, x_on_device);
+    st.out(y, (size_t)batch * m->out_dim * 4, y_on_device);
+    if (st.upload()) return 1;
     if (m->taps) w->taps.clear();
     for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
         const int64_t n = std::min(chunk, batch - b0);
-        float *yc = yd + (size_t)b0 * m->out_dim;
+        float *yc = y + (size_t)b0 * m->out_dim;
         int rc;
         if (m->kind == C3B_PILEUP) {
             PileupSrc src;
             src.dtype = x_dtype;
             src.n_cols = n_cols;
-            src.starts = starts ? sd + b0 : nullptr;
-            src.bounds = starts && bounds ? bd + 2 * b0 : nullptr;
-            src.x = starts ? xd : (const void *)((const char *)xd + (size_t)b0 * site_elems * esz);
+            src.starts = starts ? starts + b0 : nullptr;
+            src.bounds = starts && bounds ? bounds + 2 * b0 : nullptr;
+            src.x = starts ? x : (const void *)((const char *)x + (size_t)b0 * site_elems * esz);
             rc = forward_pileup_chunk(m, w, src, n, yc, b0 == 0, sync_host && (!x_on_device || !y_on_device), s);
         } else {
-            rc = forward_fa_chunk(m, w, (const char *)xd + (size_t)b0 * site_elems * esz, x_dtype, n, depth, yc, b0 == 0, s);
+            rc = forward_fa_chunk(m, w, (const char *)x + (size_t)b0 * site_elems * esz, x_dtype, n, depth, yc, b0 == 0, s);
         }
         if (rc) return rc;
     }
     m->last_batch = std::min(chunk, batch);
     m->last_depth = depth;
-    if (!y_on_device) C3B_CUDA(cudaMemcpyAsync(y, yd, (size_t)batch * m->out_dim * 4, cudaMemcpyDeviceToHost, s));
-    if ((!x_on_device || !y_on_device) && sync_host) {
-        C3B_CUDA(cudaStreamSynchronize(s));
-        C3B_CUDA(cudaGetLastError());
-    }
-    return 0;
+    return st.download(sync_host);
 }
 
 extern "C" int c3b_forward(c3b_model *m, const void *x, int x_dtype, int x_on_device, int64_t batch, int depth, float *y,
@@ -993,37 +1045,22 @@ extern "C" int c3b_decode_stage1(c3b_model *m, const float *y, const uint8_t *re
         c3b_set_error("c3b_decode_stage1: null buffer");
         return 1;
     }
-    const int nh = m->nheads;
-    if (on_device) {
-        m->launches++;
-        return c3b_launch_decode_stage1(y, ref_gt21, batch, m->out_dim, is_ref, ref_prob, argmax, maxprob, qual, nonref_idx, n_nonref, s);
-    }
-    // host buffers: stage through the stream's workspace, one packed region [qual | y | ref_prob | maxprob | argmax | idx | n | gt | flag]
-    Workspace *w = get_workspace(m, s);
-    if (!w) return 1;
-    const size_t B = (size_t)batch;
-    size_t o_qual = 0, o_y = o_qual + B * 8, o_rp = o_y + B * m->out_dim * 4, o_mp = o_rp + B * 4, o_am = o_mp + B * nh * 4,
-           o_idx = o_am + B * nh * 4, o_n = o_idx + B * 4, o_gt = o_n + 16, o_flag = o_gt + (B + 15) / 16 * 16,
-           total = o_flag + (B + 15) / 16 * 16;
-    if (w->dev_aux_bytes < total) C3B_CUDA(cudaStreamSynchronize(s));
-    if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, total)) return 1;
-    char *d = (char *)w->dev_aux;
-    C3B_CUDA(cudaMemcpyAsync(d + o_y, y, B * m->out_dim * 4, cudaMemcpyHostToDevice, s));
-    C3B_CUDA(cudaMemcpyAsync(d + o_gt, ref_gt21, B, cudaMemcpyHostToDevice, s));
+    const size_t B = (size_t)batch, nh = (size_t)m->nheads;
+    Staging st{m, s, "c3b_decode_stage1"};
+    st.in(y, B * m->out_dim * 4, on_device);
+    st.in(ref_gt21, B, on_device);
+    st.out(is_ref, B, on_device);
+    st.out(ref_prob, B * 4, on_device);
+    st.out(argmax, B * nh * 4, on_device);
+    st.out(maxprob, B * nh * 4, on_device);
+    st.out(qual, B * 8, on_device);
+    st.out(nonref_idx, B * 4, on_device);
+    st.out(n_nonref, 4, on_device);
+    if (st.upload()) return 1;
     m->launches++;
-    if (c3b_launch_decode_stage1((const float *)(d + o_y), (const uint8_t *)(d + o_gt), batch, m->out_dim, (uint8_t *)(d + o_flag),
-                                 (float *)(d + o_rp), (int32_t *)(d + o_am), (float *)(d + o_mp), (double *)(d + o_qual),
-                                 (int32_t *)(d + o_idx), (int32_t *)(d + o_n), s))
+    if (c3b_launch_decode_stage1(y, ref_gt21, batch, m->out_dim, is_ref, ref_prob, argmax, maxprob, qual, nonref_idx, n_nonref, s))
         return 1;
-    C3B_CUDA(cudaMemcpyAsync(is_ref, d + o_flag, B, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(ref_prob, d + o_rp, B * 4, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(argmax, d + o_am, B * nh * 4, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(maxprob, d + o_mp, B * nh * 4, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(qual, d + o_qual, B * 8, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(nonref_idx, d + o_idx, B * 4, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(n_nonref, d + o_n, 4, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    return st.download(true);
 }
 
 // ------------------------------------------------------------------------------------------------ decode, stage 2
@@ -1041,48 +1078,32 @@ extern "C" int c3b_decode_stage2(c3b_model *m, const float *y, const uint8_t *re
     }
     cudaStream_t s = (cudaStream_t)cuda_stream;
     C3B_CUDA(cudaSetDevice(m->device));
-    if (on_device) {
-        m->launches++;
-        return c3b_launch_decode_stage2(y, ref_gt21, batch, m->out_dim, sites, n_sites, max_sites, k, cat, idx, prob, tie_mask,
-                                        count, complete, s);
+    int64_t n = max_sites;          // host buffers: the sites to rank, checked here
+    if (!on_device) {
+        if (n_sites) n = *n_sites;
+        if (n < 0 || n > max_sites) { c3b_set_error("c3b_decode_stage2: n_sites must be in [0, max_sites]"); return 1; }
+        if (sites)
+            for (int64_t i = 0; i < n; ++i)
+                if (sites[i] < 0 || sites[i] >= batch) { c3b_set_error("c3b_decode_stage2: site index out of range [0, batch)"); return 1; }
     }
-    const int64_t n = n_sites ? (int64_t)*n_sites : max_sites;
-    if (n < 0 || n > max_sites) { c3b_set_error("c3b_decode_stage2: n_sites must be in [0, max_sites]"); return 1; }
-    if (sites)
-        for (int64_t i = 0; i < n; ++i)
-            if (sites[i] < 0 || sites[i] >= batch) { c3b_set_error("c3b_decode_stage2: site index out of range [0, batch)"); return 1; }
-    // host buffers: stage through the stream's workspace, one packed region [prob | y | sites | count | n | idx | mask | gt | cat | complete]
-    Workspace *w = get_workspace(m, s);
-    if (!w) return 1;
     const size_t B = (size_t)batch, S = (size_t)max_sites, SK = S * (size_t)k;
-    auto up16 = [](size_t v) { return (v + 15) / 16 * 16; };
-    size_t o_prob = 0, o_y = o_prob + up16(SK * 4), o_sites = o_y + up16(B * m->out_dim * 4), o_cnt = o_sites + up16(S * 4),
-           o_n = o_cnt + up16(S * 4), o_idx = o_n + 16, o_mask = o_idx + up16(SK * 2), o_gt = o_mask + up16(SK * 2),
-           o_cat = o_gt + up16(B), o_done = o_cat + up16(SK), total = o_done + up16(S);
-    if (w->dev_aux_bytes < total) C3B_CUDA(cudaStreamSynchronize(s));
-    if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, total)) return 1;
-    char *d = (char *)w->dev_aux;
-    const int32_t n32 = (int32_t)n;
-    if (B) {
-        C3B_CUDA(cudaMemcpyAsync(d + o_y, y, B * m->out_dim * 4, cudaMemcpyHostToDevice, s));
-        C3B_CUDA(cudaMemcpyAsync(d + o_gt, ref_gt21, B, cudaMemcpyHostToDevice, s));
-    }
-    if (sites && n) C3B_CUDA(cudaMemcpyAsync(d + o_sites, sites, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    C3B_CUDA(cudaMemcpyAsync(d + o_n, &n32, 4, cudaMemcpyHostToDevice, s));
+    Staging st{m, s, "c3b_decode_stage2"};
+    st.in(y, B * m->out_dim * 4, on_device);
+    st.in(ref_gt21, B, on_device);
+    st.in(sites, (size_t)n * 4, on_device);
+    st.in(n_sites, 4, on_device);
+    st.out(cat, SK, on_device);
+    st.out(idx, SK * 2, on_device);
+    st.out(prob, SK * 4, on_device);
+    st.out(tie_mask, SK * 2, on_device);
+    st.out(count, S * 4, on_device);
+    st.out(complete, S, on_device);
+    if (st.upload()) return 1;
     m->launches++;
-    if (c3b_launch_decode_stage2((const float *)(d + o_y), (const uint8_t *)(d + o_gt), batch, m->out_dim,
-                                 sites ? (const int32_t *)(d + o_sites) : nullptr, (const int32_t *)(d + o_n), max_sites, k,
-                                 (uint8_t *)(d + o_cat), (uint16_t *)(d + o_idx), (float *)(d + o_prob), (uint16_t *)(d + o_mask),
-                                 (int32_t *)(d + o_cnt), (uint8_t *)(d + o_done), s))
+    if (c3b_launch_decode_stage2(y, ref_gt21, batch, m->out_dim, sites, n_sites, max_sites, k, cat, idx, prob, tie_mask, count,
+                                 complete, s))
         return 1;
-    C3B_CUDA(cudaMemcpyAsync(cat, d + o_cat, SK, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(idx, d + o_idx, SK * 2, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(prob, d + o_prob, SK * 4, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(tie_mask, d + o_mask, SK * 2, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(count, d + o_cnt, S * 4, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(complete, d + o_done, S, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    return st.download(true);
 }
 
 // ------------------------------------------------------------------------------------------------ decode, stage 3 (calls)
@@ -1101,44 +1122,29 @@ extern "C" int c3b_decode_calls(c3b_model *m, const float *y, const uint8_t *ref
     if (batch > INT32_MAX || n_alt_bytes > ((int64_t)1 << 40)) { c3b_set_error("c3b_decode_calls: batch or alt_info too large"); return 1; }
     cudaStream_t s = (cudaStream_t)cuda_stream;
     C3B_CUDA(cudaSetDevice(m->device));
-    const size_t B = (size_t)batch, NB = (size_t)n_alt_bytes, pool = 2 * NB + 8 * B;
-    auto up = [](size_t v) { return (v + 255) / 256 * 256; };
-    const size_t scratch = up(c3b_calls_scratch_bytes(batch, m->out_dim, k, n_alt_bytes));
-    Workspace *w = get_workspace(m, s);
-    if (!w) return 1;
-    if (on_device) {
-        if (w->dev_aux_bytes < scratch) C3B_CUDA(cudaStreamSynchronize(s));
-        if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, scratch)) return 1;
-        m->launches++;
-        return c3b_launch_decode_calls(y, ref_base, batch, m->out_dim, alt_bytes, alt_offsets, n_alt_bytes, config, max_infer_len, k,
-                                       calls, text, ad, w->dev_aux, s);
+    if (!on_device) {
+        if (alt_offsets[0] < 0) { c3b_set_error("c3b_decode_calls: alt_offsets[0] < 0"); return 1; }
+        for (int64_t i = 0; i < batch; ++i)
+            if (alt_offsets[i + 1] < alt_offsets[i] || alt_offsets[i + 1] > n_alt_bytes) {
+                c3b_set_error("c3b_decode_calls: alt_offsets must be non-decreasing within [0, n_alt_bytes] (site %lld)", (long long)i);
+                return 1;
+            }
     }
-    if (alt_offsets[0] < 0) { c3b_set_error("c3b_decode_calls: alt_offsets[0] < 0"); return 1; }
-    for (int64_t i = 0; i < batch; ++i)
-        if (alt_offsets[i + 1] < alt_offsets[i] || alt_offsets[i + 1] > n_alt_bytes) {
-            c3b_set_error("c3b_decode_calls: alt_offsets must be non-decreasing within [0, n_alt_bytes] (site %lld)", (long long)i);
-            return 1;
-        }
-    // host buffers: stage through the stream's workspace after the scratch [y | offsets | ad | calls | ref_base | bytes | text]
-    size_t o_y = scratch, o_off = o_y + up(B * m->out_dim * 4), o_ad = o_off + up((B + 1) * 8), o_calls = o_ad + up(pool * 8),
-           o_ref = o_calls + up(B * sizeof(c3b_call)), o_bytes = o_ref + up(B), o_text = o_bytes + up(NB), total = o_text + up(pool);
-    if (w->dev_aux_bytes < total) C3B_CUDA(cudaStreamSynchronize(s));
-    if (ensure_dev(&w->dev_aux, &w->dev_aux_bytes, total)) return 1;
-    char *d = (char *)w->dev_aux;
-    C3B_CUDA(cudaMemcpyAsync(d + o_y, y, B * m->out_dim * 4, cudaMemcpyHostToDevice, s));
-    C3B_CUDA(cudaMemcpyAsync(d + o_off, alt_offsets, (B + 1) * 8, cudaMemcpyHostToDevice, s));
-    C3B_CUDA(cudaMemcpyAsync(d + o_ref, ref_base, B, cudaMemcpyHostToDevice, s));
-    if (NB) C3B_CUDA(cudaMemcpyAsync(d + o_bytes, alt_bytes, NB, cudaMemcpyHostToDevice, s));
+    const size_t B = (size_t)batch, NB = (size_t)n_alt_bytes, pool = 2 * NB + 8 * B;
+    Staging st{m, s, "c3b_decode_calls", (c3b_calls_scratch_bytes(batch, m->out_dim, k, n_alt_bytes) + 255) / 256 * 256};
+    st.in(y, B * m->out_dim * 4, on_device);
+    st.in(alt_offsets, (B + 1) * 8, on_device);
+    st.in(ref_base, B, on_device);
+    st.in(alt_bytes, NB, on_device);
+    st.out(calls, B * sizeof(c3b_call), on_device);
+    st.out(text, pool, on_device);
+    st.out(ad, pool * 8, on_device);
+    if (st.upload()) return 1;
     m->launches++;
-    if (c3b_launch_decode_calls((const float *)(d + o_y), (const uint8_t *)(d + o_ref), batch, m->out_dim, d + o_bytes,
-                                (const int64_t *)(d + o_off), n_alt_bytes, config, max_infer_len, k, (c3b_call *)(d + o_calls),
-                                d + o_text, (int64_t *)(d + o_ad), d, s))
+    if (c3b_launch_decode_calls(y, ref_base, batch, m->out_dim, alt_bytes, alt_offsets, n_alt_bytes, config, max_infer_len, k, calls,
+                                text, ad, st.scratch, s))
         return 1;
-    C3B_CUDA(cudaMemcpyAsync(calls, d + o_calls, B * sizeof(c3b_call), cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(text, d + o_text, pool, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaMemcpyAsync(ad, d + o_ad, pool * 8, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    return st.download(true);
 }
 
 // ------------------------------------------------------------------------------------------------ taps (debug)
@@ -1232,14 +1238,8 @@ extern "C" void c3b_destroy(c3b_model *m) {
     cudaSetDevice(m->device);
     for (Workspace *w : m->ws) {
         for (auto &r : w->prof) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
-        if (w->dev) cudaFree(w->dev);
-        if (w->dev_x) cudaFree(w->dev_x);
-        if (w->dev_y) cudaFree(w->dev_y);
-        if (w->dev_aux) cudaFree(w->dev_aux);
         delete w;
     }
-    if (m->blob) cudaFree(m->blob);
-    if (m->f32blob) cudaFree(m->f32blob);
     if (m->lstm_trace) cudaFree(m->lstm_trace);
     delete m;
 }

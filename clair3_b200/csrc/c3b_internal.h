@@ -10,6 +10,7 @@
 
 #include "../../include/clair3_b200.h"
 #include "../../include/clair3_b200_debug.h"
+#include "../../include/clair3_b200_pileup.h"
 
 #define C3B_T 33            // positions per site (shared/param_p.py:34-35)
 #define C3B_H1 128          // LSTM1 hidden (clair3/model.py:46)
@@ -77,6 +78,70 @@ float c3b_op2f(uint16_t h);     // host: fp16 bits -> fp32
             return 1;                                                                           \
         }                                                                                       \
     } while (0)
+
+// A device buffer that grows on demand and frees itself.  Sizing::exact grows to the size asked for: the model's weights,
+// workspace and staging, whose sizes follow the call shape, which rarely changes.  Sizing::headroom adds 25 %: the pileup
+// counter's and the full-alignment builder's per-call buffers, whose sizes follow the data of each call.  Growing first waits
+// for stream s, on which queued work may still use the old memory.  `what` names the owner in the error message.
+struct C3bBuf {
+    enum Sizing { headroom, exact };
+    const Sizing sizing;
+    void *p = nullptr;
+    size_t cap = 0;
+    explicit C3bBuf(Sizing z = headroom) : sizing(z) {}
+    C3bBuf(const C3bBuf &) = delete;
+    C3bBuf &operator=(const C3bBuf &) = delete;
+    ~C3bBuf() { if (p) cudaFree(p); }
+    int ensure(size_t bytes, cudaStream_t s, const char *what) {
+        if (bytes <= cap) return 0;
+        if (p) {
+            C3B_CUDA(cudaStreamSynchronize(s));
+            cudaFree(p);
+        }
+        p = nullptr;
+        cap = 0;
+        const size_t want = sizing == exact ? bytes : bytes + bytes / 4 + 256;
+        if (cudaMalloc(&p, want) != cudaSuccess) {
+            c3b_set_error("%s: cudaMalloc of %zu bytes failed", what, want);
+            return 1;
+        }
+        cap = want;
+        return 0;
+    }
+    template <class T> T *as() const { return reinterpret_cast<T *>(p); }
+};
+
+// One input array of a call: a device pointer passes through, host memory is copied into b on stream s.
+template <class T>
+int c3b_upload(C3bBuf &b, const T *src, size_t bytes, int on_device, const T *&dev, cudaStream_t s, const char *what) {
+    if (on_device) { dev = src; return 0; }
+    if (b.ensure(bytes ? bytes : 1, s, what)) return 1;
+    if (bytes) C3B_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, s));
+    dev = b.as<const T>();
+    return 0;
+}
+
+// The eight core c3b_bam_records arrays of a call, into the kernel-visible record struct R (DevReads / FaReads, which share
+// these field names) through c3b_upload.  n_cigar / n_seq: the CIGAR words and sequence bytes the arrays hold.
+template <class Reads>
+int c3b_upload_records(Reads &R, C3bBuf (&b)[8], const c3b_bam_records *r, int64_t n_cigar, int64_t n_seq, int on_device,
+                       cudaStream_t s, const char *what) {
+    const size_t n = (size_t)r->n_reads;
+    return c3b_upload(b[0], r->pos, n * 8, on_device, R.pos, s, what) || c3b_upload(b[1], r->flag, n * 2, on_device, R.flag, s, what) ||
+           c3b_upload(b[2], r->mapq, n, on_device, R.mapq, s, what) ||
+           c3b_upload(b[3], r->cigar_off, (n + 1) * 8, on_device, R.cigar_off, s, what) ||
+           c3b_upload(b[4], r->cigar, (size_t)n_cigar * 4, on_device, R.cigar, s, what) ||
+           c3b_upload(b[5], r->seq_off, (n + 1) * 8, on_device, R.seq_off, s, what) ||
+           c3b_upload(b[6], r->seq, (size_t)n_seq, on_device, R.seq, s, what) ||
+           c3b_upload(b[7], r->l_qseq, n * 4, on_device, R.l_qseq, s, what);
+}
+
+// Entry n of an offset array of n + 1 entries that lives on the host or (on_device) the device; 0 for a null array.
+int c3b_last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s, int64_t *last);
+
+// Makes device `ordinal` current after checking that it exists and is an sm_90 part.  Returns 0; `unsupported` when there
+// is no CUDA device or it is not sm_90; 1 for a bad ordinal or a failed runtime call.  sm_count (optional): its SM count.
+int c3b_use_device(int ordinal, int unsupported, int *sm_count);
 
 struct HostParam {
     std::vector<float> data;
@@ -170,16 +235,8 @@ struct Tap {
 
 struct Workspace {
     cudaStream_t stream = nullptr;
-    // generic device scratch, carved by the forward pass
-    char *dev = nullptr;
-    size_t dev_bytes = 0;
-    // staging for host-side callers
-    void *dev_x = nullptr;
-    size_t dev_x_bytes = 0;
-    float *dev_y = nullptr;
-    size_t dev_y_bytes = 0;
-    void *dev_aux = nullptr;         // window offsets / decode inputs of host-side callers
-    size_t dev_aux_bytes = 0;
+    C3bBuf dev{C3bBuf::exact};       // device scratch, carved by the forward pass
+    C3bBuf stage{C3bBuf::exact};     // host arguments of a call (Staging in c3b_api.cu), after stage 3's kernel scratch
     // full-alignment planar maps are laid out for `fa_cap_sites` sites (the largest chunk seen on this workspace); smaller
     // chunks reuse that layout (their borders / guards are already zero), so a ragged tail never re-clears the region
     int64_t fa_cap_sites = 0;
@@ -213,10 +270,8 @@ struct c3b_model {
     std::map<std::string, std::vector<int64_t>> expected_shape;
 
     // device weights
-    char *blob = nullptr;        // tensor-core images + shared fp32 head weights (broadcast unit)
-    size_t blob_bytes = 0;
-    char *f32blob = nullptr;     // fp32 debug path weights
-    size_t f32blob_bytes = 0;
+    C3bBuf blob{C3bBuf::exact};      // tensor-core images + shared fp32 head weights (broadcast unit)
+    C3bBuf f32blob{C3bBuf::exact};   // fp32 debug path weights
 
     HeadsParams heads;
     // fp32 path
@@ -306,40 +361,3 @@ int c3b_launch_pconv(const c3b_model *m, const PconvArgs &a, cudaStream_t s);
 int c3b_launch_ingest_fa_tc(const void *x, int dtype, int channels, int cpad, op_t *out, int64_t batch, int depth, const PlanarGeom &g1,
                             cudaStream_t s);
 int c3b_launch_spp_tc(const op_t *x, const PlanarGeom &g, op_t *out, int64_t batch, int c, int bp, cudaStream_t s);
-
-
-// A device buffer that grows on demand (25 % headroom); used by the pileup counter and the full-alignment builder for their
-// per-call inputs and scratch.  `what` names the owner in the error message.
-struct C3bBuf {
-    void *p = nullptr;
-    size_t cap = 0;
-    int ensure(size_t bytes, const char *what = "clair3_b200") {
-        if (bytes <= cap) return 0;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        const size_t want = bytes + bytes / 4 + 256;
-        if (cudaMalloc(&p, want) != cudaSuccess) {
-            c3b_set_error("%s: cudaMalloc of %zu bytes failed", what, want);
-            return 1;
-        }
-        cap = want;
-        return 0;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-    template <class T> T *as() const { return reinterpret_cast<T *>(p); }
-};
-
-// One input array of a call: a device pointer passes through, host memory is copied into b on stream s.
-static inline int c3b_upload(C3bBuf &b, const void *src, size_t bytes, int on_device, const void **dev, cudaStream_t s,
-                             const char *what) {
-    if (on_device) { *dev = src; return 0; }
-    if (b.ensure(bytes ? bytes : 1, what)) return 1;
-    if (bytes) C3B_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, s));
-    *dev = b.p;
-    return 0;
-}

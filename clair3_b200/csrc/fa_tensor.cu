@@ -926,10 +926,6 @@ __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) 
     }
 }
 
-struct FaBuf : C3bBuf {
-    int ensure(size_t bytes) { return C3bBuf::ensure(bytes, "c3b_fa"); }
-};
-
 // glibc's TYPE_3 generator (random_r.c): srandom_r fills r[0..30] with 16807 * r[i-1] mod (2^31 - 1) (Schrage's method on
 // int32), r[i] = r[i-31] + r[i-3] mod 2^32 from i = 34 on (r[31..33] = r[0..2]), and rand() number k is r[344 + k] >> 1.
 void glibc_state(uint32_t seed, uint32_t out[31]) {
@@ -971,15 +967,15 @@ void glibc_jump_matrices(std::vector<uint32_t> &out) {
 
 struct c3b_fa {
     int device = 0;
-    FaBuf in_pos, in_flag, in_mapq, in_coff, in_cigar, in_soff, in_seq, in_lq, in_qoff, in_qual, in_noff, in_name, in_moff, in_mv;
-    FaBuf in_ref, in_cand, in_var, jump, state0;
-    FaBuf fstart, fcnt, foff, F;
-    FaBuf rend, rlo, rov, pass, table, keep, kidx, kovr, kov_ex;
-    FaBuf k_orig, k_start, k_end, k_pmax, k_fs, k_ov, k_pi, k_sig, k_hap, sig_len, sig_ex;
-    FaBuf pool, sig;
-    FaBuf ra, rb, nsel, draws, draw_off;
-    FaBuf matrix, c_depth, c_acgt, al_off, al_n, al_meta, al_read, al_qpos, al_cnt;
-    FaBuf counters;     // int64: 0 nF, 1 n_kept, 2 pool entries, 3 signal entries, 4 draws, 5 status, 6 al_used, 7 spare
+    C3bBuf in_core[8], in_qoff, in_qual, in_noff, in_name, in_moff, in_mv;
+    C3bBuf in_ref, in_cand, in_var, jump, state0;
+    C3bBuf fstart, fcnt, foff, F;
+    C3bBuf rend, rlo, rov, pass, table, keep, kidx, kovr, kov_ex;
+    C3bBuf k_orig, k_start, k_end, k_pmax, k_fs, k_ov, k_pi, k_sig, k_hap, sig_len, sig_ex;
+    C3bBuf pool, sig;
+    C3bBuf ra, rb, nsel, draws, draw_off;
+    C3bBuf matrix, c_depth, c_acgt, al_off, al_n, al_meta, al_read, al_qpos, al_cnt;
+    C3bBuf counters;    // int64: 0 nF, 1 n_kept, 2 pool entries, 3 signal entries, 4 draws, 5 status, 6 al_used, 7 spare
     int64_t n_cand = 0, depth = 0, C = 8, n_kept = 0;
     bool built = false;
     cudaStream_t stream = nullptr;
@@ -993,27 +989,15 @@ extern "C" {
 int c3b_fa_create(c3b_fa **out, int device_ordinal) {
     if (!out) { c3b_set_error("c3b_fa_create: null out"); return 1; }
     *out = nullptr;
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0) {
-        c3b_set_error("no CUDA device: %s (clair3_b200 has no CPU fallback)", cudaGetErrorString(e));
-        return 1;
-    }
-    if (device_ordinal < 0 || device_ordinal >= ndev) { c3b_set_error("bad device ordinal %d", device_ordinal); return 1; }
-    cudaDeviceProp prop;
-    C3B_CUDA(cudaGetDeviceProperties(&prop, device_ordinal));
-    if (prop.major != 9 || prop.minor != 0) {
-        c3b_set_error("device %d is sm_%d%d; this library contains only sm_90a code", device_ordinal, prop.major, prop.minor);
-        return 1;
-    }
-    C3B_CUDA(cudaSetDevice(device_ordinal));
+    if (c3b_use_device(device_ordinal, 1, nullptr)) return 1;
     c3b_fa *w = new c3b_fa();
     w->device = device_ordinal;
     std::vector<uint32_t> J;
     glibc_jump_matrices(J);
     if (cudaEventCreate(&w->ev0) != cudaSuccess || cudaEventCreate(&w->ev1) != cudaSuccess ||
-        cudaMallocHost((void **)&w->host_counters, 8 * sizeof(int64_t)) != cudaSuccess || w->jump.ensure(J.size() * 4) ||
-        w->state0.ensure(31 * 4) || w->counters.ensure(8 * 8) ||
+        cudaMallocHost((void **)&w->host_counters, 8 * sizeof(int64_t)) != cudaSuccess ||
+        w->jump.ensure(J.size() * 4, nullptr, "c3b_fa") || w->state0.ensure(31 * 4, nullptr, "c3b_fa") ||
+        w->counters.ensure(8 * 8, nullptr, "c3b_fa") ||
         cudaMemcpy(w->jump.p, J.data(), J.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
         c3b_set_error("c3b_fa_create: allocation failed");
         c3b_fa_destroy(w);
@@ -1021,23 +1005,6 @@ int c3b_fa_create(c3b_fa **out, int device_ordinal) {
     }
     *out = w;
     return 0;
-}
-
-static int fa_upload(FaBuf &b, const void *src, size_t bytes, int on_device, const void **dev, cudaStream_t s) {
-    return c3b_upload(b, src, bytes, on_device, dev, s, "c3b_fa");
-}
-
-static int64_t last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s) {
-    int64_t v = 0;
-    if (!off) return 0;
-    if (on_device) {
-        if (cudaMemcpyAsync(&v, off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-            cudaStreamSynchronize(s) != cudaSuccess)
-            return -1;
-    } else {
-        v = off[n];
-    }
-    return v;
 }
 
 static inline unsigned blocks_for(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
@@ -1091,36 +1058,29 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     memset(&R, 0, sizeof(R));
     R.n = n;
     if (n > 0) {
-        const int64_t n_cigar = last_offset(core->cigar_off, n, on_device, s), n_seq = last_offset(core->seq_off, n, on_device, s);
-        const int64_t n_qual = last_offset(records->qual_off, n, on_device, s), n_name = last_offset(records->qname_off, n, on_device, s);
-        const int64_t n_mv = last_offset(records->mv_off, n, on_device, s);
+        int64_t n_cigar, n_seq, n_qual, n_name, n_mv;
+        if (c3b_last_offset(core->cigar_off, n, on_device, s, &n_cigar) || c3b_last_offset(core->seq_off, n, on_device, s, &n_seq) ||
+            c3b_last_offset(records->qual_off, n, on_device, s, &n_qual) || c3b_last_offset(records->qname_off, n, on_device, s, &n_name) ||
+            c3b_last_offset(records->mv_off, n, on_device, s, &n_mv))
+            return 1;
         if (n_cigar < 0 || n_seq < 0 || n_qual < 0 || n_name < 0 || n_mv < 0) { c3b_set_error("c3b_fa_build: bad offsets"); return 1; }
-        const void *d;
-        if (fa_upload(w->in_pos, core->pos, n * 8, on_device, &d, s)) return 1; R.pos = (const int64_t *)d;
-        if (fa_upload(w->in_flag, core->flag, n * 2, on_device, &d, s)) return 1; R.flag = (const uint16_t *)d;
-        if (fa_upload(w->in_mapq, core->mapq, n, on_device, &d, s)) return 1; R.mapq = (const uint8_t *)d;
-        if (fa_upload(w->in_coff, core->cigar_off, (n + 1) * 8, on_device, &d, s)) return 1; R.cigar_off = (const int64_t *)d;
-        if (fa_upload(w->in_cigar, core->cigar, n_cigar * 4, on_device, &d, s)) return 1; R.cigar = (const uint32_t *)d;
-        if (fa_upload(w->in_soff, core->seq_off, (n + 1) * 8, on_device, &d, s)) return 1; R.seq_off = (const int64_t *)d;
-        if (fa_upload(w->in_seq, core->seq, n_seq, on_device, &d, s)) return 1; R.seq = (const uint8_t *)d;
-        if (fa_upload(w->in_lq, core->l_qseq, n * 4, on_device, &d, s)) return 1; R.l_qseq = (const int32_t *)d;
-        if (records->qual_off) {
-            if (fa_upload(w->in_qoff, records->qual_off, (n + 1) * 8, on_device, &d, s)) return 1; R.qual_off = (const int64_t *)d;
-            if (fa_upload(w->in_qual, records->qual, n_qual, on_device, &d, s)) return 1; R.qual = (const uint8_t *)d;
-        }
-        if (records->qname_off) {
-            if (fa_upload(w->in_noff, records->qname_off, (n + 1) * 8, on_device, &d, s)) return 1; R.qname_off = (const int64_t *)d;
-            if (fa_upload(w->in_name, records->qname, n_name, on_device, &d, s)) return 1; R.qname = (const uint8_t *)d;
-        }
-        if (records->mv_off && params->dwell) {
-            if (fa_upload(w->in_moff, records->mv_off, (n + 1) * 8, on_device, &d, s)) return 1; R.mv_off = (const int64_t *)d;
-            if (fa_upload(w->in_mv, records->mv, n_mv * 4, on_device, &d, s)) return 1; R.mv = (const int32_t *)d;
-        }
+        if (c3b_upload_records(R, w->in_core, core, n_cigar, n_seq, on_device, s, "c3b_fa")) return 1;
+        const size_t n1 = (size_t)(n + 1) * 8;
+        if (records->qual_off && (c3b_upload(w->in_qoff, records->qual_off, n1, on_device, R.qual_off, s, "c3b_fa") ||
+                                  c3b_upload(w->in_qual, records->qual, (size_t)n_qual, on_device, R.qual, s, "c3b_fa")))
+            return 1;
+        if (records->qname_off && (c3b_upload(w->in_noff, records->qname_off, n1, on_device, R.qname_off, s, "c3b_fa") ||
+                                   c3b_upload(w->in_name, records->qname, (size_t)n_name, on_device, R.qname, s, "c3b_fa")))
+            return 1;
+        if (records->mv_off && params->dwell && (c3b_upload(w->in_moff, records->mv_off, n1, on_device, R.mv_off, s, "c3b_fa") ||
+                                                 c3b_upload(w->in_mv, records->mv, (size_t)n_mv * 4, on_device, R.mv, s, "c3b_fa")))
+            return 1;
     }
-    const void *dref = nullptr;
-    if (fa_upload(w->in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, &dref, s)) return 1;
+    const char *dref = nullptr;
+    if (c3b_upload(w->in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, dref, s, "c3b_fa")) return 1;
     const size_t Kz = (size_t)(n_cand > 0 ? n_cand : 1), Nz = (size_t)(n > 0 ? n : 1);
-    if (w->in_cand.ensure(Kz * 8) || w->in_var.ensure((size_t)(n_var > 0 ? n_var : 1) * sizeof(c3b_fa_variant))) return 1;
+    auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_fa"); };
+    if (grow(w->in_cand, Kz * 8) || grow(w->in_var, (size_t)(n_var > 0 ? n_var : 1) * sizeof(c3b_fa_variant))) return 1;
     if (n_cand) C3B_CUDA(cudaMemcpyAsync(w->in_cand.p, candidates, (size_t)n_cand * 8, cudaMemcpyHostToDevice, s));
     if (n_var) C3B_CUDA(cudaMemcpyAsync(w->in_var.p, variants, (size_t)n_var * sizeof(c3b_fa_variant), cudaMemcpyHostToDevice, s));
     uint32_t st0[31];
@@ -1131,16 +1091,16 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     const size_t Fz = Kz * 33;
     uint64_t T = 2;                                 // name table: a power of two >= 2 n (n < 2^31, so T - 1 fits 32 bits)
     while ((int64_t)T < 2 * n) T <<= 1;
-    if (w->fstart.ensure(Kz * 8) || w->fcnt.ensure(Kz * 8) || w->foff.ensure(Kz * 8) || w->F.ensure(Fz * 8) ||
-        w->rend.ensure(Nz * 8) || w->rlo.ensure(Nz * 8) || w->rov.ensure(Nz * 4) || w->pass.ensure(Nz) ||
-        w->table.ensure((size_t)T * 8) || w->keep.ensure(Nz * 8) || w->kidx.ensure(Nz * 8) || w->kovr.ensure(Nz * 8) ||
-        w->kov_ex.ensure(Nz * 8) || w->k_orig.ensure(Nz * 8) || w->k_start.ensure(Nz * 8) || w->k_end.ensure(Nz * 8) ||
-        w->k_pmax.ensure(Nz * 8) || w->k_fs.ensure(Nz * 8) || w->k_ov.ensure(Nz * 4) || w->k_pi.ensure(Nz * 8) ||
-        w->k_sig.ensure(Nz * 8) || w->k_hap.ensure(Nz * 4) || w->sig_len.ensure(Nz * 8) || w->sig_ex.ensure(Nz * 8) ||
-        w->ra.ensure(Kz * 8) || w->rb.ensure(Kz * 8) || w->nsel.ensure(Kz * 8) || w->draws.ensure(Kz * 8) ||
-        w->draw_off.ensure(Kz * 8) || w->matrix.ensure(Kz * (size_t)depth * 33 * (size_t)w->C) || w->c_depth.ensure(Kz * 4) ||
-        w->c_acgt.ensure(Kz * 16) || w->al_off.ensure(Kz * 4) || w->al_n.ensure(Kz * 4) || w->al_meta.ensure((size_t)AL_CAP * 4) ||
-        w->al_read.ensure((size_t)AL_CAP * 4) || w->al_qpos.ensure((size_t)AL_CAP * 4) || w->al_cnt.ensure((size_t)AL_CAP * 4))
+    if (grow(w->fstart, Kz * 8) || grow(w->fcnt, Kz * 8) || grow(w->foff, Kz * 8) || grow(w->F, Fz * 8) ||
+        grow(w->rend, Nz * 8) || grow(w->rlo, Nz * 8) || grow(w->rov, Nz * 4) || grow(w->pass, Nz) ||
+        grow(w->table, (size_t)T * 8) || grow(w->keep, Nz * 8) || grow(w->kidx, Nz * 8) || grow(w->kovr, Nz * 8) ||
+        grow(w->kov_ex, Nz * 8) || grow(w->k_orig, Nz * 8) || grow(w->k_start, Nz * 8) || grow(w->k_end, Nz * 8) ||
+        grow(w->k_pmax, Nz * 8) || grow(w->k_fs, Nz * 8) || grow(w->k_ov, Nz * 4) || grow(w->k_pi, Nz * 8) ||
+        grow(w->k_sig, Nz * 8) || grow(w->k_hap, Nz * 4) || grow(w->sig_len, Nz * 8) || grow(w->sig_ex, Nz * 8) ||
+        grow(w->ra, Kz * 8) || grow(w->rb, Kz * 8) || grow(w->nsel, Kz * 8) || grow(w->draws, Kz * 8) ||
+        grow(w->draw_off, Kz * 8) || grow(w->matrix, Kz * (size_t)depth * 33 * (size_t)w->C) || grow(w->c_depth, Kz * 4) ||
+        grow(w->c_acgt, Kz * 16) || grow(w->al_off, Kz * 4) || grow(w->al_n, Kz * 4) || grow(w->al_meta, (size_t)AL_CAP * 4) ||
+        grow(w->al_read, (size_t)AL_CAP * 4) || grow(w->al_qpos, (size_t)AL_CAP * 4) || grow(w->al_cnt, (size_t)AL_CAP * 4))
         return 1;
     int64_t *cnt = w->counters.as<int64_t>();
     C3B_CUDA(cudaMemsetAsync(cnt, 0, 64, s));
@@ -1190,7 +1150,7 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     }
     w->n_kept = n_kept;
     if (n_kept > 0) {
-        if (w->pool.ensure((size_t)n_pool * sizeof(PosInfo)) || w->sig.ensure((size_t)(n_sig > 0 ? n_sig : 1) * 4)) return 1;
+        if (grow(w->pool, (size_t)n_pool * sizeof(PosInfo)) || grow(w->sig, (size_t)(n_sig > 0 ? n_sig : 1) * 4)) return 1;
         C3B_CUDA(cudaMemsetAsync(w->pool.p, 0, (size_t)n_pool * sizeof(PosInfo), s));
         fa_scan_kernel<<<1, 1024, 0, s>>>(K.end, K.pmax, n_kept, nullptr, 1);
         w->launches += 1;
@@ -1201,7 +1161,7 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
         if (params->need_haplotagging && n_var > 0) {
             HapArgs H;
             H.R = R; H.K = K; H.n_kept = n_kept; H.var = w->in_var.as<c3b_fa_variant>(); H.n_var = n_var;
-            H.ref = (const char *)dref; H.ref_start = ref_start; H.ref_len = ref_len > 0 ? ref_len : 0; H.status = status;
+            H.ref = dref; H.ref_start = ref_start; H.ref_len = ref_len > 0 ? ref_len : 0; H.status = status;
             fa_haplotag_kernel<<<blocks_for(n_kept, 128), 128, 0, s>>>(H);
             w->launches += 1;
         }
@@ -1216,7 +1176,7 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
         fa_scan_kernel<<<1, 1024, 0, s>>>(w->draws.as<int64_t>(), w->draw_off.as<int64_t>(), n_cand, cnt + 4, 0);
         CandArgs A;
         A.R = R; A.K = K; A.cand = w->in_cand.as<int64_t>(); A.F = w->F.as<int64_t>(); A.nF = nF; A.pool = w->pool.as<PosInfo>();
-        A.ref = (const char *)dref; A.ref_start = ref_start; A.ref_len = ref_len > 0 ? ref_len : 0;
+        A.ref = dref; A.ref_start = ref_start; A.ref_len = ref_len > 0 ? ref_len : 0;
         A.ra = w->ra.as<int64_t>(); A.rb = w->rb.as<int64_t>(); A.nsel = w->nsel.as<int64_t>(); A.draw_off = w->draw_off.as<int64_t>();
         A.rand_skip = params->rand_skip; A.jump = w->jump.as<uint32_t>(); A.state0 = w->state0.as<uint32_t>();
         A.depth = depth; A.C = (int)w->C; A.matrix = w->matrix.as<int8_t>();
@@ -1307,14 +1267,6 @@ int c3b_fa_last_ms(c3b_fa *w, float *ms, int *launches) {
 void c3b_fa_destroy(c3b_fa *w) {
     if (!w) return;
     cudaSetDevice(w->device);
-    FaBuf *all[] = {&w->in_pos, &w->in_flag, &w->in_mapq, &w->in_coff, &w->in_cigar, &w->in_soff, &w->in_seq, &w->in_lq, &w->in_qoff,
-                    &w->in_qual, &w->in_noff, &w->in_name, &w->in_moff, &w->in_mv, &w->in_ref, &w->in_cand, &w->in_var, &w->jump,
-                    &w->state0, &w->fstart, &w->fcnt, &w->foff, &w->F, &w->rend, &w->rlo, &w->rov, &w->pass, &w->table, &w->keep,
-                    &w->kidx, &w->kovr, &w->kov_ex, &w->k_orig, &w->k_start, &w->k_end, &w->k_pmax, &w->k_fs, &w->k_ov, &w->k_pi,
-                    &w->k_sig, &w->k_hap, &w->sig_len, &w->sig_ex, &w->pool, &w->sig, &w->ra, &w->rb, &w->nsel, &w->draws,
-                    &w->draw_off, &w->matrix, &w->c_depth, &w->c_acgt, &w->al_off, &w->al_n, &w->al_meta, &w->al_read,
-                    &w->al_qpos, &w->al_cnt, &w->counters};
-    for (FaBuf *b : all) b->release();
     if (w->ev0) cudaEventDestroy(w->ev0);
     if (w->ev1) cudaEventDestroy(w->ev1);
     if (w->host_counters) cudaFreeHost(w->host_counters);

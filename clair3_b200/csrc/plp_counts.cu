@@ -606,23 +606,19 @@ __global__ void __launch_bounds__(TILE) plp_cands_kernel(CandArgs A) {
     }
 }
 
-struct DBuf : C3bBuf {
-    int ensure(size_t bytes) { return C3bBuf::ensure(bytes, "c3b_plp"); }
-};
-
 }  // namespace
 
 struct c3b_plp {
     int device = 0;
     // inputs (copies of host records)
-    DBuf in_pos, in_flag, in_mapq, in_coff, in_cigar, in_soff, in_seq, in_lq, in_ref;
+    C3bBuf in_core[8], in_ref;
     // scratch
-    DBuf opx, opy, rend, pmax, rows32, dstats, nquirk, dci, tile_cov, tile_off, tile_cand, tile_coff;
-    DBuf g_meta, g_read, g_qpos, g_cnt, g_next;
-    DBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n, ins_last;   // allele export (params.alt_info)
-    DBuf counters;      // int64 n_cols, int64 n_cand, int g_used, int status
+    C3bBuf opx, opy, rend, pmax, rows32, dstats, nquirk, dci, tile_cov, tile_off, tile_cand, tile_coff;
+    C3bBuf g_meta, g_read, g_qpos, g_cnt, g_next;
+    C3bBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n, ins_last;   // allele export (params.alt_info)
+    C3bBuf counters;    // int64 n_cols, int64 n_cand, int g_used, int status
     // outputs
-    DBuf matrix, major, stats, cand_cols, wstart, wbounds, cand_ok, gv_ref, gv_tot;
+    C3bBuf matrix, major, stats, cand_cols, wstart, wbounds, cand_ok, gv_ref, gv_tot;
     int64_t W = 0;
     bool gvcf = false, counted = false, alleles = false;
     cudaStream_t stream = nullptr;
@@ -637,34 +633,17 @@ extern "C" {
 int c3b_plp_create(c3b_plp **out, int device_ordinal) {
     if (!out) { c3b_set_error("c3b_plp_create: null out"); return 1; }
     *out = nullptr;
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0) {
-        c3b_set_error("no CUDA device: %s (clair3_b200 has no CPU fallback)", cudaGetErrorString(e));
-        return 1;
-    }
-    if (device_ordinal < 0 || device_ordinal >= ndev) { c3b_set_error("bad device ordinal %d", device_ordinal); return 1; }
-    cudaDeviceProp prop;
-    C3B_CUDA(cudaGetDeviceProperties(&prop, device_ordinal));
-    if (prop.major != 9 || prop.minor != 0) {
-        c3b_set_error("device %d is sm_%d%d; this library contains only sm_90a code", device_ordinal, prop.major, prop.minor);
-        return 1;
-    }
-    C3B_CUDA(cudaSetDevice(device_ordinal));
+    if (c3b_use_device(device_ordinal, 1, nullptr)) return 1;
     c3b_plp *w = new c3b_plp();
     w->device = device_ordinal;
     if (cudaEventCreate(&w->ev0) != cudaSuccess || cudaEventCreate(&w->ev1) != cudaSuccess ||
         cudaMallocHost((void **)&w->host_counters, 4 * sizeof(int64_t)) != cudaSuccess) {
         c3b_set_error("c3b_plp_create: event / pinned allocation failed");
-        delete w;
+        c3b_plp_destroy(w);
         return 1;
     }
     *out = w;
     return 0;
-}
-
-static int plp_upload(DBuf &b, const void *src, size_t bytes, int on_device, const void **dev, cudaStream_t s) {
-    return c3b_upload(b, src, bytes, on_device, dev, s, "c3b_plp");
 }
 
 int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64_t start, int64_t end, const char *ref_seq,
@@ -695,44 +674,31 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     R.n = n;
     int64_t n_cigar = 0, n_seq = 0;
     if (n > 0) {
-        if (on_device) {
-            C3B_CUDA(cudaMemcpyAsync(&n_cigar, reads->cigar_off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-            C3B_CUDA(cudaMemcpyAsync(&n_seq, reads->seq_off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-            C3B_CUDA(cudaStreamSynchronize(s));
-        } else {
-            n_cigar = reads->cigar_off[n];
-            n_seq = reads->seq_off[n];
-        }
+        if (c3b_last_offset(reads->cigar_off, n, on_device, s, &n_cigar) || c3b_last_offset(reads->seq_off, n, on_device, s, &n_seq))
+            return 1;
         if (n_cigar < 0 || n_seq < 0) { c3b_set_error("c3b_plp_count: negative offsets"); return 1; }
-        const void *d;
-        if (plp_upload(w->in_pos, reads->pos, n * 8, on_device, &d, s)) return 1; R.pos = (const int64_t *)d;
-        if (plp_upload(w->in_flag, reads->flag, n * 2, on_device, &d, s)) return 1; R.flag = (const uint16_t *)d;
-        if (plp_upload(w->in_mapq, reads->mapq, n, on_device, &d, s)) return 1; R.mapq = (const uint8_t *)d;
-        if (plp_upload(w->in_coff, reads->cigar_off, (n + 1) * 8, on_device, &d, s)) return 1; R.cigar_off = (const int64_t *)d;
-        if (plp_upload(w->in_cigar, reads->cigar, n_cigar * 4, on_device, &d, s)) return 1; R.cigar = (const uint32_t *)d;
-        if (plp_upload(w->in_soff, reads->seq_off, (n + 1) * 8, on_device, &d, s)) return 1; R.seq_off = (const int64_t *)d;
-        if (plp_upload(w->in_seq, reads->seq, n_seq, on_device, &d, s)) return 1; R.seq = (const uint8_t *)d;
-        if (plp_upload(w->in_lq, reads->l_qseq, n * 4, on_device, &d, s)) return 1; R.l_qseq = (const int32_t *)d;
+        if (c3b_upload_records(R, w->in_core, reads, n_cigar, n_seq, on_device, s, "c3b_plp")) return 1;
     }
-    const void *dref = nullptr;
-    if (plp_upload(w->in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, &dref, s)) return 1;
+    const char *dref = nullptr;
+    if (c3b_upload(w->in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, dref, s, "c3b_plp")) return 1;
 
     // scratch and outputs
     const size_t Wz = (size_t)(W > 0 ? W : 1), Tz = (size_t)(tiles > 0 ? tiles : 1);
-    if (w->opx.ensure((size_t)(n_cigar + 1) * 4) || w->opy.ensure((size_t)(n_cigar + 1) * 4) || w->rend.ensure((size_t)(n + 1) * 8) ||
-        w->pmax.ensure((size_t)(n + 1) * 8) || w->rows32.ensure(Wz * NFEAT * 4) || w->dstats.ensure(Wz * 6 * 4) ||
-        w->nquirk.ensure(Wz * 4) || w->dci.ensure(Wz * 4) || w->tile_cov.ensure(Tz * 4) || w->tile_off.ensure(Tz * 8) ||
-        w->tile_cand.ensure(Tz * 4) || w->tile_coff.ensure(Tz * 8) || w->g_meta.ensure((size_t)G_POOL * 4) ||
-        w->g_read.ensure((size_t)G_POOL * 4) || w->g_qpos.ensure((size_t)G_POOL * 4) || w->g_cnt.ensure((size_t)G_POOL * 4) ||
-        w->g_next.ensure((size_t)G_POOL * 4) || w->counters.ensure(32) || w->matrix.ensure(Wz * NFEAT * 8) ||
-        w->major.ensure(Wz * 8) || w->stats.ensure(Wz * 6 * 4) || w->cand_cols.ensure(Wz * 8) || w->wstart.ensure(Wz * 8) ||
-        w->wbounds.ensure(Wz * 16) || w->cand_ok.ensure(Wz))
+    auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_plp"); };
+    if (grow(w->opx, (size_t)(n_cigar + 1) * 4) || grow(w->opy, (size_t)(n_cigar + 1) * 4) || grow(w->rend, (size_t)(n + 1) * 8) ||
+        grow(w->pmax, (size_t)(n + 1) * 8) || grow(w->rows32, Wz * NFEAT * 4) || grow(w->dstats, Wz * 6 * 4) ||
+        grow(w->nquirk, Wz * 4) || grow(w->dci, Wz * 4) || grow(w->tile_cov, Tz * 4) || grow(w->tile_off, Tz * 8) ||
+        grow(w->tile_cand, Tz * 4) || grow(w->tile_coff, Tz * 8) || grow(w->g_meta, (size_t)G_POOL * 4) ||
+        grow(w->g_read, (size_t)G_POOL * 4) || grow(w->g_qpos, (size_t)G_POOL * 4) || grow(w->g_cnt, (size_t)G_POOL * 4) ||
+        grow(w->g_next, (size_t)G_POOL * 4) || grow(w->counters, 32) || grow(w->matrix, Wz * NFEAT * 8) ||
+        grow(w->major, Wz * 8) || grow(w->stats, Wz * 6 * 4) || grow(w->cand_cols, Wz * 8) || grow(w->wstart, Wz * 8) ||
+        grow(w->wbounds, Wz * 16) || grow(w->cand_ok, Wz))
         return 1;
-    if (w->gvcf && (w->gv_ref.ensure(Wz * 8) || w->gv_tot.ensure(Wz * 8))) return 1;
+    if (w->gvcf && (grow(w->gv_ref, Wz * 8) || grow(w->gv_tot, Wz * 8))) return 1;
     w->alleles = params->alt_info != 0;
-    if (w->alleles && (w->al_meta.ensure((size_t)AL_CAP * 4) || w->al_read.ensure((size_t)AL_CAP * 4) || w->al_qpos.ensure((size_t)AL_CAP * 4) ||
-                       w->al_cnt.ensure((size_t)AL_CAP * 4) || w->al_off.ensure(Wz * 4) || w->al_n.ensure(Wz * 4) ||
-                       w->ins_last.ensure(Wz * 4)))
+    if (w->alleles && (grow(w->al_meta, (size_t)AL_CAP * 4) || grow(w->al_read, (size_t)AL_CAP * 4) || grow(w->al_qpos, (size_t)AL_CAP * 4) ||
+                       grow(w->al_cnt, (size_t)AL_CAP * 4) || grow(w->al_off, Wz * 4) || grow(w->al_n, Wz * 4) ||
+                       grow(w->ins_last, Wz * 4)))
         return 1;
     C3B_CUDA(cudaMemsetAsync(w->counters.p, 0, 32, s));
     if (w->gvcf && W > 0) {
@@ -758,7 +724,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         CountArgs A;
         A.R = R;
         A.opx_end = w->opx.as<int32_t>(); A.opy = w->opy.as<int32_t>(); A.rend = w->rend.as<int64_t>(); A.pmax = w->pmax.as<int64_t>();
-        A.start = start; A.end = end; A.ref = (const char *)dref; A.ref_start = ref_start; A.ref_len = ref_len > 0 ? ref_len : 0;
+        A.start = start; A.end = end; A.ref = dref; A.ref_start = ref_start; A.ref_len = ref_len > 0 ? ref_len : 0;
         A.prm = *params;
         A.rows32 = w->rows32.as<int32_t>(); A.dstats = w->dstats.as<int32_t>(); A.nquirk = w->nquirk.as<int32_t>();
         A.gv_ref = w->gvcf ? w->gv_ref.as<int64_t>() : nullptr; A.gv_tot = w->gvcf ? w->gv_tot.as<int64_t>() : nullptr;
@@ -893,12 +859,6 @@ int c3b_plp_last_ms(c3b_plp *w, float *ms, int *launches) {
 void c3b_plp_destroy(c3b_plp *w) {
     if (!w) return;
     cudaSetDevice(w->device);
-    DBuf *all[] = {&w->in_pos, &w->in_flag, &w->in_mapq, &w->in_coff, &w->in_cigar, &w->in_soff, &w->in_seq, &w->in_lq, &w->in_ref,
-                   &w->opx, &w->opy, &w->rend, &w->pmax, &w->rows32, &w->dstats, &w->nquirk, &w->dci, &w->tile_cov, &w->tile_off,
-                   &w->tile_cand, &w->tile_coff, &w->g_meta, &w->g_read, &w->g_qpos, &w->g_cnt, &w->g_next, &w->counters,
-                   &w->matrix, &w->major, &w->stats, &w->cand_cols, &w->wstart, &w->wbounds, &w->cand_ok, &w->gv_ref, &w->gv_tot,
-                   &w->al_meta, &w->al_read, &w->al_qpos, &w->al_cnt, &w->al_off, &w->al_n, &w->ins_last};
-    for (DBuf *b : all) b->release();
     if (w->ev0) cudaEventDestroy(w->ev0);
     if (w->ev1) cudaEventDestroy(w->ev1);
     if (w->host_counters) cudaFreeHost(w->host_counters);
