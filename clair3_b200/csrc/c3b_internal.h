@@ -136,6 +136,14 @@ int c3b_upload_records(Reads &R, C3bBuf (&b)[8], const c3b_bam_records *r, int64
            c3b_upload(b[7], r->l_qseq, n * 4, on_device, R.l_qseq, s, what);
 }
 
+#ifdef __CUDACC__
+// 4-bit nt16 code of base i of a packed sequence (bam_get_seq: two per byte, high nibble first) of lq bases; 0 ('=') outside it
+__device__ __forceinline__ int c3b_nib_at(const uint8_t *sq, int lq, long long i) {
+    if (i < 0 || i >= lq) return 0;
+    return (__ldg(sq + (i >> 1)) >> ((~i & 1) << 2)) & 15;
+}
+#endif
+
 // Entry n of an offset array of n + 1 entries that lives on the host or (on_device) the device; 0 for a null array.
 int c3b_last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s, int64_t *last);
 
@@ -361,3 +369,38 @@ int c3b_launch_pconv(const c3b_model *m, const PconvArgs &a, cudaStream_t s);
 int c3b_launch_ingest_fa_tc(const void *x, int dtype, int channels, int cpad, op_t *out, int64_t batch, int depth, const PlanarGeom &g1,
                             cudaStream_t s);
 int c3b_launch_spp_tc(const op_t *x, const PlanarGeom &g, op_t *out, int64_t batch, int c, int bp, cudaStream_t s);
+
+// ---- pileup feature counter: the all_alt_info text stage (plp_alt_text.cu), enqueued by c3b_plp_alt_text in plp_counts.cu ----
+struct PlpAltTextArgs {
+    // the count's results (device)
+    int64_t start, end, ref_start, ref_len, max_indel_length;
+    int64_t W;                          // end - start: the bound on the candidates the grids are sized from
+    const int64_t *n_cand;              // device counter
+    const int64_t *cand_cols, *major, *matrix;
+    const int32_t *stats;
+    const char *ref;
+    const int64_t *seq_off;             // the records where the count left them
+    const uint8_t *seq;
+    const int32_t *l_qseq;
+    const int32_t *al_off, *al_n, *ins_last;
+    const uint32_t *al_meta, *al_read, *al_qpos, *al_cnt;
+    int64_t al_cap;                     // records the al_* arrays and mate / hash / order hold
+    // scratch
+    int32_t *mate, *order;              // [al_cap]
+    uint32_t *hash;                     // [al_cap]
+    uint32_t *table;                    // [8 * W + 3 * al_cap] khash buckets
+    int32_t *n_ins, *n_del;             // [W]
+    int32_t *len_text, *len_dec;        // [W + 1]
+    int *status;                        // the stage's status word: non-zero = a candidate's text did not fit the stage's buffers
+    // outputs
+    char *text, *dec;
+    int64_t text_cap, dec_cap;
+    int64_t *text_off, *dec_off;        // [W + 1]
+    int64_t *totals;                    // device: n_text_bytes, n_decoder_bytes
+    uint8_t *ref_base;                  // [W]
+    int64_t *position;                  // [W]
+};
+int c3b_launch_plp_alt_text(const PlpAltTextArgs &a, cudaStream_t s, int *launches);
+// plp_counts.cu: exclusive scan of int32 counts into int64 offsets on one CTA, their sum to *total; over n entries, or over
+// *n_dev + 1 of them when n_dev is given and that is fewer
+int c3b_launch_plp_scan(const int32_t *cnt, int64_t *off, int n, const int64_t *n_dev, int64_t *total, cudaStream_t s);

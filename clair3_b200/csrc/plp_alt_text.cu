@@ -1,0 +1,319 @@
+// plp_alt_text.cu - the pileup counter's all_alt_info text on the GPU (include/clair3_b200_pileup.h: c3b_plp_alt_text).
+//
+// Reference: the text loop of calculate_clair3_pileup(), HKU-BAL/Clair3 src/clair3_pileup.c:391-450, one string per candidate:
+//     "<pos+1>-<depth>-<REF>-X<b> n D<ref bases> n I<REF><inserted bases> n R<REF> n "
+// clair3_b200/pileup_counts.py: format_alt_info / khash_iteration_order state the same on the host and are what the tests hold
+// these kernels to.  Candidates are independent and their strings have data-dependent length, so the stage is
+//
+//   T1 plp_text_measure   one WARP per candidate over the column's allele records (K3's export, [al_off, al_off + al_n)):
+//                         lanes over records merge the two strands (a record's twin on the other strand: same kind, length and,
+//                         for insertions, the same bases through the representative reads' packed sequences), hash the merged
+//                         insertion strings (X31) and rank-sort the deletions by length and the insertions by first read; lane 0
+//                         then replays klib's khash (src/khash.h) over the insertions - power-of-two tables from 4, triangular
+//                         probing, growth at 0.77 load at the start of a put, kh_resize's in-place kick-out rehash, one more
+//                         growth when a put of a present string follows the last new one - and leaves the bucket order; it then
+//                         walks the string once with a counting sink: the bytes of the full text and of the decoder form.
+//   T2 plp_scan_tiles     (plp_counts.cu) the two exclusive scans over n_cand + 1 lengths: per-candidate offsets and the totals.
+//   T3 plp_text_write     one THREAD per candidate walks the same string with a writing sink.
+//
+// Everything a column needs lives in global scratch addressed by its own record range (mate / hash / order) or by that range and
+// its candidate index (the khash table: 8 buckets per candidate, or up to 3 per record - a table of n > 8 buckets holds at least
+// 0.77 n / 2 strings), so a column of thousands of distinct alleles needs no capacity of its own.  The grids are sized from the
+// region's width and read n_cand on the device.  Same records, same bytes, whatever the launch shape: nothing here is atomic but
+// the status word.
+#include <limits.h>
+
+#include "c3b_internal.h"
+
+namespace {
+
+__constant__ char NT16[17] = "=ACMGRSVTWYHKDBN";          // htslib seq_nt16_str
+constexpr int FETCH_EXPAND = 1000;                        // mpileup_expand_reference_region, src/clair3_pileup.h:63
+constexpr int32_t NOT_FIRST = -2;                         // mate[]: the record's twin comes earlier in the list
+constexpr uint32_t T_VAL = 0xffffffu, T_OCC = 1u << 24, T_TAKEN = 1u << 25;   // khash bucket: record + 1 | old flag | new flag
+
+struct CountSink {
+    long long n = 0;
+    __device__ __forceinline__ void put(char) { ++n; }
+};
+struct WriteSink {              // writes inside [p, p + lim) only: lim is the length the measure pass found
+    char *p;
+    long long lim, n = 0;
+    __device__ __forceinline__ void put(char c) { if (n < lim) p[n] = c; ++n; }
+};
+
+template <class S> struct TextOut {
+    S full, dec;                // the reference's string, and "<depth>-<alt>" as the decoder takes it
+    bool cut = false;           // the alt field of rstrip().split("-") ends at the first '-' of the alt text
+    long long n_alt = 0;
+    __device__ __forceinline__ void head(char c, bool both) {
+        full.put(c);
+        if (both) dec.put(c);
+    }
+    __device__ __forceinline__ void alt(char c) {
+        full.put(c);
+        ++n_alt;
+        if (c == '-') cut = true;
+        if (!cut) dec.put(c);
+    }
+    enum Where { HEAD_FULL, HEAD_BOTH, ALT };
+    __device__ void num(long long v, Where w) {             // %d of a non-negative count, without a digit buffer
+        unsigned long long u = (unsigned long long)v, p = 1;
+        while (u / p >= 10) p *= 10;
+        for (; p; p /= 10) {
+            const char c = (char)('0' + (u / p) % 10);
+            if (w == ALT) alt(c); else head(c, w == HEAD_BOTH);
+        }
+    }
+};
+
+// upper_base of the reference base under a column, 'N' outside the supplied reference
+__device__ __forceinline__ int ref_base_at(const PlpAltTextArgs &A, int64_t pos) {
+    const int64_t off = pos - A.ref_start;
+    const int rb = (off >= 0 && off < A.ref_len) ? (int)(unsigned char)A.ref[off] : 'N';
+    return rb >= 'a' && rb <= 'z' ? rb - 32 : rb;
+}
+
+__device__ __forceinline__ int64_t first_read(const PlpAltTextArgs &A, int i) {
+    const int m = A.mate[i];
+    const uint32_t r = A.al_read[i];
+    return (int64_t)(m >= 0 && A.al_read[m] < r ? A.al_read[m] : r);
+}
+__device__ __forceinline__ long long merged_count(const PlpAltTextArgs &A, int i) {
+    const int m = A.mate[i];
+    return (long long)A.al_cnt[i] + (m >= 0 ? (long long)A.al_cnt[m] : 0);
+}
+
+// One candidate's string, src/clair3_pileup.c:391-450, from the merged and ordered allele records T1 left in `order`.
+template <class S> __device__ void plp_text_emit(const PlpAltTextArgs &A, const int64_t j, TextOut<S> &o) {
+    const int64_t ci = A.cand_cols[j], pos = A.major[ci], off = pos - A.ref_start;
+    const int a0 = A.al_off[pos - A.start], ni = A.n_ins[j], nd = A.n_del[j];
+    const int rb = ref_base_at(A, pos);
+    const int bi = rb - 'A';
+    const int rf = bi == 2 ? 1 : bi == 6 ? 2 : bi == 19 ? 3 : 0;          // base2index, src/clair3_pileup.h:57-62
+    const long long depth = A.stats[ci * 6];
+    long long ref_depth = A.stats[ci * 6 + 1];
+    typedef TextOut<S> O;
+    o.num(pos + 1, O::HEAD_FULL); o.head('-', false);                     // "<pos+1>-<depth>-<REF>-" / "<depth>-"
+    o.num(depth, O::HEAD_BOTH); o.head('-', true);
+    o.head((char)rb, false); o.head('-', false);
+    const int64_t *row = A.matrix + ci * 18;
+    for (int i = 0; i < 4; ++i) {
+        const long long alt_sum = (long long)row[i] + (long long)row[i + 9];
+        if (alt_sum > 0 && i != rf) {
+            o.alt('X'); o.alt("ACGT"[i]); o.alt(' '); o.num(alt_sum, O::ALT); o.alt(' ');
+        }
+    }
+    for (int k = 0; k < nd; ++k) {                                        // deletions, ascending length
+        const int i = A.order[a0 + ni + k];
+        const long long len = (long long)(A.al_meta[i] & 0x3fffffffu), d = merged_count(A, i);
+        ref_depth -= d;
+        if (d > 0 && len <= A.max_indel_length) {
+            int64_t stop = off + 1 + len;                                 // the reference's FASTA fetch ends at end + 1000
+            if (stop > A.end + FETCH_EXPAND + 1 - A.ref_start) stop = A.end + FETCH_EXPAND + 1 - A.ref_start;
+            if (stop > A.ref_len) stop = A.ref_len;
+            o.alt('D');
+            for (int64_t q = off + 1; q < stop; ++q) {
+                const char c = A.ref[q];
+                if (c == 0) break;
+                o.alt(c);
+            }
+            o.alt(' '); o.num(d, O::ALT); o.alt(' ');
+        }
+    }
+    for (int k = 0; k < ni; ++k) {                                        // insertions, khash bucket order
+        const int i = A.order[a0 + k];
+        const long long len = (long long)(A.al_meta[i] & 0x3fffffffu), v = merged_count(A, i);
+        ref_depth -= v;
+        if (len <= A.max_indel_length) {
+            const uint32_t r = A.al_read[i];
+            const uint8_t *sq = A.seq + A.seq_off[r];
+            const int lq = A.l_qseq[r];
+            const long long q0 = (long long)A.al_qpos[i];
+            o.alt('I'); o.alt((char)rb);
+            for (long long q = 0; q < len; ++q) o.alt(NT16[c3b_nib_at(sq, lq, q0 + q)]);
+            o.alt(' '); o.num(v, O::ALT); o.alt(' ');
+        }
+    }
+    if (ref_depth > 0) {
+        o.alt('R'); o.alt((char)rb); o.alt(' '); o.num(ref_depth, O::ALT); o.alt(' ');
+    }
+}
+
+// kh_resize (src/khash.h:246-306) for an insert-only table of n buckets holding `size` strings; returns the new bucket count, 0
+// when the candidate's scratch cannot hold it.
+__device__ int khash_grow(const PlpAltTextArgs &A, uint32_t *slot, const int n, const int avail) {
+    const int nn = n < 4 ? 4 : 2 * n;
+    if (nn > avail) return 0;
+    for (int b = 0; b < nn; ++b) {
+        const uint32_t v = b < n ? (slot[b] & T_VAL) : 0u;
+        slot[b] = v | (v ? T_OCC : 0u);
+    }
+    const uint32_t mask = (uint32_t)nn - 1u;
+    for (int b = 0; b < n; ++b) {
+        if (!(slot[b] & T_OCC)) continue;
+        uint32_t cur = slot[b] & T_VAL;
+        slot[b] &= T_TAKEN;                                   // the bucket is free in the old table; its new flag stays
+        for (;;) {                                            // kick-out: the evicted string is placed next
+            uint32_t i = A.hash[cur - 1] & mask, step = 0;
+            while (slot[i] & T_TAKEN) i = (i + (++step)) & mask;
+            const uint32_t e = slot[i];
+            slot[i] = cur | T_TAKEN;
+            if (!(e & T_OCC)) break;
+            cur = e & T_VAL;
+        }
+    }
+    return nn;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- T1
+__global__ void __launch_bounds__(256) plp_text_measure_kernel(PlpAltTextArgs A) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const int64_t n_cand = *A.n_cand;
+    for (int64_t j = warp; j <= n_cand; j += nwarps) {
+        if (j == n_cand) {                                    // the scans run over n_cand + 1 entries: the last offset is the total
+            if (lane == 0) A.len_text[j] = A.len_dec[j] = 0;
+            continue;
+        }
+        const int64_t ci = A.cand_cols[j], pos = A.major[ci];
+        const int a0 = A.al_off[pos - A.start];
+        int n = A.al_n[pos - A.start];
+        bool fits = (int64_t)a0 + n <= A.al_cap;              // mate / hash / order / table hold al_cap records
+        if (!fits) n = 0;
+        // a record's twin on the other strand (K3 keeps each strand's alleles distinct, so there is at most one)
+        int ni = 0, nd = 0;
+        for (int i = a0 + lane; i < a0 + n; i += 32) {
+            const uint32_t meta = A.al_meta[i];
+            const long long len = (long long)(meta & 0x3fffffffu);
+            const bool ins = meta >> 31;
+            const uint8_t *sq = nullptr;
+            int lq = 0;
+            long long q0 = 0;
+            if (ins) {
+                sq = A.seq + A.seq_off[A.al_read[i]];
+                lq = A.l_qseq[A.al_read[i]];
+                q0 = (long long)A.al_qpos[i];
+            }
+            int m = -1;
+            for (int k = a0; k < a0 + n && m == -1; ++k) {
+                if (A.al_meta[k] != (meta ^ (1u << 30))) continue;
+                bool same = true;
+                if (ins) {
+                    const uint8_t *s2 = A.seq + A.seq_off[A.al_read[k]];
+                    const int lq2 = A.l_qseq[A.al_read[k]];
+                    const long long q2 = (long long)A.al_qpos[k];
+                    for (long long q = 0; q < len; ++q)
+                        if (c3b_nib_at(sq, lq, q0 + q) != c3b_nib_at(s2, lq2, q2 + q)) { same = false; break; }
+                }
+                if (same) m = k < i ? NOT_FIRST : k;
+            }
+            A.mate[i] = m;
+            if (m != NOT_FIRST) {
+                if (ins) {                                    // __ac_X31_hash_string, src/khash.h:395-400
+                    uint32_t h = len ? (uint32_t)NT16[c3b_nib_at(sq, lq, q0)] : 0u;
+                    for (long long q = 1; q < len; ++q) h = h * 31u + (uint32_t)NT16[c3b_nib_at(sq, lq, q0 + q)];
+                    A.hash[i] = h;
+                    ++ni;
+                } else {
+                    ++nd;
+                }
+            }
+        }
+#pragma unroll
+        for (int d = 16; d; d >>= 1) {
+            ni += __shfl_xor_sync(0xffffffffu, ni, d);
+            nd += __shfl_xor_sync(0xffffffffu, nd, d);
+        }
+        __syncwarp();
+        // rank sort: deletions by length, insertions by first occurrence over both strands (the reference's insertion order)
+        for (int i = a0 + lane; i < a0 + n; i += 32) {
+            if (A.mate[i] == NOT_FIRST) continue;
+            const uint32_t meta = A.al_meta[i];
+            const bool ins = meta >> 31;
+            const int64_t key = ins ? first_read(A, i) : (int64_t)(meta & 0x3fffffffu);
+            int rank = 0;
+            for (int k = a0; k < a0 + n; ++k) {
+                if (A.mate[k] == NOT_FIRST || (A.al_meta[k] >> 31) != (meta >> 31)) continue;
+                const int64_t kk = ins ? first_read(A, k) : (int64_t)(A.al_meta[k] & 0x3fffffffu);
+                rank += (kk < key || (kk == key && k < i)) ? 1 : 0;
+            }
+            A.order[a0 + (ins ? 0 : ni) + rank] = i;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            if (ni > 0) {                                     // the khash replay: a short serial walk
+                uint32_t *slot = A.table + 8 * j;
+                int avail = 8;
+                if (ni > 3) { slot = A.table + 8 * A.W + 3 * (int64_t)a0; avail = 3 * n; }
+                int nb = 0, size = 0, upper = 0;
+                for (int k = 0; k < ni && fits; ++k) {
+                    if (size >= upper) {                      // kh_put grows a full table before it looks the key up
+                        nb = khash_grow(A, slot, nb, avail);
+                        if (!nb) { fits = false; break; }
+                        upper = (int)(nb * 0.77 + 0.5);
+                    }
+                    const int rec = A.order[a0 + k];
+                    const uint32_t mask = (uint32_t)nb - 1u;
+                    uint32_t i = A.hash[rec] & mask, step = 0;
+                    while (slot[i] & T_VAL) i = (i + (++step)) & mask;
+                    slot[i] = (uint32_t)rec + 1u;
+                    ++size;
+                }
+                // a read after the last new string put a present one again: that put still grows a full table first
+                if (fits && size >= upper && (int64_t)A.ins_last[pos - A.start] > first_read(A, A.order[a0 + ni - 1])) {
+                    nb = khash_grow(A, slot, nb, avail);
+                    if (!nb) fits = false;
+                }
+                if (fits) {
+                    int k = 0;
+                    for (int b = 0; b < nb; ++b)
+                        if (slot[b] & T_VAL) A.order[a0 + k++] = (int)(slot[b] & T_VAL) - 1;
+                }
+            }
+            if (!fits) { atomicOr(A.status, 1); ni = nd = 0; }
+            A.n_ins[j] = ni;
+            A.n_del[j] = nd;
+            TextOut<CountSink> o;
+            plp_text_emit(A, j, o);
+            if (!o.cut && o.n_alt > 0) --o.dec.n;             // rstrip(): the alt text ends in one space
+            if (!fits || o.full.n > INT_MAX || o.dec.n > INT_MAX) {
+                atomicOr(A.status, 1);
+                o.full.n = o.dec.n = 0;
+            }
+            A.len_text[j] = (int32_t)o.full.n;
+            A.len_dec[j] = (int32_t)o.dec.n;
+            A.ref_base[j] = (uint8_t)ref_base_at(A, pos);
+            A.position[j] = pos + 1;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------- T3
+__global__ void __launch_bounds__(128) plp_text_write_kernel(PlpAltTextArgs A) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= *A.n_cand) return;
+    const int64_t t0 = A.text_off[j], t1 = A.text_off[j + 1], d0 = A.dec_off[j], d1 = A.dec_off[j + 1];
+    if (t1 > A.text_cap || d1 > A.dec_cap) { atomicOr(A.status, 1); return; }
+    TextOut<WriteSink> o;
+    o.full.p = A.text + t0; o.full.lim = t1 - t0;
+    o.dec.p = A.dec + d0; o.dec.lim = d1 - d0;
+    if (t1 > t0) plp_text_emit(A, j, o);
+}
+
+}  // namespace
+
+int c3b_launch_plp_alt_text(const PlpAltTextArgs &a, cudaStream_t s, int *launches) {
+    if (a.al_cap >= (int64_t)T_VAL) { c3b_set_error("c3b_plp_alt_text: %lld allele records exceed the khash replay's 24-bit record index", (long long)a.al_cap); return 1; }
+    int64_t blocks = ((a.W + 1) * 32 + 255) / 256;
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    plp_text_measure_kernel<<<(unsigned)blocks, 256, 0, s>>>(a);
+    if (c3b_launch_plp_scan(a.len_text, a.text_off, (int)(a.W + 1), a.n_cand, a.totals, s) ||
+        c3b_launch_plp_scan(a.len_dec, a.dec_off, (int)(a.W + 1), a.n_cand, a.totals + 1, s))
+        return 1;
+    plp_text_write_kernel<<<(unsigned)((a.W + 127) / 128), 128, 0, s>>>(a);
+    C3B_CUDA(cudaGetLastError());
+    *launches = 4;
+    return 0;
+}

@@ -59,10 +59,6 @@ struct DevReads {
 
 __device__ __forceinline__ bool ref_cons(uint32_t op) { return (0x18Du >> op) & 1u; }   // M D N = X
 __device__ __forceinline__ bool qry_cons(uint32_t op) { return (0x193u >> op) & 1u; }   // M I S = X
-__device__ __forceinline__ int nib_at(const uint8_t *sq, int lq, long long i) {
-    if (i < 0 || i >= lq) return 0;
-    return (__ldg(sq + (i >> 1)) >> ((~i & 1) << 2)) & 15;
-}
 
 // ---------------------------------------------------------------------------------------------------------------- K1
 __global__ void plp_scan_reads_kernel(DevReads R, int min_mq, int32_t *__restrict__ opx_end, int32_t *__restrict__ opy,
@@ -202,7 +198,7 @@ __device__ __forceinline__ void plp_event(const CountArgs &A, const Pool &P, int
             const uint8_t *s2 = A.R.seq + __ldg(A.R.seq_off + rr);
             const int lq2 = __ldg(A.R.l_qseq + rr);
             for (long long j = 0; j < len; ++j)
-                if (nib_at(sq, lq, q0 + j) != nib_at(s2, lq2, rq + j)) { same = false; break; }
+                if (c3b_nib_at(sq, lq, q0 + j) != c3b_nib_at(s2, lq2, rq + j)) { same = false; break; }
         }
         if (same) { c = (int)(NODE(cnt, i) += 1u); found = true; break; }
     }
@@ -346,7 +342,7 @@ __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
             const uint32_t op = cw & 15u;
             int nb = 0;
             if (op != 2u && op != 3u)
-                nb = nib_at(A.R.seq + __ldg(A.R.seq_off + r), __ldg(A.R.l_qseq + r), (long long)y0 + (off - (xend - (int)(cw >> 4))));
+                nb = c3b_nib_at(A.R.seq + __ldg(A.R.seq_off + r), __ldg(A.R.l_qseq + r), (long long)y0 + (off - (xend - (int)(cw >> 4))));
             if (plp_visit(A, cnt, tid, cb, nc, off, k, cw, xend, y0, rev, nb, depth, e_meta, e_q0)) {
                 plp_event(A, P, cnt, tid, e_meta, e_q0, (uint32_t)r, head);
                 if (e_meta >> 31) ins_last = (int)r;
@@ -436,8 +432,11 @@ __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------- K4 / K7
-__global__ void plp_scan_tiles_kernel(const int32_t *__restrict__ cnt, int64_t *__restrict__ off, int n, int64_t *total) {
+// n_dev (optional): the scan stops after *n_dev + 1 entries when that is fewer than n
+__global__ void plp_scan_tiles_kernel(const int32_t *__restrict__ cnt, int64_t *__restrict__ off, int n, const int64_t *n_dev,
+                                      int64_t *total) {
     __shared__ long long wsum[32];
+    if (n_dev && *n_dev + 1 < n) n = (int)(*n_dev + 1);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     long long carry = 0;
     for (int base = 0; base < n; base += 1024) {
@@ -616,7 +615,7 @@ struct c3b_plp {
     C3bBuf opx, opy, rend, pmax, rows32, dstats, nquirk, dci, tile_cov, tile_off, tile_cand, tile_coff;
     C3bBuf g_meta, g_read, g_qpos, g_cnt, g_next;
     C3bBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n, ins_last;   // allele export (params.alt_info)
-    C3bBuf counters;    // int64 n_cols, int64 n_cand, int g_used, int status
+    C3bBuf counters;    // int64 n_cols, int64 n_cand, int g_used, int status, int al_used, int text_status, int64 n_text_bytes, int64 n_decoder_bytes
     // outputs
     C3bBuf matrix, major, stats, cand_cols, wstart, wbounds, cand_ok, gv_ref, gv_tot;
     int64_t W = 0;
@@ -624,9 +623,26 @@ struct c3b_plp {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     int launches = 0;
-    int64_t *host_counters = nullptr;   // pinned: n_cols, n_cand, (g_used | status << 32)
+    int64_t *host_counters = nullptr;   // pinned copy of `counters`
     int64_t n_cols = -1, n_cand = -1;
+    // the text stage (c3b_plp_alt_text): where the count left its inputs, scratch, outputs
+    DevReads R;
+    const char *dref = nullptr;
+    int64_t start = 0, end = 0, ref_start = 0, ref_len = 0, n_cigar = 0, n_seq = 0;
+    C3bBuf tx_mate, tx_hash, tx_order, tx_table, tx_nins, tx_ndel, tx_len_text, tx_len_dec;
+    C3bBuf text, dec, text_off, dec_off, ref_base, position;
+    bool texted = false;
+    cudaEvent_t ev2 = nullptr, ev3 = nullptr;
+    int text_launches = 0;
 };
+
+constexpr int N_COUNTERS = 6;
+
+int c3b_launch_plp_scan(const int32_t *cnt, int64_t *off, int n, const int64_t *n_dev, int64_t *total, cudaStream_t s) {
+    plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(cnt, off, n, n_dev, total);
+    C3B_CUDA(cudaGetLastError());
+    return 0;
+}
 
 extern "C" {
 
@@ -637,7 +653,8 @@ int c3b_plp_create(c3b_plp **out, int device_ordinal) {
     c3b_plp *w = new c3b_plp();
     w->device = device_ordinal;
     if (cudaEventCreate(&w->ev0) != cudaSuccess || cudaEventCreate(&w->ev1) != cudaSuccess ||
-        cudaMallocHost((void **)&w->host_counters, 4 * sizeof(int64_t)) != cudaSuccess) {
+        cudaEventCreate(&w->ev2) != cudaSuccess || cudaEventCreate(&w->ev3) != cudaSuccess ||
+        cudaMallocHost((void **)&w->host_counters, N_COUNTERS * sizeof(int64_t)) != cudaSuccess) {
         c3b_set_error("c3b_plp_create: event / pinned allocation failed");
         c3b_plp_destroy(w);
         return 1;
@@ -661,7 +678,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     C3B_CUDA(cudaSetDevice(w->device));
     cudaStream_t s = (cudaStream_t)cuda_stream;
     w->stream = s;
-    w->counted = false;
+    w->counted = w->texted = false;
     w->n_cols = w->n_cand = -1;
     const int64_t W = end - start;
     w->W = W;
@@ -681,6 +698,10 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     }
     const char *dref = nullptr;
     if (c3b_upload(w->in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, dref, s, "c3b_plp")) return 1;
+    w->R = R;
+    w->dref = dref;
+    w->start = start; w->end = end; w->ref_start = ref_start; w->ref_len = ref_len > 0 ? ref_len : 0;
+    w->n_cigar = n_cigar; w->n_seq = n_seq;
 
     // scratch and outputs
     const size_t Wz = (size_t)(W > 0 ? W : 1), Tz = (size_t)(tiles > 0 ? tiles : 1);
@@ -690,7 +711,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         grow(w->nquirk, Wz * 4) || grow(w->dci, Wz * 4) || grow(w->tile_cov, Tz * 4) || grow(w->tile_off, Tz * 8) ||
         grow(w->tile_cand, Tz * 4) || grow(w->tile_coff, Tz * 8) || grow(w->g_meta, (size_t)G_POOL * 4) ||
         grow(w->g_read, (size_t)G_POOL * 4) || grow(w->g_qpos, (size_t)G_POOL * 4) || grow(w->g_cnt, (size_t)G_POOL * 4) ||
-        grow(w->g_next, (size_t)G_POOL * 4) || grow(w->counters, 32) || grow(w->matrix, Wz * NFEAT * 8) ||
+        grow(w->g_next, (size_t)G_POOL * 4) || grow(w->counters, N_COUNTERS * 8) || grow(w->matrix, Wz * NFEAT * 8) ||
         grow(w->major, Wz * 8) || grow(w->stats, Wz * 6 * 4) || grow(w->cand_cols, Wz * 8) || grow(w->wstart, Wz * 8) ||
         grow(w->wbounds, Wz * 16) || grow(w->cand_ok, Wz))
         return 1;
@@ -700,7 +721,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
                        grow(w->al_cnt, (size_t)AL_CAP * 4) || grow(w->al_off, Wz * 4) || grow(w->al_n, Wz * 4) ||
                        grow(w->ins_last, Wz * 4)))
         return 1;
-    C3B_CUDA(cudaMemsetAsync(w->counters.p, 0, 32, s));
+    C3B_CUDA(cudaMemsetAsync(w->counters.p, 0, N_COUNTERS * 8, s));
     if (w->gvcf && W > 0) {
         C3B_CUDA(cudaMemsetAsync(w->gv_ref.p, 0, (size_t)W * 8, s));
         C3B_CUDA(cudaMemsetAsync(w->gv_tot.p, 0, (size_t)W * 8, s));
@@ -736,7 +757,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         A.ins_last = w->ins_last.as<int32_t>(); A.al_used = al_used; A.al_cap = AL_CAP;
         const size_t smem = (size_t)NCNT * TILE * 4 + (size_t)NP * 20;
         plp_count_tile_kernel<<<tiles, TILE, smem, s>>>(A);
-        plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(w->tile_cov.as<int32_t>(), w->tile_off.as<int64_t>(), tiles, n_cols_dev);
+        plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(w->tile_cov.as<int32_t>(), w->tile_off.as<int64_t>(), tiles, nullptr, n_cols_dev);
         EmitArgs E;
         E.start = start; E.end = end; E.call_ht = params->call_ht;
         E.rows32 = w->rows32.as<int32_t>(); E.dstats = w->dstats.as<int32_t>(); E.tile_off = w->tile_off.as<int64_t>();
@@ -745,7 +766,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         plp_emit_kernel<<<tiles, TILE, 0, s>>>(E);
         plp_quirk_kernel<<<(unsigned)((W + 255) / 256), 256, 0, s>>>(n_cols_dev, w->major.as<int64_t>(), w->nquirk.as<int32_t>(), start,
                                                                       w->matrix.as<int64_t>(), w->stats.as<int32_t>());
-        plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(w->tile_cand.as<int32_t>(), w->tile_coff.as<int64_t>(), tiles, n_cand_dev);
+        plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(w->tile_cand.as<int32_t>(), w->tile_coff.as<int64_t>(), tiles, nullptr, n_cand_dev);
         CandArgs C;
         C.start = start; C.end = end; C.n_cols_dev = n_cols_dev; C.dci = w->dci.as<int32_t>(); C.stats = w->stats.as<int32_t>();
         C.major = w->major.as<int64_t>(); C.tile_coff = w->tile_coff.as<int64_t>(); C.cand_cols = w->cand_cols.as<int64_t>();
@@ -845,6 +866,114 @@ int c3b_plp_window_bounds(c3b_plp *w, int64_t *bounds, const int64_t **device_bo
     return 0;
 }
 
+int c3b_plp_alt_text(c3b_plp *w, int64_t max_indel_length) {
+    if (!w || !w->counted) { c3b_set_error("c3b_plp_alt_text: no c3b_plp_count has been issued"); return 1; }
+    if (!w->alleles) { c3b_set_error("c3b_plp_alt_text: the count ran without params.alt_info"); return 1; }
+    C3B_CUDA(cudaSetDevice(w->device));
+    cudaStream_t s = w->stream;
+    const int64_t W = w->W;
+    // every allele record comes from one insertion / deletion operation of one read
+    const int64_t cap = w->n_cigar < AL_CAP ? (w->n_cigar > 0 ? w->n_cigar : 1) : AL_CAP;
+    // bytes: head, SNP and R fields per candidate; key, count and separators per record; the inserted bases are query bases; a
+    // printed deletion shows at most max_indel_length reference bases
+    const int64_t del_len = max_indel_length < 0 ? 0 : (max_indel_length < w->ref_len ? max_indel_length : w->ref_len);
+    const int64_t del_bytes = cap * del_len < (1ll << 28) ? cap * del_len : (1ll << 28);
+    const int64_t text_cap = 160 * (W + 1) + 48 * cap + 2 * w->n_seq + del_bytes;
+    const size_t Wz = (size_t)W + 1;
+    auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_plp"); };
+    if (grow(w->tx_mate, (size_t)cap * 4) || grow(w->tx_hash, (size_t)cap * 4) || grow(w->tx_order, (size_t)cap * 4) ||
+        grow(w->tx_table, (8 * Wz + 3 * (size_t)cap) * 4) || grow(w->tx_nins, Wz * 4) || grow(w->tx_ndel, Wz * 4) ||
+        grow(w->tx_len_text, Wz * 4) || grow(w->tx_len_dec, Wz * 4) || grow(w->text, (size_t)text_cap) ||
+        grow(w->dec, (size_t)text_cap) || grow(w->text_off, Wz * 8) || grow(w->dec_off, Wz * 8) || grow(w->ref_base, Wz) ||
+        grow(w->position, Wz * 8))
+        return 1;
+    w->texted = false;
+    w->n_cols = w->n_cand = -1;           // the status word and the totals travel with the next c3b_plp_sizes
+    w->text_launches = 0;
+    int64_t *cnt = w->counters.as<int64_t>();
+    int *text_status = reinterpret_cast<int *>(cnt + 3) + 1;       // the stage's own word: an earlier stage's overflow is not this one's
+    C3B_CUDA(cudaMemsetAsync(text_status, 0, sizeof(int), s));
+    C3B_CUDA(cudaEventRecord(w->ev2, s));
+    if (W > 0) {
+        PlpAltTextArgs A;
+        A.start = w->start; A.end = w->end; A.ref_start = w->ref_start; A.ref_len = w->ref_len; A.max_indel_length = max_indel_length;
+        A.W = W;
+        A.n_cand = cnt + 1;
+        A.cand_cols = w->cand_cols.as<int64_t>(); A.major = w->major.as<int64_t>(); A.matrix = w->matrix.as<int64_t>();
+        A.stats = w->stats.as<int32_t>(); A.ref = w->dref;
+        A.seq_off = w->R.seq_off; A.seq = w->R.seq; A.l_qseq = w->R.l_qseq;
+        A.al_off = w->al_off.as<int32_t>(); A.al_n = w->al_n.as<int32_t>(); A.ins_last = w->ins_last.as<int32_t>();
+        A.al_meta = w->al_meta.as<uint32_t>(); A.al_read = w->al_read.as<uint32_t>(); A.al_qpos = w->al_qpos.as<uint32_t>();
+        A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_cap = cap;
+        A.mate = w->tx_mate.as<int32_t>(); A.order = w->tx_order.as<int32_t>(); A.hash = w->tx_hash.as<uint32_t>();
+        A.table = w->tx_table.as<uint32_t>(); A.n_ins = w->tx_nins.as<int32_t>(); A.n_del = w->tx_ndel.as<int32_t>();
+        A.len_text = w->tx_len_text.as<int32_t>(); A.len_dec = w->tx_len_dec.as<int32_t>();
+        A.status = text_status;
+        A.text = w->text.as<char>(); A.dec = w->dec.as<char>(); A.text_cap = A.dec_cap = text_cap;
+        A.text_off = w->text_off.as<int64_t>(); A.dec_off = w->dec_off.as<int64_t>(); A.totals = cnt + 4;
+        A.ref_base = w->ref_base.as<uint8_t>(); A.position = w->position.as<int64_t>();
+        if (c3b_launch_plp_alt_text(A, s, &w->text_launches)) return 1;
+    } else {
+        C3B_CUDA(cudaMemsetAsync(w->text_off.p, 0, 8, s));
+        C3B_CUDA(cudaMemsetAsync(w->dec_off.p, 0, 8, s));
+    }
+    C3B_CUDA(cudaEventRecord(w->ev3, s));
+    C3B_CUDA(cudaMemcpyAsync(w->host_counters, w->counters.p, N_COUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    w->texted = true;
+    return 0;
+}
+
+int c3b_plp_alt_text_sizes(c3b_plp *w, int64_t *n_text_bytes, int64_t *n_decoder_bytes) {
+    if (!w || !w->texted) { c3b_set_error("c3b_plp_alt_text_sizes: no c3b_plp_alt_text has been issued"); return 1; }
+    if (w->n_cols < 0 && c3b_plp_sizes(w, nullptr, nullptr)) return 1;
+    if ((int)(w->host_counters[3] >> 32) != 0) {
+        c3b_set_error("c3b_plp_alt_text: the all_alt_info text outgrew its buffers; count a smaller region or lower max_indel_length");
+        return 1;
+    }
+    if (n_text_bytes) *n_text_bytes = w->host_counters[4];
+    if (n_decoder_bytes) *n_decoder_bytes = w->host_counters[5];
+    return 0;
+}
+
+int c3b_plp_fetch_alt_text(c3b_plp *w, char *text, int64_t *text_off, char *decoder, int64_t *decoder_off, uint8_t *ref_base,
+                           int64_t *position) {
+    int64_t nt = 0, nd = 0;
+    if (c3b_plp_alt_text_sizes(w, &nt, &nd)) return 1;
+    cudaStream_t s = w->stream;
+    const size_t nk = (size_t)w->n_cand;
+    if (text && nt) C3B_CUDA(cudaMemcpyAsync(text, w->text.p, (size_t)nt, cudaMemcpyDeviceToHost, s));
+    if (text_off) C3B_CUDA(cudaMemcpyAsync(text_off, w->text_off.p, (nk + 1) * 8, cudaMemcpyDeviceToHost, s));
+    if (decoder && nd) C3B_CUDA(cudaMemcpyAsync(decoder, w->dec.p, (size_t)nd, cudaMemcpyDeviceToHost, s));
+    if (decoder_off) C3B_CUDA(cudaMemcpyAsync(decoder_off, w->dec_off.p, (nk + 1) * 8, cudaMemcpyDeviceToHost, s));
+    if (ref_base && nk) C3B_CUDA(cudaMemcpyAsync(ref_base, w->ref_base.p, nk, cudaMemcpyDeviceToHost, s));
+    if (position && nk) C3B_CUDA(cudaMemcpyAsync(position, w->position.p, nk * 8, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaStreamSynchronize(s));
+    return 0;
+}
+
+int c3b_plp_alt_text_device(c3b_plp *w, const char **text, const int64_t **text_off, const char **decoder,
+                            const int64_t **decoder_off, const uint8_t **ref_base, const int64_t **position) {
+    if (!w || !w->texted) { c3b_set_error("c3b_plp_alt_text_device: no c3b_plp_alt_text has been issued"); return 1; }
+    if (text) *text = w->text.as<char>();
+    if (text_off) *text_off = w->text_off.as<int64_t>();
+    if (decoder) *decoder = w->dec.as<char>();
+    if (decoder_off) *decoder_off = w->dec_off.as<int64_t>();
+    if (ref_base) *ref_base = w->ref_base.as<uint8_t>();
+    if (position) *position = w->position.as<int64_t>();
+    return 0;
+}
+
+int c3b_plp_alt_text_last_ms(c3b_plp *w, float *ms, int *launches) {
+    if (!w || !w->texted) { c3b_set_error("c3b_plp_alt_text_last_ms: no c3b_plp_alt_text has been issued"); return 1; }
+    C3B_CUDA(cudaSetDevice(w->device));
+    C3B_CUDA(cudaEventSynchronize(w->ev3));
+    float t = 0.f;
+    C3B_CUDA(cudaEventElapsedTime(&t, w->ev2, w->ev3));
+    if (ms) *ms = t;
+    if (launches) *launches = w->text_launches;
+    return 0;
+}
+
 int c3b_plp_last_ms(c3b_plp *w, float *ms, int *launches) {
     if (!w || !w->counted) { c3b_set_error("c3b_plp_last_ms: no c3b_plp_count has been issued"); return 1; }
     C3B_CUDA(cudaSetDevice(w->device));
@@ -861,6 +990,8 @@ void c3b_plp_destroy(c3b_plp *w) {
     cudaSetDevice(w->device);
     if (w->ev0) cudaEventDestroy(w->ev0);
     if (w->ev1) cudaEventDestroy(w->ev1);
+    if (w->ev2) cudaEventDestroy(w->ev2);
+    if (w->ev3) cudaEventDestroy(w->ev3);
     if (w->host_counters) cudaFreeHost(w->host_counters);
     delete w;
 }

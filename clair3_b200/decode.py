@@ -496,7 +496,6 @@ def batch_calls(model, batch_chr_pos_seq, alt_info_list, Y, output_config, k=16)
     flags, genotype code (``GENOTYPES``), printed, DP, AD's ref count, AF support, REF / ALT lengths, allele-count count),
     ``text`` / ``ad`` (the pools) and ``start`` int64 [B] (site s's REF, then ALT, at ``text[start[s]:]``, its allele counts
     at ``ad[start[s]:]``).  Raises what ``batch_output``'s host walk raises on an alt_info string it cannot decode."""
-    from .model import CALL_DTYPE
     _check_config(output_config)
     Y = np.ascontiguousarray(np.asarray(Y.cpu() if hasattr(Y, "cpu") else Y, dtype=np.float32))
     B = len(batch_chr_pos_seq)
@@ -516,7 +515,15 @@ def batch_calls(model, batch_chr_pos_seq, alt_info_list, Y, output_config, k=16)
     offsets = np.zeros(B + 1, np.int64)
     np.cumsum([len(a) for a in alts], out=offsets[1:])
     alt_bytes = np.frombuffer(bytearray(b"".join(alts)), dtype=np.uint8)
-    out = _numpy(model.decode_calls(Y, ref_base, alt_bytes, offsets, output_config, k=k))
+    return calls_result(_numpy(model.decode_calls(Y, ref_base, alt_bytes, offsets, output_config, k=k)), chromosomes, positions,
+                        offsets)
+
+
+def calls_result(out, chromosomes, positions, offsets):
+    """``batch_calls``' dict from ``model.decode_calls``' arrays (on the host) of sites whose alt_info starts at ``offsets``, or
+    the exception the host walk raises for the first site whose alt_info the decoder rejected."""
+    from .model import CALL_DTYPE
+    B = len(positions)
     calls = out["calls"].view(CALL_DTYPE).reshape(B)
     status = calls["status"]
     if status.any():

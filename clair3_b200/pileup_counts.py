@@ -132,13 +132,16 @@ class PileupCounter:
         self._h = out[0]
         self._keep = None
         self._shape = None
+        self._alt = None
+        self._sizes = None            # (n_cols, n_cand) once sizes() has waited for the work queued so far
         self._pin = {}
 
     def count(self, records, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.08, min_indel_af=0.15, min_mq=5,
               call_snp_only=False, call_ht=False, gvcf=False, alt_info=False, max_indel_length=50):
         """Arguments as ``calculate_clair3_pileup`` takes them (src/clair3_pileup.c:142) with the region as 0-based
         [start, end) and the reference bases of [ref_start, ref_start + len(ref_seq)).  ``alt_info=True`` also exports the
-        candidates' allele lists so that ``alt_info_strings()`` can format the reference's ``all_alt_info`` text."""
+        candidates' allele lists, from which ``alt_text()`` formats the reference's ``all_alt_info`` text on the device
+        (``alt_info_strings()``: the same on the host) and ``call()`` decodes every candidate."""
         on_dev = isinstance(records, DeviceBamRecords)
         rec = records if on_dev else BamRecords.from_dict(records)
         prm = ffi.new("c3b_plp_params *")
@@ -163,12 +166,14 @@ class PileupCounter:
         self._keep = (rec, ref, refbuf, st)          # buffers stay alive while the copies / kernels are in flight
         self._shape = (int(end) - int(start), bool(gvcf))
         self._alt = (bool(alt_info), int(start), int(end), int(ref_start), int(max_indel_length))
+        self._sizes = None
         return self
 
     def sizes(self):
         a, b = ffi.new("int64_t *"), ffi.new("int64_t *")
         check(lib().c3b_plp_sizes(self._h, a, b))
-        return int(a[0]), int(b[0])
+        self._sizes = int(a[0]), int(b[0])
+        return self._sizes
 
     def _pinned(self, name, shape, dtype):
         """A reusable page-locked host buffer (grown on demand): D2H into pinned memory runs at the PCIe rate, into a fresh
@@ -208,14 +213,16 @@ class PileupCounter:
         """The ``all_alt_info`` strings of ``calculate_clair3_pileup`` (src/clair3_pileup.c:391-450), one per candidate in
         candidate order: ``"<pos+1>-<depth>-<ref base>-X<b> n D<ref bases> n I<ref base><inserted bases> n R<ref base> n "`` -
         SNP alleles in A C G T order, deletions by length, insertions in the iteration order of the reference's khash string
-        counter, the remaining reference depth last.  The GPU supplies the allele lists (``c3b_plp_fetch_alleles``), the text is
-        formatted here from the HOST records of the count (the inserted bases are read from the representative reads)."""
-        want, start, end, ref_start, max_indel = self._alt
-        if not want:
+        counter, the remaining reference depth last.  With host records the GPU supplies the allele lists
+        (``c3b_plp_fetch_alleles``) and the text is formatted here (``format_alt_info``: the inserted bases are read from the
+        representative reads), which is the statement the device text is tested against; with device-resident records the
+        strings are the device's (``alt_text()``)."""
+        if not (self._alt and self._alt[0]):
             raise C3BError("alt_info_strings: count(..., alt_info=True) first")
+        want, start, end, ref_start, max_indel = self._alt
         rec, ref = self._keep[0], self._keep[1]
         if isinstance(rec, DeviceBamRecords):
-            raise C3BError("alt_info_strings needs host records (the inserted bases are read on the host)")
+            return self.alt_text().alt_text_fetch()["text"]
         r = fetched if fetched is not None else self.fetch()
         W = self._shape[0]
         n = ffi.new("int64_t *")
@@ -238,6 +245,83 @@ class PileupCounter:
                                        fetch_end=end + FETCH_EXPAND + 1))
         return out
 
+    def alt_text(self, max_indel_length=None):
+        """Enqueues the text stage (``c3b_plp_alt_text``) behind the last ``count(..., alt_info=True)``, on its stream and
+        without a host wait: the ``all_alt_info`` string of every candidate and what the decoder takes of it, formatted on the
+        device.  ``max_indel_length``: as ``calculate_clair3_pileup``'s (default: what ``count`` was given).  Device-resident
+        records must stay alive until the text has been fetched."""
+        if not self._alt:
+            raise C3BError("alt_text: count(..., alt_info=True) first")
+        if not self._alt[0]:
+            raise C3BError("alt_text: the count ran without alt_info=True")
+        if max_indel_length is None:
+            max_indel_length = self._alt[4]
+        if isinstance(max_indel_length, bool) or not isinstance(max_indel_length, (int, np.integer)):
+            raise C3BError("alt_text: max_indel_length must be an integer, got %r" % (max_indel_length,))
+        check(lib().c3b_plp_alt_text(self._h, int(max_indel_length)))
+        self._sizes = None
+        return self
+
+    def alt_text_sizes(self):
+        a, b = ffi.new("int64_t *"), ffi.new("int64_t *")
+        check(lib().c3b_plp_alt_text_sizes(self._h, a, b))
+        return int(a[0]), int(b[0])
+
+    def alt_text_fetch(self):
+        """dict: ``text`` (the ``all_alt_info`` strings, one per candidate), ``decoder`` (the ``"depth-alt"`` strings of
+        ``alt_info_list``), ``ref_base`` uint8 [n_cand], ``position`` int64 [n_cand] (1-based).  Waits for the text stage."""
+        nk = (self._sizes or self.sizes())[1]
+        nt, nd = self.alt_text_sizes()
+        text, dec = np.zeros(max(nt, 1), np.uint8), np.zeros(max(nd, 1), np.uint8)
+        toff, doff = np.zeros(nk + 1, np.int64), np.zeros(nk + 1, np.int64)
+        rb, pos = np.zeros(nk, np.uint8), np.zeros(nk, np.int64)
+        c = ffi.cast
+        check(lib().c3b_plp_fetch_alt_text(self._h, c("char *", text.ctypes.data), c("int64_t *", toff.ctypes.data),
+                                           c("char *", dec.ctypes.data), c("int64_t *", doff.ctypes.data),
+                                           c("uint8_t *", rb.ctypes.data), c("int64_t *", pos.ctypes.data)))
+        tb, db = text.tobytes(), dec.tobytes()
+        return {"text": [tb[toff[j]:toff[j + 1]].decode("latin-1") for j in range(nk)],
+                "decoder": [db[doff[j]:doff[j + 1]].decode("latin-1") for j in range(nk)], "ref_base": rb, "position": pos}
+
+    def alt_text_device(self):
+        """The text stage's results as tensors that alias the workspace (valid until the next ``count`` / ``alt_text``):
+        ``text`` uint8 [n_text_bytes], ``text_off`` int64 [n_cand + 1], ``decoder`` uint8 [n_decoder_bytes], ``decoder_off``
+        int64 [n_cand + 1], ``ref_base`` uint8 [n_cand], ``position`` int64 [n_cand]; ``decoder`` / ``decoder_off`` /
+        ``ref_base`` are ``decode_calls``' ``alt_bytes`` / ``alt_offsets`` / ``ref_base``.  Waits (``sizes()``) only when
+        nothing has waited since the last ``count`` / ``alt_text``; after that wait it touches the stream no more."""
+        nk = (self._sizes or self.sizes())[1]
+        nt, nd = self.alt_text_sizes()
+        p = [ffi.new("const char **"), ffi.new("const int64_t **"), ffi.new("const char **"), ffi.new("const int64_t **"),
+             ffi.new("const uint8_t **"), ffi.new("const int64_t **")]
+        check(lib().c3b_plp_alt_text_device(self._h, *p))
+        shapes = (("text", nt, torch.uint8), ("text_off", nk + 1, torch.int64), ("decoder", nd, torch.uint8),
+                  ("decoder_off", nk + 1, torch.int64), ("ref_base", nk, torch.uint8), ("position", nk, torch.int64))
+        return {name: _device_view(int(ffi.cast("uintptr_t", q[0])), n, dt, self._device) for (name, n, dt), q in zip(shapes, p)}
+
+    def call(self, model, output_config, ctg_name, k=16):
+        """One region from counts to call records on the current stream: after ``count(..., alt_info=True)``, the text stage,
+        Clair3_P over every candidate's window and ``model.decode_calls`` on the device views, with one host wait (the sizes)
+        before the results are copied.  Returns ``decode.batch_calls``' dict (``chromosome``, ``position``, ``calls``, ``text``,
+        ``ad``, ``start``; ``decode.calls_text`` formats it) plus ``cand_ok`` uint8 [n_cand] and ``Y``, the probabilities, on the
+        device.  Every candidate is decoded; ``cand_ok == 0``: the reference drops that candidate, ignore its row.  Raises
+        what ``batch_calls`` raises on an alt_info string the decoder rejects."""
+        from . import decode
+        decode._check_config(output_config)
+        self._check_model(model, "call")
+        if bool(output_config.add_indel_length) != model.add_indel_length:
+            raise C3BError("call: output_config.add_indel_length must match the model")
+        self.alt_text()
+        nc, nk = self.sizes()                              # the one wait: the count and the text together
+        v = self.alt_text_device()
+        y = torch.empty((nk, model.out_dim), dtype=torch.float32, device=self._device)
+        self._forward_into(model, y, nc, nk)
+        out = model.decode_calls(y, v["ref_base"], v["decoder"], v["decoder_off"], output_config, k=k)
+        ok = np.zeros(nk, np.uint8)
+        check(lib().c3b_plp_fetch(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.cast("uint8_t *", ok.ctypes.data), ffi.NULL, ffi.NULL))
+        res = decode.calls_result(decode._numpy(out), [ctg_name] * nk, v["position"].cpu().numpy(), v["decoder_off"].cpu().numpy())
+        res["cand_ok"], res["Y"] = ok, y
+        return res
+
     def window_bounds(self):
         """int64 [n_cand, 2]: the rows [lo, hi) of each candidate's 33-row window (from ``cand_cols - 16``) that lie in its
         contiguous run of positions (``c3b_plp_window_bounds``); the reference's tensor is zero on the window's other rows
@@ -253,17 +337,28 @@ class PileupCounter:
         outside it, which is the tensor the reference builds (``preprocess/CreateTensorPileupFromCffi.py:356-396``).  Returns
         (probabilities float32 [n_cand, 24|90] on the device, cand_ok uint8 [n_cand] on the host): ``cand_ok == 0``: the
         reference drops that candidate, and its row must be ignored."""
-        if getattr(model, "_handle", None) is None:
-            raise C3BError("forward: the model has no device / weights yet (.to(device), .load_state_dict())")
-        if getattr(model, "input_channels", CHANNELS) != CHANNELS or model._kind != lib_const("C3B_PILEUP"):
-            raise C3BError("forward: needs the pileup network (Clair3_P, 18 channels)")
-        if torch.device(model._device) != self._device:
-            raise C3BError("forward: the model lives on %s, the counter on %s" % (model._device, self._device))
+        self._check_model(model, "forward")
         nc, nk = self.sizes()
         y = torch.empty((nk, model.out_dim), dtype=torch.float32, device=self._device)
         ok = np.zeros(nk, np.uint8)
         if nk == 0:
             return y, ok
+        self._forward_into(model, y, nc, nk)
+        check(lib().c3b_plp_fetch(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.cast("uint8_t *", ok.ctypes.data), ffi.NULL, ffi.NULL))
+        return y, ok
+
+    def _check_model(self, model, who):
+        if getattr(model, "_handle", None) is None:
+            raise C3BError("%s: the model has no device / weights yet (.to(device), .load_state_dict())" % who)
+        if getattr(model, "input_channels", CHANNELS) != CHANNELS or model._kind != lib_const("C3B_PILEUP"):
+            raise C3BError("%s: needs the pileup network (Clair3_P, 18 channels)" % who)
+        if torch.device(model._device) != self._device:
+            raise C3BError("%s: the model lives on %s, the counter on %s" % (who, model._device, self._device))
+
+    def _forward_into(self, model, y, nc, nk):
+        """Clair3_P over the nk candidates' bounded windows into y, stream-ordered."""
+        if nk == 0:
+            return
         pm, ps, pk, pb = (ffi.new("const int64_t **"), ffi.new("const int64_t **"), ffi.new("const uint8_t **"),
                           ffi.new("const int64_t **"))
         check(lib().c3b_plp_device(self._h, pm, ffi.NULL, ffi.NULL, ps, pk))
@@ -271,12 +366,16 @@ class PileupCounter:
         stream = torch.cuda.current_stream(self._device).cuda_stream
         check(lib().c3b_forward_windows_bounded(model._handle, ffi.cast("void *", pm[0]), lib_const("C3B_DT_I64"), nc, ps[0], pb[0],
                                                 1, nk, ffi.cast("float *", y.data_ptr()), 1, 0, ffi.cast("void *", stream)))
-        check(lib().c3b_plp_fetch(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.cast("uint8_t *", ok.ctypes.data), ffi.NULL, ffi.NULL))
-        return y, ok
 
     def last_ms(self):
         ms, n = ffi.new("float *"), ffi.new("int *")
         check(lib().c3b_plp_last_ms(self._h, ms, n))
+        return float(ms[0]), int(n[0])
+
+    def alt_text_last_ms(self):
+        """Device time and kernel launches of the last ``alt_text`` (``last_ms`` reports the count alone)."""
+        ms, n = ffi.new("float *"), ffi.new("int *")
+        check(lib().c3b_plp_alt_text_last_ms(self._h, ms, n))
         return float(ms[0]), int(n[0])
 
     def close(self):
@@ -289,6 +388,19 @@ class PileupCounter:
             self.close()
         except Exception:
             pass
+
+
+class _DeviceArray:
+    def __init__(self, ptr, n, dtype):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": {torch.uint8: "|u1", torch.int64: "<i8"}[dtype],
+                                         "data": (ptr, False), "version": 2}
+
+
+def _device_view(ptr, n, dtype, device):
+    """A tensor over n elements of workspace memory at ptr (no copy; the workspace owns the memory)."""
+    if n == 0:
+        return torch.empty(0, dtype=dtype, device=device)
+    return torch.as_tensor(_DeviceArray(ptr, n, dtype), device=device)
 
 
 _NT16 = "=ACMGRSVTWYHKDBN"                      # htslib seq_nt16_str
@@ -490,7 +602,7 @@ def pileup_counts_clair3(records, ref_name, start, end, ref_seq, ref_start, coun
     (chunk_results, all_alt_info_list, gvcf_output) - contiguous (counts [n,18] int64, positions with 'major' / 'minor') chunks,
     the (pos, "ctg:pos:ref", "depth-alt") tuples of every candidate and, with ``gvcf=True``, [pos_ref_count, pos_total_count] -
     for the 0-based [start, end) that reaches ``calculate_clair3_pileup`` (see ``counting_region``).  Keyword arguments as
-    ``PileupCounter.count``; the allele text needs host records."""
+    ``PileupCounter.count``."""
     own = counter is None
     counter = counter or PileupCounter(device)
     try:

@@ -10,8 +10,10 @@
  * image), the caller hands over what bam1_t carries.  What is counted, column by column, is exactly what the reference's loop
  * over bam_mplp_auto() counts (see oracle/pileup_oracle.c for the line-by-line restatement, quirks included).
  *
- * The all_alt_info strings (src/clair3_pileup.c:391-450) are text: the GPU exports the per-candidate allele lists
- * (c3b_plp_fetch_alleles) and the host shim formats them, byte for byte as the reference does.
+ * The all_alt_info strings (src/clair3_pileup.c:391-450) are formatted on the GPU as well (c3b_plp_alt_text), byte for byte as
+ * the reference prints them, together with the form the decoder takes (c3b_decode_calls in clair3_b200.h): a region goes from
+ * records to call records on one stream.  The per-candidate allele lists the text is made from can still be exported
+ * (c3b_plp_fetch_alleles); clair3_b200/pileup_counts.py formats them on the host, which is what the tests hold the GPU text to.
  *
  * Same conventions as clair3_b200.h: int status, 0 = ok, message via c3b_last_error(); no CPU fallback.
  */
@@ -55,8 +57,8 @@ typedef struct c3b_plp_params {
     int32_t call_ht;            /* 1: no 16-column flanking requirement (src/clair3_pileup.c:385-387), and cand_ok keeps the head /
                                    tail windows of preprocess/CreateTensorPileupFromCffi.py:370-396 */
     int32_t gvcf;               /* 1: also fill pos_ref_count / pos_total_count (:205-210, :453-456) */
-    int32_t alt_info;           /* 1: also export every pre-candidate column's distinct indel alleles (c3b_plp_fetch_alleles), from
-                                   which the host formats the all_alt_info text of :391-450 */
+    int32_t alt_info;           /* 1: also keep every pre-candidate column's distinct indel alleles (c3b_plp_fetch_alleles), from
+                                   which c3b_plp_alt_text formats the all_alt_info text of :391-450 */
 } c3b_plp_params;
 
 /* A counting workspace on one device (scratch grows on demand; one call in flight per workspace). */
@@ -102,8 +104,8 @@ int c3b_plp_fetch(c3b_plp *w, int64_t *matrix, int64_t *major, int32_t *stats, i
  *   read  [n]  uint32   index (into the records of the count) of the first read that showed the allele
  *   qpos  [n]  uint32   query offset of its first inserted base in that read (insertions)
  *   cnt   [n]  uint32   reads of that strand showing it
- * Any pointer may be NULL; n_alleles alone sizes the buffers.  clair3_b200/pileup_counts.py formats the all_alt_info strings
- * (src/clair3_pileup.c:391-450, insertion alleles in the reference's khash bucket order) from these on the host. */
+ * Any pointer may be NULL; n_alleles alone sizes the buffers.  c3b_plp_alt_text formats the all_alt_info strings from these on
+ * the GPU; clair3_b200/pileup_counts.py (format_alt_info) does the same on the host. */
 int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, int32_t *ins_last, uint32_t *meta, uint32_t *read, uint32_t *qpos, uint32_t *cnt,
                           int64_t capacity, int64_t *n_alleles);
 
@@ -119,6 +121,40 @@ int c3b_plp_device(c3b_plp *w, const int64_t **matrix, const int64_t **major, co
  * (:374-391); the matrix holds the neighbouring runs' columns there.  These are the `bounds` of c3b_forward_windows_bounded.
  * bounds: host copy (waits for the count); device_bounds: device view, valid until the next c3b_plp_count.  Either may be NULL. */
 int c3b_plp_window_bounds(c3b_plp *w, int64_t *bounds, const int64_t **device_bounds);
+
+/* The all_alt_info text of every candidate (src/clair3_pileup.c:391-450), formatted on the GPU: enqueues the text stage on the
+ * stream of the last c3b_plp_count, which must have run with params.alt_info.  No host wait.  max_indel_length: the reference's
+ * argument (longer alleles are counted but not printed).  The stage reads the records and the reference bases where the count
+ * left them: the workspace's own copies, or, after a count with on_device = 1, the caller's device arrays, which must stay alive
+ * and unchanged until the text has been fetched or consumed.  Per candidate, in candidate order:
+ *   text      "<pos+1>-<depth>-<REF>-X<b> n D<ref bases> n I<REF><inserted bases> n R<REF> n ": SNP alleles in A C G T order,
+ *             deletions by length, insertions in the bucket order of the reference's khash string counter, the remaining
+ *             reference depth last; deletion text is the reference's bytes as supplied
+ *   decoder   "<depth>-<alt>", alt = the fourth '-'-separated field of the stripped string: what
+ *             preprocess/CreateTensorPileupFromCffi.py:66-73 hands on as alt_info
+ *   ref_base  the same <REF> character         position  pos + 1
+ * The next c3b_plp_sizes waits for the count and the text together. */
+int c3b_plp_alt_text(c3b_plp *w, int64_t max_indel_length);
+
+/* After c3b_plp_alt_text (waits like c3b_plp_sizes when that has not been called since): bytes of all text strings and of all
+ * decoder strings.  Fails, as c3b_plp_fetch_alt_text does, if the text outgrew the stage's buffers; the count's own results stay
+ * valid, and a later c3b_plp_alt_text (with a smaller max_indel_length, say) starts clean. */
+int c3b_plp_alt_text_sizes(c3b_plp *w, int64_t *n_text_bytes, int64_t *n_decoder_bytes);
+
+/* Host copies (any pointer may be NULL): text [n_text_bytes], text_off [n_cand + 1] int64 (candidate j is
+ * text[text_off[j] .. text_off[j + 1])), decoder [n_decoder_bytes], decoder_off [n_cand + 1], ref_base [n_cand],
+ * position [n_cand]. */
+int c3b_plp_fetch_alt_text(c3b_plp *w, char *text, int64_t *text_off, char *decoder, int64_t *decoder_off, uint8_t *ref_base,
+                           int64_t *position);
+
+/* Device views of the same, valid until the next c3b_plp_count or c3b_plp_alt_text on w: decoder / decoder_off / ref_base are
+ * the alt_bytes / alt_offsets / ref_base arguments of c3b_decode_calls(..., on_device = 1). */
+int c3b_plp_alt_text_device(c3b_plp *w, const char **text, const int64_t **text_off, const char **decoder,
+                            const int64_t **decoder_off, const uint8_t **ref_base, const int64_t **position);
+
+/* Device time of the last c3b_plp_alt_text (CUDA events around its kernels) and the number of kernels it launched;
+ * c3b_plp_last_ms keeps reporting the count alone. */
+int c3b_plp_alt_text_last_ms(c3b_plp *w, float *ms, int *launches);
 
 /* Device time of the last c3b_plp_count (CUDA events on its stream around all of its kernels, input copies excluded), and the
  * number of kernels it launched. */
