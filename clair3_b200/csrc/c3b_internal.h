@@ -121,11 +121,30 @@ int c3b_upload(C3bBuf &b, const T *src, size_t bytes, int on_device, const T *&d
     return 0;
 }
 
-// The eight core c3b_bam_records arrays of a call, into the kernel-visible record struct R (DevReads / FaReads, which share
-// these field names) through c3b_upload.  n_cigar / n_seq: the CIGAR words and sequence bytes the arrays hold.
-template <class Reads>
-int c3b_upload_records(Reads &R, C3bBuf (&b)[8], const c3b_bam_records *r, int64_t n_cigar, int64_t n_seq, int on_device,
-                       cudaStream_t s, const char *what) {
+// The alignment records as the pileup counter's and the full-alignment builder's kernels read them: the c3b_bam_records arrays
+// and c3b_fa_records' optional fields, all device pointers; an optional field is null when the call has none.
+struct C3bReads {
+    int64_t n;
+    const int64_t *pos;
+    const uint16_t *flag;
+    const uint8_t *mapq;
+    const int64_t *cigar_off;
+    const uint32_t *cigar;
+    const int64_t *seq_off;
+    const uint8_t *seq;
+    const int32_t *l_qseq;
+    const int64_t *qual_off;
+    const uint8_t *qual;
+    const int64_t *qname_off;
+    const uint8_t *qname;
+    const int64_t *mv_off;
+    const int32_t *mv;
+};
+
+// The eight core c3b_bam_records arrays of a call into R through c3b_upload.  n_cigar / n_seq: the CIGAR words and sequence
+// bytes the arrays hold.
+inline int c3b_upload_records(C3bReads &R, C3bBuf (&b)[8], const c3b_bam_records *r, int64_t n_cigar, int64_t n_seq, int on_device,
+                              cudaStream_t s, const char *what) {
     const size_t n = (size_t)r->n_reads;
     return c3b_upload(b[0], r->pos, n * 8, on_device, R.pos, s, what) || c3b_upload(b[1], r->flag, n * 2, on_device, R.flag, s, what) ||
            c3b_upload(b[2], r->mapq, n, on_device, R.mapq, s, what) ||
@@ -150,6 +169,84 @@ int c3b_last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s
 // Makes device `ordinal` current after checking that it exists and is an sm_90 part.  Returns 0; `unsupported` when there
 // is no CUDA device or it is not sm_90; 1 for a bad ordinal or a failed runtime call.  sm_count (optional): its SM count.
 int c3b_use_device(int ordinal, int unsupported, int *sm_count);
+
+// What the pileup counter (c3b_plp) and the full-alignment builder (c3b_fa) hold alike: the device and the stream of the last
+// call, a pair of CUDA events around each timed stage with the stage's kernel launches, a device counter block with its pinned
+// host mirror, and the exported allele records.  The destructor releases the events and the pinned memory.
+struct C3bRegionWorkspace {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev[2][2] = {};           // per stage: start, end
+    int launches[2] = {};
+    C3bBuf counters;
+    int64_t *host_counters = nullptr;    // pinned copy of `counters`
+    C3bBuf al_meta, al_read, al_qpos, al_cnt;
+
+    C3bRegionWorkspace() = default;
+    C3bRegionWorkspace(const C3bRegionWorkspace &) = delete;
+    C3bRegionWorkspace &operator=(const C3bRegionWorkspace &) = delete;
+    ~C3bRegionWorkspace() {
+        for (auto &p : ev)
+            for (cudaEvent_t e : p)
+                if (e) cudaEventDestroy(e);
+        if (host_counters) cudaFreeHost(host_counters);
+    }
+    // Device time between the events of stage i, after waiting for its end, and the stage's launches.
+    int elapsed(int i, float *ms, int *n) {
+        C3B_CUDA(cudaSetDevice(device));
+        C3B_CUDA(cudaEventSynchronize(ev[i][1]));
+        float t = 0.f;
+        C3B_CUDA(cudaEventElapsedTime(&t, ev[i][0], ev[i][1]));
+        if (ms) *ms = t;
+        if (n) *n = launches[i];
+        return 0;
+    }
+    // Queues the copy of the first `bytes` of src into dst on the workspace's stream; nothing for a null dst or no bytes.
+    int get(void *dst, const C3bBuf &src, size_t bytes) {
+        if (dst && bytes) C3B_CUDA(cudaMemcpyAsync(dst, src.p, bytes, cudaMemcpyDeviceToHost, stream));
+        return 0;
+    }
+    int wait() {
+        C3B_CUDA(cudaStreamSynchronize(stream));
+        return 0;
+    }
+    // Queues the copies of the first n allele records into whichever of meta / read / qpos / cnt is given; `who` names the
+    // entry point in the error when they hold fewer than n.
+    int get_alleles(const char *who, int64_t n, int64_t capacity, uint32_t *meta, uint32_t *read, uint32_t *qpos, uint32_t *cnt) {
+        if (!meta && !read && !qpos && !cnt) return 0;
+        if (capacity < n) { c3b_set_error("%s: capacity %lld < %lld records", who, (long long)capacity, (long long)n); return 1; }
+        const size_t b = (size_t)n * 4;
+        return get(meta, al_meta, b) || get(read, al_read, b) || get(qpos, al_qpos, b) || get(cnt, al_cnt, b);
+    }
+};
+
+// Creates a W (derived from C3bRegionWorkspace) on device `ordinal`: `stages` event pairs and a block of `n_counters` int64
+// counters, on the device and pinned on the host.  `who` names the entry point in the errors.
+template <class W> int c3b_region_create(W **out, int ordinal, int stages, int n_counters, const char *who) {
+    if (!out) { c3b_set_error("%s: null out", who); return 1; }
+    *out = nullptr;
+    if (c3b_use_device(ordinal, 1, nullptr)) return 1;
+    W *w = new W();
+    w->device = ordinal;
+    bool ok = w->counters.ensure((size_t)n_counters * 8, nullptr, who) == 0 &&
+              cudaMallocHost((void **)&w->host_counters, (size_t)n_counters * 8) == cudaSuccess;
+    for (int i = 0; i < stages && ok; ++i)
+        ok = cudaEventCreate(&w->ev[i][0]) == cudaSuccess && cudaEventCreate(&w->ev[i][1]) == cudaSuccess;
+    if (!ok) {
+        c3b_set_error("%s: event / pinned allocation failed", who);
+        delete w;
+        return 1;
+    }
+    *out = w;
+    return 0;
+}
+
+// Releases a workspace on its own device.
+template <class W> void c3b_region_destroy(W *w) {
+    if (!w) return;
+    cudaSetDevice(w->device);
+    delete w;
+}
 
 struct HostParam {
     std::vector<float> data;
@@ -379,9 +476,7 @@ struct PlpAltTextArgs {
     const int64_t *cand_cols, *major, *matrix;
     const int32_t *stats;
     const char *ref;
-    const int64_t *seq_off;             // the records where the count left them
-    const uint8_t *seq;
-    const int32_t *l_qseq;
+    C3bReads R;                         // the records where the count left them
     const int32_t *al_off, *al_n, *ins_last;
     const uint32_t *al_meta, *al_read, *al_qpos, *al_cnt;
     int64_t al_cap;                     // records the al_* arrays and mate / hash / order hold
@@ -401,6 +496,3 @@ struct PlpAltTextArgs {
     int64_t *position;                  // [W]
 };
 int c3b_launch_plp_alt_text(const PlpAltTextArgs &a, cudaStream_t s, int *launches);
-// plp_counts.cu: exclusive scan of int32 counts into int64 offsets on one CTA, their sum to *total; over n entries, or over
-// *n_dev + 1 of them when n_dev is given and that is fewer
-int c3b_launch_plp_scan(const int32_t *cnt, int64_t *off, int n, const int64_t *n_dev, int64_t *total, cudaStream_t s);

@@ -19,7 +19,9 @@
 //                        bq, deletion length, insertion query offset + length, dwell signal) with the same overwrite order.
 //   K9 fa_select_count   one warp per candidate: the kept reads with read_start < c+17 and read_end > c-16 (prefix max of the
 //                        read ends bounds the search); their number decides the shuffle and its rand() draws.
-//   K10 (scan)           draw offset of every candidate = prefix sum of n-1 over earlier shuffling candidates.
+//   K10 (block_scan)     draw offset of every candidate = prefix sum of n-1 over earlier shuffling candidates.  The same
+//                        one-CTA scan (block_scan.cuh) sizes F, numbers the kept reads and lays out their pools, and takes the
+//                        running maximum of the kept reads' ends.
 //   K11 fa_candidate     one CTA per candidate: counters over ALL kept reads on the candidate (depth, A/C/G/T, distinct
 //                        deletion lengths and insertion strings in first-occurrence order, exported for the host's text),
 //                        Fisher-Yates with the glibc TYPE_3 stream generated at the candidate's offset (jump-ahead by
@@ -31,10 +33,10 @@
 // candidate) written once.  DESIGN.md 5b.
 #include <limits.h>
 #include <stdlib.h>
-#include <string.h>
 
 #include <vector>
 
+#include "block_scan.cuh"
 #include "c3b_internal.h"
 #include "../../include/clair3_b200_fa.h"
 
@@ -57,24 +59,6 @@ struct PosInfo {                    // Pos_info (src/clair3_full_alignment_dwell
     int32_t ins_q;
     int32_t ins_len;
     int32_t sig;
-};
-
-struct FaReads {
-    int64_t n;
-    const int64_t *pos;
-    const uint16_t *flag;
-    const uint8_t *mapq;
-    const int64_t *cigar_off;
-    const uint32_t *cigar;
-    const int64_t *seq_off;
-    const uint8_t *seq;
-    const int32_t *l_qseq;
-    const int64_t *qual_off;
-    const uint8_t *qual;
-    const int64_t *qname_off;
-    const uint8_t *qname;
-    const int64_t *mv_off;
-    const int32_t *mv;
 };
 
 struct Kept {                       // per kept read, compacted in file order
@@ -112,42 +96,6 @@ __device__ __forceinline__ int64_t lower_bound64(const int64_t *a, int64_t lo, i
 
 __device__ __forceinline__ bool ref_op(uint32_t op) { return op == 0 || op == 2 || op == 3 || op == 7 || op == 8; }
 
-// ---------------------------------------------------------------------------------------------------------------- scan
-// One CTA of 1024 threads: exclusive prefix (sum or max) of an int64 array, total in *total.
-__global__ void fa_scan_kernel(const int64_t *__restrict__ in, int64_t *__restrict__ out, int64_t n, int64_t *total, int is_max) {
-    __shared__ long long ws[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    long long carry = is_max ? LLONG_MIN : 0;
-    for (int64_t base = 0; base < n; base += 1024) {
-        const int64_t i = base + threadIdx.x;
-        const long long x = i < n ? (long long)in[i] : (is_max ? LLONG_MIN : 0);
-        long long v = x;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const long long a = __shfl_up_sync(0xffffffffu, v, d);
-            if (lane >= d) v = is_max ? (a > v ? a : v) : v + a;
-        }
-        if (lane == 31) ws[warp] = v;
-        __syncthreads();
-        if (warp == 0) {
-            long long t = ws[lane];
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const long long a = __shfl_up_sync(0xffffffffu, t, d);
-                if (lane >= d) t = is_max ? (a > t ? a : t) : t + a;
-            }
-            ws[lane] = t;
-        }
-        __syncthreads();
-        if (warp > 0) v = is_max ? (ws[warp - 1] > v ? ws[warp - 1] : v) : v + ws[warp - 1];
-        // inclusive v -> exclusive for sums; for max the inclusive prefix is what callers want
-        if (i < n) out[i] = is_max ? (carry > v ? carry : v) : carry + v - x;
-        carry = is_max ? (ws[31] > carry ? ws[31] : carry) : carry + ws[31];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0 && total) *total = carry;
-}
-
 // ---------------------------------------------------------------------------------------------------------------- K1 / K2
 __global__ void fa_flank_count_kernel(const int64_t *__restrict__ cand, int64_t n_cand, int64_t *__restrict__ fstart,
                                       int64_t *__restrict__ fcnt) {
@@ -175,7 +123,7 @@ __device__ __forceinline__ uint32_t name_hash(const uint8_t *s, int64_t n) {
     return h;
 }
 
-__device__ __forceinline__ bool same_name(const FaReads &R, int64_t a, int64_t b) {
+__device__ __forceinline__ bool same_name(const C3bReads &R, int64_t a, int64_t b) {
     const int64_t a0 = R.qname_off[a], la = R.qname_off[a + 1] - a0, b0 = R.qname_off[b], lb = R.qname_off[b + 1] - b0;
     if (la != lb) return false;
     for (int64_t i = 0; i < la; ++i)
@@ -183,7 +131,7 @@ __device__ __forceinline__ bool same_name(const FaReads &R, int64_t a, int64_t b
     return true;
 }
 
-__global__ void fa_read_scan_kernel(FaReads R, int min_mq, const int64_t *__restrict__ F, int64_t nF, int64_t *__restrict__ rend,
+__global__ void fa_read_scan_kernel(C3bReads R, int min_mq, const int64_t *__restrict__ F, int64_t nF, int64_t *__restrict__ rend,
                                     int64_t *__restrict__ rlo, int32_t *__restrict__ rov, uint8_t *__restrict__ pass,
                                     int64_t *__restrict__ table, uint32_t tmask) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -216,7 +164,7 @@ __global__ void fa_read_scan_kernel(FaReads R, int min_mq, const int64_t *__rest
     }
 }
 
-__global__ void fa_read_keep_kernel(FaReads R, const uint8_t *__restrict__ pass, const int32_t *__restrict__ rov,
+__global__ void fa_read_keep_kernel(C3bReads R, const uint8_t *__restrict__ pass, const int32_t *__restrict__ rov,
                                     const int64_t *__restrict__ table, uint32_t tmask, int64_t *__restrict__ keep,
                                     int64_t *__restrict__ kov) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -237,7 +185,7 @@ __global__ void fa_read_keep_kernel(FaReads R, const uint8_t *__restrict__ pass,
 }
 
 // ---------------------------------------------------------------------------------------------------------------- K5
-__global__ void fa_read_compact_kernel(FaReads R, int dwell, const int64_t *__restrict__ keep, const int64_t *__restrict__ kidx,
+__global__ void fa_read_compact_kernel(C3bReads R, int dwell, const int64_t *__restrict__ keep, const int64_t *__restrict__ kidx,
                                        const int64_t *__restrict__ kov_ex, const int64_t *__restrict__ rend,
                                        const int64_t *__restrict__ rlo, const int32_t *__restrict__ rov, Kept K,
                                        int64_t *__restrict__ sig_len) {
@@ -257,7 +205,7 @@ __global__ void fa_read_compact_kernel(FaReads R, int dwell, const int64_t *__re
 }
 
 // ---------------------------------------------------------------------------------------------------------------- K6
-__global__ void fa_signal_kernel(FaReads R, Kept K, const int64_t *__restrict__ sig_len, const int64_t *__restrict__ sig_ex,
+__global__ void fa_signal_kernel(C3bReads R, Kept K, const int64_t *__restrict__ sig_len, const int64_t *__restrict__ sig_ex,
                                  int64_t n_kept, int32_t *__restrict__ sig) {
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_kept) return;
@@ -281,7 +229,7 @@ __global__ void fa_signal_kernel(FaReads R, Kept K, const int64_t *__restrict__ 
 
 // ---------------------------------------------------------------------------------------------------------------- K7
 struct HapArgs {
-    FaReads R;
+    C3bReads R;
     Kept K;
     int64_t n_kept;
     const c3b_fa_variant *var;
@@ -454,7 +402,7 @@ __global__ void fa_haplotag_kernel(HapArgs A) {
 // ---------------------------------------------------------------------------------------------------------------- K8
 __device__ __forceinline__ int8_t norm_bq(int q) { return (int8_t)(int)(q < 40 ? 100 * q / 40.0 : 100); }   // normalize_bq
 
-__global__ void fa_pos_info_kernel(FaReads R, Kept K, int64_t n_kept, const int64_t *__restrict__ F, const int32_t *__restrict__ sig,
+__global__ void fa_pos_info_kernel(C3bReads R, Kept K, int64_t n_kept, const int64_t *__restrict__ F, const int32_t *__restrict__ sig,
                                    PosInfo *__restrict__ pool) {
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_kept) return;
@@ -545,7 +493,7 @@ __global__ void fa_select_count_kernel(const int64_t *__restrict__ cand, int64_t
 
 // ---------------------------------------------------------------------------------------------------------------- K11
 struct CandArgs {
-    FaReads R;
+    C3bReads R;
     Kept K;
     const int64_t *cand;
     const int64_t *F;
@@ -565,7 +513,7 @@ struct CandArgs {
     int *status;
 };
 
-__device__ __forceinline__ bool same_ins(const FaReads &R, const Kept &K, int64_t ka, int qa, int64_t kb, int qb, int len) {
+__device__ __forceinline__ bool same_ins(const C3bReads &R, const Kept &K, int64_t ka, int qa, int64_t kb, int qb, int len) {
     const uint8_t *sa = R.seq + R.seq_off[K.orig[ka]], *sb = R.seq + R.seq_off[K.orig[kb]];
     for (int t = 0; t < len; ++t)
         if (nib(sa, qa + t) != nib(sb, qb + t)) return false;
@@ -965,8 +913,9 @@ void glibc_jump_matrices(std::vector<uint32_t> &out) {
 
 }  // namespace
 
-struct c3b_fa {
-    int device = 0;
+// One timed stage, the build.  counters: int64 0 nF, 1 n_kept, 2 pool entries, 3 signal entries, 4 draws, 5 status, 6 al_used,
+// 7 spare.
+struct c3b_fa : C3bRegionWorkspace {
     C3bBuf in_core[8], in_qoff, in_qual, in_noff, in_name, in_moff, in_mv;
     C3bBuf in_ref, in_cand, in_var, jump, state0;
     C3bBuf fstart, fcnt, foff, F;
@@ -974,36 +923,25 @@ struct c3b_fa {
     C3bBuf k_orig, k_start, k_end, k_pmax, k_fs, k_ov, k_pi, k_sig, k_hap, sig_len, sig_ex;
     C3bBuf pool, sig;
     C3bBuf ra, rb, nsel, draws, draw_off;
-    C3bBuf matrix, c_depth, c_acgt, al_off, al_n, al_meta, al_read, al_qpos, al_cnt;
-    C3bBuf counters;    // int64: 0 nF, 1 n_kept, 2 pool entries, 3 signal entries, 4 draws, 5 status, 6 al_used, 7 spare
+    C3bBuf matrix, c_depth, c_acgt, al_off, al_n;
     int64_t n_cand = 0, depth = 0, C = 8, n_kept = 0;
     bool built = false;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    int launches = 0;
-    int64_t *host_counters = nullptr;   // pinned
 };
 
 extern "C" {
 
 int c3b_fa_create(c3b_fa **out, int device_ordinal) {
-    if (!out) { c3b_set_error("c3b_fa_create: null out"); return 1; }
-    *out = nullptr;
-    if (c3b_use_device(device_ordinal, 1, nullptr)) return 1;
-    c3b_fa *w = new c3b_fa();
-    w->device = device_ordinal;
+    if (c3b_region_create(out, device_ordinal, 1, 8, "c3b_fa_create")) return 1;
+    c3b_fa *w = *out;
     std::vector<uint32_t> J;
     glibc_jump_matrices(J);
-    if (cudaEventCreate(&w->ev0) != cudaSuccess || cudaEventCreate(&w->ev1) != cudaSuccess ||
-        cudaMallocHost((void **)&w->host_counters, 8 * sizeof(int64_t)) != cudaSuccess ||
-        w->jump.ensure(J.size() * 4, nullptr, "c3b_fa") || w->state0.ensure(31 * 4, nullptr, "c3b_fa") ||
-        w->counters.ensure(8 * 8, nullptr, "c3b_fa") ||
+    if (w->jump.ensure(J.size() * 4, nullptr, "c3b_fa") || w->state0.ensure(31 * 4, nullptr, "c3b_fa") ||
         cudaMemcpy(w->jump.p, J.data(), J.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
         c3b_set_error("c3b_fa_create: allocation failed");
         c3b_fa_destroy(w);
+        *out = nullptr;
         return 1;
     }
-    *out = w;
     return 0;
 }
 
@@ -1054,8 +992,7 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     const int depth = params->matrix_depth;
 
     // inputs
-    FaReads R;
-    memset(&R, 0, sizeof(R));
+    C3bReads R{};
     R.n = n;
     if (n > 0) {
         int64_t n_cigar, n_seq, n_qual, n_name, n_mv;
@@ -1111,16 +1048,16 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     K.orig = w->k_orig.as<int64_t>(); K.start = w->k_start.as<int64_t>(); K.end = w->k_end.as<int64_t>();
     K.pmax = w->k_pmax.as<int64_t>(); K.fs = w->k_fs.as<int64_t>(); K.ov = w->k_ov.as<int32_t>(); K.pi = w->k_pi.as<int64_t>();
     K.sig = w->k_sig.as<int64_t>(); K.hap = w->k_hap.as<int32_t>();
-    w->launches = 0;
-    C3B_CUDA(cudaEventRecord(w->ev0, s));
+    w->launches[0] = 0;
+    C3B_CUDA(cudaEventRecord(w->ev[0][0], s));
     int64_t nF = 0, n_kept = 0, n_pool = 0, n_sig = 0;
     if (n_cand > 0) {
         fa_flank_count_kernel<<<blocks_for(n_cand, 256), 256, 0, s>>>(w->in_cand.as<int64_t>(), n_cand, w->fstart.as<int64_t>(),
                                                                        w->fcnt.as<int64_t>());
-        fa_scan_kernel<<<1, 1024, 0, s>>>(w->fcnt.as<int64_t>(), w->foff.as<int64_t>(), n_cand, cnt + 0, 0);
+        block_scan_sum(w->fcnt.as<int64_t>(), w->foff.as<int64_t>(), n_cand, nullptr, cnt + 0, s);
         fa_flank_fill_kernel<<<(unsigned)n_cand, 64, 0, s>>>(w->fstart.as<int64_t>(), w->fcnt.as<int64_t>(), w->foff.as<int64_t>(),
                                                              n_cand, w->F.as<int64_t>());
-        w->launches += 3;
+        w->launches[0] += 3;
         // the size of F bounds the binary searches of K3 and K11
         C3B_CUDA(cudaMemcpyAsync(&w->host_counters[0], cnt + 0, 8, cudaMemcpyDeviceToHost, s));
         C3B_CUDA(cudaStreamSynchronize(s));
@@ -1133,13 +1070,13 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
                                                                    w->table.as<int64_t>(), (uint32_t)(T - 1));
             fa_read_keep_kernel<<<blocks_for(n, 256), 256, 0, s>>>(R, w->pass.as<uint8_t>(), w->rov.as<int32_t>(), w->table.as<int64_t>(),
                                                                    (uint32_t)(T - 1), w->keep.as<int64_t>(), w->kovr.as<int64_t>());
-            fa_scan_kernel<<<1, 1024, 0, s>>>(w->keep.as<int64_t>(), w->kidx.as<int64_t>(), n, cnt + 1, 0);
-            fa_scan_kernel<<<1, 1024, 0, s>>>(w->kovr.as<int64_t>(), w->kov_ex.as<int64_t>(), n, cnt + 2, 0);
+            block_scan_sum(w->keep.as<int64_t>(), w->kidx.as<int64_t>(), n, nullptr, cnt + 1, s);
+            block_scan_sum(w->kovr.as<int64_t>(), w->kov_ex.as<int64_t>(), n, nullptr, cnt + 2, s);
             fa_read_compact_kernel<<<blocks_for(n, 256), 256, 0, s>>>(R, params->dwell, w->keep.as<int64_t>(), w->kidx.as<int64_t>(),
                                                                       w->kov_ex.as<int64_t>(), w->rend.as<int64_t>(), w->rlo.as<int64_t>(),
                                                                       w->rov.as<int32_t>(), K, w->sig_len.as<int64_t>());
-            fa_scan_kernel<<<1, 1024, 0, s>>>(w->sig_len.as<int64_t>(), w->sig_ex.as<int64_t>(), n, cnt + 3, 0);
-            w->launches += 6;
+            block_scan_sum(w->sig_len.as<int64_t>(), w->sig_ex.as<int64_t>(), n, nullptr, cnt + 3, s);
+            w->launches[0] += 6;
             // the kept-read count and the pool sizes
             C3B_CUDA(cudaMemcpyAsync(w->host_counters, cnt, 32, cudaMemcpyDeviceToHost, s));
             C3B_CUDA(cudaStreamSynchronize(s));
@@ -1152,28 +1089,28 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     if (n_kept > 0) {
         if (grow(w->pool, (size_t)n_pool * sizeof(PosInfo)) || grow(w->sig, (size_t)(n_sig > 0 ? n_sig : 1) * 4)) return 1;
         C3B_CUDA(cudaMemsetAsync(w->pool.p, 0, (size_t)n_pool * sizeof(PosInfo), s));
-        fa_scan_kernel<<<1, 1024, 0, s>>>(K.end, K.pmax, n_kept, nullptr, 1);
-        w->launches += 1;
+        block_scan_max(K.end, K.pmax, n_kept, s);
+        w->launches[0] += 1;
         if (n_sig > 0) C3B_CUDA(cudaMemsetAsync(w->sig.p, 0, (size_t)n_sig * 4, s));
         fa_signal_kernel<<<blocks_for(n_kept, 256), 256, 0, s>>>(R, K, w->sig_len.as<int64_t>(), w->sig_ex.as<int64_t>(), n_kept,
                                                                  w->sig.as<int32_t>());
-        w->launches += 1;
+        w->launches[0] += 1;
         if (params->need_haplotagging && n_var > 0) {
             HapArgs H;
             H.R = R; H.K = K; H.n_kept = n_kept; H.var = w->in_var.as<c3b_fa_variant>(); H.n_var = n_var;
             H.ref = dref; H.ref_start = ref_start; H.ref_len = ref_len > 0 ? ref_len : 0; H.status = status;
             fa_haplotag_kernel<<<blocks_for(n_kept, 128), 128, 0, s>>>(H);
-            w->launches += 1;
+            w->launches[0] += 1;
         }
         fa_pos_info_kernel<<<blocks_for(n_kept, 128), 128, 0, s>>>(R, K, n_kept, w->F.as<int64_t>(), w->sig.as<int32_t>(),
                                                                    w->pool.as<PosInfo>());
-        w->launches += 1;
+        w->launches[0] += 1;
     }
     if (n_cand > 0) {
         fa_select_count_kernel<<<blocks_for(n_cand * 32, 256), 256, 0, s>>>(w->in_cand.as<int64_t>(), n_cand, K, n_kept, depth,
                                                                           w->ra.as<int64_t>(), w->rb.as<int64_t>(),
                                                                           w->nsel.as<int64_t>(), w->draws.as<int64_t>());
-        fa_scan_kernel<<<1, 1024, 0, s>>>(w->draws.as<int64_t>(), w->draw_off.as<int64_t>(), n_cand, cnt + 4, 0);
+        block_scan_sum(w->draws.as<int64_t>(), w->draw_off.as<int64_t>(), n_cand, nullptr, cnt + 4, s);
         CandArgs A;
         A.R = R; A.K = K; A.cand = w->in_cand.as<int64_t>(); A.F = w->F.as<int64_t>(); A.nF = nF; A.pool = w->pool.as<PosInfo>();
         A.ref = dref; A.ref_start = ref_start; A.ref_len = ref_len > 0 ? ref_len : 0;
@@ -1184,9 +1121,9 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
         A.al_n = w->al_n.as<int32_t>(); A.al_meta = w->al_meta.as<uint32_t>(); A.al_read = w->al_read.as<uint32_t>();
         A.al_qpos = w->al_qpos.as<uint32_t>(); A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_used = al_used; A.status = status;
         fa_candidate_kernel<<<(unsigned)n_cand, CAND_THREADS, 0, s>>>(A);
-        w->launches += 2;
+        w->launches[0] += 2;
     }
-    C3B_CUDA(cudaEventRecord(w->ev1, s));
+    C3B_CUDA(cudaEventRecord(w->ev[0][1], s));
     C3B_CUDA(cudaGetLastError());
     C3B_CUDA(cudaMemcpyAsync(w->host_counters, cnt, 64, cudaMemcpyDeviceToHost, s));
     w->built = true;
@@ -1214,13 +1151,9 @@ int c3b_fa_sizes(c3b_fa *w, int64_t *n_cand, int64_t *n_kept, int64_t *rand_draw
 
 int c3b_fa_fetch(c3b_fa *w, int8_t *matrix, int32_t *kept_haplotype, int64_t *kept_read) {
     if (c3b_fa_sizes(w, nullptr, nullptr, nullptr)) return 1;
-    cudaStream_t s = w->stream;
-    const size_t nm = (size_t)w->n_cand * (size_t)w->depth * 33 * (size_t)w->C;
-    if (matrix && nm) C3B_CUDA(cudaMemcpyAsync(matrix, w->matrix.p, nm, cudaMemcpyDeviceToHost, s));
-    if (kept_haplotype && w->n_kept) C3B_CUDA(cudaMemcpyAsync(kept_haplotype, w->k_hap.p, (size_t)w->n_kept * 4, cudaMemcpyDeviceToHost, s));
-    if (kept_read && w->n_kept) C3B_CUDA(cudaMemcpyAsync(kept_read, w->k_orig.p, (size_t)w->n_kept * 8, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    const size_t nm = (size_t)w->n_cand * (size_t)w->depth * 33 * (size_t)w->C, nk = (size_t)w->n_kept;
+    return w->get(matrix, w->matrix, nm) || w->get(kept_haplotype, w->k_hap, nk * 4) || w->get(kept_read, w->k_orig, nk * 8) ||
+           w->wait();
 }
 
 int c3b_fa_fetch_alleles(c3b_fa *w, int32_t *depth, int32_t *acgt, int32_t *al_off, int32_t *al_n, uint32_t *meta, uint32_t *read,
@@ -1228,23 +1161,9 @@ int c3b_fa_fetch_alleles(c3b_fa *w, int32_t *depth, int32_t *acgt, int32_t *al_o
     if (c3b_fa_sizes(w, nullptr, nullptr, nullptr)) return 1;
     const int64_t used = w->host_counters[6], n = used < AL_CAP ? used : AL_CAP;
     if (n_alleles) *n_alleles = n;
-    cudaStream_t s = w->stream;
     const size_t k = (size_t)w->n_cand;
-    if (depth && k) C3B_CUDA(cudaMemcpyAsync(depth, w->c_depth.p, k * 4, cudaMemcpyDeviceToHost, s));
-    if (acgt && k) C3B_CUDA(cudaMemcpyAsync(acgt, w->c_acgt.p, k * 16, cudaMemcpyDeviceToHost, s));
-    if (al_off && k) C3B_CUDA(cudaMemcpyAsync(al_off, w->al_off.p, k * 4, cudaMemcpyDeviceToHost, s));
-    if (al_n && k) C3B_CUDA(cudaMemcpyAsync(al_n, w->al_n.p, k * 4, cudaMemcpyDeviceToHost, s));
-    if (meta || read || qpos || cnt) {
-        if (capacity < n) { c3b_set_error("c3b_fa_fetch_alleles: capacity %lld < %lld records", (long long)capacity, (long long)n); return 1; }
-        if (n) {
-            if (meta) C3B_CUDA(cudaMemcpyAsync(meta, w->al_meta.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-            if (read) C3B_CUDA(cudaMemcpyAsync(read, w->al_read.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-            if (qpos) C3B_CUDA(cudaMemcpyAsync(qpos, w->al_qpos.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-            if (cnt) C3B_CUDA(cudaMemcpyAsync(cnt, w->al_cnt.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-        }
-    }
-    C3B_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    return w->get(depth, w->c_depth, k * 4) || w->get(acgt, w->c_acgt, k * 16) || w->get(al_off, w->al_off, k * 4) ||
+           w->get(al_n, w->al_n, k * 4) || w->get_alleles("c3b_fa_fetch_alleles", n, capacity, meta, read, qpos, cnt) || w->wait();
 }
 
 int c3b_fa_device(c3b_fa *w, const int8_t **matrix) {
@@ -1255,22 +1174,9 @@ int c3b_fa_device(c3b_fa *w, const int8_t **matrix) {
 
 int c3b_fa_last_ms(c3b_fa *w, float *ms, int *launches) {
     if (!w || !w->built) { c3b_set_error("c3b_fa_last_ms: no c3b_fa_build has been issued"); return 1; }
-    C3B_CUDA(cudaSetDevice(w->device));
-    C3B_CUDA(cudaEventSynchronize(w->ev1));
-    float t = 0.f;
-    C3B_CUDA(cudaEventElapsedTime(&t, w->ev0, w->ev1));
-    if (ms) *ms = t;
-    if (launches) *launches = w->launches;
-    return 0;
+    return w->elapsed(0, ms, launches);
 }
 
-void c3b_fa_destroy(c3b_fa *w) {
-    if (!w) return;
-    cudaSetDevice(w->device);
-    if (w->ev0) cudaEventDestroy(w->ev0);
-    if (w->ev1) cudaEventDestroy(w->ev1);
-    if (w->host_counters) cudaFreeHost(w->host_counters);
-    delete w;
-}
+void c3b_fa_destroy(c3b_fa *w) { c3b_region_destroy(w); }
 
 }  // extern "C"

@@ -13,7 +13,7 @@
 //                         probing, growth at 0.77 load at the start of a put, kh_resize's in-place kick-out rehash, one more
 //                         growth when a put of a present string follows the last new one - and leaves the bucket order; it then
 //                         walks the string once with a counting sink: the bytes of the full text and of the decoder form.
-//   T2 plp_scan_tiles     (plp_counts.cu) the two exclusive scans over n_cand + 1 lengths: per-candidate offsets and the totals.
+//   T2 (block_scan)       the two exclusive scans over n_cand + 1 lengths: per-candidate offsets and the totals.
 //   T3 plp_text_write     one THREAD per candidate walks the same string with a writing sink.
 //
 // Everything a column needs lives in global scratch addressed by its own record range (mate / hash / order) or by that range and
@@ -23,6 +23,7 @@
 // the status word.
 #include <limits.h>
 
+#include "block_scan.cuh"
 #include "c3b_internal.h"
 
 namespace {
@@ -127,8 +128,8 @@ template <class S> __device__ void plp_text_emit(const PlpAltTextArgs &A, const 
         ref_depth -= v;
         if (len <= A.max_indel_length) {
             const uint32_t r = A.al_read[i];
-            const uint8_t *sq = A.seq + A.seq_off[r];
-            const int lq = A.l_qseq[r];
+            const uint8_t *sq = A.R.seq + A.R.seq_off[r];
+            const int lq = A.R.l_qseq[r];
             const long long q0 = (long long)A.al_qpos[i];
             o.alt('I'); o.alt((char)rb);
             for (long long q = 0; q < len; ++q) o.alt(NT16[c3b_nib_at(sq, lq, q0 + q)]);
@@ -192,8 +193,8 @@ __global__ void __launch_bounds__(256) plp_text_measure_kernel(PlpAltTextArgs A)
             int lq = 0;
             long long q0 = 0;
             if (ins) {
-                sq = A.seq + A.seq_off[A.al_read[i]];
-                lq = A.l_qseq[A.al_read[i]];
+                sq = A.R.seq + A.R.seq_off[A.al_read[i]];
+                lq = A.R.l_qseq[A.al_read[i]];
                 q0 = (long long)A.al_qpos[i];
             }
             int m = -1;
@@ -201,8 +202,8 @@ __global__ void __launch_bounds__(256) plp_text_measure_kernel(PlpAltTextArgs A)
                 if (A.al_meta[k] != (meta ^ (1u << 30))) continue;
                 bool same = true;
                 if (ins) {
-                    const uint8_t *s2 = A.seq + A.seq_off[A.al_read[k]];
-                    const int lq2 = A.l_qseq[A.al_read[k]];
+                    const uint8_t *s2 = A.R.seq + A.R.seq_off[A.al_read[k]];
+                    const int lq2 = A.R.l_qseq[A.al_read[k]];
                     const long long q2 = (long long)A.al_qpos[k];
                     for (long long q = 0; q < len; ++q)
                         if (c3b_nib_at(sq, lq, q0 + q) != c3b_nib_at(s2, lq2, q2 + q)) { same = false; break; }
@@ -309,9 +310,8 @@ int c3b_launch_plp_alt_text(const PlpAltTextArgs &a, cudaStream_t s, int *launch
     int64_t blocks = ((a.W + 1) * 32 + 255) / 256;
     if (blocks > 132 * 8) blocks = 132 * 8;
     plp_text_measure_kernel<<<(unsigned)blocks, 256, 0, s>>>(a);
-    if (c3b_launch_plp_scan(a.len_text, a.text_off, (int)(a.W + 1), a.n_cand, a.totals, s) ||
-        c3b_launch_plp_scan(a.len_dec, a.dec_off, (int)(a.W + 1), a.n_cand, a.totals + 1, s))
-        return 1;
+    block_scan_sum(a.len_text, a.text_off, a.W + 1, a.n_cand, a.totals, s);
+    block_scan_sum(a.len_dec, a.dec_off, a.W + 1, a.n_cand, a.totals + 1, s);
     plp_text_write_kernel<<<(unsigned)((a.W + 127) / 128), 128, 0, s>>>(a);
     C3B_CUDA(cudaGetLastError());
     *launches = 4;

@@ -10,7 +10,7 @@
 //                        position p is the first one whose end offset exceeds p - pos (binary search), and htslib's
 //                        resolve_cigar2 (is_del / is_refskip / indel / qpos) is a pure function of that operation and its
 //                        neighbours.
-//   K2 plp_prefix_max    running maximum of the read ends (reads are sorted by start, not by end): the reads that can touch a
+//   K2 (block_scan)      running maximum of the read ends (reads are sorted by start, not by end): the reads that can touch a
 //                        column tile are [first i with pmax[i] > tile start, first i with pos[i] >= tile end).
 //   K3 plp_count_tile    one CTA per tile of 256 columns, ONE THREAD PER COLUMN.  The thread walks the tile's reads and owns every
 //                        counter of its column - the 18 features (in shared memory, [feature][column], conflict-free), the
@@ -18,7 +18,7 @@
 //                        spilling to a global pool) - so nothing on the counting path needs an atomic except pool allocation, and
 //                        the per-column semantics are literally the reference's (strings compared base by base, no hashing).  The
 //                        column's statistics and the allele-frequency test (float32 divisions as in the reference) follow.
-//   K4 / K7 plp_scan_tiles   exclusive scan of the per-tile covered-column / candidate counts (htslib reports only covered columns,
+//   K4 / K7 (block_scan) exclusive scan of the per-tile covered-column / candidate counts (htslib reports only covered columns,
 //                        so the matrix is a compaction of the region).
 //   K5 plp_emit          compaction: int64 rows (plp_data.matrix is size_t), major, stats, the 16-column flanking test.
 //   K6 plp_quirk         the reference's index -1 quirk: a non-ACGT read base increments feature 17 of the PREVIOUS emitted column.
@@ -30,8 +30,8 @@
 // once) + 144 + 8 + 24 B emitted: see DESIGN.md 3.8.
 #include <limits.h>
 #include <stdlib.h>
-#include <string.h>
 
+#include "block_scan.cuh"
 #include "c3b_internal.h"
 #include "../../include/clair3_b200_pileup.h"
 
@@ -45,23 +45,11 @@ constexpr int FLANK = 16;         // pileup_flanking_base_num, src/clair3_pileup
 constexpr int G_POOL = 1 << 21;   // global overflow nodes per workspace
 constexpr int AL_CAP = 1 << 22;   // exported allele records per call (16 B each)
 
-struct DevReads {
-    int64_t n;
-    const int64_t *pos;
-    const uint16_t *flag;
-    const uint8_t *mapq;
-    const int64_t *cigar_off;
-    const uint32_t *cigar;
-    const int64_t *seq_off;
-    const uint8_t *seq;
-    const int32_t *l_qseq;
-};
-
 __device__ __forceinline__ bool ref_cons(uint32_t op) { return (0x18Du >> op) & 1u; }   // M D N = X
 __device__ __forceinline__ bool qry_cons(uint32_t op) { return (0x193u >> op) & 1u; }   // M I S = X
 
 // ---------------------------------------------------------------------------------------------------------------- K1
-__global__ void plp_scan_reads_kernel(DevReads R, int min_mq, int32_t *__restrict__ opx_end, int32_t *__restrict__ opy,
+__global__ void plp_scan_reads_kernel(C3bReads R, int min_mq, int32_t *__restrict__ opx_end, int32_t *__restrict__ opy,
                                       int64_t *__restrict__ rend, int *status) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -101,42 +89,9 @@ __global__ void plp_scan_reads_kernel(DevReads R, int min_mq, int32_t *__restric
     }
 }
 
-// ---------------------------------------------------------------------------------------------------------------- K2
-__global__ void plp_prefix_max_kernel(const int64_t *__restrict__ rend, int64_t *__restrict__ pmax, int64_t n) {
-    __shared__ long long wmax[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    long long carry = LLONG_MIN;
-    for (int64_t base = 0; base < n; base += 1024) {
-        const int64_t i = base + threadIdx.x;
-        long long v = i < n ? (long long)rend[i] : LLONG_MIN;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const long long a = __shfl_up_sync(0xffffffffu, v, d);
-            if (lane >= d && a > v) v = a;
-        }
-        if (lane == 31) wmax[warp] = v;
-        __syncthreads();
-        if (warp == 0) {
-            long long t = wmax[lane];
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const long long a = __shfl_up_sync(0xffffffffu, t, d);
-                if (lane >= d && a > t) t = a;
-            }
-            wmax[lane] = t;
-        }
-        __syncthreads();
-        if (warp > 0 && wmax[warp - 1] > v) v = wmax[warp - 1];
-        if (carry > v) v = carry;
-        if (i < n) pmax[i] = v;
-        if (wmax[31] > carry) carry = wmax[31];
-        __syncthreads();
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------------- K3
 struct CountArgs {
-    DevReads R;
+    C3bReads R;
     const int32_t *opx_end;
     const int32_t *opy;
     const int64_t *rend;
@@ -431,43 +386,6 @@ __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
     }
 }
 
-// ---------------------------------------------------------------------------------------------------------------- K4 / K7
-// n_dev (optional): the scan stops after *n_dev + 1 entries when that is fewer than n
-__global__ void plp_scan_tiles_kernel(const int32_t *__restrict__ cnt, int64_t *__restrict__ off, int n, const int64_t *n_dev,
-                                      int64_t *total) {
-    __shared__ long long wsum[32];
-    if (n_dev && *n_dev + 1 < n) n = (int)(*n_dev + 1);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    long long carry = 0;
-    for (int base = 0; base < n; base += 1024) {
-        const int i = base + threadIdx.x;
-        const long long own = i < n ? (long long)cnt[i] : 0;
-        long long v = own;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const long long a = __shfl_up_sync(0xffffffffu, v, d);
-            if (lane >= d) v += a;
-        }
-        if (lane == 31) wsum[warp] = v;
-        __syncthreads();
-        if (warp == 0) {
-            long long t = wsum[lane];
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const long long a = __shfl_up_sync(0xffffffffu, t, d);
-                if (lane >= d) t += a;
-            }
-            wsum[lane] = t;
-        }
-        __syncthreads();
-        const long long incl = v + (warp > 0 ? wsum[warp - 1] : 0) + carry;
-        if (i < n) off[i] = incl - own;
-        carry += wsum[31];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total = carry;
-}
-
 // ---------------------------------------------------------------------------------------------------------------- K5
 struct EmitArgs {
     int64_t start, end;
@@ -607,61 +525,34 @@ __global__ void __launch_bounds__(TILE) plp_cands_kernel(CandArgs A) {
 
 }  // namespace
 
-struct c3b_plp {
-    int device = 0;
+// Timed stages: 0 the count (c3b_plp_count), 1 the text (c3b_plp_alt_text).  counters: int64 n_cols, int64 n_cand, int g_used,
+// int status, int al_used, int text_status, int64 n_text_bytes, int64 n_decoder_bytes.  al_*: the allele export (params.alt_info).
+struct c3b_plp : C3bRegionWorkspace {
     // inputs (copies of host records)
     C3bBuf in_core[8], in_ref;
     // scratch
     C3bBuf opx, opy, rend, pmax, rows32, dstats, nquirk, dci, tile_cov, tile_off, tile_cand, tile_coff;
     C3bBuf g_meta, g_read, g_qpos, g_cnt, g_next;
-    C3bBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n, ins_last;   // allele export (params.alt_info)
-    C3bBuf counters;    // int64 n_cols, int64 n_cand, int g_used, int status, int al_used, int text_status, int64 n_text_bytes, int64 n_decoder_bytes
+    C3bBuf al_off, al_n, ins_last;
     // outputs
     C3bBuf matrix, major, stats, cand_cols, wstart, wbounds, cand_ok, gv_ref, gv_tot;
     int64_t W = 0;
     bool gvcf = false, counted = false, alleles = false;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    int launches = 0;
-    int64_t *host_counters = nullptr;   // pinned copy of `counters`
     int64_t n_cols = -1, n_cand = -1;
     // the text stage (c3b_plp_alt_text): where the count left its inputs, scratch, outputs
-    DevReads R;
+    C3bReads R;
     const char *dref = nullptr;
     int64_t start = 0, end = 0, ref_start = 0, ref_len = 0, n_cigar = 0, n_seq = 0;
     C3bBuf tx_mate, tx_hash, tx_order, tx_table, tx_nins, tx_ndel, tx_len_text, tx_len_dec;
     C3bBuf text, dec, text_off, dec_off, ref_base, position;
     bool texted = false;
-    cudaEvent_t ev2 = nullptr, ev3 = nullptr;
-    int text_launches = 0;
 };
 
 constexpr int N_COUNTERS = 6;
 
-int c3b_launch_plp_scan(const int32_t *cnt, int64_t *off, int n, const int64_t *n_dev, int64_t *total, cudaStream_t s) {
-    plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(cnt, off, n, n_dev, total);
-    C3B_CUDA(cudaGetLastError());
-    return 0;
-}
-
 extern "C" {
 
-int c3b_plp_create(c3b_plp **out, int device_ordinal) {
-    if (!out) { c3b_set_error("c3b_plp_create: null out"); return 1; }
-    *out = nullptr;
-    if (c3b_use_device(device_ordinal, 1, nullptr)) return 1;
-    c3b_plp *w = new c3b_plp();
-    w->device = device_ordinal;
-    if (cudaEventCreate(&w->ev0) != cudaSuccess || cudaEventCreate(&w->ev1) != cudaSuccess ||
-        cudaEventCreate(&w->ev2) != cudaSuccess || cudaEventCreate(&w->ev3) != cudaSuccess ||
-        cudaMallocHost((void **)&w->host_counters, N_COUNTERS * sizeof(int64_t)) != cudaSuccess) {
-        c3b_set_error("c3b_plp_create: event / pinned allocation failed");
-        c3b_plp_destroy(w);
-        return 1;
-    }
-    *out = w;
-    return 0;
-}
+int c3b_plp_create(c3b_plp **out, int device_ordinal) { return c3b_region_create(out, device_ordinal, 2, N_COUNTERS, "c3b_plp_create"); }
 
 int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64_t start, int64_t end, const char *ref_seq,
                   int64_t ref_start, int64_t ref_len, const c3b_plp_params *params, void *cuda_stream) {
@@ -686,8 +577,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     const int tiles = (int)((W + TILE - 1) / TILE);
 
     // inputs
-    DevReads R;
-    memset(&R, 0, sizeof(R));
+    C3bReads R{};
     R.n = n;
     int64_t n_cigar = 0, n_seq = 0;
     if (n > 0) {
@@ -711,7 +601,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         grow(w->nquirk, Wz * 4) || grow(w->dci, Wz * 4) || grow(w->tile_cov, Tz * 4) || grow(w->tile_off, Tz * 8) ||
         grow(w->tile_cand, Tz * 4) || grow(w->tile_coff, Tz * 8) || grow(w->g_meta, (size_t)G_POOL * 4) ||
         grow(w->g_read, (size_t)G_POOL * 4) || grow(w->g_qpos, (size_t)G_POOL * 4) || grow(w->g_cnt, (size_t)G_POOL * 4) ||
-        grow(w->g_next, (size_t)G_POOL * 4) || grow(w->counters, N_COUNTERS * 8) || grow(w->matrix, Wz * NFEAT * 8) ||
+        grow(w->g_next, (size_t)G_POOL * 4) || grow(w->matrix, Wz * NFEAT * 8) ||
         grow(w->major, Wz * 8) || grow(w->stats, Wz * 6 * 4) || grow(w->cand_cols, Wz * 8) || grow(w->wstart, Wz * 8) ||
         grow(w->wbounds, Wz * 16) || grow(w->cand_ok, Wz))
         return 1;
@@ -732,15 +622,15 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     int *status = g_used + 1;
     int *al_used = reinterpret_cast<int *>(n_cols_dev + 3);
 
-    w->launches = 0;
-    C3B_CUDA(cudaEventRecord(w->ev0, s));
+    w->launches[0] = 0;
+    C3B_CUDA(cudaEventRecord(w->ev[0][0], s));
     if (W > 0) {
         if (n > 0) {
             int blocks = (int)((n * 32 + 255) / 256);
             if (blocks > 132 * 8) blocks = 132 * 8;
             plp_scan_reads_kernel<<<blocks, 256, 0, s>>>(R, params->min_mq, w->opx.as<int32_t>(), w->opy.as<int32_t>(), w->rend.as<int64_t>(), status);
-            plp_prefix_max_kernel<<<1, 1024, 0, s>>>(w->rend.as<int64_t>(), w->pmax.as<int64_t>(), n);
-            w->launches += 2;
+            block_scan_max(w->rend.as<int64_t>(), w->pmax.as<int64_t>(), n, s);
+            w->launches[0] += 2;
         }
         CountArgs A;
         A.R = R;
@@ -757,7 +647,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         A.ins_last = w->ins_last.as<int32_t>(); A.al_used = al_used; A.al_cap = AL_CAP;
         const size_t smem = (size_t)NCNT * TILE * 4 + (size_t)NP * 20;
         plp_count_tile_kernel<<<tiles, TILE, smem, s>>>(A);
-        plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(w->tile_cov.as<int32_t>(), w->tile_off.as<int64_t>(), tiles, nullptr, n_cols_dev);
+        block_scan_sum(w->tile_cov.as<int32_t>(), w->tile_off.as<int64_t>(), tiles, nullptr, n_cols_dev, s);
         EmitArgs E;
         E.start = start; E.end = end; E.call_ht = params->call_ht;
         E.rows32 = w->rows32.as<int32_t>(); E.dstats = w->dstats.as<int32_t>(); E.tile_off = w->tile_off.as<int64_t>();
@@ -766,16 +656,16 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         plp_emit_kernel<<<tiles, TILE, 0, s>>>(E);
         plp_quirk_kernel<<<(unsigned)((W + 255) / 256), 256, 0, s>>>(n_cols_dev, w->major.as<int64_t>(), w->nquirk.as<int32_t>(), start,
                                                                       w->matrix.as<int64_t>(), w->stats.as<int32_t>());
-        plp_scan_tiles_kernel<<<1, 1024, 0, s>>>(w->tile_cand.as<int32_t>(), w->tile_coff.as<int64_t>(), tiles, nullptr, n_cand_dev);
+        block_scan_sum(w->tile_cand.as<int32_t>(), w->tile_coff.as<int64_t>(), tiles, nullptr, n_cand_dev, s);
         CandArgs C;
         C.start = start; C.end = end; C.n_cols_dev = n_cols_dev; C.dci = w->dci.as<int32_t>(); C.stats = w->stats.as<int32_t>();
         C.major = w->major.as<int64_t>(); C.tile_coff = w->tile_coff.as<int64_t>(); C.cand_cols = w->cand_cols.as<int64_t>();
         C.wstart = w->wstart.as<int64_t>(); C.wbounds = w->wbounds.as<int64_t>(); C.cand_ok = w->cand_ok.as<uint8_t>();
         C.call_ht = params->call_ht;
         plp_cands_kernel<<<tiles, TILE, 0, s>>>(C);
-        w->launches += 6;
+        w->launches[0] += 6;
     }
-    C3B_CUDA(cudaEventRecord(w->ev1, s));
+    C3B_CUDA(cudaEventRecord(w->ev[0][1], s));
     C3B_CUDA(cudaGetLastError());
     C3B_CUDA(cudaMemcpyAsync(w->host_counters, w->counters.p, 32, cudaMemcpyDeviceToHost, s));
     w->counted = true;
@@ -803,18 +693,11 @@ int c3b_plp_fetch(c3b_plp *w, int64_t *matrix, int64_t *major, int32_t *stats, i
                   int64_t *pos_ref_count, int64_t *pos_total_count) {
     if (!w) { c3b_set_error("c3b_plp_fetch: null workspace"); return 1; }
     if (w->n_cols < 0 && c3b_plp_sizes(w, nullptr, nullptr)) return 1;
-    cudaStream_t s = w->stream;
-    const size_t nc = (size_t)w->n_cols, nk = (size_t)w->n_cand;
-    if (matrix && nc) C3B_CUDA(cudaMemcpyAsync(matrix, w->matrix.p, nc * NFEAT * 8, cudaMemcpyDeviceToHost, s));
-    if (major && nc) C3B_CUDA(cudaMemcpyAsync(major, w->major.p, nc * 8, cudaMemcpyDeviceToHost, s));
-    if (stats && nc) C3B_CUDA(cudaMemcpyAsync(stats, w->stats.p, nc * 6 * 4, cudaMemcpyDeviceToHost, s));
-    if (cand_cols && nk) C3B_CUDA(cudaMemcpyAsync(cand_cols, w->cand_cols.p, nk * 8, cudaMemcpyDeviceToHost, s));
-    if (cand_ok && nk) C3B_CUDA(cudaMemcpyAsync(cand_ok, w->cand_ok.p, nk, cudaMemcpyDeviceToHost, s));
     if ((pos_ref_count || pos_total_count) && !w->gvcf) { c3b_set_error("c3b_plp_fetch: the count ran without params.gvcf"); return 1; }
-    if (pos_ref_count && w->W) C3B_CUDA(cudaMemcpyAsync(pos_ref_count, w->gv_ref.p, (size_t)w->W * 8, cudaMemcpyDeviceToHost, s));
-    if (pos_total_count && w->W) C3B_CUDA(cudaMemcpyAsync(pos_total_count, w->gv_tot.p, (size_t)w->W * 8, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    const size_t nc = (size_t)w->n_cols, nk = (size_t)w->n_cand, W = (size_t)w->W;
+    return w->get(matrix, w->matrix, nc * NFEAT * 8) || w->get(major, w->major, nc * 8) || w->get(stats, w->stats, nc * 6 * 4) ||
+           w->get(cand_cols, w->cand_cols, nk * 8) || w->get(cand_ok, w->cand_ok, nk) || w->get(pos_ref_count, w->gv_ref, W * 8) ||
+           w->get(pos_total_count, w->gv_tot, W * 8) || w->wait();
 }
 
 int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, int32_t *ins_last, uint32_t *meta, uint32_t *read, uint32_t *qpos, uint32_t *cnt,
@@ -824,21 +707,9 @@ int c3b_plp_fetch_alleles(c3b_plp *w, int32_t *al_off, int32_t *al_n, int32_t *i
     if (!w->alleles) { c3b_set_error("c3b_plp_fetch_alleles: the count ran without params.alt_info"); return 1; }
     const int64_t n = (int64_t)(int)(w->host_counters[3] & 0xffffffffll);
     if (n_alleles) *n_alleles = n;
-    cudaStream_t s = w->stream;
-    if (al_off && w->W) C3B_CUDA(cudaMemcpyAsync(al_off, w->al_off.p, (size_t)w->W * 4, cudaMemcpyDeviceToHost, s));
-    if (al_n && w->W) C3B_CUDA(cudaMemcpyAsync(al_n, w->al_n.p, (size_t)w->W * 4, cudaMemcpyDeviceToHost, s));
-    if (ins_last && w->W) C3B_CUDA(cudaMemcpyAsync(ins_last, w->ins_last.p, (size_t)w->W * 4, cudaMemcpyDeviceToHost, s));
-    if (meta || read || qpos || cnt) {
-        if (capacity < n) { c3b_set_error("c3b_plp_fetch_alleles: capacity %lld < %lld records", (long long)capacity, (long long)n); return 1; }
-        if (n) {
-            if (meta) C3B_CUDA(cudaMemcpyAsync(meta, w->al_meta.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-            if (read) C3B_CUDA(cudaMemcpyAsync(read, w->al_read.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-            if (qpos) C3B_CUDA(cudaMemcpyAsync(qpos, w->al_qpos.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-            if (cnt) C3B_CUDA(cudaMemcpyAsync(cnt, w->al_cnt.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-        }
-    }
-    C3B_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    const size_t W = (size_t)w->W;
+    return w->get(al_off, w->al_off, W * 4) || w->get(al_n, w->al_n, W * 4) || w->get(ins_last, w->ins_last, W * 4) ||
+           w->get_alleles("c3b_plp_fetch_alleles", n, capacity, meta, read, qpos, cnt) || w->wait();
 }
 
 int c3b_plp_device(c3b_plp *w, const int64_t **matrix, const int64_t **major, const int64_t **cand_cols,
@@ -860,8 +731,7 @@ int c3b_plp_window_bounds(c3b_plp *w, int64_t *bounds, const int64_t **device_bo
     }
     if (bounds) {
         if (w->n_cols < 0 && c3b_plp_sizes(w, nullptr, nullptr)) return 1;
-        if (w->n_cand) C3B_CUDA(cudaMemcpyAsync(bounds, w->wbounds.p, (size_t)w->n_cand * 16, cudaMemcpyDeviceToHost, w->stream));
-        C3B_CUDA(cudaStreamSynchronize(w->stream));
+        return w->get(bounds, w->wbounds, (size_t)w->n_cand * 16) || w->wait();
     }
     return 0;
 }
@@ -889,11 +759,11 @@ int c3b_plp_alt_text(c3b_plp *w, int64_t max_indel_length) {
         return 1;
     w->texted = false;
     w->n_cols = w->n_cand = -1;           // the status word and the totals travel with the next c3b_plp_sizes
-    w->text_launches = 0;
+    w->launches[1] = 0;
     int64_t *cnt = w->counters.as<int64_t>();
     int *text_status = reinterpret_cast<int *>(cnt + 3) + 1;       // the stage's own word: an earlier stage's overflow is not this one's
     C3B_CUDA(cudaMemsetAsync(text_status, 0, sizeof(int), s));
-    C3B_CUDA(cudaEventRecord(w->ev2, s));
+    C3B_CUDA(cudaEventRecord(w->ev[1][0], s));
     if (W > 0) {
         PlpAltTextArgs A;
         A.start = w->start; A.end = w->end; A.ref_start = w->ref_start; A.ref_len = w->ref_len; A.max_indel_length = max_indel_length;
@@ -901,7 +771,7 @@ int c3b_plp_alt_text(c3b_plp *w, int64_t max_indel_length) {
         A.n_cand = cnt + 1;
         A.cand_cols = w->cand_cols.as<int64_t>(); A.major = w->major.as<int64_t>(); A.matrix = w->matrix.as<int64_t>();
         A.stats = w->stats.as<int32_t>(); A.ref = w->dref;
-        A.seq_off = w->R.seq_off; A.seq = w->R.seq; A.l_qseq = w->R.l_qseq;
+        A.R = w->R;
         A.al_off = w->al_off.as<int32_t>(); A.al_n = w->al_n.as<int32_t>(); A.ins_last = w->ins_last.as<int32_t>();
         A.al_meta = w->al_meta.as<uint32_t>(); A.al_read = w->al_read.as<uint32_t>(); A.al_qpos = w->al_qpos.as<uint32_t>();
         A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_cap = cap;
@@ -912,12 +782,12 @@ int c3b_plp_alt_text(c3b_plp *w, int64_t max_indel_length) {
         A.text = w->text.as<char>(); A.dec = w->dec.as<char>(); A.text_cap = A.dec_cap = text_cap;
         A.text_off = w->text_off.as<int64_t>(); A.dec_off = w->dec_off.as<int64_t>(); A.totals = cnt + 4;
         A.ref_base = w->ref_base.as<uint8_t>(); A.position = w->position.as<int64_t>();
-        if (c3b_launch_plp_alt_text(A, s, &w->text_launches)) return 1;
+        if (c3b_launch_plp_alt_text(A, s, &w->launches[1])) return 1;
     } else {
         C3B_CUDA(cudaMemsetAsync(w->text_off.p, 0, 8, s));
         C3B_CUDA(cudaMemsetAsync(w->dec_off.p, 0, 8, s));
     }
-    C3B_CUDA(cudaEventRecord(w->ev3, s));
+    C3B_CUDA(cudaEventRecord(w->ev[1][1], s));
     C3B_CUDA(cudaMemcpyAsync(w->host_counters, w->counters.p, N_COUNTERS * 8, cudaMemcpyDeviceToHost, s));
     w->texted = true;
     return 0;
@@ -939,16 +809,10 @@ int c3b_plp_fetch_alt_text(c3b_plp *w, char *text, int64_t *text_off, char *deco
                            int64_t *position) {
     int64_t nt = 0, nd = 0;
     if (c3b_plp_alt_text_sizes(w, &nt, &nd)) return 1;
-    cudaStream_t s = w->stream;
     const size_t nk = (size_t)w->n_cand;
-    if (text && nt) C3B_CUDA(cudaMemcpyAsync(text, w->text.p, (size_t)nt, cudaMemcpyDeviceToHost, s));
-    if (text_off) C3B_CUDA(cudaMemcpyAsync(text_off, w->text_off.p, (nk + 1) * 8, cudaMemcpyDeviceToHost, s));
-    if (decoder && nd) C3B_CUDA(cudaMemcpyAsync(decoder, w->dec.p, (size_t)nd, cudaMemcpyDeviceToHost, s));
-    if (decoder_off) C3B_CUDA(cudaMemcpyAsync(decoder_off, w->dec_off.p, (nk + 1) * 8, cudaMemcpyDeviceToHost, s));
-    if (ref_base && nk) C3B_CUDA(cudaMemcpyAsync(ref_base, w->ref_base.p, nk, cudaMemcpyDeviceToHost, s));
-    if (position && nk) C3B_CUDA(cudaMemcpyAsync(position, w->position.p, nk * 8, cudaMemcpyDeviceToHost, s));
-    C3B_CUDA(cudaStreamSynchronize(s));
-    return 0;
+    return w->get(text, w->text, (size_t)nt) || w->get(text_off, w->text_off, (nk + 1) * 8) || w->get(decoder, w->dec, (size_t)nd) ||
+           w->get(decoder_off, w->dec_off, (nk + 1) * 8) || w->get(ref_base, w->ref_base, nk) ||
+           w->get(position, w->position, nk * 8) || w->wait();
 }
 
 int c3b_plp_alt_text_device(c3b_plp *w, const char **text, const int64_t **text_off, const char **decoder,
@@ -965,35 +829,14 @@ int c3b_plp_alt_text_device(c3b_plp *w, const char **text, const int64_t **text_
 
 int c3b_plp_alt_text_last_ms(c3b_plp *w, float *ms, int *launches) {
     if (!w || !w->texted) { c3b_set_error("c3b_plp_alt_text_last_ms: no c3b_plp_alt_text has been issued"); return 1; }
-    C3B_CUDA(cudaSetDevice(w->device));
-    C3B_CUDA(cudaEventSynchronize(w->ev3));
-    float t = 0.f;
-    C3B_CUDA(cudaEventElapsedTime(&t, w->ev2, w->ev3));
-    if (ms) *ms = t;
-    if (launches) *launches = w->text_launches;
-    return 0;
+    return w->elapsed(1, ms, launches);
 }
 
 int c3b_plp_last_ms(c3b_plp *w, float *ms, int *launches) {
     if (!w || !w->counted) { c3b_set_error("c3b_plp_last_ms: no c3b_plp_count has been issued"); return 1; }
-    C3B_CUDA(cudaSetDevice(w->device));
-    C3B_CUDA(cudaEventSynchronize(w->ev1));
-    float t = 0.f;
-    C3B_CUDA(cudaEventElapsedTime(&t, w->ev0, w->ev1));
-    if (ms) *ms = t;
-    if (launches) *launches = w->launches;
-    return 0;
+    return w->elapsed(0, ms, launches);
 }
 
-void c3b_plp_destroy(c3b_plp *w) {
-    if (!w) return;
-    cudaSetDevice(w->device);
-    if (w->ev0) cudaEventDestroy(w->ev0);
-    if (w->ev1) cudaEventDestroy(w->ev1);
-    if (w->ev2) cudaEventDestroy(w->ev2);
-    if (w->ev3) cudaEventDestroy(w->ev3);
-    if (w->host_counters) cudaFreeHost(w->host_counters);
-    delete w;
-}
+void c3b_plp_destroy(c3b_plp *w) { c3b_region_destroy(w); }
 
 }  // extern "C"

@@ -13,31 +13,14 @@ import gzip
 import numpy as np
 import torch
 
-from ._ffi import C3BError, check, ffi, lib
-from .pileup_counts import BamRecords, DeviceBamRecords, _insertion_bytes, khash_iteration_order
+from ._ffi import CONSTANTS, C3BError, check, ffi, lib
+from .pileup_counts import BamRecords, DeviceBamRecords, _insertion_bytes, _records_struct, _Workspace, khash_iteration_order
 
 FLANKING = 16                   # shared/param_f.py flankingBaseNum
 NO_OF_POSITIONS = 33
 MATRIX_DEPTH = {"ont": 89, "hifi": 55, "ilmn": 55}      # shared/param_f.py matrix_depth_dict
 _ACGT = "ACGT"
 _ACGT2NUM = {"C": 1, "G": 2, "T": 3}                    # acgt2num (src/clair3_full_alignment_dwell.h:49-54): others -> 0
-
-
-def _fa_struct(rec, on_dev):
-    s = ffi.new("c3b_fa_records *")
-    s.core = rec._struct()[0]
-    for k, ct in (("qual", "uint8_t"), ("qname", "uint8_t"), ("mv", "int32_t")):
-        if on_dev:
-            v, o = rec.t.get(k), rec.t.get(k + "_off")
-            vp, op = (ffi.NULL, ffi.NULL) if o is None else (v.data_ptr(), o.data_ptr())
-        else:
-            v, o = getattr(rec, k, None), getattr(rec, k + "_off", None)
-            vp, op = (ffi.NULL, ffi.NULL) if o is None else (v.ctypes.data if v.size else ffi.NULL, o.ctypes.data)
-        if o is not None and vp == ffi.NULL:
-            vp = ffi.cast("void *", 8)          # an empty value array with valid offsets: never dereferenced
-        setattr(s, k + "_off", ffi.cast("const int64_t *", op))
-        setattr(s, k, ffi.cast("const %s *" % ct, vp))
-    return s
 
 
 def _variant_array(variants):
@@ -53,20 +36,14 @@ def _variant_array(variants):
     return arr, n
 
 
-class FullAlignmentBuilder:
+class FullAlignmentBuilder(_Workspace):
     """One tensor-building workspace on one H100 (``c3b_fa``).  ``build()`` is asynchronous on the current torch stream of the
     device (apart from two short waits that size its scratch); ``fetch()`` / ``alt_info_strings()`` wait for it."""
 
+    _API = "c3b_fa"
+
     def __init__(self, device=0):
-        dev = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
-        if dev.type != "cuda":
-            raise C3BError("FullAlignmentBuilder needs a CUDA device (no CPU fallback)")
-        if dev.index is None:
-            dev = torch.device("cuda", torch.cuda.current_device())
-        self._device = dev
-        out = ffi.new("c3b_fa **")
-        check(lib().c3b_fa_create(out, dev.index or 0))
-        self._h = out[0]
+        super().__init__(device)
         self._keep = None
         self._shape = None
 
@@ -87,26 +64,13 @@ class FullAlignmentBuilder:
         prm = ffi.new("c3b_fa_params *")
         prm.matrix_depth, prm.need_haplotagging, prm.min_mq = int(matrix_depth), int(bool(need_haplotagging)), int(min_mq)
         prm.dwell, prm.rand_seed, prm.rand_skip = int(bool(dwell)), int(rand_seed) & 0xFFFFFFFF, int(rand_skip)
-        st = _fa_struct(rec, on_dev)
-        stream = torch.cuda.current_stream(self._device).cuda_stream
-        if on_dev:
-            if ref_seq is None:
-                ref_seq = rec.ref
-            if not (isinstance(ref_seq, torch.Tensor) and ref_seq.dtype == torch.uint8 and ref_seq.device == rec.device):
-                raise C3BError("build: device records need the reference bases as a uint8 tensor on the same device")
-            ref, refbuf = ref_seq.contiguous(), None
-            refptr, reflen = ffi.cast("const char *", ref.data_ptr()), ref.numel()
-            host_ref = None
-        else:
-            ref = ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq)
-            refbuf = ffi.from_buffer(ref)
-            refptr, reflen = ffi.cast("const char *", refbuf), len(ref)
-            host_ref = ref
+        st = _records_struct(rec, optional=True)
+        refptr, reflen, ref = self._reference(ref_seq, rec, "build")
         check(lib().c3b_fa_build(self._h, st, int(on_dev), ffi.cast("const int64_t *", cand.ctypes.data), len(cand), var, nv, refptr,
-                                 int(ref_start), reflen, prm, ffi.cast("void *", stream)))
-        self._keep = (rec, ref, refbuf, st, cand, var)      # buffers stay alive while the copies / kernels are in flight
+                                 int(ref_start), reflen, prm, self._stream()))
+        self._keep = (rec, ref, st, cand, var)      # buffers stay alive while the copies / kernels are in flight
         self._shape = (len(cand), int(matrix_depth), 9 if dwell else 8)
-        self._alt = (host_ref, int(ref_start), int(max_indel_length))
+        self._alt = (None if on_dev else ref, int(ref_start), int(max_indel_length))
         return self
 
     def sizes(self):
@@ -149,7 +113,7 @@ class FullAlignmentBuilder:
                                          c("int32_t *", al_off.ctypes.data), c("int32_t *", al_n.ctypes.data),
                                          c("uint32_t *", meta.ctypes.data), c("uint32_t *", rd.ctypes.data),
                                          c("uint32_t *", qp.ctypes.data), c("uint32_t *", cn.ctypes.data), len(meta), na))
-        cand = self._keep[4]
+        cand = self._keep[3]
         out = []
         for i in range(n):
             sl = slice(int(al_off[i]), int(al_off[i]) + int(al_n[i]))
@@ -163,7 +127,7 @@ class FullAlignmentBuilder:
         if getattr(model, "_handle", None) is None:
             raise C3BError("forward: the model has no device / weights yet (.to(device), .load_state_dict())")
         n, depth, C = self._shape
-        if model._kind != _const("C3B_FULL_ALIGNMENT") or model.input_channels != C:
+        if model._kind != CONSTANTS["C3B_FULL_ALIGNMENT"] or model.input_channels != C:
             raise C3BError("forward: needs the full-alignment network (Clair3_F) with %d input channels" % C)
         if torch.device(model._device) != self._device:
             raise C3BError("forward: the model lives on %s, the builder on %s" % (model._device, self._device))
@@ -172,31 +136,9 @@ class FullAlignmentBuilder:
         if n:
             pm = ffi.new("const int8_t **")
             check(lib().c3b_fa_device(self._h, pm))
-            stream = torch.cuda.current_stream(self._device).cuda_stream
-            check(lib().c3b_forward(model._handle, ffi.cast("void *", pm[0]), _const("C3B_DT_I8"), 1, n, depth,
-                                    ffi.cast("float *", y.data_ptr()), 1, ffi.cast("void *", stream)))
+            check(lib().c3b_forward(model._handle, ffi.cast("void *", pm[0]), CONSTANTS["C3B_DT_I8"], 1, n, depth,
+                                    ffi.cast("float *", y.data_ptr()), 1, self._stream()))
         return model._split(y)
-
-    def last_ms(self):
-        ms, k = ffi.new("float *"), ffi.new("int *")
-        check(lib().c3b_fa_last_ms(self._h, ms, k))
-        return float(ms[0]), int(k[0])
-
-    def close(self):
-        if getattr(self, "_h", None) is not None:
-            lib().c3b_fa_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-def _const(name):
-    from ._ffi import CONSTANTS
-    return CONSTANTS[name]
 
 
 def format_alt_info(candidate, depth, acgt, ref, ref_start, max_indel_length, meta, read, qpos, cnt, rec):

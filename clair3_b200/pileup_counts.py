@@ -11,7 +11,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from ._ffi import C3BError, check, ffi, lib
+from ._ffi import CONSTANTS, C3BError, check, ffi, lib
 
 FLANKING = 16                 # shared/param_p.py flankingBaseNum; pileup_flanking_base_num src/clair3_pileup.h:93
 CHANNELS = 18
@@ -69,13 +69,6 @@ class BamRecords:
         extra = {k: d[k] for k in names if d.get(k) is not None}
         return cls(**{k: d[k] for k, _ in _FIELDS}, **extra)
 
-    def _struct(self):
-        s = ffi.new("c3b_bam_records *")
-        s.n_reads = self.n_reads
-        for k, dt in _FIELDS:
-            setattr(s, k, ffi.cast("const %s *" % _CTYPE[np.dtype(dt).name], getattr(self, k).ctypes.data))
-        return s
-
     def nbytes(self):
         return int(sum(getattr(self, k).nbytes for k, _ in _FIELDS))
 
@@ -108,28 +101,91 @@ class DeviceBamRecords:
             b = ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq)
             self.ref = torch.from_numpy(np.frombuffer(b, dtype=np.uint8).copy()).to(self.device)
 
-    def _struct(self):
-        s = ffi.new("c3b_bam_records *")
-        s.n_reads = self.n_reads
-        for k, dt in _FIELDS:
-            setattr(s, k, ffi.cast("const %s *" % _CTYPE[np.dtype(dt).name], self.t[k].data_ptr()))
-        return s
+
+def _records_struct(rec, optional=False):
+    """The ``c3b_bam_records`` of a ``BamRecords`` or a ``DeviceBamRecords`` (``optional=True``: the ``c3b_fa_records`` around it,
+    with qual / qname / mv where the records carry them, null where they do not).  The struct holds raw addresses: the records
+    must outlive the call that reads it."""
+    on_dev = isinstance(rec, DeviceBamRecords)
+    arrays = rec.t if on_dev else vars(rec)
+    addr = (lambda a: a.data_ptr()) if on_dev else (lambda a: a.ctypes.data)
+    s = ffi.new("c3b_fa_records *" if optional else "c3b_bam_records *")
+    core = s.core if optional else s
+    core.n_reads = rec.n_reads
+    for k, dt in _FIELDS:
+        setattr(core, k, ffi.cast("const %s *" % _CTYPE[np.dtype(dt).name], addr(arrays[k])))
+    for k, dt in _OPTIONAL if optional else ():
+        v, o = arrays.get(k), arrays.get(k + "_off")
+        if o is not None:
+            setattr(s, k + "_off", ffi.cast("const int64_t *", addr(o)))
+            vp = addr(v) if len(v) else 8      # an empty value array with valid offsets: non-null, never dereferenced
+            setattr(s, k, ffi.cast("const %s *" % _CTYPE[np.dtype(dt).name], vp))
+    return s
 
 
-class PileupCounter:
-    """One counting workspace on one H100 (``c3b_plp``).  ``count()`` is asynchronous on the current torch stream of the device;
-    ``sizes()`` / ``fetch()`` wait for it."""
+class _Workspace:
+    """What ``PileupCounter`` and ``FullAlignmentBuilder`` share: a library workspace on one CUDA device, created by
+    ``<_API>_create`` and released by ``<_API>_destroy``, whose calls run on the device's current torch stream."""
 
-    def __init__(self, device=0):
+    _API = None                      # "c3b_plp" / "c3b_fa"
+
+    def __init__(self, device):
         dev = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
         if dev.type != "cuda":
-            raise C3BError("PileupCounter needs a CUDA device (no CPU fallback)")
+            raise C3BError("%s needs a CUDA device (no CPU fallback)" % type(self).__name__)
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
         self._device = dev
-        out = ffi.new("c3b_plp **")
-        check(lib().c3b_plp_create(out, dev.index or 0))
+        out = ffi.new(self._API + " **")
+        check(getattr(lib(), self._API + "_create")(out, dev.index or 0))
         self._h = out[0]
+
+    def _stream(self):
+        return ffi.cast("void *", torch.cuda.current_stream(self._device).cuda_stream)
+
+    @staticmethod
+    def _reference(ref_seq, rec, who):
+        """(pointer, length, object that owns the bytes) of a call's reference bases: str / bytes on the host, or with device
+        records a uint8 tensor on their device (default: the one ``to_device`` was given)."""
+        if isinstance(rec, DeviceBamRecords):
+            if ref_seq is None:
+                ref_seq = rec.ref
+            if not (isinstance(ref_seq, torch.Tensor) and ref_seq.dtype == torch.uint8 and ref_seq.device == rec.device):
+                raise C3BError("%s: device records need the reference bases as a uint8 tensor on the same device" % who)
+            ref = ref_seq.contiguous()
+            return ffi.cast("const char *", ref.data_ptr()), ref.numel(), ref
+        ref = ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq)
+        return ffi.cast("const char *", ffi.from_buffer(ref)), len(ref), ref
+
+    def _timing(self, fn):
+        ms, n = ffi.new("float *"), ffi.new("int *")
+        check(fn(self._h, ms, n))
+        return float(ms[0]), int(n[0])
+
+    def last_ms(self):
+        """(device milliseconds, kernel launches) of the last call, between CUDA events on its stream."""
+        return self._timing(getattr(lib(), self._API + "_last_ms"))
+
+    def close(self):
+        if getattr(self, "_h", None) is not None:
+            getattr(lib(), self._API + "_destroy")(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class PileupCounter(_Workspace):
+    """One counting workspace on one H100 (``c3b_plp``).  ``count()`` is asynchronous on the current torch stream of the device;
+    ``sizes()`` / ``fetch()`` wait for it."""
+
+    _API = "c3b_plp"
+
+    def __init__(self, device=0):
+        super().__init__(device)
         self._keep = None
         self._shape = None
         self._alt = None
@@ -148,22 +204,10 @@ class PileupCounter:
         prm.min_depth, prm.min_snp_af, prm.min_indel_af, prm.min_mq = int(min_depth), float(min_snp_af), float(min_indel_af), int(min_mq)
         prm.call_snp_only, prm.call_ht, prm.gvcf = int(bool(call_snp_only)), int(bool(call_ht)), int(bool(gvcf))
         prm.alt_info = int(bool(alt_info))
-        st = rec._struct()
-        stream = torch.cuda.current_stream(self._device).cuda_stream
-        if on_dev:
-            if ref_seq is None:
-                ref_seq = rec.ref
-            if not (isinstance(ref_seq, torch.Tensor) and ref_seq.dtype == torch.uint8 and ref_seq.device == rec.device):
-                raise C3BError("count: device records need the reference bases as a uint8 tensor on the same device")
-            ref, refbuf = ref_seq.contiguous(), None
-            refptr, reflen = ffi.cast("const char *", ref.data_ptr()), ref.numel()
-        else:
-            ref = ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq)
-            refbuf = ffi.from_buffer(ref)
-            refptr, reflen = ffi.cast("const char *", refbuf), len(ref)
-        check(lib().c3b_plp_count(self._h, st, int(on_dev), int(start), int(end), refptr, int(ref_start), reflen, prm,
-                                  ffi.cast("void *", stream)))
-        self._keep = (rec, ref, refbuf, st)          # buffers stay alive while the copies / kernels are in flight
+        st = _records_struct(rec)
+        refptr, reflen, ref = self._reference(ref_seq, rec, "count")
+        check(lib().c3b_plp_count(self._h, st, int(on_dev), int(start), int(end), refptr, int(ref_start), reflen, prm, self._stream()))
+        self._keep = (rec, ref, st)                  # buffers stay alive while the copies / kernels are in flight
         self._shape = (int(end) - int(start), bool(gvcf))
         self._alt = (bool(alt_info), int(start), int(end), int(ref_start), int(max_indel_length))
         self._sizes = None
@@ -350,7 +394,7 @@ class PileupCounter:
     def _check_model(self, model, who):
         if getattr(model, "_handle", None) is None:
             raise C3BError("%s: the model has no device / weights yet (.to(device), .load_state_dict())" % who)
-        if getattr(model, "input_channels", CHANNELS) != CHANNELS or model._kind != lib_const("C3B_PILEUP"):
+        if getattr(model, "input_channels", CHANNELS) != CHANNELS or model._kind != CONSTANTS["C3B_PILEUP"]:
             raise C3BError("%s: needs the pileup network (Clair3_P, 18 channels)" % who)
         if torch.device(model._device) != self._device:
             raise C3BError("%s: the model lives on %s, the counter on %s" % (who, model._device, self._device))
@@ -363,31 +407,12 @@ class PileupCounter:
                           ffi.new("const int64_t **"))
         check(lib().c3b_plp_device(self._h, pm, ffi.NULL, ffi.NULL, ps, pk))
         check(lib().c3b_plp_window_bounds(self._h, ffi.NULL, pb))
-        stream = torch.cuda.current_stream(self._device).cuda_stream
-        check(lib().c3b_forward_windows_bounded(model._handle, ffi.cast("void *", pm[0]), lib_const("C3B_DT_I64"), nc, ps[0], pb[0],
-                                                1, nk, ffi.cast("float *", y.data_ptr()), 1, 0, ffi.cast("void *", stream)))
-
-    def last_ms(self):
-        ms, n = ffi.new("float *"), ffi.new("int *")
-        check(lib().c3b_plp_last_ms(self._h, ms, n))
-        return float(ms[0]), int(n[0])
+        check(lib().c3b_forward_windows_bounded(model._handle, ffi.cast("void *", pm[0]), CONSTANTS["C3B_DT_I64"], nc, ps[0], pb[0],
+                                                1, nk, ffi.cast("float *", y.data_ptr()), 1, 0, self._stream()))
 
     def alt_text_last_ms(self):
         """Device time and kernel launches of the last ``alt_text`` (``last_ms`` reports the count alone)."""
-        ms, n = ffi.new("float *"), ffi.new("int *")
-        check(lib().c3b_plp_alt_text_last_ms(self._h, ms, n))
-        return float(ms[0]), int(n[0])
-
-    def close(self):
-        if getattr(self, "_h", None) is not None:
-            lib().c3b_plp_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        return self._timing(lib().c3b_plp_alt_text_last_ms)
 
 
 class _DeviceArray:
@@ -562,11 +587,6 @@ def chunks_for_rank(chunk_num, rank, world):
     from .sharding import site_range
     lo, hi = site_range(chunk_num, rank, world)
     return list(range(lo + 1, hi + 1))
-
-
-def lib_const(name):
-    from ._ffi import CONSTANTS
-    return CONSTANTS[name]
 
 
 def enforce_chunk_contiguity(counts, positions):
