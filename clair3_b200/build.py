@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libclair3b200.so")
 OBJ_DIR = os.path.join(HERE, "csrc", "_obj")
-SOURCES = ["c3b_api.cu", "kernels_common.cu", "kernels_fp32.cu", "lstm_tc.cu", "fa_tc.cu", "pconv_tc.cu", "decode.cu", "proj_tc.cu", "tail_tc.cu", "plp_counts.cu", "plp_alt_text.cu", "fa_tensor.cu"]
+SOURCES = ["c3b_api.cu", "kernels_common.cu", "kernels_fp32.cu", "lstm_tc.cu", "fa_tc.cu", "pconv_tc.cu", "decode.cu", "proj_tc.cu", "tail_tc.cu", "plp_counts.cu", "plp_alt_text.cu", "fa_tensor.cu", "fa_alt_text.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 

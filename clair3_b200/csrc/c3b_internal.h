@@ -496,3 +496,30 @@ struct PlpAltTextArgs {
     int64_t *position;                  // [W]
 };
 int c3b_launch_plp_alt_text(const PlpAltTextArgs &a, cudaStream_t s, int *launches);
+
+// ---- full-alignment builder: the all_alt_info text stage (fa_alt_text.cu), enqueued by c3b_fa_alt_text in fa_tensor.cu ----
+struct FaAltTextArgs {
+    // the build's results (device)
+    int64_t n_cand, ref_start, ref_len, max_indel_length;
+    const int64_t *cand;                // [n_cand] 0-based positions
+    const char *ref;
+    C3bReads R;                         // the records where the build left them
+    const int32_t *c_depth, *c_acgt, *al_off, *al_n;
+    const uint32_t *al_meta, *al_read, *al_qpos, *al_cnt;
+    int64_t al_cap;                     // records the al_* arrays and hash / order hold
+    // scratch
+    uint32_t *hash;                     // [al_cap]
+    int32_t *order;                     // [al_cap]
+    uint32_t *table;                    // [8 * n_cand + 3 * al_cap] khash buckets
+    int32_t *n_ins, *n_del;             // [n_cand]
+    int32_t *len_text, *len_dec;        // [n_cand + 1]
+    int *status;                        // the stage's status word: non-zero = a candidate's text did not fit the stage's buffers
+    // outputs
+    char *text, *dec;
+    int64_t text_cap, dec_cap;
+    int64_t *text_off, *dec_off;        // [n_cand + 1]
+    int64_t *totals;                    // device: n_text_bytes, n_decoder_bytes
+    uint8_t *ref_base;                  // [n_cand]
+    int64_t *position;                  // [n_cand]
+};
+int c3b_launch_fa_alt_text(const FaAltTextArgs &a, cudaStream_t s, int *launches);

@@ -23,7 +23,7 @@
 //                        one-CTA scan (block_scan.cuh) sizes F, numbers the kept reads and lays out their pools, and takes the
 //                        running maximum of the kept reads' ends.
 //   K11 fa_candidate     one CTA per candidate: counters over ALL kept reads on the candidate (depth, A/C/G/T, distinct
-//                        deletion lengths and insertion strings in first-occurrence order, exported for the host's text),
+//                        deletion lengths and insertion strings in first-occurrence order, exported for the text stage),
 //                        Fisher-Yates with the glibc TYPE_3 stream generated at the candidate's offset (jump-ahead by
 //                        precomputed matrix powers: the stream is linear mod 2^32), rank sort by (haplotype, index), padding,
 //                        and the int8 [depth][33][C] block in Clair3_F's wire layout.
@@ -31,6 +31,8 @@
 // Bound: latency of dependent global loads (integer work, no tensor cores).  Bytes per call: the records once per pass (K3, K7,
 // K8), 20 B of Pos_info per (kept read, flanking position) written once and read by K11, and the matrix (depth x 33 x C B per
 // candidate) written once.  DESIGN.md 5b.
+//
+// The all_alt_info text is a second stage (fa_alt_text.cu, c3b_fa_alt_text) that reads K11's export where the build left it.
 #include <limits.h>
 #include <stdlib.h>
 
@@ -913,8 +915,10 @@ void glibc_jump_matrices(std::vector<uint32_t> &out) {
 
 }  // namespace
 
-// One timed stage, the build.  counters: int64 0 nF, 1 n_kept, 2 pool entries, 3 signal entries, 4 draws, 5 status, 6 al_used,
-// 7 spare.
+// Timed stages: 0 the build (c3b_fa_build), 1 the text (c3b_fa_alt_text).  counters: int64 0 nF, 1 n_kept, 2 pool entries,
+// 3 signal entries, 4 draws, 5 status, 6 al_used, 7 the text stage's status, 8 n_text_bytes, 9 n_decoder_bytes.
+constexpr int N_COUNTERS = 10;
+
 struct c3b_fa : C3bRegionWorkspace {
     C3bBuf in_core[8], in_qoff, in_qual, in_noff, in_name, in_moff, in_mv;
     C3bBuf in_ref, in_cand, in_var, jump, state0;
@@ -926,12 +930,20 @@ struct c3b_fa : C3bRegionWorkspace {
     C3bBuf matrix, c_depth, c_acgt, al_off, al_n;
     int64_t n_cand = 0, depth = 0, C = 8, n_kept = 0;
     bool built = false;
+    bool synced = false;                 // c3b_fa_sizes has waited for everything queued since the last build or text stage
+    // the text stage (c3b_fa_alt_text): where the build left its inputs, scratch, outputs
+    C3bReads R{};
+    const char *dref = nullptr;
+    int64_t ref_start = 0, ref_len = 0, n_cigar = 0, n_seq = 0;
+    C3bBuf tx_hash, tx_order, tx_table, tx_nins, tx_ndel, tx_len_text, tx_len_dec;
+    C3bBuf text, dec, text_off, dec_off, ref_base, position;
+    bool texted = false;
 };
 
 extern "C" {
 
 int c3b_fa_create(c3b_fa **out, int device_ordinal) {
-    if (c3b_region_create(out, device_ordinal, 1, 8, "c3b_fa_create")) return 1;
+    if (c3b_region_create(out, device_ordinal, 2, N_COUNTERS, "c3b_fa_create")) return 1;
     c3b_fa *w = *out;
     std::vector<uint32_t> J;
     glibc_jump_matrices(J);
@@ -984,7 +996,7 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     C3B_CUDA(cudaSetDevice(w->device));
     cudaStream_t s = (cudaStream_t)cuda_stream;
     w->stream = s;
-    w->built = false;
+    w->built = w->synced = w->texted = false;
     w->n_cand = n_cand;
     w->depth = params->matrix_depth;
     w->C = params->dwell ? 9 : 8;
@@ -994,8 +1006,9 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     // inputs
     C3bReads R{};
     R.n = n;
+    int64_t n_cigar = 0, n_seq = 0;
     if (n > 0) {
-        int64_t n_cigar, n_seq, n_qual, n_name, n_mv;
+        int64_t n_qual, n_name, n_mv;
         if (c3b_last_offset(core->cigar_off, n, on_device, s, &n_cigar) || c3b_last_offset(core->seq_off, n, on_device, s, &n_seq) ||
             c3b_last_offset(records->qual_off, n, on_device, s, &n_qual) || c3b_last_offset(records->qname_off, n, on_device, s, &n_name) ||
             c3b_last_offset(records->mv_off, n, on_device, s, &n_mv))
@@ -1015,6 +1028,10 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     }
     const char *dref = nullptr;
     if (c3b_upload(w->in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, dref, s, "c3b_fa")) return 1;
+    w->R = R;
+    w->dref = dref;
+    w->ref_start = ref_start; w->ref_len = ref_len > 0 ? ref_len : 0;
+    w->n_cigar = n_cigar; w->n_seq = n_seq;
     const size_t Kz = (size_t)(n_cand > 0 ? n_cand : 1), Nz = (size_t)(n > 0 ? n : 1);
     auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_fa"); };
     if (grow(w->in_cand, Kz * 8) || grow(w->in_var, (size_t)(n_var > 0 ? n_var : 1) * sizeof(c3b_fa_variant))) return 1;
@@ -1125,7 +1142,7 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     }
     C3B_CUDA(cudaEventRecord(w->ev[0][1], s));
     C3B_CUDA(cudaGetLastError());
-    C3B_CUDA(cudaMemcpyAsync(w->host_counters, cnt, 64, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaMemcpyAsync(w->host_counters, cnt, N_COUNTERS * 8, cudaMemcpyDeviceToHost, s));
     w->built = true;
     return 0;
 }
@@ -1143,6 +1160,7 @@ int c3b_fa_sizes(c3b_fa *w, int64_t *n_cand, int64_t *n_kept, int64_t *rand_draw
                       MAX_OVERWRITTEN);
         return 1;
     }
+    w->synced = true;
     if (n_cand) *n_cand = w->n_cand;
     if (n_kept) *n_kept = w->n_kept;
     if (rand_draws) *rand_draws = w->host_counters[4];
@@ -1170,6 +1188,97 @@ int c3b_fa_device(c3b_fa *w, const int8_t **matrix) {
     if (!w || !w->built) { c3b_set_error("c3b_fa_device: no c3b_fa_build has been issued"); return 1; }
     if (matrix) *matrix = w->matrix.as<int8_t>();
     return 0;
+}
+
+int c3b_fa_alt_text(c3b_fa *w, int64_t max_indel_length) {
+    if (!w || !w->built) { c3b_set_error("c3b_fa_alt_text: no c3b_fa_build has been issued"); return 1; }
+    C3B_CUDA(cudaSetDevice(w->device));
+    cudaStream_t s = w->stream;
+    const int64_t K = w->n_cand;
+    // every allele record comes from one insertion / deletion operation of one read
+    const int64_t cap = w->n_cigar < AL_CAP ? (w->n_cigar > 0 ? w->n_cigar : 1) : AL_CAP;
+    // bytes: head, SNP and R fields per candidate; key, count and separators per record; the inserted bases are query bases; a
+    // printed deletion shows at most max_indel_length reference bases
+    const int64_t del_len = max_indel_length < 0 ? 0 : (max_indel_length < w->ref_len ? max_indel_length : w->ref_len);
+    const int64_t del_bytes = cap * del_len < (1ll << 28) ? cap * del_len : (1ll << 28);
+    const int64_t text_cap = 160 * (K + 1) + 48 * cap + 2 * w->n_seq + del_bytes;
+    const size_t Kz = (size_t)K + 1;
+    w->texted = w->synced = false;        // the status word and the totals travel with the next c3b_fa_sizes
+    auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_fa"); };
+    if (grow(w->tx_hash, (size_t)cap * 4) || grow(w->tx_order, (size_t)cap * 4) || grow(w->tx_table, (8 * Kz + 3 * (size_t)cap) * 4) ||
+        grow(w->tx_nins, Kz * 4) || grow(w->tx_ndel, Kz * 4) || grow(w->tx_len_text, Kz * 4) || grow(w->tx_len_dec, Kz * 4) ||
+        grow(w->text, (size_t)text_cap) || grow(w->dec, (size_t)text_cap) || grow(w->text_off, Kz * 8) || grow(w->dec_off, Kz * 8) ||
+        grow(w->ref_base, Kz) || grow(w->position, Kz * 8))
+        return 1;
+    w->launches[1] = 0;
+    int64_t *cnt = w->counters.as<int64_t>();
+    // the stage's own status word and totals: an earlier stage's overflow is not this one's
+    C3B_CUDA(cudaMemsetAsync(cnt + 7, 0, 3 * 8, s));
+    C3B_CUDA(cudaEventRecord(w->ev[1][0], s));
+    if (K > 0) {
+        FaAltTextArgs A;
+        A.n_cand = K; A.ref_start = w->ref_start; A.ref_len = w->ref_len; A.max_indel_length = max_indel_length;
+        A.cand = w->in_cand.as<int64_t>(); A.ref = w->dref; A.R = w->R;
+        A.c_depth = w->c_depth.as<int32_t>(); A.c_acgt = w->c_acgt.as<int32_t>();
+        A.al_off = w->al_off.as<int32_t>(); A.al_n = w->al_n.as<int32_t>();
+        A.al_meta = w->al_meta.as<uint32_t>(); A.al_read = w->al_read.as<uint32_t>(); A.al_qpos = w->al_qpos.as<uint32_t>();
+        A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_cap = cap;
+        A.hash = w->tx_hash.as<uint32_t>(); A.order = w->tx_order.as<int32_t>(); A.table = w->tx_table.as<uint32_t>();
+        A.n_ins = w->tx_nins.as<int32_t>(); A.n_del = w->tx_ndel.as<int32_t>();
+        A.len_text = w->tx_len_text.as<int32_t>(); A.len_dec = w->tx_len_dec.as<int32_t>();
+        A.status = reinterpret_cast<int *>(cnt + 7);
+        A.text = w->text.as<char>(); A.dec = w->dec.as<char>(); A.text_cap = A.dec_cap = text_cap;
+        A.text_off = w->text_off.as<int64_t>(); A.dec_off = w->dec_off.as<int64_t>(); A.totals = cnt + 8;
+        A.ref_base = w->ref_base.as<uint8_t>(); A.position = w->position.as<int64_t>();
+        if (c3b_launch_fa_alt_text(A, s, &w->launches[1])) return 1;
+    } else {
+        C3B_CUDA(cudaMemsetAsync(w->text_off.p, 0, 8, s));
+        C3B_CUDA(cudaMemsetAsync(w->dec_off.p, 0, 8, s));
+    }
+    C3B_CUDA(cudaEventRecord(w->ev[1][1], s));
+    C3B_CUDA(cudaMemcpyAsync(w->host_counters, w->counters.p, N_COUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    w->texted = true;
+    return 0;
+}
+
+int c3b_fa_alt_text_sizes(c3b_fa *w, int64_t *n_text_bytes, int64_t *n_decoder_bytes) {
+    if (!w || !w->texted) { c3b_set_error("c3b_fa_alt_text_sizes: no c3b_fa_alt_text has been issued"); return 1; }
+    if (!w->synced && c3b_fa_sizes(w, nullptr, nullptr, nullptr)) return 1;
+    if ((int)w->host_counters[7] != 0) {
+        c3b_set_error("c3b_fa_alt_text: the all_alt_info text outgrew its buffers; build fewer candidates or lower max_indel_length");
+        return 1;
+    }
+    if (n_text_bytes) *n_text_bytes = w->host_counters[8];
+    if (n_decoder_bytes) *n_decoder_bytes = w->host_counters[9];
+    return 0;
+}
+
+int c3b_fa_fetch_alt_text(c3b_fa *w, char *text, int64_t *text_off, char *decoder, int64_t *decoder_off, uint8_t *ref_base,
+                          int64_t *position) {
+    int64_t nt = 0, nd = 0;
+    if (!w || !w->texted) { c3b_set_error("c3b_fa_fetch_alt_text: no c3b_fa_alt_text has been issued"); return 1; }
+    if (c3b_fa_alt_text_sizes(w, &nt, &nd)) return 1;
+    const size_t nk = (size_t)w->n_cand;
+    return w->get(text, w->text, (size_t)nt) || w->get(text_off, w->text_off, (nk + 1) * 8) || w->get(decoder, w->dec, (size_t)nd) ||
+           w->get(decoder_off, w->dec_off, (nk + 1) * 8) || w->get(ref_base, w->ref_base, nk) ||
+           w->get(position, w->position, nk * 8) || w->wait();
+}
+
+int c3b_fa_alt_text_device(c3b_fa *w, const char **text, const int64_t **text_off, const char **decoder,
+                           const int64_t **decoder_off, const uint8_t **ref_base, const int64_t **position) {
+    if (!w || !w->texted) { c3b_set_error("c3b_fa_alt_text_device: no c3b_fa_alt_text has been issued"); return 1; }
+    if (text) *text = w->text.as<char>();
+    if (text_off) *text_off = w->text_off.as<int64_t>();
+    if (decoder) *decoder = w->dec.as<char>();
+    if (decoder_off) *decoder_off = w->dec_off.as<int64_t>();
+    if (ref_base) *ref_base = w->ref_base.as<uint8_t>();
+    if (position) *position = w->position.as<int64_t>();
+    return 0;
+}
+
+int c3b_fa_alt_text_last_ms(c3b_fa *w, float *ms, int *launches) {
+    if (!w || !w->texted) { c3b_set_error("c3b_fa_alt_text_last_ms: no c3b_fa_alt_text has been issued"); return 1; }
+    return w->elapsed(1, ms, launches);
 }
 
 int c3b_fa_last_ms(c3b_fa *w, float *ms, int *launches) {

@@ -23,50 +23,14 @@
 // the status word.
 #include <limits.h>
 
+#include "alt_text.cuh"
 #include "block_scan.cuh"
 #include "c3b_internal.h"
 
 namespace {
 
-__constant__ char NT16[17] = "=ACMGRSVTWYHKDBN";          // htslib seq_nt16_str
 constexpr int FETCH_EXPAND = 1000;                        // mpileup_expand_reference_region, src/clair3_pileup.h:63
 constexpr int32_t NOT_FIRST = -2;                         // mate[]: the record's twin comes earlier in the list
-constexpr uint32_t T_VAL = 0xffffffu, T_OCC = 1u << 24, T_TAKEN = 1u << 25;   // khash bucket: record + 1 | old flag | new flag
-
-struct CountSink {
-    long long n = 0;
-    __device__ __forceinline__ void put(char) { ++n; }
-};
-struct WriteSink {              // writes inside [p, p + lim) only: lim is the length the measure pass found
-    char *p;
-    long long lim, n = 0;
-    __device__ __forceinline__ void put(char c) { if (n < lim) p[n] = c; ++n; }
-};
-
-template <class S> struct TextOut {
-    S full, dec;                // the reference's string, and "<depth>-<alt>" as the decoder takes it
-    bool cut = false;           // the alt field of rstrip().split("-") ends at the first '-' of the alt text
-    long long n_alt = 0;
-    __device__ __forceinline__ void head(char c, bool both) {
-        full.put(c);
-        if (both) dec.put(c);
-    }
-    __device__ __forceinline__ void alt(char c) {
-        full.put(c);
-        ++n_alt;
-        if (c == '-') cut = true;
-        if (!cut) dec.put(c);
-    }
-    enum Where { HEAD_FULL, HEAD_BOTH, ALT };
-    __device__ void num(long long v, Where w) {             // %d of a non-negative count, without a digit buffer
-        unsigned long long u = (unsigned long long)v, p = 1;
-        while (u / p >= 10) p *= 10;
-        for (; p; p /= 10) {
-            const char c = (char)('0' + (u / p) % 10);
-            if (w == ALT) alt(c); else head(c, w == HEAD_BOTH);
-        }
-    }
-};
 
 // upper_base of the reference base under a column, 'N' outside the supplied reference
 __device__ __forceinline__ int ref_base_at(const PlpAltTextArgs &A, int64_t pos) {
@@ -139,32 +103,6 @@ template <class S> __device__ void plp_text_emit(const PlpAltTextArgs &A, const 
     if (ref_depth > 0) {
         o.alt('R'); o.alt((char)rb); o.alt(' '); o.num(ref_depth, O::ALT); o.alt(' ');
     }
-}
-
-// kh_resize (src/khash.h:246-306) for an insert-only table of n buckets holding `size` strings; returns the new bucket count, 0
-// when the candidate's scratch cannot hold it.
-__device__ int khash_grow(const PlpAltTextArgs &A, uint32_t *slot, const int n, const int avail) {
-    const int nn = n < 4 ? 4 : 2 * n;
-    if (nn > avail) return 0;
-    for (int b = 0; b < nn; ++b) {
-        const uint32_t v = b < n ? (slot[b] & T_VAL) : 0u;
-        slot[b] = v | (v ? T_OCC : 0u);
-    }
-    const uint32_t mask = (uint32_t)nn - 1u;
-    for (int b = 0; b < n; ++b) {
-        if (!(slot[b] & T_OCC)) continue;
-        uint32_t cur = slot[b] & T_VAL;
-        slot[b] &= T_TAKEN;                                   // the bucket is free in the old table; its new flag stays
-        for (;;) {                                            // kick-out: the evicted string is placed next
-            uint32_t i = A.hash[cur - 1] & mask, step = 0;
-            while (slot[i] & T_TAKEN) i = (i + (++step)) & mask;
-            const uint32_t e = slot[i];
-            slot[i] = cur | T_TAKEN;
-            if (!(e & T_OCC)) break;
-            cur = e & T_VAL;
-        }
-    }
-    return nn;
 }
 
 // ---------------------------------------------------------------------------------------------------------------- T1
@@ -244,34 +182,13 @@ __global__ void __launch_bounds__(256) plp_text_measure_kernel(PlpAltTextArgs A)
         }
         __syncwarp();
         if (lane == 0) {
-            if (ni > 0) {                                     // the khash replay: a short serial walk
+            if (ni > 0 && fits) {                             // the khash replay: a short serial walk
                 uint32_t *slot = A.table + 8 * j;
                 int avail = 8;
                 if (ni > 3) { slot = A.table + 8 * A.W + 3 * (int64_t)a0; avail = 3 * n; }
-                int nb = 0, size = 0, upper = 0;
-                for (int k = 0; k < ni && fits; ++k) {
-                    if (size >= upper) {                      // kh_put grows a full table before it looks the key up
-                        nb = khash_grow(A, slot, nb, avail);
-                        if (!nb) { fits = false; break; }
-                        upper = (int)(nb * 0.77 + 0.5);
-                    }
-                    const int rec = A.order[a0 + k];
-                    const uint32_t mask = (uint32_t)nb - 1u;
-                    uint32_t i = A.hash[rec] & mask, step = 0;
-                    while (slot[i] & T_VAL) i = (i + (++step)) & mask;
-                    slot[i] = (uint32_t)rec + 1u;
-                    ++size;
-                }
                 // a read after the last new string put a present one again: that put still grows a full table first
-                if (fits && size >= upper && (int64_t)A.ins_last[pos - A.start] > first_read(A, A.order[a0 + ni - 1])) {
-                    nb = khash_grow(A, slot, nb, avail);
-                    if (!nb) fits = false;
-                }
-                if (fits) {
-                    int k = 0;
-                    for (int b = 0; b < nb; ++b)
-                        if (slot[b] & T_VAL) A.order[a0 + k++] = (int)(slot[b] & T_VAL) - 1;
-                }
+                const bool again = (int64_t)A.ins_last[pos - A.start] > first_read(A, A.order[a0 + ni - 1]);
+                fits = khash_replay(A.hash, A.order + a0, ni, again, slot, avail);
             }
             if (!fits) { atomicOr(A.status, 1); ni = nd = 0; }
             A.n_ins[j] = ni;
@@ -306,7 +223,7 @@ __global__ void __launch_bounds__(128) plp_text_write_kernel(PlpAltTextArgs A) {
 }  // namespace
 
 int c3b_launch_plp_alt_text(const PlpAltTextArgs &a, cudaStream_t s, int *launches) {
-    if (a.al_cap >= (int64_t)T_VAL) { c3b_set_error("c3b_plp_alt_text: %lld allele records exceed the khash replay's 24-bit record index", (long long)a.al_cap); return 1; }
+    if (a.al_cap >= (int64_t)KH_VAL) { c3b_set_error("c3b_plp_alt_text: %lld allele records exceed the khash replay's 24-bit record index", (long long)a.al_cap); return 1; }
     int64_t blocks = ((a.W + 1) * 32 + 255) / 256;
     if (blocks > 132 * 8) blocks = 132 * 8;
     plp_text_measure_kernel<<<(unsigned)blocks, 256, 0, s>>>(a);

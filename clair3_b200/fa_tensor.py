@@ -3,8 +3,9 @@
 Mirrors the reference's ``CreateTensorFullAlignment`` (HKU-BAL/Clair3 ``preprocess/CreateTensorFullAlignmentFromCffi.py:19-170``:
 ``lib.calculate_clair3_full_alignment`` -> int8 ``[candidates, depth, 33, 8|9]`` + ``all_alt_info`` strings) from the point where
 htslib has decoded the alignment records: the caller hands over the ``bam1_t`` fields as ``BamRecords`` (with ``qual``, ``qname``
-and, for dwell time, ``mv``), the tensor is built on the H100 and can go straight into Clair3_F without leaving HBM.  No CPU
-fallback: everything here calls ``libclair3b200.so``.
+and, for dwell time, ``mv``), the tensor is built on the H100 and can go straight into Clair3_F without leaving HBM.  The
+``all_alt_info`` text is formatted on the device too (``alt_text``), and ``call`` takes the candidates from records to call
+records on one stream.  No CPU fallback: everything here calls ``libclair3b200.so``.
 """
 from __future__ import annotations
 
@@ -14,7 +15,8 @@ import numpy as np
 import torch
 
 from ._ffi import CONSTANTS, C3BError, check, ffi, lib
-from .pileup_counts import BamRecords, DeviceBamRecords, _insertion_bytes, _records_struct, _Workspace, khash_iteration_order
+from .pileup_counts import (BamRecords, DeviceBamRecords, _device_view, _insertion_bytes, _records_struct, _Workspace,
+                            khash_iteration_order)
 
 FLANKING = 16                   # shared/param_f.py flankingBaseNum
 NO_OF_POSITIONS = 33
@@ -46,6 +48,7 @@ class FullAlignmentBuilder(_Workspace):
         super().__init__(device)
         self._keep = None
         self._shape = None
+        self._alt = None
 
     def build(self, records, candidates, ref_seq, ref_start, variants=None, matrix_depth=89, need_haplotagging=True, min_mq=5,
               max_indel_length=50, dwell=False, rand_seed=1, rand_skip=0):
@@ -96,11 +99,16 @@ class FullAlignmentBuilder(_Workspace):
     def alt_info_strings(self):
         """The ``all_alt_info`` strings (src/clair3_full_alignment_dwell.c:950-1006), one per candidate: ``"<pos+1>-<depth>-<ref>-"``
         then ``X<b> n`` for the non-reference bases in A C G T order, ``I<ref><bases> n`` in the iteration order of the
-        reference's khash string counter, ``D<ref bases> n`` in the order of its khash int counter, ``R<ref> n`` last."""
+        reference's khash string counter, ``D<ref bases> n`` in the order of its khash int counter, ``R<ref> n`` last.  With host
+        records the GPU supplies the counts and allele lists (``c3b_fa_fetch_alleles``) and the text is formatted here
+        (``format_alt_info``: the inserted bases are read from the representative reads), which is the statement the device
+        text is tested against; with device-resident records the strings are the device's (``alt_text()``)."""
+        if self._alt is None:
+            raise C3BError("alt_info_strings: build() first")
         host_ref, ref_start, max_indel = self._alt
         rec = self._keep[0]
         if host_ref is None or isinstance(rec, DeviceBamRecords):
-            raise C3BError("alt_info_strings needs host records and reference (the inserted bases are read on the host)")
+            return self.alt_text().alt_text_fetch()["text"]
         n = self._shape[0]
         na = ffi.new("int64_t *")
         check(lib().c3b_fa_fetch_alleles(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, 0, na))
@@ -121,24 +129,111 @@ class FullAlignmentBuilder(_Workspace):
                                        meta[sl], rd[sl], qp[sl], cn[sl], rec))
         return out
 
+    def alt_text(self, max_indel_length=None):
+        """Enqueues the text stage (``c3b_fa_alt_text``) behind the last ``build``, on its stream and without a host wait: the
+        ``all_alt_info`` string of every candidate and what the decoder takes of it, formatted on the device.
+        ``max_indel_length``: as ``calculate_clair3_full_alignment``'s (default: what ``build`` was given).  Device-resident
+        records must stay alive until the text has been fetched."""
+        if self._alt is None:
+            raise C3BError("alt_text: build() first")
+        if max_indel_length is None:
+            max_indel_length = self._alt[2]
+        if isinstance(max_indel_length, bool) or not isinstance(max_indel_length, (int, np.integer)):
+            raise C3BError("alt_text: max_indel_length must be an integer, got %r" % (max_indel_length,))
+        check(lib().c3b_fa_alt_text(self._h, int(max_indel_length)))
+        return self
+
+    def alt_text_sizes(self):
+        """(bytes of all text strings, bytes of all decoder strings) of the last ``alt_text``."""
+        a, b = ffi.new("int64_t *"), ffi.new("int64_t *")
+        check(lib().c3b_fa_alt_text_sizes(self._h, a, b))
+        return int(a[0]), int(b[0])
+
+    def alt_text_fetch(self):
+        """dict: ``text`` (the ``all_alt_info`` strings, one per candidate), ``decoder`` (the ``"depth-alt"`` strings of
+        ``create_tensor_full_alignment``), ``ref_base`` uint8 [n_cand], ``position`` int64 [n_cand] (1-based).  Waits for the
+        text stage."""
+        nk = self._shape[0]
+        nt, nd = self.alt_text_sizes()
+        text, dec = np.zeros(max(nt, 1), np.uint8), np.zeros(max(nd, 1), np.uint8)
+        toff, doff = np.zeros(nk + 1, np.int64), np.zeros(nk + 1, np.int64)
+        rb, pos = np.zeros(nk, np.uint8), np.zeros(nk, np.int64)
+        c = ffi.cast
+        check(lib().c3b_fa_fetch_alt_text(self._h, c("char *", text.ctypes.data), c("int64_t *", toff.ctypes.data),
+                                          c("char *", dec.ctypes.data), c("int64_t *", doff.ctypes.data),
+                                          c("uint8_t *", rb.ctypes.data), c("int64_t *", pos.ctypes.data)))
+        tb, db = text.tobytes(), dec.tobytes()
+        return {"text": [tb[toff[j]:toff[j + 1]].decode("latin-1") for j in range(nk)],
+                "decoder": [db[doff[j]:doff[j + 1]].decode("latin-1") for j in range(nk)], "ref_base": rb, "position": pos}
+
+    def alt_text_device(self):
+        """The text stage's results as tensors that alias the workspace (valid until the next ``build`` / ``alt_text``):
+        ``text`` uint8 [n_text_bytes], ``text_off`` int64 [n_cand + 1], ``decoder`` uint8 [n_decoder_bytes], ``decoder_off``
+        int64 [n_cand + 1], ``ref_base`` uint8 [n_cand], ``position`` int64 [n_cand]; ``decoder`` / ``decoder_off`` /
+        ``ref_base`` are ``decode_calls``' ``alt_bytes`` / ``alt_offsets`` / ``ref_base``.  Waits (``c3b_fa_sizes``) only when
+        nothing has waited since the last ``build`` / ``alt_text``; after that wait it touches the stream no more."""
+        nk = self._shape[0]
+        nt, nd = self.alt_text_sizes()
+        p = [ffi.new("const char **"), ffi.new("const int64_t **"), ffi.new("const char **"), ffi.new("const int64_t **"),
+             ffi.new("const uint8_t **"), ffi.new("const int64_t **")]
+        check(lib().c3b_fa_alt_text_device(self._h, *p))
+        shapes = (("text", nt, torch.uint8), ("text_off", nk + 1, torch.int64), ("decoder", nd, torch.uint8),
+                  ("decoder_off", nk + 1, torch.int64), ("ref_base", nk, torch.uint8), ("position", nk, torch.int64))
+        return {name: _device_view(int(ffi.cast("uintptr_t", q[0])), n, dt, self._device) for (name, n, dt), q in zip(shapes, p)}
+
+    def alt_text_last_ms(self):
+        """Device time and kernel launches of the last ``alt_text`` (``last_ms`` reports the build alone)."""
+        return self._timing(lib().c3b_fa_alt_text_last_ms)
+
     def forward(self, model):
         """Clair3_F over every candidate of the last build, straight from the device-resident matrix (``c3b_forward`` with
         ``x_on_device = 1``, int8).  Returns what ``model(x)`` returns for the same matrix, on the device."""
-        if getattr(model, "_handle", None) is None:
-            raise C3BError("forward: the model has no device / weights yet (.to(device), .load_state_dict())")
-        n, depth, C = self._shape
-        if model._kind != CONSTANTS["C3B_FULL_ALIGNMENT"] or model.input_channels != C:
-            raise C3BError("forward: needs the full-alignment network (Clair3_F) with %d input channels" % C)
-        if torch.device(model._device) != self._device:
-            raise C3BError("forward: the model lives on %s, the builder on %s" % (model._device, self._device))
+        self._check_model(model, "forward")
         self.sizes()
-        y = torch.empty((n, model.out_dim), dtype=torch.float32, device=self._device)
-        if n:
-            pm = ffi.new("const int8_t **")
-            check(lib().c3b_fa_device(self._h, pm))
-            check(lib().c3b_forward(model._handle, ffi.cast("void *", pm[0]), CONSTANTS["C3B_DT_I8"], 1, n, depth,
-                                    ffi.cast("float *", y.data_ptr()), 1, self._stream()))
+        y = torch.empty((self._shape[0], model.out_dim), dtype=torch.float32, device=self._device)
+        self._forward_into(model, y)
         return model._split(y)
+
+    def call(self, model, output_config, ctg_name, k=16):
+        """The candidates of the last ``build`` from records to call records on the current stream: the text stage, Clair3_F
+        over the device matrix and ``model.decode_calls`` on the device views, with one host wait (the sizes) before the
+        network is queued.  Returns ``decode.batch_calls``' dict (``chromosome``, ``position``, ``calls``, ``text``, ``ad``,
+        ``start``; ``decode.calls_text`` formats it) plus ``Y``, the probabilities, on the device.  Every candidate is decoded,
+        as the reference decodes every full-alignment candidate.  Raises what ``batch_calls`` raises on an alt_info string the
+        decoder rejects."""
+        from . import decode
+        decode._check_config(output_config)
+        self._check_model(model, "call")
+        if bool(output_config.add_indel_length) != model.add_indel_length:
+            raise C3BError("call: output_config.add_indel_length must match the model")
+        self.alt_text()
+        nk = self.sizes()[0]                               # the one wait: the build and the text together
+        v = self.alt_text_device()
+        y = torch.empty((nk, model.out_dim), dtype=torch.float32, device=self._device)
+        self._forward_into(model, y)
+        out = model.decode_calls(y, v["ref_base"], v["decoder"], v["decoder_off"], output_config, k=k)
+        res = decode.calls_result(decode._numpy(out), [ctg_name] * nk, v["position"].cpu().numpy(), v["decoder_off"].cpu().numpy())
+        res["Y"] = y
+        return res
+
+    def _check_model(self, model, who):
+        if getattr(model, "_handle", None) is None:
+            raise C3BError("%s: the model has no device / weights yet (.to(device), .load_state_dict())" % who)
+        C = self._shape[2]
+        if model._kind != CONSTANTS["C3B_FULL_ALIGNMENT"] or model.input_channels != C:
+            raise C3BError("%s: needs the full-alignment network (Clair3_F) with %d input channels" % (who, C))
+        if torch.device(model._device) != self._device:
+            raise C3BError("%s: the model lives on %s, the builder on %s" % (who, model._device, self._device))
+
+    def _forward_into(self, model, y):
+        """Clair3_F over every candidate's matrix into y, stream-ordered."""
+        n, depth, _ = self._shape
+        if n == 0:
+            return
+        pm = ffi.new("const int8_t **")
+        check(lib().c3b_fa_device(self._h, pm))
+        check(lib().c3b_forward(model._handle, ffi.cast("void *", pm[0]), CONSTANTS["C3B_DT_I8"], 1, n, depth,
+                                ffi.cast("float *", y.data_ptr()), 1, self._stream()))
 
 
 def format_alt_info(candidate, depth, acgt, ref, ref_start, max_indel_length, meta, read, qpos, cnt, rec):

@@ -8,8 +8,10 @@
  *                                             enable_dwell_time)                         src/clair3_full_alignment_dwell.c:437-1054
  * as bound by preprocess/CreateTensorFullAlignmentFromCffi.py:120-134, from the point where htslib has decoded the records.  The
  * matrix is bit-exact with the reference on the same records (DESIGN.md 5b lists the inputs on which the reference itself is
- * undefined).  The all_alt_info strings are text: the GPU exports each candidate's depth, A/C/G/T counts and distinct indel
- * alleles (c3b_fa_fetch_alleles) and the host formats them (clair3_b200/fa_tensor.py).
+ * undefined).  The all_alt_info strings (:950-1006) are formatted on the GPU as well (c3b_fa_alt_text), together with the form
+ * the decoder takes (c3b_decode_calls in clair3_b200.h): candidates go from records to call records on one stream.  The
+ * per-candidate counts and allele lists the text is made from can still be exported (c3b_fa_fetch_alleles);
+ * clair3_b200/fa_tensor.py formats them on the host, which is what the tests hold the GPU text to.
  *
  * Same conventions as clair3_b200.h: int status, 0 = ok, message via c3b_last_error(); no CPU fallback.
  */
@@ -88,13 +90,49 @@ int c3b_fa_fetch(c3b_fa *w, int8_t *matrix, int32_t *kept_haplotype, int64_t *ke
  *                    an allele of that kind again, which still grows a full khash (khash.h:310-318);
  *   read [n] uint32  record index of the first read that showed the allele;
  *   qpos [n] uint32  query offset of its first inserted base (insertions);  cnt [n] uint32  reads showing it
- * Alleles are in order of first occurrence (deletions and insertions interleaved).  n_alleles alone sizes the buffers. */
+ * Alleles are in order of first occurrence (deletions and insertions interleaved).  n_alleles alone sizes the buffers.
+ * c3b_fa_alt_text formats the all_alt_info strings from these on the GPU. */
 int c3b_fa_fetch_alleles(c3b_fa *w, int32_t *depth, int32_t *acgt, int32_t *al_off, int32_t *al_n, uint32_t *meta, uint32_t *read,
                          uint32_t *qpos, uint32_t *cnt, int64_t capacity, int64_t *n_alleles);
 
 /* The device matrix, valid until the next c3b_fa_build on w: pass it to c3b_forward(model, matrix, C3B_DT_I8, 1, n_cand,
  * matrix_depth, ...) so the tensor never leaves HBM on its way into Clair3_F. */
 int c3b_fa_device(c3b_fa *w, const int8_t **matrix);
+
+/* The all_alt_info text of every candidate (:950-1006), formatted on the GPU: enqueues the text stage on the stream of the last
+ * c3b_fa_build.  No host wait.  max_indel_length: the reference's argument (longer alleles are counted but not printed).  The
+ * stage reads the records and the reference bases where the build left them: the workspace's own copies, or, after a build
+ * with on_device = 1, the caller's device arrays, which must stay alive and unchanged until the text has been fetched or
+ * consumed.  Per candidate, in candidate order:
+ *   text      "<cand+1>-<depth>-<REF>-X<b> n I<REF><inserted bases> n D<ref bases> n R<REF> n ": REF is the upper-cased
+ *             reference byte ('\0' outside ref_seq); SNP alleles in A C G T order, insertions in the bucket order of the
+ *             reference's khash string counter, deletions in that of its int counter, the remaining reference count last;
+ *             deletion text is the reference's bytes as supplied, up to the end of ref_seq or its first NUL
+ *   decoder   "<depth>-<alt>", alt = the fourth '-'-separated field of the stripped string: what
+ *             preprocess/CreateTensorFullAlignmentFromCffi.py:150-155 hands on as all_alt_info
+ *   ref_base  the same <REF> byte         position  cand + 1
+ * The next c3b_fa_sizes waits for the build and the text together. */
+int c3b_fa_alt_text(c3b_fa *w, int64_t max_indel_length);
+
+/* After c3b_fa_alt_text (waits like c3b_fa_sizes when that has not been called since): bytes of all text strings and of all
+ * decoder strings.  Fails, as c3b_fa_fetch_alt_text does, if the text outgrew the stage's buffers; the build's own results stay
+ * valid, and a later c3b_fa_alt_text (with a smaller max_indel_length, say) starts clean. */
+int c3b_fa_alt_text_sizes(c3b_fa *w, int64_t *n_text_bytes, int64_t *n_decoder_bytes);
+
+/* Host copies (any pointer may be NULL): text [n_text_bytes], text_off [n_cand + 1] int64 (candidate j is
+ * text[text_off[j] .. text_off[j + 1])), decoder [n_decoder_bytes], decoder_off [n_cand + 1], ref_base [n_cand],
+ * position [n_cand]. */
+int c3b_fa_fetch_alt_text(c3b_fa *w, char *text, int64_t *text_off, char *decoder, int64_t *decoder_off, uint8_t *ref_base,
+                          int64_t *position);
+
+/* Device views of the same, valid until the next c3b_fa_build or c3b_fa_alt_text on w: decoder / decoder_off / ref_base are
+ * the alt_bytes / alt_offsets / ref_base arguments of c3b_decode_calls(..., on_device = 1). */
+int c3b_fa_alt_text_device(c3b_fa *w, const char **text, const int64_t **text_off, const char **decoder,
+                           const int64_t **decoder_off, const uint8_t **ref_base, const int64_t **position);
+
+/* Device time of the last c3b_fa_alt_text (CUDA events around its kernels) and the number of kernels it launched;
+ * c3b_fa_last_ms keeps reporting the build alone. */
+int c3b_fa_alt_text_last_ms(c3b_fa *w, float *ms, int *launches);
 
 /* Device time of the last c3b_fa_build (CUDA events around its kernels, input copies excluded) and its kernel launches. */
 int c3b_fa_last_ms(c3b_fa *w, float *ms, int *launches);
