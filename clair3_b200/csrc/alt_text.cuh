@@ -1,8 +1,20 @@
 // alt_text.cuh - what the two all_alt_info text stages share: the pileup counter's (plp_alt_text.cu) and the full-alignment
-// builder's (fa_alt_text.cu).  Both measure each candidate's string with a counting sink, scan the lengths, and write it again
-// with a bounded sink; both order a kind of allele by replaying klib's khash (src/khash.h) over it.
+// builder's (fa_alt_text.cu).  Candidates are independent and their strings have data-dependent length, so each stage is
+//
+//   measure   the stage's own kernel, one WARP per candidate: orders the candidate's allele records - each kind by replaying
+//             klib's khash (src/khash.h) over it - then lane 0 walks the string once with a counting sink (text_measure_tail)
+//   scan      two one-CTA exclusive scans (block_scan.cuh) over n_cand + 1 lengths: per-candidate offsets and the byte totals
+//   write     text_write_kernel, one THREAD per candidate: walks the same string with a sink bounded by what measure found
+//
+// launched by text_launch.  A stage is a struct with its argument type (derived from C3bAltText), the candidate count as the
+// kernels read it and as the scans take it, a candidate's position and the reference byte there, and emit: the walk over one
+// candidate's string into a TextOut.  Same records, same bytes, whatever the launch shape: nothing is atomic but the status word.
 #pragma once
+#include <limits.h>
 #include <stdint.h>
+
+#include "block_scan.cuh"
+#include "c3b_internal.h"
 
 // Each translation unit keeps its own copies: the library is built without relocatable device code.
 namespace {
@@ -99,6 +111,62 @@ __device__ bool khash_replay(const uint32_t *hash, int32_t *keys, const int n, c
     for (int b = 0; b < nb; ++b)
         if (slot[b] & KH_VAL) keys[k++] = (int32_t)(slot[b] & KH_VAL) - 1;
     return true;
+}
+
+// Lane 0 of a measure kernel, once the stage has left candidate j's ni insertions and nd deletions in `order` (fits: its records
+// and khash tables fitted the scratch): measures the string and stores what the scans, the write kernel and the decoder read.
+template <class Stage>
+__device__ void text_measure_tail(const typename Stage::Args &A, const int64_t j, bool fits, int ni, int nd) {
+    if (!fits) { atomicOr(A.status, 1); ni = nd = 0; }
+    A.n_ins[j] = ni;
+    A.n_del[j] = nd;
+    TextOut<CountSink> o;
+    Stage::emit(A, j, ni, nd, o);
+    if (!o.cut && o.n_alt > 0) --o.dec.n;                     // rstrip(): the alt text ends in one space
+    if (!fits || o.full.n > INT_MAX || o.dec.n > INT_MAX) {
+        atomicOr(A.status, 1);
+        o.full.n = o.dec.n = 0;
+    }
+    A.len_text[j] = (int32_t)o.full.n;
+    A.len_dec[j] = (int32_t)o.dec.n;
+    const int64_t pos = Stage::pos(A, j);
+    A.ref_base[j] = (uint8_t)Stage::ref_base(A, pos);
+    A.position[j] = pos + 1;
+}
+
+template <class Stage> __global__ void __launch_bounds__(128) text_write_kernel(typename Stage::Args A) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= Stage::n_cand(A)) return;
+    const int64_t t0 = A.text_off[j], t1 = A.text_off[j + 1], d0 = A.dec_off[j], d1 = A.dec_off[j + 1];
+    if (t1 > A.text_cap || d1 > A.dec_cap) { atomicOr(A.status, 1); return; }
+    TextOut<WriteSink> o;
+    o.full.p = A.text + t0; o.full.lim = t1 - t0;
+    o.dec.p = A.dec + d0; o.dec.lim = d1 - d0;
+    if (t1 > t0) Stage::emit(A, j, A.n_ins[j], A.n_del[j], o);
+}
+
+// Queues a stage on stream s: measure, the two scans and text_write_kernel, sized from the bound a.n.  An empty stage writes the
+// one offset of each scan instead.  `who` names the entry point in the errors.
+template <class Stage>
+int text_launch(const typename Stage::Args &a, void (*measure)(typename Stage::Args), cudaStream_t s, int *launches, const char *who) {
+    if (a.n == 0) {
+        C3B_CUDA(cudaMemsetAsync(a.text_off, 0, 8, s));
+        C3B_CUDA(cudaMemsetAsync(a.dec_off, 0, 8, s));
+        return 0;
+    }
+    if (a.al_cap >= (int64_t)KH_VAL) {
+        c3b_set_error("%s: %lld allele records exceed the khash replay's 24-bit record index", who, (long long)a.al_cap);
+        return 1;
+    }
+    int64_t blocks = ((a.n + 1) * 32 + 255) / 256;
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    measure<<<(unsigned)blocks, 256, 0, s>>>(a);
+    block_scan_sum(a.len_text, a.text_off, a.n + 1, Stage::n_cand_dev(a), a.totals, s);
+    block_scan_sum(a.len_dec, a.dec_off, a.n + 1, Stage::n_cand_dev(a), a.totals + 1, s);
+    text_write_kernel<Stage><<<(unsigned)((a.n + 127) / 128), 128, 0, s>>>(a);
+    C3B_CUDA(cudaGetLastError());
+    *launches = 4;
+    return 0;
 }
 
 }  // namespace

@@ -170,9 +170,39 @@ int c3b_last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s
 // is no CUDA device or it is not sm_90; 1 for a bad ordinal or a failed runtime call.  sm_count (optional): its SM count.
 int c3b_use_device(int ordinal, int unsupported, int *sm_count);
 
+constexpr int C3B_AL_CAP = 1 << 22;     // allele records the pileup counter or the full-alignment builder exports per call
+
+// What both all_alt_info text stages (alt_text.cuh) take: the records and the reference where the count or build left them, the
+// exported allele records, the stage's scratch and outputs, and its status word and byte totals in the counter block.  The
+// pileup counter's PlpAltTextArgs and the full-alignment builder's FaAltTextArgs add their own candidate data.
+struct C3bAltText {
+    int64_t n;                          // the bound on the candidates the grids and buffers are sized from
+    int64_t ref_start, ref_len, max_indel_length;
+    const char *ref;
+    C3bReads R;
+    const int32_t *al_off, *al_n;       // per column / candidate: its first record and number of records
+    const uint32_t *al_meta, *al_read, *al_qpos, *al_cnt;
+    int64_t al_cap;                     // records the al_* arrays and the per-record scratch hold
+    // scratch
+    uint32_t *hash;                     // [al_cap]
+    int32_t *order;                     // [al_cap]
+    uint32_t *table;                    // [8 * n + 3 * al_cap] khash buckets
+    int32_t *n_ins, *n_del;             // [n]
+    int32_t *len_text, *len_dec;        // [n + 1]
+    int *status;                        // the stage's status word: non-zero = a candidate's text did not fit the stage's buffers
+    // outputs
+    char *text, *dec;
+    int64_t text_cap, dec_cap;
+    int64_t *text_off, *dec_off;        // [n + 1]
+    int64_t *totals;                    // device: n_text_bytes, n_decoder_bytes
+    uint8_t *ref_base;                  // [n]
+    int64_t *position;                  // [n]
+};
+
 // What the pileup counter (c3b_plp) and the full-alignment builder (c3b_fa) hold alike: the device and the stream of the last
 // call, a pair of CUDA events around each timed stage with the stage's kernel launches, a device counter block with its pinned
-// host mirror, and the exported allele records.  The destructor releases the events and the pinned memory.
+// host mirror, the exported allele records, and the all_alt_info text stage (stage 1).  The destructor releases the events and
+// the pinned memory.
 struct C3bRegionWorkspace {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -180,7 +210,16 @@ struct C3bRegionWorkspace {
     int launches[2] = {};
     C3bBuf counters;
     int64_t *host_counters = nullptr;    // pinned copy of `counters`
-    C3bBuf al_meta, al_read, al_qpos, al_cnt;
+    int n_counters = 0;
+    int text_word = 0;                   // counters[text_word .. +2]: the text stage's status, text bytes, decoder bytes
+    C3bBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n;
+    // the text stage: where the last count / build left the records and the reference, the stage's scratch and outputs
+    C3bReads R{};
+    const char *dref = nullptr;
+    int64_t ref_start = 0, ref_len = 0, n_cigar = 0, n_seq = 0;
+    C3bBuf tx_hash, tx_order, tx_table, tx_nins, tx_ndel, tx_len_text, tx_len_dec;
+    C3bBuf tx_text, tx_dec, tx_text_off, tx_dec_off, tx_ref_base, tx_position;
+    bool texted = false;
 
     C3bRegionWorkspace() = default;
     C3bRegionWorkspace(const C3bRegionWorkspace &) = delete;
@@ -218,16 +257,99 @@ struct C3bRegionWorkspace {
         const size_t b = (size_t)n * 4;
         return get(meta, al_meta, b) || get(read, al_read, b) || get(qpos, al_qpos, b) || get(cnt, al_cnt, b);
     }
+
+    // The text stage over up to n candidates (the counter's region width, the builder's candidate count): sizes and grows its
+    // buffers from what the host knows when the stage is enqueued, and fills the arguments both stages share.  `what` names
+    // the owner in allocation errors.
+    int text_prepare(int64_t n, int64_t max_indel_length, const char *what, C3bAltText &t) {
+        C3B_CUDA(cudaSetDevice(device));
+        texted = false;
+        // every allele record comes from one insertion / deletion operation of one read
+        const int64_t cap = n_cigar < C3B_AL_CAP ? (n_cigar > 0 ? n_cigar : 1) : C3B_AL_CAP;
+        // bytes: head, SNP and R fields per candidate; key, count and separators per record; the inserted bases are query bases;
+        // a printed deletion shows at most max_indel_length reference bases
+        const int64_t del_len = max_indel_length < 0 ? 0 : (max_indel_length < ref_len ? max_indel_length : ref_len);
+        const int64_t del_bytes = cap * del_len < (1ll << 28) ? cap * del_len : (1ll << 28);
+        const int64_t text_cap = 160 * (n + 1) + 48 * cap + 2 * n_seq + del_bytes;
+        const size_t nz = (size_t)n + 1;
+        auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, stream, what); };
+        if (grow(tx_hash, (size_t)cap * 4) || grow(tx_order, (size_t)cap * 4) || grow(tx_table, (8 * nz + 3 * (size_t)cap) * 4) ||
+            grow(tx_nins, nz * 4) || grow(tx_ndel, nz * 4) || grow(tx_len_text, nz * 4) || grow(tx_len_dec, nz * 4) ||
+            grow(tx_text, (size_t)text_cap) || grow(tx_dec, (size_t)text_cap) || grow(tx_text_off, nz * 8) ||
+            grow(tx_dec_off, nz * 8) || grow(tx_ref_base, nz) || grow(tx_position, nz * 8))
+            return 1;
+        int64_t *cnt = counters.as<int64_t>();
+        t.n = n; t.ref_start = ref_start; t.ref_len = ref_len; t.max_indel_length = max_indel_length;
+        t.ref = dref; t.R = R;
+        t.al_off = al_off.as<int32_t>(); t.al_n = al_n.as<int32_t>();
+        t.al_meta = al_meta.as<uint32_t>(); t.al_read = al_read.as<uint32_t>(); t.al_qpos = al_qpos.as<uint32_t>();
+        t.al_cnt = al_cnt.as<uint32_t>(); t.al_cap = cap;
+        t.hash = tx_hash.as<uint32_t>(); t.order = tx_order.as<int32_t>(); t.table = tx_table.as<uint32_t>();
+        t.n_ins = tx_nins.as<int32_t>(); t.n_del = tx_ndel.as<int32_t>();
+        t.len_text = tx_len_text.as<int32_t>(); t.len_dec = tx_len_dec.as<int32_t>();
+        t.status = reinterpret_cast<int *>(cnt + text_word);
+        t.text = tx_text.as<char>(); t.dec = tx_dec.as<char>(); t.text_cap = t.dec_cap = text_cap;
+        t.text_off = tx_text_off.as<int64_t>(); t.dec_off = tx_dec_off.as<int64_t>(); t.totals = cnt + text_word + 1;
+        t.ref_base = tx_ref_base.as<uint8_t>(); t.position = tx_position.as<int64_t>();
+        return 0;
+    }
+    // Queues the stage text_prepare sized: clears its three counter words (an earlier stage's overflow is not this one's), runs
+    // launch(a, stream, launches) between the stage's events, and copies the counter block back, so the workspace's next wait
+    // also brings the stage's status and byte totals.
+    template <class Args> int text_enqueue(const Args &a, int (*launch)(const Args &, cudaStream_t, int *)) {
+        launches[1] = 0;
+        C3B_CUDA(cudaMemsetAsync(counters.as<int64_t>() + text_word, 0, 3 * 8, stream));
+        C3B_CUDA(cudaEventRecord(ev[1][0], stream));
+        if (launch(a, stream, &launches[1])) return 1;
+        C3B_CUDA(cudaEventRecord(ev[1][1], stream));
+        C3B_CUDA(cudaMemcpyAsync(host_counters, counters.p, (size_t)n_counters * 8, cudaMemcpyDeviceToHost, stream));
+        texted = true;
+        return 0;
+    }
+    // The stage's byte totals, once the workspace's own wait has brought the counter block.  `who` names the entry point in the
+    // error, `hint` what its caller can do when the text outgrew the stage's buffers.
+    int text_sizes(const char *who, const char *hint, int64_t *n_text_bytes, int64_t *n_decoder_bytes) {
+        if (host_counters[text_word] != 0) {
+            c3b_set_error("%s: the all_alt_info text outgrew its buffers; %s or lower max_indel_length", who, hint);
+            return 1;
+        }
+        if (n_text_bytes) *n_text_bytes = host_counters[text_word + 1];
+        if (n_decoder_bytes) *n_decoder_bytes = host_counters[text_word + 2];
+        return 0;
+    }
+    // Copies the stage's outputs for n_cand candidates into whichever host arrays are given, and waits for them.
+    int text_fetch(const char *who, const char *hint, int64_t n_cand, char *text, int64_t *text_off, char *decoder,
+                   int64_t *decoder_off, uint8_t *ref_base, int64_t *position) {
+        int64_t nt = 0, nd = 0;
+        if (text_sizes(who, hint, &nt, &nd)) return 1;
+        const size_t nk = (size_t)n_cand;
+        return get(text, tx_text, (size_t)nt) || get(text_off, tx_text_off, (nk + 1) * 8) || get(decoder, tx_dec, (size_t)nd) ||
+               get(decoder_off, tx_dec_off, (nk + 1) * 8) || get(ref_base, tx_ref_base, nk) || get(position, tx_position, nk * 8) ||
+               wait();
+    }
+    // The stage's outputs where they live on the device.
+    void text_device(const char **text, const int64_t **text_off, const char **decoder, const int64_t **decoder_off,
+                     const uint8_t **ref_base, const int64_t **position) const {
+        if (text) *text = tx_text.as<char>();
+        if (text_off) *text_off = tx_text_off.as<int64_t>();
+        if (decoder) *decoder = tx_dec.as<char>();
+        if (decoder_off) *decoder_off = tx_dec_off.as<int64_t>();
+        if (ref_base) *ref_base = tx_ref_base.as<uint8_t>();
+        if (position) *position = tx_position.as<int64_t>();
+    }
 };
 
 // Creates a W (derived from C3bRegionWorkspace) on device `ordinal`: `stages` event pairs and a block of `n_counters` int64
-// counters, on the device and pinned on the host.  `who` names the entry point in the errors.
-template <class W> int c3b_region_create(W **out, int ordinal, int stages, int n_counters, const char *who) {
+// counters, on the device and pinned on the host, of which `text_word` and the two after it are the text stage's.  `who` names
+// the entry point in the errors.
+template <class W> int c3b_region_create(W **out, int ordinal, int stages, int n_counters, int text_word, const char *who) {
     if (!out) { c3b_set_error("%s: null out", who); return 1; }
     *out = nullptr;
     if (c3b_use_device(ordinal, 1, nullptr)) return 1;
     W *w = new W();
     w->device = ordinal;
+    w->n_counters = n_counters;
+    w->text_word = text_word;
     bool ok = w->counters.ensure((size_t)n_counters * 8, nullptr, who) == 0 &&
               cudaMallocHost((void **)&w->host_counters, (size_t)n_counters * 8) == cudaSuccess;
     for (int i = 0; i < stages && ok; ++i)
@@ -468,58 +590,20 @@ int c3b_launch_ingest_fa_tc(const void *x, int dtype, int channels, int cpad, op
 int c3b_launch_spp_tc(const op_t *x, const PlanarGeom &g, op_t *out, int64_t batch, int c, int bp, cudaStream_t s);
 
 // ---- pileup feature counter: the all_alt_info text stage (plp_alt_text.cu), enqueued by c3b_plp_alt_text in plp_counts.cu ----
-struct PlpAltTextArgs {
-    // the count's results (device)
-    int64_t start, end, ref_start, ref_len, max_indel_length;
-    int64_t W;                          // end - start: the bound on the candidates the grids are sized from
+// n is the region's width, end - start; the candidates are the count's, their number a device counter
+struct PlpAltTextArgs : C3bAltText {
+    int64_t start, end;
     const int64_t *n_cand;              // device counter
     const int64_t *cand_cols, *major, *matrix;
-    const int32_t *stats;
-    const char *ref;
-    C3bReads R;                         // the records where the count left them
-    const int32_t *al_off, *al_n, *ins_last;
-    const uint32_t *al_meta, *al_read, *al_qpos, *al_cnt;
-    int64_t al_cap;                     // records the al_* arrays and mate / hash / order hold
-    // scratch
-    int32_t *mate, *order;              // [al_cap]
-    uint32_t *hash;                     // [al_cap]
-    uint32_t *table;                    // [8 * W + 3 * al_cap] khash buckets
-    int32_t *n_ins, *n_del;             // [W]
-    int32_t *len_text, *len_dec;        // [W + 1]
-    int *status;                        // the stage's status word: non-zero = a candidate's text did not fit the stage's buffers
-    // outputs
-    char *text, *dec;
-    int64_t text_cap, dec_cap;
-    int64_t *text_off, *dec_off;        // [W + 1]
-    int64_t *totals;                    // device: n_text_bytes, n_decoder_bytes
-    uint8_t *ref_base;                  // [W]
-    int64_t *position;                  // [W]
+    const int32_t *stats, *ins_last;
+    int32_t *mate;                      // scratch [al_cap]
 };
 int c3b_launch_plp_alt_text(const PlpAltTextArgs &a, cudaStream_t s, int *launches);
 
 // ---- full-alignment builder: the all_alt_info text stage (fa_alt_text.cu), enqueued by c3b_fa_alt_text in fa_tensor.cu ----
-struct FaAltTextArgs {
-    // the build's results (device)
-    int64_t n_cand, ref_start, ref_len, max_indel_length;
-    const int64_t *cand;                // [n_cand] 0-based positions
-    const char *ref;
-    C3bReads R;                         // the records where the build left them
-    const int32_t *c_depth, *c_acgt, *al_off, *al_n;
-    const uint32_t *al_meta, *al_read, *al_qpos, *al_cnt;
-    int64_t al_cap;                     // records the al_* arrays and hash / order hold
-    // scratch
-    uint32_t *hash;                     // [al_cap]
-    int32_t *order;                     // [al_cap]
-    uint32_t *table;                    // [8 * n_cand + 3 * al_cap] khash buckets
-    int32_t *n_ins, *n_del;             // [n_cand]
-    int32_t *len_text, *len_dec;        // [n_cand + 1]
-    int *status;                        // the stage's status word: non-zero = a candidate's text did not fit the stage's buffers
-    // outputs
-    char *text, *dec;
-    int64_t text_cap, dec_cap;
-    int64_t *text_off, *dec_off;        // [n_cand + 1]
-    int64_t *totals;                    // device: n_text_bytes, n_decoder_bytes
-    uint8_t *ref_base;                  // [n_cand]
-    int64_t *position;                  // [n_cand]
+// n is the number of candidates, known on the host
+struct FaAltTextArgs : C3bAltText {
+    const int64_t *cand;                // [n] 0-based positions
+    const int32_t *c_depth, *c_acgt;
 };
 int c3b_launch_fa_alt_text(const FaAltTextArgs &a, cudaStream_t s, int *launches);

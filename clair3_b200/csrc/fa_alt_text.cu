@@ -5,40 +5,42 @@
 //     "<cand+1>-<depth>-<REF>-X<b> n I<REF><inserted bases> n D<ref bases> n R<REF> n "
 // clair3_b200/fa_tensor.py: format_alt_info / khash_iteration_order state the same on the host and are what the tests hold these
 // kernels to.  K11 (fa_candidate_kernel) already exports each candidate's depth, A/C/G/T counts and its distinct indel alleles,
-// merged over the strands and in put order (the order in which the reference's two khash counters saw them), so the stage is
+// merged over the strands and in put order (the order in which the reference's two khash counters saw them).  The stage is
+// alt_text.cuh's measure -> scan -> write (F2 the scans, F3 text_write_kernel); what is the builder's own is
 //
 //   F1 fa_text_measure    one WARP per candidate over its allele records [al_off, al_off + al_n): lanes hash them (X31 over the
 //                         NT16 bases of an insertion string, the length of a deletion: kh_int_hash_func) and split them, in put
-//                         order, into the insertions and then the deletions; lane 0 replays the two khash tables (alt_text.cuh)
-//                         and walks the string once with a counting sink: the bytes of the full text and of the decoder form.
-//   F2 (block_scan)       the two exclusive scans over n_cand + 1 lengths: per-candidate offsets and the totals.
-//   F3 fa_text_write      one THREAD per candidate walks the same string with a writing sink.
+//                         order, into the insertions and then the deletions; lane 0 replays the two khash tables (alt_text.cuh).
+//   FaText::emit          the string, from the candidate's counters and its ordered records.
 //
 // Scratch is global and addressed by the candidate's own record range (hash / order) or by that range and the candidate index
 // (the khash table: 8 buckets per candidate, or up to 3 per record; both tables of a candidate use the same buckets, one after
-// the other), so a candidate with thousands of distinct alleles needs no capacity of its own.  Same records, same bytes, whatever
-// the launch shape: nothing here is atomic but the status word.
-#include <limits.h>
-
+// the other), so a candidate with thousands of distinct alleles needs no capacity of its own.  The candidate count is a host value.
 #include "alt_text.cuh"
-#include "block_scan.cuh"
-#include "c3b_internal.h"
 
 namespace {
 
-// upper_base of the reference base under a candidate, '\0' outside the supplied reference (as the host formatter writes it)
-__device__ __forceinline__ char fa_ref_base_at(const FaAltTextArgs &A, int64_t pos) {
-    const int64_t off = pos - A.ref_start;
-    const char c = (off >= 0 && off < A.ref_len) ? A.ref[off] : '\0';
-    return (c >= 'a' && c <= 'z') ? (char)(c - 32) : c;
-}
+// The stage for alt_text.cuh: the candidate count is known on the host.
+struct FaText {
+    typedef FaAltTextArgs Args;
+    static __device__ __forceinline__ int64_t n_cand(const Args &A) { return A.n; }
+    static const int64_t *n_cand_dev(const Args &) { return nullptr; }
+    static __device__ __forceinline__ int64_t pos(const Args &A, int64_t j) { return A.cand[j]; }
+    // upper_base of the reference base under a candidate, '\0' outside the supplied reference (as the host formatter writes it)
+    static __device__ __forceinline__ char ref_base(const Args &A, int64_t pos) {
+        const int64_t off = pos - A.ref_start;
+        const char c = (off >= 0 && off < A.ref_len) ? A.ref[off] : '\0';
+        return (c >= 'a' && c <= 'z') ? (char)(c - 32) : c;
+    }
+    template <class S> static __device__ void emit(const Args &A, int64_t j, int ni, int nd, TextOut<S> &o);
+};
 
 // One candidate's string, src/clair3_full_alignment_dwell.c:950-1006, from its counters and the allele records F1 left in
 // `order`: ni insertions, then nd deletions, each kind in bucket order.
-template <class S> __device__ void fa_text_emit(const FaAltTextArgs &A, const int64_t j, const int ni, const int nd, TextOut<S> &o) {
+template <class S> __device__ void FaText::emit(const Args &A, const int64_t j, const int ni, const int nd, TextOut<S> &o) {
     const int64_t c = A.cand[j], off = c - A.ref_start;
     const int a0 = A.al_off[j];
-    const char rb = fa_ref_base_at(A, c);
+    const char rb = ref_base(A, c);
     const int rf = rb == 'C' ? 1 : rb == 'G' ? 2 : rb == 'T' ? 3 : 0;    // acgt2num, src/clair3_full_alignment_dwell.h:49-54
     const int32_t *acgt = A.c_acgt + 4 * j;
     long long ref_count = acgt[rf];
@@ -93,8 +95,8 @@ __global__ void __launch_bounds__(256) fa_text_measure_kernel(FaAltTextArgs A) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    for (int64_t j = warp; j <= A.n_cand; j += nwarps) {
-        if (j == A.n_cand) {                                  // the scans run over n_cand + 1 entries: the last offset is the total
+    for (int64_t j = warp; j <= A.n; j += nwarps) {
+        if (j == A.n) {                                       // the scans run over n_cand + 1 entries: the last offset is the total
             if (lane == 0) A.len_text[j] = A.len_dec[j] = 0;
             continue;
         }
@@ -143,55 +145,21 @@ __global__ void __launch_bounds__(256) fa_text_measure_kernel(FaAltTextArgs A) {
         }
         __syncwarp();
         if (lane == 0) {
-            int nd = n - ni;
+            const int nd = n - ni;
             if (fits && n > 0) {                              // the two khash replays: short serial walks on the same buckets
                 uint32_t *slot = A.table + 8 * j;
                 int avail = 8;
-                if (ni > 3 || nd > 3) { slot = A.table + 8 * A.n_cand + 3 * (int64_t)a0; avail = 3 * n; }
+                if (ni > 3 || nd > 3) { slot = A.table + 8 * A.n + 3 * (int64_t)a0; avail = 3 * n; }
                 fits = khash_replay(A.hash, A.order + a0, ni, again_i, slot, avail) &&
                        khash_replay(A.hash, A.order + a0 + ni, nd, again_d, slot, avail);
             }
-            if (!fits) { atomicOr(A.status, 1); ni = nd = 0; }
-            A.n_ins[j] = ni;
-            A.n_del[j] = nd;
-            TextOut<CountSink> o;
-            fa_text_emit(A, j, ni, nd, o);
-            if (!o.cut && o.n_alt > 0) --o.dec.n;             // rstrip(): the alt text ends in one space
-            if (!fits || o.full.n > INT_MAX || o.dec.n > INT_MAX) {
-                atomicOr(A.status, 1);
-                o.full.n = o.dec.n = 0;
-            }
-            A.len_text[j] = (int32_t)o.full.n;
-            A.len_dec[j] = (int32_t)o.dec.n;
-            A.ref_base[j] = (uint8_t)fa_ref_base_at(A, A.cand[j]);
-            A.position[j] = A.cand[j] + 1;
+            text_measure_tail<FaText>(A, j, fits, ni, nd);
         }
     }
-}
-
-// ---------------------------------------------------------------------------------------------------------------- F3
-__global__ void __launch_bounds__(128) fa_text_write_kernel(FaAltTextArgs A) {
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= A.n_cand) return;
-    const int64_t t0 = A.text_off[j], t1 = A.text_off[j + 1], d0 = A.dec_off[j], d1 = A.dec_off[j + 1];
-    if (t1 > A.text_cap || d1 > A.dec_cap) { atomicOr(A.status, 1); return; }
-    TextOut<WriteSink> o;
-    o.full.p = A.text + t0; o.full.lim = t1 - t0;
-    o.dec.p = A.dec + d0; o.dec.lim = d1 - d0;
-    if (t1 > t0) fa_text_emit(A, j, A.n_ins[j], A.n_del[j], o);
 }
 
 }  // namespace
 
 int c3b_launch_fa_alt_text(const FaAltTextArgs &a, cudaStream_t s, int *launches) {
-    if (a.al_cap >= (int64_t)KH_VAL) { c3b_set_error("c3b_fa_alt_text: %lld allele records exceed the khash replay's 24-bit record index", (long long)a.al_cap); return 1; }
-    int64_t blocks = ((a.n_cand + 1) * 32 + 255) / 256;
-    if (blocks > 132 * 8) blocks = 132 * 8;
-    fa_text_measure_kernel<<<(unsigned)blocks, 256, 0, s>>>(a);
-    block_scan_sum(a.len_text, a.text_off, a.n_cand + 1, nullptr, a.totals, s);
-    block_scan_sum(a.len_dec, a.dec_off, a.n_cand + 1, nullptr, a.totals + 1, s);
-    fa_text_write_kernel<<<(unsigned)((a.n_cand + 127) / 128), 128, 0, s>>>(a);
-    C3B_CUDA(cudaGetLastError());
-    *launches = 4;
-    return 0;
+    return text_launch<FaText>(a, fa_text_measure_kernel, s, launches, "c3b_fa_alt_text");
 }

@@ -51,7 +51,6 @@ constexpr int CAND_THREADS = 256;
 constexpr int MAX_PS = 64;          // distinct phase sets one read may touch (K7)
 constexpr int MAX_OVERWRITTEN = 64; // insertions on one candidate that a later insertion of the same read and anchor overwrote (K11)
 constexpr int JUMP_BITS = 63;       // rand() offsets below 2^63
-constexpr int AL_CAP = 1 << 22;     // exported allele records per call
 
 struct PosInfo {                    // Pos_info (src/clair3_full_alignment_dwell.h:138-146); alt 0 = not covered by M / D
     int8_t alt;                     // nt16 code, -1 deleted
@@ -676,7 +675,7 @@ __global__ void __launch_bounds__(CAND_THREADS) fa_candidate_kernel(CandArgs A) 
         for (int i = 0; i < n_all; ++i) nal += (ev_dcnt[i] > 0) + (ev_icnt[i] > 0);
         for (int x = 0; x < n_ow; ++x) nal += ow_cnt[x] > 0;
         const unsigned long long o = nal ? atomicAdd(A.al_used, (unsigned long long)nal) : 0ull;
-        if (o + (unsigned long long)nal > (unsigned long long)AL_CAP) {
+        if (o + (unsigned long long)nal > (unsigned long long)C3B_AL_CAP) {
             atomicOr(A.status, 2);
             A.al_off[ci] = 0;
             A.al_n[ci] = 0;
@@ -917,7 +916,7 @@ void glibc_jump_matrices(std::vector<uint32_t> &out) {
 
 // Timed stages: 0 the build (c3b_fa_build), 1 the text (c3b_fa_alt_text).  counters: int64 0 nF, 1 n_kept, 2 pool entries,
 // 3 signal entries, 4 draws, 5 status, 6 al_used, 7 the text stage's status, 8 n_text_bytes, 9 n_decoder_bytes.
-constexpr int N_COUNTERS = 10;
+constexpr int N_COUNTERS = 10, TEXT_WORD = 7;
 
 struct c3b_fa : C3bRegionWorkspace {
     C3bBuf in_core[8], in_qoff, in_qual, in_noff, in_name, in_moff, in_mv;
@@ -927,23 +926,24 @@ struct c3b_fa : C3bRegionWorkspace {
     C3bBuf k_orig, k_start, k_end, k_pmax, k_fs, k_ov, k_pi, k_sig, k_hap, sig_len, sig_ex;
     C3bBuf pool, sig;
     C3bBuf ra, rb, nsel, draws, draw_off;
-    C3bBuf matrix, c_depth, c_acgt, al_off, al_n;
+    C3bBuf matrix, c_depth, c_acgt;
     int64_t n_cand = 0, depth = 0, C = 8, n_kept = 0;
     bool built = false;
     bool synced = false;                 // c3b_fa_sizes has waited for everything queued since the last build or text stage
-    // the text stage (c3b_fa_alt_text): where the build left its inputs, scratch, outputs
-    C3bReads R{};
-    const char *dref = nullptr;
-    int64_t ref_start = 0, ref_len = 0, n_cigar = 0, n_seq = 0;
-    C3bBuf tx_hash, tx_order, tx_table, tx_nins, tx_ndel, tx_len_text, tx_len_dec;
-    C3bBuf text, dec, text_off, dec_off, ref_base, position;
-    bool texted = false;
 };
+
+// The text stage's results need an issued c3b_fa_alt_text and, to read its counter words, the build's wait.  `who` names the
+// entry point in the error.
+static int fa_texted(c3b_fa *w, const char *who, bool wait) {
+    if (!w || !w->texted) { c3b_set_error("%s: no c3b_fa_alt_text has been issued", who); return 1; }
+    return wait && !w->synced && c3b_fa_sizes(w, nullptr, nullptr, nullptr);
+}
+static const char *const FA_TEXT_HINT = "build fewer candidates";
 
 extern "C" {
 
 int c3b_fa_create(c3b_fa **out, int device_ordinal) {
-    if (c3b_region_create(out, device_ordinal, 2, N_COUNTERS, "c3b_fa_create")) return 1;
+    if (c3b_region_create(out, device_ordinal, 2, N_COUNTERS, TEXT_WORD, "c3b_fa_create")) return 1;
     c3b_fa *w = *out;
     std::vector<uint32_t> J;
     glibc_jump_matrices(J);
@@ -1053,8 +1053,8 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
         grow(w->k_sig, Nz * 8) || grow(w->k_hap, Nz * 4) || grow(w->sig_len, Nz * 8) || grow(w->sig_ex, Nz * 8) ||
         grow(w->ra, Kz * 8) || grow(w->rb, Kz * 8) || grow(w->nsel, Kz * 8) || grow(w->draws, Kz * 8) ||
         grow(w->draw_off, Kz * 8) || grow(w->matrix, Kz * (size_t)depth * 33 * (size_t)w->C) || grow(w->c_depth, Kz * 4) ||
-        grow(w->c_acgt, Kz * 16) || grow(w->al_off, Kz * 4) || grow(w->al_n, Kz * 4) || grow(w->al_meta, (size_t)AL_CAP * 4) ||
-        grow(w->al_read, (size_t)AL_CAP * 4) || grow(w->al_qpos, (size_t)AL_CAP * 4) || grow(w->al_cnt, (size_t)AL_CAP * 4))
+        grow(w->c_acgt, Kz * 16) || grow(w->al_off, Kz * 4) || grow(w->al_n, Kz * 4) || grow(w->al_meta, (size_t)C3B_AL_CAP * 4) ||
+        grow(w->al_read, (size_t)C3B_AL_CAP * 4) || grow(w->al_qpos, (size_t)C3B_AL_CAP * 4) || grow(w->al_cnt, (size_t)C3B_AL_CAP * 4))
         return 1;
     int64_t *cnt = w->counters.as<int64_t>();
     C3B_CUDA(cudaMemsetAsync(cnt, 0, 64, s));
@@ -1153,7 +1153,7 @@ int c3b_fa_sizes(c3b_fa *w, int64_t *n_cand, int64_t *n_kept, int64_t *rand_draw
     C3B_CUDA(cudaStreamSynchronize(w->stream));
     const int status = (int)w->host_counters[5];
     if (status & 1) { c3b_set_error("c3b_fa_build: more than %d reads overlap one candidate window", MAXSEL); return 1; }
-    if (status & 2) { c3b_set_error("c3b_fa_build: more than %d distinct indel alleles to export; build fewer candidates per call", AL_CAP); return 1; }
+    if (status & 2) { c3b_set_error("c3b_fa_build: more than %d distinct indel alleles to export; build fewer candidates per call", C3B_AL_CAP); return 1; }
     if (status & 4) { c3b_set_error("c3b_fa_build: a read touches variants of more than %d phase sets", MAX_PS); return 1; }
     if (status & 8) {
         c3b_set_error("c3b_fa_build: more than %d insertions on one candidate are overwritten by a later insertion on the same anchor",
@@ -1177,7 +1177,7 @@ int c3b_fa_fetch(c3b_fa *w, int8_t *matrix, int32_t *kept_haplotype, int64_t *ke
 int c3b_fa_fetch_alleles(c3b_fa *w, int32_t *depth, int32_t *acgt, int32_t *al_off, int32_t *al_n, uint32_t *meta, uint32_t *read,
                          uint32_t *qpos, uint32_t *cnt, int64_t capacity, int64_t *n_alleles) {
     if (c3b_fa_sizes(w, nullptr, nullptr, nullptr)) return 1;
-    const int64_t used = w->host_counters[6], n = used < AL_CAP ? used : AL_CAP;
+    const int64_t used = w->host_counters[6], n = used < C3B_AL_CAP ? used : C3B_AL_CAP;
     if (n_alleles) *n_alleles = n;
     const size_t k = (size_t)w->n_cand;
     return w->get(depth, w->c_depth, k * 4) || w->get(acgt, w->c_acgt, k * 16) || w->get(al_off, w->al_off, k * 4) ||
@@ -1192,93 +1192,34 @@ int c3b_fa_device(c3b_fa *w, const int8_t **matrix) {
 
 int c3b_fa_alt_text(c3b_fa *w, int64_t max_indel_length) {
     if (!w || !w->built) { c3b_set_error("c3b_fa_alt_text: no c3b_fa_build has been issued"); return 1; }
-    C3B_CUDA(cudaSetDevice(w->device));
-    cudaStream_t s = w->stream;
-    const int64_t K = w->n_cand;
-    // every allele record comes from one insertion / deletion operation of one read
-    const int64_t cap = w->n_cigar < AL_CAP ? (w->n_cigar > 0 ? w->n_cigar : 1) : AL_CAP;
-    // bytes: head, SNP and R fields per candidate; key, count and separators per record; the inserted bases are query bases; a
-    // printed deletion shows at most max_indel_length reference bases
-    const int64_t del_len = max_indel_length < 0 ? 0 : (max_indel_length < w->ref_len ? max_indel_length : w->ref_len);
-    const int64_t del_bytes = cap * del_len < (1ll << 28) ? cap * del_len : (1ll << 28);
-    const int64_t text_cap = 160 * (K + 1) + 48 * cap + 2 * w->n_seq + del_bytes;
-    const size_t Kz = (size_t)K + 1;
-    w->texted = w->synced = false;        // the status word and the totals travel with the next c3b_fa_sizes
-    auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_fa"); };
-    if (grow(w->tx_hash, (size_t)cap * 4) || grow(w->tx_order, (size_t)cap * 4) || grow(w->tx_table, (8 * Kz + 3 * (size_t)cap) * 4) ||
-        grow(w->tx_nins, Kz * 4) || grow(w->tx_ndel, Kz * 4) || grow(w->tx_len_text, Kz * 4) || grow(w->tx_len_dec, Kz * 4) ||
-        grow(w->text, (size_t)text_cap) || grow(w->dec, (size_t)text_cap) || grow(w->text_off, Kz * 8) || grow(w->dec_off, Kz * 8) ||
-        grow(w->ref_base, Kz) || grow(w->position, Kz * 8))
-        return 1;
-    w->launches[1] = 0;
-    int64_t *cnt = w->counters.as<int64_t>();
-    // the stage's own status word and totals: an earlier stage's overflow is not this one's
-    C3B_CUDA(cudaMemsetAsync(cnt + 7, 0, 3 * 8, s));
-    C3B_CUDA(cudaEventRecord(w->ev[1][0], s));
-    if (K > 0) {
-        FaAltTextArgs A;
-        A.n_cand = K; A.ref_start = w->ref_start; A.ref_len = w->ref_len; A.max_indel_length = max_indel_length;
-        A.cand = w->in_cand.as<int64_t>(); A.ref = w->dref; A.R = w->R;
-        A.c_depth = w->c_depth.as<int32_t>(); A.c_acgt = w->c_acgt.as<int32_t>();
-        A.al_off = w->al_off.as<int32_t>(); A.al_n = w->al_n.as<int32_t>();
-        A.al_meta = w->al_meta.as<uint32_t>(); A.al_read = w->al_read.as<uint32_t>(); A.al_qpos = w->al_qpos.as<uint32_t>();
-        A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_cap = cap;
-        A.hash = w->tx_hash.as<uint32_t>(); A.order = w->tx_order.as<int32_t>(); A.table = w->tx_table.as<uint32_t>();
-        A.n_ins = w->tx_nins.as<int32_t>(); A.n_del = w->tx_ndel.as<int32_t>();
-        A.len_text = w->tx_len_text.as<int32_t>(); A.len_dec = w->tx_len_dec.as<int32_t>();
-        A.status = reinterpret_cast<int *>(cnt + 7);
-        A.text = w->text.as<char>(); A.dec = w->dec.as<char>(); A.text_cap = A.dec_cap = text_cap;
-        A.text_off = w->text_off.as<int64_t>(); A.dec_off = w->dec_off.as<int64_t>(); A.totals = cnt + 8;
-        A.ref_base = w->ref_base.as<uint8_t>(); A.position = w->position.as<int64_t>();
-        if (c3b_launch_fa_alt_text(A, s, &w->launches[1])) return 1;
-    } else {
-        C3B_CUDA(cudaMemsetAsync(w->text_off.p, 0, 8, s));
-        C3B_CUDA(cudaMemsetAsync(w->dec_off.p, 0, 8, s));
-    }
-    C3B_CUDA(cudaEventRecord(w->ev[1][1], s));
-    C3B_CUDA(cudaMemcpyAsync(w->host_counters, w->counters.p, N_COUNTERS * 8, cudaMemcpyDeviceToHost, s));
-    w->texted = true;
-    return 0;
+    w->synced = false;                    // the status word and the totals travel with the next c3b_fa_sizes
+    FaAltTextArgs A;
+    if (w->text_prepare(w->n_cand, max_indel_length, "c3b_fa", A)) return 1;
+    A.cand = w->in_cand.as<int64_t>(); A.c_depth = w->c_depth.as<int32_t>(); A.c_acgt = w->c_acgt.as<int32_t>();
+    return w->text_enqueue(A, c3b_launch_fa_alt_text);
 }
 
 int c3b_fa_alt_text_sizes(c3b_fa *w, int64_t *n_text_bytes, int64_t *n_decoder_bytes) {
-    if (!w || !w->texted) { c3b_set_error("c3b_fa_alt_text_sizes: no c3b_fa_alt_text has been issued"); return 1; }
-    if (!w->synced && c3b_fa_sizes(w, nullptr, nullptr, nullptr)) return 1;
-    if ((int)w->host_counters[7] != 0) {
-        c3b_set_error("c3b_fa_alt_text: the all_alt_info text outgrew its buffers; build fewer candidates or lower max_indel_length");
-        return 1;
-    }
-    if (n_text_bytes) *n_text_bytes = w->host_counters[8];
-    if (n_decoder_bytes) *n_decoder_bytes = w->host_counters[9];
-    return 0;
+    const char *who = "c3b_fa_alt_text_sizes";
+    return fa_texted(w, who, true) || w->text_sizes(who, FA_TEXT_HINT, n_text_bytes, n_decoder_bytes);
 }
 
 int c3b_fa_fetch_alt_text(c3b_fa *w, char *text, int64_t *text_off, char *decoder, int64_t *decoder_off, uint8_t *ref_base,
                           int64_t *position) {
-    int64_t nt = 0, nd = 0;
-    if (!w || !w->texted) { c3b_set_error("c3b_fa_fetch_alt_text: no c3b_fa_alt_text has been issued"); return 1; }
-    if (c3b_fa_alt_text_sizes(w, &nt, &nd)) return 1;
-    const size_t nk = (size_t)w->n_cand;
-    return w->get(text, w->text, (size_t)nt) || w->get(text_off, w->text_off, (nk + 1) * 8) || w->get(decoder, w->dec, (size_t)nd) ||
-           w->get(decoder_off, w->dec_off, (nk + 1) * 8) || w->get(ref_base, w->ref_base, nk) ||
-           w->get(position, w->position, nk * 8) || w->wait();
+    const char *who = "c3b_fa_fetch_alt_text";
+    return fa_texted(w, who, true) ||
+           w->text_fetch(who, FA_TEXT_HINT, w->n_cand, text, text_off, decoder, decoder_off, ref_base, position);
 }
 
 int c3b_fa_alt_text_device(c3b_fa *w, const char **text, const int64_t **text_off, const char **decoder,
                            const int64_t **decoder_off, const uint8_t **ref_base, const int64_t **position) {
-    if (!w || !w->texted) { c3b_set_error("c3b_fa_alt_text_device: no c3b_fa_alt_text has been issued"); return 1; }
-    if (text) *text = w->text.as<char>();
-    if (text_off) *text_off = w->text_off.as<int64_t>();
-    if (decoder) *decoder = w->dec.as<char>();
-    if (decoder_off) *decoder_off = w->dec_off.as<int64_t>();
-    if (ref_base) *ref_base = w->ref_base.as<uint8_t>();
-    if (position) *position = w->position.as<int64_t>();
+    if (fa_texted(w, "c3b_fa_alt_text_device", false)) return 1;
+    w->text_device(text, text_off, decoder, decoder_off, ref_base, position);
     return 0;
 }
 
 int c3b_fa_alt_text_last_ms(c3b_fa *w, float *ms, int *launches) {
-    if (!w || !w->texted) { c3b_set_error("c3b_fa_alt_text_last_ms: no c3b_fa_alt_text has been issued"); return 1; }
-    return w->elapsed(1, ms, launches);
+    return fa_texted(w, "c3b_fa_alt_text_last_ms", false) || w->elapsed(1, ms, launches);
 }
 
 int c3b_fa_last_ms(c3b_fa *w, float *ms, int *launches) {

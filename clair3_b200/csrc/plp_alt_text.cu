@@ -3,7 +3,8 @@
 // Reference: the text loop of calculate_clair3_pileup(), HKU-BAL/Clair3 src/clair3_pileup.c:391-450, one string per candidate:
 //     "<pos+1>-<depth>-<REF>-X<b> n D<ref bases> n I<REF><inserted bases> n R<REF> n "
 // clair3_b200/pileup_counts.py: format_alt_info / khash_iteration_order state the same on the host and are what the tests hold
-// these kernels to.  Candidates are independent and their strings have data-dependent length, so the stage is
+// these kernels to.  The stage is alt_text.cuh's measure -> scan -> write (T2 the scans, T3 text_write_kernel); what is the
+// pileup counter's own is
 //
 //   T1 plp_text_measure   one WARP per candidate over the column's allele records (K3's export, [al_off, al_off + al_n)):
 //                         lanes over records merge the two strands (a record's twin on the other strand: same kind, length and,
@@ -11,33 +12,19 @@
 //                         insertion strings (X31) and rank-sort the deletions by length and the insertions by first read; lane 0
 //                         then replays klib's khash (src/khash.h) over the insertions - power-of-two tables from 4, triangular
 //                         probing, growth at 0.77 load at the start of a put, kh_resize's in-place kick-out rehash, one more
-//                         growth when a put of a present string follows the last new one - and leaves the bucket order; it then
-//                         walks the string once with a counting sink: the bytes of the full text and of the decoder form.
-//   T2 (block_scan)       the two exclusive scans over n_cand + 1 lengths: per-candidate offsets and the totals.
-//   T3 plp_text_write     one THREAD per candidate walks the same string with a writing sink.
+//                         growth when a put of a present string follows the last new one - and leaves the bucket order.
+//   PlpText::emit         the string, from the merged and ordered records.
 //
 // Everything a column needs lives in global scratch addressed by its own record range (mate / hash / order) or by that range and
 // its candidate index (the khash table: 8 buckets per candidate, or up to 3 per record - a table of n > 8 buckets holds at least
 // 0.77 n / 2 strings), so a column of thousands of distinct alleles needs no capacity of its own.  The grids are sized from the
-// region's width and read n_cand on the device.  Same records, same bytes, whatever the launch shape: nothing here is atomic but
-// the status word.
-#include <limits.h>
-
+// region's width and read n_cand on the device.
 #include "alt_text.cuh"
-#include "block_scan.cuh"
-#include "c3b_internal.h"
 
 namespace {
 
 constexpr int FETCH_EXPAND = 1000;                        // mpileup_expand_reference_region, src/clair3_pileup.h:63
 constexpr int32_t NOT_FIRST = -2;                         // mate[]: the record's twin comes earlier in the list
-
-// upper_base of the reference base under a column, 'N' outside the supplied reference
-__device__ __forceinline__ int ref_base_at(const PlpAltTextArgs &A, int64_t pos) {
-    const int64_t off = pos - A.ref_start;
-    const int rb = (off >= 0 && off < A.ref_len) ? (int)(unsigned char)A.ref[off] : 'N';
-    return rb >= 'a' && rb <= 'z' ? rb - 32 : rb;
-}
 
 __device__ __forceinline__ int64_t first_read(const PlpAltTextArgs &A, int i) {
     const int m = A.mate[i];
@@ -49,11 +36,27 @@ __device__ __forceinline__ long long merged_count(const PlpAltTextArgs &A, int i
     return (long long)A.al_cnt[i] + (m >= 0 ? (long long)A.al_cnt[m] : 0);
 }
 
-// One candidate's string, src/clair3_pileup.c:391-450, from the merged and ordered allele records T1 left in `order`.
-template <class S> __device__ void plp_text_emit(const PlpAltTextArgs &A, const int64_t j, TextOut<S> &o) {
+// The stage for alt_text.cuh: the candidate count is the count's device counter.
+struct PlpText {
+    typedef PlpAltTextArgs Args;
+    static __device__ __forceinline__ int64_t n_cand(const Args &A) { return *A.n_cand; }
+    static const int64_t *n_cand_dev(const Args &A) { return A.n_cand; }
+    static __device__ __forceinline__ int64_t pos(const Args &A, int64_t j) { return A.major[A.cand_cols[j]]; }
+    // upper_base of the reference base under a column, 'N' outside the supplied reference
+    static __device__ __forceinline__ int ref_base(const Args &A, int64_t pos) {
+        const int64_t off = pos - A.ref_start;
+        const int rb = (off >= 0 && off < A.ref_len) ? (int)(unsigned char)A.ref[off] : 'N';
+        return rb >= 'a' && rb <= 'z' ? rb - 32 : rb;
+    }
+    template <class S> static __device__ void emit(const Args &A, int64_t j, int ni, int nd, TextOut<S> &o);
+};
+
+// One candidate's string, src/clair3_pileup.c:391-450, from the merged and ordered allele records T1 left in `order`: ni
+// insertions in bucket order, then nd deletions by length.
+template <class S> __device__ void PlpText::emit(const Args &A, const int64_t j, const int ni, const int nd, TextOut<S> &o) {
     const int64_t ci = A.cand_cols[j], pos = A.major[ci], off = pos - A.ref_start;
-    const int a0 = A.al_off[pos - A.start], ni = A.n_ins[j], nd = A.n_del[j];
-    const int rb = ref_base_at(A, pos);
+    const int a0 = A.al_off[pos - A.start];
+    const int rb = ref_base(A, pos);
     const int bi = rb - 'A';
     const int rf = bi == 2 ? 1 : bi == 6 ? 2 : bi == 19 ? 3 : 0;          // base2index, src/clair3_pileup.h:57-62
     const long long depth = A.stats[ci * 6];
@@ -185,52 +188,18 @@ __global__ void __launch_bounds__(256) plp_text_measure_kernel(PlpAltTextArgs A)
             if (ni > 0 && fits) {                             // the khash replay: a short serial walk
                 uint32_t *slot = A.table + 8 * j;
                 int avail = 8;
-                if (ni > 3) { slot = A.table + 8 * A.W + 3 * (int64_t)a0; avail = 3 * n; }
+                if (ni > 3) { slot = A.table + 8 * A.n + 3 * (int64_t)a0; avail = 3 * n; }
                 // a read after the last new string put a present one again: that put still grows a full table first
                 const bool again = (int64_t)A.ins_last[pos - A.start] > first_read(A, A.order[a0 + ni - 1]);
                 fits = khash_replay(A.hash, A.order + a0, ni, again, slot, avail);
             }
-            if (!fits) { atomicOr(A.status, 1); ni = nd = 0; }
-            A.n_ins[j] = ni;
-            A.n_del[j] = nd;
-            TextOut<CountSink> o;
-            plp_text_emit(A, j, o);
-            if (!o.cut && o.n_alt > 0) --o.dec.n;             // rstrip(): the alt text ends in one space
-            if (!fits || o.full.n > INT_MAX || o.dec.n > INT_MAX) {
-                atomicOr(A.status, 1);
-                o.full.n = o.dec.n = 0;
-            }
-            A.len_text[j] = (int32_t)o.full.n;
-            A.len_dec[j] = (int32_t)o.dec.n;
-            A.ref_base[j] = (uint8_t)ref_base_at(A, pos);
-            A.position[j] = pos + 1;
+            text_measure_tail<PlpText>(A, j, fits, ni, nd);
         }
     }
-}
-
-// ---------------------------------------------------------------------------------------------------------------- T3
-__global__ void __launch_bounds__(128) plp_text_write_kernel(PlpAltTextArgs A) {
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= *A.n_cand) return;
-    const int64_t t0 = A.text_off[j], t1 = A.text_off[j + 1], d0 = A.dec_off[j], d1 = A.dec_off[j + 1];
-    if (t1 > A.text_cap || d1 > A.dec_cap) { atomicOr(A.status, 1); return; }
-    TextOut<WriteSink> o;
-    o.full.p = A.text + t0; o.full.lim = t1 - t0;
-    o.dec.p = A.dec + d0; o.dec.lim = d1 - d0;
-    if (t1 > t0) plp_text_emit(A, j, o);
 }
 
 }  // namespace
 
 int c3b_launch_plp_alt_text(const PlpAltTextArgs &a, cudaStream_t s, int *launches) {
-    if (a.al_cap >= (int64_t)KH_VAL) { c3b_set_error("c3b_plp_alt_text: %lld allele records exceed the khash replay's 24-bit record index", (long long)a.al_cap); return 1; }
-    int64_t blocks = ((a.W + 1) * 32 + 255) / 256;
-    if (blocks > 132 * 8) blocks = 132 * 8;
-    plp_text_measure_kernel<<<(unsigned)blocks, 256, 0, s>>>(a);
-    block_scan_sum(a.len_text, a.text_off, a.W + 1, a.n_cand, a.totals, s);
-    block_scan_sum(a.len_dec, a.dec_off, a.W + 1, a.n_cand, a.totals + 1, s);
-    plp_text_write_kernel<<<(unsigned)((a.W + 127) / 128), 128, 0, s>>>(a);
-    C3B_CUDA(cudaGetLastError());
-    *launches = 4;
-    return 0;
+    return text_launch<PlpText>(a, plp_text_measure_kernel, s, launches, "c3b_plp_alt_text");
 }

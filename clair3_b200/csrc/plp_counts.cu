@@ -43,7 +43,6 @@ constexpr int NCNT = 19;          // 18 features + the index -1 counter
 constexpr int NP = 704;           // shared-memory indel nodes per tile (20 B each): 33.5 KB per CTA with the counters -> 6 CTAs per SM
 constexpr int FLANK = 16;         // pileup_flanking_base_num, src/clair3_pileup.h:93
 constexpr int G_POOL = 1 << 21;   // global overflow nodes per workspace
-constexpr int AL_CAP = 1 << 22;   // exported allele records per call (16 B each)
 
 __device__ __forceinline__ bool ref_cons(uint32_t op) { return (0x18Du >> op) & 1u; }   // M D N = X
 __device__ __forceinline__ bool qry_cons(uint32_t op) { return (0x193u >> op) & 1u; }   // M I S = X
@@ -526,33 +525,37 @@ __global__ void __launch_bounds__(TILE) plp_cands_kernel(CandArgs A) {
 }  // namespace
 
 // Timed stages: 0 the count (c3b_plp_count), 1 the text (c3b_plp_alt_text).  counters: int64 n_cols, int64 n_cand, int g_used,
-// int status, int al_used, int text_status, int64 n_text_bytes, int64 n_decoder_bytes.  al_*: the allele export (params.alt_info).
+// int status, int al_used, then the text stage's int64 status, n_text_bytes, n_decoder_bytes.  al_*: the allele export
+// (params.alt_info).
+constexpr int N_COUNTERS = 7, TEXT_WORD = 4;
+
 struct c3b_plp : C3bRegionWorkspace {
     // inputs (copies of host records)
     C3bBuf in_core[8], in_ref;
     // scratch
     C3bBuf opx, opy, rend, pmax, rows32, dstats, nquirk, dci, tile_cov, tile_off, tile_cand, tile_coff;
     C3bBuf g_meta, g_read, g_qpos, g_cnt, g_next;
-    C3bBuf al_off, al_n, ins_last;
+    C3bBuf ins_last, tx_mate;
     // outputs
     C3bBuf matrix, major, stats, cand_cols, wstart, wbounds, cand_ok, gv_ref, gv_tot;
-    int64_t W = 0;
+    int64_t W = 0, start = 0, end = 0;
     bool gvcf = false, counted = false, alleles = false;
     int64_t n_cols = -1, n_cand = -1;
-    // the text stage (c3b_plp_alt_text): where the count left its inputs, scratch, outputs
-    C3bReads R;
-    const char *dref = nullptr;
-    int64_t start = 0, end = 0, ref_start = 0, ref_len = 0, n_cigar = 0, n_seq = 0;
-    C3bBuf tx_mate, tx_hash, tx_order, tx_table, tx_nins, tx_ndel, tx_len_text, tx_len_dec;
-    C3bBuf text, dec, text_off, dec_off, ref_base, position;
-    bool texted = false;
 };
 
-constexpr int N_COUNTERS = 6;
+// The text stage's results need an issued c3b_plp_alt_text and, to read its counter words, the count's wait.  `who` names the
+// entry point in the error.
+static int plp_texted(c3b_plp *w, const char *who, bool wait) {
+    if (!w || !w->texted) { c3b_set_error("%s: no c3b_plp_alt_text has been issued", who); return 1; }
+    return wait && w->n_cols < 0 && c3b_plp_sizes(w, nullptr, nullptr);
+}
+static const char *const PLP_TEXT_HINT = "count a smaller region";
 
 extern "C" {
 
-int c3b_plp_create(c3b_plp **out, int device_ordinal) { return c3b_region_create(out, device_ordinal, 2, N_COUNTERS, "c3b_plp_create"); }
+int c3b_plp_create(c3b_plp **out, int device_ordinal) {
+    return c3b_region_create(out, device_ordinal, 2, N_COUNTERS, TEXT_WORD, "c3b_plp_create");
+}
 
 int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64_t start, int64_t end, const char *ref_seq,
                   int64_t ref_start, int64_t ref_len, const c3b_plp_params *params, void *cuda_stream) {
@@ -607,8 +610,9 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         return 1;
     if (w->gvcf && (grow(w->gv_ref, Wz * 8) || grow(w->gv_tot, Wz * 8))) return 1;
     w->alleles = params->alt_info != 0;
-    if (w->alleles && (grow(w->al_meta, (size_t)AL_CAP * 4) || grow(w->al_read, (size_t)AL_CAP * 4) || grow(w->al_qpos, (size_t)AL_CAP * 4) ||
-                       grow(w->al_cnt, (size_t)AL_CAP * 4) || grow(w->al_off, Wz * 4) || grow(w->al_n, Wz * 4) ||
+    if (w->alleles && (grow(w->al_meta, (size_t)C3B_AL_CAP * 4) || grow(w->al_read, (size_t)C3B_AL_CAP * 4) ||
+                       grow(w->al_qpos, (size_t)C3B_AL_CAP * 4) || grow(w->al_cnt, (size_t)C3B_AL_CAP * 4) ||
+                       grow(w->al_off, Wz * 4) || grow(w->al_n, Wz * 4) ||
                        grow(w->ins_last, Wz * 4)))
         return 1;
     C3B_CUDA(cudaMemsetAsync(w->counters.p, 0, N_COUNTERS * 8, s));
@@ -644,7 +648,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         A.g_cnt = w->g_cnt.as<uint32_t>(); A.g_next = w->g_next.as<int32_t>(); A.g_used = g_used; A.status = status;
         A.al_meta = w->alleles ? w->al_meta.as<uint32_t>() : nullptr; A.al_read = w->al_read.as<uint32_t>(); A.al_qpos = w->al_qpos.as<uint32_t>();
         A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_off = w->al_off.as<int32_t>(); A.al_n = w->al_n.as<int32_t>();
-        A.ins_last = w->ins_last.as<int32_t>(); A.al_used = al_used; A.al_cap = AL_CAP;
+        A.ins_last = w->ins_last.as<int32_t>(); A.al_used = al_used; A.al_cap = C3B_AL_CAP;
         const size_t smem = (size_t)NCNT * TILE * 4 + (size_t)NP * 20;
         plp_count_tile_kernel<<<tiles, TILE, smem, s>>>(A);
         block_scan_sum(w->tile_cov.as<int32_t>(), w->tile_off.as<int64_t>(), tiles, nullptr, n_cols_dev, s);
@@ -681,7 +685,7 @@ int c3b_plp_sizes(c3b_plp *w, int64_t *n_cols, int64_t *n_candidates) {
     if (status & 1) { c3b_set_error("c3b_plp_count: more than %d distinct indel alleles spilled from the tiles' shared-memory pools", G_POOL); return 1; }
     if (status & 2) { c3b_set_error("c3b_plp_count: a read spans more than 2^31 reference or query bases"); return 1; }
     if (status & 4) { c3b_set_error("c3b_plp_count: an indel of 2^30 bases or more"); return 1; }
-    if (status & 8) { c3b_set_error("c3b_plp_count: more than %d allele records to export (params.alt_info); count a smaller region", AL_CAP); return 1; }
+    if (status & 8) { c3b_set_error("c3b_plp_count: more than %d allele records to export (params.alt_info); count a smaller region", C3B_AL_CAP); return 1; }
     w->n_cols = w->host_counters[0];
     w->n_cand = w->host_counters[1];
     if (n_cols) *n_cols = w->n_cols;
@@ -739,97 +743,38 @@ int c3b_plp_window_bounds(c3b_plp *w, int64_t *bounds, const int64_t **device_bo
 int c3b_plp_alt_text(c3b_plp *w, int64_t max_indel_length) {
     if (!w || !w->counted) { c3b_set_error("c3b_plp_alt_text: no c3b_plp_count has been issued"); return 1; }
     if (!w->alleles) { c3b_set_error("c3b_plp_alt_text: the count ran without params.alt_info"); return 1; }
-    C3B_CUDA(cudaSetDevice(w->device));
-    cudaStream_t s = w->stream;
-    const int64_t W = w->W;
-    // every allele record comes from one insertion / deletion operation of one read
-    const int64_t cap = w->n_cigar < AL_CAP ? (w->n_cigar > 0 ? w->n_cigar : 1) : AL_CAP;
-    // bytes: head, SNP and R fields per candidate; key, count and separators per record; the inserted bases are query bases; a
-    // printed deletion shows at most max_indel_length reference bases
-    const int64_t del_len = max_indel_length < 0 ? 0 : (max_indel_length < w->ref_len ? max_indel_length : w->ref_len);
-    const int64_t del_bytes = cap * del_len < (1ll << 28) ? cap * del_len : (1ll << 28);
-    const int64_t text_cap = 160 * (W + 1) + 48 * cap + 2 * w->n_seq + del_bytes;
-    const size_t Wz = (size_t)W + 1;
-    auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_plp"); };
-    if (grow(w->tx_mate, (size_t)cap * 4) || grow(w->tx_hash, (size_t)cap * 4) || grow(w->tx_order, (size_t)cap * 4) ||
-        grow(w->tx_table, (8 * Wz + 3 * (size_t)cap) * 4) || grow(w->tx_nins, Wz * 4) || grow(w->tx_ndel, Wz * 4) ||
-        grow(w->tx_len_text, Wz * 4) || grow(w->tx_len_dec, Wz * 4) || grow(w->text, (size_t)text_cap) ||
-        grow(w->dec, (size_t)text_cap) || grow(w->text_off, Wz * 8) || grow(w->dec_off, Wz * 8) || grow(w->ref_base, Wz) ||
-        grow(w->position, Wz * 8))
+    PlpAltTextArgs A;
+    if (w->text_prepare(w->W, max_indel_length, "c3b_plp", A) || w->tx_mate.ensure((size_t)A.al_cap * 4, w->stream, "c3b_plp"))
         return 1;
-    w->texted = false;
     w->n_cols = w->n_cand = -1;           // the status word and the totals travel with the next c3b_plp_sizes
-    w->launches[1] = 0;
-    int64_t *cnt = w->counters.as<int64_t>();
-    int *text_status = reinterpret_cast<int *>(cnt + 3) + 1;       // the stage's own word: an earlier stage's overflow is not this one's
-    C3B_CUDA(cudaMemsetAsync(text_status, 0, sizeof(int), s));
-    C3B_CUDA(cudaEventRecord(w->ev[1][0], s));
-    if (W > 0) {
-        PlpAltTextArgs A;
-        A.start = w->start; A.end = w->end; A.ref_start = w->ref_start; A.ref_len = w->ref_len; A.max_indel_length = max_indel_length;
-        A.W = W;
-        A.n_cand = cnt + 1;
-        A.cand_cols = w->cand_cols.as<int64_t>(); A.major = w->major.as<int64_t>(); A.matrix = w->matrix.as<int64_t>();
-        A.stats = w->stats.as<int32_t>(); A.ref = w->dref;
-        A.R = w->R;
-        A.al_off = w->al_off.as<int32_t>(); A.al_n = w->al_n.as<int32_t>(); A.ins_last = w->ins_last.as<int32_t>();
-        A.al_meta = w->al_meta.as<uint32_t>(); A.al_read = w->al_read.as<uint32_t>(); A.al_qpos = w->al_qpos.as<uint32_t>();
-        A.al_cnt = w->al_cnt.as<uint32_t>(); A.al_cap = cap;
-        A.mate = w->tx_mate.as<int32_t>(); A.order = w->tx_order.as<int32_t>(); A.hash = w->tx_hash.as<uint32_t>();
-        A.table = w->tx_table.as<uint32_t>(); A.n_ins = w->tx_nins.as<int32_t>(); A.n_del = w->tx_ndel.as<int32_t>();
-        A.len_text = w->tx_len_text.as<int32_t>(); A.len_dec = w->tx_len_dec.as<int32_t>();
-        A.status = text_status;
-        A.text = w->text.as<char>(); A.dec = w->dec.as<char>(); A.text_cap = A.dec_cap = text_cap;
-        A.text_off = w->text_off.as<int64_t>(); A.dec_off = w->dec_off.as<int64_t>(); A.totals = cnt + 4;
-        A.ref_base = w->ref_base.as<uint8_t>(); A.position = w->position.as<int64_t>();
-        if (c3b_launch_plp_alt_text(A, s, &w->launches[1])) return 1;
-    } else {
-        C3B_CUDA(cudaMemsetAsync(w->text_off.p, 0, 8, s));
-        C3B_CUDA(cudaMemsetAsync(w->dec_off.p, 0, 8, s));
-    }
-    C3B_CUDA(cudaEventRecord(w->ev[1][1], s));
-    C3B_CUDA(cudaMemcpyAsync(w->host_counters, w->counters.p, N_COUNTERS * 8, cudaMemcpyDeviceToHost, s));
-    w->texted = true;
-    return 0;
+    A.start = w->start; A.end = w->end;
+    A.n_cand = w->counters.as<int64_t>() + 1;
+    A.cand_cols = w->cand_cols.as<int64_t>(); A.major = w->major.as<int64_t>(); A.matrix = w->matrix.as<int64_t>();
+    A.stats = w->stats.as<int32_t>(); A.ins_last = w->ins_last.as<int32_t>(); A.mate = w->tx_mate.as<int32_t>();
+    return w->text_enqueue(A, c3b_launch_plp_alt_text);
 }
 
 int c3b_plp_alt_text_sizes(c3b_plp *w, int64_t *n_text_bytes, int64_t *n_decoder_bytes) {
-    if (!w || !w->texted) { c3b_set_error("c3b_plp_alt_text_sizes: no c3b_plp_alt_text has been issued"); return 1; }
-    if (w->n_cols < 0 && c3b_plp_sizes(w, nullptr, nullptr)) return 1;
-    if ((int)(w->host_counters[3] >> 32) != 0) {
-        c3b_set_error("c3b_plp_alt_text: the all_alt_info text outgrew its buffers; count a smaller region or lower max_indel_length");
-        return 1;
-    }
-    if (n_text_bytes) *n_text_bytes = w->host_counters[4];
-    if (n_decoder_bytes) *n_decoder_bytes = w->host_counters[5];
-    return 0;
+    const char *who = "c3b_plp_alt_text_sizes";
+    return plp_texted(w, who, true) || w->text_sizes(who, PLP_TEXT_HINT, n_text_bytes, n_decoder_bytes);
 }
 
 int c3b_plp_fetch_alt_text(c3b_plp *w, char *text, int64_t *text_off, char *decoder, int64_t *decoder_off, uint8_t *ref_base,
                            int64_t *position) {
-    int64_t nt = 0, nd = 0;
-    if (c3b_plp_alt_text_sizes(w, &nt, &nd)) return 1;
-    const size_t nk = (size_t)w->n_cand;
-    return w->get(text, w->text, (size_t)nt) || w->get(text_off, w->text_off, (nk + 1) * 8) || w->get(decoder, w->dec, (size_t)nd) ||
-           w->get(decoder_off, w->dec_off, (nk + 1) * 8) || w->get(ref_base, w->ref_base, nk) ||
-           w->get(position, w->position, nk * 8) || w->wait();
+    const char *who = "c3b_plp_fetch_alt_text";
+    return plp_texted(w, who, true) ||
+           w->text_fetch(who, PLP_TEXT_HINT, w->n_cand, text, text_off, decoder, decoder_off, ref_base, position);
 }
 
 int c3b_plp_alt_text_device(c3b_plp *w, const char **text, const int64_t **text_off, const char **decoder,
                             const int64_t **decoder_off, const uint8_t **ref_base, const int64_t **position) {
-    if (!w || !w->texted) { c3b_set_error("c3b_plp_alt_text_device: no c3b_plp_alt_text has been issued"); return 1; }
-    if (text) *text = w->text.as<char>();
-    if (text_off) *text_off = w->text_off.as<int64_t>();
-    if (decoder) *decoder = w->dec.as<char>();
-    if (decoder_off) *decoder_off = w->dec_off.as<int64_t>();
-    if (ref_base) *ref_base = w->ref_base.as<uint8_t>();
-    if (position) *position = w->position.as<int64_t>();
+    if (plp_texted(w, "c3b_plp_alt_text_device", false)) return 1;
+    w->text_device(text, text_off, decoder, decoder_off, ref_base, position);
     return 0;
 }
 
 int c3b_plp_alt_text_last_ms(c3b_plp *w, float *ms, int *launches) {
-    if (!w || !w->texted) { c3b_set_error("c3b_plp_alt_text_last_ms: no c3b_plp_alt_text has been issued"); return 1; }
-    return w->elapsed(1, ms, launches);
+    return plp_texted(w, "c3b_plp_alt_text_last_ms", false) || w->elapsed(1, ms, launches);
 }
 
 int c3b_plp_last_ms(c3b_plp *w, float *ms, int *launches) {

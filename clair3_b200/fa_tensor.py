@@ -15,8 +15,7 @@ import numpy as np
 import torch
 
 from ._ffi import CONSTANTS, C3BError, check, ffi, lib
-from .pileup_counts import (BamRecords, DeviceBamRecords, _device_view, _insertion_bytes, _records_struct, _Workspace,
-                            khash_iteration_order)
+from .pileup_counts import BamRecords, DeviceBamRecords, _insertion_bytes, _records_struct, _Workspace, khash_iteration_order
 
 FLANKING = 16                   # shared/param_f.py flankingBaseNum
 NO_OF_POSITIONS = 33
@@ -43,6 +42,7 @@ class FullAlignmentBuilder(_Workspace):
     device (apart from two short waits that size its scratch); ``fetch()`` / ``alt_info_strings()`` wait for it."""
 
     _API = "c3b_fa"
+    _OWNER = "builder"
 
     def __init__(self, device=0):
         super().__init__(device)
@@ -129,61 +129,16 @@ class FullAlignmentBuilder(_Workspace):
                                        meta[sl], rd[sl], qp[sl], cn[sl], rec))
         return out
 
-    def alt_text(self, max_indel_length=None):
-        """Enqueues the text stage (``c3b_fa_alt_text``) behind the last ``build``, on its stream and without a host wait: the
-        ``all_alt_info`` string of every candidate and what the decoder takes of it, formatted on the device.
-        ``max_indel_length``: as ``calculate_clair3_full_alignment``'s (default: what ``build`` was given).  Device-resident
-        records must stay alive until the text has been fetched."""
+    def _lib(self):
+        return lib()
+
+    def _text_max_indel(self):
         if self._alt is None:
             raise C3BError("alt_text: build() first")
-        if max_indel_length is None:
-            max_indel_length = self._alt[2]
-        if isinstance(max_indel_length, bool) or not isinstance(max_indel_length, (int, np.integer)):
-            raise C3BError("alt_text: max_indel_length must be an integer, got %r" % (max_indel_length,))
-        check(lib().c3b_fa_alt_text(self._h, int(max_indel_length)))
-        return self
+        return self._alt[2]
 
-    def alt_text_sizes(self):
-        """(bytes of all text strings, bytes of all decoder strings) of the last ``alt_text``."""
-        a, b = ffi.new("int64_t *"), ffi.new("int64_t *")
-        check(lib().c3b_fa_alt_text_sizes(self._h, a, b))
-        return int(a[0]), int(b[0])
-
-    def alt_text_fetch(self):
-        """dict: ``text`` (the ``all_alt_info`` strings, one per candidate), ``decoder`` (the ``"depth-alt"`` strings of
-        ``create_tensor_full_alignment``), ``ref_base`` uint8 [n_cand], ``position`` int64 [n_cand] (1-based).  Waits for the
-        text stage."""
-        nk = self._shape[0]
-        nt, nd = self.alt_text_sizes()
-        text, dec = np.zeros(max(nt, 1), np.uint8), np.zeros(max(nd, 1), np.uint8)
-        toff, doff = np.zeros(nk + 1, np.int64), np.zeros(nk + 1, np.int64)
-        rb, pos = np.zeros(nk, np.uint8), np.zeros(nk, np.int64)
-        c = ffi.cast
-        check(lib().c3b_fa_fetch_alt_text(self._h, c("char *", text.ctypes.data), c("int64_t *", toff.ctypes.data),
-                                          c("char *", dec.ctypes.data), c("int64_t *", doff.ctypes.data),
-                                          c("uint8_t *", rb.ctypes.data), c("int64_t *", pos.ctypes.data)))
-        tb, db = text.tobytes(), dec.tobytes()
-        return {"text": [tb[toff[j]:toff[j + 1]].decode("latin-1") for j in range(nk)],
-                "decoder": [db[doff[j]:doff[j + 1]].decode("latin-1") for j in range(nk)], "ref_base": rb, "position": pos}
-
-    def alt_text_device(self):
-        """The text stage's results as tensors that alias the workspace (valid until the next ``build`` / ``alt_text``):
-        ``text`` uint8 [n_text_bytes], ``text_off`` int64 [n_cand + 1], ``decoder`` uint8 [n_decoder_bytes], ``decoder_off``
-        int64 [n_cand + 1], ``ref_base`` uint8 [n_cand], ``position`` int64 [n_cand]; ``decoder`` / ``decoder_off`` /
-        ``ref_base`` are ``decode_calls``' ``alt_bytes`` / ``alt_offsets`` / ``ref_base``.  Waits (``c3b_fa_sizes``) only when
-        nothing has waited since the last ``build`` / ``alt_text``; after that wait it touches the stream no more."""
-        nk = self._shape[0]
-        nt, nd = self.alt_text_sizes()
-        p = [ffi.new("const char **"), ffi.new("const int64_t **"), ffi.new("const char **"), ffi.new("const int64_t **"),
-             ffi.new("const uint8_t **"), ffi.new("const int64_t **")]
-        check(lib().c3b_fa_alt_text_device(self._h, *p))
-        shapes = (("text", nt, torch.uint8), ("text_off", nk + 1, torch.int64), ("decoder", nd, torch.uint8),
-                  ("decoder_off", nk + 1, torch.int64), ("ref_base", nk, torch.uint8), ("position", nk, torch.int64))
-        return {name: _device_view(int(ffi.cast("uintptr_t", q[0])), n, dt, self._device) for (name, n, dt), q in zip(shapes, p)}
-
-    def alt_text_last_ms(self):
-        """Device time and kernel launches of the last ``alt_text`` (``last_ms`` reports the build alone)."""
-        return self._timing(lib().c3b_fa_alt_text_last_ms)
+    def _n_cand(self):
+        return self._shape[0]
 
     def forward(self, model):
         """Clair3_F over every candidate of the last build, straight from the device-resident matrix (``c3b_forward`` with
@@ -194,42 +149,13 @@ class FullAlignmentBuilder(_Workspace):
         self._forward_into(model, y)
         return model._split(y)
 
-    def call(self, model, output_config, ctg_name, k=16):
-        """The candidates of the last ``build`` from records to call records on the current stream: the text stage, Clair3_F
-        over the device matrix and ``model.decode_calls`` on the device views, with one host wait (the sizes) before the
-        network is queued.  Returns ``decode.batch_calls``' dict (``chromosome``, ``position``, ``calls``, ``text``, ``ad``,
-        ``start``; ``decode.calls_text`` formats it) plus ``Y``, the probabilities, on the device.  Every candidate is decoded,
-        as the reference decodes every full-alignment candidate.  Raises what ``batch_calls`` raises on an alt_info string the
-        decoder rejects."""
-        from . import decode
-        decode._check_config(output_config)
-        self._check_model(model, "call")
-        if bool(output_config.add_indel_length) != model.add_indel_length:
-            raise C3BError("call: output_config.add_indel_length must match the model")
-        self.alt_text()
-        nk = self.sizes()[0]                               # the one wait: the build and the text together
-        v = self.alt_text_device()
-        y = torch.empty((nk, model.out_dim), dtype=torch.float32, device=self._device)
-        self._forward_into(model, y)
-        out = model.decode_calls(y, v["ref_base"], v["decoder"], v["decoder_off"], output_config, k=k)
-        res = decode.calls_result(decode._numpy(out), [ctg_name] * nk, v["position"].cpu().numpy(), v["decoder_off"].cpu().numpy())
-        res["Y"] = y
-        return res
-
-    def _check_model(self, model, who):
-        if getattr(model, "_handle", None) is None:
-            raise C3BError("%s: the model has no device / weights yet (.to(device), .load_state_dict())" % who)
+    def _network(self):
         C = self._shape[2]
-        if model._kind != CONSTANTS["C3B_FULL_ALIGNMENT"] or model.input_channels != C:
-            raise C3BError("%s: needs the full-alignment network (Clair3_F) with %d input channels" % (who, C))
-        if torch.device(model._device) != self._device:
-            raise C3BError("%s: the model lives on %s, the builder on %s" % (who, model._device, self._device))
+        return CONSTANTS["C3B_FULL_ALIGNMENT"], C, "the full-alignment network (Clair3_F) with %d input channels" % C
 
-    def _forward_into(self, model, y):
-        """Clair3_F over every candidate's matrix into y, stream-ordered."""
+    def _queue_forward(self, model, y):
+        """Clair3_F over every candidate's matrix."""
         n, depth, _ = self._shape
-        if n == 0:
-            return
         pm = ffi.new("const int8_t **")
         check(lib().c3b_fa_device(self._h, pm))
         check(lib().c3b_forward(model._handle, ffi.cast("void *", pm[0]), CONSTANTS["C3B_DT_I8"], 1, n, depth,
