@@ -17,6 +17,7 @@ HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200.h")
 DEBUG_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_debug.h")     # taps / probes, not the drop-in surface
 PILEUP_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_pileup.h")   # pileup feature counter (SURVEY 8f N4)
 FA_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_fa.h")           # full-alignment tensor builder (N4)
+BAM_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_bam.h")         # BAM reader: BGZF blocks to device records
 LIB_PATH = os.path.join(_HERE, "libclair3b200.so")
 
 ffi = cffi.FFI()
@@ -35,11 +36,13 @@ _body, CONSTANTS = _cdef_source(HEADER)
 _dbg_body, _ = _cdef_source(DEBUG_HEADER)
 _plp_body, _ = _cdef_source(PILEUP_HEADER)
 _fa_body, _ = _cdef_source(FA_HEADER)
+_bam_body, _ = _cdef_source(BAM_HEADER)
 ffi.cdef(_body)
 ffi.cdef(_dbg_body)
 ffi.cdef(_plp_body)
 ffi.cdef(_fa_body)
-DECLARED_FUNCTIONS = sorted(set(re.findall(r"\b(c3b_\w+)\s*\(", _body + _dbg_body + _plp_body + _fa_body)))
+ffi.cdef(_bam_body)
+DECLARED_FUNCTIONS = sorted(set(re.findall(r"\b(c3b_\w+)\s*\(", _body + _dbg_body + _plp_body + _fa_body + _bam_body)))
 
 _lib = None
 

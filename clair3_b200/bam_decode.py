@@ -1,0 +1,100 @@
+"""The BAM reader on the GPU (``include/clair3_b200_bam.h``): a region's alignment records straight from the file into device memory.
+
+The host reads what it must to find the bytes - the header and the first record's virtual offset (``bam_io.read_bam_header``),
+and with a ``.bai`` index the compressed byte range of the region (``bam_io.read_bai`` / ``bam_io.bai_range``) - and checks the
+BGZF block headers.  The GPU inflates the blocks, finds the record chain, parses and filters the records exactly as
+``bam_io.read_bam(path, contig, start, end)`` does and scatters them into packed arrays.  The result is a
+``pileup_counts.DeviceBamRecords`` that ``PileupCounter.count`` and ``FullAlignmentBuilder.build`` take as they are: a region goes
+from compressed bytes to call records on the device.  No CPU fallback: everything here calls ``libclair3b200.so``.
+"""
+from __future__ import annotations
+
+import os
+
+import torch
+
+from . import bam_io
+from ._ffi import check, ffi
+from .pileup_counts import DeviceBamRecords, _Handle
+
+_NO_START, _NO_END = -1, 1 << 62            # read_bam's bounds when start / end are not given
+
+
+class BamDecoder(_Handle):
+    """One decoding workspace on one H100 (``c3b_bam``).  ``decode`` / ``decode_bytes`` queue the decode on the device's current
+    torch stream, wait once for the sizes, and return records in tensors the decoder allocated: a later decode does not touch
+    them."""
+
+    _API = "c3b_bam"
+
+    def __init__(self, device=0):
+        super().__init__(device)
+        self._headers = {}
+
+    def _header(self, path):
+        key = (os.path.abspath(path), os.path.getmtime(path), os.path.getsize(path))
+        if key not in self._headers:
+            self._headers[key] = bam_io.read_bam_header(path)
+        return self._headers[key]
+
+    def decode(self, path, ctg, start=None, end=None, fa_fields=False, ref_seq=None, index=None):
+        """The records of contig ``ctg`` overlapping [start, end) (0-based, end-exclusive; None = unbounded) of the BAM at
+        ``path``, as ``bam_io.read_bam(path, ctg, start, end, fa_fields=fa_fields)`` returns them, in device memory.
+        ``index``: a ``.bai`` path or a ``bam_io.read_bai`` result; by default ``path + ".bai"`` when that file exists.  With an
+        index only the region's byte range is read; without one, every block after the header.  ``ref_seq``: reference bases to
+        keep with the records (``DeviceBamRecords.ref``)."""
+        refs, first = self._header(path)
+        names = [n for n, _ in refs]
+        if ctg not in names:
+            raise ValueError("contig %r is not in the BAM header" % ctg)
+        tid = names.index(ctg)
+        if index is None and os.path.exists(str(path) + ".bai"):
+            index = str(path) + ".bai"
+        with open(path, "rb") as f:
+            if index is not None:
+                idx = bam_io.read_bai(index) if isinstance(index, (str, os.PathLike)) else index
+                lo = 0 if start is None else int(start)
+                hi = (1 << 29) if end is None else int(end)
+                c0, c1, u0, u1 = bam_io.bai_range(idx, tid, lo, hi, path)
+                f.seek(c0)
+                data = f.read(c1 - c0)
+            else:
+                f.seek(first >> 16)
+                data = f.read()
+                u0, u1 = first & 0xFFFF, -1
+        return self.decode_bytes(data, u0, u1, tid, start, end, fa_fields=fa_fields, ref_seq=ref_seq)
+
+    def decode_bytes(self, data, first_uoff, end_uoff, tid, start=None, end=None, fa_fields=False, ref_seq=None):
+        """``decode`` on whole BGZF blocks already in memory: ``data`` (bytes-like), the first record's offset in the first
+        block's data and the uncompressed offset where the records end (-1: the end of the data), and the contig's index in the
+        header."""
+        data = memoryview(data).cast("B") if not isinstance(data, (bytes, bytearray)) else data
+        lo = _NO_START if start is None else int(start)
+        hi = _NO_END if end is None else int(end)
+        L = self._lib()
+        buf = ffi.from_buffer(data) if len(data) else ffi.NULL
+        check(L.c3b_bam_decode(self._h, buf, len(data), int(first_uoff), int(end_uoff), int(tid), lo, hi, int(bool(fa_fields)),
+                               self._stream()))
+        n = [ffi.new("int64_t *") for _ in range(6)]
+        check(L.c3b_bam_sizes(self._h, *n))
+        n_reads, n_cigar, n_seq, n_qual, n_name, n_mv = (int(x[0]) for x in n)
+        dev = self._device
+
+        def alloc(count, dtype):
+            return torch.empty(max(count, 1), dtype=dtype, device=dev)[:count]     # never a null pointer, even when empty
+
+        t = {"pos": alloc(n_reads, torch.int64), "flag": alloc(n_reads, torch.int16), "mapq": alloc(n_reads, torch.uint8),
+             "cigar_off": alloc(n_reads + 1, torch.int64), "cigar": alloc(n_cigar, torch.int32),
+             "seq_off": alloc(n_reads + 1, torch.int64), "seq": alloc(n_seq, torch.uint8), "l_qseq": alloc(n_reads, torch.int32)}
+        if fa_fields:
+            t.update(qual_off=alloc(n_reads + 1, torch.int64), qual=alloc(n_qual, torch.uint8),
+                     qname_off=alloc(n_reads + 1, torch.int64), qname=alloc(n_name, torch.uint8),
+                     mv_off=alloc(n_reads + 1, torch.int64), mv=alloc(n_mv, torch.int32))
+        out = ffi.new("c3b_bam_out *")
+        ctype = {torch.int64: "int64_t *", torch.int16: "uint16_t *", torch.uint8: "uint8_t *", torch.int32: "int32_t *"}
+        for k, v in t.items():
+            c = "uint32_t *" if k == "cigar" else ctype[v.dtype]
+            setattr(out, k, ffi.cast(c, v.data_ptr()))
+        check(L.c3b_bam_fetch(self._h, out, 1))
+        return DeviceBamRecords.from_tensors(t, dev, ref_seq)
+

@@ -1,16 +1,24 @@
-"""Host-side BAM / FASTA reading for the pileup feature counter when htslib is not at hand.
+"""Host-side BAM / FASTA reading: the plain-Python record reader, and the header, index and byte ranges the GPU reader takes.
 
 The reference decodes alignments with htslib inside libclair3 (``sam_itr_next`` / ``bam_mplp_auto``, HKU-BAL/Clair3
-``src/medaka_bamiter.c:13-55``, ``src/clair3_pileup.c:160-176``) and fetches the reference with ``faidx_fetch_seq`` (``:184-186``).  The GPU
-counter (``clair3_b200.pileup_counts``) starts from DECODED records; this module is the plain-Python way to get them out of a
-coordinate-sorted ``.bam`` (BGZF blocks are gzip members, so ``gzip`` decodes the container; the records are parsed per the SAM/BAM
-specification, section 4.2) and the reference bases out of a FASTA file - decoding stays on the CPU, as in the reference.  A writer
-is included so that tests (and users without samtools) can produce valid files.  CRAM and the ``.bai`` index are not handled: the
-file is scanned, which is what a chunk-per-process deployment amortises poorly - with htslib available, fill ``BamRecords`` from
-``bam1_t`` directly (INTEGRATION.md).
+``src/medaka_bamiter.c:13-55``, ``src/clair3_pileup.c:160-176``) and fetches the reference with ``faidx_fetch_seq`` (``:184-186``).
+Two readers produce the records the GPU counter and builder take:
+
+- ``clair3_b200.bam_decode.BamDecoder`` inflates the BGZF blocks and parses the records on the GPU, into device-resident records.
+  This module gives it what the host has to know first: the header and the first record's virtual offset
+  (``read_bam_header``), the ``.bai`` index (``read_bai``) and the compressed byte range of a region (``bai_range``), and the
+  checked BGZF block headers (``bgzf_blocks``).
+- ``read_bam`` is the plain-Python reader: it inflates the whole file with ``gzip`` (BGZF blocks are gzip members) and parses the
+  records per the SAM/BAM specification, section 4.2, on the CPU.  It states the region filter both readers apply, and the tests
+  hold the GPU reader to it.
+
+A writer is included so that tests (and users without samtools) can produce valid files, and ``write_bai`` indexes them as the
+specification's section 5.2 describes.  CRAM and CSI indexes are not handled.  The reference bases come out of a FASTA file
+(``read_fasta``).
 """
 from __future__ import annotations
 
+import bisect
 import gzip
 import struct
 import zlib
@@ -232,3 +240,248 @@ def write_fasta(path, seqs, width=60):
             f.write(">%s\n" % name)
             for i in range(0, len(seq), width):
                 f.write(seq[i:i + width] + "\n")
+
+
+# ---- BGZF blocks, the header and the .bai index: what the GPU reader (clair3_b200.bam_decode) needs from the host ----
+
+BGZF_MAX = 65536             # a BGZF block holds at most 64 KiB, compressed or not (SAM/BAM specification 4.1)
+
+
+def bgzf_block(buf, off):
+    """(total size, payload offset, payload size, ISIZE) of the BGZF block at ``buf[off:]``, after the checks the GPU reader's
+    ``c3b_bam_decode`` makes: the gzip magic ``1f 8b 08 04``, a ``BC`` subfield anywhere in the extra field, a ``BSIZE`` that
+    covers the header and footer and fits the data, and ``ISIZE <= 65536``.  Raises ValueError naming the block's offset."""
+    if len(buf) - off < 18:
+        raise ValueError("%d trailing bytes at offset %d are not a BGZF block" % (len(buf) - off, off))
+    if bytes(buf[off:off + 4]) != b"\x1f\x8b\x08\x04":
+        raise ValueError("the block at offset %d is not a BGZF block (gzip header %s, want 1f 8b 08 04)"
+                         % (off, bytes(buf[off:off + 4]).hex(" ")))
+    xlen, = struct.unpack_from("<H", buf, off + 10)
+    if off + 12 + xlen > len(buf):
+        raise ValueError("the extra field of the block at offset %d runs past the data" % off)
+    bsize, x = None, 0
+    while x + 4 <= xlen:
+        si1, si2, slen = struct.unpack_from("<BBH", buf, off + 12 + x)
+        if x + 4 + slen > xlen:
+            break
+        if si1 == 66 and si2 == 67 and slen == 2:
+            bsize, = struct.unpack_from("<H", buf, off + 16 + x)
+            break
+        x += 4 + slen
+    if bsize is None:
+        raise ValueError("the block at offset %d has no BC subfield" % off)
+    size = bsize + 1
+    if size < 12 + xlen + 8 or off + size > len(buf):
+        raise ValueError("BSIZE %d of the block at offset %d is out of range" % (bsize, off))
+    isize, = struct.unpack_from("<I", buf, off + size - 4)
+    if isize > BGZF_MAX:
+        raise ValueError("ISIZE %d of the block at offset %d exceeds 65536" % (isize, off))
+    return size, off + 12 + xlen, size - 12 - xlen - 8, isize
+
+
+def bgzf_blocks(buf):
+    """[(offset, total size, ISIZE)] of the BGZF blocks that make up ``buf`` (whole blocks only), checked as ``bgzf_block``."""
+    out, off = [], 0
+    while off < len(buf):
+        size, _, _, isize = bgzf_block(buf, off)
+        out.append((off, size, isize))
+        off += size
+    return out
+
+
+def _inflate_block(buf, off):
+    size, p0, n, isize = bgzf_block(buf, off)
+    data = zlib.decompress(bytes(buf[p0:p0 + n]), -15)
+    if len(data) != isize:
+        raise ValueError("the block at offset %d inflates to %d bytes, not its ISIZE %d" % (off, len(data), isize))
+    return size, data
+
+
+def _read_block(f, off):
+    """(total size, the block's bytes) of the BGZF block at byte ``off`` of the open file ``f``; (0, b"") at the end of the file."""
+    f.seek(off)
+    head = f.read(18)
+    if not head:
+        return 0, b""
+    xlen, = struct.unpack_from("<H", head, 10) if len(head) >= 12 else (0,)
+    head += f.read(max(0, 12 + xlen - len(head)))
+    size = bgzf_block(head + bytes(BGZF_MAX), 0)[0]     # the header alone decides the size; the padding stands in for the rest
+    return size, head + f.read(size - len(head))
+
+
+def read_bam_header(path):
+    """(references [(name, length)], virtual offset of the first record) of a BAM file, inflating only the blocks that hold the
+    header.  The virtual offset is ``block offset << 16 | offset in the block's data`` (SAM/BAM specification 4.1.1)."""
+    with open(path, "rb") as f:
+        data, starts, off = bytearray(), [], 0
+        while True:
+            size, block = _read_block(f, off)
+            if not size:
+                raise ValueError("%s: the file ends inside the BAM header" % path)
+            starts.append((off, len(data)))
+            data += _inflate_block(block, 0)[1]
+            off += size
+            if len(data) < 4 or data[:4] != b"BAM\x01":
+                if len(data) >= 4:
+                    raise ValueError("not a BAM stream (magic %r)" % bytes(data[:4]))
+                continue
+            try:
+                refs, end = read_header(data)
+            except (struct.error, UnicodeDecodeError):
+                continue
+            if end == len(data):                   # the header ends with the block: the first record starts the next one
+                return refs, off << 16
+            c, u = starts[bisect.bisect_right([u for _, u in starts], end) - 1]
+            return refs, c << 16 | (end - u)
+
+
+_PSEUDO_BIN = 37450          # the .bai pseudo-bin that holds a reference's offsets and mapped / unmapped counts
+
+
+def _reg2bins(beg, end):
+    """Every bin that can hold a record overlapping [beg, end) (SAM/BAM specification 5.3, reg2bins)."""
+    end -= 1
+    bins = [0]
+    for shift, base in ((26, 1), (23, 9), (20, 73), (17, 585), (14, 4681)):
+        bins.extend(range(base + (beg >> shift), base + (end >> shift) + 1))
+    return bins
+
+
+def read_bai(path):
+    """A ``.bai`` index (SAM/BAM specification 5.2) as one dict per reference: ``bins`` {bin: [(begin, end) virtual offsets]}
+    without the pseudo-bin 37450, and ``linear``, the 16 kb linear index (uint64 virtual offsets)."""
+    with open(path, "rb") as f:
+        buf = f.read()
+    if buf[:4] != b"BAI\x01":
+        raise ValueError("%s: not a BAI index (magic %r)" % (path, buf[:4]))
+    n_ref, = struct.unpack_from("<i", buf, 4)
+    off, out = 8, []
+    for _ in range(n_ref):
+        n_bin, = struct.unpack_from("<i", buf, off)
+        off += 4
+        bins = {}
+        for _ in range(n_bin):
+            b, n_chunk = struct.unpack_from("<Ii", buf, off)
+            off += 8
+            chunks = np.frombuffer(buf, dtype="<u8", count=2 * n_chunk, offset=off).reshape(-1, 2)
+            off += 16 * n_chunk
+            if b != _PSEUDO_BIN:
+                bins[b] = [(int(x), int(y)) for x, y in chunks]
+        n_intv, = struct.unpack_from("<i", buf, off)
+        off += 4
+        linear = np.frombuffer(buf, dtype="<u8", count=n_intv, offset=off).astype(np.uint64)
+        off += 8 * n_intv
+        out.append({"bins": bins, "linear": linear})
+    return out
+
+
+def _bai_span(index, tid, start, end):
+    """(first virtual offset, end virtual offset) covering every record of contig ``tid`` the index puts in [start, end), or
+    None: the chunks of the bins of reg2bins, less those that end before the linear index's offset for ``start``."""
+    if tid >= len(index):
+        return None
+    beg = max(int(start), 0)
+    hi = min(int(end), 1 << 29)
+    if hi <= beg:                                  # read_bam keeps pos < end and pos + span > start: those start before end
+        beg, hi = 0, hi
+    if hi <= 0:
+        return None
+    ref = index[tid]
+    lin = ref["linear"]
+    min_off = int(lin[min(beg >> 14, len(lin) - 1)]) if len(lin) else 0
+    chunks = [c for b in _reg2bins(beg, hi) for c in ref["bins"].get(b, ()) if c[1] > min_off]
+    if not chunks:
+        return None
+    return min(c[0] for c in chunks), max(c[1] for c in chunks)
+
+
+def bai_range(index, tid, start, end, bam_path):
+    """One compressed byte range of whole BGZF blocks ``(coff_begin, coff_end, first_uoff, end_uoff)`` that holds every record of
+    contig ``tid`` overlapping [start, end), from the index (``read_bai``): the union of the chunks of the bins of
+    ``reg2bins(start, end)``, pruned by the linear index.  ``first_uoff`` is the first record's offset in the first block's data
+    and ``end_uoff`` where the records end, counted from the range's first uncompressed byte: the arguments of
+    ``c3b_bam_decode``.  The union is a superset of the region's records; the decoder's filter makes it exact.  The block sizes
+    come from the headers of the range's blocks in ``bam_path``.  (0, 0, 0, 0) when the index holds nothing there."""
+    span = _bai_span(index, tid, start, end)
+    if span is None:
+        return 0, 0, 0, 0
+    (c0, u0), (ce, ue) = divmod(span[0], 1 << 16), divmod(span[1], 1 << 16)
+    acc, c = 0, c0
+    with open(bam_path, "rb") as f:
+        while c < ce:
+            size, block = _read_block(f, c)
+            if not size:
+                break
+            acc += bgzf_block(block, 0)[3]
+            c += size
+        if c != ce:
+            raise ValueError("%s: the index's offset %d is not the start of a BGZF block" % (bam_path, ce))
+        if ue == 0:
+            return c0, ce, u0, acc
+        size, block = _read_block(f, ce)
+        return c0, ce + size, u0, acc + ue
+
+
+def write_bai(bam_path, bai_path=None):
+    """Writes the ``.bai`` index of a coordinate-sorted BAM (default ``bam_path + ".bai"``) as the SAM/BAM specification (5.2)
+    describes it: per reference the bins of reg2bin(pos, pos + max(span, 1)) with their chunks of virtual offsets (adjacent
+    records of a bin merged into one chunk), the pseudo-bin 37450 (offsets of the reference's records, mapped and unmapped
+    counts) and the 16 kb linear index, then the number of records without a coordinate.  Returns the path written."""
+    with open(bam_path, "rb") as f:
+        raw = f.read()
+    blocks = bgzf_blocks(raw)
+    parts, ustart, u = [], [], 0
+    for off, _, isize in blocks:
+        ustart.append(u)
+        parts.append(_inflate_block(raw, off)[1])
+        u += isize
+    buf = b"".join(parts)
+
+    def voff(x):
+        i = bisect.bisect_right(ustart, x) - 1
+        return blocks[i][0] << 16 | (x - ustart[i])
+
+    refs, off = read_header(buf)
+    idx = [{"bins": {}, "lin": {}, "first": None, "last": 0, "mapped": 0, "unmapped": 0} for _ in refs]
+    n_no_coor = 0
+    while off + 4 <= len(buf):
+        block_size, = struct.unpack_from("<i", buf, off)
+        tid, p, l_name, _, _, n_cig, fl = struct.unpack_from("<iiBBHHH", buf, off + 4)
+        beg, nxt = voff(off), voff(off + 4 + block_size)
+        cig = np.frombuffer(buf, dtype="<u4", count=n_cig, offset=off + 36 + l_name)
+        off += 4 + block_size
+        if tid < 0 or p < 0:
+            n_no_coor += 1
+            continue
+        span = int((cig >> 4)[np.isin(cig & 15, _REF_CONSUMING)].sum()) if n_cig else 0
+        e = p + max(span, 1)
+        r = idx[tid]
+        chunks = r["bins"].setdefault(_reg2bin(p, e), [])
+        if chunks and chunks[-1][1] == beg:
+            chunks[-1][1] = nxt
+        else:
+            chunks.append([beg, nxt])
+        for w in range(p >> 14, ((e - 1) >> 14) + 1):
+            r["lin"].setdefault(w, beg)
+        r["first"] = beg if r["first"] is None else r["first"]
+        r["last"] = nxt
+        r["unmapped" if fl & 4 else "mapped"] += 1
+    out = bytearray(b"BAI\x01" + struct.pack("<i", len(refs)))
+    for r in idx:
+        bins = dict(r["bins"])
+        if r["first"] is not None:
+            bins[_PSEUDO_BIN] = [[r["first"], r["last"]], [r["mapped"], r["unmapped"]]]
+        out += struct.pack("<i", len(bins))
+        for b, chunks in bins.items():
+            out += struct.pack("<Ii", b, len(chunks)) + b"".join(struct.pack("<QQ", x, y) for x, y in chunks)
+        n_intv = max(r["lin"]) + 1 if r["lin"] else 0
+        lin, prev = [], r["first"] or 0             # windows before the first record's: its offset; gaps: the previous window's
+        for w in range(n_intv):
+            prev = r["lin"].get(w, prev)
+            lin.append(prev)
+        out += struct.pack("<i", n_intv) + b"".join(struct.pack("<Q", x) for x in lin)
+    out += struct.pack("<Q", n_no_coor)
+    path = bai_path or str(bam_path) + ".bai"
+    with open(path, "wb") as f:
+        f.write(out)
+    return path

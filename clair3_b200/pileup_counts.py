@@ -84,6 +84,11 @@ _TORCH_VIEW = {"uint16": np.int16, "uint32": np.int32}          # torch has no u
 
 
 class DeviceBamRecords:
+    """Alignment records in device memory (``c3b_plp_count`` / ``c3b_fa_build`` with ``on_device = 1``): the tensors ``t`` by field
+    name (unsigned fields as same-width signed tensors; an optional field absent is None) and, optionally, the reference bases
+    ``ref`` as a uint8 tensor on the same device.  Made from host records (``BamRecords.to_device``) or from tensors a device
+    decoder wrote (``from_tensors``)."""
+
     def __init__(self, rec, device, ref_seq=None):
         self.n_reads = rec.n_reads
         self.device = torch.device(device)
@@ -96,10 +101,44 @@ class DeviceBamRecords:
             for name in (k, k + "_off"):
                 a = getattr(rec, name, None)
                 self.t[name] = None if a is None else torch.from_numpy(np.ascontiguousarray(a if a.size else np.zeros(1, a.dtype))).to(self.device)
-        self.ref = None
-        if ref_seq is not None:
-            b = ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq)
-            self.ref = torch.from_numpy(np.frombuffer(b, dtype=np.uint8).copy()).to(self.device)
+        self.ref = _device_ref(ref_seq, self.device)
+
+    @classmethod
+    def from_tensors(cls, tensors, device, ref_seq=None):
+        """Records from device tensors, taken over without a copy: ``tensors`` maps every ``BamRecords`` field to a contiguous
+        tensor on ``device`` of that field's width (int16 for ``flag``, int32 for ``cigar``), and each optional field and its
+        ``_off`` to tensors or None.  The tensors must satisfy what ``BamRecords`` checks on the host."""
+        self = cls.__new__(cls)
+        self.device = torch.device(device)
+        self.n_reads = int(tensors["pos"].numel())
+        self.t = {k: tensors[k] for k, _ in _FIELDS}
+        for k, _ in _OPTIONAL:
+            for name in (k, k + "_off"):
+                self.t[name] = tensors.get(name)
+        for k, v in self.t.items():
+            if v is not None and (v.device != self.device or not v.is_contiguous()):
+                raise C3BError("DeviceBamRecords: %s must be a contiguous tensor on %s" % (k, self.device))
+        self.ref = _device_ref(ref_seq, self.device)
+        return self
+
+    def host(self):
+        """The records as ``bam_io.read_bam`` returns them (numpy arrays of its dtypes; the optional fields where present)."""
+        out = {}
+        for k, dt in _FIELDS + _OPTIONAL + tuple((k + "_off", np.int64) for k, _ in _OPTIONAL):
+            v = self.t.get(k)
+            if v is not None:
+                out[k] = v.cpu().numpy().view(dt) if np.dtype(dt).itemsize == v.element_size() else v.cpu().numpy().astype(dt)
+        return out
+
+
+def _device_ref(ref_seq, device):
+    """Reference bases (str / bytes, or a uint8 tensor) as a uint8 tensor on ``device``; None stays None."""
+    if ref_seq is None:
+        return None
+    if isinstance(ref_seq, torch.Tensor):
+        return ref_seq.to(device=device, dtype=torch.uint8).contiguous()
+    b = ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq)
+    return torch.from_numpy(np.frombuffer(b, dtype=np.uint8).copy()).to(device)
 
 
 def _records_struct(rec, optional=False):
@@ -123,11 +162,11 @@ def _records_struct(rec, optional=False):
     return s
 
 
-class _Workspace:
-    """What ``PileupCounter`` and ``FullAlignmentBuilder`` share: a library workspace on one CUDA device, created by
-    ``<_API>_create`` and released by ``<_API>_destroy``, whose calls run on the device's current torch stream."""
+class _Handle:
+    """A library workspace on one CUDA device, created by ``<_API>_create`` and released by ``<_API>_destroy``, whose calls run
+    on the device's current torch stream (``PileupCounter``, ``FullAlignmentBuilder``, ``bam_decode.BamDecoder``)."""
 
-    _API = None                      # "c3b_plp" / "c3b_fa"
+    _API = None                      # "c3b_plp" / "c3b_fa" / "c3b_bam"
 
     def __init__(self, device):
         dev = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
@@ -152,6 +191,31 @@ class _Workspace:
     def _stream(self):
         return ffi.cast("void *", torch.cuda.current_stream(self._device).cuda_stream)
 
+    def _timing(self, fn):
+        ms, n = ffi.new("float *"), ffi.new("int *")
+        check(fn(self._h, ms, n))
+        return float(ms[0]), int(n[0])
+
+    def last_ms(self):
+        """(device milliseconds, kernel launches) of the last call, between CUDA events on its stream."""
+        return self._timing(self._entry("_last_ms"))
+
+    def close(self):
+        if getattr(self, "_h", None) is not None:
+            self._entry("_destroy")(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class _Workspace(_Handle):
+    """What ``PileupCounter`` and ``FullAlignmentBuilder`` share beyond the workspace itself: the reference bases of a call, and
+    the all_alt_info text stage with the call path behind it."""
+
     @staticmethod
     def _reference(ref_seq, rec, who):
         """(pointer, length, object that owns the bytes) of a call's reference bases: str / bytes on the host, or with device
@@ -165,15 +229,6 @@ class _Workspace:
             return ffi.cast("const char *", ref.data_ptr()), ref.numel(), ref
         ref = ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq)
         return ffi.cast("const char *", ffi.from_buffer(ref)), len(ref), ref
-
-    def _timing(self, fn):
-        ms, n = ffi.new("float *"), ffi.new("int *")
-        check(fn(self._h, ms, n))
-        return float(ms[0]), int(n[0])
-
-    def last_ms(self):
-        """(device milliseconds, kernel launches) of the last call, between CUDA events on its stream."""
-        return self._timing(self._entry("_last_ms"))
 
     # The all_alt_info text stage and the call path behind it, the same for both workspaces.  Each class states what differs:
     # _text_max_indel (whether a text stage can follow the last call, and its default max_indel_length), _text_queued (what a
@@ -282,17 +337,6 @@ class _Workspace:
         """The network over every candidate into y, stream-ordered."""
         if len(y):
             self._queue_forward(model, y)
-
-    def close(self):
-        if getattr(self, "_h", None) is not None:
-            self._entry("_destroy")(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class PileupCounter(_Workspace):
