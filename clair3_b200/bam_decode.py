@@ -4,7 +4,7 @@ The host reads what it must to find the bytes - the header and the first record'
 and with a ``.bai`` index the compressed byte range of the region (``bam_io.read_bai`` / ``bam_io.bai_range``) - and checks the
 BGZF block headers.  The GPU inflates the blocks, finds the record chain, parses and filters the records exactly as
 ``bam_io.read_bam(path, contig, start, end)`` does and scatters them into packed arrays.  The result is a
-``pileup_counts.DeviceBamRecords`` that ``PileupCounter.count`` and ``FullAlignmentBuilder.build`` take as they are: a region goes
+``records.DeviceBamRecords`` that ``PileupCounter.count`` and ``FullAlignmentBuilder.build`` take as they are: a region goes
 from compressed bytes to call records on the device.  No CPU fallback: everything here calls ``libclair3b200.so``.
 """
 from __future__ import annotations
@@ -14,8 +14,9 @@ import os
 import torch
 
 from . import bam_io
-from ._ffi import check, ffi
-from .pileup_counts import DeviceBamRecords, _Handle
+from ._ffi import check, ffi, lib
+from ._workspace import _Handle
+from .records import FIELDS, VALUES, DeviceBamRecords
 
 _NO_START, _NO_END = -1, 1 << 62            # read_bam's bounds when start / end are not given
 
@@ -30,6 +31,9 @@ class BamDecoder(_Handle):
     def __init__(self, device=0):
         super().__init__(device)
         self._headers = {}
+
+    def _lib(self):
+        return lib()
 
     def _header(self, path):
         key = (os.path.abspath(path), os.path.getmtime(path), os.path.getsize(path))
@@ -77,24 +81,15 @@ class BamDecoder(_Handle):
                                self._stream()))
         n = [ffi.new("int64_t *") for _ in range(6)]
         check(L.c3b_bam_sizes(self._h, *n))
-        n_reads, n_cigar, n_seq, n_qual, n_name, n_mv = (int(x[0]) for x in n)
-        dev = self._device
-
-        def alloc(count, dtype):
-            return torch.empty(max(count, 1), dtype=dtype, device=dev)[:count]     # never a null pointer, even when empty
-
-        t = {"pos": alloc(n_reads, torch.int64), "flag": alloc(n_reads, torch.int16), "mapq": alloc(n_reads, torch.uint8),
-             "cigar_off": alloc(n_reads + 1, torch.int64), "cigar": alloc(n_cigar, torch.int32),
-             "seq_off": alloc(n_reads + 1, torch.int64), "seq": alloc(n_seq, torch.uint8), "l_qseq": alloc(n_reads, torch.int32)}
-        if fa_fields:
-            t.update(qual_off=alloc(n_reads + 1, torch.int64), qual=alloc(n_qual, torch.uint8),
-                     qname_off=alloc(n_reads + 1, torch.int64), qname=alloc(n_name, torch.uint8),
-                     mv_off=alloc(n_reads + 1, torch.int64), mv=alloc(n_mv, torch.int32))
-        out = ffi.new("c3b_bam_out *")
-        ctype = {torch.int64: "int64_t *", torch.int16: "uint16_t *", torch.uint8: "uint8_t *", torch.int32: "int32_t *"}
-        for k, v in t.items():
-            c = "uint32_t *" if k == "cigar" else ctype[v.dtype]
-            setattr(out, k, ffi.cast(c, v.data_ptr()))
+        n_reads = int(n[0][0])          # then the length of each value field, in table order
+        n_values = dict(zip((f.name for f in FIELDS if f.length == VALUES), (int(x[0]) for x in n[1:])))
+        t, out = {}, ffi.new("c3b_bam_out *")
+        for f in FIELDS:
+            if f.optional and not fa_fields:
+                continue
+            count = f.size(n_reads, n_values.get(f.name))
+            t[f.name] = v = torch.empty(max(count, 1), dtype=f.torch_dtype, device=self._device)[:count]    # never null, even empty
+            setattr(out, f.name, ffi.cast(f.ctype + " *", v.data_ptr()))
         check(L.c3b_bam_fetch(self._h, out, 1))
-        return DeviceBamRecords.from_tensors(t, dev, ref_seq)
+        return DeviceBamRecords.from_tensors(t, self._device, ref_seq)
 

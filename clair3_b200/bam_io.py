@@ -72,7 +72,7 @@ def _aux_mv(buf, p, e):
 
 
 def read_bam(path, ref_name=None, start=None, end=None, with_names=False, fa_fields=False):
-    """Alignment records of a coordinate-sorted BAM as the arrays of ``clair3_b200.pileup_counts.BamRecords`` (plus ``tid``), in
+    """Alignment records of a coordinate-sorted BAM as the arrays of ``clair3_b200.records.BamRecords`` (plus ``tid``), in
     file order.  ``ref_name`` / ``start`` / ``end`` (0-based, end-exclusive) keep what an indexed fetch of that region returns:
     records of that contig whose alignment overlaps [start, end).  Unmapped-without-position records (refID -1) are skipped.
     ``fa_fields``: also the fields the full-alignment tensor builder reads (``clair3_b200.fa_tensor``): ``qual`` / ``qual_off``

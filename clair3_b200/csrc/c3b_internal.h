@@ -10,6 +10,7 @@
 
 #include "../../include/clair3_b200.h"
 #include "../../include/clair3_b200_debug.h"
+#include "../../include/clair3_b200_fa.h"
 #include "../../include/clair3_b200_pileup.h"
 
 #define C3B_T 33            // positions per site (shared/param_p.py:34-35)
@@ -141,20 +142,6 @@ struct C3bReads {
     const int32_t *mv;
 };
 
-// The eight core c3b_bam_records arrays of a call into R through c3b_upload.  n_cigar / n_seq: the CIGAR words and sequence
-// bytes the arrays hold.
-inline int c3b_upload_records(C3bReads &R, C3bBuf (&b)[8], const c3b_bam_records *r, int64_t n_cigar, int64_t n_seq, int on_device,
-                              cudaStream_t s, const char *what) {
-    const size_t n = (size_t)r->n_reads;
-    return c3b_upload(b[0], r->pos, n * 8, on_device, R.pos, s, what) || c3b_upload(b[1], r->flag, n * 2, on_device, R.flag, s, what) ||
-           c3b_upload(b[2], r->mapq, n, on_device, R.mapq, s, what) ||
-           c3b_upload(b[3], r->cigar_off, (n + 1) * 8, on_device, R.cigar_off, s, what) ||
-           c3b_upload(b[4], r->cigar, (size_t)n_cigar * 4, on_device, R.cigar, s, what) ||
-           c3b_upload(b[5], r->seq_off, (n + 1) * 8, on_device, R.seq_off, s, what) ||
-           c3b_upload(b[6], r->seq, (size_t)n_seq, on_device, R.seq, s, what) ||
-           c3b_upload(b[7], r->l_qseq, n * 4, on_device, R.l_qseq, s, what);
-}
-
 #ifdef __CUDACC__
 // 4-bit nt16 code of base i of a packed sequence (bam_get_seq: two per byte, high nibble first) of lq bases; 0 ('=') outside it
 __device__ __forceinline__ int c3b_nib_at(const uint8_t *sq, int lq, long long i) {
@@ -201,8 +188,9 @@ struct C3bAltText {
 
 // What the pileup counter (c3b_plp) and the full-alignment builder (c3b_fa) hold alike: the device and the stream of the last
 // call, a pair of CUDA events around each timed stage with the stage's kernel launches, a device counter block with its pinned
-// host mirror, the exported allele records, and the all_alt_info text stage (stage 1).  The destructor releases the events and
-// the pinned memory.
+// host mirror, the record intake, the exported allele records, and the all_alt_info text stage (stage 1).  The destructor
+// releases the events and the pinned memory.  The BAM reader (c3b_bam) uses the events and the counter block; its intake buffers
+// stay unallocated.
 struct C3bRegionWorkspace {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -213,10 +201,13 @@ struct C3bRegionWorkspace {
     int n_counters = 0;
     int text_word = 0;                   // counters[text_word .. +2]: the text stage's status, text bytes, decoder bytes
     C3bBuf al_meta, al_read, al_qpos, al_cnt, al_off, al_n;
-    // the text stage: where the last count / build left the records and the reference, the stage's scratch and outputs
+    // the records and the reference of the last count / build where they live on the device (intake), with the CIGAR words and
+    // sequence bytes the records hold, and the device copies of the host arrays among them
     C3bReads R{};
     const char *dref = nullptr;
     int64_t ref_start = 0, ref_len = 0, n_cigar = 0, n_seq = 0;
+    C3bBuf in_core[8], in_qoff, in_qual, in_noff, in_name, in_moff, in_mv, in_ref;
+    // the text stage's scratch and outputs
     C3bBuf tx_hash, tx_order, tx_table, tx_nins, tx_ndel, tx_len_text, tx_len_dec;
     C3bBuf tx_text, tx_dec, tx_text_off, tx_dec_off, tx_ref_base, tx_position;
     bool texted = false;
@@ -256,6 +247,63 @@ struct C3bRegionWorkspace {
         if (capacity < n) { c3b_set_error("%s: capacity %lld < %lld records", who, (long long)capacity, (long long)n); return 1; }
         const size_t b = (size_t)n * 4;
         return get(meta, al_meta, b) || get(read, al_read, b) || get(qpos, al_qpos, b) || get(cnt, al_cnt, b);
+    }
+
+    // The records and the reference of a count / build on `stream`: checks the records (n_reads below max_reads, no null array
+    // when there are reads, an optional field's values with its offsets) and the reference, reads the closing offsets (with
+    // device records a host wait each), copies host arrays to the device in field order, the reference last, and fills R, dref,
+    // ref_start, ref_len, n_cigar and n_seq.  opt: the optional fields, null for none; mv only with want_mv.  `who` names the
+    // entry point in the errors.
+    int intake(const char *who, const c3b_bam_records *core, const c3b_fa_records *opt, bool want_mv, int64_t max_reads,
+               int on_device, const char *ref_seq, int64_t ref_start, int64_t ref_len) {
+        const int64_t n = core->n_reads;
+        if (n < 0 || n >= max_reads) { c3b_set_error("%s: bad n_reads", who); return 1; }
+        if (n > 0 && (!core->pos || !core->flag || !core->mapq || !core->cigar_off || !core->cigar || !core->seq_off ||
+                      !core->seq || !core->l_qseq)) {
+            c3b_set_error("%s: null record array", who);
+            return 1;
+        }
+        if (opt && ((opt->qual_off && !opt->qual) || (opt->qname_off && !opt->qname) || (opt->mv_off && !opt->mv))) {
+            c3b_set_error("%s: an optional record field has offsets but no values", who);
+            return 1;
+        }
+        if (ref_len > 0 && !ref_seq) { c3b_set_error("%s: null ref_seq", who); return 1; }
+        C3bReads r{};
+        r.n = n;
+        int64_t nc = 0, ns = 0;
+        if (n > 0) {
+            int64_t nq = 0, nn = 0, nm = 0;
+            auto last = [&](const int64_t *off, int64_t *v) { return c3b_last_offset(off, n, on_device, stream, v); };
+            if (last(core->cigar_off, &nc) || last(core->seq_off, &ns) ||
+                (opt && (last(opt->qual_off, &nq) || last(opt->qname_off, &nn) || last(opt->mv_off, &nm))))
+                return 1;
+            if (nc < 0 || ns < 0 || nq < 0 || nn < 0 || nm < 0) { c3b_set_error("%s: negative closing offset", who); return 1; }
+            const size_t n0 = (size_t)n, n1 = (n0 + 1) * 8;
+            auto up = [&](C3bBuf &b, const auto *src, size_t bytes, auto &dev) {
+                return c3b_upload(b, src, bytes, on_device, dev, stream, who);
+            };
+            if (up(in_core[0], core->pos, n0 * 8, r.pos) || up(in_core[1], core->flag, n0 * 2, r.flag) ||
+                up(in_core[2], core->mapq, n0, r.mapq) || up(in_core[3], core->cigar_off, n1, r.cigar_off) ||
+                up(in_core[4], core->cigar, (size_t)nc * 4, r.cigar) || up(in_core[5], core->seq_off, n1, r.seq_off) ||
+                up(in_core[6], core->seq, (size_t)ns, r.seq) || up(in_core[7], core->l_qseq, n0 * 4, r.l_qseq))
+                return 1;
+            if (opt && opt->qual_off && (up(in_qoff, opt->qual_off, n1, r.qual_off) || up(in_qual, opt->qual, (size_t)nq, r.qual)))
+                return 1;
+            if (opt && opt->qname_off &&
+                (up(in_noff, opt->qname_off, n1, r.qname_off) || up(in_name, opt->qname, (size_t)nn, r.qname)))
+                return 1;
+            if (opt && opt->mv_off && want_mv && (up(in_moff, opt->mv_off, n1, r.mv_off) || up(in_mv, opt->mv, (size_t)nm * 4, r.mv)))
+                return 1;
+        }
+        const char *d = nullptr;
+        if (c3b_upload(in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, d, stream, who)) return 1;
+        R = r;
+        dref = d;
+        this->ref_start = ref_start;
+        this->ref_len = ref_len > 0 ? ref_len : 0;
+        n_cigar = nc;
+        n_seq = ns;
+        return 0;
     }
 
     // The text stage over up to n candidates (the counter's region width, the builder's candidate count): sizes and grows its

@@ -919,8 +919,7 @@ void glibc_jump_matrices(std::vector<uint32_t> &out) {
 constexpr int N_COUNTERS = 10, TEXT_WORD = 7;
 
 struct c3b_fa : C3bRegionWorkspace {
-    C3bBuf in_core[8], in_qoff, in_qual, in_noff, in_name, in_moff, in_mv;
-    C3bBuf in_ref, in_cand, in_var, jump, state0;
+    C3bBuf in_cand, in_var, jump, state0;
     C3bBuf fstart, fcnt, foff, F;
     C3bBuf rend, rlo, rov, pass, table, keep, kidx, kovr, kov_ex;
     C3bBuf k_orig, k_start, k_end, k_pmax, k_fs, k_ov, k_pi, k_sig, k_hap, sig_len, sig_ex;
@@ -963,18 +962,6 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
                  const c3b_fa_variant *variants, int64_t n_var, const char *ref_seq, int64_t ref_start, int64_t ref_len,
                  const c3b_fa_params *params, void *cuda_stream) {
     if (!w || !records || !params) { c3b_set_error("c3b_fa_build: null argument"); return 1; }
-    const c3b_bam_records *core = &records->core;
-    const int64_t n = core->n_reads;
-    if (n < 0 || n >= (int64_t)INT_MAX) { c3b_set_error("c3b_fa_build: bad n_reads"); return 1; }
-    if (n > 0 && (!core->pos || !core->flag || !core->mapq || !core->cigar_off || !core->cigar || !core->seq_off || !core->seq ||
-                  !core->l_qseq)) {
-        c3b_set_error("c3b_fa_build: null record array");
-        return 1;
-    }
-    if ((records->qual_off && !records->qual) || (records->qname_off && !records->qname) || (records->mv_off && !records->mv)) {
-        c3b_set_error("c3b_fa_build: an optional record field has offsets but no values");
-        return 1;
-    }
     if (params->matrix_depth < 1 || params->matrix_depth > 256) {
         c3b_set_error("c3b_fa_build: matrix_depth %d outside 1..256", params->matrix_depth);
         return 1;
@@ -992,7 +979,6 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
             c3b_set_error("c3b_fa_build: variants must be sorted by position (index %lld)", (long long)i);
             return 1;
         }
-    if (ref_len > 0 && !ref_seq) { c3b_set_error("c3b_fa_build: null ref_seq"); return 1; }
     C3B_CUDA(cudaSetDevice(w->device));
     cudaStream_t s = (cudaStream_t)cuda_stream;
     w->stream = s;
@@ -1003,35 +989,10 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     w->n_kept = 0;
     const int depth = params->matrix_depth;
 
-    // inputs
-    C3bReads R{};
-    R.n = n;
-    int64_t n_cigar = 0, n_seq = 0;
-    if (n > 0) {
-        int64_t n_qual, n_name, n_mv;
-        if (c3b_last_offset(core->cigar_off, n, on_device, s, &n_cigar) || c3b_last_offset(core->seq_off, n, on_device, s, &n_seq) ||
-            c3b_last_offset(records->qual_off, n, on_device, s, &n_qual) || c3b_last_offset(records->qname_off, n, on_device, s, &n_name) ||
-            c3b_last_offset(records->mv_off, n, on_device, s, &n_mv))
-            return 1;
-        if (n_cigar < 0 || n_seq < 0 || n_qual < 0 || n_name < 0 || n_mv < 0) { c3b_set_error("c3b_fa_build: bad offsets"); return 1; }
-        if (c3b_upload_records(R, w->in_core, core, n_cigar, n_seq, on_device, s, "c3b_fa")) return 1;
-        const size_t n1 = (size_t)(n + 1) * 8;
-        if (records->qual_off && (c3b_upload(w->in_qoff, records->qual_off, n1, on_device, R.qual_off, s, "c3b_fa") ||
-                                  c3b_upload(w->in_qual, records->qual, (size_t)n_qual, on_device, R.qual, s, "c3b_fa")))
-            return 1;
-        if (records->qname_off && (c3b_upload(w->in_noff, records->qname_off, n1, on_device, R.qname_off, s, "c3b_fa") ||
-                                   c3b_upload(w->in_name, records->qname, (size_t)n_name, on_device, R.qname, s, "c3b_fa")))
-            return 1;
-        if (records->mv_off && params->dwell && (c3b_upload(w->in_moff, records->mv_off, n1, on_device, R.mv_off, s, "c3b_fa") ||
-                                                 c3b_upload(w->in_mv, records->mv, (size_t)n_mv * 4, on_device, R.mv, s, "c3b_fa")))
-            return 1;
-    }
-    const char *dref = nullptr;
-    if (c3b_upload(w->in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, dref, s, "c3b_fa")) return 1;
-    w->R = R;
-    w->dref = dref;
-    w->ref_start = ref_start; w->ref_len = ref_len > 0 ? ref_len : 0;
-    w->n_cigar = n_cigar; w->n_seq = n_seq;
+    if (w->intake("c3b_fa_build", &records->core, records, params->dwell != 0, INT_MAX, on_device, ref_seq, ref_start, ref_len)) return 1;
+    const C3bReads &R = w->R;
+    const int64_t n = R.n;
+    const char *dref = w->dref;
     const size_t Kz = (size_t)(n_cand > 0 ? n_cand : 1), Nz = (size_t)(n > 0 ? n : 1);
     auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_fa"); };
     if (grow(w->in_cand, Kz * 8) || grow(w->in_var, (size_t)(n_var > 0 ? n_var : 1) * sizeof(c3b_fa_variant))) return 1;

@@ -530,8 +530,6 @@ __global__ void __launch_bounds__(TILE) plp_cands_kernel(CandArgs A) {
 constexpr int N_COUNTERS = 7, TEXT_WORD = 4;
 
 struct c3b_plp : C3bRegionWorkspace {
-    // inputs (copies of host records)
-    C3bBuf in_core[8], in_ref;
     // scratch
     C3bBuf opx, opy, rend, pmax, rows32, dstats, nquirk, dci, tile_cov, tile_off, tile_cand, tile_coff;
     C3bBuf g_meta, g_read, g_qpos, g_cnt, g_next;
@@ -562,13 +560,6 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     if (!w || !reads || !params) { c3b_set_error("c3b_plp_count: null argument"); return 1; }
     if (end < start) { c3b_set_error("c3b_plp_count: end < start"); return 1; }
     if (end - start > (int64_t)INT_MAX / 32) { c3b_set_error("c3b_plp_count: region of %lld columns is too large for one call", (long long)(end - start)); return 1; }
-    const int64_t n = reads->n_reads;
-    if (n < 0 || n >= (int64_t)UINT_MAX) { c3b_set_error("c3b_plp_count: bad n_reads"); return 1; }
-    if (n > 0 && (!reads->pos || !reads->flag || !reads->mapq || !reads->cigar_off || !reads->cigar || !reads->seq_off || !reads->seq || !reads->l_qseq)) {
-        c3b_set_error("c3b_plp_count: null record array");
-        return 1;
-    }
-    if (ref_len > 0 && !ref_seq) { c3b_set_error("c3b_plp_count: null ref_seq"); return 1; }
     C3B_CUDA(cudaSetDevice(w->device));
     cudaStream_t s = (cudaStream_t)cuda_stream;
     w->stream = s;
@@ -579,22 +570,11 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     w->gvcf = params->gvcf != 0;
     const int tiles = (int)((W + TILE - 1) / TILE);
 
-    // inputs
-    C3bReads R{};
-    R.n = n;
-    int64_t n_cigar = 0, n_seq = 0;
-    if (n > 0) {
-        if (c3b_last_offset(reads->cigar_off, n, on_device, s, &n_cigar) || c3b_last_offset(reads->seq_off, n, on_device, s, &n_seq))
-            return 1;
-        if (n_cigar < 0 || n_seq < 0) { c3b_set_error("c3b_plp_count: negative offsets"); return 1; }
-        if (c3b_upload_records(R, w->in_core, reads, n_cigar, n_seq, on_device, s, "c3b_plp")) return 1;
-    }
-    const char *dref = nullptr;
-    if (c3b_upload(w->in_ref, ref_seq, (size_t)(ref_len > 0 ? ref_len : 0), on_device, dref, s, "c3b_plp")) return 1;
-    w->R = R;
-    w->dref = dref;
-    w->start = start; w->end = end; w->ref_start = ref_start; w->ref_len = ref_len > 0 ? ref_len : 0;
-    w->n_cigar = n_cigar; w->n_seq = n_seq;
+    if (w->intake("c3b_plp_count", reads, nullptr, false, UINT_MAX, on_device, ref_seq, ref_start, ref_len)) return 1;
+    const C3bReads &R = w->R;
+    const int64_t n = R.n, n_cigar = w->n_cigar;
+    const char *dref = w->dref;
+    w->start = start; w->end = end;
 
     // scratch and outputs
     const size_t Wz = (size_t)(W > 0 ? W : 1), Tz = (size_t)(tiles > 0 ? tiles : 1);

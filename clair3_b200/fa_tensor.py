@@ -15,7 +15,9 @@ import numpy as np
 import torch
 
 from ._ffi import CONSTANTS, C3BError, check, ffi, lib
-from .pileup_counts import BamRecords, DeviceBamRecords, _insertion_bytes, _records_struct, _Workspace, khash_iteration_order
+from ._workspace import _Workspace
+from .pileup_counts import khash_iteration_order
+from .records import BamRecords, DeviceBamRecords, insertion_bytes, records_struct
 
 FLANKING = 16                   # shared/param_f.py flankingBaseNum
 NO_OF_POSITIONS = 33
@@ -67,7 +69,7 @@ class FullAlignmentBuilder(_Workspace):
         prm = ffi.new("c3b_fa_params *")
         prm.matrix_depth, prm.need_haplotagging, prm.min_mq = int(matrix_depth), int(bool(need_haplotagging)), int(min_mq)
         prm.dwell, prm.rand_seed, prm.rand_skip = int(bool(dwell)), int(rand_seed) & 0xFFFFFFFF, int(rand_skip)
-        st = _records_struct(rec, optional=True)
+        st = records_struct(rec, optional=True)
         refptr, reflen, ref = self._reference(ref_seq, rec, "build")
         check(lib().c3b_fa_build(self._h, st, int(on_dev), ffi.cast("const int64_t *", cand.ctypes.data), len(cand), var, nv, refptr,
                                  int(ref_start), reflen, prm, self._stream()))
@@ -179,7 +181,7 @@ def format_alt_info(candidate, depth, acgt, ref, ref_start, max_indel_length, me
         length = m & 0x3FFFFFFF
         again[m >> 31] |= bool(m >> 30 & 1)
         if m >> 31:
-            key = _insertion_bytes(rec, r, q, length)
+            key = insertion_bytes(rec, r, q, length)
             ins_keys.append(key)
             ins_cnt[key] = c
         else:
