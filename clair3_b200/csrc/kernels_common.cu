@@ -38,6 +38,7 @@ __global__ void gather_windows_f32_kernel(const T *__restrict__ cols, const int6
 constexpr int HEADS_THREADS = 256;
 constexpr int HEADS_KT = 32;      // k rows of an L5 weight tile staged in shared memory
 constexpr int HEADS_STAGES = 3;   // L5 weight tiles in the shared-memory ring
+constexpr int HEADS_ROWS = 4;     // split-K sums per thread whose partial loads are in flight together
 
 __device__ __forceinline__ void heads_cp16(float *dst_smem, const float *src) {
     const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
@@ -71,24 +72,34 @@ __global__ void __launch_bounds__(HEADS_THREADS) heads_kernel(const float *__res
     // wait of the L5 loop); the 128-long dot products of the Y stage would otherwise wait on L2 once per four terms
     for (int i = tid * 4; i < 128 * hp.out_dim; i += HEADS_THREADS * 4) heads_cp16(wys + i, hp.wy_all + i);
     asm volatile("cp.async.commit_group;" ::: "memory");
-    // a is stored [k][G] so the L5 loop reads the 8 sites of one k with two 16-byte broadcast loads
-    // (all split-K partial loads of a thread are independent: issue them together, then add in a fixed order - a rolled
-    //  loop with a running sum serialises up to 16 L2 round trips per thread)
-#pragma unroll 2
-    for (int i = tid; i < HEADS_G * d4; i += HEADS_THREADS) {
-        const int g = i / d4, k = i - g * d4;              // consecutive threads -> consecutive k: coalesced partial-sum reads
-        float v = 0.f;
-        if (g < g_n) {
+    // a is stored [k][G] so the L5 loop reads the 8 sites of one k with two 16-byte broadcast loads.  Each thread issues the
+    // split-K partial loads of HEADS_ROWS elements together and only then adds them, each element in a fixed order: one L2
+    // round trip per HEADS_ROWS elements instead of one per element.
+    for (int i0 = tid; i0 < HEADS_G * d4; i0 += HEADS_ROWS * HEADS_THREADS) {
+        float part[HEADS_ROWS][16];
+#pragma unroll
+        for (int r = 0; r < HEADS_ROWS; ++r) {
+            const int i = i0 + r * HEADS_THREADS;
+            const int g = i / d4, k = i - g * d4;          // consecutive threads -> consecutive k: coalesced partial-sum reads
+            const bool live = i < HEADS_G * d4 && g < g_n;
             const float *zp = z4 + (b0 + g) * d4 + k;
-            float part[16];
 #pragma unroll
-            for (int sp = 0; sp < 16; ++sp) part[sp] = sp < nsplit ? __ldg(zp + (size_t)sp * split_stride) : 0.f;
-            v = __ldg(hp.b4 + k);
-#pragma unroll
-            for (int sp = 0; sp < 16; ++sp) v += part[sp];                                          // split-K partials, fixed order
-            v = selu(v);
+            for (int sp = 0; sp < 16; ++sp) part[r][sp] = live && sp < nsplit ? __ldg(zp + (size_t)sp * split_stride) : 0.f;
         }
-        a[k * HEADS_G + g] = v;
+#pragma unroll
+        for (int r = 0; r < HEADS_ROWS; ++r) {
+            const int i = i0 + r * HEADS_THREADS;
+            if (i >= HEADS_G * d4) break;
+            const int g = i / d4, k = i - g * d4;
+            float v = 0.f;
+            if (g < g_n) {
+                v = __ldg(hp.b4 + k);
+#pragma unroll
+                for (int sp = 0; sp < 16; ++sp) v += part[r][sp];                                   // split-K partials, fixed order
+                v = selu(v);
+            }
+            a[k * HEADS_G + g] = v;
+        }
     }
 
     const int j = tid & 127;

@@ -13,8 +13,11 @@
 //   * the 1280 columns are 5 slabs of 256; a CTA loads its slab (128 KB, the whole K) and the slab's bias once, then walks a
 //     contiguous range of 128-row h1 tiles.  CTA c serves slab c % 5 and tile range c / 5, so the five CTAs that read one h1 tile
 //     run side by side and the later four reads of a tile can be served from L2.
-//   * a producer warp streams the tile-major h1 tiles (one K-half = one contiguous 32 KB run) through a three-stage ring with
-//     full / empty mbarriers; two consumer warpgroups each own 64 rows of the tile and issue 16 wgmma.m64n256k16 per tile.
+//   * a producer warp streams the tile-major h1 tiles through a six-stage ring with full / empty mbarriers.  A stage is one
+//     warpgroup's 64 rows of one K-half (16 KB, sixteen 1 KB runs of the tile), so each stage has one consumer.
+//   * two consumer warpgroups each own 64 rows of every tile and take turns on the tensor pipe (ping-pong): warpgroup 0 issues
+//     its 16 wgmma.m64n256k16 for tile t, then warpgroup 1 issues its 16 for tile t while warpgroup 0 runs tile t's epilogue,
+//     then warpgroup 0 issues tile t+1's while warpgroup 1 stores, and so on.  Two named barriers hand the turn over.
 //   * epilogue: fp32 bias from shared memory, one fp16 rounding, a 4 x 4 word transpose inside each lane quad so that every
 //     lane stores 16 contiguous bytes (a warp store covers 8 rows x 64 bytes).
 // fp16 output: the recurrent kernel adds these pre-gates to its fp32 accumulators.
@@ -26,11 +29,10 @@ namespace {
 constexpr int kSlabCols = 256;                                    // output columns per CTA (wgmma N)
 constexpr int kSlabs = 1280 / kSlabCols;
 constexpr uint32_t kSlabBytes = 32 * kSlabCols * 16;              // [32 k-groups][256 columns][8] fp16 = 128 KB
-constexpr uint32_t kTileBytes = 32 * 128 * 16;                    // h1 tile: [32 k-groups][128 rows][8] fp16 = 64 KB
 constexpr int kStageKG = 16;                                      // k-groups per ring stage (a K-half of a tile)
-constexpr int kParts = 32 / kStageKG;                             // stages per tile
-constexpr int kStages = 3;
-constexpr uint32_t kStageBytes = kStageKG * 128 * 16;
+constexpr int kParts = 32 / kStageKG;                             // stages per warpgroup and tile
+constexpr int kStages = 6;
+constexpr uint32_t kStageBytes = kStageKG * 64 * 16;              // [16 k-groups][64 rows][8] fp16 = 16 KB
 constexpr int kSmem = kSlabBytes + kStages * kStageBytes + kSlabCols * 4;   // 225 KB
 constexpr int kThreads = 288;                                     // consumer warpgroups 0 and 1, producer warp 8
 
@@ -64,13 +66,15 @@ __global__ void __launch_bounds__(kThreads, 1) proj2_kernel(const ProjDev p) {
     if (tid == 0) {
         for (int s = 0; s < kStages; ++s) {
             ptx::mbar_init(&full[s], 1);
-            ptx::mbar_init(&empty[s], 8);             // lane 0 of each consumer warp
+            ptx::mbar_init(&empty[s], 4);             // lane 0 of each warp of the consuming warpgroup
         }
         ptx::mbar_init(&w_bar, 1);
         ptx::fence_barrier_init();
     }
     __syncthreads();
 
+    // ring slot g = 2 * (2 * (t - t0) + wg) + part: tile t's rows 64 wg .. +63, k-groups 16 part .. +15, in the order the two
+    // warpgroups take their turns
     if (wg == 2) {                                    // producer warp: one thread issues every copy
         if (tid == 256) {
             ptx::mbar_arrive_expect_tx(&w_bar, kSlabBytes + kSlabCols * 4);
@@ -79,13 +83,15 @@ __global__ void __launch_bounds__(kThreads, 1) proj2_kernel(const ProjDev p) {
             ptx::bulk_g2s(ptx::smem_u32(bias_s), p.bias + slab * kSlabCols, kSlabCols * 4, &w_bar);
             int g = 0;
             for (int t = t0; t < t1; ++t)
-                for (int part = 0; part < kParts; ++part, ++g) {
-                    const int st = g % kStages;
-                    if (g >= kStages) ptx::mbar_wait(&empty[st], (g / kStages - 1) & 1);
-                    ptx::mbar_arrive_expect_tx(&full[st], kStageBytes);
-                    ptx::bulk_g2s(a_addr + st * kStageBytes, p.h1 + (size_t)t * (kTileBytes / 2) + part * (kStageBytes / 2),
-                                  kStageBytes, &full[st]);
-                }
+                for (int half = 0; half < 2; ++half)
+                    for (int part = 0; part < kParts; ++part, ++g) {
+                        const int st = g % kStages;
+                        if (g >= kStages) ptx::mbar_wait(&empty[st], (g / kStages - 1) & 1);
+                        ptx::mbar_arrive_expect_tx(&full[st], kStageBytes);
+                        const op_t *src = p.h1 + ((size_t)t * 32 + part * kStageKG) * 128 * 8 + half * 64 * 8;
+                        for (int kg = 0; kg < kStageKG; ++kg)          // one 1 KB run per k-group: 64 rows x 16 bytes
+                            ptx::bulk_g2s(a_addr + st * kStageBytes + kg * 1024, src + kg * 128 * 8, 1024, &full[st]);
+                    }
         }
         return;
     }
@@ -93,28 +99,33 @@ __global__ void __launch_bounds__(kThreads, 1) proj2_kernel(const ProjDev p) {
     const int w = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
     ptx::mbar_wait(&w_bar, 0);
     float acc[128];
-    int g = 0;
-    for (int t = t0; t < t1; ++t, g += kParts) {
+    for (int t = t0; t < t1; ++t) {
+        const int g = 2 * (2 * (t - t0) + wg);
+        // take the tensor pipe: warpgroup 0 after warpgroup 1's MMAs of the previous tile, warpgroup 1 after warpgroup 0's of
+        // this tile (barrier 1: warpgroup 0 -> 1, barrier 2: warpgroup 1 -> 0)
+        if (wg == 1) ptx::named_bar_sync(1, 256);
+        else if (t > t0) ptx::named_bar_sync(2, 256);
         ptx::wgmma_fence();
 #pragma unroll
         for (int part = 0; part < kParts; ++part) {
             const int st = (g + part) % kStages;
             ptx::mbar_wait(&full[st], ((g + part) / kStages) & 1);
-            const uint32_t a = a_addr + st * kStageBytes + wg * 64 * 16;
+            const uint32_t a = a_addr + st * kStageBytes;
 #pragma unroll
             for (int ks = 0; ks < kStageKG / 2; ++ks)
-                ptx::wgmma_m64n256k16(acc, ptx::wgmma_desc(a + ks * 2 * 2048, 2048, 128),
+                ptx::wgmma_m64n256k16(acc, ptx::wgmma_desc(a + ks * 2 * 1024, 1024, 128),
                                       ptx::wgmma_desc(w_addr + (part * kStageKG + ks * 2) * (kSlabCols * 16), kSlabCols * 16, 128),
                                       part > 0 || ks > 0);
             ptx::wgmma_commit();
-            if (part > 0) {                                    // the previous stage's MMAs are done: hand it back
-                ptx::wgmma_wait<1>();
-                if (lane == 0) ptx::mbar_arrive(&empty[(g + part - 1) % kStages]);
-            }
         }
+        // every MMA of this tile is issued: hand the turn over (warpgroup 1's last hand-over would have no taker)
+        if (wg == 0) ptx::named_bar_arrive(1, 256);
+        else if (t + 1 < t1) ptx::named_bar_arrive(2, 256);
+        ptx::wgmma_wait<1>();                                  // the first K-half's MMAs are done: hand its stage back
+        if (lane == 0) ptx::mbar_arrive(&empty[g % kStages]);
         ptx::wgmma_wait<0>();
         ptx::fence_operand(acc);
-        if (lane == 0) ptx::mbar_arrive(&empty[(g + kParts - 1) % kStages]);
+        if (lane == 0) ptx::mbar_arrive(&empty[(g + 1) % kStages]);
 
         // acc[4i + 2h + e] = row 16w + lane/4 + 8h, column 8i + 2q + e; after the quad transpose lane q stores columns
         // 32j + 8q .. +7 of both its rows

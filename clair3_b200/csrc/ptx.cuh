@@ -73,6 +73,10 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Arrive on a named barrier without waiting: with bar.sync on the same id, one group signals another.
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ---------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor, K-major, no swizzle ("interleave") canonical layout: 8x8 (16-byte-row) core matrices stored
