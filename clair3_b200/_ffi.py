@@ -18,6 +18,7 @@ DEBUG_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_debu
 PILEUP_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_pileup.h")   # pileup feature counter (SURVEY 8f N4)
 FA_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_fa.h")           # full-alignment tensor builder (N4)
 BAM_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_bam.h")         # BAM reader: BGZF blocks to device records
+CASCADE_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_cascade.h")  # pileup -> full-alignment selection
 LIB_PATH = os.path.join(_HERE, "libclair3b200.so")
 
 ffi = cffi.FFI()
@@ -37,12 +38,15 @@ _dbg_body, _ = _cdef_source(DEBUG_HEADER)
 _plp_body, _ = _cdef_source(PILEUP_HEADER)
 _fa_body, _ = _cdef_source(FA_HEADER)
 _bam_body, _ = _cdef_source(BAM_HEADER)
+_cascade_body, _ = _cdef_source(CASCADE_HEADER)
 ffi.cdef(_body)
 ffi.cdef(_dbg_body)
 ffi.cdef(_plp_body)
 ffi.cdef(_fa_body)
 ffi.cdef(_bam_body)
-DECLARED_FUNCTIONS = sorted(set(re.findall(r"\b(c3b_\w+)\s*\(", _body + _dbg_body + _plp_body + _fa_body + _bam_body)))
+ffi.cdef(_cascade_body)
+DECLARED_FUNCTIONS = sorted(set(re.findall(r"\b(c3b_\w+)\s*\(", _body + _dbg_body + _plp_body + _fa_body + _bam_body +
+                                           _cascade_body)))
 
 _lib = None
 

@@ -150,7 +150,10 @@ class _Workspace(_Handle):
         network is queued.  Returns ``decode.batch_calls``' dict (``chromosome``, ``position``, ``calls``, ``text``, ``ad``,
         ``start``; ``decode.calls_text`` formats it) plus ``Y``, the probabilities, on the device, and for the counter
         ``cand_ok`` uint8 [n_cand].  Every candidate is decoded, as the reference decodes every full-alignment candidate;
-        ``cand_ok == 0``: the reference drops that pileup candidate, ignore its row.  Raises what ``batch_calls`` raises on an
+        ``cand_ok == 0``: the reference drops that pileup candidate, ignore its row.  ``device`` holds the same results where
+        they are on the device, for stream-ordered work that follows (``cascade.select_device``): ``calls``, ``text``,
+        ``decoder_off``, ``position`` and for the counter ``cand_ok``; ``decoder_off``, ``position`` and ``cand_ok`` alias the
+        workspace and are valid until its next count / build / ``alt_text``.  Raises what ``batch_calls`` raises on an
         alt_info string the decoder rejects."""
         from . import decode
         decode._check_config(output_config)
@@ -167,6 +170,8 @@ class _Workspace(_Handle):
         fields = self._call_fields()
         res = decode.calls_result(decode._numpy(out), [ctg_name] * nk, v["position"].cpu().numpy(), v["decoder_off"].cpu().numpy())
         res.update(fields, Y=y)
+        res.setdefault("device", {}).update(calls=out["calls"], text=out["text"], decoder_off=v["decoder_off"],
+                                            position=v["position"])
         return res
 
     def _call_fields(self):

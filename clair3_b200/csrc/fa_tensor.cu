@@ -98,10 +98,12 @@ __device__ __forceinline__ int64_t lower_bound64(const int64_t *a, int64_t lo, i
 __device__ __forceinline__ bool ref_op(uint32_t op) { return op == 0 || op == 2 || op == 3 || op == 7 || op == 8; }
 
 // ---------------------------------------------------------------------------------------------------------------- K1 / K2
-__global__ void fa_flank_count_kernel(const int64_t *__restrict__ cand, int64_t n_cand, int64_t *__restrict__ fstart,
-                                      int64_t *__restrict__ fcnt) {
+// n_dev: with device candidates, the launch covers the capacity and the count is read here; slots past it add nothing to F.
+__global__ void fa_flank_count_kernel(const int64_t *__restrict__ cand, int64_t n_cand, const int64_t *__restrict__ n_dev,
+                                      int64_t *__restrict__ fstart, int64_t *__restrict__ fcnt) {
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_cand) return;
+    if (n_dev && k >= *n_dev) { fcnt[k] = 0; return; }
     const int64_t c = cand[k];
     const int64_t lo = c - FLANK < 0 ? 0 : c - FLANK;
     const int64_t prev_hi = k > 0 ? cand[k - 1] + FLANK : -1;
@@ -111,10 +113,26 @@ __global__ void fa_flank_count_kernel(const int64_t *__restrict__ cand, int64_t 
 }
 
 __global__ void fa_flank_fill_kernel(const int64_t *__restrict__ fstart, const int64_t *__restrict__ fcnt,
-                                     const int64_t *__restrict__ foff, int64_t n_cand, int64_t *__restrict__ F) {
+                                     const int64_t *__restrict__ foff, int64_t n_cand, const int64_t *__restrict__ n_dev,
+                                     int64_t *__restrict__ F) {
     const int64_t k = blockIdx.x;
-    if (k >= n_cand) return;
+    if (k >= n_cand || (n_dev && k >= *n_dev)) return;
     for (int64_t i = threadIdx.x; i < fcnt[k]; i += blockDim.x) F[foff[k] + i] = fstart[k] + i;
+}
+
+// K0 (device candidates): candidates[first .. first + n) into the workspace, n = the device count less first, clipped to
+// [0, cap]; n and the device count go to counters 10 / 11, which the first sizing wait reads.  The host path's checks stay:
+// a position that is negative, at or above 2^31 - 17, or not above its predecessor sets status bit 16.
+__global__ void fa_cand_intake_kernel(const int64_t *__restrict__ cand, const int64_t *__restrict__ n_total, int64_t first,
+                                      int64_t cap, int64_t *__restrict__ out, int64_t *__restrict__ cnt, int *status) {
+    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t n = *n_total - first;
+    n = n < 0 ? 0 : n > cap ? cap : n;
+    if (k == 0) { cnt[10] = n; cnt[11] = *n_total; }
+    if (k >= n) return;
+    const int64_t c = cand[first + k];
+    out[k] = c;
+    if (c < 0 || c >= (int64_t)INT_MAX - FLANK || (k > 0 && c <= cand[first + k - 1])) atomicOr(status, 16);
 }
 
 // ---------------------------------------------------------------------------------------------------------------- K3 / K4
@@ -915,8 +933,9 @@ void glibc_jump_matrices(std::vector<uint32_t> &out) {
 }  // namespace
 
 // Timed stages: 0 the build (c3b_fa_build), 1 the text (c3b_fa_alt_text).  counters: int64 0 nF, 1 n_kept, 2 pool entries,
-// 3 signal entries, 4 draws, 5 status, 6 al_used, 7 the text stage's status, 8 n_text_bytes, 9 n_decoder_bytes.
-constexpr int N_COUNTERS = 10, TEXT_WORD = 7;
+// 3 signal entries, 4 draws, 5 status, 6 al_used, 7 the text stage's status, 8 n_text_bytes, 9 n_decoder_bytes, and with device
+// candidates 10 the build's candidate count, 11 the device count it was cut from.
+constexpr int N_COUNTERS = 12, TEXT_WORD = 7;
 
 struct c3b_fa : C3bRegionWorkspace {
     C3bBuf in_cand, in_var, jump, state0;
@@ -958,25 +977,32 @@ int c3b_fa_create(c3b_fa **out, int device_ordinal) {
 
 static inline unsigned blocks_for(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
-int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const int64_t *candidates, int64_t n_cand,
-                 const c3b_fa_variant *variants, int64_t n_var, const char *ref_seq, int64_t ref_start, int64_t ref_len,
-                 const c3b_fa_params *params, void *cuda_stream) {
-    if (!w || !records || !params) { c3b_set_error("c3b_fa_build: null argument"); return 1; }
+// The build behind both entry points.  Host candidates: candidates[0 .. n_cand).  Device candidates (dcand != nullptr):
+// dcand[first ..] up to n_cand of them, as many as *dn allows; the count is read at the first sizing wait.
+static int fa_build(c3b_fa *w, const char *who, const c3b_fa_records *records, int on_device, const int64_t *candidates,
+                    int64_t n_cand, const int64_t *dcand, const int64_t *dn, int64_t first, int64_t *n_cand_out, int64_t *n_total,
+                    const c3b_fa_variant *variants, int64_t n_var, const char *ref_seq, int64_t ref_start, int64_t ref_len,
+                    const c3b_fa_params *params, void *cuda_stream) {
+    if (!w || !records || !params) { c3b_set_error("%s: null argument", who); return 1; }
     if (params->matrix_depth < 1 || params->matrix_depth > 256) {
-        c3b_set_error("c3b_fa_build: matrix_depth %d outside 1..256", params->matrix_depth);
+        c3b_set_error("%s: matrix_depth %d outside 1..256", who, params->matrix_depth);
         return 1;
     }
-    if (n_cand < 0 || n_cand >= (int64_t)INT_MAX / 33 || (n_cand > 0 && !candidates)) { c3b_set_error("c3b_fa_build: bad candidates"); return 1; }
-    for (int64_t i = 0; i < n_cand; ++i)
-        if (candidates[i] < 0 || candidates[i] >= (int64_t)INT_MAX - FLANK || (i && candidates[i] <= candidates[i - 1])) {
-            c3b_set_error("c3b_fa_build: candidates must be 0-based positions below 2^31 - 17, strictly ascending (index %lld)",
-                          (long long)i);
-            return 1;
-        }
-    if (n_var < 0 || (n_var > 0 && !variants)) { c3b_set_error("c3b_fa_build: bad variants"); return 1; }
+    if (dcand) {
+        if (!dn || first < 0 || n_cand < 0 || n_cand >= (int64_t)INT_MAX / 33) { c3b_set_error("%s: bad candidates", who); return 1; }
+    } else {
+        if (n_cand < 0 || n_cand >= (int64_t)INT_MAX / 33 || (n_cand > 0 && !candidates)) { c3b_set_error("%s: bad candidates", who); return 1; }
+        for (int64_t i = 0; i < n_cand; ++i)
+            if (candidates[i] < 0 || candidates[i] >= (int64_t)INT_MAX - FLANK || (i && candidates[i] <= candidates[i - 1])) {
+                c3b_set_error("%s: candidates must be 0-based positions below 2^31 - 17, strictly ascending (index %lld)", who,
+                              (long long)i);
+                return 1;
+            }
+    }
+    if (n_var < 0 || (n_var > 0 && !variants)) { c3b_set_error("%s: bad variants", who); return 1; }
     for (int64_t i = 1; i < n_var; ++i)
         if (variants[i].position < variants[i - 1].position) {
-            c3b_set_error("c3b_fa_build: variants must be sorted by position (index %lld)", (long long)i);
+            c3b_set_error("%s: variants must be sorted by position (index %lld)", who, (long long)i);
             return 1;
         }
     C3B_CUDA(cudaSetDevice(w->device));
@@ -989,14 +1015,14 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     w->n_kept = 0;
     const int depth = params->matrix_depth;
 
-    if (w->intake("c3b_fa_build", &records->core, records, params->dwell != 0, INT_MAX, on_device, ref_seq, ref_start, ref_len)) return 1;
+    if (w->intake(who, &records->core, records, params->dwell != 0, INT_MAX, on_device, ref_seq, ref_start, ref_len)) return 1;
     const C3bReads &R = w->R;
     const int64_t n = R.n;
     const char *dref = w->dref;
     const size_t Kz = (size_t)(n_cand > 0 ? n_cand : 1), Nz = (size_t)(n > 0 ? n : 1);
     auto grow = [&](C3bBuf &b, size_t bytes) { return b.ensure(bytes, s, "c3b_fa"); };
     if (grow(w->in_cand, Kz * 8) || grow(w->in_var, (size_t)(n_var > 0 ? n_var : 1) * sizeof(c3b_fa_variant))) return 1;
-    if (n_cand) C3B_CUDA(cudaMemcpyAsync(w->in_cand.p, candidates, (size_t)n_cand * 8, cudaMemcpyHostToDevice, s));
+    if (n_cand && !dcand) C3B_CUDA(cudaMemcpyAsync(w->in_cand.p, candidates, (size_t)n_cand * 8, cudaMemcpyHostToDevice, s));
     if (n_var) C3B_CUDA(cudaMemcpyAsync(w->in_var.p, variants, (size_t)n_var * sizeof(c3b_fa_variant), cudaMemcpyHostToDevice, s));
     uint32_t st0[31];
     glibc_state(params->rand_seed, st0);
@@ -1013,7 +1039,7 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
         grow(w->k_pmax, Nz * 8) || grow(w->k_fs, Nz * 8) || grow(w->k_ov, Nz * 4) || grow(w->k_pi, Nz * 8) ||
         grow(w->k_sig, Nz * 8) || grow(w->k_hap, Nz * 4) || grow(w->sig_len, Nz * 8) || grow(w->sig_ex, Nz * 8) ||
         grow(w->ra, Kz * 8) || grow(w->rb, Kz * 8) || grow(w->nsel, Kz * 8) || grow(w->draws, Kz * 8) ||
-        grow(w->draw_off, Kz * 8) || grow(w->matrix, Kz * (size_t)depth * 33 * (size_t)w->C) || grow(w->c_depth, Kz * 4) ||
+        grow(w->draw_off, Kz * 8) || (!dcand && grow(w->matrix, Kz * (size_t)depth * 33 * (size_t)w->C)) || grow(w->c_depth, Kz * 4) ||
         grow(w->c_acgt, Kz * 16) || grow(w->al_off, Kz * 4) || grow(w->al_n, Kz * 4) || grow(w->al_meta, (size_t)C3B_AL_CAP * 4) ||
         grow(w->al_read, (size_t)C3B_AL_CAP * 4) || grow(w->al_qpos, (size_t)C3B_AL_CAP * 4) || grow(w->al_cnt, (size_t)C3B_AL_CAP * 4))
         return 1;
@@ -1028,19 +1054,38 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     K.sig = w->k_sig.as<int64_t>(); K.hap = w->k_hap.as<int32_t>();
     w->launches[0] = 0;
     C3B_CUDA(cudaEventRecord(w->ev[0][0], s));
+    const int64_t *n_dev = nullptr;                 // device candidates: their count, known to the host after the first wait
+    if (dcand) {
+        fa_cand_intake_kernel<<<blocks_for(n_cand > 0 ? n_cand : 1, 256), 256, 0, s>>>(dcand, dn, first, n_cand,
+                                                                                        w->in_cand.as<int64_t>(), cnt, status);
+        w->launches[0] += 1;
+        n_dev = cnt + 10;
+    }
     int64_t nF = 0, n_kept = 0, n_pool = 0, n_sig = 0;
     if (n_cand > 0) {
-        fa_flank_count_kernel<<<blocks_for(n_cand, 256), 256, 0, s>>>(w->in_cand.as<int64_t>(), n_cand, w->fstart.as<int64_t>(),
-                                                                       w->fcnt.as<int64_t>());
+        fa_flank_count_kernel<<<blocks_for(n_cand, 256), 256, 0, s>>>(w->in_cand.as<int64_t>(), n_cand, n_dev,
+                                                                       w->fstart.as<int64_t>(), w->fcnt.as<int64_t>());
         block_scan_sum(w->fcnt.as<int64_t>(), w->foff.as<int64_t>(), n_cand, nullptr, cnt + 0, s);
         fa_flank_fill_kernel<<<(unsigned)n_cand, 64, 0, s>>>(w->fstart.as<int64_t>(), w->fcnt.as<int64_t>(), w->foff.as<int64_t>(),
-                                                             n_cand, w->F.as<int64_t>());
+                                                             n_cand, n_dev, w->F.as<int64_t>());
         w->launches[0] += 3;
-        // the size of F bounds the binary searches of K3 and K11
-        C3B_CUDA(cudaMemcpyAsync(&w->host_counters[0], cnt + 0, 8, cudaMemcpyDeviceToHost, s));
+    }
+    if (n_cand > 0 || dcand) {
+        // the size of F bounds the binary searches of K3 and K11; device candidates: their count sizes everything after
+        C3B_CUDA(cudaMemcpyAsync(&w->host_counters[0], cnt + 0, dcand ? N_COUNTERS * 8 : 8, cudaMemcpyDeviceToHost, s));
         C3B_CUDA(cudaStreamSynchronize(s));
         nF = w->host_counters[0];
-        if (n > 0) {
+        if (dcand) {
+            if ((int)w->host_counters[5] & 16) {
+                c3b_set_error("%s: candidates must be 0-based positions below 2^31 - 17, strictly ascending", who);
+                return 1;
+            }
+            w->n_cand = n_cand = w->host_counters[10];
+            if (n_total) *n_total = w->host_counters[11];
+            // the matrix, the one large per-candidate buffer, for the candidates the build has rather than its capacity
+            if (grow(w->matrix, (size_t)(n_cand > 0 ? n_cand : 1) * (size_t)depth * 33 * (size_t)w->C)) return 1;
+        }
+        if (n > 0 && n_cand > 0) {
             C3B_CUDA(cudaMemsetAsync(w->table.p, 0xff, (size_t)T * 8, s));
             C3B_CUDA(cudaMemsetAsync(w->sig_len.p, 0, Nz * 8, s));
             fa_read_scan_kernel<<<blocks_for(n, 256), 256, 0, s>>>(R, params->min_mq, w->F.as<int64_t>(), nF, w->rend.as<int64_t>(),
@@ -1105,7 +1150,24 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
     C3B_CUDA(cudaGetLastError());
     C3B_CUDA(cudaMemcpyAsync(w->host_counters, cnt, N_COUNTERS * 8, cudaMemcpyDeviceToHost, s));
     w->built = true;
+    if (n_cand_out) *n_cand_out = n_cand;
     return 0;
+}
+
+int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const int64_t *candidates, int64_t n_cand,
+                 const c3b_fa_variant *variants, int64_t n_var, const char *ref_seq, int64_t ref_start, int64_t ref_len,
+                 const c3b_fa_params *params, void *cuda_stream) {
+    return fa_build(w, "c3b_fa_build", records, on_device, candidates, n_cand, nullptr, nullptr, 0, nullptr, nullptr, variants,
+                    n_var, ref_seq, ref_start, ref_len, params, cuda_stream);
+}
+
+int c3b_fa_build_device_candidates(c3b_fa *w, const c3b_fa_records *records, int on_device, const int64_t *candidates,
+                                   const int64_t *n_candidates, int64_t first, int64_t max_cand, const c3b_fa_variant *variants,
+                                   int64_t n_var, const char *ref_seq, int64_t ref_start, int64_t ref_len,
+                                   const c3b_fa_params *params, void *cuda_stream, int64_t *n_cand, int64_t *n_total) {
+    if ((!candidates && max_cand > 0) || !n_candidates) { c3b_set_error("c3b_fa_build_device_candidates: null argument"); return 1; }
+    return fa_build(w, "c3b_fa_build_device_candidates", records, on_device, nullptr, max_cand, candidates, n_candidates, first,
+                    n_cand, n_total, variants, n_var, ref_seq, ref_start, ref_len, params, cuda_stream);
 }
 
 int c3b_fa_sizes(c3b_fa *w, int64_t *n_cand, int64_t *n_kept, int64_t *rand_draws) {

@@ -536,13 +536,14 @@ def calls_result(out, chromosomes, positions, offsets):
 
 def calls_text(res, output_config):
     """The VCF rows of ``batch_calls``' printed calls (QUAL, FILTER and AF formatted here)."""
-    calls, text, ad, start = res["calls"], res["text"], res["ad"], res["start"]
-    rows = []
-    for s in np.nonzero(calls["printed"])[0]:
-        c = calls[s]
-        o, rl, al, na = int(start[s]), int(c["ref_len"]), int(c["alt_len"]), int(c["n_ad"])
-        fields = (GENOTYPES[int(c["genotype"])], text[o:o + rl].tobytes().decode(), text[o + rl:o + rl + al].tobytes().decode(),
-                  int(c["ref_count"]), [int(v) for v in ad[o:o + na]], int(c["support"]))
-        rows.append(row_text(res["chromosome"][s], int(res["position"][s]), int(c["dp"]), c["prob"], bool(c["flags"] & 1), fields,
-                             output_config))
-    return "".join(rows)
+    return "".join(call_row(res, s, output_config) for s in np.nonzero(res["calls"]["printed"])[0])
+
+
+def call_row(res, s, output_config):
+    """The VCF row of ``batch_calls``' printed call ``s``."""
+    c, text, ad = res["calls"][s], res["text"], res["ad"]
+    o, rl, al, na = int(res["start"][s]), int(c["ref_len"]), int(c["alt_len"]), int(c["n_ad"])
+    fields = (GENOTYPES[int(c["genotype"])], text[o:o + rl].tobytes().decode(), text[o + rl:o + rl + al].tobytes().decode(),
+              int(c["ref_count"]), [int(v) for v in ad[o:o + na]], int(c["support"]))
+    return row_text(res["chromosome"][s], int(res["position"][s]), int(c["dp"]), c["prob"], bool(c["flags"] & 1), fields,
+                    output_config)

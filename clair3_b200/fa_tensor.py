@@ -51,32 +51,65 @@ class FullAlignmentBuilder(_Workspace):
         self._keep = None
         self._shape = None
         self._alt = None
+        self._device_count = None
 
     def build(self, records, candidates, ref_seq, ref_start, variants=None, matrix_depth=89, need_haplotagging=True, min_mq=5,
-              max_indel_length=50, dwell=False, rand_seed=1, rand_skip=0):
+              max_indel_length=50, dwell=False, rand_seed=1, rand_skip=0, cand_count=None, cand_first=0, cand_max=None):
         """``calculate_clair3_full_alignment`` (src/clair3_full_alignment_dwell.c:437) on decoded records.  ``candidates``: 0-based
         positions, strictly ascending.  ``ref_seq``: the reference bases from ``ref_start`` (str / bytes, or a uint8 tensor on the
         device with device records).  ``variants``: phased heterozygous SNPs as (position, ref_base, alt_base, genotype 1|2,
         phase_set) sorted by position (``phased_variants_from_vcf``).  ``dwell``: 9 channels, the last from the ``mv`` tag.
         The shuffle of candidates with more than ``matrix_depth`` reads draws from glibc ``rand()`` after ``srand(rand_seed)`` and
-        ``rand_skip`` draws; ``rand_seed=1, rand_skip=0`` is what a fresh process sees (``draws`` in ``sizes()`` chains calls)."""
+        ``rand_skip`` draws; ``rand_seed=1, rand_skip=0`` is what a fresh process sees (``draws`` in ``sizes()`` chains calls).
+
+        Device candidates (``c3b_fa_build_device_candidates``): ``candidates`` an int64 tensor on the builder's device, of which
+        the build takes ``candidates[cand_first:]``, as many as the int64 device scalar ``cand_count`` (default: all of them)
+        leaves after ``cand_first`` and at most ``cand_max`` (default: all).  The count is read at the build's first sizing
+        wait, and ``device_count()`` returns the full device count then.  ``cascade.select_device`` leaves its candidates so."""
         on_dev = isinstance(records, DeviceBamRecords)
         rec = records if on_dev else BamRecords.from_dict(records)
-        cand = np.ascontiguousarray(candidates, dtype=np.int64)
-        if cand.ndim != 1 or (len(cand) and (cand[0] < 0 or (np.diff(cand) <= 0).any())):
-            raise C3BError("build: candidates must be 0-based positions in strictly ascending order")
+        dev_cand = isinstance(candidates, torch.Tensor) and candidates.device.type == "cuda"
+        if dev_cand:
+            if candidates.dtype != torch.int64 or candidates.ndim != 1 or candidates.device != self._device:
+                raise C3BError("build: device candidates must be a 1-D int64 tensor on %s" % self._device)
+            cand = candidates.contiguous()
+            if cand_count is None:
+                cand_count = torch.full((1,), len(cand), dtype=torch.int64, device=self._device)
+            if not (isinstance(cand_count, torch.Tensor) and cand_count.dtype == torch.int64 and cand_count.numel() == 1
+                    and cand_count.device == self._device):
+                raise C3BError("build: cand_count must be one int64 on %s" % self._device)
+            first = int(cand_first)
+            cap = max(0, len(cand) - first) if cand_max is None else min(int(cand_max), max(0, len(cand) - first))
+        else:
+            cand = np.ascontiguousarray(candidates, dtype=np.int64)
+            if cand.ndim != 1 or (len(cand) and (cand[0] < 0 or (np.diff(cand) <= 0).any())):
+                raise C3BError("build: candidates must be 0-based positions in strictly ascending order")
         var, nv = _variant_array(list(variants) if variants is not None else [])
         prm = ffi.new("c3b_fa_params *")
         prm.matrix_depth, prm.need_haplotagging, prm.min_mq = int(matrix_depth), int(bool(need_haplotagging)), int(min_mq)
         prm.dwell, prm.rand_seed, prm.rand_skip = int(bool(dwell)), int(rand_seed) & 0xFFFFFFFF, int(rand_skip)
         st = records_struct(rec, optional=True)
         refptr, reflen, ref = self._reference(ref_seq, rec, "build")
-        check(lib().c3b_fa_build(self._h, st, int(on_dev), ffi.cast("const int64_t *", cand.ctypes.data), len(cand), var, nv, refptr,
-                                 int(ref_start), reflen, prm, self._stream()))
+        if dev_cand:
+            n, total = ffi.new("int64_t *"), ffi.new("int64_t *")
+            check(lib().c3b_fa_build_device_candidates(
+                self._h, st, int(on_dev), ffi.cast("const int64_t *", cand.data_ptr()),
+                ffi.cast("const int64_t *", cand_count.data_ptr()), first, cap, var, nv, refptr, int(ref_start), reflen, prm,
+                self._stream(), n, total))
+            n_cand, self._device_count = int(n[0]), int(total[0])
+        else:
+            check(lib().c3b_fa_build(self._h, st, int(on_dev), ffi.cast("const int64_t *", cand.ctypes.data), len(cand), var, nv,
+                                     refptr, int(ref_start), reflen, prm, self._stream()))
+            n_cand, self._device_count = len(cand), None
         self._keep = (rec, ref, st, cand, var)      # buffers stay alive while the copies / kernels are in flight
-        self._shape = (len(cand), int(matrix_depth), 9 if dwell else 8)
+        self._shape = (n_cand, int(matrix_depth), 9 if dwell else 8)
         self._alt = (None if on_dev else ref, int(ref_start), int(max_indel_length))
         return self
+
+    def device_count(self):
+        """The device count ``cand_count`` held when the last build with device candidates read it (None after a build with host
+        candidates)."""
+        return self._device_count
 
     def sizes(self):
         """(candidates, kept reads, glibc rand() draws consumed)."""
@@ -109,7 +142,7 @@ class FullAlignmentBuilder(_Workspace):
             raise C3BError("alt_info_strings: build() first")
         host_ref, ref_start, max_indel = self._alt
         rec = self._keep[0]
-        if host_ref is None or isinstance(rec, DeviceBamRecords):
+        if host_ref is None or isinstance(rec, DeviceBamRecords) or self._device_count is not None:
             return self.alt_text().alt_text_fetch()["text"]
         n = self._shape[0]
         na = ffi.new("int64_t *")

@@ -12,7 +12,7 @@ import numpy as np
 import torch
 
 from ._ffi import CONSTANTS, C3BError, check, ffi, lib
-from ._workspace import _Workspace
+from ._workspace import _Workspace, _device_view
 from .records import CORE, BamRecords, DeviceBamRecords, insertion_bytes, records_struct
 
 FLANKING = 16                 # shared/param_p.py flankingBaseNum; pileup_flanking_base_num src/clair3_pileup.h:93
@@ -151,10 +151,13 @@ class PileupCounter(_Workspace):
 
     def _call_fields(self):
         """``cand_ok`` uint8 [n_cand]: 0 where the reference drops the candidate; ``call`` decodes it all the same, so ignore its
-        row."""
-        ok = np.zeros(self._sizes[1], np.uint8)
+        row.  ``device``: ``cand_ok`` where the count left it."""
+        nk = self._sizes[1]
+        ok = np.zeros(nk, np.uint8)
         check(lib().c3b_plp_fetch(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.cast("uint8_t *", ok.ctypes.data), ffi.NULL, ffi.NULL))
-        return {"cand_ok": ok}
+        pk = ffi.new("const uint8_t **")
+        check(lib().c3b_plp_device(self._h, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, pk))
+        return {"cand_ok": ok, "device": {"cand_ok": _device_view(int(ffi.cast("uintptr_t", pk[0])), nk, torch.uint8, self._device)}}
 
     def window_bounds(self):
         """int64 [n_cand, 2]: the rows [lo, hi) of each candidate's 33-row window (from ``cand_cols - 16``) that lie in its

@@ -73,6 +73,19 @@ int c3b_fa_build(c3b_fa *w, const c3b_fa_records *records, int on_device, const 
                  const c3b_fa_variant *variants, int64_t n_var, const char *ref_seq, int64_t ref_start, int64_t ref_len,
                  const c3b_fa_params *params, void *cuda_stream);
 
+/* c3b_fa_build with the candidates in device memory, as c3b_cascade_select (clair3_b200_cascade.h) leaves them: the build
+ * takes candidates[first ..], at most max_cand of them and as many as the device count *n_candidates leaves after first.  The
+ * count is read at the build's first sizing wait (which device candidates always take, even with no reads or max_cand = 0, when
+ * candidates may be NULL), so selecting and
+ * building add no host wait between them; the same checks as c3b_fa_build hold (0-based, strictly ascending, below 2^31 - 17)
+ * and are reported at that wait.  On return *n_cand is this build's candidate count and *n_total the device count (either
+ * pointer may be NULL); everything after that wait is as in c3b_fa_build, and the matrix is sized at that wait for the
+ * candidates the build has (the other per-candidate scratch, a few dozen bytes a slot, for max_cand). */
+int c3b_fa_build_device_candidates(c3b_fa *w, const c3b_fa_records *records, int on_device, const int64_t *candidates,
+                                   const int64_t *n_candidates, int64_t first, int64_t max_cand, const c3b_fa_variant *variants,
+                                   int64_t n_var, const char *ref_seq, int64_t ref_start, int64_t ref_len,
+                                   const c3b_fa_params *params, void *cuda_stream, int64_t *n_cand, int64_t *n_total);
+
 /* Waits for the last c3b_fa_build: candidates, reads kept (passed the filters, first of their name, overlapping a candidate
  * window: the reference's read_array) and glibc rand() draws consumed.  Fails if the call overflowed a capacity. */
 int c3b_fa_sizes(c3b_fa *w, int64_t *n_cand, int64_t *n_kept, int64_t *rand_draws);
