@@ -94,13 +94,23 @@ int c3b_last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s
 
 namespace {
 
-struct Blob {
+// One packed weight image, built on the host into the device buffer `dev`: put() appends an array at the next 256-byte boundary
+// and records the pointer that is to address it; upload() copies the image to the device and points each recorded pointer there.
+struct WeightImage {
+    C3bBuf &dev;
     std::vector<uint8_t> data;
-    size_t add(const void *src, size_t bytes) {
-        size_t off = (data.size() + 255) / 256 * 256;
+    std::vector<std::pair<size_t, const void **>> fixes;
+    template <class S, class T> void put(const std::vector<S> &src, const T **dst) {
+        const size_t off = (data.size() + 255) / 256 * 256, bytes = src.size() * sizeof(S);
         data.resize(off + bytes);
-        if (src) memcpy(data.data() + off, src, bytes);
-        return off;
+        memcpy(data.data() + off, src.data(), bytes);
+        fixes.push_back({off, reinterpret_cast<const void **>(dst)});
+    }
+    int upload() {
+        if (dev.ensure((data.size() + 255) / 256 * 256, nullptr, "c3b_finalize")) return 1;
+        C3B_CUDA(cudaMemcpy(dev.p, data.data(), data.size(), cudaMemcpyHostToDevice));
+        for (const auto &f : fixes) *f.second = dev.as<char>() + f.first;
+        return 0;
     }
 };
 
@@ -125,6 +135,21 @@ const int kHeadDims[4] = {21, 3, 33, 33};
 
 int conv_cin(const c3b_model *m, int i) { return i == 0 ? m->channels : kConvCout[i - 1]; }
 
+// The state_dict keys of each layer kind, spelled only here: build_expected declares them and finalize_impl reads them.
+struct LstmKeys { std::string w_ih, w_hh, b_ih, b_hh; };
+LstmKeys lstm_keys(int layer, int dir) {
+    const std::string l = std::string("LSTM") + char('1' + layer) + ".", d = dir ? "_l0_reverse" : "_l0";
+    return {l + "weight_ih" + d, l + "weight_hh" + d, l + "bias_ih" + d, l + "bias_hh" + d};
+}
+struct ConvKeys { std::string w, b, bn_w, bn_b, bn_mean, bn_var, bn_batches; };
+ConvKeys conv_keys(int i) {
+    const std::string c = kConvNames[i][0], n = kConvNames[i][1];
+    return {c + ".weight", c + ".bias", n + ".weight", n + ".bias", n + ".running_mean", n + ".running_var",
+            n + ".num_batches_tracked"};
+}
+struct DenseKeys { std::string w, b; };
+DenseKeys dense_keys(const char *layer) { return {std::string(layer) + ".weight", std::string(layer) + ".bias"}; }
+
 void expect(c3b_model *m, const std::string &key, std::vector<int64_t> shape) {
     m->expected.push_back(key);
     m->expected_shape[key] = shape;
@@ -136,32 +161,33 @@ void build_expected(c3b_model *m) {
         const int inp[2] = {m->channels, 2 * C3B_H1};
         for (int l = 0; l < 2; ++l)
             for (int d = 0; d < 2; ++d) {
-                const std::string sfx = d ? "_l0_reverse" : "_l0";
-                const std::string base = std::string("LSTM") + char('1' + l) + ".";
-                expect(m, base + "weight_ih" + sfx, {4 * hid[l], inp[l]});
-                expect(m, base + "weight_hh" + sfx, {4 * hid[l], hid[l]});
-                expect(m, base + "bias_ih" + sfx, {4 * hid[l]});
-                expect(m, base + "bias_hh" + sfx, {4 * hid[l]});
+                const LstmKeys k = lstm_keys(l, d);
+                expect(m, k.w_ih, {4 * hid[l], inp[l]});
+                expect(m, k.w_hh, {4 * hid[l], hid[l]});
+                expect(m, k.b_ih, {4 * hid[l]});
+                expect(m, k.b_hh, {4 * hid[l]});
             }
     } else {
         for (int i = 0; i < 9; ++i) {
-            const std::string c = kConvNames[i][0], b = kConvNames[i][1];
-            expect(m, c + ".weight", {kConvCout[i], conv_cin(m, i), 3, 3});
-            expect(m, c + ".bias", {kConvCout[i]});
-            expect(m, b + ".weight", {kConvCout[i]});
-            expect(m, b + ".bias", {kConvCout[i]});
-            expect(m, b + ".running_mean", {kConvCout[i]});
-            expect(m, b + ".running_var", {kConvCout[i]});
-            expect(m, b + ".num_batches_tracked", {});
+            const ConvKeys k = conv_keys(i);
+            expect(m, k.w, {kConvCout[i], conv_cin(m, i), 3, 3});
+            expect(m, k.b, {kConvCout[i]});
+            expect(m, k.bn_w, {kConvCout[i]});
+            expect(m, k.bn_b, {kConvCout[i]});
+            expect(m, k.bn_mean, {kConvCout[i]});
+            expect(m, k.bn_var, {kConvCout[i]});
+            expect(m, k.bn_batches, {});
         }
     }
-    expect(m, "L4.weight", {m->d4, m->l4_in});
-    expect(m, "L4.bias", {m->d4});
+    const DenseKeys l4 = dense_keys("L4");
+    expect(m, l4.w, {m->d4, m->l4_in});
+    expect(m, l4.b, {m->d4});
     for (int h = 0; h < m->nheads; ++h) {
-        expect(m, std::string(kHeadNames[h][0]) + ".weight", {128, m->d4});
-        expect(m, std::string(kHeadNames[h][0]) + ".bias", {128});
-        expect(m, std::string(kHeadNames[h][1]) + ".weight", {kHeadDims[h], 128});
-        expect(m, std::string(kHeadNames[h][1]) + ".bias", {kHeadDims[h]});
+        const DenseKeys l5 = dense_keys(kHeadNames[h][0]), y = dense_keys(kHeadNames[h][1]);
+        expect(m, l5.w, {128, m->d4});
+        expect(m, l5.b, {128});
+        expect(m, y.w, {kHeadDims[h], 128});
+        expect(m, y.b, {kHeadDims[h]});
     }
 }
 
@@ -302,56 +328,47 @@ static int finalize_impl(c3b_model *m) {
         if (!m->params.count(k)) { c3b_set_error("Missing key in state_dict: \"%s\"", k.c_str()); return 1; }
     C3B_CUDA(cudaSetDevice(m->device));
 
-    Blob blob, fb;
-    struct Fix { size_t off; const void **dst; bool f32blob; };
-    std::vector<Fix> fixes;
-    auto put = [&](Blob &b, const void *src, size_t bytes, const void **dst, bool f32b) {
-        fixes.push_back({b.add(src, bytes), dst, f32b});
-    };
+    // image 0: everything the tensor-core forward reads; image 1: what only the fp32 path reads
+    WeightImage tc{m->blob}, f32{m->f32blob};
 
-    // ---- dense heads of the fp32 debug path: transposed for coalesced reads
+    // ---- dense heads, read by both paths: L5 transposed for coalesced reads, every head's Y weights side by side
     m->heads = HeadsParams();
     m->heads.nheads = m->nheads;
     m->heads.d4 = m->d4;
     m->heads.out_dim = m->out_dim;
-    put(fb, P(m, "L4.bias").data(), (size_t)m->d4 * 4, (const void **)&m->heads.b4, true);
+    const DenseKeys l4 = dense_keys("L4");
+    tc.put(P(m, l4.b), &m->heads.b4);
     int off = 0;
     std::vector<float> wy_all((size_t)128 * m->out_dim);
     for (int h = 0; h < m->nheads; ++h) {
-        const std::vector<float> &w5 = P(m, std::string(kHeadNames[h][0]) + ".weight");   // [128][d4]
-        const std::vector<float> &wy = P(m, std::string(kHeadNames[h][1]) + ".weight");   // [n][128]
+        const DenseKeys l5 = dense_keys(kHeadNames[h][0]), y = dense_keys(kHeadNames[h][1]);
+        const std::vector<float> &w5 = P(m, l5.w);   // [128][d4]
+        const std::vector<float> &wy = P(m, y.w);    // [n][128]
         const int n = kHeadDims[h];
-        std::vector<float> w5t((size_t)m->d4 * 128), wyt((size_t)128 * n);
+        std::vector<float> w5t((size_t)m->d4 * 128);
         for (int j = 0; j < 128; ++j)
             for (int k = 0; k < m->d4; ++k) w5t[(size_t)k * 128 + j] = w5[(size_t)j * m->d4 + k];
         for (int o = 0; o < n; ++o)
-            for (int j = 0; j < 128; ++j) {
-                wyt[(size_t)j * n + o] = wy[(size_t)o * 128 + j];
-                wy_all[(size_t)j * m->out_dim + off + o] = wy[(size_t)o * 128 + j];
-            }
-        put(fb, w5t.data(), w5t.size() * 4, (const void **)&m->heads.h[h].w5t, true);
-        put(fb, P(m, std::string(kHeadNames[h][0]) + ".bias").data(), 128 * 4, (const void **)&m->heads.h[h].b5, true);
-        put(fb, wyt.data(), wyt.size() * 4, (const void **)&m->heads.h[h].wyt, true);
-        put(fb, P(m, std::string(kHeadNames[h][1]) + ".bias").data(), (size_t)n * 4, (const void **)&m->heads.h[h].by, true);
+            for (int j = 0; j < 128; ++j) wy_all[(size_t)j * m->out_dim + off + o] = wy[(size_t)o * 128 + j];
+        tc.put(w5t, &m->heads.h[h].w5t);
+        tc.put(P(m, l5.b), &m->heads.h[h].b5);
+        tc.put(P(m, y.b), &m->heads.h[h].by);
         m->heads.h[h].n = n;
         m->heads.h[h].out_off = off;
         off += n;
     }
-    put(fb, wy_all.data(), wy_all.size() * 4, (const void **)&m->heads.wy_all, true);
+    tc.put(wy_all, &m->heads.wy_all);
 
-    // ---- L4 + heads: fp32 transposed (debug) + tensor-core operand images of the fused tail
+    // ---- L4: fp32 transposed + tensor-core operand image
     {
-        const std::vector<float> &w4 = P(m, "L4.weight");   // [d4][l4_in]
+        const std::vector<float> &w4 = P(m, l4.w);   // [d4][l4_in]
         std::vector<float> w4t((size_t)m->l4_in * m->d4);
         for (int o = 0; o < m->d4; ++o)
             for (int k = 0; k < m->l4_in; ++k) w4t[(size_t)k * m->d4 + o] = w4[(size_t)o * m->l4_in + k];
-        put(fb, w4t.data(), w4t.size() * 4, (const void **)&m->l4_f32_t, true);
+        f32.put(w4t, &m->l4_f32_t);
         // tensor-core L4 (tail_tc.cu): the B operand of a sites-on-rows GEMM, one contiguous piece per 64-wide k-chunk
-        const int kg = m->l4_in / 8;
         const int l4_in = m->l4_in, d4 = m->d4;
-        m->tail = TailW();
-        std::vector<uint16_t> img = pack_operand(d4, kg, d4, [&](int r, int k) { return w4[(size_t)r * l4_in + k]; });
-        put(blob, img.data(), img.size() * 2, (const void **)&m->tail.w4, false);
+        tc.put(pack_operand(d4, l4_in / 8, d4, [&](int r, int k) { return w4[(size_t)r * l4_in + k]; }), &m->l4_tc);
     }
 
     if (m->kind == C3B_PILEUP) {
@@ -360,10 +377,8 @@ static int finalize_impl(c3b_model *m) {
         // fp32 debug weights: transposed [K][4H], summed bias
         for (int l = 0; l < 2; ++l)
             for (int d = 0; d < 2; ++d) {
-                const std::string sfx = d ? "_l0_reverse" : "_l0";
-                const std::string base = std::string("LSTM") + char('1' + l) + ".";
-                const std::vector<float> &wih = P(m, base + "weight_ih" + sfx), &whh = P(m, base + "weight_hh" + sfx);
-                const std::vector<float> &bih = P(m, base + "bias_ih" + sfx), &bhh = P(m, base + "bias_hh" + sfx);
+                const LstmKeys key = lstm_keys(l, d);
+                const std::vector<float> &wih = P(m, key.w_ih), &whh = P(m, key.w_hh), &bih = P(m, key.b_ih), &bhh = P(m, key.b_hh);
                 const int H = hid[l], I = inp[l], G = 4 * H;
                 std::vector<float> wih_t((size_t)I * G), whh_t((size_t)H * G), bias(G);
                 for (int r = 0; r < G; ++r) {
@@ -371,9 +386,9 @@ static int finalize_impl(c3b_model *m) {
                     for (int k = 0; k < H; ++k) whh_t[(size_t)k * G + r] = whh[(size_t)r * H + k];
                     bias[r] = bih[r] + bhh[r];
                 }
-                put(fb, wih_t.data(), wih_t.size() * 4, (const void **)&m->lstm_f32[l][d].wih_t, true);
-                put(fb, whh_t.data(), whh_t.size() * 4, (const void **)&m->lstm_f32[l][d].whh_t, true);
-                put(fb, bias.data(), bias.size() * 4, (const void **)&m->lstm_f32[l][d].bias, true);
+                f32.put(wih_t, &m->lstm_f32[l][d].wih_t);
+                f32.put(whh_t, &m->lstm_f32[l][d].whh_t);
+                f32.put(bias, &m->lstm_f32[l][d].bias);
             }
         // tensor-core LSTM1 image: [dir][8 blocks][22 kgroups][64][8], rows in c3b_lstm_row order; K = [x columns (48) ; h (128)]
         // with the x columns [hi(x) (I) | 1 | lo(x) (I) | 0..]: W_ih multiplies both halves of the hi/lo split of the raw counts, the
@@ -382,9 +397,8 @@ static int finalize_impl(c3b_model *m) {
             const int KX = C3B_X1_COLS, KG = (KX + 128) / 8;
             std::vector<uint16_t> img((size_t)2 * 512 * KG * 8, 0);
             for (int d = 0; d < 2; ++d) {
-                const std::string sfx = d ? "_l0_reverse" : "_l0";
-                const std::vector<float> &wih = P(m, "LSTM1.weight_ih" + sfx), &whh = P(m, "LSTM1.weight_hh" + sfx);
-                const std::vector<float> &bih = P(m, "LSTM1.bias_ih" + sfx), &bhh = P(m, "LSTM1.bias_hh" + sfx);
+                const LstmKeys key = lstm_keys(0, d);
+                const std::vector<float> &wih = P(m, key.w_ih), &whh = P(m, key.w_hh), &bih = P(m, key.b_ih), &bhh = P(m, key.b_hh);
                 const int I = m->channels;
                 for (int R = 0; R < 512; ++R) {
                     const int row = c3b_lstm_row(R, C3B_H1);
@@ -400,8 +414,7 @@ static int finalize_impl(c3b_model *m) {
                     }
                 }
             }
-            put(blob, img.data(), img.size() * 2, (const void **)&m->lstm_tc[0][0].w_img, false);
-            m->lstm_tc[0][0].bias = nullptr;
+            tc.put(img, &m->lstm_tc[0]);
         }
         // tensor-core LSTM2: recurrent image [dir][10 blocks][20][64][8] (c3b_lstm_row order) + input projection GEMM (1280 columns,
         // gate-quad order c3b_lstm2_pg_row per direction, bias folded into the projection)
@@ -410,10 +423,9 @@ static int finalize_impl(c3b_model *m) {
             std::vector<float> pbias(1280);
             const std::vector<float> *wih_d[2];
             for (int d = 0; d < 2; ++d) {
-                const std::string sfx = d ? "_l0_reverse" : "_l0";
-                const std::vector<float> &whh = P(m, "LSTM2.weight_hh" + sfx);
-                const std::vector<float> &bih = P(m, "LSTM2.bias_ih" + sfx), &bhh = P(m, "LSTM2.bias_hh" + sfx);
-                wih_d[d] = &P(m, "LSTM2.weight_ih" + sfx);
+                const LstmKeys key = lstm_keys(1, d);
+                const std::vector<float> &whh = P(m, key.w_hh), &bih = P(m, key.b_ih), &bhh = P(m, key.b_hh);
+                wih_d[d] = &P(m, key.w_ih);
                 for (int R = 0; R < 640; ++R) {
                     const int row = c3b_lstm_row(R, C3B_H2);
                     const float gs = (row / C3B_H2 == 2) ? 1.0f : 0.5f;      // pre-halved sigmoid gates
@@ -425,8 +437,7 @@ static int finalize_impl(c3b_model *m) {
                     pbias[(size_t)d * 640 + C] = (bih[row] + bhh[row]) * ((row / C3B_H2 == 2) ? 1.0f : 0.5f);
                 }
             }
-            put(blob, img.data(), img.size() * 2, (const void **)&m->lstm_tc[1][0].w_img, false);
-            m->lstm_tc[1][0].bias = nullptr;
+            tc.put(img, &m->lstm_tc[1]);
             // one 256-column weight slab per CTA of the projection kernel (proj_tc.cu): [chunk 4][slab 5][8 kg][256 rows][8]
             std::vector<uint16_t> pimg = pack_operand(1280, 32, 256, [&](int C, int k) {
                 const int row = c3b_lstm2_pg_row(C % 640);
@@ -436,15 +447,14 @@ static int finalize_impl(c3b_model *m) {
             m->proj2.n = 1280;
             m->proj2.kgroups = 32;
             m->proj2.nchunks = 4;
-            put(blob, pimg.data(), pimg.size() * 2, (const void **)&m->proj2.w_img, false);
-            put(blob, pbias.data(), pbias.size() * 4, (const void **)&m->proj2.bias, false);
+            tc.put(pimg, &m->proj2.w_img);
+            tc.put(pbias, &m->proj2.bias);
         }
     } else {
         for (int i = 0; i < 9; ++i) {
-            const std::string c = kConvNames[i][0], b = kConvNames[i][1];
-            const std::vector<float> &w = P(m, c + ".weight"), &cb = P(m, c + ".bias");
-            const std::vector<float> &g = P(m, b + ".weight"), &be = P(m, b + ".bias");
-            const std::vector<float> &mu = P(m, b + ".running_mean"), &var = P(m, b + ".running_var");
+            const ConvKeys key = conv_keys(i);
+            const std::vector<float> &w = P(m, key.w), &cb = P(m, key.b), &g = P(m, key.bn_w), &be = P(m, key.bn_b);
+            const std::vector<float> &mu = P(m, key.bn_mean), &var = P(m, key.bn_var);
             const int cout = kConvCout[i], cin = conv_cin(m, i);
             const float in_scale = (i == 0) ? 1.0f / 100.0f : 1.0f;      // x.float()/NORMALIZE_NUM (clair3/model.py:378)
             std::vector<float> wf((size_t)9 * cin * cout), bf(cout);
@@ -458,8 +468,8 @@ static int finalize_impl(c3b_model *m) {
             m->conv_f32[i].cin = cin;
             m->conv_f32[i].cout = cout;
             m->conv_f32[i].stride = kConvStride[i];
-            put(fb, wf.data(), wf.size() * 4, (const void **)&m->conv_f32[i].w, true);
-            put(fb, bf.data(), bf.size() * 4, (const void **)&m->conv_f32[i].bias, true);
+            f32.put(wf, &m->conv_f32[i].w);
+            f32.put(bf, &m->conv_f32[i].bias);
             // tensor-core image: k = tap*cin_pad + ci; conv1's input channels are padded to one wgmma k-step (16)
             const int cin_pad = (i == 0) ? 16 : cin;
             const int kg = 9 * cin_pad / 8;
@@ -471,19 +481,12 @@ static int finalize_impl(c3b_model *m) {
             m->conv_tc[i].n = cout;
             m->conv_tc[i].kgroups = kg;
             m->conv_tc[i].nchunks = (kg + 7) / 8;
-            put(blob, img.data(), img.size() * 2, (const void **)&m->conv_tc[i].w_img, false);
-            put(blob, bf.data(), bf.size() * 4, (const void **)&m->conv_tc[i].bias, false);
+            tc.put(img, &m->conv_tc[i].w_img);
+            tc.put(bf, &m->conv_tc[i].bias);
         }
     }
 
-    if (m->blob.ensure((blob.data.size() + 255) / 256 * 256, nullptr, "c3b_finalize") ||
-        m->f32blob.ensure((fb.data.size() + 255) / 256 * 256, nullptr, "c3b_finalize"))
-        return 1;
-    C3B_CUDA(cudaMemcpy(m->blob.p, blob.data.data(), blob.data.size(), cudaMemcpyHostToDevice));
-    C3B_CUDA(cudaMemcpy(m->f32blob.p, fb.data.data(), fb.data.size(), cudaMemcpyHostToDevice));
-    for (const Fix &f : fixes) *f.dst = (f.f32blob ? m->f32blob : m->blob).as<char>() + f.off;
-    m->lstm_tc[0][1] = m->lstm_tc[0][0];
-    m->lstm_tc[1][1] = m->lstm_tc[1][0];
+    if (tc.upload() || f32.upload()) return 1;
     m->finalized = true;
     return 0;
 }
@@ -500,7 +503,7 @@ extern "C" int c3b_finalize(c3b_model *m) {
 
 extern "C" int c3b_weight_blob(c3b_model *m, int which, void **device_ptr, size_t *bytes) {
     if (!m || !m->finalized) { c3b_set_error("c3b_weight_blob: model not finalized"); return 1; }
-    if (which != 0 && which != 1) { c3b_set_error("c3b_weight_blob: image %d (0 = tensor-core operands + heads, 1 = fp32 debug weights)", which); return 1; }
+    if (which != 0 && which != 1) { c3b_set_error("c3b_weight_blob: image %d (0 = tensor-core forward, 1 = fp32-path-only weights)", which); return 1; }
     const C3bBuf &b = which ? m->f32blob : m->blob;
     if (device_ptr) *device_ptr = b.p;
     if (bytes) *bytes = b.cap;
@@ -522,8 +525,8 @@ extern "C" int c3b_bcast_weights(c3b_model *m, void *nccl_comm, int root, void *
         if (!fn) { c3b_set_error("c3b_bcast_weights: ncclBroadcast not found"); return 1; }
     }
     C3B_CUDA(cudaSetDevice(m->device));
-    // both packed images travel: the tensor-core operands / head weights and the fp32 debug weights, so every option keeps
-    // working on the receiving ranks
+    // both packed images travel: image 0 is all the tensor-core forward reads and image 1 adds what the fp32 path reads, so every
+    // option keeps working on the receiving ranks
     int rc = fn(m->blob.p, m->blob.p, m->blob.cap, /*ncclUint8*/ 1, root, nccl_comm, (cudaStream_t)cuda_stream);
     if (rc == 0) rc = fn(m->f32blob.p, m->f32blob.p, m->f32blob.cap, /*ncclUint8*/ 1, root, nccl_comm, (cudaStream_t)cuda_stream);
     if (rc != 0) { c3b_set_error("ncclBroadcast failed with %d", rc); return 1; }
@@ -996,7 +999,6 @@ static int forward_impl(c3b_model *m, const void *x, int x_dtype, int x_on_devic
         if (rc) return rc;
     }
     m->last_batch = std::min(chunk, batch);
-    m->last_depth = depth;
     return st.download(sync_host);
 }
 

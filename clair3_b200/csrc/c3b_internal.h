@@ -427,7 +427,6 @@ struct HostParam {
 struct HeadWeights {
     const float *w5t;   // [D4][128]
     const float *b5;    // [128]
-    const float *wyt;   // [128][n]
     const float *by;    // [n]
     int n;
     int out_off;
@@ -454,26 +453,13 @@ struct ConvF32 {
     int cin, cout, stride;
 };
 
-// ---- tensor-core path packed operands (device pointers into the weight blob) ----
-struct LstmTC {
-    const op_t *w_img;   // wgmma A-operand image: [dir][2H/64 blocks][K/8][64 rows][8] fp16, rows permuted (c3b_lstm_row)
-    const float *bias;            // unused (LSTM1's bias is a weight column against the constant-1 input; LSTM2's rides in the projection)
-};
+// ---- tensor-core path packed operands (device pointers into weight image 0) ----
 struct IgemmW {
     const op_t *w_img;   // wgmma B-operand image per k-chunk: [nchunks][8 kgroups][N rows][8] fp16
     const float *bias;            // [N]
     int n;                        // output columns (Cout / gate rows / dense units)
     int kgroups;                  // K/8 (16-byte k-groups), real
     int nchunks;                  // ceil(kgroups/8)
-};
-
-// dense tail (tail_tc.cu): L4 as a [d4 rows] B-operand image per k-chunk (the heads run on the fp32 HeadsParams weights)
-struct TailW {
-    const op_t *w4;                      // [l4_in/64 chunks][8 kg][d4 rows][8]
-};
-
-struct ConvGeom {
-    int hin, win, cin, hout, wout, cout, stride;
 };
 
 // Zero-padded channel-group-planar feature map [C/8][p][8]: slot(b,h,w) = g + b*s + (h+1)*wp + (w+1)  (see pconv_tc.cu)
@@ -544,24 +530,26 @@ struct c3b_model {
     std::vector<std::string> expected;
     std::map<std::string, std::vector<int64_t>> expected_shape;
 
-    // device weights
-    C3bBuf blob{C3bBuf::exact};      // tensor-core images + shared fp32 head weights (broadcast unit)
-    C3bBuf f32blob{C3bBuf::exact};   // fp32 debug path weights
+    // device weights, the units c3b_weight_blob exposes and c3b_bcast_weights sends: image 0 holds everything the tensor-core
+    // forward reads, image 1 what only the fp32 path reads (the fp32 path reads both)
+    C3bBuf blob{C3bBuf::exact};      // image 0
+    C3bBuf f32blob{C3bBuf::exact};   // image 1
 
-    HeadsParams heads;
-    // fp32 path
+    HeadsParams heads;                 // image 0, read by both paths
+    // fp32 path, image 1
     LstmF32 lstm_f32[2][2];
     const float *l4_f32_t = nullptr;   // [l4_in][d4]
     ConvF32 conv_f32[9];
-    // tc path
-    LstmTC lstm_tc[2][2];
+    // tc path, image 0
+    // LSTM1 / LSTM2 wgmma A-operand image, both directions: [dir][2H/64 blocks][K/8][64 rows][8] fp16, rows permuted
+    // (c3b_lstm_row).  LSTM1's bias is a weight column against the constant-1 input; LSTM2's rides in the projection.
+    const op_t *lstm_tc[2] = {};
     IgemmW proj2;                      // LSTM2 input projection, both directions: N = 1280 (column order c3b_lstm2_pg_row)
-    TailW tail;                        // L4 on the tensor cores
+    const op_t *l4_tc = nullptr;       // L4 B-operand image (tail_tc.cu): [l4_in/64 chunks][8 kg][d4 rows][8]
     IgemmW conv_tc[9];
 
     std::vector<Workspace *> ws;
     int64_t launches = 0;
-    int last_depth = 0;
     int64_t last_batch = 0;
 };
 

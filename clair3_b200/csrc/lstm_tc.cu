@@ -401,7 +401,7 @@ int c3b_launch_ingest_pileup_tc(const void *x, int dtype, int channels, const in
 // `tile` = sites per warpgroup sub-tile.
 int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s) {
     LstmDev p = {};
-    p.w_img = m->lstm_tc[0][0].w_img;     // both directions are contiguous
+    p.w_img = m->lstm_tc[0];
     p.xs = b.xs;
     p.hout = b.h1;
     p.trace = m->lstm_trace;
@@ -418,7 +418,7 @@ int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t ba
 
 int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s) {
     LstmDev p = {};
-    p.w_img = m->lstm_tc[1][0].w_img;
+    p.w_img = m->lstm_tc[1];
     p.pg = b.pg;
     p.hout = b.h2;
     p.trace = m->lstm_trace ? m->lstm_trace + C3B_T * 4 : nullptr;

@@ -127,7 +127,7 @@ int launch_l4(const L4Dev &p, int tiles, int nsplit, cudaStream_t s) {
 int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, float *out, float *z4, int *nsplit_out, cudaStream_t s) {
     L4Dev p;
     p.act = act;
-    p.w4 = m->tail.w4;
+    p.w4 = m->l4_tc;
     p.z4 = z4;
     p.kg = m->l4_in / 8;
     p.bp = bp;

@@ -458,7 +458,8 @@ class _C3BModule:
 
     def weight_blob(self, which=0):
         """(device_ptr, nbytes) of a packed weight image (the broadcast units of clair3_b200.sharding):
-        0 = fp16 tensor-core operand images + head weights, 1 = fp32 debug-path weights."""
+        0 = everything the default fp16 tensor-core forward reads (operand images, biases, head weights), 1 = the weights
+        only the fp32 debug path (precision=1) reads.  The fp32 path reads both images."""
         p = ffi.new("void **")
         n = ffi.new("size_t *")
         check(lib().c3b_weight_blob(self._handle, int(which), p, n))

@@ -196,7 +196,8 @@ int c3b_decode_calls(c3b_model *m, const float *y, const uint8_t *ref_base, int6
                      c3b_call *calls, char *text, int64_t *ad, void *cuda_stream);
 
 /* Packed device weight images (what one rank broadcasts to the others at start-up; SURVEY.md 8e).
- * which: 0 = fp16 tensor-core operand images + fp32 head weights, 1 = fp32 debug-path weights. */
+ * which: 0 = everything the default fp16 tensor-core forward reads (operand images, biases, fp32 L4 bias and head weights),
+ * 1 = the weights only the fp32 debug path reads (L4, LSTMs, convolutions).  The fp32 path reads both images. */
 int c3b_weight_blob(c3b_model *m, int which, void **device_ptr, size_t *bytes);
 
 /* One-time ncclBroadcast of both packed weight images from rank `root` over NVLink (libnccl is dlopen'ed; the comm is
