@@ -71,10 +71,62 @@ def _aux_mv(buf, p, e):
     return None
 
 
+_CG_MAX = 1 << 29             # htslib moves a CG tag of fewer words than this
+
+
+def _aux_find(buf, p, e, tag):
+    """(offset, type byte) of the first auxiliary field named ``tag`` in buf[p:e], or None when there is none or the fields
+    before it are malformed (htslib's ``bam_aux_get``)."""
+    while p + 3 <= e:
+        t = buf[p + 2]
+        if buf[p:p + 2] == tag:
+            return p, t
+        if t == ord("B"):
+            if p + 8 > e:
+                return None
+            cnt, = struct.unpack_from("<i", buf, p + 4)
+            q = p + 8 + cnt * _AUX_SIZE.get(buf[p + 3], 4)
+            if cnt < 0 or q > e:
+                return None
+            p = q
+        elif t in (ord("Z"), ord("H")):
+            z = buf.find(b"\0", p + 3, e)
+            if z < 0:
+                return None
+            p = z + 1
+        elif t in _AUX_SIZE:
+            p += 3 + _AUX_SIZE[t]
+        else:
+            return None
+    return None
+
+
+def _cg_cigar(buf, core, c0, aux0, e):
+    """The real CIGAR of a record whose operations did not fit the 16-bit ``n_cigar_op``, or None.  A writer stores such a
+    record's CIGAR as the placeholder ``<l_seq>S<ref_len>N`` and the real one in a ``CG:B,I`` tag (SAM/BAM specification 4.2.2);
+    htslib's ``bam_tag2cigar`` moves it back when the record has a position, its first operation is ``S`` of length l_seq, and the
+    first ``CG`` tag is a ``B,I`` or ``B,i`` array of at least n_cigar_op (and fewer than 2^29) words."""
+    tid, p, _, _, _, n_cig, _, l_seq = core[:8]
+    if n_cig == 0 or tid < 0 or p < 0:
+        return None
+    w0, = struct.unpack_from("<I", buf, c0)
+    if w0 & 15 != 4 or w0 >> 4 != l_seq:
+        return None
+    hit = _aux_find(buf, aux0, e, b"CG")
+    if hit is None or hit[1] != ord("B") or hit[0] + 8 > e or buf[hit[0] + 3] not in (ord("I"), ord("i")):
+        return None
+    cnt, = struct.unpack_from("<I", buf, hit[0] + 4)
+    if cnt < n_cig or cnt >= _CG_MAX or hit[0] + 8 + 4 * cnt > e:
+        return None
+    return np.frombuffer(buf, dtype="<u4", count=cnt, offset=hit[0] + 8)
+
+
 def read_bam(path, ref_name=None, start=None, end=None, with_names=False, fa_fields=False):
     """Alignment records of a coordinate-sorted BAM as the arrays of ``clair3_b200.records.BamRecords`` (plus ``tid``), in
     file order.  ``ref_name`` / ``start`` / ``end`` (0-based, end-exclusive) keep what an indexed fetch of that region returns:
     records of that contig whose alignment overlaps [start, end).  Unmapped-without-position records (refID -1) are skipped.
+    A record of more than 65,535 CIGAR operations, stored as a placeholder CIGAR and a ``CG`` tag, gets its real CIGAR back as
+    htslib reads it (``_cg_cigar``).
     ``fa_fields``: also the fields the full-alignment tensor builder reads (``clair3_b200.fa_tensor``): ``qual`` / ``qual_off``
     (bam_get_qual), ``qname`` / ``qname_off`` (read names without the NUL, concatenated bytes) and ``mv`` / ``mv_off`` (the
     ``mv`` B-array including its leading stride element, any integer subtype widened to int32; an empty range when the record has
@@ -109,10 +161,13 @@ def read_bam(path, ref_name=None, start=None, end=None, with_names=False, fa_fie
             break
         c0 = rec0 + 32 + l_name
         cig = np.frombuffer(buf, dtype="<u4", count=n_cig, offset=c0)
+        cg = _cg_cigar(buf, (tid, p, l_name, mq, _bin, n_cig, fl, l_seq), c0, c0 + 4 * n_cig + (l_seq + 1) // 2 + l_seq, off)
+        s0 = c0 + 4 * n_cig
+        if cg is not None:
+            cig, n_cig = cg, len(cg)
         span = int((cig >> 4)[np.isin(cig & 15, _REF_CONSUMING)].sum()) if n_cig else 0
         if p + max(span, 1) <= lo:
             continue
-        s0 = c0 + 4 * n_cig
         nb = (l_seq + 1) // 2
         pos.append(p)
         flag.append(fl)
@@ -172,7 +227,8 @@ def write_bam(path, rec, refs, tid=0, names=None, header_text=None):
     BGZF-compressed BAM: ``refs`` = [(name, length)].  Without ``rec['qual']`` the qualities are written as 0xFF (absent); read names
     come from ``names``, else ``rec['qname']`` / ``rec['qname_off']``, else ``r<i>``; ``rec['mv']`` / ``rec['mv_off']`` become an
     ``mv:B:c`` tag (``mv:B:i`` when a value does not fit int8) on every record with a non-empty range, as ``read_bam(...,
-    fa_fields=True)`` returns them."""
+    fa_fields=True)`` returns them.  A record of more than 65,535 CIGAR operations is written as htslib writes it: the placeholder
+    CIGAR ``<l_seq>S<ref_len>N`` and the real one in a ``CG:B,I`` tag after the other tags."""
     text = (header_text or "@HD\tVN:1.6\tSO:coordinate\n" + "".join("@SQ\tSN:%s\tLN:%d\n" % r for r in refs)).encode()
     out = bytearray(b"BAM\x01" + struct.pack("<i", len(text)) + text + struct.pack("<i", len(refs)))
     for name, length in refs:
@@ -201,6 +257,9 @@ def write_bam(path, rec, refs, tid=0, names=None, header_text=None):
             aux = b"mvB" + (b"c" if small else b"i") + struct.pack("<i", len(mv)) + mv.astype("<i1" if small else "<i4").tobytes()
         p = int(rec["pos"][i])
         span = int((cig >> 4)[np.isin(cig & 15, _REF_CONSUMING)].sum())
+        if len(cig) > 0xFFFF:                                 # as htslib writes it: the placeholder, and the CIGAR in CG:B,I last
+            aux += b"CGBI" + struct.pack("<I", len(cig)) + cig.tobytes()
+            cig = np.array([l_seq << 4 | 4, span << 4 | 3], dtype="<u4")
         body = _CORE.pack(int(tids[i]), p, len(nm), int(rec["mapq"][i]), _reg2bin(p, p + max(span, 1)), len(cig), int(rec["flag"][i]),
                           l_seq, -1, -1, 0) + nm + cig.tobytes() + seq[:(l_seq + 1) // 2] + qual + aux
         out += struct.pack("<i", len(body)) + body

@@ -22,7 +22,8 @@
 //   B6 bam_offsets      one warp per block: the offset of every record, in file order, and the first record that ends the run
 //                       (a later contig, or pos >= end: read_bam's "stop" conditions), min-reduced.
 //   B7 bam_parse        one thread per record: checks block_size against the fields, applies the filter below the first stop,
-//                       sums the reference span, walks the aux fields for mv (with fa_fields) and writes the kept record's counts.
+//                       walks the aux fields for mv (with fa_fields) and for the CG tag of a placeholder CIGAR (read_bam's
+//                       _cg_cigar), sums the reference span of the real CIGAR and writes the kept record's counts.
 //   B8 block scans      record index, CIGAR words, sequence bytes (and qualities, names, mv values) of each kept record.
 //   B9 bam_scatter      one warp per kept record: every array into the packed outputs.
 //
@@ -63,6 +64,7 @@ constexpr int WARPS = 8;                    // warps per CTA of the per-record w
 constexpr int N_COUNTERS = 12;
 enum ChainError : int { CHAIN_OK = 0, CHAIN_TRUNCATED = 1, CHAIN_SHORT_BLOCK_SIZE = 2 };
 enum RecordError : int { REC_FIELDS = 1, REC_AUX = 2 };
+constexpr uint32_t CG_MAX = 1u << 29;       // htslib's bam_tag2cigar moves a CG tag of fewer words than this
 
 __device__ __forceinline__ uint32_t rd32(const uint8_t *u, int64_t o) {
     return (uint32_t)u[o] | (uint32_t)u[o + 1] << 8 | (uint32_t)u[o + 2] << 16 | (uint32_t)u[o + 3] << 24;
@@ -256,6 +258,7 @@ struct ParseArgs {
     int32_t *keep, *n_cig, *n_seq, *n_qual, *n_name, *n_mv;   // [records + 1], 0 for a record not kept
     int64_t *mv_at;                             // first byte of the kept record's mv values
     uint8_t *mv_type;                           // their B subtype
+    int64_t *cig_src;                           // first byte of the kept record's CIGAR: inline, or its CG tag's words
 };
 
 __device__ __forceinline__ int aux_size(uint8_t t) {
@@ -280,59 +283,79 @@ __global__ void bam_parse_kernel(ParseArgs A) {
         const int64_t need = o + REC_MIN <= A.end_u ? fields_bytes(U, o) : -1;
         if (need < 0 || bs < need || o + 4 + (int64_t)bs > A.end_u) {
             atomicMin(A.err, (unsigned long long)i << 4 | REC_FIELDS);
-        } else if ((unsigned long long)i < stop) {
-            const int32_t ref = (int32_t)rd32(U, o + 4), pos = (int32_t)rd32(U, o + 8);
-            const int l_name = U[o + 12], n_cig = (int)rd16(U, o + 16);
+        } else if ((unsigned long long)i < stop && (int32_t)rd32(U, o + 4) == A.F.tid) {
+            const int32_t pos = (int32_t)rd32(U, o + 8);
+            const int l_name = U[o + 12];
             const int32_t l_seq = (int32_t)rd32(U, o + 20);
-            if (ref == A.F.tid) {
-                const int64_t c0 = o + 36 + l_name;
-                int64_t span = 0;
-                for (int j = 0; j < n_cig; ++j) {
-                    const uint32_t w = rd32(U, c0 + 4ll * j), op = w & 15;
-                    if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) span += w >> 4;
-                }
-                keep = (int64_t)pos + (span > 1 ? span : 1) > A.F.start;
+            int64_t c0 = o + 36 + l_name;
+            int n_cig = (int)rd16(U, o + 16);
+            ns = (l_seq + 1) / 2;
+            // the aux walk: read_bam's _aux_mv with fa_fields (the first "mv" B-array of an integer subtype, widened to int32),
+            // and the first CG tag of a record whose CIGAR is the placeholder <l_seq>S<ref_len>N (read_bam's _cg_cigar)
+            bool want_mv = A.fa_fields != 0;
+            bool want_cg = false;
+            if (n_cig > 0 && pos >= 0) {
+                const uint32_t w0 = rd32(U, c0);
+                want_cg = (w0 & 15) == 4 && w0 >> 4 == (uint32_t)l_seq;
             }
-            if (keep) {
-                nc = n_cig; ns = (l_seq + 1) / 2;
-                if (A.fa_fields) {
-                    nq = l_seq; nn = l_name - 1;
-                    // read_bam's _aux_mv: the first "mv" B-array of an integer subtype, widened to int32
-                    int64_t p = o + 36 + l_name + 4ll * n_cig + ns + l_seq;
-                    const int64_t e = o + 4 + (int64_t)bs;
-                    bool bad = false;
-                    while (p + 3 <= e) {
-                        const uint8_t t = U[p + 2];
-                        if (t == 'B') {
-                            if (p + 8 > e) { bad = true; break; }
-                            const uint8_t sub = U[p + 3];
-                            const int32_t cnt = (int32_t)rd32(U, p + 4);
-                            const int sz = aux_size(sub) ? aux_size(sub) : 4;
-                            if (cnt < 0 || p + 8 + (int64_t)cnt * sz > e) { bad = true; break; }
-                            if (U[p] == 'm' && U[p + 1] == 'v' && sub != 'A' && sub != 'f' && aux_size(sub)) {
-                                nm = cnt;
-                                A.mv_at[i] = p + 8;
-                                A.mv_type[i] = sub;
-                                break;
-                            }
-                            p += 8 + (int64_t)cnt * sz;
-                        } else if (t == 'Z' || t == 'H') {
-                            int64_t z = p + 3;
-                            while (z < e && U[z]) ++z;
-                            if (z >= e) { bad = true; break; }
-                            p = z + 1;
-                        } else if (aux_size(t)) {
-                            p += 3 + aux_size(t);
-                        } else {
-                            bad = true;
-                            break;
+            int64_t p = c0 + 4ll * n_cig + ns + l_seq;
+            const int64_t e = o + 4 + (int64_t)bs;
+            bool bad = false;
+            while ((want_mv || want_cg) && p + 3 <= e) {
+                const uint8_t t = U[p + 2];
+                const bool cg = U[p] == 'C' && U[p + 1] == 'G';
+                if (want_cg && cg) {                        // only the first CG tag counts, whatever its type
+                    want_cg = false;
+                    if (t == 'B' && p + 8 <= e && (U[p + 3] == 'I' || U[p + 3] == 'i')) {
+                        const uint32_t cnt = rd32(U, p + 4);
+                        if (cnt >= (uint32_t)n_cig && cnt < CG_MAX && p + 8 + 4ll * cnt <= e) {
+                            c0 = p + 8;
+                            n_cig = (int)cnt;
                         }
                     }
-                    if (bad) {
-                        atomicMin(A.err, (unsigned long long)i << 4 | REC_AUX);
-                        keep = nc = ns = nq = nn = nm = 0;
-                    }
                 }
+                if (t == 'B') {
+                    if (p + 8 > e) { bad = true; break; }
+                    const uint8_t sub = U[p + 3];
+                    const int32_t cnt = (int32_t)rd32(U, p + 4);
+                    const int sz = aux_size(sub) ? aux_size(sub) : 4;
+                    if (cnt < 0 || p + 8 + (int64_t)cnt * sz > e) { bad = true; break; }
+                    if (want_mv && U[p] == 'm' && U[p + 1] == 'v' && sub != 'A' && sub != 'f' && aux_size(sub)) {
+                        nm = cnt;
+                        A.mv_at[i] = p + 8;
+                        A.mv_type[i] = sub;
+                        want_mv = false;
+                    }
+                    p += 8 + (int64_t)cnt * sz;
+                } else if (t == 'Z' || t == 'H') {
+                    int64_t z = p + 3;
+                    while (z < e && U[z]) ++z;
+                    if (z >= e) { bad = true; break; }
+                    p = z + 1;
+                } else if (aux_size(t)) {
+                    p += 3 + aux_size(t);
+                } else {
+                    bad = true;
+                    break;
+                }
+            }
+            int64_t span = 0;
+            for (int j = 0; j < n_cig; ++j) {
+                const uint32_t w = rd32(U, c0 + 4ll * j), op = w & 15;
+                if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) span += w >> 4;
+            }
+            keep = (int64_t)pos + (span > 1 ? span : 1) > A.F.start;
+            // malformed aux fields are an error only where read_bam's mv walk meets them: in a kept record, before its mv
+            if (keep && bad && want_mv) {
+                atomicMin(A.err, (unsigned long long)i << 4 | REC_AUX);
+                keep = 0;
+            }
+            if (keep) {
+                nc = n_cig;
+                A.cig_src[i] = c0;
+                if (A.fa_fields) { nq = l_seq; nn = l_name - 1; }
+            } else {
+                ns = nm = 0;
             }
         }
     }
@@ -345,7 +368,7 @@ struct ScatterArgs {
     const int64_t *rec_off, *n_rec;
     const int32_t *keep, *n_mv;
     const int64_t *kidx, *cig_at, *seq_at, *qual_at, *name_at, *mv_at_out;   // exclusive scans: where each record goes
-    const int64_t *mv_at;
+    const int64_t *mv_at, *cig_src;
     const uint8_t *mv_type;
     int fa_fields;
     // outputs
@@ -375,10 +398,10 @@ __global__ void __launch_bounds__(WARPS * 32) bam_scatter_kernel(ScatterArgs A) 
     if (!A.keep[i]) return;
     const uint8_t *U = A.U;
     const int64_t o = A.rec_off[i];
-    const int l_name = U[o + 12], n_cig = (int)rd16(U, o + 16);
+    const int l_name = U[o + 12];
     const int32_t l_seq = (int32_t)rd32(U, o + 20);
-    const int64_t c0 = o + 36 + l_name, s0 = c0 + 4ll * n_cig, ns = (l_seq + 1) / 2, q0 = s0 + ns;
-    const int64_t ca = A.cig_at[i], sa = A.seq_at[i];
+    const int64_t s0 = o + 36 + l_name + 4ll * rd16(U, o + 16), ns = (l_seq + 1) / 2, q0 = s0 + ns;
+    const int64_t ca = A.cig_at[i], sa = A.seq_at[i], c0 = A.cig_src[i], n_cig = A.cig_at[i + 1] - ca;
     if (lane == 0) {
         A.pos[k] = (int32_t)rd32(U, o + 8);
         A.mapq[k] = U[o + 13];
@@ -386,7 +409,7 @@ __global__ void __launch_bounds__(WARPS * 32) bam_scatter_kernel(ScatterArgs A) 
         A.l_qseq[k] = l_seq;
         A.cigar_off[k] = ca; A.seq_off[k] = sa;
     }
-    for (int j = lane; j < n_cig; j += 32) A.cigar[ca + j] = rd32(U, c0 + 4ll * j);
+    for (int64_t j = lane; j < n_cig; j += 32) A.cigar[ca + j] = rd32(U, c0 + 4 * j);
     for (int64_t j = lane; j < ns; j += 32) A.seq[sa + j] = U[s0 + j];
     if (!A.fa_fields) return;
     const int64_t qa = A.qual_at[i], na = A.name_at[i], ma = A.mv_at_out[i];
@@ -437,7 +460,7 @@ struct c3b_bam : C3bRegionWorkspace {
     size_t staging_cap = 0;
     cudaEvent_t uploaded = nullptr;              // the staging buffer is free again
     C3bBuf in, U, mark, spec_exit, entry, merge, bcount, bbase, rec_off;
-    C3bBuf keep, c_cig, c_seq, c_qual, c_name, c_mv, mv_at, mv_type;     // per record: kept, and its counts
+    C3bBuf keep, c_cig, c_seq, c_qual, c_name, c_mv, mv_at, mv_type, cig_src;     // per record: kept, its counts, its CIGAR
     C3bBuf kidx, cig_at, seq_at, qual_at, name_at, mvo_at;
     C3bBuf pos, flag, mapq, lq, cig_off, seq_off, qual_off, name_off, mv_off, cigar, seq, qual, name, mv;
     std::vector<Block> blocks;
@@ -556,7 +579,7 @@ int c3b_bam_decode(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t fi
     if (grow(w->in, up) || grow(w->U, (size_t)Uz) || grow(w->mark, (size_t)Uz) || grow(w->spec_exit, nbz * 8) ||
         grow(w->entry, nbz * 8) || grow(w->merge, nbz * 8) || grow(w->bcount, (nbz + 1) * 4) || grow(w->bbase, (nbz + 1) * 8) ||
         grow(w->rec_off, (size_t)cap * 8) || grow(w->keep, c1 * 4) || grow(w->c_cig, c1 * 4) || grow(w->c_seq, c1 * 4) ||
-        grow(w->kidx, c1 * 8) || grow(w->cig_at, c1 * 8) || grow(w->seq_at, c1 * 8) || grow(w->pos, (size_t)cap * 8) ||
+        grow(w->kidx, c1 * 8) || grow(w->cig_src, c1 * 8) || grow(w->cig_at, c1 * 8) || grow(w->seq_at, c1 * 8) || grow(w->pos, (size_t)cap * 8) ||
         grow(w->flag, (size_t)cap * 2) || grow(w->mapq, (size_t)cap) || grow(w->lq, (size_t)cap * 4) || grow(w->cig_off, c1 * 8) ||
         grow(w->seq_off, c1 * 8) || grow(w->cigar, (size_t)Uz) || grow(w->seq, (size_t)Uz))
         return 1;
@@ -595,7 +618,7 @@ int c3b_bam_decode(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t fi
         P.fa_fields = w->fa_fields;
         P.keep = w->keep.as<int32_t>(); P.n_cig = w->c_cig.as<int32_t>(); P.n_seq = w->c_seq.as<int32_t>();
         P.n_qual = w->c_qual.as<int32_t>(); P.n_name = w->c_name.as<int32_t>(); P.n_mv = w->c_mv.as<int32_t>();
-        P.mv_at = w->mv_at.as<int64_t>(); P.mv_type = w->mv_type.as<uint8_t>();
+        P.mv_at = w->mv_at.as<int64_t>(); P.mv_type = w->mv_type.as<uint8_t>(); P.cig_src = w->cig_src.as<int64_t>();
         bam_parse_kernel<<<bam_grid(cap + 1, 256), 256, 0, s>>>(P);
         // record counts: the scans read records + 1 entries (the last is 0) and leave the totals in the counter block
         block_scan_sum(w->keep.as<int32_t>(), w->kidx.as<int64_t>(), cap + 1, cnt + 5, cnt + 6, s);
@@ -612,7 +635,7 @@ int c3b_bam_decode(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t fi
         S.U = U; S.rec_off = w->rec_off.as<int64_t>(); S.n_rec = cnt + 5; S.keep = w->keep.as<int32_t>(); S.n_mv = w->c_mv.as<int32_t>();
         S.kidx = w->kidx.as<int64_t>(); S.cig_at = w->cig_at.as<int64_t>(); S.seq_at = w->seq_at.as<int64_t>();
         S.qual_at = w->qual_at.as<int64_t>(); S.name_at = w->name_at.as<int64_t>(); S.mv_at_out = w->mvo_at.as<int64_t>();
-        S.mv_at = w->mv_at.as<int64_t>(); S.mv_type = w->mv_type.as<uint8_t>(); S.fa_fields = w->fa_fields;
+        S.mv_at = w->mv_at.as<int64_t>(); S.cig_src = w->cig_src.as<int64_t>(); S.mv_type = w->mv_type.as<uint8_t>(); S.fa_fields = w->fa_fields;
         S.pos = w->pos.as<int64_t>(); S.flag = w->flag.as<uint16_t>(); S.mapq = w->mapq.as<uint8_t>(); S.l_qseq = w->lq.as<int32_t>();
         S.cigar_off = w->cig_off.as<int64_t>(); S.seq_off = w->seq_off.as<int64_t>(); S.qual_off = w->qual_off.as<int64_t>();
         S.qname_off = w->name_off.as<int64_t>(); S.mv_off = w->mv_off.as<int64_t>();

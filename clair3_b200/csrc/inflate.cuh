@@ -142,6 +142,7 @@ C3B_HD int inflate(const uint8_t *in, int n_in, uint8_t *out, int cap, int *n_ou
         if (type == 0) {
             b.drop(b.cnt & 7);
             const uint32_t len = b.bits(16), nlen = b.bits(16);
+            if (b.overran()) return INPUT_OVERRUN;
             if (len != (~nlen & 0xffffu)) return BAD_STORED_LENGTH;
             if (o + (int)len > cap) return OUTPUT_OVERFLOW;
             for (uint32_t i = 0; i < len; ++i) out[o++] = (uint8_t)b.bits(8);
@@ -166,7 +167,8 @@ C3B_HD int inflate(const uint8_t *in, int n_in, uint8_t *out, int cap, int *n_ou
             int idx = 0;
             while (idx < nlen + ndist) {
                 const int sym = decode(b, t.lit);
-                if (sym < 0 || b.overran()) return BAD_CODE_LENGTHS;
+                if (b.overran()) return INPUT_OVERRUN;
+                if (sym < 0) return BAD_CODE_LENGTHS;
                 if (sym < 16) {
                     L[idx++] = (uint8_t)sym;
                     continue;
