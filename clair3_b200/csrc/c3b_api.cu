@@ -782,6 +782,7 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
         if (c3b_launch_heads(z4, 1, 0, m->heads, y, n, s)) return 1;
         m->launches += 5;
         if (tap) {
+            taps["lstm1_in"] = {xf, 0, 0, (int64_t)C3B_T * m->channels, 0, {}};
             taps["lstm1"] = {l1, 0, 0, (int64_t)C3B_T * 256, 0, {}};
             taps["lstm2"] = {l2, 0, 0, (int64_t)C3B_T * 320, 0, {}};
             taps["l4_pre"] = {z4, 0, 0, 128, 0, {}};
@@ -846,6 +847,7 @@ static int forward_fa_chunk(c3b_model *m, Workspace *w, const void *x, int x_dty
             for (int l = 0; l < 3; ++l) {
                 const int64_t inner = (int64_t)hh[l + 1] * ww[l + 1] * chans[l + 1];
                 taps[tapname[l][0]] = {c.act32[l][0], 0, 0, inner, 0, {}};
+                taps[tapname[l][2]] = {c.act32[l][1], 0, 0, inner, 0, {}};
                 taps[tapname[l][1]] = {c.act32[l][2], 0, 0, inner, 0, {}};
             }
             taps["spp"] = {sp, 0, 0, 3584, 0, {}};

@@ -17,12 +17,14 @@ extern "C" {
 
 /* Copy an intermediate activation of the most recent forward (option "taps" on; first chunk) to the host as float32.
  * names: pileup "lstm1"[B,33,256] "lstm2"[B,33,320] "l4_pre"[B,128]; full-alignment "conv1" "res_block1" "conv3" "res_block2"
- * "conv5" "res_block3" (NHWC) "spp"[B,3584] "l4_pre"[B,256].  *count_inout: capacity in / elements out.
+ * "conv5" "res_block3" (NHWC) "spp"[B,3584] "l4_pre"[B,256], and "res_block1_mid" "res_block2_mid" "res_block3_mid" (NHWC): the
+ * first convolution inside each residual block.  *count_inout: capacity in / elements out.
  * Tensor-core path only, so that every kernel's input and output can be read:
  *   pileup "lstm1_x"[B,33,48]: LSTM1's input operand, columns [hi(x) (channels) | 1 | lo(x) (channels) | 0..];
  *   pileup "lstm2_pregates"[B,33,1280]: the input projection's fp16 output, column dir*640 + C in gate-quad order
- *     (c3b_lstm2_pg_row), sigmoid gates pre-halved, bias included;
- *   full-alignment "res_block1_mid" "res_block2_mid" "res_block3_mid" (NHWC): the first convolution inside each residual block. */
+ *     (c3b_lstm2_pg_row), sigmoid gates pre-halved, bias included.
+ * fp32 path (precision 1) only:
+ *   pileup "lstm1_in"[B,33,channels]: LSTM1's fp32 input, the (float) cast of the counts the ingest or window gather read. */
 int c3b_get_tap(c3b_model *m, const char *name, float *host_out, int64_t *count_inout);
 
 /* With option "lstm_trace" on, CTA (0,0) of each LSTM kernel stamps clock64 at four points of every step (operands ready,

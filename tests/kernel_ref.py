@@ -1,4 +1,5 @@
-"""Operand-precision float64 references of the tensor-core kernels, one layer at a time.
+"""Operand-precision float64 references of the tensor-core kernels, one layer at a time (and, in the last section, of the fp32
+CUDA-core debug path's kernels).
 
 Every function here computes ONE kernel's output from that kernel's own inputs as the GPU saw them (its input tap), with the
 weights rebuilt from the state dict exactly as ``finalize`` in ``c3b_api.cu`` packs them (fp32 folding, then the fp16 cast).
@@ -81,11 +82,15 @@ def lstm1_x(x):
     return out
 
 
-def windows(cols, starts):
-    """The dense [B,33,C] tensor ``forward_windows`` reads: rows starts[b] .. +32 of the column matrix, zero outside it."""
+def windows(cols, starts, bounds=None):
+    """The dense [B,33,C] tensor ``forward_windows`` reads: rows starts[b] .. +32 of the column matrix, zero outside it and,
+    with bounds [B,2], outside rows [bounds[b,0], bounds[b,1])."""
     cols = np.asarray(cols)
     rows = np.asarray(starts, dtype=np.int64)[:, None] + np.arange(T)[None, :]
     ok = (rows >= 0) & (rows < cols.shape[0])
+    if bounds is not None:
+        bounds = np.asarray(bounds, dtype=np.int64)
+        ok &= (rows >= bounds[:, :1]) & (rows < bounds[:, 1:])
     out = cols[np.clip(rows, 0, cols.shape[0] - 1)]
     out[~ok] = 0
     return out
@@ -154,8 +159,9 @@ def lstm2_weights(sd, d):
     return whh, wp, bp
 
 
-def conv_weights(sd, i):
-    """Convolution i (CONV_KEYS order) with BatchNorm folded in fp32 as finalize does: ([9 taps][cin][cout] fp16, bias fp32)."""
+def _conv_folded(sd, i):
+    """Convolution i (CONV_KEYS order) with BatchNorm (and conv1's 1/100 input scale) folded in fp32 as finalize does:
+    (weights [9 taps][cin][cout] fp32, bias fp32)."""
     conv, bn = CONV_KEYS[i]
     w, cb = _f32(sd, conv + ".weight"), _f32(sd, conv + ".bias")
     g, be = _f32(sd, bn + ".weight"), _f32(sd, bn + ".bias")
@@ -166,7 +172,13 @@ def conv_weights(sd, i):
     if i == 0:
         wf = wf * (np.float32(1.0) / np.float32(100.0))
     cout, cin = w.shape[:2]
-    return f16(wf).transpose(2, 3, 1, 0).reshape(9, cin, cout), bias.astype(np.float64)
+    return wf.transpose(2, 3, 1, 0).reshape(9, cin, cout), bias
+
+
+def conv_weights(sd, i):
+    """Convolution i as the tensor-core path reads it: ([9 taps][cin][cout] fp16, bias fp32)."""
+    w, bias = _conv_folded(sd, i)
+    return f16(w), bias.astype(np.float64)
 
 
 def l4_weights(sd):
@@ -174,15 +186,15 @@ def l4_weights(sd):
 
 
 # ------------------------------------------------------------------------------------------------ checks (max err / bound)
-def bound_ratio(gpu, ref, S, fp16_out):
-    """(max err / bound, max share of the accumulation allowance EPS*S + 2^-24 used once the fp16 output rounding's own
+def bound_ratio(gpu, ref, S, fp16_out, eps=EPS):
+    """(max err / bound, max share of the accumulation allowance eps*S + 2^-24 used once the fp16 output rounding's own
     allowance is taken off).  The first is what the checks assert; for fp16 outputs it can approach 1 by the rounding alone,
-    so the second is what shows how much room EPS leaves."""
+    so the second is what shows how much room eps leaves."""
     if not np.size(ref):
         return 0.0, 0.0
     err = np.abs(np.asarray(gpu, dtype=np.float64) - ref)
     rnd = F16_ULP * np.abs(ref) if fp16_out else 0.0
-    acc = EPS * S + TINY
+    acc = eps * S + TINY
     return float(np.max(err / (acc + rnd))), float(np.max(np.maximum(err - rnd, 0.0) / acc))
 
 
@@ -217,11 +229,12 @@ def proj2_ratio(h1, pg, sd):
     return r
 
 
-def lstm_ratio(u, su, whh, h, reverse, tau):
+def lstm_ratio(u, su, whh, h, reverse, tau, eps=EPS, halved=True):
     """Teacher-forced check of one direction of a recurrence.
 
-    u, su [B,33,4H]: the input part of the (pre-halved) gate pre-activations in torch row order and its S; whh [4H][H] the
-    recurrent operand; h [B,33,H] the GPU's output of this direction.  Returns max |h - ref| / (tau + 2 EPS S_gates)."""
+    u, su [B,33,4H]: the input part of the gate pre-activations in torch row order (sigmoid rows pre-halved unless
+    ``halved`` is False) and its S; whh [4H][H] the recurrent operand; h [B,33,H] the GPU's output of this direction.
+    Returns max |h - ref| / (tau + 2 eps S_gates)."""
     B, _, G = u.shape
     H = G // 4
     hp = np.zeros_like(h, dtype=np.float64)
@@ -232,17 +245,18 @@ def lstm_ratio(u, su, whh, h, reverse, tau):
     z = u + hp @ whh.T
     S = su + np.abs(hp) @ np.abs(whh).T
     sg = S[..., :H] + S[..., H:2 * H] + S[..., 2 * H:3 * H] + S[..., 3 * H:]
+    sig_scale = 1.0 if halved else 0.5      # sigmoid(z) = 0.5 tanh(z / 2) + 0.5
     c = np.zeros((B, H))
     r = 0.0
     for t in (range(T - 1, -1, -1) if reverse else range(T)):
         zt = z[:, t]
-        i = 0.5 * np.tanh(zt[:, :H]) + 0.5
-        f = 0.5 * np.tanh(zt[:, H:2 * H]) + 0.5
+        i = 0.5 * np.tanh(sig_scale * zt[:, :H]) + 0.5
+        f = 0.5 * np.tanh(sig_scale * zt[:, H:2 * H]) + 0.5
         g = np.tanh(zt[:, 2 * H:3 * H])
-        o = 0.5 * np.tanh(zt[:, 3 * H:]) + 0.5
+        o = 0.5 * np.tanh(sig_scale * zt[:, 3 * H:]) + 0.5
         c = f * c + i * g
         ref = o * np.tanh(c)
-        r = max(r, float(np.max(np.abs(h[:, t] - ref) / (tau + 2 * EPS * sg[:, t]))))
+        r = max(r, float(np.max(np.abs(h[:, t] - ref) / (tau + 2 * eps * sg[:, t]))))
     return r
 
 
@@ -320,3 +334,79 @@ def heads(z4, sd, nheads):
 def spp(x):
     """Pyramid pooling (3x3, 2x2, 1x1; TF-'SAME' zero padding, NHWC flatten) of an NHWC map: exact on fp16 values."""
     return pyramid_pool(np.asarray(x, dtype=np.float64).transpose(0, 3, 1, 2))
+
+
+# ------------------------------------------------------------------------------------------------ fp32 CUDA-core path
+# The same checks for ``kernels_fp32.cu``: weights rebuilt as finalize packs image 1 and the shared heads (fp32, no pre-halving,
+# no fp16 rounding; LSTM bias b_ih + b_hh summed in fp32; BN and conv1's 1/100 input scale folded in fp32), every output fp32.
+# * GEMM-type (the nine convolutions, L4): ``|gpu - ref| <= EPS32 * S + 2^-24`` (no output-rounding term).
+# * Recurrences, teacher-forced from the GPU's own fp32 h, standard sigmoid / tanh: ``TAU32 + 2 * EPS32 * S_gates``; TAU32
+#   covers expf / tanhf and the fp32 cell state drifting over 33 steps.
+# * Exact: the ingest / window gather (the (float) cast of the counts) and the pyramid pooling (a max of fp32 values).
+# * Heads: ``heads`` on the fp32 "l4_pre" tap within HEADS_TOL (the same kernel, fed with one split-K partial).
+EPS32 = 2.0 ** -19          # fp32 accumulation error relative to S; K_MAX * EPS32 = 0.02, well below 1/8
+TAU32 = 2.0 ** -16          # recurrences with expf / tanhf gate activations
+
+
+def fp32_input(x):
+    """What the fp32 ingest / window gather writes for raw counts x: the (float) cast, which rounds above 2^24."""
+    return np.asarray(x).astype(np.float32)
+
+
+def lstm32_weights(sd, layer, d):
+    """LSTM{layer+1} of direction d as image 1 holds it, in torch row order: (W_ih [4H][I], W_hh [4H][H], b_ih + b_hh [4H])."""
+    p = "LSTM%d." % (layer + 1)
+    b = _f32(sd, p + "bias_ih" + _sfx(d)) + _f32(sd, p + "bias_hh" + _sfx(d))
+    return (_f32(sd, p + "weight_ih" + _sfx(d)).astype(np.float64), _f32(sd, p + "weight_hh" + _sfx(d)).astype(np.float64),
+            b.astype(np.float64))
+
+
+def lstm32_ratio(x, h, sd, layer, tau=TAU32):
+    """One fp32 recurrence from its input x (layer 0: the "lstm1_in" tap [B,33,C]; layer 1: the "lstm1" tap [B,33,256]) to
+    its output h [B,33,2H] (the "lstm1" / "lstm2" tap).  Returns max |h - ref| / (tau + 2 EPS32 S_gates)."""
+    H = (H1, H2)[layer]
+    x = np.asarray(x, dtype=np.float64)
+    r = 0.0
+    for d in range(2):
+        wih, whh, b = lstm32_weights(sd, layer, d)
+        u, su = x @ wih.T + b, np.abs(x) @ np.abs(wih).T + np.abs(b)
+        r = max(r, lstm_ratio(u, su, whh, h[..., d * H:(d + 1) * H], d == 1, tau, EPS32, halved=False))
+    return r
+
+
+def conv32_weights(sd, i):
+    w, bias = _conv_folded(sd, i)
+    return w.astype(np.float64), bias.astype(np.float64)
+
+
+def im2col_at(x, stride, pix, ho, wo):
+    """Rows of ``im2col(x, stride)`` at the flat output pixels pix (site * ho * wo + row * wo + col) only."""
+    B, h, w, c = x.shape
+    b, rem = np.divmod(np.asarray(pix, dtype=np.int64), ho * wo)
+    i, j = np.divmod(rem, wo)
+    cols = np.zeros((len(b), 9, c))
+    for dh in range(3):
+        for dw in range(3):
+            hi, wi = i * stride - 1 + dh, j * stride - 1 + dw
+            ok = (hi >= 0) & (hi < h) & (wi >= 0) & (wi < w)
+            cols[ok, dh * 3 + dw] = x[b[ok], hi[ok], wi[ok]]
+    return cols.reshape(len(b), 9 * c)
+
+
+def conv32_ratio(x, out, wb, stride, residual=None, pix=None):
+    """One fp32 convolution (+bias, +residual, ReLU) from its NHWC input x to the GPU's NHWC output, at the flat output
+    pixels pix (default: all); wb = conv32_weights(...).  Returns max err / (EPS32 * S + 2^-24)."""
+    w, bias = wb
+    B, h, wd, _ = x.shape
+    ho, wo = (conv_out(h), conv_out(wd)) if stride == 2 else (h, wd)
+    cout = w.shape[2]
+    pix = np.arange(B * ho * wo) if pix is None else np.asarray(pix, dtype=np.int64)
+    res = None if residual is None else np.asarray(residual).reshape(-1, cout)[pix].astype(np.float64)
+    ref, S = gemm(im2col_at(x, stride, pix, ho, wo), w.reshape(-1, cout).T, bias=bias, residual=res, relu=True)
+    return bound_ratio(np.asarray(out).reshape(-1, cout)[pix], ref, S, False, EPS32)[0]
+
+
+def l4_32_ratio(act, z4, sd):
+    """fp32 L4 (no bias) from its [B, l4_in] input.  Returns max err / (EPS32 * S + 2^-24)."""
+    ref, S = gemm(act, _f32(sd, "L4.weight").astype(np.float64))
+    return bound_ratio(z4, ref, S, False, EPS32)[0]

@@ -1,6 +1,7 @@
 """The per-layer checker of ``kernel_ref.py`` on the CPU: it must accept an fp32 emulation of each kernel that carries the
 kernel's own rounding (fp32 accumulation noise, ``tanh.approx`` error, fp16 outputs), and it must reject each of a set of
-one-line kernel mistakes.  Also pins the hi/lo split of LSTM1's raw counts."""
+one-line kernel mistakes.  The same for the fp32 section and the fp32 CUDA-core path: float32 emulations in each kernel's own
+work split pass, one-line mistakes of each fail.  Also pins the hi/lo split of LSTM1's raw counts."""
 import numpy as np
 import pytest
 
@@ -245,3 +246,200 @@ def test_checker_rejects_one_line_mistakes(mutation):
     pg = emu_proj2(sd, h1, r)
     act = emu_lstm2(sd, pg, r).reshape(len(x), -1)
     assert kr.l4_ratio(act, emu_l4(act, sd, r, mutation=mutation), sd)[0] > 1.0
+
+
+# ---------------------------------------------------------------------------------------------- fp32 CUDA-core path
+# float32 emulations of kernels_fp32.cu / the fp32 ingest and window gather, in the kernels' own work split, and one-line
+# mistakes of each that the fp32 checks must reject.
+F32 = np.float32
+
+
+def emu32_input(x):
+    return np.asarray(x).astype(F32)
+
+
+def emu32_gather(cols, starts, bounds, mutation=None):
+    """gather_windows_f32_kernel.  mutation 'bound_inclusive': the window also reads row bounds[b, 1]."""
+    rows = starts[:, None] + np.arange(kr.T)[None, :]
+    hi = bounds[:, 1:] + (1 if mutation == "bound_inclusive" else 0)
+    ok = (rows >= 0) & (rows < len(cols)) & (rows >= bounds[:, :1]) & (rows < hi)
+    out = cols[np.clip(rows, 0, len(cols) - 1)].astype(F32)
+    out[~ok] = 0
+    return out
+
+
+def emu32_lstm(x, sd, layer, mutation=None):
+    """lstm_f32_kernel: fp32 gates, expf / tanhf activations, fp32 cell state.  mutations: 'bias_on_wrong_gate' (gate f reads
+    gate i's bias); 'stages_first_160' (LSTM2 stages only the first 160 of its 256 inputs; the rest read as zero)."""
+    H = (kr.H1, kr.H2)[layer]
+    x = np.asarray(x, dtype=F32)
+    if mutation == "stages_first_160":
+        x = x.copy()
+        x[..., H:] = 0
+    B = x.shape[0]
+    out = np.zeros((B, kr.T, 2 * H), dtype=F32)
+    for d in range(2):
+        wih, whh, b = (v.astype(F32) for v in kr.lstm32_weights(sd, layer, d))
+        if mutation == "bias_on_wrong_gate":
+            b = b.copy()
+            b[H:2 * H] = b[:H]
+        h, c = np.zeros((B, H), F32), np.zeros((B, H), F32)
+        sig = lambda v: F32(1) / (F32(1) + np.exp(-v))      # noqa: E731
+        for t in (range(kr.T - 1, -1, -1) if d else range(kr.T)):
+            z = x[:, t] @ wih.T + b + h @ whh.T
+            with np.errstate(over="ignore"):                # expf(-z) -> inf: the gate is 0, as on the GPU
+                c = sig(z[:, H:2 * H]) * c + sig(z[:, :H]) * np.tanh(z[:, 2 * H:3 * H])
+                h = sig(z[:, 3 * H:]) * np.tanh(c)
+            out[:, t, d * H:(d + 1) * H] = h
+    return out
+
+
+def emu32_dense(x, w, mutation=None):
+    """dense_f32_kernel: fp32 sums over 256-wide k-chunks, in order.  mutation 'drops_partial_chunk': the last, partial chunk
+    is lost."""
+    K = x.shape[1]
+    acc = np.zeros((x.shape[0], w.shape[0]), F32)
+    for k0 in range(0, K, 256):
+        if mutation == "drops_partial_chunk" and K - k0 < 256:
+            break
+        acc += x[:, k0:k0 + 256].astype(F32) @ w[:, k0:k0 + 256].T.astype(F32)
+    return acc
+
+
+def emu32_conv(x, wb, stride, residual=None, mutation=None):
+    """conv3x3_f32_kernel.  mutation 'block_site': a pixel's site is taken from the first pixel of its 4-pixel block, so the
+    pixels of the next site in a block that straddles two sites read the previous site's map."""
+    w, bias = wb
+    B, h, wd, _ = x.shape
+    ho, wo = (kr.conv_out(h), kr.conv_out(wd)) if stride == 2 else (h, wd)
+    P, cout = ho * wo, w.shape[2]
+    pix = np.arange(B * P)
+    src = pix
+    if mutation == "block_site":
+        src = pix - (pix // P - (pix // 4 * 4) // P) * P
+    cols = kr.im2col_at(np.asarray(x, dtype=np.float64), stride, src, ho, wo).astype(F32)
+    acc = cols @ w.reshape(-1, cout).astype(F32) + bias.astype(F32)
+    if residual is not None:
+        acc = acc + residual.reshape(-1, cout).astype(F32)
+    return np.maximum(acc, 0).reshape(B, ho, wo, cout)
+
+
+def emu32_spp(x, mutation=None):
+    """spp_f32_kernel: TF-'SAME' windows, a max over the real pixels and 0 when the window overlaps the padding.  mutation
+    'pad_off_by_one': the leading pad is one larger than half the total pad."""
+    B, h, w, c = x.shape
+    out = []
+    for p in (3, 2, 1):
+        wh, ww = -(-h // p), -(-w // p)
+        oh, ow = -(-h // wh), -(-w // ww)
+        pt, pl = max((oh - 1) * wh + wh - h, 0) // 2, max((ow - 1) * ww + ww - w, 0) // 2
+        if mutation == "pad_off_by_one":
+            pt, pl = pt + 1, pl + 1
+        for idx in range(p * p):
+            h0, w0 = idx // ow * wh - pt, idx % ow * ww - pl
+            win = x[:, max(h0, 0):min(h0 + wh, h), max(w0, 0):min(w0 + ww, w)].reshape(B, -1, c)
+            m = win.max(axis=1) if win.shape[1] else np.full((B, c), -1e30, F32)
+            if h0 < 0 or w0 < 0 or h0 + wh > h or w0 + ww > w:
+                m = np.maximum(m, 0)
+            out.append(m)
+    return np.stack(out, axis=1).reshape(B, -1)
+
+
+def _pileup32_case(seed=7, batch=5):
+    sd = synth.pileup_state_dict(False, seed=seed)
+    x = synth.pileup_inputs(batch, seed=seed)
+    x[0, 3, :4] = [70000, -90000, (1 << 24) + 1, 2 ** 31 - 1]      # counts the (float) cast rounds
+    return sd, x
+
+
+def _fa32_case(batch=3, depth=17, seed=8):
+    sd = synth.fa_state_dict(True, channels=8, seed=seed)
+    return sd, synth.fa_inputs(batch, depth=depth, channels=8, seed=seed)
+
+
+def _fa32_convs(sd, x, mutation=None):
+    """Every convolution of the fp32 path: [(input, output, weights, stride, residual)]."""
+    out, cur = [], emu32_input(x)
+    for lvl in range(3):
+        wb = [kr.conv32_weights(sd, 3 * lvl + j) for j in range(3)]
+        a0 = emu32_conv(cur, wb[0], 2, mutation=mutation)
+        a1 = emu32_conv(a0, wb[1], 1, mutation=mutation)
+        a2 = emu32_conv(a1, wb[2], 1, residual=a0, mutation=mutation)
+        out += [(cur, a0, wb[0], 2, None), (a0, a1, wb[1], 1, None), (a1, a2, wb[2], 1, a0)]
+        cur = a2
+    return out
+
+
+def test_fp32_pileup_emulation_passes_the_checker():
+    sd, x = _pileup32_case()
+    xf = emu32_input(x)
+    assert np.array_equal(xf, kr.fp32_input(x)) and xf[0, 3, 2] == 1 << 24
+    h1 = emu32_lstm(xf, sd, 0)
+    h2 = emu32_lstm(h1, sd, 1)
+    act = h2.reshape(len(x), -1)
+    z4 = emu32_dense(act, kr._f32(sd, "L4.weight"))
+    assert kr.lstm32_ratio(xf, h1, sd, 0) <= 1.0
+    assert kr.lstm32_ratio(h1, h2, sd, 1) <= 1.0
+    assert kr.l4_32_ratio(act, z4, sd) <= 1.0
+    assert np.abs(kr.heads(z4, sd, 2) - kr.heads(z4.astype(np.float64), sd, 2)).max() <= kr.HEADS_TOL
+
+
+def test_fp32_saturated_recurrence_emulation_passes_the_checker():
+    """LSTM weights x4: gates saturate and the fp32 cell state runs far from zero, where its rounding is largest."""
+    sd, x = _pileup32_case(seed=9, batch=4)
+    for k in sd:
+        if k.startswith("LSTM"):
+            sd[k] = (np.asarray(sd[k]) * 4).astype(F32)
+    xf = emu32_input(x)
+    h1 = emu32_lstm(xf, sd, 0)
+    assert kr.lstm32_ratio(xf, h1, sd, 0) <= 1.0
+    assert kr.lstm32_ratio(h1, emu32_lstm(h1, sd, 1), sd, 1) <= 1.0
+
+
+@pytest.mark.parametrize("depth", [17, 512])
+def test_fp32_conv_emulation_passes_the_checker(depth):
+    """depth 17: 153 pixels per site at level 1, so 4-pixel blocks straddle sites; both depths pad the pyramid windows."""
+    sd, x = _fa32_case(batch=3 if depth == 17 else 1, depth=depth)
+    convs = _fa32_convs(sd, x)
+    for inp, out, wb, stride, res in convs:
+        assert kr.conv32_ratio(inp, out, wb, stride, res) <= 1.0
+    rb3 = convs[-1][1]
+    sp = emu32_spp(rb3)
+    assert np.array_equal(sp, kr.spp(rb3))
+    assert kr.l4_32_ratio(sp, emu32_dense(sp, kr._f32(sd, "L4.weight")), sd) <= 1.0
+
+
+def test_fp32_window_gather_emulation_is_exact():
+    r = _rng(10)
+    cols = r.integers(-(1 << 30), 1 << 30, size=(300, 18))
+    starts = np.arange(-40, 320, 9)
+    lo = starts + r.integers(-5, 20, len(starts))
+    bounds = np.stack([lo, lo + r.integers(0, 40, len(starts))], axis=1)
+    assert np.array_equal(emu32_gather(cols, starts, bounds), kr.fp32_input(kr.windows(cols, starts, bounds)))
+
+
+@pytest.mark.parametrize("mutation", ["drops_partial_chunk", "block_site", "stages_first_160", "bias_on_wrong_gate",
+                                      "pad_off_by_one", "bound_inclusive"])
+def test_fp32_checks_reject_one_line_mistakes(mutation):
+    if mutation == "drops_partial_chunk":           # pileup L4: K = 10 560 = 41 * 256 + 64
+        sd, x = _pileup32_case()
+        act = _rng(11).uniform(-1, 1, (9, 33 * 320)).astype(F32)
+        ratio = kr.l4_32_ratio(act, emu32_dense(act, kr._f32(sd, "L4.weight"), mutation), sd)
+    elif mutation == "block_site":
+        sd, x = _fa32_case()
+        ratio = max(kr.conv32_ratio(i, o, wb, s, res) for i, o, wb, s, res in _fa32_convs(sd, x, mutation))
+    elif mutation in ("stages_first_160", "bias_on_wrong_gate"):
+        sd, x = _pileup32_case()
+        h1 = emu32_lstm(emu32_input(x), sd, 0)
+        ratio = kr.lstm32_ratio(h1, emu32_lstm(h1, sd, 1, mutation), sd, 1)
+    elif mutation == "pad_off_by_one":
+        rb3 = _fa32_convs(*_fa32_case())[-1][1]
+        err = np.abs(emu32_spp(rb3, mutation) - kr.spp(rb3)).max()
+        ratio = err / kr.TINY                           # the pooling is checked for equality
+    else:
+        cols = _rng(12).integers(1, 100, size=(200, 18))
+        starts = np.arange(-20, 200, 11)
+        bounds = np.stack([starts + 3, starts + 20], axis=1)
+        err = np.abs(emu32_gather(cols, starts, bounds, mutation) - kr.fp32_input(kr.windows(cols, starts, bounds))).max()
+        ratio = err / kr.TINY                           # the gather is checked for equality
+    assert ratio > 1.0, ratio
