@@ -133,9 +133,10 @@ int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, 
     p.bp = bp;
     p.nchunks = p.kg / 8;
     const int tiles = bp / 128;
-    // enough CTAs for two waves of the GPU, at least four k-chunks per split
-    int nsplit = (2 * m->sm_count + tiles - 1) / tiles;
-    nsplit = std::max(1, std::min(std::min(nsplit, kMaxSplit), p.nchunks / 4));
+    // The split count comes from K alone, never from the batch or the device: the split boundaries decide how each site's fp32
+    // partial sums are grouped, so a site's output would otherwise change with the chunk it shares and the card it runs on.
+    // At most 16 splits of at least four k-chunks each: 15 x 11 chunks for the pileup net, 14 x 4 for full alignment.
+    int nsplit = std::max(1, std::min(kMaxSplit, p.nchunks / 4));
     p.chunks_per_split = (p.nchunks + nsplit - 1) / nsplit;
     nsplit = (p.nchunks + p.chunks_per_split - 1) / p.chunks_per_split;
     const int rc = m->d4 == 128 ? launch_l4<128>(p, tiles, nsplit, s) : launch_l4<256>(p, tiles, nsplit, s);

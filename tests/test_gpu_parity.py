@@ -99,15 +99,15 @@ def test_ragged_empty_and_host_buffers():
     # host in / host out (the _torch_predict shape: numpy in, numpy out)
     y_host = m(torch.from_numpy(x))
     assert y_host.device.type == "cpu"
-    assert np.abs(y_host.numpy() - full).max() < 1e-5
-    # ragged batches: any B >= 1, every site independent of its batch neighbours
+    assert np.array_equal(y_host.numpy(), full)
+    # ragged batches: any B >= 1, every site independent of its batch neighbours, bit for bit
     for b in (1, 7, 33):
         yb = m(torch.from_numpy(x[:b]).cuda()).cpu().numpy()
-        assert np.abs(yb - full[:b]).max() < 1e-5
+        assert np.array_equal(yb, full[:b])
     assert m(torch.from_numpy(x[:0]).cuda()).shape == (0, 24)
     # chunked internal passes give the same answer
     m.set_option("chunk_sites", 16)
-    assert np.abs(m(torch.from_numpy(x).cuda()).cpu().numpy() - full).max() < 1e-5
+    assert np.array_equal(m(torch.from_numpy(x).cuda()).cpu().numpy(), full)
 
 
 def test_lstm_tiles_agree():
@@ -116,7 +116,7 @@ def test_lstm_tiles_agree():
     for tile in (16, 32, 64):
         m = _model(meta, sd, TC, lstm_tile=tile)
         outs.append(m(torch.from_numpy(x).cuda()).cpu().numpy())
-    assert np.abs(outs[0] - outs[1]).max() < 1e-5 and np.abs(outs[0] - outs[2]).max() < 1e-5
+    assert np.array_equal(outs[0], outs[1]) and np.array_equal(outs[0], outs[2])
 
 
 @pytest.mark.parametrize("tile", [16, 32, 64])
@@ -128,7 +128,7 @@ def test_lstm_warpgroup_layouts_agree(tile):
     for wg in (1, 2):
         m = _model(meta, sd, TC, lstm_tile=tile, lstm_wg=wg)
         outs.append(m(torch.from_numpy(x).cuda()).cpu().numpy())
-    assert np.abs(outs[0] - outs[1]).max() < 1e-6
+    assert np.array_equal(outs[0], outs[1])
     _check_probs(outs[1], z["y"], 2e-2, 2e-3, 0.99)
 
 
@@ -153,7 +153,7 @@ def test_forward_async_pinned_host_pipeline():
             m.forward_async(xs[i % 3], ys[i % 3])
     torch.cuda.synchronize()
     for y in ys:
-        assert np.abs(y.numpy() - ref).max() < 1e-5
+        assert np.array_equal(y.numpy(), ref)
 
 
 @pytest.mark.parametrize("tile", [16, 64])
@@ -175,7 +175,7 @@ def test_concurrent_streams_are_consistent(tile):
                 outs[i] = m(xd[i])
         torch.cuda.synchronize()
         for i in range(8):
-            assert np.abs(outs[i].cpu().numpy() - ref[i]).max() < 1e-4
+            assert np.array_equal(outs[i].cpu().numpy(), ref[i])
 
 
 def test_input_dtypes_agree():
@@ -184,7 +184,7 @@ def test_input_dtypes_agree():
     y8 = m(torch.from_numpy(x).cuda()).cpu().numpy()
     y32 = m(torch.from_numpy(x.astype(np.int32)).cuda()).cpu().numpy()
     yf = m(torch.from_numpy(x.astype(np.float32)).cuda()).cpu().numpy()
-    assert np.abs(y8 - y32).max() < 1e-5 and np.abs(y8 - yf).max() < 1e-5    # split-K atomics reorder fp32 sums
+    assert np.array_equal(y8, y32) and np.array_equal(y8, yf)
 
 
 def test_strict_state_dict_errors():
@@ -216,7 +216,7 @@ def test_large_batch_properties():
     assert np.isfinite(y).all() and np.allclose(y[:, :21].sum(1), 1, atol=1e-4) and np.allclose(y[:, 21:].sum(1), 1, atol=1e-4)
     perm = np.random.default_rng(0).permutation(1024)
     yp = m(torch.from_numpy(x[perm]).cuda()).cpu().numpy()
-    assert np.abs(yp - y[perm]).max() < 1e-5
+    assert np.array_equal(yp, y[perm])
     m32 = _model(meta, sd, FP32)
     y32 = m32(torch.from_numpy(x[:256]).cuda()).cpu().numpy()
     assert np.abs(y[:256] - y32).max() < 2e-2
@@ -231,7 +231,7 @@ def test_large_batch_properties():
         assert np.allclose(yf[:, lo:hi].sum(1), 1, atol=1e-4)
     permf = np.random.default_rng(1).permutation(256)
     ypf = mf(torch.from_numpy(xf[permf]).cuda()).cpu().numpy()
-    assert np.abs(ypf - yf[permf]).max() < 1e-5
+    assert np.array_equal(ypf, yf[permf])
     # all-zero rows beyond read depth (calloc'ed tensors): an all-zero site must still give finite probabilities
     z0 = mf(torch.zeros((4, 89, 33, 8), dtype=torch.int8).cuda()).cpu().numpy()
     assert np.isfinite(z0).all()
