@@ -13,6 +13,10 @@ records, in three layers each usable on its own:
 * ``call_region``: the whole route on one stream, and ``call_region_host``, the same calls with host records and host
   candidates, which is what the device route is tested against.
 
+Both routes take the reference's two ways of restricting a run (DESIGN.md 5f): a BED (``--bed_fn``) and a known-sites VCF
+(``--vcf_fn``, genotyping mode, which ``add_back_missing`` finishes as AddBackMissingVariantsInGenotyping does).  The device
+route drops the other candidates inside the counter, the host route drops them from the host call results.
+
 Not implemented (``NotImplementedError``): ``platform="ilmn"`` (``MergeVcf_illumina`` and another bed geometry), the haploid
 modes and gVCF output.
 """
@@ -79,15 +83,17 @@ def _kth_qual(probs, pct):
     return decode.quality_score_from(np.partition(p, k - 1)[k - 1])
 
 
-def qual_cutoffs(results, platform="ont", var_pct_full=None, ref_pct_full=None):
+def qual_cutoffs(results, platform="ont", var_pct_full=None, ref_pct_full=None, genotyping=False):
     """``SelectQual`` without ``--phase`` (preprocess/SelectQual.py:select_qual_from_stdin) over any number of pileup ``call``
     results (every region of a genome for the genome-wide cut-offs): returns (var_qual, ref_qual).  Rows whose GT prints as
-    ``0/0`` give the reference cut-off, all others the variant cut-off; ``ref_pct_full`` 0 means ``var_pct_full``, as there.
-    The percentages default to run_clair3.py's for the platform."""
+    ``0/0`` give the reference cut-off, all others the variant cut-off; ``ref_pct_full`` 0 means ``var_pct_full``, as there,
+    except in genotyping mode (``--vcf_fn``, ``genotyping=True``), where ``ref_pct_full`` is used as given (:97).  The
+    percentages default to run_clair3.py's for the platform."""
     _check_platform(platform)
     var_pct = PCT_FULL[platform][0] if var_pct_full is None else var_pct_full
     ref_pct = PCT_FULL[platform][1] if ref_pct_full is None else ref_pct_full
-    ref_pct = ref_pct if ref_pct else var_pct
+    if not genotyping:
+        ref_pct = ref_pct if ref_pct else var_pct
     ref_p, var_p = [], []
     for res in results:
         c = res["calls"][_rows(res)]
@@ -199,6 +205,85 @@ def merge(pileup_result, fa_results, output_config_p, output_config_f, qual=2, p
     return "".join(rows[i] for i in order)
 
 
+# ------------------------------------------------------------------------------------------------ targets
+def contig_targets(ctg, bed=None, known_sites=None):
+    """One contig's ``targets.ContigTargets`` from ``bed`` / ``known_sites``: a path (gzip or plain), a ``targets.Targets``
+    (``read_bed`` / ``read_vcf``) or already a ``ContigTargets`` (``Targets.contig(ctg, chunk=...)``); None for neither.
+    Giving both is a ValueError, as CheckEnvs refuses ``--bed_fn`` with ``--vcf_fn``."""
+    from . import targets as tg
+    if bed is not None and known_sites is not None:
+        raise ValueError("cascade: give either bed or known_sites, not both (the reference refuses --bed_fn with --vcf_fn)")
+    src, read = (bed, tg.read_bed) if bed is not None else (known_sites, tg.read_vcf)
+    if src is None:
+        return None
+    if isinstance(src, tg.ContigTargets):
+        t = src
+    else:
+        t = (src if isinstance(src, tg.Targets) else read(src)).contig(ctg)
+    if (t.known is not None) != (known_sites is not None):
+        raise ValueError("cascade: bed needs a BED's targets and known_sites a VCF's")
+    return t
+
+
+def take_calls(res, idx):
+    """The call result ``res`` (``PileupCounter.call``) at the candidates ``idx`` only, as a targeted count gives it; the
+    ``device`` views are left out."""
+    idx = np.asarray(idx, np.int64)
+    out = {k: v for k, v in res.items() if k != "device"}
+    for k in ("position", "calls", "start", "cand_ok"):
+        if k in res:
+            out[k] = np.asarray(res[k])[idx]
+    out["chromosome"] = [res["chromosome"][i] for i in idx]
+    if "Y" in res:
+        out["Y"] = res["Y"][torch.as_tensor(idx, device=res["Y"].device)]
+    return out
+
+
+# major_contigs_order of preprocess/CheckEnvs.py and postprocess/AddBackMissingVariantsInGenotyping.py
+MAJOR_CONTIGS = ["chr%s" % a for a in list(range(1, 23)) + ["X", "Y"]] + [str(a) for a in list(range(1, 23)) + ["X", "Y"]]
+
+
+def _known_rows(known_vcf):
+    from . import targets as tg
+    if isinstance(known_vcf, tg.ContigTargets):
+        return {(known_vcf.ctg, p): r for p, r in known_vcf.rows.items()}
+    return (known_vcf if isinstance(known_vcf, tg.Targets) else tg.read_vcf(known_vcf)).rows
+
+
+def add_back_missing(merged_body, known_vcf, region=None):
+    """AddBackMissingVariantsInGenotyping (postprocess/AddBackMissingVariantsInGenotyping.py:94-159, ``switch_genotype`` at
+    its default) on a merged VCF body: one row per known site and nothing else - Clair3's row where it called the site, the
+    known row otherwise, padded to 10 columns with REF cut to its first base (``.`` if empty), ALT / QUAL / FILTER / INFO
+    ``.``, FORMAT ``GT`` and sample ``./.``.  The major contigs come first in their order, then the others in the order the
+    known VCF first names them (the reference takes a set's order there, which changes from run to run); sites by position;
+    of duplicate (contig, position) keys the last row wins.  ``known_vcf``: a path, ``targets.read_vcf``'s ``Targets`` or a
+    ``ContigTargets`` (its known sites only).  ``region`` = (ctg, start, end): only the known sites inside the 0-based
+    [start, end), which ``call_region`` is responsible for."""
+    known = _known_rows(known_vcf)
+    if region is not None:
+        c, a, b = region
+        known = {k: r for k, r in known.items() if k[0] == c and a < k[1] <= b}
+    called = {}
+    for row in merged_body.splitlines(keepends=True):
+        cols = row.strip().split()
+        if cols and cols[0][0] != "#":
+            called[(cols[0], int(cols[1]))] = row
+    by_ctg = {}
+    for (ctg, pos), row in known.items():
+        if (ctg, pos) in called:
+            row = called[(ctg, pos)]
+        else:
+            cols = row.rstrip().split("\t")
+            cols += ["."] * (10 - len(cols))
+            cols[3] = cols[3][0] if len(cols[3]) > 0 else "."
+            cols[4] = cols[5] = cols[6] = cols[7] = "."
+            cols[8], cols[9] = "GT", "./."
+            row = "\t".join(cols) + "\n"
+        by_ctg.setdefault(ctg, []).append((pos, row))
+    order = [c for c in MAJOR_CONTIGS if c in by_ctg] + [c for c in by_ctg if c not in MAJOR_CONTIGS]
+    return "".join(r for c in order for _, r in sorted(by_ctg[c], key=lambda x: x[0]))
+
+
 # ------------------------------------------------------------------------------------------------ the route
 class Workspaces:
     """The BAM reader, the pileup counter and the full-alignment builder of a region route on one device."""
@@ -252,7 +337,7 @@ def _span(start, end):
 
 def call_region(bam_path, ctg, start, end, ref_seq, ref_start, model_p, model_f, output_config_p, output_config_f, var_qual=None,
                 ref_qual=None, phased_variants=None, platform="ont", print_ref=False, qual=2, split_bed_size=SPLIT_BED_SIZE,
-                count_params=None, fa_params=None, index=None, workspaces=None, device=0, k=16):
+                count_params=None, fa_params=None, index=None, workspaces=None, device=0, k=16, bed=None, known_sites=None):
     """Clair3's cascade for the 0-based region [start, end) of contig ``ctg``: one ``BamDecoder.decode`` (fa_fields) whose
     device records feed the counter and every full-alignment build, Clair3_P over the pileup candidates, the selection on the
     device, one full-alignment build per ``split_bed_size`` candidates with a fresh glibc ``rand()`` stream (each of the
@@ -262,11 +347,17 @@ def call_region(bam_path, ctg, start, end, ref_seq, ref_start, model_p, model_f,
     ``qual_cutoffs`` over every region's pileup calls first).  ``phased_variants``: ``fa_tensor.phased_variants_from_vcf`` of
     the contig.  ``output_config_p`` / ``_f``: the two decoders' configs (the reference prints the pileup's RefCall rows:
     ``is_show_reference=True``).  ``count_params`` / ``fa_params``: extra keyword arguments of ``PileupCounter.count`` /
-    ``FullAlignmentBuilder.build`` (the matrix depth defaults to the platform's).
+    ``FullAlignmentBuilder.build`` (the matrix depth defaults to the platform's).  ``bed`` / ``known_sites``: call only
+    inside a BED's targets, or only at a VCF's known sites (``contig_targets``: a path, a ``targets.Targets`` or a
+    ``ContigTargets``); the counter drops the other candidates on the device, and with known sites the cut-offs follow
+    SelectQual's genotyping rule and ``add_back_missing`` finishes the body.
 
     Returns a dict: ``vcf`` (the merged body), ``pileup`` and ``full_alignment`` (the ``call`` results), ``qual_cutoffs``,
-    ``candidates`` (int64 0-based, host), ``chunks`` and ``stages`` (wall and device ms per stage)."""
+    ``candidates`` (int64 0-based, host), ``chunks`` and ``stages`` (wall and device ms per stage); with ``known_sites`` also
+    ``genotyped``, the body after ``add_back_missing`` over the known sites inside the region."""
     fa = _route_args(platform, output_config_p, output_config_f, fa_params)
+    tgt = contig_targets(ctg, bed, known_sites)
+    genotyping = known_sites is not None
     own = workspaces is None
     ws = workspaces or Workspaces(device)
     dev = ws.counter._device
@@ -276,11 +367,11 @@ def call_region(bam_path, ctg, start, end, ref_seq, ref_start, model_p, model_f,
         ref = torch.from_numpy(np.frombuffer(ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq), np.uint8).copy())
         rec = ws.decoder.decode(bam_path, ctg, lo, hi, fa_fields=True, ref_seq=ref.to(dev), index=index)
         st.mark("decode")
-        pres = ws.counter.count(rec, start, end, None, ref_start, alt_info=True, **(count_params or {})).call(model_p, output_config_p,
-                                                                                                          ctg, k=k)
+        pres = ws.counter.count(rec, start, end, None, ref_start, alt_info=True, targets=tgt,
+                                **(count_params or {})).call(model_p, output_config_p, ctg, k=k)
         st.mark("pileup")
         if var_qual is None or ref_qual is None:
-            own_var, own_ref = qual_cutoffs([pres], platform)
+            own_var, own_ref = qual_cutoffs([pres], platform, genotyping=genotyping)
             var_qual = own_var if var_qual is None else var_qual
             ref_qual = own_ref if ref_qual is None else ref_qual
         selected, count = select_device(pres, var_qual, ref_qual)
@@ -298,8 +389,11 @@ def call_region(bam_path, ctg, start, end, ref_seq, ref_start, model_p, model_f,
         vcf = merge(pres, fres, output_config_p, output_config_f, qual=qual, print_ref=print_ref)
         st.mark("merge")
         stages = st.report()
-        return {"vcf": vcf, "pileup": pres, "full_alignment": fres, "qual_cutoffs": (var_qual, ref_qual),
-                "candidates": selected[:total].cpu().numpy(), "chunks": _chunks(total, split_bed_size), "stages": stages}
+        out = {"vcf": vcf, "pileup": pres, "full_alignment": fres, "qual_cutoffs": (var_qual, ref_qual),
+               "candidates": selected[:total].cpu().numpy(), "chunks": _chunks(total, split_bed_size), "stages": stages}
+        if genotyping:
+            out["genotyped"] = add_back_missing(vcf, tgt, region=(ctg, start, end))
+        return out
     finally:
         if own:
             ws.close()
@@ -307,11 +401,14 @@ def call_region(bam_path, ctg, start, end, ref_seq, ref_start, model_p, model_f,
 
 def call_region_host(bam_path, ctg, start, end, ref_seq, ref_start, model_p, model_f, output_config_p, output_config_f, var_qual=None,
                      ref_qual=None, phased_variants=None, platform="ont", print_ref=False, qual=2, split_bed_size=SPLIT_BED_SIZE,
-                     count_params=None, fa_params=None, workspaces=None, device=0, k=16):
+                     count_params=None, fa_params=None, workspaces=None, device=0, k=16, bed=None, known_sites=None):
     """``call_region`` through host records and host candidates: ``bam_io.read_bam`` -> count -> call -> ``select`` on the
-    host -> one host-candidate build per chunk -> call -> ``merge``.  Same arguments and result (without ``stages``)."""
+    host -> one host-candidate build per chunk -> call -> ``merge``.  Same arguments and result (without ``stages``); the
+    count is untargeted and ``bed`` / ``known_sites`` drop the other candidates from its call results (``ContigTargets.keep``)."""
     from . import bam_io
     fa = _route_args(platform, output_config_p, output_config_f, fa_params)
+    tgt = contig_targets(ctg, bed, known_sites)
+    genotyping = known_sites is not None
     own = workspaces is None
     ws = workspaces or Workspaces(device)
     try:
@@ -319,16 +416,21 @@ def call_region_host(bam_path, ctg, start, end, ref_seq, ref_start, model_p, mod
         rec, _ = bam_io.read_bam(bam_path, ctg, lo, hi, fa_fields=True)
         pres = ws.counter.count(rec, start, end, ref_seq, ref_start, alt_info=True, **(count_params or {})).call(model_p, output_config_p,
                                                                                                               ctg, k=k)
+        if tgt is not None:
+            pres = take_calls(pres, np.nonzero(tgt.keep(pres["position"]))[0])
         if var_qual is None or ref_qual is None:
-            own_var, own_ref = qual_cutoffs([pres], platform)
+            own_var, own_ref = qual_cutoffs([pres], platform, genotyping=genotyping)
             var_qual = own_var if var_qual is None else var_qual
             ref_qual = own_ref if ref_qual is None else ref_qual
         pos, chunks = select(pres, var_qual, ref_qual, split_bed_size)
         fres = [ws.builder.build(rec, pos[a:b], ref_seq, ref_start, variants=phased_variants, rand_seed=1, rand_skip=0, **fa)
                 .call(model_f, output_config_f, ctg, k=k) for a, b in chunks]
         vcf = merge(pres, fres, output_config_p, output_config_f, qual=qual, print_ref=print_ref)
-        return {"vcf": vcf, "pileup": pres, "full_alignment": fres, "qual_cutoffs": (var_qual, ref_qual), "candidates": pos,
-                "chunks": chunks}
+        out = {"vcf": vcf, "pileup": pres, "full_alignment": fres, "qual_cutoffs": (var_qual, ref_qual), "candidates": pos,
+               "chunks": chunks}
+        if genotyping:
+            out["genotyped"] = add_back_missing(vcf, tgt, region=(ctg, start, end))
+        return out
     finally:
         if own:
             ws.close()

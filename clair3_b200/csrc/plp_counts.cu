@@ -24,6 +24,9 @@
 //   K6 plp_quirk         the reference's index -1 quirk: a non-ACGT read base increments feature 17 of the PREVIOUS emitted column.
 //   K8 plp_cands         candidate list, window starts and run bounds for c3b_forward_windows_bounded, and the reference's verdict
 //                        on each candidate's window (plain, or with call_ht the zero-padded head / tail windows).
+//   targets              (c3b_plp_count_targeted) K5 counts and K8 places only the candidates inside the BED / known sites: two
+//                        binary searches per candidate column, fused into both kernels; K0 plp_targets_check checks device
+//                        target arrays on the stream.
 //
 // Bound: HBM / L2 latency (integer work, no tensor cores).  Algorithmic bytes per call: 8 B per CIGAR word (read + offsets
 // written and re-read), 0.5 B per aligned base (packed sequence), ~27 B per read, and per column 72 + 24 + 4 B dense (written, read
@@ -385,10 +388,48 @@ __global__ void __launch_bounds__(TILE, 6) plp_count_tile_kernel(CountArgs A) {
     }
 }
 
+// ------------------------------------------------------------------------------------------------------- targets (K0)
+// The BED / known-sites test of preprocess/CreateTensorPileupFromCffi.py:347-355 on the device (c3b_plp_targets): is_region_in
+// over [q - 1, q + 1) of the half-open interval tree is, for the 1-based position q, some interval with s <= q <= e.  The
+// intervals are sorted by start and carry the running maximum of their ends, so the last interval with s <= q holds the largest
+// end among all of them.  Every search stays inside [0, n) whatever the arrays hold: K0 only reports arrays out of order.
+struct Targets {
+    const int64_t *starts, *end_max, *sites;
+    int64_t n_iv, n_sites;     // n_sites < 0: no known-site test
+    int on;
+};
+
+__device__ __forceinline__ bool plp_targeted(const Targets &T, const int64_t q) {
+    int64_t a = 0, b = T.n_iv;                               // first interval with s > q
+    while (a < b) { const int64_t m = (a + b) >> 1; if (__ldg(T.starts + m) > q) b = m; else a = m + 1; }
+    if (a == 0 || __ldg(T.end_max + a - 1) < q) return false;
+    if (T.n_sites < 0) return true;
+    a = 0;
+    b = T.n_sites;                                           // first known site >= q
+    while (a < b) { const int64_t m = (a + b) >> 1; if (__ldg(T.sites + m) >= q) b = m; else a = m + 1; }
+    return a < T.n_sites && __ldg(T.sites + a) == q;
+}
+
+// K0: device target arrays cannot be checked on the host without a wait; this pass reports arrays out of order through the
+// status word (bit 16), which the count's own wait in c3b_plp_sizes reads.
+__global__ void plp_targets_check_kernel(Targets T, const int64_t *__restrict__ ends, int *status) {
+    const int64_t n = T.n_iv > T.n_sites ? T.n_iv : T.n_sites;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        bool bad = false;
+        if (i < T.n_iv) {
+            const int64_t s = T.starts[i], e = ends[i], m = T.end_max[i];
+            bad = e < s || m != (i ? (T.end_max[i - 1] > e ? T.end_max[i - 1] : e) : e) || (i && T.starts[i - 1] > s);
+        }
+        if (i < T.n_sites && i) bad = bad || T.sites[i - 1] >= T.sites[i];
+        if (bad) atomicOr(status, 16);
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------------- K5
 struct EmitArgs {
     int64_t start, end;
     int call_ht;
+    Targets tg;
     const int32_t *rows32;
     const int32_t *dstats;
     const int64_t *tile_off;
@@ -424,7 +465,7 @@ __global__ void __launch_bounds__(TILE) plp_emit_kernel(EmitArgs A) {
     }
     const int lci = pre + __popc(bal & ((1u << lane) - 1u));
     const int64_t t_off = A.tile_off[blockIdx.x];
-    bool cand = false;
+    bool cand = false, kept = false;
     if (covered) {
         const int64_t ci = t_off + lci;
         map_s[lci] = tid;
@@ -442,11 +483,12 @@ __global__ void __launch_bounds__(TILE) plp_emit_kernel(EmitArgs A) {
         const int32_t *ds = A.dstats + (p - A.start) * 6;
         int32_t *st = A.stats + ci * 6;
         st[0] = ds[0]; st[1] = ds[1]; st[2] = ds[2]; st[3] = ds[3]; st[4] = ds[4];
-        st[5] = (cand ? 1 : 0) | (zero ? 2 : 0);
+        st[5] = (cand ? 1 : 0) | (zero ? 2 : 0);        // bit 0 before the target test
+        kept = cand && (!A.tg.on || plp_targeted(A.tg, p + 1));
     } else if (active) {
         A.dci[p - A.start] = -1;
     }
-    const int ncand = __syncthreads_count(cand);
+    const int ncand = __syncthreads_count(kept);
     if (tid == 0) A.tile_cand[blockIdx.x] = ncand;
     int64_t *dst = A.matrix + t_off * NFEAT;
     for (int e = tid; e < ntile * NFEAT; e += TILE) {
@@ -473,6 +515,7 @@ __global__ void plp_quirk_kernel(const int64_t *n_cols_dev, const int64_t *__res
 struct CandArgs {
     int64_t start, end;
     int call_ht;
+    Targets tg;
     const int64_t *n_cols_dev;
     const int32_t *dci;
     const int32_t *stats;
@@ -491,7 +534,7 @@ __global__ void __launch_bounds__(TILE) plp_cands_kernel(CandArgs A) {
     const int64_t n = *A.n_cols_dev;
     int64_t ci = -1;
     if (p < A.end) ci = A.dci[p - A.start];
-    const bool cand = ci >= 0 && (A.stats[ci * 6 + 5] & 1);
+    const bool cand = ci >= 0 && (A.stats[ci * 6 + 5] & 1) && (!A.tg.on || plp_targeted(A.tg, p + 1));   // K5's tile_cand
     const unsigned bal = __ballot_sync(0xffffffffu, cand);
     if (lane == 0) wsum[warp] = __popc(bal);
     __syncthreads();
@@ -534,6 +577,7 @@ struct c3b_plp : C3bRegionWorkspace {
     C3bBuf opx, opy, rend, pmax, rows32, dstats, nquirk, dci, tile_cov, tile_off, tile_cand, tile_coff;
     C3bBuf g_meta, g_read, g_qpos, g_cnt, g_next;
     C3bBuf ins_last, tx_mate;
+    C3bBuf tg_starts, tg_ends, tg_emax, tg_sites;     // host target arrays, copied
     // outputs
     C3bBuf matrix, major, stats, cand_cols, wstart, wbounds, cand_ok, gv_ref, gv_tot;
     int64_t W = 0, start = 0, end = 0;
@@ -555,9 +599,36 @@ int c3b_plp_create(c3b_plp **out, int device_ordinal) {
     return c3b_region_create(out, device_ordinal, 2, N_COUNTERS, TEXT_WORD, "c3b_plp_create");
 }
 
+// The host checks of a c3b_plp_targets: its counts always, and its arrays when they are host memory.
+static int plp_targets_valid(const c3b_plp_targets *t) {
+    const char *who = "c3b_plp_count_targeted";
+    if (t->n_intervals < 0 || t->n_sites < -1) { c3b_set_error("%s: negative target count", who); return 1; }
+    if ((t->n_intervals && (!t->starts || !t->ends || !t->end_max)) || (t->n_sites > 0 && !t->sites)) {
+        c3b_set_error("%s: null target array", who);
+        return 1;
+    }
+    if (t->on_device) return 0;
+    for (int64_t i = 0; i < t->n_intervals; ++i) {
+        if (t->ends[i] < t->starts[i]) { c3b_set_error("%s: interval %lld ends before it starts", who, (long long)i); return 1; }
+        if (i && t->starts[i - 1] > t->starts[i]) { c3b_set_error("%s: interval starts are not ascending at %lld", who, (long long)i); return 1; }
+        const int64_t m = i && t->end_max[i - 1] > t->ends[i] ? t->end_max[i - 1] : t->ends[i];
+        if (t->end_max[i] != m) { c3b_set_error("%s: end_max is not the running maximum of the ends at %lld", who, (long long)i); return 1; }
+    }
+    for (int64_t i = 1; i < t->n_sites; ++i)
+        if (t->sites[i - 1] >= t->sites[i]) { c3b_set_error("%s: known sites are not strictly ascending at %lld", who, (long long)i); return 1; }
+    return 0;
+}
+
 int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64_t start, int64_t end, const char *ref_seq,
                   int64_t ref_start, int64_t ref_len, const c3b_plp_params *params, void *cuda_stream) {
+    return c3b_plp_count_targeted(w, reads, on_device, start, end, ref_seq, ref_start, ref_len, params, nullptr, cuda_stream);
+}
+
+int c3b_plp_count_targeted(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64_t start, int64_t end, const char *ref_seq,
+                           int64_t ref_start, int64_t ref_len, const c3b_plp_params *params, const c3b_plp_targets *targets,
+                           void *cuda_stream) {
     if (!w || !reads || !params) { c3b_set_error("c3b_plp_count: null argument"); return 1; }
+    if (targets && plp_targets_valid(targets)) return 1;
     if (end < start) { c3b_set_error("c3b_plp_count: end < start"); return 1; }
     if (end - start > (int64_t)INT_MAX / 32) { c3b_set_error("c3b_plp_count: region of %lld columns is too large for one call", (long long)(end - start)); return 1; }
     C3B_CUDA(cudaSetDevice(w->device));
@@ -605,9 +676,29 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
     int *g_used = reinterpret_cast<int *>(n_cols_dev + 2);
     int *status = g_used + 1;
     int *al_used = reinterpret_cast<int *>(n_cols_dev + 3);
+    Targets tg = {nullptr, nullptr, nullptr, 0, -1, 0};
+    const int64_t *tg_ends = nullptr;
+    if (targets) {
+        const int dv = targets->on_device;
+        const size_t ni = (size_t)targets->n_intervals * 8, ns = (size_t)(targets->n_sites > 0 ? targets->n_sites : 0) * 8;
+        if (c3b_upload(w->tg_starts, targets->starts, ni, dv, tg.starts, s, "c3b_plp") ||
+            c3b_upload(w->tg_ends, targets->ends, ni, dv, tg_ends, s, "c3b_plp") ||
+            c3b_upload(w->tg_emax, targets->end_max, ni, dv, tg.end_max, s, "c3b_plp") ||
+            c3b_upload(w->tg_sites, targets->sites, ns, dv, tg.sites, s, "c3b_plp"))
+            return 1;
+        tg.n_iv = targets->n_intervals;
+        tg.n_sites = targets->n_sites;
+        tg.on = 1;
+    }
 
     w->launches[0] = 0;
     C3B_CUDA(cudaEventRecord(w->ev[0][0], s));
+    const int64_t nt = tg.n_iv > tg.n_sites ? tg.n_iv : tg.n_sites;
+    if (targets && targets->on_device && nt > 0) {
+        const int blocks = (int)((nt + 255) / 256 < 132 * 4 ? (nt + 255) / 256 : 132 * 4);
+        plp_targets_check_kernel<<<blocks, 256, 0, s>>>(tg, tg_ends, status);
+        w->launches[0] += 1;
+    }
     if (W > 0) {
         if (n > 0) {
             int blocks = (int)((n * 32 + 255) / 256);
@@ -633,7 +724,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         plp_count_tile_kernel<<<tiles, TILE, smem, s>>>(A);
         block_scan_sum(w->tile_cov.as<int32_t>(), w->tile_off.as<int64_t>(), tiles, nullptr, n_cols_dev, s);
         EmitArgs E;
-        E.start = start; E.end = end; E.call_ht = params->call_ht;
+        E.start = start; E.end = end; E.call_ht = params->call_ht; E.tg = tg;
         E.rows32 = w->rows32.as<int32_t>(); E.dstats = w->dstats.as<int32_t>(); E.tile_off = w->tile_off.as<int64_t>();
         E.matrix = w->matrix.as<int64_t>(); E.major = w->major.as<int64_t>(); E.stats = w->stats.as<int32_t>();
         E.dci = w->dci.as<int32_t>(); E.tile_cand = w->tile_cand.as<int32_t>();
@@ -645,7 +736,7 @@ int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64
         C.start = start; C.end = end; C.n_cols_dev = n_cols_dev; C.dci = w->dci.as<int32_t>(); C.stats = w->stats.as<int32_t>();
         C.major = w->major.as<int64_t>(); C.tile_coff = w->tile_coff.as<int64_t>(); C.cand_cols = w->cand_cols.as<int64_t>();
         C.wstart = w->wstart.as<int64_t>(); C.wbounds = w->wbounds.as<int64_t>(); C.cand_ok = w->cand_ok.as<uint8_t>();
-        C.call_ht = params->call_ht;
+        C.call_ht = params->call_ht; C.tg = tg;
         plp_cands_kernel<<<tiles, TILE, 0, s>>>(C);
         w->launches[0] += 6;
     }
@@ -666,6 +757,11 @@ int c3b_plp_sizes(c3b_plp *w, int64_t *n_cols, int64_t *n_candidates) {
     if (status & 2) { c3b_set_error("c3b_plp_count: a read spans more than 2^31 reference or query bases"); return 1; }
     if (status & 4) { c3b_set_error("c3b_plp_count: an indel of 2^30 bases or more"); return 1; }
     if (status & 8) { c3b_set_error("c3b_plp_count: more than %d allele records to export (params.alt_info); count a smaller region", C3B_AL_CAP); return 1; }
+    if (status & 16) {
+        c3b_set_error("c3b_plp_count_targeted: device targets out of order (starts ascending, ends >= starts, end_max the running "
+                      "maximum of the ends, known sites strictly ascending)");
+        return 1;
+    }
     w->n_cols = w->host_counters[0];
     w->n_cand = w->host_counters[1];
     if (n_cols) *n_cols = w->n_cols;

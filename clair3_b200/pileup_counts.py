@@ -37,11 +37,14 @@ class PileupCounter(_Workspace):
         self._pin = {}
 
     def count(self, records, start, end, ref_seq, ref_start, min_depth=2, min_snp_af=0.08, min_indel_af=0.15, min_mq=5,
-              call_snp_only=False, call_ht=False, gvcf=False, alt_info=False, max_indel_length=50):
+              call_snp_only=False, call_ht=False, gvcf=False, alt_info=False, max_indel_length=50, targets=None):
         """Arguments as ``calculate_clair3_pileup`` takes them (src/clair3_pileup.c:142) with the region as 0-based
         [start, end) and the reference bases of [ref_start, ref_start + len(ref_seq)).  ``alt_info=True`` also exports the
         candidates' allele lists, from which ``alt_text()`` formats the reference's ``all_alt_info`` text on the device
-        (``alt_info_strings()``: the same on the host) and ``call()`` decodes every candidate."""
+        (``alt_info_strings()``: the same on the host) and ``call()`` decodes every candidate.  ``targets``: a
+        ``targets.ContigTargets`` (a BED's or a known-sites VCF's targets on this contig); the candidates outside them are
+        dropped on the device before anything keyed by candidate (``c3b_plp_count_targeted``), the matrix, ``major`` and
+        ``stats`` stay as they are."""
         on_dev = isinstance(records, DeviceBamRecords)
         rec = records if on_dev else BamRecords.from_dict(records)
         prm = ffi.new("c3b_plp_params *")
@@ -50,8 +53,14 @@ class PileupCounter(_Workspace):
         prm.alt_info = int(bool(alt_info))
         st = records_struct(rec)
         refptr, reflen, ref = self._reference(ref_seq, rec, "count")
-        check(lib().c3b_plp_count(self._h, st, int(on_dev), int(start), int(end), refptr, int(ref_start), reflen, prm, self._stream()))
-        self._keep = (rec, ref, st)                  # buffers stay alive while the copies / kernels are in flight
+        tg, tg_keep = None, None
+        if targets is None:
+            check(lib().c3b_plp_count(self._h, st, int(on_dev), int(start), int(end), refptr, int(ref_start), reflen, prm, self._stream()))
+        else:
+            tg, tg_keep = targets.struct(self._device)
+            check(lib().c3b_plp_count_targeted(self._h, st, int(on_dev), int(start), int(end), refptr, int(ref_start), reflen, prm,
+                                               tg, self._stream()))
+        self._keep = (rec, ref, st, tg, tg_keep)     # buffers stay alive while the copies / kernels are in flight
         self._shape = (int(end) - int(start), bool(gvcf))
         self._alt = (bool(alt_info), int(start), int(end), int(ref_start), int(max_indel_length))
         self._sizes = None
@@ -316,13 +325,40 @@ def format_alt_info(pos, row, stats, ref, ref_start, max_indel_length, meta, rea
 
 def chunk_region(contig_length, chunk_id, chunk_num):
     """The 1-based contig slice [ctg_start, ctg_end] of chunk ``chunk_id`` (1-based, as ``--chunk_id``) of ``chunk_num``:
-    ``preprocess/CreateTensorPileupFromCffi.py:249,281-292`` (no BED / VCF restriction)."""
+    ``preprocess/CreateTensorPileupFromCffi.py:249,281-292``, for a run without ``--bed_fn`` / ``--vcf_fn`` (with them:
+    ``bed_chunk_region`` / ``known_sites_chunk``)."""
     if not 1 <= chunk_id <= chunk_num:
         raise C3BError("chunk_region: chunk_id %d outside 1..%d" % (chunk_id, chunk_num))
     cid = chunk_id - 1
     chunk_size = contig_length // chunk_num + 1 if contig_length % chunk_num else contig_length // chunk_num
     ctg_start = chunk_size * cid
     return ctg_start, ctg_start + chunk_size
+
+
+def bed_chunk_region(bed_start, bed_end, chunk_id, chunk_num):
+    """The 1-based contig slice [ctg_start, ctg_end] of chunk ``chunk_id`` of ``chunk_num`` over the span of an extended BED
+    (``targets.ContigTargets.bed_region``): ``preprocess/CreateTensorPileupFromCffi.py:295-298``."""
+    if not 1 <= chunk_id <= chunk_num:
+        raise C3BError("bed_chunk_region: chunk_id %d outside 1..%d" % (chunk_id, chunk_num))
+    span = bed_end - bed_start
+    chunk_size = span // chunk_num + 1 if span % chunk_num else span // chunk_num
+    ctg_start = bed_start + 1 + chunk_size * (chunk_id - 1)
+    return ctg_start, ctg_start + chunk_size
+
+
+def known_sites_chunk(sites, chunk_id, chunk_num):
+    """Chunk ``chunk_id`` of ``chunk_num`` in genotyping mode (``preprocess/CreateTensorPileupFromCffi.py:300-308``): the
+    contig's sorted unique known 1-based positions cut into equal slices.  Returns (ctg_start, ctg_end, the slice) - the
+    1-based slice from its smallest to its largest site - or None for an empty slice, which the reference skips."""
+    if not 1 <= chunk_id <= chunk_num:
+        raise C3BError("known_sites_chunk: chunk_id %d outside 1..%d" % (chunk_id, chunk_num))
+    sites = np.asarray(sites, np.int64)
+    n = len(sites)
+    size = n // chunk_num if n % chunk_num == 0 else n // chunk_num + 1
+    part = sites[(chunk_id - 1) * size:chunk_id * size]
+    if not len(part):
+        return None
+    return int(part.min()), int(part.max()), part
 
 
 def counting_region(ctg_start, ctg_end, no_of_positions=2 * FLANKING + 1):

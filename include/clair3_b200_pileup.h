@@ -71,8 +71,32 @@ int c3b_plp_create(c3b_plp **out, int device_ordinal);
 int c3b_plp_count(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64_t start, int64_t end, const char *ref_seq,
                   int64_t ref_start, int64_t ref_len, const c3b_plp_params *params, void *cuda_stream);
 
+/* The targets of a run with a BED (--bed_fn) or a known-sites VCF (--vcf_fn) on one contig, as the reference's pileup step reads
+ * them from the extended BED CheckEnvs writes (preprocess/CreateTensorPileupFromCffi.py:347-355; clair3_b200/targets.py builds
+ * these arrays).  A candidate at 1-based position q is kept when some interval has starts[i] <= q <= ends[i] and, with known
+ * sites, q is one of them.  Zero-length rows must already be [s, s + 1), as the reference's interval tree stores them. */
+typedef struct c3b_plp_targets {
+    int64_t n_intervals;
+    const int64_t *starts;      /* [n_intervals] 0-based interval starts, ascending                                        */
+    const int64_t *ends;        /* [n_intervals] end-exclusive ends, ends[i] >= starts[i]                                  */
+    const int64_t *end_max;     /* [n_intervals] running maximum of ends[0..i]: one binary search over starts decides the test */
+    int64_t n_sites;            /* -1: no known-site test; otherwise the number of known sites (0 keeps nothing)           */
+    const int64_t *sites;       /* [n_sites] 1-based known positions, strictly ascending                                   */
+    int32_t on_device;          /* 1: the arrays are device pointers, checked on the stream (c3b_plp_sizes reports a
+                                   violation); 0: host arrays, checked here and copied on the call's stream               */
+} c3b_plp_targets;
+
+/* c3b_plp_count that keeps only the candidates inside `targets` (NULL: c3b_plp_count itself).  The matrix, major, stats (bit 0
+ * still marks every candidate column before the target test), the allele export and the gVCF counts do not change; cand_cols,
+ * cand_ok, the window starts and bounds, n_candidates and everything keyed by candidate after them (c3b_plp_alt_text, the
+ * network, the decoder) cover only the kept candidates.  An empty target set is valid and keeps none.  The arrays must stay
+ * alive until the count has been waited for. */
+int c3b_plp_count_targeted(c3b_plp *w, const c3b_bam_records *reads, int on_device, int64_t start, int64_t end, const char *ref_seq,
+                           int64_t ref_start, int64_t ref_len, const c3b_plp_params *params, const c3b_plp_targets *targets,
+                           void *cuda_stream);
+
 /* Waits for the last c3b_plp_count and reports plp_data.n_cols (covered columns) and plp_data.candidates_num.  Fails if the
- * call overflowed a capacity (message says which). */
+ * call overflowed a capacity or was given device target arrays out of order (message says which). */
 int c3b_plp_sizes(c3b_plp *w, int64_t *n_cols, int64_t *n_candidates);
 
 /* Copies the results to host buffers (any pointer may be NULL):
