@@ -14,12 +14,14 @@ Two readers produce the records the GPU counter and builder take:
 
 A writer is included so that tests (and users without samtools) can produce valid files, and ``write_bai`` indexes them as the
 specification's section 5.2 describes.  CRAM and CSI indexes are not handled.  The reference bases come out of a FASTA file
-(``read_fasta``).
+(``read_fasta``, or ``fetch_fasta`` at random access through its ``.fai``).  ``idxstats`` reads the mapped counts of the
+``.bai``; ``write_bgzf`` and ``write_tbi`` write a bgzipped, tabix-indexed VCF as ``bgzip`` and ``tabix -p vcf`` do.
 """
 from __future__ import annotations
 
 import bisect
 import gzip
+import os
 import struct
 import zlib
 
@@ -264,9 +266,36 @@ def write_bam(path, rec, refs, tid=0, names=None, header_text=None):
                           l_seq, -1, -1, 0) + nm + cig.tobytes() + seq[:(l_seq + 1) // 2] + qual + aux
         out += struct.pack("<i", len(body)) + body
     with open(path, "wb") as f:
-        for b0 in range(0, len(out), 0xFF00):                # BGZF: at most 64 KiB of payload per block
-            f.write(_bgzf_block(bytes(out[b0:b0 + 0xFF00])))
-        f.write(_EOF)
+        _write_bgzf_blocks(f, out)
+
+
+_BGZF_PAYLOAD = 0xFF00        # payload per block, as bgzip and htslib cut it
+
+
+def _write_bgzf_blocks(f, data):
+    """Writes ``data`` to the open file ``f`` as BGZF blocks of ``_BGZF_PAYLOAD`` bytes and the EOF block; returns the file
+    offset of each block."""
+    offsets = []
+    for b0 in range(0, len(data), _BGZF_PAYLOAD):           # BGZF: at most 64 KiB of payload per block
+        offsets.append(f.tell())
+        f.write(_bgzf_block(bytes(data[b0:b0 + _BGZF_PAYLOAD])))
+    f.write(_EOF)
+    return offsets
+
+
+def write_bgzf(path, data):
+    """Writes ``data`` (bytes or str) as a BGZF file with the end-of-file block, as ``bgzip`` does (the blocks ``write_bam``
+    writes).  Returns the virtual offset (SAM/BAM specification 4.1.1) of every uncompressed byte position as a function
+    ``voffset(u)``, which ``write_tbi`` indexes with."""
+    data = data.encode() if isinstance(data, str) else bytes(data)
+    with open(path, "wb") as f:
+        offsets = _write_bgzf_blocks(f, data)
+        end = f.tell() - len(_EOF)
+
+    def voffset(u):
+        i = u // _BGZF_PAYLOAD
+        return offsets[i] << 16 | (u - i * _BGZF_PAYLOAD) if i < len(offsets) else end << 16
+    return voffset
 
 
 def read_fasta(path, name, start=0, end=None):
@@ -299,6 +328,65 @@ def write_fasta(path, seqs, width=60):
             f.write(">%s\n" % name)
             for i in range(0, len(seq), width):
                 f.write(seq[i:i + width] + "\n")
+
+
+def write_fai(fasta_path, fai_path=None):
+    """Writes the ``.fai`` of a plain FASTA (default ``fasta_path + ".fai"``) as ``samtools faidx`` does: per sequence its name,
+    length, the byte offset of its first base, bases per line and bytes per line.  Every line but a sequence's last must be
+    full.  Returns the path written."""
+    rows, cur = [], None
+    with open(fasta_path, "rb") as f:
+        if f.read(2) == b"\x1f\x8b":
+            raise ValueError("%s: a compressed FASTA cannot be indexed here; decompress it first" % fasta_path)
+        f.seek(0)
+        off = 0
+        for line in f:
+            if line.startswith(b">"):
+                cur = [line[1:].split()[0].decode(), 0, off + len(line), 0, 0]
+                rows.append(cur)
+            elif cur is not None:
+                n = len(line.rstrip(b"\r\n"))
+                if cur[3] == 0:
+                    cur[3], cur[4] = n, len(line)
+                cur[1] += n
+            off += len(line)
+    path = fai_path or str(fasta_path) + ".fai"
+    with open(path, "w") as f:
+        f.write("".join("%s\t%d\t%d\t%d\t%d\n" % tuple(r) for r in rows))
+    return path
+
+
+def read_fai(path):
+    """The rows of a ``.fai`` index in file order: [(name, length, offset, line bases, line bytes)]."""
+    out = []
+    with open(path) as f:
+        for row in f:
+            c = row.rstrip("\n").split("\t")
+            if len(c) >= 5:
+                out.append((c[0], int(c[1]), int(c[2]), int(c[3]), int(c[4])))
+    return out
+
+
+def fetch_fasta(path, name, start=0, end=None, fai=None):
+    """Bases [start, end) of sequence ``name`` of a plain FASTA through its ``.fai`` (default ``path + ".fai"``), clipped to the
+    sequence, case kept: what ``read_fasta`` returns, read at random access as ``faidx_fetch_seq`` reads it.  A bgzip-compressed
+    FASTA is refused (ValueError)."""
+    rows = {r[0]: r for r in read_fai(fai or str(path) + ".fai")}
+    if name not in rows:
+        raise ValueError("sequence %r not found in the index of %s" % (name, path))
+    _, length, off, lb, lw = rows[name]
+    start = max(0, int(start))
+    end = length if end is None else min(int(end), length)
+    if end <= start:
+        return ""
+    with open(path, "rb") as f:
+        if f.read(2) == b"\x1f\x8b":
+            raise ValueError("%s: compressed FASTA is not supported; decompress it (and re-index it)" % path)
+        a = off + start // lb * lw + start % lb
+        b = off + (end - 1) // lb * lw + (end - 1) % lb + 1
+        f.seek(a)
+        raw = f.read(b - a)
+    return raw.replace(b"\n", b"").replace(b"\r", b"").decode()
 
 
 # ---- BGZF blocks, the header and the .bai index: what the GPU reader (clair3_b200.bam_decode) needs from the host ----
@@ -501,7 +589,7 @@ def write_bai(bam_path, bai_path=None):
         return blocks[i][0] << 16 | (x - ustart[i])
 
     refs, off = read_header(buf)
-    idx = [{"bins": {}, "lin": {}, "first": None, "last": 0, "mapped": 0, "unmapped": 0} for _ in refs]
+    idx = [_index_ref() for _ in refs]
     n_no_coor = 0
     while off + 4 <= len(buf):
         block_size, = struct.unpack_from("<i", buf, off)
@@ -513,34 +601,152 @@ def write_bai(bam_path, bai_path=None):
             n_no_coor += 1
             continue
         span = int((cig >> 4)[np.isin(cig & 15, _REF_CONSUMING)].sum()) if n_cig else 0
-        e = p + max(span, 1)
-        r = idx[tid]
-        chunks = r["bins"].setdefault(_reg2bin(p, e), [])
-        if chunks and chunks[-1][1] == beg:
-            chunks[-1][1] = nxt
-        else:
-            chunks.append([beg, nxt])
-        for w in range(p >> 14, ((e - 1) >> 14) + 1):
-            r["lin"].setdefault(w, beg)
-        r["first"] = beg if r["first"] is None else r["first"]
-        r["last"] = nxt
-        r["unmapped" if fl & 4 else "mapped"] += 1
+        _index_push(idx[tid], p, p + max(span, 1), beg, nxt, not fl & 4)
     out = bytearray(b"BAI\x01" + struct.pack("<i", len(refs)))
     for r in idx:
-        bins = dict(r["bins"])
-        if r["first"] is not None:
-            bins[_PSEUDO_BIN] = [[r["first"], r["last"]], [r["mapped"], r["unmapped"]]]
-        out += struct.pack("<i", len(bins))
-        for b, chunks in bins.items():
-            out += struct.pack("<Ii", b, len(chunks)) + b"".join(struct.pack("<QQ", x, y) for x, y in chunks)
-        n_intv = max(r["lin"]) + 1 if r["lin"] else 0
-        lin, prev = [], r["first"] or 0             # windows before the first record's: its offset; gaps: the previous window's
-        for w in range(n_intv):
-            prev = r["lin"].get(w, prev)
-            lin.append(prev)
-        out += struct.pack("<i", n_intv) + b"".join(struct.pack("<Q", x) for x in lin)
+        out += _index_ref_bytes(r)
     out += struct.pack("<Q", n_no_coor)
     path = bai_path or str(bam_path) + ".bai"
     with open(path, "wb") as f:
         f.write(out)
     return path
+
+
+# ---- the binning and linear index one reference of a .bai or a .tbi holds (SAM/BAM specification 5.2, tabix 1.1) ----
+
+def _index_ref():
+    return {"bins": {}, "lin": {}, "first": None, "last": 0, "mapped": 0, "unmapped": 0}
+
+
+def _index_push(r, beg, end, voff_beg, voff_end, mapped=True):
+    """Adds the record [beg, end) stored at virtual offsets [voff_beg, voff_end) to one reference's index: its bin's chunks
+    (adjacent records of a bin merged into one chunk), the 16 kb windows it overlaps and the pseudo-bin's offsets and counts."""
+    chunks = r["bins"].setdefault(_reg2bin(beg, end), [])
+    if chunks and chunks[-1][1] == voff_beg:
+        chunks[-1][1] = voff_end
+    else:
+        chunks.append([voff_beg, voff_end])
+    for w in range(beg >> 14, ((end - 1) >> 14) + 1):
+        r["lin"].setdefault(w, voff_beg)
+    r["first"] = voff_beg if r["first"] is None else r["first"]
+    r["last"] = voff_end
+    r["mapped" if mapped else "unmapped"] += 1
+
+
+def _index_ref_bytes(r):
+    """One reference's bins (with the pseudo-bin 37450) and linear index, serialised."""
+    bins = dict(r["bins"])
+    if r["first"] is not None:
+        bins[_PSEUDO_BIN] = [[r["first"], r["last"]], [r["mapped"], r["unmapped"]]]
+    out = bytearray(struct.pack("<i", len(bins)))
+    for b, chunks in bins.items():
+        out += struct.pack("<Ii", b, len(chunks)) + b"".join(struct.pack("<QQ", x, y) for x, y in chunks)
+    n_intv = max(r["lin"]) + 1 if r["lin"] else 0
+    lin, prev = [], r["first"] or 0             # windows before the first record's: its offset; gaps: the previous window's
+    for w in range(n_intv):
+        prev = r["lin"].get(w, prev)
+        lin.append(prev)
+    out += struct.pack("<i", n_intv) + b"".join(struct.pack("<Q", x) for x in lin)
+    return bytes(out)
+
+
+def _read_index_refs(buf, off, n_ref):
+    """(per reference {"bins": {bin: [(beg, end)]} without the pseudo-bin, "linear": uint64 [], "mapped", "unmapped"}, end
+    offset) of the reference sections of a .bai / .tbi starting at ``buf[off:]``."""
+    out = []
+    for _ in range(n_ref):
+        n_bin, = struct.unpack_from("<i", buf, off)
+        off += 4
+        bins, mapped, unmapped = {}, 0, 0
+        for _ in range(n_bin):
+            b, n_chunk = struct.unpack_from("<Ii", buf, off)
+            off += 8
+            chunks = np.frombuffer(buf, dtype="<u8", count=2 * n_chunk, offset=off).reshape(-1, 2)
+            off += 16 * n_chunk
+            if b == _PSEUDO_BIN:
+                mapped, unmapped = (int(x) for x in chunks[1]) if n_chunk >= 2 else (0, 0)
+            else:
+                bins[b] = [(int(x), int(y)) for x, y in chunks]
+        n_intv, = struct.unpack_from("<i", buf, off)
+        off += 4
+        linear = np.frombuffer(buf, dtype="<u8", count=n_intv, offset=off).astype(np.uint64)
+        off += 8 * n_intv
+        out.append({"bins": bins, "linear": linear, "mapped": mapped, "unmapped": unmapped})
+    return out, off
+
+
+def idxstats(bam_path, bai_path=None):
+    """``samtools idxstats`` without its last ``*`` row: [(name, length, mapped, unmapped)] per reference of the BAM header, the
+    counts read from the ``.bai`` pseudo-bin (default ``bam_path + ".bai"``; 0 and 0 for a reference without one).  A missing
+    index is an error (FileNotFoundError), as there."""
+    bai_path = bai_path or str(bam_path) + ".bai"
+    if not os.path.exists(bai_path):
+        raise FileNotFoundError("%s: no BAM index (.bai) found; index the BAM first (a CSI index is not supported)" % bai_path)
+    refs, _ = read_bam_header(bam_path)
+    with open(bai_path, "rb") as f:
+        buf = f.read()
+    if buf[:4] != b"BAI\x01":
+        raise ValueError("%s: not a BAI index (magic %r)" % (bai_path, buf[:4]))
+    n_ref, = struct.unpack_from("<i", buf, 4)
+    idx, _ = _read_index_refs(buf, 8, n_ref)
+    return [(name, length, idx[i]["mapped"] if i < n_ref else 0, idx[i]["unmapped"] if i < n_ref else 0)
+            for i, (name, length) in enumerate(refs)]
+
+
+# ---- tabix (.tbi) over a BGZF-compressed VCF ----
+
+TBI_VCF = (2, 1, 2, 0, ord("#"), 0)     # format (VCF), col_seq, col_beg, col_end, meta char, skip: ``tabix -p vcf``
+
+
+def write_tbi(vcf_gz_path, text, voffset, tbi_path=None):
+    """Writes the tabix index (``tabix -p vcf``) of a VCF whose text ``text`` was written by ``write_bgzf`` (``voffset``: what it
+    returned).  Rows starting with ``#`` are skipped; a record covers [POS - 1, POS - 1 + len(REF)); the contigs are named in
+    the order the file first holds them.  The index is BGZF-compressed as tabix writes it.  Returns the path written."""
+    data = text.encode() if isinstance(text, str) else bytes(text)
+    names, idx, u = [], {}, 0
+    for line in data.splitlines(keepends=True):
+        nxt = u + len(line)
+        if not line.startswith(b"#") and line.strip():
+            c = line.rstrip(b"\r\n").split(b"\t")
+            ctg, beg = c[0].decode(), int(c[1]) - 1
+            end = beg + max(len(c[3]) if len(c) > 3 else 1, 1)
+            if ctg not in idx:
+                names.append(ctg)
+                idx[ctg] = _index_ref()
+            _index_push(idx[ctg], beg, end, voffset(u), voffset(nxt))
+        u = nxt
+    nm = b"".join(n.encode() + b"\0" for n in names)
+    out = bytearray(b"TBI\x01" + struct.pack("<i", len(names)) + struct.pack("<6i", *TBI_VCF) + struct.pack("<i", len(nm)) + nm)
+    for n in names:
+        out += _index_ref_bytes(idx[n])
+    out += struct.pack("<Q", 0)
+    path = tbi_path or str(vcf_gz_path) + ".tbi"
+    write_bgzf(path, bytes(out))
+    return path
+
+
+def read_tbi(path):
+    """A tabix index: {"header": (format, col_seq, col_beg, col_end, meta, skip), "names": [...], "refs": per contig as
+    ``_read_index_refs``, "n_no_coor"}."""
+    with gzip.open(path, "rb") as f:
+        buf = f.read()
+    if buf[:4] != b"TBI\x01":
+        raise ValueError("%s: not a tabix index (magic %r)" % (path, buf[:4]))
+    n_ref, = struct.unpack_from("<i", buf, 4)
+    header = struct.unpack_from("<6i", buf, 8)
+    l_nm, = struct.unpack_from("<i", buf, 32)
+    names = [n.decode() for n in buf[36:36 + l_nm].split(b"\0")[:n_ref]]
+    refs, off = _read_index_refs(buf, 36 + l_nm, n_ref)
+    n_no_coor = struct.unpack_from("<Q", buf, off)[0] if off + 8 <= len(buf) else None
+    return {"header": header, "names": names, "refs": refs, "n_no_coor": n_no_coor}
+
+
+def tbi_chunks(tbi, ctg, start, end):
+    """The chunks [(begin, end) virtual offsets] a tabix query of the 0-based [start, end) on ``ctg`` reads: the chunks of the
+    bins of reg2bins(start, end), less those that end before the linear index's offset for ``start``."""
+    if ctg not in tbi["names"]:
+        return []
+    ref = tbi["refs"][tbi["names"].index(ctg)]
+    lin = ref["linear"]
+    min_off = int(lin[min(start >> 14, len(lin) - 1)]) if len(lin) else 0
+    return sorted(c for b in _reg2bins(max(start, 0), max(end, start + 1)) for c in ref["bins"].get(b, ()) if c[1] > min_off)

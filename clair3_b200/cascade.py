@@ -185,6 +185,14 @@ def merge(pileup_result, fa_results, output_config_p, output_config_f, qual=2, p
     for res in fa_results:
         pos, rows = _vcf(res, output_config_f)
         f_pos, f_rows = np.concatenate([f_pos, pos]), f_rows + rows
+    return merge_rows(p_pos, p_rows, f_pos, f_rows, qual=qual, print_ref=print_ref)
+
+
+def merge_rows(p_pos, p_rows, f_pos, f_rows, qual=2, print_ref=False):
+    """``merge`` on row text: one contig's pileup rows and full-alignment rows (1-based positions, ascending, and their row
+    texts).  With no full-alignment rows this is SortVcf's ``--pileup_only`` post-processing (``postprocess_row_with_params``
+    without the haploid modes)."""
+    p_pos, f_pos = np.asarray(p_pos, np.int64), np.asarray(f_pos, np.int64)
     j = np.searchsorted(f_pos, p_pos)
     replaced = (j < len(f_pos)) & (f_pos[np.minimum(j, max(len(f_pos) - 1, 0))] == p_pos) if len(f_pos) else np.zeros(len(p_pos), bool)
     pos, rows = [], []
