@@ -6,8 +6,9 @@ pileup VCF, ``SelectCandidates`` writes bed files of full-alignment candidates, 
 file re-calls them with Clair3_F, and ``MergeVcf`` merges the two VCFs.  Here the same decisions are taken from the call
 records, in three layers each usable on its own:
 
-* ``qual_cutoffs`` (``SelectQual``), ``prob_threshold``, ``select`` / ``bed_text`` (``SelectCandidates``) and ``merge``
-  (``MergeVcf``) on host call results (``PileupCounter.call`` / ``FullAlignmentBuilder.call``);
+* ``qual_cutoffs_from`` (``SelectQual``), ``prob_threshold`` and ``candidates_from`` (``SelectCandidates``) on the rows'
+  positions, probabilities and flags (``row_summary``), and on host call results (``PileupCounter.call`` /
+  ``FullAlignmentBuilder.call``) ``qual_cutoffs``, ``select`` / ``bed_text`` and ``merge`` (``MergeVcf``);
 * ``select_device``: the same selection on the device (``c3b_cascade_select``), whose candidates a full-alignment build takes
   where they are (``FullAlignmentBuilder.build(..., cand_count=...)``);
 * ``call_region``: the whole route on one stream, and ``call_region_host``, the same calls with host records and host
@@ -27,7 +28,7 @@ import time
 import numpy as np
 import torch
 
-from . import decode
+from . import decode, targets
 from ._ffi import C3BError, check, ffi, lib
 from .fa_tensor import MATRIX_DEPTH
 
@@ -38,7 +39,10 @@ FLANK = 16                                                   # shared/param_f.py
 _ONE = 0x3F800000                                            # float32 1.0: QUAL is undefined above it (log of a negative)
 
 
-def _check_platform(platform):
+FLAG_GT00, FLAG_REF = 1, 2                                   # row_summary's flags: GT prints 0/0, ALT is "." or REF
+
+
+def check_platform(platform):
     if platform == "ilmn":
         raise NotImplementedError("cascade: platform 'ilmn' (MergeVcf_illumina and its bed geometry) is not implemented")
     if platform not in PCT_FULL:
@@ -53,7 +57,7 @@ def _check_config(cfg):
 
 
 # ------------------------------------------------------------------------------------------------ rows of a call result
-def _rows(res):
+def row_indices(res):
     """Indices of the calls that are rows of the VCF: printed, and for pileup calls ``cand_ok``."""
     m = res["calls"]["printed"] != 0
     if "cand_ok" in res:
@@ -61,7 +65,7 @@ def _rows(res):
     return np.nonzero(m)[0]
 
 
-def _is_reference(res, idx):
+def is_reference(res, idx):
     """SelectCandidates' and MergeVcf's test on the row text: ALT is "." or ALT == REF (not the genotype)."""
     calls, text, start = res["calls"], res["text"], res["start"]
     out = np.zeros(len(idx), bool)
@@ -72,35 +76,55 @@ def _is_reference(res, idx):
     return out
 
 
+def row_texts(res, cfg):
+    """(1-based positions, row texts) of a call result's VCF rows."""
+    idx = row_indices(res)
+    return np.asarray(res["position"])[idx].astype(np.int64), [decode.call_row(res, s, cfg) for s in idx]
+
+
+def row_summary(res):
+    """(1-based positions, probabilities, flags, row indices) of a pileup ``call`` result's VCF rows: what SelectQual and
+    SelectCandidates read of them, without their text (``FLAG_GT00`` | ``FLAG_REF``)."""
+    idx = row_indices(res)
+    c = res["calls"][idx]
+    flags = np.where(c["genotype"] == 0, FLAG_GT00, 0) | np.where(is_reference(res, idx), FLAG_REF, 0)
+    return np.asarray(res["position"])[idx].astype(np.int64), c["prob"].astype(np.float32), flags.astype(np.uint8), idx
+
+
+_rows, _is_reference, _vcf = row_indices, is_reference, row_texts    # the names earlier callers use
+
+
 # ------------------------------------------------------------------------------------------------ SelectQual
-def _kth_qual(probs, pct):
+def _kth_qual(p, pct):
     """The last of the lowest ``int(pct * n)`` QUALs, or 0.0 when that is none.  QUAL is monotone non-decreasing in the
     float32 probability (``prob_threshold``), so it is the QUAL of the k-th lowest probability: one host call, not one per row."""
-    p = np.concatenate(probs) if probs else np.zeros(0, np.float32)
     k = int(pct * len(p))
     if k == 0:
         return 0.0
     return decode.quality_score_from(np.partition(p, k - 1)[k - 1])
 
 
-def qual_cutoffs(results, platform="ont", var_pct_full=None, ref_pct_full=None, genotyping=False):
-    """``SelectQual`` without ``--phase`` (preprocess/SelectQual.py:select_qual_from_stdin) over any number of pileup ``call``
-    results (every region of a genome for the genome-wide cut-offs): returns (var_qual, ref_qual).  Rows whose GT prints as
-    ``0/0`` give the reference cut-off, all others the variant cut-off; ``ref_pct_full`` 0 means ``var_pct_full``, as there,
-    except in genotyping mode (``--vcf_fn``, ``genotyping=True``), where ``ref_pct_full`` is used as given (:97).  The
-    percentages default to run_clair3.py's for the platform."""
-    _check_platform(platform)
+def qual_cutoffs_from(prob, gt00, platform="ont", var_pct_full=None, ref_pct_full=None, genotyping=False):
+    """``SelectQual`` without ``--phase`` (preprocess/SelectQual.py:select_qual_from_stdin) on the (probability, GT prints as
+    ``0/0``) pairs of pileup rows (every row of a genome for the genome-wide cut-offs): returns (var_qual, ref_qual).  Rows
+    whose GT prints as ``0/0`` give the reference cut-off, all others the variant cut-off; ``ref_pct_full`` 0 means
+    ``var_pct_full``, as there, except in genotyping mode (``--vcf_fn``, ``genotyping=True``), where ``ref_pct_full`` is used as
+    given (:97).  The percentages default to run_clair3.py's for the platform."""
+    check_platform(platform)
     var_pct = PCT_FULL[platform][0] if var_pct_full is None else var_pct_full
     ref_pct = PCT_FULL[platform][1] if ref_pct_full is None else ref_pct_full
     if not genotyping:
         ref_pct = ref_pct if ref_pct else var_pct
-    ref_p, var_p = [], []
-    for res in results:
-        c = res["calls"][_rows(res)]
-        gt00 = c["genotype"] == 0                       # decode.GENOTYPES: 0 prints "0/0"
-        ref_p.append(c["prob"][gt00])
-        var_p.append(c["prob"][~gt00])
-    return _kth_qual(var_p, var_pct), _kth_qual(ref_p, ref_pct)
+    prob, gt00 = np.asarray(prob, np.float32), np.asarray(gt00, bool)
+    return _kth_qual(prob[~gt00], var_pct), _kth_qual(prob[gt00], ref_pct)
+
+
+def qual_cutoffs(results, platform="ont", var_pct_full=None, ref_pct_full=None, genotyping=False):
+    """``qual_cutoffs_from`` over the VCF rows of any number of pileup ``call`` results."""
+    calls = [res["calls"][row_indices(res)] for res in results]
+    prob = np.concatenate([c["prob"] for c in calls] + [np.zeros(0, np.float32)])
+    gt00 = np.concatenate([c["genotype"] == 0 for c in calls] + [np.zeros(0, bool)])      # decode.GENOTYPES: 0 prints "0/0"
+    return qual_cutoffs_from(prob, gt00, platform, var_pct_full, ref_pct_full, genotyping)
 
 
 def _qual_of_bits(bits):
@@ -122,19 +146,27 @@ def prob_threshold(cut):
 
 
 # ------------------------------------------------------------------------------------------------ SelectCandidates
-def _chunks(n, split_bed_size):
+def bed_chunks(n, split_bed_size):
+    """[(lo, hi)] index ranges of the bed files over ``n`` candidates, ``split_bed_size`` each."""
     return [(i, min(i + split_bed_size, n)) for i in range(0, n, split_bed_size)]
 
 
+def candidates_from(pos, prob, is_ref, var_qual, ref_qual):
+    """``SelectCandidates`` (preprocess/SelectCandidates.py:187-270, ``--phasing_info_in_bam`` at its default) on one contig's
+    pileup rows (1-based positions, probabilities, ALT is "." or REF): the reference rows with QUAL < ``ref_qual`` and the
+    other rows with QUAL < ``var_qual``.  Returns their 0-based positions, int64, sorted and unique."""
+    bits = np.asarray(prob, np.float32).view(np.uint32).astype(np.int64)
+    t = np.where(np.asarray(is_ref, bool), prob_threshold(ref_qual), prob_threshold(var_qual))
+    return np.unique(np.asarray(pos, np.int64)[bits < t] - 1).astype(np.int64)
+
+
 def select(pileup_result, var_qual, ref_qual, split_bed_size=SPLIT_BED_SIZE):
-    """``SelectCandidates`` (preprocess/SelectCandidates.py:187-270, ``--phasing_info_in_bam`` at its default) on one region's
-    pileup ``call`` result: reference rows (by ALT text) with QUAL < ``ref_qual`` and the other rows with QUAL < ``var_qual``.
-    Returns (0-based positions int64, sorted and unique; [(lo, hi)] index ranges of the bed files, ``split_bed_size`` each)."""
-    idx = _rows(pileup_result)
-    bits = pileup_result["calls"]["prob"][idx].view(np.uint32)
-    t = np.where(_is_reference(pileup_result, idx), prob_threshold(ref_qual), prob_threshold(var_qual)).astype(np.int64)
-    pos = np.unique(np.asarray(pileup_result["position"])[idx][bits.astype(np.int64) < t] - 1).astype(np.int64)
-    return pos, _chunks(len(pos), split_bed_size)
+    """``candidates_from`` on one region's pileup ``call`` result, the reference rows by ALT text.  Returns (0-based positions
+    int64, sorted and unique; ``bed_chunks`` of them)."""
+    idx = row_indices(pileup_result)
+    pos = candidates_from(np.asarray(pileup_result["position"])[idx], pileup_result["calls"]["prob"][idx],
+                          is_reference(pileup_result, idx), var_qual, ref_qual)
+    return pos, bed_chunks(len(pos), split_bed_size)
 
 
 def bed_text(ctg, positions):
@@ -166,12 +198,6 @@ def select_device(pileup_result, var_qual, ref_qual):
 
 
 # ------------------------------------------------------------------------------------------------ MergeVcf
-def _vcf(res, cfg):
-    """(1-based positions, row texts) of a call result's VCF rows."""
-    idx = _rows(res)
-    return np.asarray(res["position"])[idx].astype(np.int64), [decode.call_row(res, s, cfg) for s in idx]
-
-
 def merge(pileup_result, fa_results, output_config_p, output_config_f, qual=2, print_ref=False):
     """``MergeVcf`` (preprocess/MergeVcf.py, the non-ilmn ``MergeVcf``) of one region: the merged VCF body, byte for byte
     what it writes after the header.  A full-alignment row of any kind drops the pileup row at its position; reference rows
@@ -180,10 +206,10 @@ def merge(pileup_result, fa_results, output_config_p, output_config_f, qual=2, p
     order."""
     for cfg in (output_config_p, output_config_f):
         _check_config(cfg)
-    p_pos, p_rows = _vcf(pileup_result, output_config_p)
+    p_pos, p_rows = row_texts(pileup_result, output_config_p)
     f_pos, f_rows = np.zeros(0, np.int64), []
     for res in fa_results:
-        pos, rows = _vcf(res, output_config_f)
+        pos, rows = row_texts(res, output_config_f)
         f_pos, f_rows = np.concatenate([f_pos, pos]), f_rows + rows
     return merge_rows(p_pos, p_rows, f_pos, f_rows, qual=qual, print_ref=print_ref)
 
@@ -215,19 +241,13 @@ def merge_rows(p_pos, p_rows, f_pos, f_rows, qual=2, print_ref=False):
 
 # ------------------------------------------------------------------------------------------------ targets
 def contig_targets(ctg, bed=None, known_sites=None):
-    """One contig's ``targets.ContigTargets`` from ``bed`` / ``known_sites``: a path (gzip or plain), a ``targets.Targets``
-    (``read_bed`` / ``read_vcf``) or already a ``ContigTargets`` (``Targets.contig(ctg, chunk=...)``); None for neither.
-    Giving both is a ValueError, as CheckEnvs refuses ``--bed_fn`` with ``--vcf_fn``."""
-    from . import targets as tg
-    if bed is not None and known_sites is not None:
-        raise ValueError("cascade: give either bed or known_sites, not both (the reference refuses --bed_fn with --vcf_fn)")
-    src, read = (bed, tg.read_bed) if bed is not None else (known_sites, tg.read_vcf)
-    if src is None:
+    """One contig's ``targets.ContigTargets`` from ``bed`` / ``known_sites`` (``targets.resolve``: a path, a ``targets.Targets``
+    or already a ``ContigTargets``, ``Targets.contig(ctg, chunk=...)``); None for neither."""
+    t = targets.resolve(bed, known_sites)
+    if t is None:
         return None
-    if isinstance(src, tg.ContigTargets):
-        t = src
-    else:
-        t = (src if isinstance(src, tg.Targets) else read(src)).contig(ctg)
+    if isinstance(t, targets.Targets):
+        t = t.contig(ctg)
     if (t.known is not None) != (known_sites is not None):
         raise ValueError("cascade: bed needs a BED's targets and known_sites a VCF's")
     return t
@@ -251,13 +271,6 @@ def take_calls(res, idx):
 MAJOR_CONTIGS = ["chr%s" % a for a in list(range(1, 23)) + ["X", "Y"]] + [str(a) for a in list(range(1, 23)) + ["X", "Y"]]
 
 
-def _known_rows(known_vcf):
-    from . import targets as tg
-    if isinstance(known_vcf, tg.ContigTargets):
-        return {(known_vcf.ctg, p): r for p, r in known_vcf.rows.items()}
-    return (known_vcf if isinstance(known_vcf, tg.Targets) else tg.read_vcf(known_vcf)).rows
-
-
 def add_back_missing(merged_body, known_vcf, region=None):
     """AddBackMissingVariantsInGenotyping (postprocess/AddBackMissingVariantsInGenotyping.py:94-159, ``switch_genotype`` at
     its default) on a merged VCF body: one row per known site and nothing else - Clair3's row where it called the site, the
@@ -267,7 +280,8 @@ def add_back_missing(merged_body, known_vcf, region=None):
     of duplicate (contig, position) keys the last row wins.  ``known_vcf``: a path, ``targets.read_vcf``'s ``Targets`` or a
     ``ContigTargets`` (its known sites only).  ``region`` = (ctg, start, end): only the known sites inside the 0-based
     [start, end), which ``call_region`` is responsible for."""
-    known = _known_rows(known_vcf)
+    t = targets.resolve(known_sites=known_vcf)
+    known = {(t.ctg, p): r for p, r in t.rows.items()} if isinstance(t, targets.ContigTargets) else t.rows
     if region is not None:
         c, a, b = region
         known = {k: r for k, r in known.items() if k[0] == c and a < k[1] <= b}
@@ -307,7 +321,7 @@ class Workspaces:
             w.close()
 
 
-class _Stages:
+class Stages:
     """CUDA events and host clock at the stage boundaries of a route (no host wait: read after the route has waited)."""
 
     def __init__(self, device):
@@ -320,13 +334,27 @@ class _Stages:
         self.marks.append((name, ev, time.perf_counter()))
 
     def report(self):
+        """[{stage, wall_ms, device_ms}] per stage, in order."""
         torch.cuda.current_stream(self.device).synchronize()
         return [{"stage": b[0], "wall_ms": 1e3 * (b[2] - a[2]), "device_ms": a[1].elapsed_time(b[1])}
                 for a, b in zip(self.marks, self.marks[1:])]
 
+    def summed(self):
+        """``report`` summed per stage name, {name: {wall_ms, device_ms, count}}, and ``total``: {wall_ms} since the start."""
+        out = {}
+        for r in self.report():
+            s = out.setdefault(r["stage"], {"wall_ms": 0.0, "device_ms": 0.0, "count": 0})
+            s["wall_ms"] += r["wall_ms"]
+            s["device_ms"] += r["device_ms"]
+            s["count"] += 1
+        out["total"] = {"wall_ms": 1e3 * (time.perf_counter() - self.marks[0][2])}
+        return out
 
-def _route_args(platform, output_config_p, output_config_f, fa_params):
-    _check_platform(platform)
+
+def _route_args(ctg, platform, output_config_p, output_config_f, fa_params, bed, known_sites):
+    """What both routes check and take from their arguments: (the full-alignment builds' keyword arguments, the contig's
+    ``ContigTargets`` or None, genotyping mode)."""
+    check_platform(platform)
     for cfg in (output_config_p, output_config_f):
         _check_config(cfg)
         if not cfg.is_show_reference:
@@ -335,7 +363,25 @@ def _route_args(platform, output_config_p, output_config_f, fa_params):
             raise ValueError("cascade: both output configs need is_show_reference=True, as the reference's pipeline runs")
     fa = {"matrix_depth": MATRIX_DEPTH[platform]}
     fa.update(fa_params or {})
-    return fa
+    return fa, contig_targets(ctg, bed, known_sites), known_sites is not None
+
+
+def _own_cutoffs(pres, var_qual, ref_qual, platform, genotyping):
+    """(var_qual, ref_qual), each None replaced by the region's own: ``qual_cutoffs`` of its pileup calls."""
+    if var_qual is None or ref_qual is None:
+        own_var, own_ref = qual_cutoffs([pres], platform, genotyping=genotyping)
+        var_qual = own_var if var_qual is None else var_qual
+        ref_qual = own_ref if ref_qual is None else ref_qual
+    return var_qual, ref_qual
+
+
+def _route_result(region, tgt, genotyping, vcf, pres, fres, cuts, candidates, chunks, **more):
+    """Both routes' result dict; in genotyping mode with ``genotyped``, the body after ``add_back_missing``."""
+    out = {"vcf": vcf, "pileup": pres, "full_alignment": fres, "qual_cutoffs": cuts, "candidates": candidates, "chunks": chunks,
+           **more}
+    if genotyping:
+        out["genotyped"] = add_back_missing(vcf, tgt, region=region)
+    return out
 
 
 def _span(start, end):
@@ -363,25 +409,18 @@ def call_region(bam_path, ctg, start, end, ref_seq, ref_start, model_p, model_f,
     Returns a dict: ``vcf`` (the merged body), ``pileup`` and ``full_alignment`` (the ``call`` results), ``qual_cutoffs``,
     ``candidates`` (int64 0-based, host), ``chunks`` and ``stages`` (wall and device ms per stage); with ``known_sites`` also
     ``genotyped``, the body after ``add_back_missing`` over the known sites inside the region."""
-    fa = _route_args(platform, output_config_p, output_config_f, fa_params)
-    tgt = contig_targets(ctg, bed, known_sites)
-    genotyping = known_sites is not None
+    fa, tgt, genotyping = _route_args(ctg, platform, output_config_p, output_config_f, fa_params, bed, known_sites)
     own = workspaces is None
     ws = workspaces or Workspaces(device)
-    dev = ws.counter._device
     try:
-        st = _Stages(dev)
+        st = Stages(ws.counter._device)
         lo, hi = _span(start, end)
-        ref = torch.from_numpy(np.frombuffer(ref_seq.encode() if isinstance(ref_seq, str) else bytes(ref_seq), np.uint8).copy())
-        rec = ws.decoder.decode(bam_path, ctg, lo, hi, fa_fields=True, ref_seq=ref.to(dev), index=index)
+        rec = ws.decoder.decode(bam_path, ctg, lo, hi, fa_fields=True, ref_seq=ref_seq, index=index)
         st.mark("decode")
         pres = ws.counter.count(rec, start, end, None, ref_start, alt_info=True, targets=tgt,
                                 **(count_params or {})).call(model_p, output_config_p, ctg, k=k)
         st.mark("pileup")
-        if var_qual is None or ref_qual is None:
-            own_var, own_ref = qual_cutoffs([pres], platform, genotyping=genotyping)
-            var_qual = own_var if var_qual is None else var_qual
-            ref_qual = own_ref if ref_qual is None else ref_qual
+        var_qual, ref_qual = _own_cutoffs(pres, var_qual, ref_qual, platform, genotyping)
         selected, count = select_device(pres, var_qual, ref_qual)
         st.mark("select")
         fres, first, total = [], 0, None
@@ -397,11 +436,8 @@ def call_region(bam_path, ctg, start, end, ref_seq, ref_start, model_p, model_f,
         vcf = merge(pres, fres, output_config_p, output_config_f, qual=qual, print_ref=print_ref)
         st.mark("merge")
         stages = st.report()
-        out = {"vcf": vcf, "pileup": pres, "full_alignment": fres, "qual_cutoffs": (var_qual, ref_qual),
-               "candidates": selected[:total].cpu().numpy(), "chunks": _chunks(total, split_bed_size), "stages": stages}
-        if genotyping:
-            out["genotyped"] = add_back_missing(vcf, tgt, region=(ctg, start, end))
-        return out
+        return _route_result((ctg, start, end), tgt, genotyping, vcf, pres, fres, (var_qual, ref_qual),
+                             selected[:total].cpu().numpy(), bed_chunks(total, split_bed_size), stages=stages)
     finally:
         if own:
             ws.close()
@@ -414,9 +450,7 @@ def call_region_host(bam_path, ctg, start, end, ref_seq, ref_start, model_p, mod
     host -> one host-candidate build per chunk -> call -> ``merge``.  Same arguments and result (without ``stages``); the
     count is untargeted and ``bed`` / ``known_sites`` drop the other candidates from its call results (``ContigTargets.keep``)."""
     from . import bam_io
-    fa = _route_args(platform, output_config_p, output_config_f, fa_params)
-    tgt = contig_targets(ctg, bed, known_sites)
-    genotyping = known_sites is not None
+    fa, tgt, genotyping = _route_args(ctg, platform, output_config_p, output_config_f, fa_params, bed, known_sites)
     own = workspaces is None
     ws = workspaces or Workspaces(device)
     try:
@@ -426,19 +460,12 @@ def call_region_host(bam_path, ctg, start, end, ref_seq, ref_start, model_p, mod
                                                                                                               ctg, k=k)
         if tgt is not None:
             pres = take_calls(pres, np.nonzero(tgt.keep(pres["position"]))[0])
-        if var_qual is None or ref_qual is None:
-            own_var, own_ref = qual_cutoffs([pres], platform, genotyping=genotyping)
-            var_qual = own_var if var_qual is None else var_qual
-            ref_qual = own_ref if ref_qual is None else ref_qual
+        var_qual, ref_qual = _own_cutoffs(pres, var_qual, ref_qual, platform, genotyping)
         pos, chunks = select(pres, var_qual, ref_qual, split_bed_size)
         fres = [ws.builder.build(rec, pos[a:b], ref_seq, ref_start, variants=phased_variants, rand_seed=1, rand_skip=0, **fa)
                 .call(model_f, output_config_f, ctg, k=k) for a, b in chunks]
         vcf = merge(pres, fres, output_config_p, output_config_f, qual=qual, print_ref=print_ref)
-        out = {"vcf": vcf, "pileup": pres, "full_alignment": fres, "qual_cutoffs": (var_qual, ref_qual), "candidates": pos,
-               "chunks": chunks}
-        if genotyping:
-            out["genotyped"] = add_back_missing(vcf, tgt, region=(ctg, start, end))
-        return out
+        return _route_result((ctg, start, end), tgt, genotyping, vcf, pres, fres, (var_qual, ref_qual), pos, chunks)
     finally:
         if own:
             ws.close()

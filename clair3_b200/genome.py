@@ -8,7 +8,9 @@ bed file, SortVcf, MergeVcf per contig, SortVcf and, with ``--vcf_fn``, AddBackM
 * ``plan`` is CheckEnvs: the contigs to call and the CHUNK_LIST;
 * ``header``, ``sort_rows`` and ``vcf_text`` are SortVcf's file text, ``write_vcf_gz`` its ``bgzip`` and ``tabix -p vcf``;
 * ``exchange`` takes every pileup chunk's rows to the genome-wide decisions: the duplicate rows of overlapping chunks dropped
-  as SortVcf drops them, SelectQual's cut-offs (``qual_cutoffs_from``) and SelectCandidates' bed files (``candidates_from``);
+  as SortVcf drops them, SelectQual's cut-offs (``cascade.qual_cutoffs_from``) and SelectCandidates' bed files
+  (``cascade.candidates_from``);
+* ``file_texts`` turns the rows of the whole run into the files' texts: SortVcf, MergeVcf, the add-back and the early exits;
 * ``call_genome`` runs it all on one ``cascade.Workspaces``, on one GPU or, with a ``torch.distributed`` group, one process per
   GPU: contiguous runs of pileup chunks and of bed files per rank, with only the rows' (position, probability, flags) sent to
   every rank and the row texts sent to rank 0, which writes the files.
@@ -22,13 +24,13 @@ haploid modes and ``platform="ilmn"`` (``NotImplementedError``); CRAM input and 
 """
 from __future__ import annotations
 
+import functools
 import os
-import time
 
 import numpy as np
 import torch
 
-from . import bam_io, cascade, decode
+from . import bam_io, cascade, decode, targets
 from .fa_tensor import MATRIX_DEPTH
 from .pileup_counts import FETCH_EXPAND, bed_chunk_region, chunk_region, counting_region, known_sites_chunk
 from .sharding import site_range
@@ -37,14 +39,14 @@ CHUNK_SIZE = 5_000_000                # CheckEnvs --chunk_size
 CLAIR3_VERSION = "2.0.2"              # shared/version.py: the ##clair3_version line of the reference this project restates
 LONG_INDEL = 100000                   # shared/param_{p,f}.py maximum_variant_length_that_need_infer_include_long_indel
 
-_FLAG_GT00, _FLAG_REF = 1, 2          # per pileup row: GT prints 0/0 (SelectQual's split), ALT is "." or REF (SelectCandidates')
+row_summary = cascade.row_summary     # where earlier callers find it
 
 
 # ------------------------------------------------------------------------------------------------ options
 def resolve_options(platform="ont", var_pct_full=None, ref_pct_full=None, snp_min_af=None, indel_min_af=None, genotyping=False):
     """run_clair3.py's per-platform defaults (:303-321, :393-395): (var_pct_full, ref_pct_full, snp_min_af, indel_min_af), where
     None or 0 means the platform's value, and a known-sites VCF sets both allele-frequency thresholds to 0."""
-    cascade._check_platform(platform)
+    cascade.check_platform(platform)
     var = var_pct_full or cascade.PCT_FULL[platform][0]
     ref = ref_pct_full or cascade.PCT_FULL[platform][1]
     snp = snp_min_af or 0.08
@@ -67,17 +69,6 @@ def output_configs(enable_long_indel=False):
 
 
 # ------------------------------------------------------------------------------------------------ CheckEnvs
-def _targets(bed=None, known_sites=None):
-    from . import targets as tg
-    if bed is not None and known_sites is not None:
-        raise ValueError("genome: give either a BED or a known-sites VCF, not both (CheckEnvs refuses --bed_fn with --vcf_fn)")
-    if bed is not None:
-        return bed if isinstance(bed, tg.Targets) else tg.read_bed(bed)
-    if known_sites is not None:
-        return known_sites if isinstance(known_sites, tg.Targets) else tg.read_vcf(known_sites)
-    return None
-
-
 def bam_index(bam_fn):
     """The ``.bai`` of a BAM as run_clair3.py and the pipeline look for it (clair3_c_impl_pipeline.py:366-382):
     ``<bam>.bai``, else ``<bam without its extension>.bai``; None when neither exists."""
@@ -121,7 +112,7 @@ def plan(bam_fn, ref_fn, ctg_name=None, include_all_ctgs=False, min_contig_size=
     (the reference keeps it and then fails writing the CHUNK_LIST).  ``idxstats``: ``bam_io.idxstats``' rows, read from the
     BAM's index (``bam_index``) by default."""
     bai = check_inputs(bam_fn, ref_fn)
-    tgt = _targets(bed, known_sites)
+    tgt = targets.resolve(bed, known_sites)
     names = [n for n in (ctg_name.split(",") if ctg_name and ctg_name != "EMPTY" else []) if n]
     given = bool(names)
     wanted = set(names)
@@ -220,43 +211,15 @@ def write_vcf_gz(path, text):
 
 
 # ------------------------------------------------------------------------------------------------ the genome-wide decisions
-def qual_cutoffs_from(prob, gt00, platform="ont", var_pct_full=None, ref_pct_full=None, genotyping=False):
-    """``cascade.qual_cutoffs`` on the (probability, GT is 0/0) pairs of every pileup row of the genome."""
-    cascade._check_platform(platform)
-    var_pct = cascade.PCT_FULL[platform][0] if var_pct_full is None else var_pct_full
-    ref_pct = cascade.PCT_FULL[platform][1] if ref_pct_full is None else ref_pct_full
-    if not genotyping:
-        ref_pct = ref_pct if ref_pct else var_pct
-    prob, gt00 = np.asarray(prob, np.float32), np.asarray(gt00, bool)
-    return cascade._kth_qual([prob[~gt00]], var_pct), cascade._kth_qual([prob[gt00]], ref_pct)
-
-
-def candidates_from(pos, prob, is_ref, var_qual, ref_qual):
-    """``cascade.select``'s positions on one contig's pileup rows (1-based positions, probabilities, ALT is "." or REF): 0-based,
-    sorted and unique."""
-    bits = np.asarray(prob, np.float32).view(np.uint32).astype(np.int64)
-    t = np.where(np.asarray(is_ref, bool), cascade.prob_threshold(ref_qual), cascade.prob_threshold(var_qual))
-    return np.unique(np.asarray(pos, np.int64)[bits < t] - 1).astype(np.int64)
-
-
-def row_summary(res):
-    """(1-based positions, probabilities, flags, row indices) of a pileup ``call`` result's VCF rows: what the other ranks need
-    of them."""
-    idx = cascade._rows(res)
-    c = res["calls"][idx]
-    flags = np.where(c["genotype"] == 0, _FLAG_GT00, 0) | np.where(cascade._is_reference(res, idx), _FLAG_REF, 0)
-    return np.asarray(res["position"])[idx].astype(np.int64), c["prob"].astype(np.float32), flags.astype(np.uint8), idx
-
-
 def exchange(chunk_rows, contigs, platform="ont", var_pct_full=None, ref_pct_full=None, genotyping=False,
              split_bed_size=cascade.SPLIT_BED_SIZE):
     """The genome-wide decisions from every pileup chunk's rows.  ``chunk_rows``: per CHUNK_LIST row, in its order, (contig,
-    positions, probabilities, flags) as ``row_summary`` gives them.  Returns (keep: per chunk a bool mask of its rows that
-    pileup.vcf keeps - of a position repeated by overlapping chunks the last chunk's row, as SortVcf keeps it -, (var_qual,
-    ref_qual), beds: [(contig, 0-based candidate positions)] per bed file, in contig order).  The rows a position repeats are
-    identical except under head / tail calling, where a candidate near a chunk's edge gets a padded window in one chunk and a
-    whole one in the next; the reference then keeps whichever file ``os.listdir`` lists last, which has no fixed order, and
-    this route keeps the last chunk's row."""
+    positions, probabilities, flags) as ``cascade.row_summary`` gives them.  Returns (keep: per chunk a bool mask of its rows
+    that pileup.vcf keeps - of a position repeated by overlapping chunks the last chunk's row, as SortVcf keeps it -,
+    (var_qual, ref_qual), beds: [(contig, 0-based candidate positions)] per bed file, in contig order).  The rows a position
+    repeats are identical except under head / tail calling, where a candidate near a chunk's edge gets a padded window in one
+    chunk and a whole one in the next; the reference then keeps whichever file ``os.listdir`` lists last, which has no fixed
+    order, and this route keeps the last chunk's row."""
     keep = [np.zeros(len(r[1]), bool) for r in chunk_rows]
     for ctg in {r[0] for r in chunk_rows}:
         gs = [g for g, r in enumerate(chunk_rows) if r[0] == ctg]
@@ -271,15 +234,15 @@ def exchange(chunk_rows, contigs, platform="ont", var_pct_full=None, ref_pct_ful
             keep[g][row[hit]] = True
     cat = lambda k: np.concatenate([np.asarray(r[k])[m] for r, m in zip(chunk_rows, keep)]) if chunk_rows else np.zeros(0)  # noqa: E731
     prob, flags = cat(2).astype(np.float32), cat(3).astype(np.uint8)
-    cuts = qual_cutoffs_from(prob, flags & _FLAG_GT00, platform, var_pct_full, ref_pct_full, genotyping)
+    cuts = cascade.qual_cutoffs_from(prob, flags & cascade.FLAG_GT00, platform, var_pct_full, ref_pct_full, genotyping)
     beds = []
     for ctg in [c for c, _ in contigs]:
         sel = [(np.asarray(r[1])[m], np.asarray(r[2])[m], np.asarray(r[3])[m]) for r, m in zip(chunk_rows, keep) if r[0] == ctg]
         if not sel:
             continue
-        pos = candidates_from(np.concatenate([s[0] for s in sel]), np.concatenate([s[1] for s in sel]).astype(np.float32),
-                              np.concatenate([s[2] for s in sel]) & _FLAG_REF, *cuts)
-        beds.extend((ctg, pos[a:b]) for a, b in cascade._chunks(len(pos), split_bed_size))
+        pos = cascade.candidates_from(np.concatenate([s[0] for s in sel]), np.concatenate([s[1] for s in sel]),
+                                      np.concatenate([s[2] for s in sel]) & cascade.FLAG_REF, *cuts)
+        beds.extend((ctg, pos[a:b]) for a, b in cascade.bed_chunks(len(pos), split_bed_size))
     return keep, cuts, beds
 
 
@@ -330,27 +293,6 @@ def pileup_chunk_region(ctg, length, chunk_id, chunk_num, tgt=None):
 
 
 # ------------------------------------------------------------------------------------------------ the route
-class _StageClock:
-    """``cascade._Stages`` summed per stage name over a whole run."""
-
-    def __init__(self, device):
-        self.st = cascade._Stages(device)
-        self.t0 = time.perf_counter()
-
-    def mark(self, name):
-        self.st.mark(name)
-
-    def report(self):
-        out = {}
-        for r in self.st.report():
-            s = out.setdefault(r["stage"], {"wall_ms": 0.0, "device_ms": 0.0, "count": 0})
-            s["wall_ms"] += r["wall_ms"]
-            s["device_ms"] += r["device_ms"]
-            s["count"] += 1
-        out["total"] = {"wall_ms": 1e3 * (time.perf_counter() - self.t0)}
-        return out
-
-
 def _rank(group):
     if group is None:
         return 0, 1
@@ -385,9 +327,7 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
                 device=None, group=None, k=16):
     """Clair3's pipeline (scripts/clair3_c_impl_pipeline.py with ``--no_phasing_for_fa True``) over the genome: writes
     ``pileup.vcf.gz``, ``full_alignment.vcf.gz`` and ``merge_output.vcf.gz`` with their ``.tbi`` into ``out_dir``, as the
-    reference does with its early exits (no contig: a header-only ``merge_output``; no pileup row, no full-alignment
-    candidate or no full-alignment row: ``merge_output`` is a copy of ``pileup.vcf.gz``; ``pileup_only``: ``pileup.vcf.gz``
-    alone).  Options as run_clair3.py names them (None / 0 percentages and allele frequencies: the platform's defaults, see
+    reference does with its early exits (``file_texts``).  Options as run_clair3.py names them (None / 0 percentages and allele frequencies: the platform's defaults, see
     ``resolve_options``); ``bed_fn`` / ``vcf_fn`` also take ``targets.read_bed`` / ``read_vcf`` results.  ``cmdline``: the
     ``##cmdline=`` header line (None: none).  ``chunk_size`` / ``split_bed_size``: CheckEnvs' and SelectCandidates' sizes.
     ``group``: a ``torch.distributed`` process group (one process per GPU, each on its own ``device``); every rank must call
@@ -403,131 +343,139 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
         raise NotImplementedError("genome: gVCF output is not implemented")
     if haploid_precise or haploid_sensitive:
         raise NotImplementedError("genome: the haploid modes are not implemented")
-    cascade._check_platform(platform)
+    cascade.check_platform(platform)
     if enable_dwell_time and platform != "ont":
         raise ValueError("genome: dwell time is only supported for platform 'ont' (run_clair3.py refuses it too)")
-    tgt = _targets(bed_fn, vcf_fn)
+    tgt = targets.resolve(bed_fn, vcf_fn)
     genotyping = tgt is not None and tgt.kind == "vcf"
     var_pct, ref_pct, snp_af, indel_af = resolve_options(platform, var_pct_full, ref_pct_full, snp_min_af, indel_min_af, genotyping)
     cfg_p, cfg_f = output_configs(enable_long_indel)
     max_indel = LONG_INDEL if enable_long_indel else decode.MAX_INFER_LENGTH
     rank, world = _rank(group)
     contigs, chunks = plan(bam_fn, ref_fn, ctg_name, include_all_ctgs, min_contig_size, chunk_size,
-                           bed=tgt if tgt is not None and tgt.kind == "bed" else None, known_sites=tgt if genotyping else None)
-    out_dir = str(out_dir)
-    paths = {n: os.path.join(out_dir, n + ".vcf.gz") for n in ("pileup", "full_alignment", "merge_output")}
+                           bed=None if genotyping else tgt, known_sites=tgt if genotyping else None)
     head = header(ref_fn, sample_name, cmdline)
-    texts = {}
-
-    def finish(stages=None):
-        if rank != 0:
-            return None
-        os.makedirs(out_dir, exist_ok=True)
-        for name, text in texts.items():
-            write_vcf_gz(paths[name], text)
-        return {"files": {n: paths[n] for n in texts}, "texts": dict(texts), "contigs": contigs, "chunks": chunks,
-                "qual_cutoffs": cuts, "beds": len(beds), "rows": {n: _records(t) for n, t in texts.items()},
-                "stages": stages}
-
-    cuts, beds = None, []
+    names = [c for c, _ in contigs]
+    out = {"contigs": contigs, "chunks": chunks, "qual_cutoffs": None, "beds": 0, "stages": None}
     if not contigs:
-        texts["merge_output"] = head
-        return finish()
+        return _write(out_dir, file_texts(head, names, [], []), out) if rank == 0 else None
+    lengths = dict(contigs)
+    index = bam_io.read_bai(bam_index(bam_fn))          # parsed once; the decoder reads each region's byte range through it
     own = workspaces is None
     if device is None:
         device = workspaces.counter._device if workspaces is not None else torch.cuda.current_device()
     ws = workspaces or cascade.Workspaces(device)
-    dev = ws.counter._device
-    lengths = dict(contigs)
-    index = bam_io.read_bai(bam_index(bam_fn))          # parsed once; the decoder reads each region's byte range through it
     try:
-        clock = _StageClock(dev)
-        # ---- pileup: a contiguous run of CHUNK_LIST rows per rank
-        lo, hi = site_range(len(chunks), rank, world)
-        mine = []
-        for g in range(lo, hi):
-            ctg, cid, n = chunks[g]
-            region = pileup_chunk_region(ctg, lengths[ctg], cid, n, tgt)
-            if region is None:
-                mine.append((g, ctg, np.zeros(0, np.int64), np.zeros(0, np.float32), np.zeros(0, np.uint8), []))
-                continue
-            (start, end), ct = region
-            r0, r1 = max(0, start - FETCH_EXPAND), min(lengths[ctg], end + FETCH_EXPAND + 1)
-            ref = bam_io.fetch_fasta(ref_fn, ctg, r0, r1)
-            rec = ws.decoder.decode(bam_fn, ctg, start, end, fa_fields=False, index=index,
-                                    ref_seq=torch.from_numpy(np.frombuffer(ref.encode(), np.uint8).copy()).to(dev))
-            clock.mark("decode")
-            res = ws.counter.count(rec, start, end, None, r0, min_depth=min_coverage, min_snp_af=snp_af, min_indel_af=indel_af,
-                                   min_mq=min_mq, call_snp_only=call_snp_only,
-                                   call_ht=enable_variant_calling_at_sequence_head_and_tail, alt_info=True,
-                                   max_indel_length=max_indel, targets=ct).call(model_p, cfg_p, ctg, k=k)
-            clock.mark("pileup")
-            pos, prob, flags, idx = row_summary(res)
-            rows = [decode.call_row(res, s, cfg_p) for s in idx]
-            mine.append((g, ctg, pos, prob, flags, rows))
-            del rec, res
-            clock.mark("pileup format")
-        # ---- every rank: the rows' positions, probabilities and flags -> duplicates, cut-offs, bed files
+        st = cascade.Stages(ws.counter._device)
+        read = functools.partial(_read_span, ws.decoder, bam_fn, ref_fn, index, lengths)
+        count = {"min_depth": min_coverage, "min_snp_af": snp_af, "min_indel_af": indel_af, "min_mq": min_mq,
+                 "call_snp_only": call_snp_only, "call_ht": enable_variant_calling_at_sequence_head_and_tail,
+                 "max_indel_length": max_indel}
+        mine = _pileup_chunks(ws.counter, st, read, lengths, chunks, range(*site_range(len(chunks), rank, world)), tgt,
+                              model_p, cfg_p, k, count)
+        # every rank: the rows' positions, probabilities and flags -> duplicates, cut-offs, bed files
         keep, cuts, beds = decisions([m[:5] for m in mine], contigs, platform, var_pct, ref_pct, genotyping, split_bed_size, group)
-        clock.mark("cutoffs and select")
-        n_rows = sum(int(m.sum()) for m in keep)
-        # ---- full alignment: a contiguous run of bed files per rank
+        st.mark("cutoffs and select")
         fa_rows = []
-        if n_rows and not pileup_only:
-            b0, b1 = site_range(len(beds), rank, world)
+        if not pileup_only:
             fa = {"matrix_depth": MATRIX_DEPTH[platform], "need_haplotagging": False, "min_mq": min_mq,
                   "max_indel_length": max_indel, "dwell": bool(enable_dwell_time), "rand_seed": 1, "rand_skip": 0}
-            for b in range(b0, b1):
-                ctg, cand = beds[b]
-                s, e = bed_span(cand)
-                r0, r1 = max(0, s - FETCH_EXPAND), min(lengths[ctg], e + FETCH_EXPAND + 1)
-                ref = bam_io.fetch_fasta(ref_fn, ctg, r0, r1)
-                rec = ws.decoder.decode(bam_fn, ctg, s, e, fa_fields=True, index=index,
-                                        ref_seq=torch.from_numpy(np.frombuffer(ref.encode(), np.uint8).copy()).to(dev))
-                clock.mark("fa decode")
-                res = ws.builder.build(rec, cand, None, r0, **fa).call(model_f, cfg_f, ctg, k=k)
-                clock.mark("fa build and call")
-                pos, rows = cascade._vcf(res, cfg_f)
-                fa_rows.append((b, ctg, pos, rows))
-                del rec, res
-                clock.mark("fa format")
-        # ---- rank 0: the row texts
+            fa_rows = _bed_files(ws.builder, st, read, beds, range(*site_range(len(beds), rank, world)), model_f, cfg_f, k, fa)
+        # rank 0: the row texts
         kept = [(g, ctg, pos[keep[g]], [r for r, k_ in zip(rows, keep[g]) if k_]) for g, ctg, pos, _, _, rows in mine]
         parts = _gather0((kept, fa_rows), group, world, rank)
-        clock.mark("gather")
+        st.mark("gather")
         if rank != 0:
             return None
-        p_chunks = sorted((c for part in parts for c in part[0]), key=lambda c: c[0])
-        f_beds = sorted((c for part in parts for c in part[1]), key=lambda c: c[0])
-        names = [c for c, _ in contigs]
-        p_body = sort_rows((r for c in p_chunks for r in c[3]), names)
-        if not n_rows:
-            texts["pileup"] = texts["merge_output"] = head                   # SortVcf: no variant found
-        elif pileup_only:
-            texts["pileup"] = vcf_text(head, postprocess_pileup(p_body, qual, print_ref_calls), True)
-            if not has_records(texts["pileup"]):
-                texts["merge_output"] = texts["pileup"]
-        else:
-            texts["pileup"] = vcf_text(head, p_body, True)
-            if beds:
-                f_body = sort_rows((r for c in f_beds for r in c[3]), names)
-                texts["full_alignment"] = vcf_text(head, f_body, bool(f_body))
-            if not beds or not has_records(texts["full_alignment"]):
-                texts["merge_output"] = texts["pileup"]                      # ensure_merge_output
-            else:
-                merged = sort_rows("".join(_merge_contig(p_chunks, f_beds, ctg, qual, print_ref_calls) for ctg in names)
-                                   .splitlines(keepends=True), names)
-                texts["merge_output"] = vcf_text(head, merged, bool(merged))
-                if genotyping and merged:
-                    texts["merge_output"] = head + "\n" + cascade.add_back_missing(merged, tgt)
-        clock.mark("merge and format")
-        out = finish()
-        clock.mark("write")
-        out["stages"] = clock.report()
+        texts = file_texts(head, names, [c[1:] for c in sorted((c for part in parts for c in part[0]), key=lambda c: c[0])],
+                           [c[1:] for c in sorted((c for part in parts for c in part[1]), key=lambda c: c[0])],
+                           qual, print_ref_calls, pileup_only, tgt if genotyping else None)
+        st.mark("merge and format")
+        out.update(qual_cutoffs=cuts, beds=len(beds))
+        _write(out_dir, texts, out)
+        st.mark("write")
+        out["stages"] = st.summed()
         return out
     finally:
         if own:
             ws.close()
+
+
+def _read_span(decoder, bam_fn, ref_fn, index, lengths, ctg, start, end, fa_fields):
+    """The records of the 0-based [start, end) of contig ``ctg``, decoded with the FASTA window the counter and the builder
+    read around it (``FETCH_EXPAND`` bases either side, clipped to the contig): (records, the window's start)."""
+    r0 = max(0, start - FETCH_EXPAND)
+    ref = bam_io.fetch_fasta(ref_fn, ctg, r0, min(lengths[ctg], end + FETCH_EXPAND + 1))
+    return decoder.decode(bam_fn, ctg, start, end, fa_fields=fa_fields, index=index, ref_seq=ref), r0
+
+
+def _pileup_chunks(counter, st, read, lengths, chunks, mine, tgt, model_p, cfg_p, k, count):
+    """The pileup calls of the CHUNK_LIST rows ``mine`` (indices into ``chunks``): per row (index, contig, positions,
+    probabilities, flags, row texts) of its VCF rows (``cascade.row_summary``), none for a row the reference skips.
+    ``count``: ``PileupCounter.count``'s thresholds and read filters."""
+    out = []
+    for g in mine:
+        ctg, cid, n = chunks[g]
+        region = pileup_chunk_region(ctg, lengths[ctg], cid, n, tgt)
+        if region is None:
+            out.append((g, ctg, np.zeros(0, np.int64), np.zeros(0, np.float32), np.zeros(0, np.uint8), []))
+            continue
+        (start, end), ct = region
+        rec, r0 = read(ctg, start, end, False)
+        st.mark("decode")
+        res = counter.count(rec, start, end, None, r0, alt_info=True, targets=ct, **count).call(model_p, cfg_p, ctg, k=k)
+        st.mark("pileup")
+        pos, prob, flags, idx = cascade.row_summary(res)
+        out.append((g, ctg, pos, prob, flags, [decode.call_row(res, s, cfg_p) for s in idx]))
+        del rec, res
+        st.mark("pileup format")
+    return out
+
+
+def _bed_files(builder, st, read, beds, mine, model_f, cfg_f, k, fa):
+    """The full-alignment calls of the bed files ``mine`` (indices into ``beds``), each over its ``bed_span``: per bed file
+    (index, contig, 1-based positions, row texts) of its VCF rows.  ``fa``: ``FullAlignmentBuilder.build``'s arguments."""
+    out = []
+    for b in mine:
+        ctg, cand = beds[b]
+        rec, r0 = read(ctg, *bed_span(cand), True)
+        st.mark("fa decode")
+        res = builder.build(rec, cand, None, r0, **fa).call(model_f, cfg_f, ctg, k=k)
+        st.mark("fa build and call")
+        pos, rows = cascade.row_texts(res, cfg_f)
+        out.append((b, ctg, pos, rows))
+        del rec, res
+        st.mark("fa format")
+    return out
+
+
+def file_texts(head, contigs, pileup_chunks, fa_beds, qual=2, print_ref=False, pileup_only=False, known=None):
+    """The files' texts, {name: text}, from the rows of the whole run: SortVcf, MergeVcf per contig and, with ``known`` (the
+    known-sites ``Targets``), AddBackMissingVariantsInGenotyping.  ``head``: ``header``'s text; ``contigs``: the contig names
+    in CONTIGS order; ``pileup_chunks`` / ``fa_beds``: per pileup chunk (the rows pileup.vcf keeps) / per bed file, in order,
+    (contig, 1-based positions, row texts).  The reference's early exits: no contig - a header-only ``merge_output`` alone; no
+    pileup row - header-only ``pileup`` and ``merge_output``; ``pileup_only`` - ``pileup`` alone, and ``merge_output`` a copy
+    of it when it holds no row; no bed file or no full-alignment row - ``merge_output`` a copy of ``pileup``."""
+    if not contigs:
+        return {"merge_output": head}
+    p_body = sort_rows((r for c in pileup_chunks for r in c[2]), contigs)
+    if not p_body:
+        return {"pileup": head, "merge_output": head}                  # SortVcf: no variant found
+    if pileup_only:
+        pileup = vcf_text(head, postprocess_pileup(p_body, qual, print_ref), True)
+        return {"pileup": pileup} if has_records(pileup) else {"pileup": pileup, "merge_output": pileup}
+    texts = {"pileup": vcf_text(head, p_body, True)}
+    if fa_beds:
+        texts["full_alignment"] = vcf_text(head, sort_rows((r for c in fa_beds for r in c[2]), contigs))
+    if not fa_beds or not has_records(texts["full_alignment"]):
+        texts["merge_output"] = texts["pileup"]                         # ensure_merge_output
+        return texts
+    merged = sort_rows("".join(_merge_contig(pileup_chunks, fa_beds, ctg, qual, print_ref) for ctg in contigs)
+                       .splitlines(keepends=True), contigs)
+    texts["merge_output"] = vcf_text(head, merged)
+    if known is not None and merged:
+        texts["merge_output"] = head + "\n" + cascade.add_back_missing(merged, known)
+    return texts
 
 
 def _merge_contig(p_chunks, f_beds, ctg, qual, print_ref):
@@ -535,12 +483,22 @@ def _merge_contig(p_chunks, f_beds, ctg, qual, print_ref):
     full-alignment rows."""
     p = {}
     for c in p_chunks:
-        if c[1] == ctg:
-            p.update(zip(np.asarray(c[2]).tolist(), c[3]))
+        if c[0] == ctg:
+            p.update(zip(np.asarray(c[1]).tolist(), c[2]))
     p_pos = sorted(p)
     f_pos, f_rows = [], []
     for c in f_beds:
-        if c[1] == ctg:
-            f_pos.extend(np.asarray(c[2]).tolist())
-            f_rows.extend(c[3])
+        if c[0] == ctg:
+            f_pos.extend(np.asarray(c[1]).tolist())
+            f_rows.extend(c[2])
     return cascade.merge_rows(p_pos, [p[x] for x in p_pos], f_pos, f_rows, qual=qual, print_ref=print_ref)
+
+
+def _write(out_dir, texts, out):
+    """Writes each of ``texts`` as ``<name>.vcf.gz`` with its ``.tbi`` into ``out_dir``, and adds ``files``, ``texts`` and
+    ``rows`` (the row count per file) to the result ``out``."""
+    out_dir = str(out_dir)
+    os.makedirs(out_dir, exist_ok=True)
+    out.update(files={n: write_vcf_gz(os.path.join(out_dir, n + ".vcf.gz"), t) for n, t in texts.items()}, texts=texts,
+               rows={n: _records(t) for n, t in texts.items()})
+    return out

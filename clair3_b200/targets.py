@@ -117,6 +117,18 @@ def read_vcf(source):
                    {c: np.array(sorted(v), np.int64) for c, v in sites.items()}, rows)
 
 
+def resolve(bed=None, known_sites=None):
+    """A run's targets from ``bed`` / ``known_sites``: a path (gzip or plain) or a file's contents, read by ``read_bed`` /
+    ``read_vcf``; a ``Targets`` or a ``ContigTargets`` is returned as it is.  None for neither.  Giving both is a ValueError,
+    as CheckEnvs refuses ``--bed_fn`` with ``--vcf_fn``."""
+    if bed is not None and known_sites is not None:
+        raise ValueError("targets: give either bed or known_sites, not both (the reference refuses --bed_fn with --vcf_fn)")
+    src, read = (bed, read_bed) if bed is not None else (known_sites, read_vcf)
+    if src is None or isinstance(src, (Targets, ContigTargets)):
+        return src
+    return read(src)
+
+
 class ContigTargets:
     """One contig's targets as the counter's test reads them (``c3b_plp_targets``): the intervals sorted by start (a zero-length
     row stored as [s, s + 1), as the reference's interval tree stores it), the running maximum of their ends, and in genotyping

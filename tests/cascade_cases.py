@@ -150,4 +150,4 @@ def _rows_of(res):
 
 def vcf_text(res, cfg):
     """The VCF a call result prints: header and its rows (printed, cand_ok)."""
-    return HEADER + "".join(cascade._vcf(res, cfg)[1])
+    return HEADER + "".join(cascade.row_texts(res, cfg)[1])

@@ -69,7 +69,7 @@ for name in cases.NAMES:
         fa = cases.fa_results(pileup, np.array(positions, np.int64), chunks, seed=len(name))
         fvcf = os.path.join(d, "full_alignment.vcf")
         with open(fvcf, "w") as f:
-            f.write(cases.HEADER + "".join("".join(cascade._vcf(r, cases.CFG_F)[1]) for r in fa))
+            f.write(cases.HEADER + "".join("".join(cascade.row_texts(r, cases.CFG_F)[1]) for r in fa))
         merged = []
         for print_ref in ("False", "True"):
             mo = os.path.join(d, "merge_%s.vcf" % print_ref)

@@ -182,7 +182,7 @@ with tempfile.TemporaryDirectory() as d:
 
     # SelectQual + SelectCandidates over one contig's rows from three overlapping chunks (tests/cascade_cases.py "hifi")
     platform, pres, _ = cc.case("hifi")
-    rows = cascade._vcf(pres, cc.CFG_P)[1]
+    rows = cascade.row_texts(pres, cc.CFG_P)[1]
     rows = [r.replace(cc.CTG + "\t", "chr1\t", 1) for r in rows]
     n = len(rows)
     cuts = [(0, n // 3 + 20), (n // 3, 2 * n // 3 + 20), (2 * n // 3, n)]       # overlapping: 20 rows appear twice

@@ -1,8 +1,8 @@
 """The genome route's host layer (clair3_b200/genome.py and the file I/O of bam_io.py) on the CPU: CheckEnvs (``plan``), the
 VCF header, SortVcf (``sort_rows`` / ``vcf_text`` / ``postprocess_pileup``) and SelectQual + SelectCandidates over
 overlapping chunks (``exchange``) against tests/golden/genome_cases.npz, minted from the reference's own Python
-(tests/golden/make_genome_golden.py); the ``.fai`` fetch, ``idxstats``, BGZF and tabix against what was written; and the
-two-rank exchange (gloo) against the single-process one."""
+(tests/golden/make_genome_golden.py); the files' early exits (``file_texts``) on synthetic rows; the ``.fai`` fetch,
+``idxstats``, BGZF and tabix against what was written; and the two-rank exchange (gloo) against the single-process one."""
 import gzip
 import json
 import os
@@ -103,9 +103,9 @@ def test_select_over_overlapping_chunks():
     case = G["select"]
     platform, pres, _ = cc.case("hifi")
     pres = dict(pres, chromosome=["chr1"] * len(pres["position"]))
-    chunk_rows, idx = [], cascade._rows(pres)              # the fixture's chunks cut the VCF rows
+    chunk_rows, idx = [], cascade.row_indices(pres)              # the fixture's chunks cut the VCF rows
     for a, b in case["chunks"]:
-        pos, prob, flags, _ = genome.row_summary(cascade.take_calls(pres, idx[a:b]))
+        pos, prob, flags, _ = cascade.row_summary(cascade.take_calls(pres, idx[a:b]))
         chunk_rows.append(("chr1", pos, prob, flags))
     keep, cuts, beds = genome.exchange(chunk_rows, [("chr1", 10 ** 6)], platform, split_bed_size=case["split_bed_size"])
     assert sum(int(k.sum()) for k in keep) == len(set(np.concatenate([r[1] for r in chunk_rows]).tolist()))
@@ -115,6 +115,52 @@ def test_select_over_overlapping_chunks():
     assert cuts == cascade.qual_cutoffs([pres], platform)
     want, chunks = cascade.select(pres, *cuts, split_bed_size=case["split_bed_size"])
     assert [p.tolist() for _, p in beds] == [want[a:b].tolist() for a, b in chunks]
+
+
+# ---------------------------------------------------------------------------------------------- the files' early exits
+HEAD = "##fileformat=VCFv4.2\n#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO\tFORMAT\tSAMPLE"
+CONTIGS = ["chr1", "chr2"]
+
+
+def _row(ctg, pos, alt="C"):
+    filt, gt = ("RefCall", "0/0") if alt == "." else ("PASS", "0/1")
+    return "%s\t%d\t.\tA\t%s\t12.00\t%s\tP\tGT:GQ:DP:AF\t%s:12:30:0.5000\n" % (ctg, pos, alt, filt, gt)
+
+
+def _chunk(ctg, positions, alt="C"):
+    """One pileup chunk's or bed file's rows as ``file_texts`` takes them: (contig, 1-based positions, row texts)."""
+    return ctg, np.array(positions, np.int64), [_row(ctg, p, alt) for p in positions]
+
+
+def test_file_texts_without_contig():
+    assert genome.file_texts(HEAD, [], [], []) == {"merge_output": HEAD}
+
+
+def test_file_texts_without_pileup_row():
+    assert genome.file_texts(HEAD, CONTIGS, [_chunk("chr1", []), _chunk("chr2", [])], []) == {"pileup": HEAD, "merge_output": HEAD}
+
+
+def test_file_texts_pileup_only():
+    chunks = [_chunk("chr2", [30, 10]), _chunk("chr1", [50])]
+    got = genome.file_texts(HEAD, CONTIGS, chunks, [], pileup_only=True)
+    assert got == {"pileup": HEAD + "\n" + _row("chr1", 50) + _row("chr2", 10) + _row("chr2", 30)}
+    # only reference rows, not printed: the pileup file holds no row, and merge_output is a copy of it
+    got = genome.file_texts(HEAD, CONTIGS, [_chunk("chr1", [5, 7], alt=".")], [], pileup_only=True)
+    assert sorted(got) == ["merge_output", "pileup"] and not genome.has_records(got["pileup"])
+    assert got["merge_output"] == got["pileup"] == HEAD + "\n"
+
+
+def test_file_texts_without_bed_file():
+    got = genome.file_texts(HEAD, CONTIGS, [_chunk("chr2", [30]), _chunk("chr1", [50, 20], alt=".")], [])
+    assert sorted(got) == ["merge_output", "pileup"]
+    assert got["merge_output"] == got["pileup"] == HEAD + "\n" + _row("chr1", 20, ".") + _row("chr1", 50, ".") + _row("chr2", 30)
+
+
+def test_file_texts_without_full_alignment_row():
+    pileup = [_chunk("chr1", [50]), _chunk("chr2", [30])]
+    got = genome.file_texts(HEAD, CONTIGS, pileup, [_chunk("chr1", []), _chunk("chr2", [])])
+    assert sorted(got) == ["full_alignment", "merge_output", "pileup"] and got["full_alignment"] == HEAD
+    assert got["merge_output"] == got["pileup"] == HEAD + "\n" + _row("chr1", 50) + _row("chr2", 30)
 
 
 def test_fai_fetch_matches_read_fasta(tmp_path):
@@ -217,7 +263,7 @@ def _synthetic_chunks():
         n = len(pres["position"])
         contigs.append((ctg, int(pres["position"].max()) + 10))
         for a, b in ((0, n // 3 + 15), (n // 3, 2 * n // 3 + 15), (2 * n // 3, n)):
-            pos, prob, flags, _ = genome.row_summary(cascade.take_calls(pres, np.arange(a, b)))
+            pos, prob, flags, _ = cascade.row_summary(cascade.take_calls(pres, np.arange(a, b)))
             out.append((ctg, pos, prob, flags))
     return out, contigs
 

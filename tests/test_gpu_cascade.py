@@ -72,8 +72,8 @@ def test_device_selection_matches_host(ws, models, region, cuts):
     sel, count = cascade.select_device(res, var_q, ref_q)
     n = int(count.item())
     assert np.array_equal(sel[:n].cpu().numpy(), want)
-    rows = cascade._rows(res)
-    is_ref = cascade._is_reference(res, rows)
+    rows = cascade.row_indices(res)
+    is_ref = cascade.is_reference(res, rows)
     # the reference / variant split by ALT text: (0, 1000) keeps exactly the reference rows, (1000, 0) exactly the others
     expect = {"none": 0, "all": len(rows), "references": int(is_ref.sum()), "variants": int((~is_ref).sum())}
     if cuts in expect:

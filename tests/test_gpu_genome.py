@@ -168,13 +168,13 @@ def host_route(ws, m_p, m_f, bam, fa, out_cmd=None, tgt=None, platform="ont", qu
         res = ws.counter.count(rec, s, e, bam_io.read_fasta(fa, ctg, r0, r1), r0, min_depth=min_coverage, min_snp_af=snp,
                                min_indel_af=indel, min_mq=min_mq, call_snp_only=call_snp_only, call_ht=call_ht, alt_info=True,
                                max_indel_length=max_indel).call(m_p, cfg_p, ctg)
-        res = cascade.take_calls(res, cascade._rows(res))
+        res = cascade.take_calls(res, cascade.row_indices(res))
         if ct is not None:
             res = cascade.take_calls(res, np.nonzero(ct.keep(res["position"]))[0])
         per.append((ctg, res))
     first, repeated, differing = {}, 0, 0
     for ctg, res in per:
-        for p, row in zip(*cascade._vcf(res, cfg_p)):
+        for p, row in zip(*cascade.row_texts(res, cfg_p)):
             if (ctg, int(p)) in first:
                 repeated += 1
                 differing += first[(ctg, int(p))] != row
@@ -188,7 +188,7 @@ def host_route(ws, m_p, m_f, bam, fa, out_cmd=None, tgt=None, platform="ont", qu
         keep = [i for i, p in enumerate(res["position"].tolist()) if (ctg, p) not in seen]
         seen.update((ctg, p) for p in res["position"].tolist())
         per[j] = (ctg, cascade.take_calls(res, keep))
-    rows = [r for _, res in per for r in cascade._vcf(res, cfg_p)[1]]
+    rows = [r for _, res in per for r in cascade.row_texts(res, cfg_p)[1]]
     texts = {}
     if not rows:
         return {"pileup": head, "merge_output": head}
@@ -214,7 +214,7 @@ def host_route(ws, m_p, m_f, bam, fa, out_cmd=None, tgt=None, platform="ont", qu
             fres.append(ws.builder.build(rec, cand, bam_io.read_fasta(fa, ctg, r0, r1), r0, matrix_depth=MATRIX_DEPTH[platform],
                                          need_haplotagging=False, min_mq=min_mq, max_indel_length=max_indel, dwell=dwell,
                                          rand_seed=1, rand_skip=0).call(m_f, cfg_f, ctg))
-            f_rows += cascade._vcf(fres[-1], cfg_f)[1]
+            f_rows += cascade.row_texts(fres[-1], cfg_f)[1]
         merged.append(cascade.merge(res, fres, cfg_p, cfg_f, qual=qual, print_ref=print_ref))
     if not any_bed:
         texts["merge_output"] = texts["pileup"]
