@@ -635,7 +635,7 @@ static PileupChunk carve_pileup(const c3b_model *m, Carver &cv, int64_t n) {
         c.l2 = cv.take<float>((size_t)n * C3B_T * 320 * 4);
         c.z4 = cv.take<float>((size_t)bp * 128 * 4);
     } else {
-        c.tc.xs = cv.take<op_t>((size_t)C3B_T * bp * C3B_X1_COLS * 2);
+        c.tc.x_tap = m->taps ? cv.take<op_t>((size_t)C3B_T * bp * C3B_X1_COLS * 2) : nullptr;
         c.tc.h1 = cv.take<op_t>((size_t)C3B_T * bp * 256 * 2);
         c.tc.pg = cv.take<__half>((size_t)C3B_T * bp * 1280 * 2);
         c.tc.h2 = cv.take<op_t>((size_t)bp * C3B_T * 320 * 2);
@@ -749,17 +749,6 @@ extern "C" int c3b_get_profile_ctas(c3b_model *m, const char *kernel, double *ct
 }
 
 // ------------------------------------------------------------------------------------------------ forward passes
-// Where a pileup chunk's sites come from: a dense [n,33,C] tensor, or 33-row windows of a per-column count matrix
-// ([n_cols][C], libclair3's plp_data.matrix) starting at rows starts[b] (rows outside the matrix, or outside [bounds[b][0],
-// bounds[b][1]) when bounds are given, read as zero)
-struct PileupSrc {
-    const void *x;          // dense: first site of the chunk; windows: the column matrix
-    int dtype;
-    const int64_t *starts;  // windows: device pointer to this chunk's first start row; nullptr = dense
-    const int64_t *bounds;  // windows: device pointer to this chunk's first [lo, hi) row pair; nullptr = [0, n_cols)
-    int64_t n_cols;
-};
-
 // latency: the call is a synchronous host-buffer forward (the reference's _torch_predict shape: one batch in flight, the caller
 // waits) -> kernel variants that finish ONE batch soonest (many short CTAs); otherwise the variants with the smallest SM-time,
 // for callers that keep several batches in flight (forward_async / predict_stream / device-resident calls on several streams).
@@ -796,9 +785,7 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
     int tile1 = m->lstm_tile;
     if (tile1 == 0) tile1 = !latency ? 64 : (bp / 64 >= m->sm_count) ? 64 : (bp / 32 >= m->sm_count) ? 32 : 16;
     const int tile2 = tile1 > 32 ? 32 : tile1;
-    { PROF("ingest"); if (c3b_launch_ingest_pileup_tc(x, x_dtype, m->channels, src.starts, src.bounds, src.n_cols, b.xs, n, (int)bp, s)) return 1; }
-    m->launches += 1;
-    { PROF("lstm1"); if (c3b_launch_lstm1_tc(m, b, n, tile1, s)) return 1; }
+    { PROF("lstm1"); if (c3b_launch_lstm1_tc(m, b, src, n, tile1, s)) return 1; }
     { PROF("proj2"); if (c3b_launch_proj2(m, b.h1, m->proj2, b.pg, (int)bp, s)) return 1; }
     { PROF("lstm2"); if (c3b_launch_lstm2_tc(m, b, n, tile2, s)) return 1; }
     int nsplit = 1;
@@ -808,7 +795,7 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
         taps["lstm2"] = {b.h2, 1, 2, (int64_t)C3B_T * 320, (int)bp, {}};
         taps["l4_pre"] = {b.z4, 0, 5, 128, (int)bp, {}};
         taps["l4_pre"].nsplit = nsplit;
-        taps["lstm1_x"] = {b.xs, 1, 7, C3B_X1_COLS, (int)bp, {}};
+        taps["lstm1_x"] = {b.x_tap, 1, 7, C3B_X1_COLS, (int)bp, {}};
         taps["lstm2_pregates"] = {b.pg, 1, 7, 1280, (int)bp, {}};
     }
     return 0;

@@ -585,23 +585,30 @@ int c3b_launch_spp_f32(const float *x, float *out, int64_t batch, int h, int w, 
 
 // ---- tensor-core path ----
 struct TcPileupBuffers {
-    op_t *xs;     // [33][B][48] fp16, time-major: hi(x) | 1 | lo(x) columns
+    op_t *x_tap;  // [33][B][48] fp16, time-major: LSTM1's hi(x) | 1 | lo(x) operand columns; only with the "taps" option, else nullptr
     op_t *h1;     // tile-major k-group-planar, 32 k-groups: row = t*Bp + b, k = dir*128 + j  (projection GEMM operand)
     __half *pg;            // [33*B][1280] fp16 pre-gates of LSTM2 (bias included), column dir*640 + C in gate-quad order (c3b_lstm2_pg_row)
     op_t *h2;     // tile-major k-group-planar, 1320 k-groups: row = b, k = t*320 + dir*160 + j (flatten order of clair3/model.py:135)
     float *z4;             // [16][B][128] fp32 split-K partial sums of the L4 pre-activation (no bias)
     int bp;                // padded batch: multiple of 128
 };
-// starts == nullptr: x is the dense [batch][33][channels] tensor; otherwise x is the per-column matrix [n_cols][channels] and
-// site b is its rows [starts[b], starts[b] + 33) (rows outside the matrix, and with bounds != nullptr rows outside
-// [bounds[2b], bounds[2b+1]), read as zero)
-int c3b_launch_ingest_pileup_tc(const void *x, int dtype, int channels, const int64_t *starts, const int64_t *bounds, int64_t n_cols,
-                                op_t *xs, int64_t batch, int bp, cudaStream_t s);
+// Where a pileup chunk's sites come from: a dense [n,33,C] tensor, or 33-row windows of a per-column count matrix
+// ([n_cols][C], libclair3's plp_data.matrix) starting at rows starts[b] (rows outside the matrix, or outside [bounds[b][0],
+// bounds[b][1]) when bounds are given, read as zero)
+struct PileupSrc {
+    const void *x;          // dense: first site of the chunk; windows: the column matrix
+    int dtype;
+    const int64_t *starts;  // windows: device pointer to this chunk's first start row; nullptr = dense
+    const int64_t *bounds;  // windows: device pointer to this chunk's first [lo, hi) row pair; nullptr = [0, n_cols)
+    int64_t n_cols;
+};
 int c3b_launch_gather_windows_f32(const void *cols, int dtype, int channels, const int64_t *starts, const int64_t *bounds,
                                   int64_t n_cols, float *out, int64_t batch, cudaStream_t s);
 int c3b_launch_proj2(const c3b_model *m, const op_t *h1, const IgemmW &w, __half *pg, int bp, cudaStream_t s);
 int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, float *out, float *z4, int *nsplit_out, cudaStream_t s);
-int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s);
+// LSTM1 reads the chunk's `batch` sites straight from src and builds its x operand columns itself
+int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, const PileupSrc &src, int64_t batch, int tile,
+                        cudaStream_t s);
 int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s);
 
 struct PconvArgs {

@@ -17,7 +17,10 @@
 // (the reference's GPU branch does not rescale depth, clair3/CallVariantsFromCffi.py:299-353), fp16 is exact only to 2048, so
 // every count is split as x = hi + lo with hi = fp16(x) and lo = fp16(x - hi) - exact for |x| <= 67 552; beyond that lo is
 // rounded (error <= 16, <= 2^-12 relative) up to 131 008, and saturates past it - and W_ih multiplies both parts (fp32 accumulate: the same result as an exact-input product).  Column 18 is a constant 1 that
-// carries b_ih + b_hh, so the x projection and the bias are fused into the same MMAs.
+// carries b_ih + b_hh, so the x projection and the bias are fused into the same MMAs.  The kernel builds these columns itself
+// from the caller's raw counts (int8 / int32 / int64 / float32, one instance per dtype): from the dense [batch][33][C] tensor or
+// from the 33-row windows of forward_windows' column matrix, one step ahead, in registers, straight into the operand buffer - the
+// x operand never goes through HBM (with the "taps" option a copy goes to a [33][Bp][48] tap buffer).
 // LSTM2 (H=160, input 256): the input projection W_ih*h1 (+bias) is a separate big GEMM (proj_tc.cu) that leaves fp16
 // pre-gates pg[t*bp + site][dir*640 + C] in gate-quad order (c3b_lstm2_pg_row: columns 128p + 4u .. +3 = gates i, f, g, o of
 // unit 32p + u), so a thread loads its unit's four pre-gates of one site as one 8-byte word; a warp load covers 4 sites x 64
@@ -30,6 +33,8 @@
 // no faster for LSTM2: it serialises the two warpgroups' MMA chains, which otherwise overlap.)  LSTM2's pre-gates of block pair
 // p + 1 (after the last pair: the next step's first) are loaded right after the MMAs of pair p are issued, so their DRAM
 // latency hides behind a whole MMA / cell-math phase instead of stalling the start of every pair.
+#include <type_traits>
+
 #include "c3b_internal.h"
 #include "ptx.cuh"
 
@@ -37,7 +42,10 @@ namespace {
 
 struct LstmDev {
     const op_t *w_img;             // [dir][2H/64 blocks][K/8][64][8]
-    const op_t *xs;                // LSTM1 input  [33][Bp][48]: hi | 1 | lo columns
+    PileupSrc x;                   // LSTM1 input: the caller's dense tensor or column matrix (PileupSrc), read by the kernel itself
+    int64_t batch;                 // LSTM1: real sites; sites b >= batch read as 0
+    int channels;                  // LSTM1: counts per site-step
+    op_t *x_tap;                   // LSTM1, optional: [33][Bp][48] copy of the x operand columns it built (option "taps")
     const __half *pg;              // LSTM2 pre-gates [33*Bp][1280]
     op_t *hout;                    // tile-major k-group-planar: LSTM1 h1 (rows t*Bp+b, 32 k-groups); LSTM2 h2 (rows b, 1320 k-groups)
     int bp;                        // padded batch
@@ -110,7 +118,110 @@ __device__ __forceinline__ void wgmma_nb(float (&d)[NB / 2], uint64_t a, uint64_
     else ptx::wgmma_m64n64k16(d, a, b, acc);
 }
 
-template <int NB, bool LAYER2, bool MUFU16, int WG>
+// ---- LSTM1's x operand columns from the caller's counts (see the header): column k is hi(x_k) for k < C, 1 for k == C,
+// lo(x_{k-C-1}) for C < k <= 2C and 0 beyond, so k-group kg holds columns 8kg .. 8kg+7.
+
+// Row t of site b, or nullptr where it reads as 0: padded sites, and window rows outside the matrix or outside the site's bounds
+// (preprocess/CreateTensorPileupFromCffi.py:356-396 zero-pads a window where it overhangs its contiguous run)
+template <typename T>
+__device__ __forceinline__ const T *x_row(const LstmDev &p, int b, int t) {
+    if (b >= p.batch) return nullptr;
+    const T *x = static_cast<const T *>(p.x.x);
+    if (!p.x.starts) return x + ((int64_t)b * C3B_T + t) * p.channels;
+    const int64_t row = p.x.starts[b] + t;
+    if (row < 0 || row >= p.x.n_cols || (p.x.bounds && (row < p.x.bounds[2 * b] || row >= p.x.bounds[2 * b + 1]))) return nullptr;
+    return x + row * p.channels;
+}
+
+template <typename T>
+struct alignas(2 * sizeof(T)) XPair { T v[2]; };
+
+// The 18 counts of a row (the reference's pileup shape, shared/param_p.py:32-36): nine 2-count loads when the input's base is
+// aligned for them (every row then is: rows are 18 counts apart), else one load per count
+template <typename T>
+__device__ __forceinline__ void load_row18(const T *row, bool pairs, T (&r)[18]) {
+    if (!row) {
+#pragma unroll
+        for (int c = 0; c < 18; ++c) r[c] = T(0);
+    } else if (pairs) {
+#pragma unroll
+        for (int j = 0; j < 9; ++j) {
+            const XPair<T> q = reinterpret_cast<const XPair<T> *>(row)[j];
+            r[2 * j] = q.v[0];
+            r[2 * j + 1] = q.v[1];
+        }
+    } else {
+#pragma unroll
+        for (int c = 0; c < 18; ++c) r[c] = row[c];
+    }
+}
+
+// The 18 counts as floats, (float)v exactly.  Small integers (|v| < 2^22: every realistic count) go through the float bit
+// pattern of 1.5 * 2^23 + v on the ALU: int8 and int64 conversions otherwise issue to the quarter-rate unit that the cell math's
+// tanh already saturates.
+template <typename T>
+__device__ __forceinline__ void counts_to_float18(const T (&r)[18], float (&xf)[18]) {
+    if constexpr (std::is_same<T, float>::value || std::is_same<T, int32_t>::value) {
+#pragma unroll
+        for (int c = 0; c < 18; ++c) xf[c] = (float)r[c];
+    } else {
+        bool small = true;                          // int8: always
+#pragma unroll
+        for (int c = 0; c < 18 && sizeof(T) > 1; ++c) small &= (uint64_t)((int64_t)r[c] + (1 << 22)) < (1u << 23);
+        if (small) {
+#pragma unroll
+            for (int c = 0; c < 18; ++c) xf[c] = __int_as_float(0x4B400000 + (int)r[c]) - 12582912.f;
+        } else {
+#pragma unroll
+            for (int c = 0; c < 18; ++c) xf[c] = (float)r[c];
+        }
+    }
+}
+
+// hi(x) of channel c as a float: fp16(x) saturating, from one packed conversion of c's channel pair
+__device__ __forceinline__ float x_hi18(const float (&xf)[18], int c) {
+    const uint32_t h = f2op2_sat(xf[c & ~1], xf[c | 1]);
+    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&h));
+    return (c & 1) ? f.y : f.x;
+}
+
+// column k before its fp16 rounding: x_k, 1, x - hi(x), 0
+__device__ __forceinline__ float x_col18(const float (&xf)[18], int k) {
+    if (k < 18) return xf[k];
+    if (k == 18) return 1.f;
+    if (k < 37) return xf[k - 19] - x_hi18(xf, k - 19);
+    return 0.f;
+}
+
+// k-group kg of a row with 18 counts, two columns per (saturating) conversion; kg must be a compile-time constant, so every
+// index is one
+__device__ __forceinline__ uint4 x_kgroup18(const float (&xf)[18], int kg) {
+    uint32_t w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) w[j] = f2op2_sat(x_col18(xf, 8 * kg + 2 * j), x_col18(xf, 8 * kg + 2 * j + 1));
+    return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// k-group kg of a row with any other channel count c (row == nullptr: a zero row): one load per column
+template <typename T>
+__device__ __forceinline__ uint4 x_kgroup(const T *row, int c, int kg) {
+    __align__(16) op_t v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int k = 8 * kg + j;
+        float f = (k == c) ? 1.f : 0.f;
+        if (row && k != c && k <= 2 * c) {
+            const float x = (float)row[k < c ? k : k - c - 1];
+            const op_t hi = f2op_sat(x);
+            f = k < c ? op2f(hi) : x - op2f(hi);
+        }
+        v[j] = f2op_sat(f);
+    }
+    return *reinterpret_cast<const uint4 *>(v);
+}
+
+// T: LSTM1's input dtype (LSTM2 reads no input and is instantiated with float)
+template <int NB, bool LAYER2, bool MUFU16, int WG, typename T>
 __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
     constexpr int H = LAYER2 ? 160 : 128;
     constexpr int KX = LAYER2 ? 0 : C3B_X1_COLS;
@@ -121,7 +232,9 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
     static_assert(K % 16 == 0, "whole k-steps");
     constexpr uint32_t LBO_B = (NB + 1) * 16;       // padded: fewer bank conflicts on the h stores
     constexpr uint32_t B_BYTES = (K / 8) * LBO_B;
+    // LSTM1: a thread builds the x k-groups (wt + 128 i) / NB, i < XN, of site wt % NB - all of them from one row
     constexpr int XN = LAYER2 ? 1 : (NB * (KX / 8) + 127) / 128;
+    constexpr int XR = LAYER2 ? 1 : 18;
 
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t w_bar;
@@ -154,13 +267,43 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
     // h_{-1} = 0 and (LSTM1) x of the first step
     for (uint32_t i = wt * 16; i < B_BYTES; i += 128 * 16) *reinterpret_cast<uint4 *>(b_smem + i) = make_uint4(0, 0, 0, 0);
     ptx::named_bar_sync(bar_id, 128);
+    const int xn = wt % NB;
+    const bool c18 = p.channels == 18;
+    const bool pairs = (reinterpret_cast<uintptr_t>(p.x.x) & (2 * sizeof(T) - 1)) == 0;
+    // x k-group of item i (a compile-time constant: it bounds the k-groups the item can hold), from the row's counts xf (as
+    // floats) when channels == 18, else from the row itself
+    auto x_item = [&](int i, const float(&xf)[XR], const T *row) {
+        const int kg = (wt + 128 * i) / NB;
+        uint4 v = make_uint4(0, 0, 0, 0);
+        if constexpr (!LAYER2) {
+            if (c18) {
+#pragma unroll
+                for (int g = 0; g < KX / 8; ++g)
+                    if (g >= 128 * i / NB && g <= (128 * i + 127) / NB && kg == g) v = x_kgroup18(xf, g);
+            } else {
+                v = x_kgroup(row, p.channels, kg);
+            }
+        }
+        return v;
+    };
+    // store item i of x_t into the operand buffer (and the tap)
+    auto x_store = [&](int i, int t, uint4 v) {
+        const int kg = (wt + 128 * i) / NB;
+        *reinterpret_cast<uint4 *>(b_smem + kg * LBO_B + xn * 16) = v;
+        if (p.x_tap) *reinterpret_cast<uint4 *>(p.x_tap + ((size_t)t * p.bp + b0 + xn) * KX + kg * 8) = v;
+    };
     if constexpr (!LAYER2) {
         const int t = dir ? C3B_T - 1 : 0;
-        for (int idx = wt; idx < NB * (KX / 8); idx += 128) {
-            const int n = idx / (KX / 8), kg = idx % (KX / 8);
-            *reinterpret_cast<uint4 *>(b_smem + kg * LBO_B + n * 16) =
-                *reinterpret_cast<const uint4 *>(p.xs + ((size_t)t * p.bp + b0 + n) * KX + kg * 8);
+        const T *row = x_row<T>(p, b0 + xn, t);
+        T r[XR];
+        float xf[XR];
+        if (c18) {
+            load_row18(row, pairs, r);
+            counts_to_float18(r, xf);
         }
+#pragma unroll
+        for (int i = 0; i < XN; ++i)
+            if (wt + 128 * i < NB * (KX / 8)) x_store(i, t, x_item(i, xf, row));
     }
 
     float c[NP][NB / 4];
@@ -199,17 +342,17 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
                     *reinterpret_cast<const uint4 *>(b_smem + (KX / 8 + kgh) * LBO_B + n * 16);
             }
         }
-        // LSTM1: fetch x_{t+1} now, store it once every MMA of this step has read the operand buffer
+        // LSTM1: start loading x_{t+1}'s counts now; they become operand columns while the second block pair's MMAs run (a whole
+        // block pair later, so the loads have arrived; hq holds one pair then), and go into the operand buffer once every MMA of
+        // this step has read it
+        const int tn = dir ? t - 1 : t + 1;
+        const T *xrow = nullptr;
+        T xr[XR];
         uint4 xnext[XN];
         if constexpr (!LAYER2) {
             if (step + 1 < C3B_T) {
-                const int tn = dir ? t - 1 : t + 1;
-#pragma unroll
-                for (int i = 0; i < XN; ++i) {
-                    const int idx = wt + i * 128;
-                    if (idx < NB * (KX / 8))
-                        xnext[i] = *reinterpret_cast<const uint4 *>(p.xs + ((size_t)tn * p.bp + b0 + idx / (KX / 8)) * KX + (idx % (KX / 8)) * 8);
-                }
+                xrow = x_row<T>(p, b0 + xn, tn);
+                if (c18) load_row18(xrow, pairs, xr);
             }
         }
 #pragma unroll
@@ -231,7 +374,15 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
 #pragma unroll
                 for (int i = 0; i < PGN; ++i) pgv[i] = pgn[i];
                 if (pp + 1 < NP) load_pg(t, pp + 1);
-                else if (step + 1 < C3B_T) load_pg(dir ? t - 1 : t + 1, 0);
+                else if (step + 1 < C3B_T) load_pg(tn, 0);
+            } else {
+                if (pp == 1 && step + 1 < C3B_T) {
+                    float xf[XR];
+                    if (c18) counts_to_float18(xr, xf);
+#pragma unroll
+                    for (int i = 0; i < XN; ++i)
+                        if (wt + 128 * i < NB * (KX / 8)) xnext[i] = x_item(i, xf, xrow);
+                }
             }
             ptx::wgmma_wait<0>();
             ptx::fence_operand(acc0);
@@ -278,10 +429,8 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
         if constexpr (!LAYER2) {
             if (step + 1 < C3B_T) {
 #pragma unroll
-                for (int i = 0; i < XN; ++i) {
-                    const int idx = wt + i * 128;
-                    if (idx < NB * (KX / 8)) *reinterpret_cast<uint4 *>(b_smem + (idx % (KX / 8)) * LBO_B + (idx / (KX / 8)) * 16) = xnext[i];
-                }
+                for (int i = 0; i < XN; ++i)
+                    if (wt + 128 * i < NB * (KX / 8)) x_store(i, tn, xnext[i]);
             }
         }
         if (tr) p.trace[step * 4 + 3] = clock64();
@@ -297,74 +446,12 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
     }
 }
 
-template <typename T>
-__device__ __forceinline__ float ingest_to_float(T v) { return (float)v; }
-
-// Dense [batch][33][channels] tensor, or (starts != nullptr) 33-row windows of the per-column count matrix [n_cols][channels]
-// (libclair3's plp_data.matrix; preprocess/CreateTensorPileupFromCffi.py:356-396 slices the same windows on the host, zero
-// rows where a window overhangs its contiguous run: rows outside [bounds[b][0], bounds[b][1]) and outside the matrix read as 0) -> xs[t][bp][48] fp16 with columns [hi(x) | 1 | lo(x) | 0..]: hi = fp16(x)
-// (saturating at +-65504), lo = fp16(x - hi), so hi + lo == x exactly for |x| <= 67 552 (past 65 519 hi stays at 65 504 and
-// lo > 2048 is itself rounded: error <= 16, <= 2^-12 relative, up to 131 008; saturating beyond); column `channels` = constant 1
-// (LSTM1's bias column).
-template <typename T>
-__global__ void ingest_pileup_tc_kernel(const T *__restrict__ x, const int64_t *__restrict__ starts,
-                                        const int64_t *__restrict__ bounds, int64_t n_cols, op_t *__restrict__ xs, int64_t batch,
-                                        int bp, int channels) {
-    // one thread per (t, site): six 16-byte stores
-    const int64_t total = (int64_t)C3B_T * bp;
-    for (int64_t tb = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; tb < total; tb += (int64_t)gridDim.x * blockDim.x) {
-        const int b = (int)(tb % bp);
-        const int t = (int)(tb / bp);
-        bool have = b < batch;
-        const T *src = x;
-        if (have) {
-            if (starts) {
-                const int64_t row = starts[b] + t;
-                have = row >= 0 && row < n_cols && (!bounds || (row >= bounds[2 * b] && row < bounds[2 * b + 1]));
-                src = x + row * channels;
-            } else {
-                src = x + ((int64_t)b * C3B_T + t) * channels;
-            }
-        }
-        __align__(16) op_t v[C3B_X1_COLS];
-        if (channels == 18) {
-            // the reference's pileup shape (shared/param_p.py:32-36): every index is a compile-time constant, one load per count
-            float xv[18];
-#pragma unroll
-            for (int c = 0; c < 18; ++c) xv[c] = have ? ingest_to_float(src[c]) : 0.f;
-#pragma unroll
-            for (int c = 0; c < 18; ++c) {
-                const op_t hi = f2op_sat(xv[c]);
-                v[c] = hi;
-                v[19 + c] = f2op_sat(xv[c] - op2f(hi));
-            }
-            v[18] = f2op(1.f);
-#pragma unroll
-            for (int k = 37; k < C3B_X1_COLS; ++k) v[k] = f2op(0.f);
-        } else {
-#pragma unroll
-            for (int k = 0; k < C3B_X1_COLS; ++k) {          // static indices: v stays in registers
-                float f = (k == channels) ? 1.f : 0.f;
-                if (have && k != channels && k <= 2 * channels) {
-                    const float xvv = ingest_to_float(src[k < channels ? k : k - channels - 1]);
-                    const op_t hi = f2op_sat(xvv);
-                    f = k < channels ? op2f(hi) : xvv - op2f(hi);
-                }
-                v[k] = f2op_sat(f);
-            }
-        }
-        uint4 *dst = reinterpret_cast<uint4 *>(xs + tb * C3B_X1_COLS);
-#pragma unroll
-        for (int k = 0; k < C3B_X1_COLS / 8; ++k) dst[k] = reinterpret_cast<const uint4 *>(v)[k];
-    }
-}
-
-template <int NB, bool LAYER2, bool MUFU16, int WG>
+template <int NB, bool LAYER2, bool MUFU16, int WG, typename T>
 int launch_lstm_impl(const LstmDev &p, cudaStream_t s) {
     constexpr int K = (LAYER2 ? 0 : C3B_X1_COLS) + (LAYER2 ? 160 : 128);
     constexpr int H = LAYER2 ? 160 : 128;
     const size_t smem = (size_t)4 * H * K * 2 + (size_t)WG * (K / 8) * (NB + 1) * 16;   // 4H gate rows of fp16 weights + operands
-    auto kern = lstm_tc_kernel<NB, LAYER2, MUFU16, WG>;
+    auto kern = lstm_tc_kernel<NB, LAYER2, MUFU16, WG, T>;
     C3B_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid(p.bp / (WG * NB), 2);
     c3b_note_grid((long long)grid.x * grid.y);
@@ -374,43 +461,43 @@ int launch_lstm_impl(const LstmDev &p, cudaStream_t s) {
 }
 
 // wg = warpgroups per CTA (each owns one NB-site sub-tile; they share the CTA's copy of the weights)
-template <int NB, bool LAYER2>
+template <int NB, bool LAYER2, typename T = float>
 int launch_lstm(const LstmDev &p, bool mufu16, int wg, cudaStream_t s) {
-    if (mufu16) return wg == 1 ? launch_lstm_impl<NB, LAYER2, true, 1>(p, s) : launch_lstm_impl<NB, LAYER2, true, 2>(p, s);
-    return wg == 1 ? launch_lstm_impl<NB, LAYER2, false, 1>(p, s) : launch_lstm_impl<NB, LAYER2, false, 2>(p, s);
+    if (mufu16) return wg == 1 ? launch_lstm_impl<NB, LAYER2, true, 1, T>(p, s) : launch_lstm_impl<NB, LAYER2, true, 2, T>(p, s);
+    return wg == 1 ? launch_lstm_impl<NB, LAYER2, false, 1, T>(p, s) : launch_lstm_impl<NB, LAYER2, false, 2, T>(p, s);
+}
+
+template <int NB>
+int launch_lstm1(const LstmDev &p, bool mufu16, int wg, cudaStream_t s) {
+    switch (p.x.dtype) {
+        case C3B_DT_I8: return launch_lstm<NB, false, int8_t>(p, mufu16, wg, s);
+        case C3B_DT_I32: return launch_lstm<NB, false, int32_t>(p, mufu16, wg, s);
+        case C3B_DT_I64: return launch_lstm<NB, false, int64_t>(p, mufu16, wg, s);
+        case C3B_DT_F32: return launch_lstm<NB, false, float>(p, mufu16, wg, s);
+    }
+    c3b_set_error("lstm1: unsupported input dtype %d", p.x.dtype);
+    return 1;
 }
 
 }  // namespace
 
-int c3b_launch_ingest_pileup_tc(const void *x, int dtype, int channels, const int64_t *starts, const int64_t *bounds, int64_t n_cols,
-                                op_t *xs, int64_t batch, int bp, cudaStream_t s) {
-    const int64_t total = (int64_t)C3B_T * bp;
-    const int blocks = (int)((total + 127) / 128 < 2048 ? (total + 127) / 128 : 2048);
-    c3b_note_grid(blocks);
-    switch (dtype) {
-        case C3B_DT_I8: ingest_pileup_tc_kernel<int8_t><<<blocks, 128, 0, s>>>((const int8_t *)x, starts, bounds, n_cols, xs, batch, bp, channels); break;
-        case C3B_DT_I32: ingest_pileup_tc_kernel<int32_t><<<blocks, 128, 0, s>>>((const int32_t *)x, starts, bounds, n_cols, xs, batch, bp, channels); break;
-        case C3B_DT_I64: ingest_pileup_tc_kernel<int64_t><<<blocks, 128, 0, s>>>((const int64_t *)x, starts, bounds, n_cols, xs, batch, bp, channels); break;
-        case C3B_DT_F32: ingest_pileup_tc_kernel<float><<<blocks, 128, 0, s>>>((const float *)x, starts, bounds, n_cols, xs, batch, bp, channels); break;
-        default: c3b_set_error("unsupported input dtype %d", dtype); return 1;
-    }
-    C3B_CUDA(cudaGetLastError());
-    return 0;
-}
-
 // `tile` = sites per warpgroup sub-tile.
-int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s) {
+int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, const PileupSrc &src, int64_t batch, int tile,
+                        cudaStream_t s) {
     LstmDev p = {};
     p.w_img = m->lstm_tc[0];
-    p.xs = b.xs;
+    p.x = src;
+    p.batch = batch;
+    p.channels = m->channels;
+    p.x_tap = b.x_tap;
     p.hout = b.h1;
     p.trace = m->lstm_trace;
     p.bp = b.bp;
     const_cast<c3b_model *>(m)->launches++;
     switch (tile) {
-        case 16: return launch_lstm<16, false>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
-        case 32: return launch_lstm<32, false>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
-        case 64: return launch_lstm<64, false>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
+        case 16: return launch_lstm1<16>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
+        case 32: return launch_lstm1<32>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
+        case 64: return launch_lstm1<64>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
     }
     c3b_set_error("lstm1: unsupported tile %d", tile);
     return 1;
