@@ -293,6 +293,9 @@ extern "C" int c3b_set_option(c3b_model *m, const char *name, int value) {
     } else if (!strcmp(name, "lstm_wg")) {
         if (value != 1 && value != 2) { c3b_set_error("lstm_wg must be 1 or 2"); return 1; }
         m->lstm_wg = (int)value;
+    } else if (!strcmp(name, "lstm2_split")) {
+        if (value != 0 && value != 1) { c3b_set_error("lstm2_split must be 0 or 1"); return 1; }
+        m->lstm2_split = value;
     } else if (!strcmp(name, "lstm_mufu16")) {
         m->lstm_mufu16 = value ? 1 : 0;
     } else if (!strcmp(name, "tap_ws")) {
@@ -787,7 +790,7 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
     const int tile2 = tile1 > 32 ? 32 : tile1;
     { PROF("lstm1"); if (c3b_launch_lstm1_tc(m, b, src, n, tile1, s)) return 1; }
     { PROF("proj2"); if (c3b_launch_proj2(m, b.h1, m->proj2, b.pg, (int)bp, s)) return 1; }
-    { PROF("lstm2"); if (c3b_launch_lstm2_tc(m, b, n, tile2, s)) return 1; }
+    { PROF("lstm2"); if (c3b_launch_lstm2_tc(m, b, n, tile2, m->lstm2_split != 0, s)) return 1; }
     int nsplit = 1;
     { PROF("tail"); if (c3b_launch_tail(m, b.h2, n, (int)bp, y, b.z4, &nsplit, s)) return 1; }
     if (tap) {

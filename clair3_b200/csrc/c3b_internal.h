@@ -517,6 +517,7 @@ struct c3b_model {
     int lstm_tile = 0;
     int profile = 0;
     int lstm_wg = 2;                   // warpgroups (one sub-tile of sites each) per LSTM CTA (option "lstm_wg": 1 or 2)
+    int lstm2_split = 1;               // LSTM2 split by block pair (option "lstm2_split"): 1 lstm2_split_kernel, 0 the sub-tile kernel
     int lstm_mufu16 = 0;               // 1: packed tanh.approx.f16x2 gate activations, 0 (default, faster: the epilogue is issue-bound): fp32 tanh.approx
     int tap_ws = -1;                   // debug: workspace index c3b_get_tap reads
     int taps = 0;                      // debug option "taps": record where the intermediate activations of a forward live
@@ -609,7 +610,7 @@ int c3b_launch_tail(const c3b_model *m, const op_t *act, int64_t batch, int bp, 
 // LSTM1 reads the chunk's `batch` sites straight from src and builds its x operand columns itself
 int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, const PileupSrc &src, int64_t batch, int tile,
                         cudaStream_t s);
-int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s);
+int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, bool split, cudaStream_t s);
 
 struct PconvArgs {
     const op_t *in;            // planar padded, c channels

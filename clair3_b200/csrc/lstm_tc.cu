@@ -33,6 +33,16 @@
 // no faster for LSTM2: it serialises the two warpgroups' MMA chains, which otherwise overlap.)  LSTM2's pre-gates of block pair
 // p + 1 (after the last pair: the next step's first) are loaded right after the MMAs of pair p are issued, so their DRAM
 // latency hides behind a whole MMA / cell-math phase instead of stalling the start of every pair.
+//
+// LSTM2 split by block pair (lstm2_split_kernel).  One CTA = one direction x NB sites (32, or 16 under the latency tile rule)
+// with five warpgroups, 640 threads; warpgroup p issues only block pair p's 2 x K/16 wgmmas (same descriptors, k order and N),
+// runs the cell math of units 32p .. 32p+31 and writes their h_t into a double-buffered operand (step s reads buffer s & 1 and
+// writes the other), so one CTA barrier per step is the only exchange.  W_hh 200 KB + 2 x 20 x (NB+1) x 16 B = 221 KB at NB = 32;
+// 94 registers per thread.  The five chains share one tensor pipe (one m64n32k16 from shared memory every ~46 cycles on H100);
+// issued together they interleave and all finish last, so no cell math overlaps an MMA (6.2 k cycles per 32-site step).  Issued
+// in block-pair order they finish in turn, and each warpgroup's cell math runs under the later chains (5.0 k cycles, against
+// 10.8 k for 64 sites in the sub-tile kernel).  Each block pair's weights have their own mbarrier, so warpgroup 0 starts step 0
+// once its 40 KB have arrived.
 #include <type_traits>
 
 #include "c3b_internal.h"
@@ -446,6 +456,163 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
     }
 }
 
+// LSTM2 split by block pair (option "lstm2_split", see the header): one CTA = one direction x NB sites, five warpgroups, and
+// warpgroup pp owns block pair pp (hidden units 32pp .. 32pp + 31) of all NB sites.  The per-site arithmetic is lstm_tc_kernel's
+// for LAYER2: the same A blocks, B columns, k order and N per wgmma chain, the same cell math.
+template <int NB, bool MUFU16>
+__global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
+    constexpr int H = 160;
+    constexpr int K = H;
+    constexpr int NP = H / 32;
+    constexpr uint32_t kBlkBytes = (K / 8) * 64 * 16;
+    constexpr uint32_t W_BYTES = 2 * NP * kBlkBytes;
+    constexpr uint32_t LBO_B = (NB + 1) * 16;
+    constexpr uint32_t B_BYTES = (K / 8) * LBO_B;
+
+    extern __shared__ __align__(128) uint8_t smem[];
+    __shared__ uint64_t w_bar[NP];                  // one per block pair: a warpgroup starts once its own 40 KB have arrived
+
+    const int tid = threadIdx.x;
+    const int pp = tid >> 7;                        // this warpgroup's block pair
+    const int wt = tid & 127;
+    const int w = wt >> 5;
+    const int lane = tid & 31;
+    const int q0 = lane >> 2;
+    const int s0 = 2 * (lane & 3);
+    const int dir = blockIdx.y;
+    const int b0 = blockIdx.x * NB;
+    // two operand buffers of h: step s reads buffer s & 1 and writes h_t into the other, so one CTA barrier per step orders both
+    // the reads of step s - 1 before the writes of step s + 1 and the writes of step s before the reads of step s + 1
+    uint8_t *b_smem = smem + W_BYTES;
+    const uint32_t w_addr = ptx::smem_u32(smem);
+    const uint32_t b_addr = ptx::smem_u32(b_smem);
+
+    if (tid == 0) {
+#pragma unroll
+        for (int m = 0; m < NP; ++m) ptx::mbar_init(&w_bar[m], 1);
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+    if (tid == 0) {
+        const char *src = reinterpret_cast<const char *>(p.w_img) + (size_t)dir * W_BYTES;
+#pragma unroll 1
+        for (int m = 0; m < NP; ++m) {
+            ptx::mbar_arrive_expect_tx(&w_bar[m], 2 * kBlkBytes);
+            ptx::bulk_g2s(w_addr + 2 * m * kBlkBytes, src + (size_t)2 * m * kBlkBytes, 2 * kBlkBytes, &w_bar[m]);
+        }
+    }
+    for (uint32_t i = tid * 16; i < B_BYTES; i += 640 * 16) *reinterpret_cast<uint4 *>(b_smem + i) = make_uint4(0, 0, 0, 0);   // h_{-1}
+
+    float c[NB / 4];
+#pragma unroll
+    for (int i = 0; i < NB / 4; ++i) c[i] = 0.f;
+
+    // pre-gates of this thread's unit, one 8-byte word (i, f, g, o) per site, for the next step: loaded a whole step early
+    uint2 pgn[NB / 4];
+    const __half *pgp = p.pg + (size_t)dir * 640 + pp * 128 + 4 * (8 * w + q0);
+    auto load_pg = [&](int tt) {
+#pragma unroll
+        for (int i = 0; i < NB / 8; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+                pgn[2 * i + e] = *reinterpret_cast<const uint2 *>(pgp + ((size_t)tt * p.bp + b0 + 8 * i + s0 + e) * 1280);
+    };
+    load_pg(dir ? C3B_T - 1 : 0);
+    // h of time tt (in operand buffer `buf`) -> hout: this warpgroup's four k-groups
+    auto copy_out = [&](int tt, int buf) {
+        for (int idx = wt; idx < NB * 4; idx += 128) {
+            const int kgh = 4 * pp + idx / NB, n = idx % NB;
+            *reinterpret_cast<uint4 *>(p.hout + h_out_offset<true>(tt, dir, kgh, b0 + n, p.bp)) =
+                *reinterpret_cast<const uint4 *>(b_smem + buf * B_BYTES + kgh * LBO_B + n * 16);
+        }
+    };
+
+    const bool tr = p.trace != nullptr && tid == 0 && blockIdx.x == 0 && blockIdx.y == 0;
+    for (int step = 0; step < C3B_T; ++step) {
+        const int t = dir ? (C3B_T - 1 - step) : step;
+        const int cur = step & 1;
+        ptx::fence_proxy_async_smem();
+        __syncthreads();                            // h_{t-1} is in buffer cur; every read of buffer cur ^ 1 is done
+        if (tr) p.trace[step * 4 + 0] = clock64();
+        float acc0[NB / 2], acc1[NB / 2];
+        // the warpgroups issue their chains in block-pair order (named barrier pp: warpgroup pp - 1 arrives once its chain is
+        // issued), so the tensor pipe finishes them one after another and each warpgroup's cell math runs under the later
+        // warpgroups' MMAs; issued together, the five chains interleave and every cell math waits for the last MMA
+        if (step == 0) ptx::mbar_wait(&w_bar[pp], 0);
+        if (pp > 0) ptx::named_bar_sync(pp, 256);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < K / 16; ++ks) {
+            const uint64_t bd = ptx::wgmma_desc(b_addr + cur * B_BYTES + ks * 2 * LBO_B, LBO_B, 128);
+            const uint32_t a0 = w_addr + (2 * pp) * kBlkBytes + ks * 2 * 1024;
+            wgmma_nb<NB>(acc0, ptx::wgmma_desc(a0, 1024, 128), bd, ks > 0);
+            wgmma_nb<NB>(acc1, ptx::wgmma_desc(a0 + kBlkBytes, 1024, 128), bd, ks > 0);
+        }
+        ptx::wgmma_commit();
+        if (pp + 1 < NP) ptx::named_bar_arrive(pp + 1, 256);
+        // this step's pre-gates arrived during the last step; start the next step's, and ship h_{t-1} while the MMAs run
+        uint2 pgv[NB / 4];
+#pragma unroll
+        for (int i = 0; i < NB / 4; ++i) pgv[i] = pgn[i];
+        if (step + 1 < C3B_T) load_pg(dir ? t - 1 : t + 1);
+        if (step > 0) copy_out(dir ? t + 1 : t - 1, cur);
+        ptx::wgmma_wait<0>();
+        ptx::fence_operand(acc0);
+        ptx::fence_operand(acc1);
+        if (tr) p.trace[step * 4 + 1] = clock64();
+        uint32_t hq[NB / 8];
+#pragma unroll
+        for (int i = 0; i < NB / 8; ++i) {
+            float gi[2], gf[2], gg[2], go[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                gi[e] = acc0[4 * i + e] + half_lo(pgv[2 * i + e].x);
+                gf[e] = acc0[4 * i + 2 + e] + half_hi(pgv[2 * i + e].x);
+                gg[e] = acc1[4 * i + e] + half_lo(pgv[2 * i + e].y);
+                go[e] = acc1[4 * i + 2 + e] + half_hi(pgv[2 * i + e].y);
+            }
+            if (MUFU16) {
+                hq[i] = lstm_cell_h2(gi, gf, gg, go, &c[2 * i]);
+            } else {
+                const float h0 = lstm_cell(gi[0], gf[0], gg[0], go[0], c[2 * i]);
+                const float h1 = lstm_cell(gi[1], gf[1], gg[1], go[1], c[2 * i + 1]);
+                hq[i] = pack_f16x2(h0, h1);
+            }
+        }
+        if (tr) p.trace[step * 4 + 2] = clock64();
+        // h_t -> buffer cur ^ 1, element (site n, k = unit)
+        const uint32_t kcol = 32 * pp + 8 * w + q0;
+        uint8_t *dst = b_smem + (cur ^ 1) * B_BYTES + (kcol >> 3) * LBO_B + (kcol & 7) * 2;
+#pragma unroll
+        for (int i = 0; i < NB / 8; ++i) {
+            *reinterpret_cast<uint16_t *>(dst + (8 * i + s0) * 16) = (uint16_t)(hq[i] & 0xffffu);
+            *reinterpret_cast<uint16_t *>(dst + (8 * i + s0 + 1) * 16) = (uint16_t)(hq[i] >> 16);
+        }
+        if (tr) p.trace[step * 4 + 3] = clock64();
+    }
+
+    // last h
+    __syncthreads();
+    copy_out(dir ? 0 : C3B_T - 1, C3B_T & 1);
+}
+
+template <int NB, bool MUFU16>
+int launch_lstm2_split_impl(const LstmDev &p, cudaStream_t s) {
+    const size_t smem = (size_t)4 * 160 * 160 * 2 + (size_t)2 * (160 / 8) * (NB + 1) * 16;   // W_hh + two h operand buffers
+    auto kern = lstm2_split_kernel<NB, MUFU16>;
+    C3B_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid(p.bp / NB, 2);
+    c3b_note_grid((long long)grid.x * grid.y);
+    kern<<<grid, 640, smem, s>>>(p);
+    C3B_CUDA(cudaGetLastError());
+    return 0;
+}
+
+template <int NB>
+int launch_lstm2_split(const LstmDev &p, bool mufu16, cudaStream_t s) {
+    return mufu16 ? launch_lstm2_split_impl<NB, true>(p, s) : launch_lstm2_split_impl<NB, false>(p, s);
+}
+
 template <int NB, bool LAYER2, bool MUFU16, int WG, typename T>
 int launch_lstm_impl(const LstmDev &p, cudaStream_t s) {
     constexpr int K = (LAYER2 ? 0 : C3B_X1_COLS) + (LAYER2 ? 160 : 128);
@@ -503,7 +670,7 @@ int c3b_launch_lstm1_tc(const c3b_model *m, const TcPileupBuffers &b, const Pile
     return 1;
 }
 
-int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, cudaStream_t s) {
+int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t batch, int tile, bool split, cudaStream_t s) {
     LstmDev p = {};
     p.w_img = m->lstm_tc[1];
     p.pg = b.pg;
@@ -511,9 +678,16 @@ int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t ba
     p.trace = m->lstm_trace ? m->lstm_trace + C3B_T * 4 : nullptr;
     p.bp = b.bp;
     const_cast<c3b_model *>(m)->launches++;
-    switch (tile) {
-        case 16: return launch_lstm<16, true>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
-        case 32: return launch_lstm<32, true>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
+    if (split) {
+        switch (tile) {
+            case 16: return launch_lstm2_split<16>(p, m->lstm_mufu16 != 0, s);
+            case 32: return launch_lstm2_split<32>(p, m->lstm_mufu16 != 0, s);
+        }
+    } else {
+        switch (tile) {
+            case 16: return launch_lstm<16, true>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
+            case 32: return launch_lstm<32, true>(p, m->lstm_mufu16 != 0, m->lstm_wg, s);
+        }
     }
     c3b_set_error("lstm2: unsupported tile %d", tile);
     return 1;

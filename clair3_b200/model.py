@@ -110,7 +110,8 @@ class _C3BModule:
         return self
 
     def set_option(self, name, value):
-        """Kernel options: precision (0 fp16 tensor cores | 1 fp32 debug), chunk_sites, lstm_tile, lstm_wg, profile, taps."""
+        """Kernel options: precision (0 fp16 tensor cores | 1 fp32 debug), chunk_sites, lstm_tile, lstm_wg, lstm2_split, profile,
+        taps."""
         self._options[name] = int(value)
         if self._handle is not None:
             check(lib().c3b_set_option(self._handle, name.encode(), int(value)))

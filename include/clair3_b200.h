@@ -62,9 +62,10 @@ int c3b_set_param(c3b_model *m, const char *key, const void *host_data, int dtyp
 int c3b_finalize(c3b_model *m);
 
 /* name: "precision" (C3B_PREC_*), "chunk_sites" (sites per internal pass), "lstm_tile" (batch columns per LSTM CTA sub-tile:
- * 16|32|64, 0 = auto; LSTM2 uses at most 32), "lstm_wg" (warpgroups per LSTM CTA, one sub-tile each: 1|2).  With lstm_tile 0
- * the library picks by call shape between bit-identical variants: synchronous host-buffer calls (one batch in flight) get the
- * LSTM tile with the shortest latency, stream-ordered calls the one with the least SM-time,
+ * 16|32|64, 0 = auto; LSTM2 uses at most 32), "lstm_wg" (warpgroups per LSTM CTA, one sub-tile each: 1|2; LSTM2 only with
+ * lstm2_split 0), "lstm2_split" (1, default: LSTM2 with five warpgroups per CTA, one gate block pair each; 0: lstm_wg
+ * sub-tiles).  With lstm_tile 0 the library picks by call shape between bit-identical variants: synchronous host-buffer calls
+ * (one batch in flight) get the LSTM tile with the shortest latency, stream-ordered calls the one with the least SM-time,
  * "profile" (1: bracket every kernel launch with CUDA events on its stream and accumulate per-kernel time; setting it resets the
  * totals), "taps" (1: remember where the intermediate activations of a forward live, for c3b_get_tap in clair3_b200_debug.h).
  * Debug-only options are listed in clair3_b200_debug.h. */
