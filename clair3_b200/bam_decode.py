@@ -5,7 +5,9 @@ and with a ``.bai`` index the compressed byte range of the region (``bam_io.read
 BGZF block headers.  The GPU inflates the blocks, finds the record chain, parses and filters the records exactly as
 ``bam_io.read_bam(path, contig, start, end)`` does and scatters them into packed arrays.  The result is a
 ``records.DeviceBamRecords`` that ``PileupCounter.count`` and ``FullAlignmentBuilder.build`` take as they are: a region goes
-from compressed bytes to call records on the device.  No CPU fallback: everything here calls ``libclair3b200.so``.
+from compressed bytes to call records on the device.  ``fetch_fasta`` does the same for a window of a bgzip-compressed
+reference FASTA: the host finds the covering blocks through the ``.fai`` and ``.gzi``, the GPU inflates them and gathers the
+bases.  No CPU fallback: everything here calls ``libclair3b200.so``.
 """
 from __future__ import annotations
 
@@ -31,6 +33,7 @@ class BamDecoder(_Handle):
     def __init__(self, device=0):
         super().__init__(device)
         self._headers = {}
+        self._fasta = {}
 
     def _lib(self):
         return lib()
@@ -92,4 +95,52 @@ class BamDecoder(_Handle):
             setattr(out, f.name, ffi.cast(f.ctype + " *", v.data_ptr()))
         check(L.c3b_bam_fetch(self._h, out, 1))
         return DeviceBamRecords.from_tensors(t, self._device, ref_seq)
+
+    def _fasta_index(self, path, fai, gzi):
+        """({name: .fai row}, .gzi table) of a BGZF FASTA, read once per file."""
+        key = (os.path.abspath(path), os.path.getmtime(path), os.path.getsize(path), fai, gzi)
+        if key not in self._fasta:
+            gzi_path = bam_io.fasta_bgzf_gzi(path, gzi)
+            if gzi_path is None:
+                raise ValueError("%s: not a bgzip-compressed FASTA; read a plain FASTA with bam_io.fetch_fasta" % path)
+            self._fasta[key] = ({r[0]: r for r in bam_io.read_fai(fai or str(path) + ".fai")}, bam_io.read_gzi(gzi_path))
+        return self._fasta[key]
+
+    def fetch_fasta(self, path, name, start=0, end=None, fai=None, gzi=None, wait=True):
+        """Bases [start, end) of sequence ``name`` of a bgzip-compressed FASTA, clipped to the sequence, as a uint8 tensor on the
+        decoder's device whose bytes equal ``bam_io.fetch_fasta(path, name, start, end)``.  The host reads the ``.fai`` (default
+        ``path + ".fai"``), the ``.gzi`` (default ``path + ".gzi"``) and the compressed blocks that cover the window; the GPU
+        inflates them and gathers the bases (``c3b_fasta_fetch``), on the device's current torch stream.  ``wait=False``
+        returns without waiting for the status of the blocks: the caller then calls ``fasta_status`` after its own next wait
+        (``decode`` makes one), before it trusts the bases."""
+        rows, gzi_table = self._fasta_index(path, fai, gzi)
+        if name not in rows:
+            raise ValueError("sequence %r not found in the index of %s" % (name, path))
+        _, length, _, lb, lw = row = rows[name]
+        start = max(0, int(start))
+        end = length if end is None else min(int(end), length)
+        if end <= start:
+            return torch.empty(0, dtype=torch.uint8, device=self._device)
+        _, _, c0, c1, u0 = bam_io.fasta_span(row, start, end, gzi_table)
+        with open(path, "rb") as f:
+            f.seek(c0)
+            data = f.read() if c1 is None else f.read(c1 - c0)
+        return self.fetch_fasta_bytes(data, u0, start, lb, lw, end - start, wait=wait)
+
+    def fetch_fasta_bytes(self, data, first_uoff, start, line_bases, line_bytes, n_bases, wait=True):
+        """``fetch_fasta`` on whole BGZF blocks already in memory: ``data`` (bytes-like), the window's offset in the first
+        block's data, its first base on the sequence, the sequence's line geometry from the ``.fai`` and the number of bases."""
+        data = memoryview(data).cast("B") if not isinstance(data, (bytes, bytearray)) else data
+        out = torch.empty(max(int(n_bases), 1), dtype=torch.uint8, device=self._device)[:int(n_bases)]
+        buf = ffi.from_buffer(data) if len(data) else ffi.NULL
+        check(self._lib().c3b_fasta_fetch(self._h, buf, len(data), int(first_uoff), int(start), int(line_bases), int(line_bytes),
+                                          int(n_bases), ffi.cast("uint8_t *", out.data_ptr()), self._stream()))
+        if wait:
+            self.fasta_status()
+        return out
+
+    def fasta_status(self):
+        """Raises when a block of the last ``fetch_fasta`` did not inflate (C3BError naming the block and the reason); waits for
+        that fetch's kernels unless the stream has passed them."""
+        check(self._lib().c3b_fasta_status(self._h))
 

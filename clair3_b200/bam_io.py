@@ -14,7 +14,8 @@ Two readers produce the records the GPU counter and builder take:
 
 A writer is included so that tests (and users without samtools) can produce valid files, and ``write_bai`` indexes them as the
 specification's section 5.2 describes.  CRAM and CSI indexes are not handled.  The reference bases come out of a FASTA file
-(``read_fasta``, or ``fetch_fasta`` at random access through its ``.fai``).  ``idxstats`` reads the mapped counts of the
+(``read_fasta``, or ``fetch_fasta`` at random access through its ``.fai``; for a bgzip-compressed FASTA also its ``.gzi``,
+through which ``read_gzi`` / ``fasta_span`` find the blocks that ``BamDecoder.fetch_fasta`` inflates on the GPU).  ``idxstats`` reads the mapped counts of the
 ``.bai``; ``write_bgzf`` and ``write_tbi`` write a bgzipped, tabix-indexed VCF as ``bgzip`` and ``tabix -p vcf`` do.
 """
 from __future__ import annotations
@@ -367,26 +368,108 @@ def read_fai(path):
     return out
 
 
-def fetch_fasta(path, name, start=0, end=None, fai=None):
-    """Bases [start, end) of sequence ``name`` of a plain FASTA through its ``.fai`` (default ``path + ".fai"``), clipped to the
-    sequence, case kept: what ``read_fasta`` returns, read at random access as ``faidx_fetch_seq`` reads it.  A bgzip-compressed
-    FASTA is refused (ValueError)."""
+def fasta_row(path, name, fai=None):
+    """The ``.fai`` row (name, length, offset, line bases, line bytes) of sequence ``name`` (index default ``path + ".fai"``)."""
     rows = {r[0]: r for r in read_fai(fai or str(path) + ".fai")}
     if name not in rows:
         raise ValueError("sequence %r not found in the index of %s" % (name, path))
-    _, length, off, lb, lw = rows[name]
+    return rows[name]
+
+
+def fasta_bgzf_gzi(path, gzi=None):
+    """The ``.gzi`` path of a FASTA at ``path``: None for a plain FASTA, ``gzi`` (default ``path + ".gzi"``, as htslib and
+    samtools name it) for a BGZF one.  A gzip file that is not BGZF is refused (ValueError), as ``samtools faidx`` refuses it;
+    a BGZF file without its ``.gzi`` raises FileNotFoundError."""
+    with open(path, "rb") as f:
+        gz = f.read(2) == b"\x1f\x8b"
+    if not gz:
+        return None
+    if not is_bgzf(path):
+        raise ValueError("%s: compressed FASTA is not supported unless bgzip-compressed; decompress it (and re-index it), or "
+                         "recompress it with bgzip" % path)
+    gzi = gzi or str(path) + ".gzi"
+    if not os.path.exists(gzi):
+        raise FileNotFoundError("%s: the BGZF index %s is missing; run samtools faidx on the FASTA to write it" % (path, gzi))
+    return gzi
+
+
+def fasta_span(fai_row, start, end, gzi):
+    """Where the bases [start, end) (0 <= start < end <= length) of a ``.fai`` row lie in a BGZF FASTA: (a, b, c0, c1, u0).
+    [a, b) is the uncompressed byte range ``fetch_fasta`` reads, line ends included; [c0, c1) the compressed byte range of the
+    whole blocks that cover it (c1 None: to the end of the file), from ``gzi`` (``read_gzi``'s table); u0 = a less the
+    uncompressed offset of the first of those blocks."""
+    _, _, off, lb, lw = fai_row
+    a = off + start // lb * lw + start % lb
+    b = off + (end - 1) // lb * lw + (end - 1) % lb + 1
+    gzi = np.asarray(gzi, np.int64).reshape(-1, 2)
+    # block k > 0 starts at gzi[k - 1]; block 0 at (0, 0)
+    i = int(np.searchsorted(gzi[:, 1], a, side="right"))       # the last block that starts at or before a
+    j = int(np.searchsorted(gzi[:, 1], b - 1, side="right"))   # and the one holding b - 1
+    c0, u = (int(gzi[i - 1, 0]), int(gzi[i - 1, 1])) if i else (0, 0)
+    return a, b, c0, int(gzi[j, 0]) if j < len(gzi) else None, a - u
+
+
+def fetch_fasta(path, name, start=0, end=None, fai=None, gzi=None):
+    """Bases [start, end) of sequence ``name`` of a FASTA through its ``.fai`` (default ``path + ".fai"``), clipped to the
+    sequence, case kept: what ``read_fasta`` returns, read at random access as ``faidx_fetch_seq`` reads it.  A bgzip-compressed
+    FASTA is read through its ``.gzi`` (``fasta_bgzf_gzi``): the blocks that cover the window are inflated with zlib.  A gzip
+    FASTA that is not BGZF is refused (ValueError)."""
+    _, length, _, lb, lw = row = fasta_row(path, name, fai)
+    gzi = fasta_bgzf_gzi(path, gzi)
     start = max(0, int(start))
     end = length if end is None else min(int(end), length)
     if end <= start:
         return ""
+    a, b, c0, c1, u0 = fasta_span(row, start, end, read_gzi(gzi) if gzi else [])
     with open(path, "rb") as f:
-        if f.read(2) == b"\x1f\x8b":
-            raise ValueError("%s: compressed FASTA is not supported; decompress it (and re-index it)" % path)
-        a = off + start // lb * lw + start % lb
-        b = off + (end - 1) // lb * lw + (end - 1) % lb + 1
-        f.seek(a)
-        raw = f.read(b - a)
+        if gzi is None:
+            f.seek(a)
+            raw = f.read(b - a)
+        else:
+            f.seek(c0)
+            data = f.read() if c1 is None else f.read(c1 - c0)
+            parts, off, have = [], 0, 0
+            while off < len(data) and have < u0 + b - a:
+                size, part = _inflate_block(data, off)
+                parts.append(part)
+                off += size
+                have += len(part)
+            raw = b"".join(parts)[u0:u0 + b - a]
+            if len(raw) != b - a:
+                raise ValueError("%s: the blocks the .gzi names for %s:%d-%d hold %d of its %d bytes" % (path, name, start, end,
+                                                                                                         len(raw), b - a))
     return raw.replace(b"\n", b"").replace(b"\r", b"").decode()
+
+
+def read_gzi(path):
+    """htslib's ``.gzi`` index of a BGZF file: a little-endian uint64 count, then that many (compressed offset, uncompressed
+    offset) uint64 pairs, one per block after the first (whose (0, 0) is implicit).  Returns the pairs as an int64 [count, 2]
+    array; a file whose size does not match its count, or whose columns are not ascending, raises ValueError."""
+    with open(path, "rb") as f:
+        buf = f.read()
+    if len(buf) < 8:
+        raise ValueError("%s: a .gzi index starts with an 8-byte count; the file holds %d bytes" % (path, len(buf)))
+    n, = struct.unpack_from("<Q", buf, 0)
+    if len(buf) != 8 + 16 * n:
+        raise ValueError("%s: a .gzi index of %d entries holds %d bytes, not %d" % (path, n, len(buf), 8 + 16 * n))
+    t = np.frombuffer(buf, dtype="<u8", count=2 * n, offset=8).reshape(-1, 2)
+    if (t >= 1 << 63).any():
+        raise ValueError("%s: a .gzi offset exceeds 2^63" % path)
+    t = t.astype(np.int64)
+    col = np.concatenate([np.zeros((1, 2), np.int64), t])
+    if (np.diff(col[:, 0]) <= 0).any() or (np.diff(col[:, 1]) < 0).any():
+        raise ValueError("%s: the .gzi offsets are not ascending" % path)
+    return t
+
+
+def is_bgzf(path):
+    """Whether the file at ``path`` starts with a BGZF block: its header passes ``bgzf_block``'s checks, the ones the GPU
+    reader's ``c3b_bam_decode`` makes."""
+    with open(path, "rb") as f:
+        try:
+            return _read_block(f, 0)[0] > 0
+        except (ValueError, struct.error):
+            return False
 
 
 # ---- BGZF blocks, the header and the .bai index: what the GPU reader (clair3_b200.bam_decode) needs from the host ----

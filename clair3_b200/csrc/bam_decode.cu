@@ -27,6 +27,9 @@
 //   B8 block scans      record index, CIGAR words, sequence bytes (and qualities, names, mv values) of each kept record.
 //   B9 bam_scatter      one warp per kept record: every array into the packed outputs.
 //
+// c3b_fasta_fetch reuses the upload and B1 for the blocks of a bgzip-compressed FASTA window, then gathers the window's bases
+// with one thread each, skipping the line ends by arithmetic; c3b_fasta_status reads its bad-block word.
+//
 // The only host wait is c3b_bam_sizes, after the totals.  Every buffer is sized from what the host knows before the decode: the
 // compressed bytes and the sum of ISIZE (U): a record takes at least 36 bytes of U, so there are at most U / 36 + 1 records, and
 // every value array holds at most U entries.  Valid input never reaches a capacity; malformed input is bounds-checked at every
@@ -434,6 +437,16 @@ __global__ void __launch_bounds__(WARPS * 32) bam_scatter_kernel(ScatterArgs A) 
     }
 }
 
+// c3b_fasta_fetch's gather, after bam_inflate has inflated the window's blocks: one thread per base of the window.  Base i sits (r + i) / lb lines and (r + i) % lb bases past the
+// start of the line that holds the window's first base, which lies r bases before u0; the line ends between are skipped.
+__global__ void fasta_gather_kernel(const uint8_t *__restrict__ U, int64_t u0, int64_t r, int64_t lb, int64_t lw, int64_t n,
+                                    uint8_t *__restrict__ out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t k = r + i;
+    out[i] = U[u0 - r + k / lb * lw + k % lb];
+}
+
 size_t inflate_smem() { return 65536 + (sizeof(Tables) + 15) / 16 * 16 + 256 * 4; }
 
 const char *status_name(int st) {
@@ -468,9 +481,18 @@ struct c3b_bam : C3bRegionWorkspace {
     int64_t n_bytes = 0;
     bool decoded = false, sized = false, fa_fields = false;
     int64_t n_reads = 0, n_cigar_out = 0, n_seq_out = 0, n_qual = 0, n_name = 0, n_mv_out = 0;   // totals
+    // the last FASTA fetch: its bad-block word on the device and its pinned copy, the event after that copy, and the offsets of
+    // its blocks for the error
+    C3bBuf fasta_bad;
+    unsigned long long *fasta_bad_host = nullptr;
+    cudaEvent_t fetched = nullptr;
+    std::vector<int64_t> fasta_block_start;
+    bool fasta_pending = false, timed = false;
     ~c3b_bam() {
         if (staging) cudaFreeHost(staging);
         if (uploaded) cudaEventDestroy(uploaded);
+        if (fasta_bad_host) cudaFreeHost(fasta_bad_host);
+        if (fetched) cudaEventDestroy(fetched);
     }
 };
 
@@ -522,6 +544,30 @@ static int bam_blocks(const uint8_t *p, int64_t n, std::vector<Block> &out, std:
     return 0;
 }
 
+// Copies the block table (w->blocks) and bytes[0 .. n_bytes) into the pinned staging buffer, after the previous upload has left
+// it.  bam_upload then queues the staged bytes into w->in.
+static int bam_stage(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, const char *who) {
+    const size_t table = w->blocks.size() * sizeof(Block), up = table + (size_t)n_bytes;
+    C3B_CUDA(cudaEventSynchronize(w->uploaded));
+    if (up > w->staging_cap) {
+        if (w->staging) cudaFreeHost(w->staging);
+        w->staging = nullptr;
+        w->staging_cap = 0;
+        const size_t want = up + up / 4 + 4096;
+        if (cudaMallocHost((void **)&w->staging, want) != cudaSuccess) { c3b_set_error("%s: pinned allocation of %zu bytes failed", who, want); return 1; }
+        w->staging_cap = want;
+    }
+    if (table) memcpy(w->staging, w->blocks.data(), table);
+    if (n_bytes) memcpy(w->staging + table, bytes, (size_t)n_bytes);
+    return 0;
+}
+
+static int bam_upload(c3b_bam *w, size_t up, cudaStream_t s) {
+    if (up) C3B_CUDA(cudaMemcpyAsync(w->in.p, w->staging, up, cudaMemcpyHostToDevice, s));
+    C3B_CUDA(cudaEventRecord(w->uploaded, s));
+    return 0;
+}
+
 static inline unsigned bam_grid(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
 extern "C" {
@@ -530,8 +576,10 @@ int c3b_bam_create(c3b_bam **out, int device_ordinal) {
     if (c3b_region_create(out, device_ordinal, 1, N_COUNTERS, 0, "c3b_bam_create")) return 1;
     c3b_bam *w = *out;
     if (cudaEventCreateWithFlags(&w->uploaded, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&w->fetched, cudaEventDisableTiming) != cudaSuccess ||
+        cudaMallocHost((void **)&w->fasta_bad_host, 8) != cudaSuccess || w->fasta_bad.ensure(8, nullptr, "c3b_bam_create") ||
         cudaFuncSetAttribute(bam_inflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)inflate_smem()) != cudaSuccess) {
-        c3b_set_error("c3b_bam_create: event creation or the inflate kernel's shared-memory setting failed");
+        c3b_set_error("c3b_bam_create: event creation, a small allocation or the inflate kernel's shared-memory setting failed");
         c3b_bam_destroy(w);
         *out = nullptr;
         return 1;
@@ -559,24 +607,13 @@ int c3b_bam_decode(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t fi
     w->fa_fields = fa_fields != 0;
     w->n_bytes = n_bytes;
     const int nb = (int)w->blocks.size();
-    const size_t table = (size_t)nb * sizeof(Block), up = table + (size_t)n_bytes;
-    // staging: wait until the previous decode's upload has left it
-    C3B_CUDA(cudaEventSynchronize(w->uploaded));
-    if (up > w->staging_cap) {
-        if (w->staging) cudaFreeHost(w->staging);
-        w->staging = nullptr;
-        w->staging_cap = 0;
-        const size_t want = up + up / 4 + 4096;
-        if (cudaMallocHost((void **)&w->staging, want) != cudaSuccess) { c3b_set_error("%s: pinned allocation of %zu bytes failed", who, want); return 1; }
-        w->staging_cap = want;
-    }
-    if (nb) memcpy(w->staging, w->blocks.data(), table);
-    if (n_bytes) memcpy(w->staging + table, bytes, (size_t)n_bytes);
+    const size_t table = (size_t)nb * sizeof(Block);
+    if (bam_stage(w, bytes, n_bytes, who)) return 1;
 
     const int64_t Uz = total > 0 ? total : 1, cap = total / REC_MIN + 1, nbz = nb > 0 ? nb : 1;
     auto grow = [&](C3bBuf &b, size_t bytes_) { return b.ensure(bytes_ ? bytes_ : 1, s, "c3b_bam"); };
     const size_t c1 = (size_t)cap + 1;
-    if (grow(w->in, up) || grow(w->U, (size_t)Uz) || grow(w->mark, (size_t)Uz) || grow(w->spec_exit, nbz * 8) ||
+    if (grow(w->in, table + (size_t)n_bytes) || grow(w->U, (size_t)Uz) || grow(w->mark, (size_t)Uz) || grow(w->spec_exit, nbz * 8) ||
         grow(w->entry, nbz * 8) || grow(w->merge, nbz * 8) || grow(w->bcount, (nbz + 1) * 4) || grow(w->bbase, (nbz + 1) * 8) ||
         grow(w->rec_off, (size_t)cap * 8) || grow(w->keep, c1 * 4) || grow(w->c_cig, c1 * 4) || grow(w->c_seq, c1 * 4) ||
         grow(w->kidx, c1 * 8) || grow(w->cig_src, c1 * 8) || grow(w->cig_at, c1 * 8) || grow(w->seq_at, c1 * 8) || grow(w->pos, (size_t)cap * 8) ||
@@ -589,8 +626,7 @@ int c3b_bam_decode(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t fi
          grow(w->qual_off, c1 * 8) || grow(w->name_off, c1 * 8) || grow(w->mv_off, c1 * 8) || grow(w->qual, (size_t)Uz) ||
          grow(w->name, (size_t)Uz) || grow(w->mv, (size_t)Uz * 4)))
         return 1;
-    if (up) C3B_CUDA(cudaMemcpyAsync(w->in.p, w->staging, up, cudaMemcpyHostToDevice, s));
-    C3B_CUDA(cudaEventRecord(w->uploaded, s));
+    if (bam_upload(w, table + (size_t)n_bytes, s)) return 1;
 
     int64_t *cnt = w->counters.as<int64_t>();
     unsigned long long *bad = reinterpret_cast<unsigned long long *>(cnt), *stop = bad + 1, *err = bad + 2;
@@ -651,7 +687,70 @@ int c3b_bam_decode(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t fi
     C3B_CUDA(cudaEventRecord(w->ev[0][1], s));
     C3B_CUDA(cudaGetLastError());
     C3B_CUDA(cudaMemcpyAsync(w->host_counters, cnt, N_COUNTERS * 8, cudaMemcpyDeviceToHost, s));
-    w->decoded = true;
+    w->decoded = w->timed = true;
+    return 0;
+}
+
+int c3b_fasta_fetch(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t first_uoff, int64_t start, int64_t line_bases,
+                    int64_t line_bytes, int64_t n_bases, uint8_t *out, void *cuda_stream) {
+    const char *who = "c3b_fasta_fetch";
+    if (!w || (n_bytes > 0 && !bytes) || n_bytes < 0 || n_bases < 0 || (n_bases > 0 && !out)) {
+        c3b_set_error("%s: null or negative argument", who);
+        return 1;
+    }
+    w->fasta_pending = false;
+    if (n_bases == 0) return 0;
+    if (line_bases <= 0 || line_bytes < line_bases || start < 0 || first_uoff < 0) {
+        c3b_set_error("%s: line bases %lld / line bytes %lld / start %lld / first_uoff %lld are not a FASTA window's", who,
+                      (long long)line_bases, (long long)line_bytes, (long long)start, (long long)first_uoff);
+        return 1;
+    }
+    int64_t total = 0;
+    if (bam_blocks(bytes, n_bytes, w->blocks, w->fasta_block_start, &total, who)) return 1;
+    const int64_t r = start % line_bases, k = r + n_bases - 1;
+    const int64_t last = first_uoff - r + k / line_bases * line_bytes + k % line_bases;
+    if (last >= total) {
+        c3b_set_error("%s: the window's last base at uncompressed offset %lld lies past the %lld bytes its blocks inflate to", who,
+                      (long long)last, (long long)total);
+        return 1;
+    }
+    C3B_CUDA(cudaSetDevice(w->device));
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    w->stream = s;
+    const int nb = (int)w->blocks.size();
+    const size_t table = (size_t)nb * sizeof(Block);
+    if (bam_stage(w, bytes, n_bytes, who)) return 1;
+    if (w->in.ensure(table + (size_t)n_bytes, s, "c3b_bam") || w->U.ensure((size_t)total, s, "c3b_bam")) return 1;
+    if (bam_upload(w, table + (size_t)n_bytes, s)) return 1;
+    unsigned long long *bad = w->fasta_bad.as<unsigned long long>();
+    C3B_CUDA(cudaMemsetAsync(bad, 0xff, 8, s));
+    C3B_CUDA(cudaEventRecord(w->ev[0][0], s));
+    bam_inflate_kernel<<<nb, 32, inflate_smem(), s>>>(w->in.as<uint8_t>() + table, w->in.as<Block>(), w->U.as<uint8_t>(), bad);
+    fasta_gather_kernel<<<bam_grid(n_bases, 256), 256, 0, s>>>(w->U.as<uint8_t>(), first_uoff, r, line_bases, line_bytes, n_bases, out);
+    C3B_CUDA(cudaEventRecord(w->ev[0][1], s));
+    C3B_CUDA(cudaGetLastError());
+    w->launches[0] = 2;
+    w->timed = true;
+    C3B_CUDA(cudaMemcpyAsync(w->fasta_bad_host, bad, 8, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaEventRecord(w->fetched, s));
+    w->fasta_pending = true;
+    return 0;
+}
+
+int c3b_fasta_status(c3b_bam *w) {
+    const char *who = "c3b_fasta_status";
+    if (!w) { c3b_set_error("%s: null argument", who); return 1; }
+    if (!w->fasta_pending) return 0;
+    C3B_CUDA(cudaSetDevice(w->device));
+    C3B_CUDA(cudaEventSynchronize(w->fetched));
+    w->fasta_pending = false;
+    const unsigned long long bad = *w->fasta_bad_host;
+    if (bad != ~0ull) {
+        const size_t b = (size_t)(bad >> 4);
+        c3b_set_error("%s: BGZF block %zu (at byte %lld of the data): %s", who, b, (long long)w->fasta_block_start[b],
+                      status_name((int)(bad & 15)));
+        return 1;
+    }
     return 0;
 }
 
@@ -724,7 +823,7 @@ int c3b_bam_fetch(c3b_bam *w, const c3b_bam_out *out, int on_device) {
 }
 
 int c3b_bam_last_ms(c3b_bam *w, float *ms, int *launches) {
-    if (!w || !w->decoded) { c3b_set_error("c3b_bam_last_ms: no c3b_bam_decode has been issued"); return 1; }
+    if (!w || !w->timed) { c3b_set_error("c3b_bam_last_ms: no c3b_bam_decode or c3b_fasta_fetch has been issued"); return 1; }
     return w->elapsed(0, ms, launches);
 }
 

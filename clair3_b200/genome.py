@@ -20,7 +20,8 @@ own, and a site's network output does not depend on the sites it is batched with
 the number of ranks.
 
 Not implemented: phasing (``no_phasing_for_fa`` must be True: WhatsHap / LongPhase are not part of this project), gVCF, the
-haploid modes and ``platform="ilmn"`` (``NotImplementedError``); CRAM input and CSI indexes (``NotImplementedError``).
+haploid modes and ``platform="ilmn"`` (``NotImplementedError``); CRAM input and CSI indexes (``NotImplementedError``).  The
+reference FASTA may be bgzip-compressed with its ``.gzi`` (DESIGN.md 5g.1): each window is then inflated on the GPU.
 """
 from __future__ import annotations
 
@@ -56,12 +57,14 @@ def resolve_options(platform="ont", var_pct_full=None, ref_pct_full=None, snp_mi
     return var, ref, snp, indel
 
 
-def output_configs(enable_long_indel=False):
+def output_configs(enable_long_indel=False, keep_iupac_bases=False):
     """The two decoders' OutputConfig as the pipeline's CallVariantsFromCffi runs them: showRef on, ``--qual`` at its default 2
-    (the pipeline passes none), ``--add_indel_length`` for full alignment only, and the long-indel limit."""
+    (the pipeline passes none), ``--add_indel_length`` for full alignment only, the long-indel limit and
+    ``--keep_iupac_bases``, which both calls take."""
     out = []
     for pileup in (True, False):
-        cfg = decode.replay_config(pileup=pileup, add_indel_length=not pileup)._replace(is_show_reference=True)
+        cfg = decode.replay_config(pileup=pileup, add_indel_length=not pileup)._replace(is_show_reference=True,
+                                                                                        keep_iupac_bases=bool(keep_iupac_bases))
         if enable_long_indel:
             cfg = cfg._replace(enable_long_indel=True, maximum_variant_length_that_need_infer=LONG_INDEL)
         out.append(cfg)
@@ -79,8 +82,10 @@ def bam_index(bam_fn):
 
 
 def check_inputs(bam_fn, ref_fn):
-    """The files CheckEnvs and run_clair3.py require: the BAM with a ``.bai`` (``bam_index``) and the FASTA with a ``.fai``.
-    CRAM input and a BAM indexed only by a ``.csi`` are not supported here (NotImplementedError).  Returns the ``.bai`` path."""
+    """The files CheckEnvs and run_clair3.py require: the BAM with a ``.bai`` (``bam_index``) and the FASTA with a ``.fai`` -
+    plain, or bgzip-compressed with its ``.gzi`` too, as ``samtools faidx`` indexes it.  CRAM input and a BAM indexed only by a
+    ``.csi`` are not supported here (NotImplementedError); a gzip FASTA that is not BGZF is refused (ValueError).  Returns the
+    ``.bai`` path."""
     bam_fn, ref_fn = str(bam_fn), str(ref_fn)
     if bam_fn.endswith(".cram"):
         raise NotImplementedError("genome: CRAM input is not supported; give a BAM")
@@ -94,9 +99,13 @@ def check_inputs(bam_fn, ref_fn):
         if os.path.exists(bam_fn + ".csi") or os.path.exists(os.path.splitext(bam_fn)[0] + ".csi"):
             raise NotImplementedError("genome: CSI indexes are not supported; index the BAM with a .bai")
         raise FileNotFoundError("genome: BAM index %s.bai not found (samtools index the BAM first)" % bam_fn)
-    with open(ref_fn, "rb") as f:
-        if f.read(2) == b"\x1f\x8b":
-            raise ValueError("genome: compressed FASTA is not supported; decompress %s and index it" % ref_fn)
+    try:
+        bam_io.fasta_bgzf_gzi(ref_fn)
+    except ValueError:
+        raise ValueError("genome: compressed FASTA is not supported unless bgzip-compressed; decompress %s and index it, or "
+                         "recompress it with bgzip and samtools faidx it" % ref_fn) from None
+    except FileNotFoundError:
+        raise FileNotFoundError("genome: BGZF index %s.gzi not found (samtools faidx the FASTA first)" % ref_fn) from None
     return bai
 
 
@@ -323,8 +332,8 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
                 var_pct_full=None, ref_pct_full=None, snp_min_af=None, indel_min_af=None, min_mq=5, min_coverage=2,
                 call_snp_only=False, enable_long_indel=False, enable_variant_calling_at_sequence_head_and_tail=False,
                 print_ref_calls=False, pileup_only=False, no_phasing_for_fa=True, enable_dwell_time=False, gvcf=False,
-                haploid_precise=False, haploid_sensitive=False, split_bed_size=cascade.SPLIT_BED_SIZE, workspaces=None,
-                device=None, group=None, k=16):
+                haploid_precise=False, haploid_sensitive=False, keep_iupac_bases=False, split_bed_size=cascade.SPLIT_BED_SIZE,
+                workspaces=None, device=None, group=None, k=16):
     """Clair3's pipeline (scripts/clair3_c_impl_pipeline.py with ``--no_phasing_for_fa True``) over the genome: writes
     ``pileup.vcf.gz``, ``full_alignment.vcf.gz`` and ``merge_output.vcf.gz`` with their ``.tbi`` into ``out_dir``, as the
     reference does with its early exits (``file_texts``).  Options as run_clair3.py names them (None / 0 percentages and allele frequencies: the platform's defaults, see
@@ -349,7 +358,7 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
     tgt = targets.resolve(bed_fn, vcf_fn)
     genotyping = tgt is not None and tgt.kind == "vcf"
     var_pct, ref_pct, snp_af, indel_af = resolve_options(platform, var_pct_full, ref_pct_full, snp_min_af, indel_min_af, genotyping)
-    cfg_p, cfg_f = output_configs(enable_long_indel)
+    cfg_p, cfg_f = output_configs(enable_long_indel, keep_iupac_bases)
     max_indel = LONG_INDEL if enable_long_indel else decode.MAX_INFER_LENGTH
     rank, world = _rank(group)
     contigs, chunks = plan(bam_fn, ref_fn, ctg_name, include_all_ctgs, min_contig_size, chunk_size,
@@ -367,7 +376,7 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
     ws = workspaces or cascade.Workspaces(device)
     try:
         st = cascade.Stages(ws.counter._device)
-        read = functools.partial(_read_span, ws.decoder, bam_fn, ref_fn, index, lengths)
+        read = functools.partial(_read_span, ws.decoder, bam_fn, ref_fn, bam_io.is_bgzf(ref_fn), index, lengths)
         count = {"min_depth": min_coverage, "min_snp_af": snp_af, "min_indel_af": indel_af, "min_mq": min_mq,
                  "call_snp_only": call_snp_only, "call_ht": enable_variant_calling_at_sequence_head_and_tail,
                  "max_indel_length": max_indel}
@@ -401,12 +410,19 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
             ws.close()
 
 
-def _read_span(decoder, bam_fn, ref_fn, index, lengths, ctg, start, end, fa_fields):
+def _read_span(decoder, bam_fn, ref_fn, bgzf, index, lengths, ctg, start, end, fa_fields):
     """The records of the 0-based [start, end) of contig ``ctg``, decoded with the FASTA window the counter and the builder
-    read around it (``FETCH_EXPAND`` bases either side, clipped to the contig): (records, the window's start)."""
-    r0 = max(0, start - FETCH_EXPAND)
-    ref = bam_io.fetch_fasta(ref_fn, ctg, r0, min(lengths[ctg], end + FETCH_EXPAND + 1))
-    return decoder.decode(bam_fn, ctg, start, end, fa_fields=fa_fields, index=index, ref_seq=ref), r0
+    read around it (``FETCH_EXPAND`` bases either side, clipped to the contig): (records, the window's start).  A plain
+    FASTA's window is read on the host; a bgzip-compressed one's is inflated on the device, and its status is read after the
+    decode's own wait."""
+    r0, r1 = max(0, start - FETCH_EXPAND), min(lengths[ctg], end + FETCH_EXPAND + 1)
+    if not bgzf:
+        ref = bam_io.fetch_fasta(ref_fn, ctg, r0, r1)
+        return decoder.decode(bam_fn, ctg, start, end, fa_fields=fa_fields, index=index, ref_seq=ref), r0
+    ref = decoder.fetch_fasta(ref_fn, ctg, r0, r1, wait=False)
+    rec = decoder.decode(bam_fn, ctg, start, end, fa_fields=fa_fields, index=index, ref_seq=ref)
+    decoder.fasta_status()
+    return rec, r0
 
 
 def _pileup_chunks(counter, st, read, lengths, chunks, mine, tgt, model_p, cfg_p, k, count):

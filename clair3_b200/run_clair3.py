@@ -6,7 +6,8 @@
 Loads ``pileup.pt`` and ``full_alignment.pt`` from ``--model_path`` and writes ``pileup.vcf.gz``, ``full_alignment.vcf.gz`` and
 ``merge_output.vcf.gz`` with their ``.tbi`` into ``--output`` (``genome.call_genome``).  Several GPUs: start one process per GPU
 with ``torchrun --nproc_per_node N -m clair3_b200.run_clair3 ...``; each rank takes the GPU of its ``LOCAL_RANK``.
-``--threads`` is accepted and ignored.  Phasing (``--no_phasing_for_fa`` not True), ``--gvcf``, the haploid modes and
+``--ref_fn`` may be bgzip-compressed, with the ``.fai`` and ``.gzi`` ``samtools faidx`` writes.  ``--threads`` is accepted and
+ignored.  Phasing (``--no_phasing_for_fa`` not True), ``--gvcf``, the haploid modes and
 platform ``ilmn`` are refused.
 """
 from __future__ import annotations
@@ -51,7 +52,7 @@ def parser():
     p.add_argument("--min_coverage", type=int, default=2)
     for flag in ("--include_all_ctgs", "--call_snp_only", "--enable_long_indel", "--enable_variant_calling_at_sequence_head_and_tail",
                  "--print_ref_calls", "--pileup_only", "--no_phasing_for_fa", "--enable_dwell_time", "--gvcf", "--haploid_precise",
-                 "--haploid_sensitive"):
+                 "--haploid_sensitive", "--keep_iupac_bases"):
         p.add_argument(flag, nargs="?", const=True, default=False, type=_bool)
     return p
 
@@ -99,7 +100,7 @@ def main(argv=None):
             enable_variant_calling_at_sequence_head_and_tail=args.enable_variant_calling_at_sequence_head_and_tail,
             print_ref_calls=args.print_ref_calls, pileup_only=args.pileup_only, no_phasing_for_fa=args.no_phasing_for_fa,
             enable_dwell_time=args.enable_dwell_time, gvcf=args.gvcf, haploid_precise=args.haploid_precise,
-            haploid_sensitive=args.haploid_sensitive, device=dev, group=group)
+            haploid_sensitive=args.haploid_sensitive, keep_iupac_bases=args.keep_iupac_bases, device=dev, group=group)
     finally:
         if group is not None:
             import torch.distributed as dist

@@ -71,7 +71,27 @@ int c3b_bam_sizes(c3b_bam *w, int64_t *n_reads, int64_t *n_cigar, int64_t *n_seq
  * memory otherwise (waits for the copies).  Needs c3b_bam_sizes first. */
 int c3b_bam_fetch(c3b_bam *w, const c3b_bam_out *out, int on_device);
 
-/* Device time of the last c3b_bam_decode (CUDA events around its kernels, the upload excluded) and its kernel launches. */
+/* One window of a bgzip-compressed FASTA, from its compressed blocks to bases in device memory, on the same workspace: the blocks
+ * are inflated by the decode's inflater, and one thread per base gathers the window, skipping the line ends by arithmetic.
+ * bytes[0 .. n_bytes): host memory holding the whole BGZF blocks that cover the window (clair3_b200/bam_io.py: fasta_span
+ * finds them through the .gzi).  first_uoff: the uncompressed offset of the window's first base in the first block's data.
+ * start: the window's first base, 0-based on its sequence; line_bases / line_bytes: the sequence's line geometry from the .fai.
+ * Base i of the window is read at uncompressed offset
+ *     first_uoff + (start + i) / line_bases * line_bytes + (start + i) % line_bases - (start / line_bases * line_bytes + start % line_bases)
+ * and written to out[i] (device memory, n_bases bytes), case kept.  Checks the block headers as c3b_bam_decode does, and that
+ * the window's last base lies inside the inflated data; then queues the upload, the inflate and the gather on cuda_stream: no
+ * host wait.  n_bases = 0 queues nothing. */
+int c3b_fasta_fetch(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t first_uoff, int64_t start, int64_t line_bases,
+                    int64_t line_bytes, int64_t n_bases, uint8_t *out, void *cuda_stream);
+
+/* The status of the last c3b_fasta_fetch: waits for its kernels (no wait when the caller's stream has already passed them, for
+ * example after a later c3b_bam_sizes) and fails with the block's number and reason when a block did not inflate (a DEFLATE
+ * stream that does not decode, a CRC-32 or ISIZE mismatch); out's bytes are then not the window's.  0 when no fetch is
+ * pending. */
+int c3b_fasta_status(c3b_bam *w);
+
+/* Device time of the last c3b_bam_decode or c3b_fasta_fetch (CUDA events around its kernels, the upload excluded) and its
+ * kernel launches. */
 int c3b_bam_last_ms(c3b_bam *w, float *ms, int *launches);
 
 void c3b_bam_destroy(c3b_bam *w);
