@@ -7,7 +7,8 @@ BGZF block headers.  The GPU inflates the blocks, finds the record chain, parses
 ``records.DeviceBamRecords`` that ``PileupCounter.count`` and ``FullAlignmentBuilder.build`` take as they are: a region goes
 from compressed bytes to call records on the device.  ``fetch_fasta`` does the same for a window of a bgzip-compressed
 reference FASTA: the host finds the covering blocks through the ``.fai`` and ``.gzi``, the GPU inflates them and gathers the
-bases.  No CPU fallback: everything here calls ``libclair3b200.so``.
+bases.  ``write_bgzf`` runs the other direction: it compresses a text into a BGZF file on the GPU, byte for byte as
+``bam_io.write_bgzf`` writes it.  No CPU fallback: everything here calls ``libclair3b200.so``.
 """
 from __future__ import annotations
 
@@ -16,7 +17,7 @@ import os
 import torch
 
 from . import bam_io
-from ._ffi import check, ffi, lib
+from ._ffi import C3BError, check, ffi, lib
 from ._workspace import _Handle
 from .records import FIELDS, VALUES, DeviceBamRecords
 
@@ -144,3 +145,35 @@ class BamDecoder(_Handle):
         that fetch's kernels unless the stream has passed them."""
         check(self._lib().c3b_fasta_status(self._h))
 
+
+    def compress_bgzf(self, data):
+        """``data`` as BGZF blocks of 0xFF00 bytes, compressed on the GPU (``c3b_bgzf_compress``) to exactly the bytes
+        ``bam_io.write_bgzf`` writes before its end-of-file block: (the file image as bytes, the offset of every block in it
+        and then the image's length).  ``data``: bytes-like or str on the host, or a uint8 tensor on the decoder's device.  One
+        host wait, on the device's current torch stream."""
+        L = self._lib()
+        if isinstance(data, torch.Tensor):
+            if data.dtype != torch.uint8 or data.device != self._device:
+                raise C3BError("compress_bgzf: a tensor must be uint8 on the decoder's device %s" % self._device)
+            data = data.contiguous()
+            n, ptr, on_device = data.numel(), ffi.cast("const uint8_t *", data.data_ptr()), 1
+        else:
+            data = data.encode() if isinstance(data, str) else data
+            data = memoryview(data).cast("B") if not isinstance(data, (bytes, bytearray)) else data
+            n, ptr, on_device = len(data), ffi.from_buffer(data) if len(data) else ffi.NULL, 0
+        check(L.c3b_bgzf_compress(self._h, ptr, n, on_device, self._stream()))
+        nb = -(-n // bam_io._BGZF_PAYLOAD)
+        size, off = ffi.new("int64_t *"), ffi.new("int64_t[]", nb + 1)
+        check(L.c3b_bgzf_sizes(self._h, size, off))
+        image = bytearray(int(size[0]))
+        check(L.c3b_bgzf_fetch(self._h, ffi.from_buffer(image) if image else ffi.NULL, 0))
+        return bytes(image), [int(off[i]) for i in range(nb + 1)]
+
+    def write_bgzf(self, path, data):
+        """``bam_io.write_bgzf`` on the GPU: writes ``data`` (as ``compress_bgzf`` takes it) to ``path`` as a BGZF file with
+        the end-of-file block, the same bytes, and returns the same ``voffset(u)``, which ``bam_io.write_tbi`` indexes with."""
+        image, off = self.compress_bgzf(data)
+        with open(path, "wb") as f:
+            f.write(image)
+            f.write(bam_io._EOF)
+        return bam_io.bgzf_voffset(off[:-1], off[-1])

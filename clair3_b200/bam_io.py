@@ -292,7 +292,12 @@ def write_bgzf(path, data):
     with open(path, "wb") as f:
         offsets = _write_bgzf_blocks(f, data)
         end = f.tell() - len(_EOF)
+    return bgzf_voffset(offsets, end)
 
+
+def bgzf_voffset(offsets, end):
+    """``write_bgzf``'s ``voffset(u)`` for a file whose ``_BGZF_PAYLOAD``-byte blocks start at ``offsets`` and whose EOF block
+    starts at ``end``."""
     def voffset(u):
         i = u // _BGZF_PAYLOAD
         return offsets[i] << 16 | (u - i * _BGZF_PAYLOAD) if i < len(offsets) else end << 16
@@ -785,6 +790,13 @@ def write_tbi(vcf_gz_path, text, voffset, tbi_path=None):
     """Writes the tabix index (``tabix -p vcf``) of a VCF whose text ``text`` was written by ``write_bgzf`` (``voffset``: what it
     returned).  Rows starting with ``#`` are skipped; a record covers [POS - 1, POS - 1 + len(REF)); the contigs are named in
     the order the file first holds them.  The index is BGZF-compressed as tabix writes it.  Returns the path written."""
+    path = tbi_path or str(vcf_gz_path) + ".tbi"
+    write_bgzf(path, tbi_bytes(text, voffset))
+    return path
+
+
+def tbi_bytes(text, voffset):
+    """The uncompressed bytes of ``write_tbi``'s index."""
     data = text.encode() if isinstance(text, str) else bytes(text)
     names, idx, u = [], {}, 0
     for line in data.splitlines(keepends=True):
@@ -803,9 +815,7 @@ def write_tbi(vcf_gz_path, text, voffset, tbi_path=None):
     for n in names:
         out += _index_ref_bytes(idx[n])
     out += struct.pack("<Q", 0)
-    path = tbi_path or str(vcf_gz_path) + ".tbi"
-    write_bgzf(path, bytes(out))
-    return path
+    return bytes(out)
 
 
 def read_tbi(path):

@@ -30,6 +30,13 @@
 // c3b_fasta_fetch reuses the upload and B1 for the blocks of a bgzip-compressed FASTA window, then gathers the window's bases
 // with one thread each, skipping the line ends by arithmetic; c3b_fasta_status reads its bad-block word.
 //
+// The BGZF writer runs the other direction on the same workspace and upload (c3b_bgzf_compress):
+//   Z1 bgzf_deflate     one CTA per SM, striding over the 0xFF00-byte payloads: the CTA loads a payload into its shared
+//                       window, thread 0 compresses it exactly as zlib level 6 does (deflate.cuh) into the block's
+//                       64 KiB slot, warp 1 computes its CRC-32 with bam_inflate's lane split, and thread 0 frames the block.
+//   Z2 block scan       each block's offset in the file from the compressed sizes, and the file size.
+//   Z3 bgzf_pack        one CTA per block: the slots into one contiguous file image.
+//
 // The only host wait is c3b_bam_sizes, after the totals.  Every buffer is sized from what the host knows before the decode: the
 // compressed bytes and the sum of ISIZE (U): a record takes at least 36 bytes of U, so there are at most U / 36 + 1 records, and
 // every value array holds at most U entries.  Valid input never reaches a capacity; malformed input is bounds-checked at every
@@ -41,6 +48,7 @@
 
 #include "block_scan.cuh"
 #include "c3b_internal.h"
+#include "deflate.cuh"
 #include "inflate.cuh"
 #include "../../include/clair3_b200_bam.h"
 
@@ -124,13 +132,12 @@ __global__ void __launch_bounds__(32) bam_inflate_kernel(const uint8_t *__restri
     st = __shfl_sync(0xffffffffu, st, 0);
     __syncwarp();
     if (st == OK) {
-        const int n = B.isize, chunk = (n + 31) / 32, a = lane * chunk, e = a + chunk < n ? a + chunk : n;
+        const int n = B.isize;
         uint8_t *dst = U + B.uoff;
         for (int i = lane; i < n; i += 32) dst[i] = out[i];
-        uint32_t term = 0;
-        if (a < e) term = crc_shift(crc_update(crc_tab, 0, out + a, e - a), (uint32_t)(n - e));
+        uint32_t term = crc_lane_term(crc_tab, out, n, lane);
         for (int d = 16; d; d >>= 1) term ^= __shfl_xor_sync(0xffffffffu, term, d);
-        if (~(term ^ crc_shift(0xffffffffu, (uint32_t)n)) != B.crc) st = CRC_MISMATCH;
+        if (crc_lanes_done(term, n) != B.crc) st = CRC_MISMATCH;
     }
     if (lane == 0 && st != OK) atomicMin(bad, (unsigned long long)b << 4 | (unsigned)st);
 }
@@ -447,6 +454,80 @@ __global__ void fasta_gather_kernel(const uint8_t *__restrict__ U, int64_t u0, i
     out[i] = U[u0 - r + k / lb * lw + k % lb];
 }
 
+constexpr int Z_THREADS = 128;              // warp 0: the compressor (one thread), warp 1: the CRC; all four load
+constexpr int SYM_SLOT = 49152;             // a CTA's symbol buffer in global memory: deflate.cuh's SYM_END bytes, rounded up
+constexpr size_t Z_TREES_AT = c3b_deflate::WINDOW + 2 * 32768 * 2;
+constexpr size_t Z_CRC_AT = Z_TREES_AT + (sizeof(c3b_deflate::Trees) + 15) / 16 * 16;
+constexpr size_t Z_SMEM = Z_CRC_AT + 256 * 4;
+
+// Z1.  Shared memory: the 64 KiB window, head and prev (32 Ki uint16 each), the Huffman trees (8,104 B) and the CRC table:
+// 205,744 B, so one encoder per SM.  The symbol buffer, 16,383 x 3 bytes, does not fit beside them and lives in the CTA's slot of sym.
+// size[b]: the block's total bytes; 0 and a bad word (b << 4 | status) when its stream would not fit the 64 KiB block.
+__global__ void __launch_bounds__(Z_THREADS) bgzf_deflate_kernel(const uint8_t *__restrict__ src, int64_t n, int nb,
+                                                                 uint8_t *__restrict__ slots, int32_t *__restrict__ size,
+                                                                 uint8_t *__restrict__ sym, unsigned long long *bad) {
+    using namespace c3b_deflate;
+    extern __shared__ __align__(16) uint8_t smem[];
+    uint8_t *window = smem;
+    uint16_t *head = reinterpret_cast<uint16_t *>(smem + WINDOW), *prev = head + 32768;
+    Trees *trees = reinterpret_cast<Trees *>(smem + Z_TREES_AT);
+    uint32_t *crc_tab = reinterpret_cast<uint32_t *>(smem + Z_CRC_AT);
+    __shared__ uint32_t crc;
+    __shared__ int clen;
+    const int tid = threadIdx.x;
+    for (int i = tid; i < 256; i += Z_THREADS) crc_tab[i] = crc_table_entry(i);
+    for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+        const int64_t p0 = (int64_t)b * PAYLOAD;
+        const int len = (int)(n - p0 < PAYLOAD ? n - p0 : PAYLOAD);
+        const uint8_t *p = src + p0;
+        for (int i = tid; i < len; i += Z_THREADS) window[i] = p[i];
+        // fill_window's high-water zeroing past the data; head starts empty (prev is zeroed too, though zlib's is not: no
+        // entry of prev is read before it is written)
+        const int zend = len + WIN_INIT < WINDOW ? len + WIN_INIT : WINDOW;
+        for (int i = len + tid; i < zend; i += Z_THREADS) window[i] = 0;
+        uint32_t *hp = reinterpret_cast<uint32_t *>(head);
+        for (int i = tid; i < 32768; i += Z_THREADS) hp[i] = 0;
+        __syncthreads();
+        uint8_t *blk = slots + (int64_t)b * BLOCK_MAX;
+        if (tid == 0) {
+            Deflater z;
+            z.window = window;
+            z.head = head;
+            z.prev = prev;
+            z.sym = sym + (int64_t)blockIdx.x * SYM_SLOT;
+            z.t = trees;
+            z.out = blk + HEADER;
+            z.cap = BLOCK_MAX - HEADER - FOOTER;
+            clen = z.run(len);
+        } else if (tid >= 32 && tid < 64) {
+            uint32_t term = crc_lane_term(crc_tab, p, len, tid - 32);
+            for (int d = 16; d; d >>= 1) term ^= __shfl_xor_sync(0xffffffffu, term, d);
+            if (tid == 32) crc = crc_lanes_done(term, len);
+        }
+        __syncthreads();
+        if (tid == 0) {
+            if (clen < 0) {
+                size[b] = 0;
+                atomicMin(bad, (unsigned long long)b << 4 | c3b_deflate::OUTPUT_OVERFLOW);
+            } else {
+                bgzf_header(blk, clen);
+                put32(blk + HEADER + clen, crc);
+                put32(blk + HEADER + clen + 4, (uint32_t)len);
+                size[b] = HEADER + clen + FOOTER;
+            }
+        }
+    }
+}
+
+// Z3
+__global__ void __launch_bounds__(256) bgzf_pack_kernel(const uint8_t *__restrict__ slots, const int32_t *__restrict__ size,
+                                                        const int64_t *__restrict__ off, uint8_t *__restrict__ image) {
+    const int b = blockIdx.x;
+    const uint8_t *s = slots + (int64_t)b * c3b_deflate::BLOCK_MAX;
+    uint8_t *d = image + off[b];
+    for (int i = threadIdx.x; i < size[b]; i += 256) d[i] = s[i];
+}
+
 size_t inflate_smem() { return 65536 + (sizeof(Tables) + 15) / 16 * 16 + 256 * 4; }
 
 const char *status_name(int st) {
@@ -488,7 +569,17 @@ struct c3b_bam : C3bRegionWorkspace {
     cudaEvent_t fetched = nullptr;
     std::vector<int64_t> fasta_block_start;
     bool fasta_pending = false, timed = false;
+    // the last BGZF write: its slots, sizes, symbol buffers and file image; on the device its bad word, file size and block
+    // offsets, and their pinned copy; the event after that copy
+    C3bBuf z_slots, z_size, z_sym, z_image, z_meta;
+    int64_t *z_host = nullptr;
+    size_t z_host_cap = 0;
+    cudaEvent_t compressed = nullptr;
+    int64_t z_blocks = 0, z_bytes = 0;
+    bool z_pending = false, z_sized = false;
     ~c3b_bam() {
+        if (z_host) cudaFreeHost(z_host);
+        if (compressed) cudaEventDestroy(compressed);
         if (staging) cudaFreeHost(staging);
         if (uploaded) cudaEventDestroy(uploaded);
         if (fasta_bad_host) cudaFreeHost(fasta_bad_host);
@@ -544,10 +635,8 @@ static int bam_blocks(const uint8_t *p, int64_t n, std::vector<Block> &out, std:
     return 0;
 }
 
-// Copies the block table (w->blocks) and bytes[0 .. n_bytes) into the pinned staging buffer, after the previous upload has left
-// it.  bam_upload then queues the staged bytes into w->in.
-static int bam_stage(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, const char *who) {
-    const size_t table = w->blocks.size() * sizeof(Block), up = table + (size_t)n_bytes;
+// Waits until the previous upload has left the pinned staging buffer, and grows it to hold up bytes.
+static int bam_staging(c3b_bam *w, size_t up, const char *who) {
     C3B_CUDA(cudaEventSynchronize(w->uploaded));
     if (up > w->staging_cap) {
         if (w->staging) cudaFreeHost(w->staging);
@@ -557,6 +646,14 @@ static int bam_stage(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, const ch
         if (cudaMallocHost((void **)&w->staging, want) != cudaSuccess) { c3b_set_error("%s: pinned allocation of %zu bytes failed", who, want); return 1; }
         w->staging_cap = want;
     }
+    return 0;
+}
+
+// Copies the block table (w->blocks) and bytes[0 .. n_bytes) into the pinned staging buffer.  bam_upload then queues the
+// staged bytes into w->in.
+static int bam_stage(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, const char *who) {
+    const size_t table = w->blocks.size() * sizeof(Block), up = table + (size_t)n_bytes;
+    if (bam_staging(w, up, who)) return 1;
     if (table) memcpy(w->staging, w->blocks.data(), table);
     if (n_bytes) memcpy(w->staging + table, bytes, (size_t)n_bytes);
     return 0;
@@ -577,9 +674,11 @@ int c3b_bam_create(c3b_bam **out, int device_ordinal) {
     c3b_bam *w = *out;
     if (cudaEventCreateWithFlags(&w->uploaded, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&w->fetched, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&w->compressed, cudaEventDisableTiming) != cudaSuccess ||
         cudaMallocHost((void **)&w->fasta_bad_host, 8) != cudaSuccess || w->fasta_bad.ensure(8, nullptr, "c3b_bam_create") ||
-        cudaFuncSetAttribute(bam_inflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)inflate_smem()) != cudaSuccess) {
-        c3b_set_error("c3b_bam_create: event creation, a small allocation or the inflate kernel's shared-memory setting failed");
+        cudaFuncSetAttribute(bam_inflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)inflate_smem()) != cudaSuccess ||
+        cudaFuncSetAttribute(bgzf_deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Z_SMEM) != cudaSuccess) {
+        c3b_set_error("c3b_bam_create: event creation, a small allocation or a kernel's shared-memory setting failed");
         c3b_bam_destroy(w);
         *out = nullptr;
         return 1;
@@ -822,8 +921,92 @@ int c3b_bam_fetch(c3b_bam *w, const c3b_bam_out *out, int on_device) {
     return on_device ? 0 : w->wait();
 }
 
+int c3b_bgzf_compress(c3b_bam *w, const uint8_t *src, int64_t n, int on_device, void *cuda_stream) {
+    const char *who = "c3b_bgzf_compress";
+    if (!w || (n > 0 && !src) || n < 0) { c3b_set_error("%s: null or negative argument", who); return 1; }
+    w->z_pending = w->z_sized = false;
+    C3B_CUDA(cudaSetDevice(w->device));
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    w->stream = s;
+    const int64_t nb = (n + c3b_deflate::PAYLOAD - 1) / c3b_deflate::PAYLOAD;
+    if (nb > INT_MAX) { c3b_set_error("%s: %lld bytes are more BGZF blocks than one call takes", who, (long long)n); return 1; }
+    int sms = 0;
+    C3B_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, w->device));
+    const int grid = (int)(nb < sms ? nb : sms);
+    const size_t meta = (size_t)(nb + 2) * 8, slots = (size_t)nb * c3b_deflate::BLOCK_MAX;
+    if (w->z_slots.ensure(slots ? slots : 1, s, "c3b_bam") || w->z_image.ensure(slots ? slots : 1, s, "c3b_bam") ||
+        w->z_size.ensure((size_t)(nb ? nb : 1) * 4, s, "c3b_bam") || w->z_sym.ensure((size_t)(grid ? grid : 1) * SYM_SLOT, s, "c3b_bam") ||
+        w->z_meta.ensure(meta, s, "c3b_bam"))
+        return 1;
+    if (meta > w->z_host_cap) {
+        C3B_CUDA(cudaEventSynchronize(w->compressed));
+        if (w->z_host) cudaFreeHost(w->z_host);
+        w->z_host = nullptr;
+        w->z_host_cap = 0;
+        if (cudaMallocHost((void **)&w->z_host, meta) != cudaSuccess) { c3b_set_error("%s: pinned allocation of %zu bytes failed", who, meta); return 1; }
+        w->z_host_cap = meta;
+    }
+    const uint8_t *d_src = src;
+    if (!on_device && n > 0) {
+        if (bam_staging(w, (size_t)n, who) || w->in.ensure((size_t)n, s, "c3b_bam")) return 1;
+        memcpy(w->staging, src, (size_t)n);
+        if (bam_upload(w, (size_t)n, s)) return 1;
+        d_src = w->in.as<uint8_t>();
+    }
+    int64_t *m = w->z_meta.as<int64_t>();
+    C3B_CUDA(cudaMemsetAsync(m, 0xff, 8, s));
+    C3B_CUDA(cudaMemsetAsync(m + 1, 0, 8, s));
+    C3B_CUDA(cudaEventRecord(w->ev[0][0], s));
+    w->launches[0] = 0;
+    if (nb > 0) {
+        bgzf_deflate_kernel<<<grid, Z_THREADS, Z_SMEM, s>>>(d_src, n, (int)nb, w->z_slots.as<uint8_t>(), w->z_size.as<int32_t>(),
+                                                           w->z_sym.as<uint8_t>(), reinterpret_cast<unsigned long long *>(m));
+        block_scan_sum(w->z_size.as<int32_t>(), m + 2, nb, nullptr, m + 1, s);
+        bgzf_pack_kernel<<<(unsigned)nb, 256, 0, s>>>(w->z_slots.as<uint8_t>(), w->z_size.as<int32_t>(), m + 2, w->z_image.as<uint8_t>());
+        w->launches[0] = 3;
+    }
+    C3B_CUDA(cudaEventRecord(w->ev[0][1], s));
+    C3B_CUDA(cudaGetLastError());
+    C3B_CUDA(cudaMemcpyAsync(w->z_host, m, meta, cudaMemcpyDeviceToHost, s));
+    C3B_CUDA(cudaEventRecord(w->compressed, s));
+    w->z_blocks = nb;
+    w->z_pending = w->timed = true;
+    return 0;
+}
+
+int c3b_bgzf_sizes(c3b_bam *w, int64_t *n_out, int64_t *block_off) {
+    const char *who = "c3b_bgzf_sizes";
+    if (!w || !w->z_pending) { c3b_set_error("%s: no c3b_bgzf_compress has been issued", who); return 1; }
+    C3B_CUDA(cudaSetDevice(w->device));
+    C3B_CUDA(cudaEventSynchronize(w->compressed));
+    const int64_t *h = w->z_host;
+    const unsigned long long bad = (unsigned long long)h[0];
+    if (bad != ~0ull) {
+        c3b_set_error("%s: BGZF block %llu's DEFLATE stream does not fit a 64 KiB block", who, bad >> 4);
+        return 1;
+    }
+    w->z_bytes = h[1];
+    w->z_sized = true;
+    if (n_out) *n_out = w->z_bytes;
+    if (block_off) {
+        if (w->z_blocks) memcpy(block_off, h + 2, (size_t)w->z_blocks * 8);
+        block_off[w->z_blocks] = w->z_bytes;
+    }
+    return 0;
+}
+
+int c3b_bgzf_fetch(c3b_bam *w, uint8_t *out, int on_device) {
+    const char *who = "c3b_bgzf_fetch";
+    if (!w || (!out && w->z_bytes)) { c3b_set_error("%s: null argument", who); return 1; }
+    if (!w->z_sized) { c3b_set_error("%s: call c3b_bgzf_sizes after c3b_bgzf_compress first", who); return 1; }
+    C3B_CUDA(cudaSetDevice(w->device));
+    if (w->z_bytes)
+        C3B_CUDA(cudaMemcpyAsync(out, w->z_image.p, (size_t)w->z_bytes, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, w->stream));
+    return on_device ? 0 : w->wait();
+}
+
 int c3b_bam_last_ms(c3b_bam *w, float *ms, int *launches) {
-    if (!w || !w->timed) { c3b_set_error("c3b_bam_last_ms: no c3b_bam_decode or c3b_fasta_fetch has been issued"); return 1; }
+    if (!w || !w->timed) { c3b_set_error("c3b_bam_last_ms: no c3b_bam_decode, c3b_fasta_fetch or c3b_bgzf_compress has been issued"); return 1; }
     return w->elapsed(0, ms, launches);
 }
 

@@ -283,4 +283,12 @@ C3B_HD uint32_t crc_update(const uint32_t *table, uint32_t s, const uint8_t *p, 
     return s;
 }
 
+// The lane split of a warp's CRC-32 over p[0 .. n): lane l of 32 takes the chunk [l * c, min((l + 1) * c, n)), c = ceil(n / 32),
+// and returns R(0, chunk) shifted past the bytes after it.  The CRC is crc_lanes_done(the XOR of the 32 terms, n).
+C3B_HD uint32_t crc_lane_term(const uint32_t *table, const uint8_t *p, int n, int lane) {
+    const int chunk = (n + 31) / 32, a = lane * chunk, e = a + chunk < n ? a + chunk : n;
+    return a < e ? crc_shift(crc_update(table, 0, p + a, e - a), (uint32_t)(n - e)) : 0;
+}
+C3B_HD uint32_t crc_lanes_done(uint32_t x, int n) { return ~(x ^ crc_shift(0xffffffffu, (uint32_t)n)); }
+
 }  // namespace c3b_inflate

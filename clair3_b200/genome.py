@@ -212,10 +212,19 @@ def has_records(text):
     return _records(text) > 0
 
 
-def write_vcf_gz(path, text):
-    """``bgzip -f`` and ``tabix -p vcf``: ``path`` (ending in ``.vcf.gz``) and ``path.tbi``."""
-    voff = bam_io.write_bgzf(path, text)
-    bam_io.write_tbi(path, text, voff)
+def write_vcf_gz(path, text, decoder=None, stages=None):
+    """``bgzip -f`` and ``tabix -p vcf``: ``path`` (ending in ``.vcf.gz``) and ``path.tbi``.  With ``decoder`` (a
+    ``BamDecoder``) both files are compressed on its GPU (``BamDecoder.write_bgzf``), otherwise on the host
+    (``bam_io.write_bgzf``); the bytes are the same.  ``stages``: a ``cascade.Stages`` that marks the compression and the
+    file writes ("compress") apart from building the index ("write")."""
+    write = decoder.write_bgzf if decoder is not None else bam_io.write_bgzf
+    mark = stages.mark if stages is not None else (lambda name: None)
+    voff = write(path, text)
+    mark("compress")
+    index = bam_io.tbi_bytes(text, voff)
+    mark("write")
+    write(str(path) + ".tbi", index)
+    mark("compress")
     return path
 
 
@@ -401,7 +410,7 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
                            qual, print_ref_calls, pileup_only, tgt if genotyping else None)
         st.mark("merge and format")
         out.update(qual_cutoffs=cuts, beds=len(beds))
-        _write(out_dir, texts, out)
+        _write(out_dir, texts, out, ws.decoder, st)
         st.mark("write")
         out["stages"] = st.summed()
         return out
@@ -510,11 +519,12 @@ def _merge_contig(p_chunks, f_beds, ctg, qual, print_ref):
     return cascade.merge_rows(p_pos, [p[x] for x in p_pos], f_pos, f_rows, qual=qual, print_ref=print_ref)
 
 
-def _write(out_dir, texts, out):
-    """Writes each of ``texts`` as ``<name>.vcf.gz`` with its ``.tbi`` into ``out_dir``, and adds ``files``, ``texts`` and
-    ``rows`` (the row count per file) to the result ``out``."""
+def _write(out_dir, texts, out, decoder=None, stages=None):
+    """Writes each of ``texts`` as ``<name>.vcf.gz`` with its ``.tbi`` into ``out_dir`` (``write_vcf_gz`` with ``decoder`` and
+    ``stages``), and adds ``files``, ``texts`` and ``rows`` (the row count per file) to the result ``out``."""
     out_dir = str(out_dir)
     os.makedirs(out_dir, exist_ok=True)
-    out.update(files={n: write_vcf_gz(os.path.join(out_dir, n + ".vcf.gz"), t) for n, t in texts.items()}, texts=texts,
+    out.update(files={n: write_vcf_gz(os.path.join(out_dir, n + ".vcf.gz"), t, decoder, stages) for n, t in texts.items()},
+               texts=texts,
                rows={n: _records(t) for n, t in texts.items()})
     return out

@@ -90,8 +90,26 @@ int c3b_fasta_fetch(c3b_bam *w, const uint8_t *bytes, int64_t n_bytes, int64_t f
  * pending. */
 int c3b_fasta_status(c3b_bam *w);
 
-/* Device time of the last c3b_bam_decode or c3b_fasta_fetch (CUDA events around its kernels, the upload excluded) and its
- * kernel launches. */
+/* The BGZF writer, on the same workspace: src[0 .. n) (host memory, or device memory with on_device = 1) is cut into blocks
+ * of 0xFF00 bytes, as bgzip and htslib cut them, and each block is compressed on the GPU, one per CTA, to exactly the bytes
+ * zlib 1.3 writes at level 6 with a raw window of 15 bits (zlib.compressobj(6, zlib.DEFLATED, -15)), framed as
+ * clair3_b200/bam_io.py's BGZF writer frames it (gzip header with the BC subfield, CRC-32 and ISIZE footer).  The blocks are
+ * then packed into one file image; the end-of-file block is not part of it.  A host src is copied through the reader's pinned
+ * staging before the call returns; a device src must stay valid until the stream has passed the compression.  Queues the work
+ * on cuda_stream: no host wait. */
+int c3b_bgzf_compress(c3b_bam *w, const uint8_t *src, int64_t n, int on_device, void *cuda_stream);
+
+/* The one wait of a BGZF write: the file image's bytes (*n_out) and, when block_off is not NULL, the offset of every block in
+ * it, block_off[0 .. ceil(n / 0xFF00)], the last entry being *n_out.  Fails, naming the block, if a block's stream would not fit
+ * the 64 KiB a BGZF block may take (zlib's own bound keeps every 0xFF00-byte payload well inside it). */
+int c3b_bgzf_sizes(c3b_bam *w, int64_t *n_out, int64_t *block_off);
+
+/* Copies the file image of the last c3b_bgzf_compress into out (*n_out bytes): device memory with on_device = 1 (queued on the
+ * compression's stream, no wait), host memory otherwise (waits for the copy).  Needs c3b_bgzf_sizes first. */
+int c3b_bgzf_fetch(c3b_bam *w, uint8_t *out, int on_device);
+
+/* Device time of the last c3b_bam_decode, c3b_fasta_fetch or c3b_bgzf_compress (CUDA events around its kernels, the upload
+ * excluded) and its kernel launches. */
 int c3b_bam_last_ms(c3b_bam *w, float *ms, int *launches);
 
 void c3b_bam_destroy(c3b_bam *w);
