@@ -480,13 +480,7 @@ __global__ void __launch_bounds__(Z_THREADS) bgzf_deflate_kernel(const uint8_t *
         const int64_t p0 = (int64_t)b * PAYLOAD;
         const int len = (int)(n - p0 < PAYLOAD ? n - p0 : PAYLOAD);
         const uint8_t *p = src + p0;
-        for (int i = tid; i < len; i += Z_THREADS) window[i] = p[i];
-        // fill_window's high-water zeroing past the data; head starts empty (prev is zeroed too, though zlib's is not: no
-        // entry of prev is read before it is written)
-        const int zend = len + WIN_INIT < WINDOW ? len + WIN_INIT : WINDOW;
-        for (int i = len + tid; i < zend; i += Z_THREADS) window[i] = 0;
-        uint32_t *hp = reinterpret_cast<uint32_t *>(head);
-        for (int i = tid; i < 32768; i += Z_THREADS) hp[i] = 0;
+        reset_block(window, head, prev, p, len, tid, Z_THREADS);
         __syncthreads();
         uint8_t *blk = slots + (int64_t)b * BLOCK_MAX;
         if (tid == 0) {

@@ -122,6 +122,19 @@ C3B_HD void static_trees(Trees &t) {
     }
 }
 
+// What comes before Deflater::run(len) on a compressor's window, head and prev, which may hold whatever an earlier block left
+// there: the payload into window[0 .. len), fill_window's high-water zeroing of the 258 bytes past it (as far as the window
+// goes), and head emptied.  prev is zeroed too, though zlib's is not: no entry of prev is read before it is written.  Thread
+// tid of nthreads does its share (the kernel's CTA: tid of Z_THREADS, then a barrier; the host build: 0 of 1).  head and prev
+// are zeroed a 32-bit word at a time, so both must be 4-byte aligned.
+C3B_HD void reset_block(uint8_t *window, uint16_t *head, uint16_t *prev, const uint8_t *src, int len, int tid, int nthreads) {
+    for (int i = tid; i < len; i += nthreads) window[i] = src[i];
+    const int zend = len + WIN_INIT < WINDOW ? len + WIN_INIT : WINDOW;
+    for (int i = len + tid; i < zend; i += nthreads) window[i] = 0;
+    uint32_t *h = reinterpret_cast<uint32_t *>(head), *p = reinterpret_cast<uint32_t *>(prev);
+    for (int i = tid; i < W_SIZE / 2; i += nthreads) h[i] = 0, p[i] = 0;      // head: 2^15 entries (hash_bits 15), prev: W_SIZE
+}
+
 // The compressor of one block.  window: WINDOW bytes, head / prev: 32 Ki entries each, sym: SYM_END bytes; out: cap bytes.
 struct Deflater {
     uint8_t *window;
@@ -474,8 +487,7 @@ struct Deflater {
         return (unsigned)best_len <= lookahead ? (unsigned)best_len : lookahead;
     }
 
-    // The stream of window[0 .. n): the caller has put the payload there, zeroed window[n .. n + 258) (as far as the window goes:
-    // fill_window's high-water zeroing) and head.  Returns the bytes written to out, or -1 past cap.
+    // The stream of window[0 .. n), after reset_block.  Returns the bytes written to out, or -1 past cap.
     C3B_HD int run(int n) {
         L = Tree{t->l.freq, t->l.dad, t->l.len, t->l.code, L_CODES, END_BLOCK + 1, MAX_BITS, 0, 0, t->s_llen};
         D = Tree{t->d.freq, t->d.dad, t->d.len, t->d.code, D_CODES, 0, MAX_BITS, 0, 1, t->s_dlen};

@@ -573,8 +573,8 @@ def build_host_inflater(out_dir):
 
 
 def run_host(exe, mode, payload):
-    """The driver's stdout; fails on a non-zero exit or any sanitizer report."""
-    r = subprocess.run([exe, mode], input=payload, capture_output=True, env=_SAN_ENV, timeout=600)
+    """The driver's stdout; fails on a non-zero exit or any sanitizer report.  ``mode``: its arguments, split on spaces."""
+    r = subprocess.run([exe] + mode.split(), input=payload, capture_output=True, env=_SAN_ENV, timeout=600)
     err = r.stderr.decode(errors="replace")
     assert r.returncode == 0 and "Sanitizer" not in err and "runtime error" not in err, err[-4000:]
     return r.stdout

@@ -6,6 +6,7 @@ import os
 import struct
 import sys
 import zlib
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import pytest
@@ -34,8 +35,8 @@ def _cases(payloads):
     return b"".join(struct.pack("<I", len(p)) + p for p in payloads)
 
 
-def run_blocks(exe, payloads):
-    out = dc.run_host(exe, "bgzf", _cases(payloads))
+def run_blocks(exe, payloads, mode="bgzf"):
+    out = dc.run_host(exe, mode, _cases(payloads))
     res, o = [], 0
     for _ in payloads:
         n, = struct.unpack_from("<i", out, o)
@@ -44,6 +45,12 @@ def run_blocks(exe, payloads):
         o += max(n, 0)
     assert o == len(out)
     return res
+
+
+def run_parallel(exe, jobs, mode="bgzf"):
+    """run_blocks over each payload list of ``jobs``, one driver process per list, as many at once as there are CPUs."""
+    with ThreadPoolExecutor(max_workers=max(1, min(len(jobs), os.cpu_count() or 1))) as ex:
+        return list(ex.map(lambda ps: run_blocks(exe, ps, mode), jobs))
 
 
 def test_corpus_has_its_features(driver):
@@ -63,9 +70,42 @@ def test_corpus_has_its_features(driver):
 def test_blocks_equal_zlibs(driver):
     """The named cases and 3,000 seeded mixtures, block for block."""
     cases = bc.payloads(1, mixtures=3000)
-    got = run_blocks(driver, [p for _, p in cases])
+    ps = [p for _, p in cases]
+    got = [g for gs in run_parallel(driver, [ps[i:i + 400] for i in range(0, len(ps), 400)]) for g in gs]
     for (name, p), g in zip(cases, got):
         assert g == bam_io._bgzf_block(p), (name, len(p))
+
+
+def _cta_jobs(cases, k, seed):
+    """The payload sequences the ``cta k`` runs take: the cases in three seeded orders, then every case on a state that has
+    just compressed a full-size random block and one that has just compressed a full-size run block (per group of k cases:
+    k random blocks, the k cases, k run blocks, the k cases again, so case j of the group lands on state j after each).  The
+    second part is cut into several runs (every run starts on fresh, poisoned states) so that they can go in parallel."""
+    rng = np.random.default_rng(seed)
+    rnd = rng.integers(0, 256, bc.PAYLOAD, dtype=np.uint8).tobytes()
+    run = b"".join(bytes([65 + i]) * (bc.PAYLOAD // 4) for i in range(4))
+    jobs = [[cases[i] for i in rng.permutation(len(cases))] for _ in range(3)]
+    after = []
+    for g in range(0, len(cases), k):
+        grp = cases[g:g + k]
+        after += [rnd] * len(grp) + grp + [run] * len(grp) + grp
+    step = -(-len(after) // (4 * 4 * k)) * 4 * k       # whole groups per run
+    return jobs + [after[i:i + step] for i in range(0, len(after), step)], (rnd, run)
+
+
+@pytest.mark.parametrize("k", [1, 3])
+def test_blocks_equal_zlibs_on_reused_state(driver, k):
+    """The kernel's CTA c compresses blocks c, c + grid, ... on one state: its window, head, prev, trees and symbol buffer keep
+    whatever the block before left there, and only reset_block runs between.  ``cta k`` holds k such states, every byte
+    poisoned first, and sends payload i to state i % k: each block must still be exactly zlib's.  The named cases and 1,500
+    mixtures in three orders, and each of them right after a full-size random block and a full-size run block."""
+    cases = [p for _, p in bc.payloads(5, mixtures=1500)]
+    jobs, full = _cta_jobs(cases, k, 17 + k)
+    want = {p: bam_io._bgzf_block(p) for p in cases + list(full)}
+    got = run_parallel(driver, jobs, "cta %d" % k)
+    for ps, gs in zip(jobs, got):
+        for i, (p, g) in enumerate(zip(ps, gs)):
+            assert g == want[p], (k, i, len(p))
 
 
 def test_vcf_texts_equal_the_host_writer(driver, tmp_path):
