@@ -83,12 +83,32 @@ int c3b_use_device(int ordinal, int unsupported, int *sm_count) {
     return 0;
 }
 
-int c3b_last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s, int64_t *last) {
-    *last = 0;
-    if (!off) return 0;
-    if (!on_device) { *last = off[n]; return 0; }
-    C3B_CUDA(cudaMemcpyAsync(last, off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+// One thread per offset entry i in [0, n]: the smallest fault key of the run, min-reduced over each warp and then into *key.
+__global__ void records_check_kernel(const C3bRecordsView v, unsigned long long *key) {
+    unsigned long long k = C3B_REC_OK;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= v.n; i += (int64_t)gridDim.x * blockDim.x) {
+        const unsigned long long f = c3b_records_fault_at(v, i);
+        k = f < k ? f : k;
+    }
+    for (int d = 16; d; d >>= 1) {
+        const unsigned long long o = __shfl_down_sync(0xffffffffu, k, d);
+        k = o < k ? o : k;
+    }
+    if ((threadIdx.x & 31) == 0 && k != C3B_REC_OK) atomicMin(key, k);
+}
+
+int c3b_records_check_device(const C3bRecordsView &v, C3bBuf &scratch, cudaStream_t s, uint64_t *key) {
+    *key = C3B_REC_OK;
+    if (v.n == 0 && !v.off[2] && !v.off[3] && !v.off[4]) return 0;      // BamRecords checks no core field of an empty run
+    if (scratch.ensure(8, s, "record check")) return 1;
+    const int64_t blocks = (v.n + 1 + 255) / 256 < 132 * 8 ? (v.n + 1 + 255) / 256 : 132 * 8;
+    unsigned long long h = C3B_REC_OK;
+    C3B_CUDA(cudaMemsetAsync(scratch.p, 0xff, 8, s));
+    records_check_kernel<<<(unsigned)blocks, 256, 0, s>>>(v, scratch.as<unsigned long long>());
+    C3B_CUDA(cudaGetLastError());
+    C3B_CUDA(cudaMemcpyAsync(&h, scratch.p, 8, cudaMemcpyDeviceToHost, s));
     C3B_CUDA(cudaStreamSynchronize(s));
+    *key = h;
     return 0;
 }
 

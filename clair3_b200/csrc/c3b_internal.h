@@ -12,6 +12,7 @@
 #include "../../include/clair3_b200_debug.h"
 #include "../../include/clair3_b200_fa.h"
 #include "../../include/clair3_b200_pileup.h"
+#include "records_check.cuh"
 
 #define C3B_T 33            // positions per site (shared/param_p.py:34-35)
 #define C3B_H1 128          // LSTM1 hidden (clair3/model.py:46)
@@ -150,8 +151,9 @@ __device__ __forceinline__ int c3b_nib_at(const uint8_t *sq, int lq, long long i
 }
 #endif
 
-// Entry n of an offset array of n + 1 entries that lives on the host or (on_device) the device; 0 for a null array.
-int c3b_last_offset(const int64_t *off, int64_t n, int on_device, cudaStream_t s, int64_t *last);
+// The fault key (records_check.cuh) of records on the device: runs records_check_kernel on stream s into the 8 bytes of
+// `scratch` and waits for it.  Launches nothing for a run with nothing to check.
+int c3b_records_check_device(const C3bRecordsView &v, C3bBuf &scratch, cudaStream_t s, uint64_t *key);
 
 // Makes device `ordinal` current after checking that it exists and is an sm_90 part.  Returns 0; `unsupported` when there
 // is no CUDA device or it is not sm_90; 1 for a bad ordinal or a failed runtime call.  sm_count (optional): its SM count.
@@ -206,7 +208,7 @@ struct C3bRegionWorkspace {
     C3bReads R{};
     const char *dref = nullptr;
     int64_t ref_start = 0, ref_len = 0, n_cigar = 0, n_seq = 0;
-    C3bBuf in_core[8], in_qoff, in_qual, in_noff, in_name, in_moff, in_mv, in_ref;
+    C3bBuf in_core[8], in_qoff, in_qual, in_noff, in_name, in_moff, in_mv, in_ref, in_check;
     // the text stage's scratch and outputs
     C3bBuf tx_hash, tx_order, tx_table, tx_nins, tx_ndel, tx_len_text, tx_len_dec;
     C3bBuf tx_text, tx_dec, tx_text_off, tx_dec_off, tx_ref_base, tx_position;
@@ -250,10 +252,10 @@ struct C3bRegionWorkspace {
     }
 
     // The records and the reference of a count / build on `stream`: checks the records (n_reads below max_reads, no null array
-    // when there are reads, an optional field's values with its offsets) and the reference, reads the closing offsets (with
-    // device records a host wait each), copies host arrays to the device in field order, the reference last, and fills R, dref,
-    // ref_start, ref_len, n_cigar and n_seq.  opt: the optional fields, null for none; mv only with want_mv.  `who` names the
-    // entry point in the errors.
+    // when there are reads, then everything records_check.cuh checks: on the host for host records, for device records in one
+    // kernel whose verdict the call waits for) and the reference, copies host arrays to the device in field order, the
+    // reference last, and fills R, dref, ref_start, ref_len, n_cigar and n_seq.  Nothing is copied or launched after a failed
+    // check.  opt: the optional fields, null for none; mv only with want_mv.  `who` names the entry point in the errors.
     int intake(const char *who, const c3b_bam_records *core, const c3b_fa_records *opt, bool want_mv, int64_t max_reads,
                int on_device, const char *ref_seq, int64_t ref_start, int64_t ref_len) {
         const int64_t n = core->n_reads;
@@ -263,21 +265,23 @@ struct C3bRegionWorkspace {
             c3b_set_error("%s: null record array", who);
             return 1;
         }
-        if (opt && ((opt->qual_off && !opt->qual) || (opt->qname_off && !opt->qname) || (opt->mv_off && !opt->mv))) {
-            c3b_set_error("%s: an optional record field has offsets but no values", who);
+        if (ref_len > 0 && !ref_seq) { c3b_set_error("%s: null ref_seq", who); return 1; }
+        uint64_t fault = C3B_REC_OK;
+        if (!on_device) fault = c3b_records_check(core, opt);
+        else if (c3b_records_check_device(c3b_records_view(core, opt), in_check, stream, &fault)) return 1;
+        if (on_device && c3b_records_pairs(opt) < fault) fault = c3b_records_pairs(opt);
+        if (fault != C3B_REC_OK) {
+            c3b_set_error("%s: records: read %lld: %s", who, (long long)c3b_records_fault_read(fault), c3b_records_fault_text(fault));
             return 1;
         }
-        if (ref_len > 0 && !ref_seq) { c3b_set_error("%s: null ref_seq", who); return 1; }
         C3bReads r{};
         r.n = n;
         int64_t nc = 0, ns = 0;
         if (n > 0) {
-            int64_t nq = 0, nn = 0, nm = 0;
-            auto last = [&](const int64_t *off, int64_t *v) { return c3b_last_offset(off, n, on_device, stream, v); };
-            if (last(core->cigar_off, &nc) || last(core->seq_off, &ns) ||
-                (opt && (last(opt->qual_off, &nq) || last(opt->qname_off, &nn) || last(opt->mv_off, &nm))))
-                return 1;
-            if (nc < 0 || ns < 0 || nq < 0 || nn < 0 || nm < 0) { c3b_set_error("%s: negative closing offset", who); return 1; }
+            // the check has held each closing offset to its count
+            nc = core->n_cigar;
+            ns = core->n_seq;
+            const int64_t nq = opt ? opt->n_qual : 0, nn = opt ? opt->n_qname : 0, nm = opt ? opt->n_mv : 0;
             const size_t n0 = (size_t)n, n1 = (n0 + 1) * 8;
             auto up = [&](C3bBuf &b, const auto *src, size_t bytes, auto &dev) {
                 return c3b_upload(b, src, bytes, on_device, dev, stream, who);

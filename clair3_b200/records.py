@@ -57,6 +57,12 @@ CORE = tuple(f for f in FIELDS if not f.optional)
 OPTIONAL = tuple(f for f in FIELDS if f.optional and f.length == VALUES)     # each goes with its offsets, name + "_off"
 
 
+def _decreases(a):
+    """Whether a step of ``a`` goes down.  Compared, not differenced: ``np.diff`` wraps at 2^63, so an offset near -2^63 between
+    two small ones would pass as two steps up."""
+    return bool((a[1:] < a[:-1]).any())
+
+
 class BamRecords:
     """A coordinate-sorted run of alignment records of one contig in htslib's in-memory layout (``c3b_bam_records``):
     pos / flag / mapq / l_qseq per read, CIGAR words ``len << 4 | op`` and 4-bit packed sequences addressed through
@@ -76,9 +82,9 @@ class BamRecords:
         if n:
             if self.cigar_off[0] != 0 or self.seq_off[0] != 0 or self.cigar_off[-1] != len(self.cigar) or self.seq_off[-1] != len(self.seq):
                 raise C3BError("BamRecords: offsets do not span cigar / seq")
-            if (np.diff(self.cigar_off) < 0).any() or (np.diff(self.seq_off) < 0).any():
+            if _decreases(self.cigar_off) or _decreases(self.seq_off):
                 raise C3BError("BamRecords: offsets must not decrease")
-            if (np.diff(self.pos) < 0).any():
+            if _decreases(self.pos):
                 raise C3BError("BamRecords: records must be sorted by pos (a coordinate-sorted BAM)")
             if ((self.l_qseq.astype(np.int64) + 1) // 2 > np.diff(self.seq_off)).any():
                 raise C3BError("BamRecords: a packed sequence is shorter than (l_qseq + 1) / 2 bytes")
@@ -92,7 +98,7 @@ class BamRecords:
             if v is not None:
                 v = np.frombuffer(v, dtype=np.uint8).copy() if isinstance(v, (bytes, bytearray)) else v
                 v, o = np.ascontiguousarray(v, dtype=f.dtype), np.ascontiguousarray(o, dtype=np.int64)
-                if len(o) != n + 1 or o[0] != 0 or o[-1] != len(v) or (np.diff(o) < 0).any():
+                if len(o) != n + 1 or o[0] != 0 or o[-1] != len(v) or _decreases(o):
                     raise C3BError("BamRecords: %s_off must be n_reads + 1 non-decreasing offsets from 0 to len(%s)" % (k, k))
                 if k == "qual" and (np.diff(o) != self.l_qseq).any():
                     raise C3BError("BamRecords: every read needs l_qseq base qualities")
@@ -135,9 +141,11 @@ class DeviceBamRecords:
         """Records from device tensors, taken over without a copy: ``tensors`` maps every core field of ``FIELDS`` to a
         contiguous integer tensor on ``device`` of that field's width (2 bytes for ``flag``, 4 for ``cigar``: torch's signed
         views serve), and each optional field and its ``_off`` to tensors or None.  Checked here, from the tensors' metadata
-        alone: device, contiguity, width, ``n_reads`` entries per read and ``n_reads + 1`` offsets.  Not checked, because that
-        would read device memory: that each value array holds what its last offset says, and the rest of what ``BamRecords``
-        checks on the host."""
+        alone: device, contiguity, width, ``n_reads`` entries per read, ``n_reads + 1`` offsets, and each optional field with
+        its offsets.  The values are checked by every call that takes the records, before any kernel indexes through an
+        offset: one kernel (``clair3_b200/csrc/records_check.cuh``) holds the offsets, ``pos`` and ``l_qseq`` to everything
+        ``BamRecords`` checks on the host, each last offset to its value array's length (``records_struct`` passes the
+        lengths), and the call raises ``C3BError`` naming the field and the first read that breaks it."""
         self = cls.__new__(cls)
         self.device = torch.device(device)
         self.n_reads = n = int(tensors["pos"].numel())
@@ -177,8 +185,8 @@ def _device_ref(ref_seq, device):
 
 def records_struct(rec, optional=False):
     """The ``c3b_bam_records`` of a ``BamRecords`` or a ``DeviceBamRecords`` (``optional=True``: the ``c3b_fa_records`` around it,
-    with qual / qname / mv where the records carry them, null where they do not).  The struct holds raw addresses: the records
-    must outlive the call that reads it."""
+    with qual / qname / mv where the records carry them, null where they do not), with the length of each value array.  The
+    struct holds raw addresses: the records must outlive the call that reads it."""
     on_dev = isinstance(rec, DeviceBamRecords)
     arrays = rec.t if on_dev else vars(rec)
     addr = (lambda a: a.data_ptr()) if on_dev else (lambda a: a.ctypes.data)
@@ -190,6 +198,8 @@ def records_struct(rec, optional=False):
         if a is not None:
             p = 8 if f.optional and f.length == VALUES and not len(a) else addr(a)    # an empty value array: non-null, never read
             setattr(s if f.optional else core, f.name, ffi.cast("const %s *" % f.ctype, p))
+            if f.length == VALUES:
+                setattr(s if f.optional else core, "n_" + f.name, len(a))
     return s
 
 

@@ -30,7 +30,9 @@ extern "C" {
 typedef struct c3b_fa c3b_fa;
 
 /* The pileup record layout (c3b_bam_records, coordinate-sorted, one contig) plus the fields the full-alignment tensor reads.
- * Each pair is an [n+1] offset array and the concatenated values; a NULL offset array means the field is absent for every read. */
+ * Each pair is an [n+1] offset array and the concatenated values; a NULL offset array means the field is absent for every read,
+ * and then its values must be NULL too.  Each offset array present must start at 0, never decrease and end at its n_ count, and
+ * qual must hold l_qseq values per read; checked as c3b_bam_records is. */
 typedef struct c3b_fa_records {
     c3b_bam_records core;
     const int64_t *qual_off;    /* bam_get_qual(): l_qseq phred values per read; absent = 0xFF (no qualities, as BAM stores it)  */
@@ -40,6 +42,9 @@ typedef struct c3b_fa_records {
     const uint8_t *qname;
     const int64_t *mv_off;      /* the "mv" B-array values, leading stride element included; an empty range = no tag          */
     const int32_t *mv;
+    int64_t n_qual;             /* entries of qual[], qname[] and mv[] (0 for an absent field)                                */
+    int64_t n_qname;
+    int64_t n_mv;
 } c3b_fa_records;
 
 /* struct Variant (src/clair3_full_alignment_dwell.h:111-118): a phased heterozygous SNP; genotype 1 = 0|1, 2 = 1|0. */

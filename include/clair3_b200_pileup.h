@@ -30,9 +30,11 @@ extern "C" {
 typedef struct c3b_plp c3b_plp;
 
 /* A coordinate-sorted run of alignment records of ONE contig, fields as htslib lays them out in bam1_t
- * (the vendored public header src/sam.h: bam1_core_t, bam_get_cigar, bam_get_seq).  The library trusts the offsets: cigar_off and
- * seq_off must be non-decreasing, start at 0 and address cigar[] / seq[] in bounds, every packed sequence must hold
- * (l_qseq + 1) / 2 bytes (clair3_b200/pileup_counts.py: BamRecords checks all of this on the host). */
+ * (the vendored public header src/sam.h: bam1_core_t, bam_get_cigar, bam_get_seq).  cigar_off and seq_off must start at 0, never
+ * decrease and end at n_cigar / n_seq, pos must not decrease, and every packed sequence must hold at least (l_qseq + 1) / 2
+ * bytes: what clair3_b200/records.py's BamRecords enforces.  Every entry point that takes records checks this before any kernel
+ * indexes through an offset (host records on the host, device records in one kernel that reads only the per-read arrays and
+ * the offsets, whose result the call waits for), and fails naming the field and the first read that breaks it. */
 typedef struct c3b_bam_records {
     int64_t n_reads;
     const int64_t *pos;         /* [n]   bam1_core_t.pos: 0-based leftmost coordinate, ascending                         */
@@ -44,6 +46,8 @@ typedef struct c3b_bam_records {
     const int64_t *seq_off;     /* [n+1] first BYTE of read i's packed sequence in seq[]                                  */
     const uint8_t *seq;         /*       bam_get_seq(): 4-bit nt16 codes, two per byte, high nibble first                 */
     const int32_t *l_qseq;      /* [n]   bam1_core_t.l_qseq                                                               */
+    int64_t n_cigar;            /*       entries of cigar[]                                                               */
+    int64_t n_seq;              /*       bytes of seq[]                                                                   */
 } c3b_bam_records;
 
 /* The arguments of calculate_clair3_pileup that shape the counts (max_indel_length only formats all_alt_info, max_depth is
