@@ -19,6 +19,7 @@ PILEUP_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_pil
 FA_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_fa.h")           # full-alignment tensor builder (N4)
 BAM_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_bam.h")         # BAM reader: BGZF blocks to device records
 CASCADE_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_cascade.h")  # pileup -> full-alignment selection
+PHASE_HEADER = os.path.join(os.path.dirname(_HERE), "include", "clair3_b200_phase.h")      # read-based phasing
 LIB_PATH = os.path.join(_HERE, "libclair3b200.so")
 
 ffi = cffi.FFI()
@@ -39,14 +40,16 @@ _plp_body, _ = _cdef_source(PILEUP_HEADER)
 _fa_body, _ = _cdef_source(FA_HEADER)
 _bam_body, _ = _cdef_source(BAM_HEADER)
 _cascade_body, _ = _cdef_source(CASCADE_HEADER)
+_phase_body, PHASE_CONSTANTS = _cdef_source(PHASE_HEADER)
 ffi.cdef(_body)
 ffi.cdef(_dbg_body)
 ffi.cdef(_plp_body)
 ffi.cdef(_fa_body)
 ffi.cdef(_bam_body)
 ffi.cdef(_cascade_body)
+ffi.cdef(_phase_body)
 DECLARED_FUNCTIONS = sorted(set(re.findall(r"\b(c3b_\w+)\s*\(", _body + _dbg_body + _plp_body + _fa_body + _bam_body +
-                                           _cascade_body)))
+                                           _cascade_body + _phase_body)))
 
 _lib = None
 

@@ -19,9 +19,14 @@ Each bed file's build starts a fresh ``rand()`` stream, as each of the reference
 own, and a site's network output does not depend on the sites it is batched with (DESIGN.md 8): the files do not depend on
 the number of ranks.
 
-Not implemented: phasing (``no_phasing_for_fa`` must be True: WhatsHap / LongPhase are not part of this project), gVCF, the
-haploid modes and ``platform="ilmn"`` (``NotImplementedError``); CRAM input and CSI indexes (``NotImplementedError``).  The
-reference FASTA may be bgzip-compressed with its ``.gzi`` (DESIGN.md 5g.1): each window is then inflated on the GPU.
+With ``enable_phasing`` the merged calls are phased on the GPU after MergeVcf (``clair3_b200.phasing``, DESIGN.md 5g.3) into
+``phased_merge_output.vcf.gz``: the phase sets come from WhatsHap's model (all-heterozygous wMEC, coverage cap 15), but the
+file is not WhatsHap's byte for byte.
+
+Not implemented: phasing for full alignment (``no_phasing_for_fa`` must be True: WhatsHap / LongPhase are not part of this
+project), gVCF, the haploid modes and ``platform="ilmn"`` (``NotImplementedError``); CRAM input and CSI indexes
+(``NotImplementedError``).  The reference FASTA may be bgzip-compressed with its ``.gzi`` (DESIGN.md 5g.1): each window is then
+inflated on the GPU.
 """
 from __future__ import annotations
 
@@ -31,7 +36,7 @@ import os
 import numpy as np
 import torch
 
-from . import bam_io, cascade, decode, targets
+from . import bam_io, cascade, decode, phasing, targets
 from .fa_tensor import MATRIX_DEPTH
 from .pileup_counts import FETCH_EXPAND, bed_chunk_region, chunk_region, counting_region, known_sites_chunk
 from .sharding import site_range
@@ -342,7 +347,7 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
                 call_snp_only=False, enable_long_indel=False, enable_variant_calling_at_sequence_head_and_tail=False,
                 print_ref_calls=False, pileup_only=False, no_phasing_for_fa=True, enable_dwell_time=False, gvcf=False,
                 haploid_precise=False, haploid_sensitive=False, keep_iupac_bases=False, split_bed_size=cascade.SPLIT_BED_SIZE,
-                workspaces=None, device=None, group=None, k=16):
+                workspaces=None, device=None, group=None, k=16, enable_phasing=False):
     """Clair3's pipeline (scripts/clair3_c_impl_pipeline.py with ``--no_phasing_for_fa True``) over the genome: writes
     ``pileup.vcf.gz``, ``full_alignment.vcf.gz`` and ``merge_output.vcf.gz`` with their ``.tbi`` into ``out_dir``, as the
     reference does with its early exits (``file_texts``).  Options as run_clair3.py names them (None / 0 percentages and allele frequencies: the platform's defaults, see
@@ -353,7 +358,12 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
 
     Returns, on rank 0, a dict: ``files`` {name: path}, ``texts`` {name: decompressed text}, ``contigs``, ``chunks``,
     ``qual_cutoffs``, ``beds`` (number of bed files), ``rows`` {name: row count}, ``stages`` (wall and device ms per stage,
-    this rank's); None on the other ranks."""
+    this rank's); None on the other ranks.
+
+    ``enable_phasing`` (run_clair3.py's ``--enable_phasing``): when the run reaches MergeVcf and ``merge_output`` has a record,
+    each contig's merged rows are phased (``_phase``; rank r takes a contiguous run of the contigs) and
+    ``phased_merge_output.vcf.gz`` is written with its ``.tbi`` too.  The phase sets follow WhatsHap's model
+    (``clair3_b200.phasing``); the file is not WhatsHap's byte for byte."""
     if no_phasing_for_fa is not True:
         raise NotImplementedError("genome: phasing for full alignment (WhatsHap / LongPhase) is not implemented; "
                                   "run with no_phasing_for_fa=True")
@@ -403,12 +413,20 @@ def call_genome(bam_fn, ref_fn, model_p, model_f, out_dir, platform="ont", sampl
         kept = [(g, ctg, pos[keep[g]], [r for r, k_ in zip(rows, keep[g]) if k_]) for g, ctg, pos, _, _, rows in mine]
         parts = _gather0((kept, fa_rows), group, world, rank)
         st.mark("gather")
+        merged = None
+        if rank == 0:
+            texts, merged = _file_texts(head, names,
+                                        [c[1:] for c in sorted((c for part in parts for c in part[0]), key=lambda c: c[0])],
+                                        [c[1:] for c in sorted((c for part in parts for c in part[1]), key=lambda c: c[0])],
+                                        qual, print_ref_calls, pileup_only, tgt if genotyping else None)
+            st.mark("merge and format")
+        phased = None
+        if enable_phasing:
+            phased = _phase(ws.decoder, st, bam_fn, index, lengths, merged, chunk_size, group, world, rank)
         if rank != 0:
             return None
-        texts = file_texts(head, names, [c[1:] for c in sorted((c for part in parts for c in part[0]), key=lambda c: c[0])],
-                           [c[1:] for c in sorted((c for part in parts for c in part[1]), key=lambda c: c[0])],
-                           qual, print_ref_calls, pileup_only, tgt if genotyping else None)
-        st.mark("merge and format")
+        if phased is not None:
+            texts["phased_merge_output"] = vcf_text(phasing.phase_header(head), phased)
         out.update(qual_cutoffs=cuts, beds=len(beds))
         _write(out_dir, texts, out, ws.decoder, st)
         st.mark("write")
@@ -475,32 +493,69 @@ def _bed_files(builder, st, read, beds, mine, model_f, cfg_f, k, fa):
 
 
 def file_texts(head, contigs, pileup_chunks, fa_beds, qual=2, print_ref=False, pileup_only=False, known=None):
-    """The files' texts, {name: text}, from the rows of the whole run: SortVcf, MergeVcf per contig and, with ``known`` (the
+    """``_file_texts``' texts alone."""
+    return _file_texts(head, contigs, pileup_chunks, fa_beds, qual, print_ref, pileup_only, known)[0]
+
+
+def _file_texts(head, contigs, pileup_chunks, fa_beds, qual=2, print_ref=False, pileup_only=False, known=None):
+    """(texts, merged): the files' texts, {name: text}, from the rows of the whole run: SortVcf, MergeVcf per contig and, with ``known`` (the
     known-sites ``Targets``), AddBackMissingVariantsInGenotyping.  ``head``: ``header``'s text; ``contigs``: the contig names
     in CONTIGS order; ``pileup_chunks`` / ``fa_beds``: per pileup chunk (the rows pileup.vcf keeps) / per bed file, in order,
     (contig, 1-based positions, row texts).  The reference's early exits: no contig - a header-only ``merge_output`` alone; no
     pileup row - header-only ``pileup`` and ``merge_output``; ``pileup_only`` - ``pileup`` alone, and ``merge_output`` a copy
-    of it when it holds no row; no bed file or no full-alignment row - ``merge_output`` a copy of ``pileup``."""
+    of it when it holds no row; no bed file or no full-alignment row - ``merge_output`` a copy of ``pileup``.  ``merged``: the
+    sorted MergeVcf body before the add-back, which ``--enable_phasing`` phases; None on every early exit, and when it holds no
+    row (the pipeline's exit in variant merging)."""
     if not contigs:
-        return {"merge_output": head}
+        return {"merge_output": head}, None
     p_body = sort_rows((r for c in pileup_chunks for r in c[2]), contigs)
     if not p_body:
-        return {"pileup": head, "merge_output": head}                  # SortVcf: no variant found
+        return {"pileup": head, "merge_output": head}, None              # SortVcf: no variant found
     if pileup_only:
         pileup = vcf_text(head, postprocess_pileup(p_body, qual, print_ref), True)
-        return {"pileup": pileup} if has_records(pileup) else {"pileup": pileup, "merge_output": pileup}
+        return ({"pileup": pileup} if has_records(pileup) else {"pileup": pileup, "merge_output": pileup}), None
     texts = {"pileup": vcf_text(head, p_body, True)}
     if fa_beds:
         texts["full_alignment"] = vcf_text(head, sort_rows((r for c in fa_beds for r in c[2]), contigs))
     if not fa_beds or not has_records(texts["full_alignment"]):
         texts["merge_output"] = texts["pileup"]                         # ensure_merge_output
-        return texts
+        return texts, None
     merged = sort_rows("".join(_merge_contig(pileup_chunks, fa_beds, ctg, qual, print_ref) for ctg in contigs)
                        .splitlines(keepends=True), contigs)
     texts["merge_output"] = vcf_text(head, merged)
     if known is not None and merged:
         texts["merge_output"] = head + "\n" + cascade.add_back_missing(merged, known)
-    return texts
+    return texts, (merged if has_records(merged) else None)
+
+
+def _broadcast0(obj, group, world):
+    if world == 1:
+        return obj
+    import torch.distributed as dist
+    box = [obj]
+    dist.broadcast_object_list(box, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+    return box[0]
+
+
+def _phase(decoder, st, bam_fn, index, lengths, merged, span, group, world, rank):
+    """``--enable_phasing``: the phased body of ``merged`` (rank 0's MergeVcf body; None: the run left early, and nothing is
+    phased) on every rank's GPU - rank r the contigs ``site_range`` gives it, in the body's order, each decoded in spans of
+    ``span`` bases (``phase_gpu.phase_contig``) - gathered on rank 0.  Returns the body on rank 0, None elsewhere."""
+    from . import phase_gpu
+    merged = _broadcast0(merged, group, world)
+    if merged is None:
+        return None
+    by = phasing.split_contigs(merged)
+    ctgs = list(by)
+    mine = {}
+    for ctg in ctgs[slice(*site_range(len(ctgs), rank, world))]:
+        mine[ctg] = phase_gpu.phase_contig(decoder, bam_fn, ctg, lengths[ctg], by[ctg], span, index)[0]
+    st.mark("phase")
+    parts = _gather0(mine, group, world, rank)
+    if rank != 0:
+        return None
+    done = {k: v for part in parts for k, v in part.items()}
+    return "".join("".join(done[c]) for c in ctgs)
 
 
 def _merge_contig(p_chunks, f_beds, ctg, qual, print_ref):

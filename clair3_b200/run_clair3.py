@@ -7,8 +7,11 @@ Loads ``pileup.pt`` and ``full_alignment.pt`` from ``--model_path`` and writes `
 ``merge_output.vcf.gz`` with their ``.tbi`` into ``--output`` (``genome.call_genome``).  Several GPUs: start one process per GPU
 with ``torchrun --nproc_per_node N -m clair3_b200.run_clair3 ...``; each rank takes the GPU of its ``LOCAL_RANK``.
 ``--ref_fn`` may be bgzip-compressed, with the ``.fai`` and ``.gzi`` ``samtools faidx`` writes.  ``--threads`` is accepted and
-ignored.  Phasing (``--no_phasing_for_fa`` not True), ``--gvcf``, the haploid modes and
-platform ``ilmn`` are refused.
+ignored.  ``--enable_phasing`` (or ``--use_whatshap_for_final_output_phasing``, as run_clair3.py takes either) also writes
+``phased_merge_output.vcf.gz``, phased on the GPU: its phase sets come from WhatsHap's model (all-heterozygous weighted
+minimum error correction over at most 15 reads per variant, ``clair3_b200.phasing``), but the file is not WhatsHap's byte for
+byte - alleles are read from the aligned base rather than by realignment.  Phasing for full alignment
+(``--no_phasing_for_fa`` not True), ``--gvcf``, the haploid modes and platform ``ilmn`` are refused.
 """
 from __future__ import annotations
 
@@ -52,7 +55,7 @@ def parser():
     p.add_argument("--min_coverage", type=int, default=2)
     for flag in ("--include_all_ctgs", "--call_snp_only", "--enable_long_indel", "--enable_variant_calling_at_sequence_head_and_tail",
                  "--print_ref_calls", "--pileup_only", "--no_phasing_for_fa", "--enable_dwell_time", "--gvcf", "--haploid_precise",
-                 "--haploid_sensitive", "--keep_iupac_bases"):
+                 "--haploid_sensitive", "--keep_iupac_bases", "--enable_phasing", "--use_whatshap_for_final_output_phasing"):
         p.add_argument(flag, nargs="?", const=True, default=False, type=_bool)
     return p
 
@@ -100,7 +103,8 @@ def main(argv=None):
             enable_variant_calling_at_sequence_head_and_tail=args.enable_variant_calling_at_sequence_head_and_tail,
             print_ref_calls=args.print_ref_calls, pileup_only=args.pileup_only, no_phasing_for_fa=args.no_phasing_for_fa,
             enable_dwell_time=args.enable_dwell_time, gvcf=args.gvcf, haploid_precise=args.haploid_precise,
-            haploid_sensitive=args.haploid_sensitive, keep_iupac_bases=args.keep_iupac_bases, device=dev, group=group)
+            haploid_sensitive=args.haploid_sensitive, keep_iupac_bases=args.keep_iupac_bases, device=dev, group=group,
+            enable_phasing=bool(args.enable_phasing or args.use_whatshap_for_final_output_phasing))
     finally:
         if group is not None:
             import torch.distributed as dist
