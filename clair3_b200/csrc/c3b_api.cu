@@ -314,7 +314,7 @@ extern "C" int c3b_set_option(c3b_model *m, const char *name, int value) {
         if (value != 1 && value != 2) { c3b_set_error("lstm_wg must be 1 or 2"); return 1; }
         m->lstm_wg = (int)value;
     } else if (!strcmp(name, "lstm2_split")) {
-        if (value != 0 && value != 1) { c3b_set_error("lstm2_split must be 0 or 1"); return 1; }
+        if (value < 0 || value > 2) { c3b_set_error("lstm2_split must be 0, 1 or 2"); return 1; }
         m->lstm2_split = value;
     } else if (!strcmp(name, "lstm_mufu16")) {
         m->lstm_mufu16 = value ? 1 : 0;
@@ -804,10 +804,11 @@ static int forward_pileup_chunk(c3b_model *m, Workspace *w, const PileupSrc &src
     const TcPileupBuffers &b = c.tc;
     const int64_t bp = b.bp;
     // sub-tile width of lstm_tc_kernel (sites per warpgroup): 64 = fewest SM-microseconds per site, the smallest tile that still
-    // fills the GPU = shortest single-batch latency.  LSTM2's weights leave room for at most 32-site sub-tiles.
+    // fills the GPU = shortest single-batch latency.  LSTM2's weights and registers leave room for at most 48 sites per CTA, in
+    // the split kernel's single-buffer form (lstm2_split 2), and for 32 otherwise; it takes that in place of LSTM1's 64.
     int tile1 = m->lstm_tile;
     if (tile1 == 0) tile1 = !latency ? 64 : (bp / 64 >= m->sm_count) ? 64 : (bp / 32 >= m->sm_count) ? 32 : 16;
-    const int tile2 = tile1 > 32 ? 32 : tile1;
+    const int tile2 = tile1 <= 32 ? tile1 : m->lstm2_split == 2 ? 48 : 32;
     { PROF("lstm1"); if (c3b_launch_lstm1_tc(m, b, src, n, tile1, s)) return 1; }
     { PROF("proj2"); if (c3b_launch_proj2(m, b.h1, m->proj2, b.pg, (int)bp, s)) return 1; }
     { PROF("lstm2"); if (c3b_launch_lstm2_tc(m, b, n, tile2, m->lstm2_split != 0, s)) return 1; }

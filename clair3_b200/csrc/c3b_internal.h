@@ -521,7 +521,8 @@ struct c3b_model {
     int lstm_tile = 0;
     int profile = 0;
     int lstm_wg = 2;                   // warpgroups (one sub-tile of sites each) per LSTM CTA (option "lstm_wg": 1 or 2)
-    int lstm2_split = 1;               // LSTM2 split by block pair (option "lstm2_split"): 1 lstm2_split_kernel, 0 the sub-tile kernel
+    int lstm2_split = 1;               // LSTM2 split by block pair (option "lstm2_split"): 1 lstm2_split_kernel at 32 sites at most;
+                                       // 2 the same kernel at 48 sites where LSTM1 runs 64-site tiles; 0 the sub-tile kernel
     int lstm_mufu16 = 0;               // 1: packed tanh.approx.f16x2 gate activations, 0 (default, faster: the epilogue is issue-bound): fp32 tanh.approx
     int tap_ws = -1;                   // debug: workspace index c3b_get_tap reads
     int taps = 0;                      // debug option "taps": record where the intermediate activations of a forward live

@@ -43,6 +43,10 @@
 // in block-pair order they finish in turn, and each warpgroup's cell math runs under the later chains (5.0 k cycles, against
 // 10.8 k for 64 sites in the sub-tile kernel).  Each block pair's weights have their own mbarrier, so warpgroup 0 starts step 0
 // once its 40 KB have arrived.
+// Every LSTM2 kernel writes the pre-gates into the accumulators and starts each chain from them (scale-d = 1): the same fp32
+// addition order in all of them, so they stay bit-identical to each other.  Option lstm2_split 2 runs the split kernel at 48
+// sites with one h operand buffer (see lstm2_split_kernel): 6.8 k cycles per 48-site step against 5.0 k (now 4.7 k) per 32-site
+// step, ~3 % fewer cycles per site, no measurable end-to-end gain on H100, so not the default.
 #include <type_traits>
 
 #include "c3b_internal.h"
@@ -125,6 +129,7 @@ template <int NB>
 __device__ __forceinline__ void wgmma_nb(float (&d)[NB / 2], uint64_t a, uint64_t b, uint32_t acc) {
     if constexpr (NB == 16) ptx::wgmma_m64n16k16(d, a, b, acc);
     else if constexpr (NB == 32) ptx::wgmma_m64n32k16(d, a, b, acc);
+    else if constexpr (NB == 48) ptx::wgmma_m64n48k16(d, a, b, acc);
     else ptx::wgmma_m64n64k16(d, a, b, acc);
 }
 
@@ -368,21 +373,30 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
 #pragma unroll
         for (int pp = 0; pp < NP; ++pp) {
             float acc0[NB / 2], acc1[NB / 2];
+            // LSTM2: this pair's pre-gates, loaded one block pair ago, are where the chain starts accumulating
+            if constexpr (LAYER2) {
+#pragma unroll
+                for (int i = 0; i < NB / 8; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        acc0[4 * i + e] = half_lo(pgn[2 * i + e].x);
+                        acc0[4 * i + 2 + e] = half_hi(pgn[2 * i + e].x);
+                        acc1[4 * i + e] = half_lo(pgn[2 * i + e].y);
+                        acc1[4 * i + 2 + e] = half_hi(pgn[2 * i + e].y);
+                    }
+            }
             ptx::wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < K / 16; ++ks) {
                 const uint64_t bd = ptx::wgmma_desc(b_addr + ks * 2 * LBO_B, LBO_B, 128);
                 const uint32_t a0 = w_addr + (2 * pp) * kBlkBytes + ks * 2 * 1024;
-                wgmma_nb<NB>(acc0, ptx::wgmma_desc(a0, 1024, 128), bd, ks > 0);
-                wgmma_nb<NB>(acc1, ptx::wgmma_desc(a0 + kBlkBytes, 1024, 128), bd, ks > 0);
+                wgmma_nb<NB>(acc0, ptx::wgmma_desc(a0, 1024, 128), bd, LAYER2 || ks > 0);
+                wgmma_nb<NB>(acc1, ptx::wgmma_desc(a0 + kBlkBytes, 1024, 128), bd, LAYER2 || ks > 0);
             }
             ptx::wgmma_commit();
-            // LSTM2: this pair's pre-gates were loaded one block pair ago; start the next pair's (after the last pair: the next
-            // step's first) so that they arrive while this pair's MMAs and cell math run
-            uint2 pgv[PGN];
+            // LSTM2: start the next pair's pre-gates (after the last pair: the next step's first) so that they arrive while this
+            // pair's MMAs and cell math run
             if constexpr (LAYER2) {
-#pragma unroll
-                for (int i = 0; i < PGN; ++i) pgv[i] = pgn[i];
                 if (pp + 1 < NP) load_pg(t, pp + 1);
                 else if (step + 1 < C3B_T) load_pg(tn, 0);
             } else {
@@ -407,12 +421,6 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
                     gf[e] = acc0[4 * i + 2 + e];
                     gg[e] = acc1[4 * i + e];
                     go[e] = acc1[4 * i + 2 + e];
-                    if constexpr (LAYER2) {
-                        gi[e] += half_lo(pgv[2 * i + e].x);
-                        gf[e] += half_hi(pgv[2 * i + e].x);
-                        gg[e] += half_lo(pgv[2 * i + e].y);
-                        go[e] += half_hi(pgv[2 * i + e].y);
-                    }
                 }
                 if (MUFU16) {
                     hq[pp][i] = lstm_cell_h2(gi, gf, gg, go, &c[pp][2 * i]);
@@ -458,7 +466,11 @@ __global__ void __launch_bounds__(128 * WG, 1) lstm_tc_kernel(const LstmDev p) {
 
 // LSTM2 split by block pair (option "lstm2_split", see the header): one CTA = one direction x NB sites, five warpgroups, and
 // warpgroup pp owns block pair pp (hidden units 32pp .. 32pp + 31) of all NB sites.  The per-site arithmetic is lstm_tc_kernel's
-// for LAYER2: the same A blocks, B columns, k order and N per wgmma chain, the same cell math.
+// for LAYER2: the same A blocks, B columns, k order per wgmma chain, the same accumulator start (the pre-gates), the same cell
+// math; a site's column does not depend on N.  NB = 48 keeps one h operand buffer (two do not fit beside W_hh) and loads the next
+// step's pre-gates after the cell math, where the accumulators are free: during the chain, beside the 48 accumulators, they
+// would spill (96 registers per thread at 640 threads; at NB = 64 the accumulators and cell state alone leave too few).  bp is
+// a multiple of 128, so the last 48-site CTA runs past it; its sites >= bp read zero pre-gates and write no h.
 template <int NB, bool MUFU16>
 __global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
     constexpr int H = 160;
@@ -468,6 +480,8 @@ __global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
     constexpr uint32_t W_BYTES = 2 * NP * kBlkBytes;
     constexpr uint32_t LBO_B = (NB + 1) * 16;
     constexpr uint32_t B_BYTES = (K / 8) * LBO_B;
+    constexpr bool ONE_BUF = NB == 48;
+    constexpr int NBUF = ONE_BUF ? 1 : 2;
 
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t w_bar[NP];                  // one per block pair: a warpgroup starts once its own 40 KB have arrived
@@ -481,8 +495,9 @@ __global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
     const int s0 = 2 * (lane & 3);
     const int dir = blockIdx.y;
     const int b0 = blockIdx.x * NB;
-    // two operand buffers of h: step s reads buffer s & 1 and writes h_t into the other, so one CTA barrier per step orders both
-    // the reads of step s - 1 before the writes of step s + 1 and the writes of step s before the reads of step s + 1
+    // NB < 48: two operand buffers of h: step s reads buffer s & 1 and writes h_t into the other, so one CTA barrier per step
+    // orders both the reads of step s - 1 before the writes of step s + 1 and the writes of step s before the reads of step s + 1.
+    // NB = 48: one buffer; a second CTA barrier per step, after every chain has read h_{t-1}, comes before the h_t stores.
     uint8_t *b_smem = smem + W_BYTES;
     const uint32_t w_addr = ptx::smem_u32(smem);
     const uint32_t b_addr = ptx::smem_u32(b_smem);
@@ -508,20 +523,29 @@ __global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
     for (int i = 0; i < NB / 4; ++i) c[i] = 0.f;
 
     // pre-gates of this thread's unit, one 8-byte word (i, f, g, o) per site, for the next step: loaded a whole step early
+    // (NB = 48: most of a step early)
     uint2 pgn[NB / 4];
-    const __half *pgp = p.pg + (size_t)dir * 640 + pp * 128 + 4 * (8 * w + q0);
     auto load_pg = [&](int tt) {
+        int col = dir * 640 + pp * 128 + 4 * (8 * w + q0);
+        asm volatile("" : "+r"(col));               // opaque, as i0 in copy_out: a pointer kept across steps spills at NB = 48
+        const __half *pgp = p.pg + col;
 #pragma unroll
         for (int i = 0; i < NB / 8; ++i)
 #pragma unroll
-            for (int e = 0; e < 2; ++e)
-                pgn[2 * i + e] = *reinterpret_cast<const uint2 *>(pgp + ((size_t)tt * p.bp + b0 + 8 * i + s0 + e) * 1280);
+            for (int e = 0; e < 2; ++e) {
+                const int b = b0 + 8 * i + s0 + e;
+                pgn[2 * i + e] = NB % 128 == 0 || b < p.bp ? *reinterpret_cast<const uint2 *>(pgp + ((size_t)tt * p.bp + b) * 1280)
+                                                           : make_uint2(0, 0);
+            }
     };
     load_pg(dir ? C3B_T - 1 : 0);
     // h of time tt (in operand buffer `buf`) -> hout: this warpgroup's four k-groups
     auto copy_out = [&](int tt, int buf) {
-        for (int idx = wt; idx < NB * 4; idx += 128) {
+        int i0 = wt;                                // opaque: else its addresses are kept across steps (NB = 48: spilled)
+        asm volatile("" : "+r"(i0));
+        for (int idx = i0; idx < NB * 4; idx += 128) {
             const int kgh = 4 * pp + idx / NB, n = idx % NB;
+            if (NB % 128 != 0 && b0 + n >= p.bp) continue;
             *reinterpret_cast<uint4 *>(p.hout + h_out_offset<true>(tt, dir, kgh, b0 + n, p.bp)) =
                 *reinterpret_cast<const uint4 *>(b_smem + buf * B_BYTES + kgh * LBO_B + n * 16);
         }
@@ -530,32 +554,43 @@ __global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
     const bool tr = p.trace != nullptr && tid == 0 && blockIdx.x == 0 && blockIdx.y == 0;
     for (int step = 0; step < C3B_T; ++step) {
         const int t = dir ? (C3B_T - 1 - step) : step;
-        const int cur = step & 1;
+        const int cur = ONE_BUF ? 0 : step & 1;
         ptx::fence_proxy_async_smem();
-        __syncthreads();                            // h_{t-1} is in buffer cur; every read of buffer cur ^ 1 is done
+        __syncthreads();                            // h_{t-1} is in buffer cur; (NB < 48) every read of buffer cur ^ 1 is done
         if (tr) p.trace[step * 4 + 0] = clock64();
+        // the chain adds W_hh h_{t-1} onto the pre-gates
         float acc0[NB / 2], acc1[NB / 2];
+#pragma unroll
+        for (int i = 0; i < NB / 8; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                acc0[4 * i + e] = half_lo(pgn[2 * i + e].x);
+                acc0[4 * i + 2 + e] = half_hi(pgn[2 * i + e].x);
+                acc1[4 * i + e] = half_lo(pgn[2 * i + e].y);
+                acc1[4 * i + 2 + e] = half_hi(pgn[2 * i + e].y);
+            }
         // the warpgroups issue their chains in block-pair order (named barrier pp: warpgroup pp - 1 arrives once its chain is
         // issued), so the tensor pipe finishes them one after another and each warpgroup's cell math runs under the later
         // warpgroups' MMAs; issued together, the five chains interleave and every cell math waits for the last MMA
         if (step == 0) ptx::mbar_wait(&w_bar[pp], 0);
         if (pp > 0) ptx::named_bar_sync(pp, 256);
+        // the operand addresses, opaque to the compiler within a step: else it keeps the chain's 30 descriptors live through the
+        // whole loop (NB = 48: beside the 48 accumulators and 12 cells, they spill)
+        uint32_t wa = w_addr + (2 * pp) * kBlkBytes, ba = b_addr + cur * B_BYTES;
+        asm volatile("" : "+r"(wa), "+r"(ba));
         ptx::wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < K / 16; ++ks) {
-            const uint64_t bd = ptx::wgmma_desc(b_addr + cur * B_BYTES + ks * 2 * LBO_B, LBO_B, 128);
-            const uint32_t a0 = w_addr + (2 * pp) * kBlkBytes + ks * 2 * 1024;
-            wgmma_nb<NB>(acc0, ptx::wgmma_desc(a0, 1024, 128), bd, ks > 0);
-            wgmma_nb<NB>(acc1, ptx::wgmma_desc(a0 + kBlkBytes, 1024, 128), bd, ks > 0);
+            const uint64_t bd = ptx::wgmma_desc(ba + ks * 2 * LBO_B, LBO_B, 128);
+            const uint32_t a0 = wa + ks * 2 * 1024;
+            wgmma_nb<NB>(acc0, ptx::wgmma_desc(a0, 1024, 128), bd, 1);
+            wgmma_nb<NB>(acc1, ptx::wgmma_desc(a0 + kBlkBytes, 1024, 128), bd, 1);
         }
         ptx::wgmma_commit();
         if (pp + 1 < NP) ptx::named_bar_arrive(pp + 1, 256);
-        // this step's pre-gates arrived during the last step; start the next step's, and ship h_{t-1} while the MMAs run
-        uint2 pgv[NB / 4];
-#pragma unroll
-        for (int i = 0; i < NB / 4; ++i) pgv[i] = pgn[i];
-        if (step + 1 < C3B_T) load_pg(dir ? t - 1 : t + 1);
-        if (step > 0) copy_out(dir ? t + 1 : t - 1, cur);
+        // start the next step's pre-gates, and ship h_{t-1} while the MMAs run (NB < 48)
+        if (!ONE_BUF && step + 1 < C3B_T) load_pg(dir ? t - 1 : t + 1);
+        if (!ONE_BUF && step > 0) copy_out(dir ? t + 1 : t - 1, cur);
         ptx::wgmma_wait<0>();
         ptx::fence_operand(acc0);
         ptx::fence_operand(acc1);
@@ -566,10 +601,10 @@ __global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
             float gi[2], gf[2], gg[2], go[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                gi[e] = acc0[4 * i + e] + half_lo(pgv[2 * i + e].x);
-                gf[e] = acc0[4 * i + 2 + e] + half_hi(pgv[2 * i + e].x);
-                gg[e] = acc1[4 * i + e] + half_lo(pgv[2 * i + e].y);
-                go[e] = acc1[4 * i + 2 + e] + half_hi(pgv[2 * i + e].y);
+                gi[e] = acc0[4 * i + e];
+                gf[e] = acc0[4 * i + 2 + e];
+                gg[e] = acc1[4 * i + e];
+                go[e] = acc1[4 * i + 2 + e];
             }
             if (MUFU16) {
                 hq[i] = lstm_cell_h2(gi, gf, gg, go, &c[2 * i]);
@@ -580,9 +615,14 @@ __global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
             }
         }
         if (tr) p.trace[step * 4 + 2] = clock64();
-        // h_t -> buffer cur ^ 1, element (site n, k = unit)
+        if constexpr (ONE_BUF) {
+            if (step + 1 < C3B_T) load_pg(dir ? t - 1 : t + 1);
+            if (step > 0) copy_out(dir ? t + 1 : t - 1, cur);
+            __syncthreads();                        // every chain and copy-out of this step has read h_{t-1}
+        }
+        // h_t -> buffer cur ^ 1 (NB = 48: buffer 0), element (site n, k = unit)
         const uint32_t kcol = 32 * pp + 8 * w + q0;
-        uint8_t *dst = b_smem + (cur ^ 1) * B_BYTES + (kcol >> 3) * LBO_B + (kcol & 7) * 2;
+        uint8_t *dst = b_smem + (cur ^ 1) % NBUF * B_BYTES + (kcol >> 3) * LBO_B + (kcol & 7) * 2;
 #pragma unroll
         for (int i = 0; i < NB / 8; ++i) {
             *reinterpret_cast<uint16_t *>(dst + (8 * i + s0) * 16) = (uint16_t)(hq[i] & 0xffffu);
@@ -593,15 +633,15 @@ __global__ void __launch_bounds__(640, 1) lstm2_split_kernel(const LstmDev p) {
 
     // last h
     __syncthreads();
-    copy_out(dir ? 0 : C3B_T - 1, C3B_T & 1);
+    copy_out(dir ? 0 : C3B_T - 1, C3B_T % NBUF);
 }
 
 template <int NB, bool MUFU16>
 int launch_lstm2_split_impl(const LstmDev &p, cudaStream_t s) {
-    const size_t smem = (size_t)4 * 160 * 160 * 2 + (size_t)2 * (160 / 8) * (NB + 1) * 16;   // W_hh + two h operand buffers
+    const size_t smem = (size_t)4 * 160 * 160 * 2 + (size_t)(NB == 48 ? 1 : 2) * (160 / 8) * (NB + 1) * 16;   // W_hh + h operand buffers
     auto kern = lstm2_split_kernel<NB, MUFU16>;
     C3B_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(p.bp / NB, 2);
+    dim3 grid((p.bp + NB - 1) / NB, 2);
     c3b_note_grid((long long)grid.x * grid.y);
     kern<<<grid, 640, smem, s>>>(p);
     C3B_CUDA(cudaGetLastError());
@@ -682,6 +722,7 @@ int c3b_launch_lstm2_tc(const c3b_model *m, const TcPileupBuffers &b, int64_t ba
         switch (tile) {
             case 16: return launch_lstm2_split<16>(p, m->lstm_mufu16 != 0, s);
             case 32: return launch_lstm2_split<32>(p, m->lstm_mufu16 != 0, s);
+            case 48: return launch_lstm2_split<48>(p, m->lstm_mufu16 != 0, s);
         }
     } else {
         switch (tile) {

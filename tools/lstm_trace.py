@@ -1,12 +1,13 @@
 """Per-step SM-cycle breakdown of the two recurrent kernels (lstm1, lstm2) of one pileup forward.
 
-    python tools/lstm_trace.py [--batch 1024] [--lstm-wg 1|2] [--lstm-tile 16|32|64] [--lstm2-split 0|1] [--per-step]
+    python tools/lstm_trace.py [--batch 1024] [--lstm-wg 1|2] [--lstm-tile 16|32|64] [--lstm2-split 0|1|2] [--per-step]
 
 Builds a ``Clair3_P`` from the seeded synthetic weights (``clair3_b200.synth``), turns on the debug option ``lstm_trace`` and
 runs one device-resident forward after a warm-up forward. Thread 0 of CTA (0, 0) of each LSTM kernel stamps ``clock64`` at four
 points of every step (``c3b_debug_lstm_trace``): operands ready, first accumulator ready, cell math of the step done, h_t in
-the operand buffer. In LSTM2's split kernel (option ``lstm2_split`` 1) that thread is in warpgroup 0, so the stamps follow block
-pair 0 of the CTA's sites. Printed per layer, as medians over the steps (and per step with ``--per-step``):
+the operand buffer. In LSTM2's split kernel (option ``lstm2_split`` 1: 32 sites per CTA, 2: 48 sites, one operand buffer) that
+thread is in warpgroup 0, so the stamps follow block pair 0 of the CTA's sites; with one buffer, ``h_store`` includes the wait
+for every warpgroup's chain and copy-out before h_t overwrites h_{t-1}. Printed per layer, as medians over the steps (and per step with ``--per-step``):
 
     period      operands ready of step s -> operands ready of step s + 1
     first_acc   operands ready -> the first block pair's accumulators are in registers
@@ -46,7 +47,7 @@ def main():
     ap.add_argument("--batch", type=int, default=1024)
     ap.add_argument("--lstm-wg", type=int, default=0, help="warpgroups per LSTM CTA (0 = library default)")
     ap.add_argument("--lstm-tile", type=int, default=0, help="sites per LSTM1 sub-tile (0 = library choice)")
-    ap.add_argument("--lstm2-split", type=int, default=-1, help="LSTM2 split by block pair: 0 | 1 (-1 = library default)")
+    ap.add_argument("--lstm2-split", type=int, default=-1, help="LSTM2 split by block pair: 0 | 1 | 2 (-1 = library default)")
     ap.add_argument("--per-step", action="store_true")
     args = ap.parse_args()
 
